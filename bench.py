@@ -4,6 +4,7 @@ fixture-backed Composition per step (BASELINE.json metric: frames/s and
 pixel-segments/s).
 
     python bench.py --gpus N --steps K --warmup W [--workload paris4k|cubics100k|circles8k] [--impl reference]
+                    [--dump-outputs DIR]
 
 One JSON line on stdout (rank 0). Keys follow the driver's contract:
   value        frames/s with the composition resident in HBM and the frame left
@@ -15,6 +16,8 @@ One JSON line on stdout (rank 0). Keys follow the driver's contract:
   cpu_baseline the CPU oracle ("forma CPU path, restated") on the host cores
 `--impl reference` times that CPU restatement as its own arm (the Rust crate
 cannot be built here: no cargo/rustc, see DESIGN.md).
+`--dump-outputs DIR` writes the frame of the headline workload's last timed step as .npy files
+(see dump_frames), so that two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -111,7 +114,23 @@ def measured_peak_gbs():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "H100 SXM data sheet"
+
+
+DUMP_PIXELS = 1 << 20  # pixels sampled per dumped frame: 2 frames x 16 MB + 8 MB of indices
+
+
+def dump_frames(out_dir, frames, w, h, stride):
+    """Writes RGBA8 frames (name -> uint8 buffer of h rows of `stride` bytes) to out_dir/<name>.npy
+    as float32 (n, 4) arrays of channel values. Frames of more than DUMP_PIXELS pixels are sampled
+    at the same seeded, sorted pixel indices every run; out_dir/pixel_index.npy (float64) holds them."""
+    os.makedirs(out_dir, exist_ok=True)
+    n = w * h
+    idx = np.arange(n) if n <= DUMP_PIXELS else np.sort(np.random.default_rng(0).choice(n, DUMP_PIXELS, replace=False))
+    np.save(os.path.join(out_dir, "pixel_index.npy"), idx.astype(np.float64))
+    for name, buf in frames.items():
+        px = np.asarray(buf, np.uint8).reshape(h, stride)[:, :w * 4].reshape(n, 4)
+        np.save(os.path.join(out_dir, f"{name}.npy"), px[idx].astype(np.float32))
 
 
 def usable_cpus():
@@ -217,6 +236,9 @@ def run_reference(args):
         return
     leg = cpu_leg(args.workload, args.steps, args.warmup)
     fps = leg["fps"]
+    if args.dump_outputs:
+        w, h, _ = WORKLOADS[args.workload]
+        dump_frames(args.dump_outputs, {"frame": leg["frame"], "frame_e2e": leg["frame"]}, w, h, w * 4)
     out = {
         "impl": "reference", "metric": "frames/sec", "value": fps, "unit": "frames/s", "n_gpus": args.gpus,
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": leg["ms_per_step"], "higher_is_better": True,
@@ -465,6 +487,8 @@ def bench_workload(env, args, name, steps, warmup, headline):
             a["launches"] += v["launches"]
     dev_ms, wall_ms = timed(frame_device, steps, device_acc)
     c1 = renderer.counters()
+    # The frame of the last timed step, as a caller of render_device receives it (untimed copy).
+    dev_frame = (whole if world > 1 else fb).cpu().numpy() if headline and args.dump_outputs and rank == 0 else None
     gather_ms = sum(a.elapsed_time(b) for a, b in gather_events[-steps:]) / steps if gather_events else 0.0
     render_ms = stage_acc["total"] / steps
     for _ in range(max(warmup, 1)):
@@ -536,16 +560,8 @@ def bench_workload(env, args, name, steps, warmup, headline):
     kname = max(kerns, key=lambda k: kerns[k]["ms_per_step"]) if kerns else None
     dom = kerns.get(kname, {"GBps": 0.0, "ms_per_launch": 0.0, "algorithmic_bytes_per_launch": 0.0})
     sort_ms = stages["sort"]
-    # dram__bytes_read + dram__bytes_write of one launch of that kernel, from the committed
-    # `ncu --set full` capture of this command (profiles/ncu_traffic.json), or null.
-    traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            traffic = json.load(f).get(name, {}).get(kname)
-    except Exception:
-        pass
     roofline = {"kernel": kname, "bound": "hbm", "achieved": dom["GBps"], "peak": peak, "peak_source": peak_kind,
-                "unit": "GB/s", "frac": dom["GBps"] / peak, "traffic": traffic,
+                "unit": "GB/s", "frac": dom["GBps"] / peak,
                 "algorithmic_bytes": dom["algorithmic_bytes_per_launch"], "kernel_ms": dom["ms_per_launch"],
                 "kernels": kerns,
                 # The whole sort against its algorithm-independent bound (SURVEY.md 8d: 16 N).
@@ -576,6 +592,8 @@ def bench_workload(env, args, name, steps, warmup, headline):
     }
     out["_frame"] = frame_copy
     out["_frame_no"] = frame_no[0]
+    if dev_frame is not None:
+        dump_frames(args.dump_outputs, {"frame": dev_frame, "frame_e2e": frame_copy}, w, h, stride)
     return out
 
 
@@ -601,7 +619,7 @@ def run_cuda(args):
     sampler = ClockSampler(local)
     env = {"torch": torch, "dist": dist, "api": forma_b200.load(), "rank": rank, "world": world, "local": local, "dev": dev,
            "stream": torch.cuda.current_stream(), "sampler": sampler,
-           "flush": torch.empty(384 << 20, dtype=torch.uint8, device=dev)}  # > 126 MB L2
+           "flush": torch.empty(384 << 20, dtype=torch.uint8, device=dev)}  # > 50 MB L2
     sampler.init_nvml()
     sampler.start()
     res = bench_workload(env, args, args.workload, args.steps, args.warmup, True)
@@ -663,8 +681,11 @@ def oracle_frame_matches(workload, frame_no, gpu_frame):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
-    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--steps", type=int, default=20,
+                    help="timed steps of the headline workload (both the device and the end-to-end leg) and of "
+                         "--impl reference; an --extra workload times max(3, min(steps, 10)) steps, the "
+                         "cpu_baseline leg at most 40 frames in 12 s")
+    ap.add_argument("--warmup", type=int, default=3, help="untimed steps before each timed leg of the headline workload (at least 3; 3 for an --extra workload)")
     ap.add_argument("--impl", default="cuda", choices=["cuda", "reference"])
     ap.add_argument("--workload", default="paris4k", choices=sorted(WORKLOADS))
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
@@ -673,6 +694,9 @@ def main():
                          "(default: circles8k_1m, BASELINE config 5, when the headline workload is paris4k)")
     ap.add_argument("--no-extra", action="store_true", help="headline workload only")
     ap.add_argument("--equal-bands", action="store_true", help="multi-GPU: equal tile-row bands instead of cost-balanced ones")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the headline workload's frame of the last timed step (device and host-buffer path) "
+                         "to DIR/frame.npy and DIR/frame_e2e.npy (float32 RGBA, a seeded pixel sample of large frames)")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3

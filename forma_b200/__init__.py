@@ -1,10 +1,10 @@
-"""forma_b200 — B200-native replacement for google/forma's rendering hot path.
+"""forma_b200 — H100-native replacement for google/forma's rendering hot path.
 
-The compute path lives in ``libforma_b200.so`` (hand-written CUDA for sm_100a,
+The compute path lives in ``libforma_b200.so`` (hand-written CUDA for sm_90a,
 built in-tree by ``forma_b200/csrc/Makefile``); this package is only the
 ctypes stub over its C ABI (``include/forma_b200.h``). There is no CPU
 fallback: importing works without a GPU (so the ABI can be inspected), but
-``Renderer()`` raises when no B200 is present, and loading fails loudly when
+``Renderer()`` raises when no H100 (sm_90) is present, and loading fails loudly when
 the shared library has not been built.
 """
 from __future__ import annotations

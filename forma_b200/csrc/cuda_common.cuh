@@ -1,5 +1,5 @@
 // Shared device helpers. All translation units are compiled with
-//   -gencode arch=compute_100a,code=sm_100a --fmad=false -prec-div=true -prec-sqrt=true
+//   -gencode arch=compute_90a,code=sm_90a --fmad=false -prec-div=true -prec-sqrt=true
 // so that `a * b + c` is never contracted: every fused multiply-add of the
 // reference (`mul_add`) is an explicit fmaf()/fma() here (SURVEY.md Appendix A).
 #pragma once
@@ -48,15 +48,15 @@ inline int device_sm_count() {
     const int d = current_device_index();
     int v = sms[d].load(std::memory_order_relaxed);
     if (!v) {
-        v = 148;
+        v = 132;
         cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, d);
-        if (v <= 0) v = 148;
+        if (v <= 0) v = 132;
         sms[d].store(v, std::memory_order_relaxed);
     }
     return v;
 }
 
-// Growable device buffer (never shrinks). 180 GB of HBM3e makes "keep the high
+// Growable device buffer (never shrinks). 80 GB of HBM3 still makes "keep the high
 // water mark" the right policy for per-frame scratch.
 template <class T>
 struct DeviceBuffer {

@@ -15,10 +15,10 @@ namespace forma {
 struct Options {
     int speculate = 1;       // launch kernels ahead of their count read-backs (0: strictly after)
     int band_copy = 1;       // host frames: paint / copy back in bands of tile rows
-    int copy_bands = 4;      //   ... how many (1..16; paris@4K end to end, r2 final build: 4 -> 582.7, 8 -> 567.9, 16 -> 553.8 frames/s; cubics100k 303.6 / 298.6 / 291.1; circles8k 102.3 / 101.1 / 97.7)
+    int copy_bands = 4;      //   ... how many (1..16)
     int sort_full_key = 0;   // 1: sort the layer digits even when the inserts are in layer order
     int sort_big_log2 = 19;  // key count from which the 4096-key tiles / reduce-then-scan passes are used
-    int sort_scan_log2 = 22; // key-only sorts: key count from which the reduce-then-scan passes replace the single-sweep ones (measured on paris@4K bands: 0.7 M keys 0.044 vs 0.055 ms, 3 M equal, 5.9 M 0.130 vs 0.105 ms)
+    int sort_scan_log2 = 22; // key-only sorts: key count from which the reduce-then-scan passes replace the single-sweep ones
     int test_gap_cap = 0;    // test hook: cap of the speculative carry-only-entry launch (0 = none)
     int paint_lpt = 1;       // heavy tiles first (longest-processing-time order) in the paint kernel
     int paint_wide = 0;      // 1: the paint kernel built for 6 CTAs / SM (up to 168 registers) instead of 8 (128)
@@ -26,8 +26,7 @@ struct Options {
     int sync_free = 1;       // painter tables without count read-backs when the previous frame's counts bound this one's (redone the slow way if they do not)
     int test_fast_shrink = 0;  // test hook: halve the bounds of the sync-free tables (forces the redo)
     int host_slices = 1;     // host frames: > 1 = that many tile-row slices rendered as independent upload -> render -> copy-back pipelines on their own streams.
-                             //   Off by default: measured on paris@4K 578.9 (off) vs 544-587 frames/s (2-4 slices), 509 (6), 422 (8); cubics100k 298.6 vs 280 / 237;
-                             //   the slices' kernel chains do not overlap on the device (latency-bound kernels that fill the SMs), see DESIGN.md section 3
+                             //   Off by default: the slices' kernel chains do not overlap on the device (latency-bound kernels that fill the SMs), see DESIGN.md section 3
     int slice_bands = 2;     //   ... copy bands inside a slice
     int slice_min_points = 65536;  //   ... only for compositions of at least this many points
     int slice_chain = 1;     //   ... uploads issued slice after slice, each waiting for the one before (0: all at once from the slices' threads)
@@ -197,7 +196,7 @@ void launch_paint(const PaintScene& S, const uint64_t* segs, const EntryRec* rec
                   const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st);
 // GradRec of every style slot (see device_types.h).
 void launch_grad_setup(const StyleRec* styles, const StopRec* stops, uint32_t n_styles, GradRec* grads, cudaStream_t st);
-// Packed fp32 (f32x2) arithmetic of the painter against scalar IEEE operations; mismatches are added to out[0].
+// Pixel-pair fp32 arithmetic of the painter against scalar IEEE operations; mismatches are added to out[0].
 void launch_f32x2_selftest(const float* a, const float* b, const float* c, uint32_t n, uint32_t* out, cudaStream_t st);
 // out[row] = 32 x entries + pixel segments of tile row `row` (see row_cost_kernel).
 void launch_row_costs(const uint2* tile_range, uint32_t tiles_x, uint32_t tiles_y, const uint64_t* segs, uint32_t n,

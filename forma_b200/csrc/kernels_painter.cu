@@ -23,10 +23,10 @@
 // one entry ahead of the blend: while entry k is blended from one cell buffer, entry k + 1
 // is accumulated into the other and the segments of entry k + 2 are in flight.
 //
-// Blend arithmetic runs on pixel pairs with Blackwell's packed fp32 instructions
-// (fma.rn.f32x2 / mul.rn.f32x2 -> FFMA2 / FMUL2): each half is the IEEE operation the
-// reference performs; additions and subtractions are written as fma(x, +-1, y), which is
-// the same single rounding, so that no product is ever contracted into a sum.
+// Blend arithmetic is written on pixel pairs (f2). sm_90 has no packed fp32 instructions,
+// so each half is one scalar IEEE operation, the one the reference performs; additions and
+// subtractions are written as fma(x, +-1, y), which is the same single rounding, so that no
+// product is ever contracted into a sum.
 //
 // Warps are persistent and take tiles by ticket. Tiles with many entries come first
 // (tile_index_kernel sorts them into four classes by entry count): a tile is painted by
@@ -62,28 +62,9 @@ __device__ __forceinline__ uint32_t meta_blend(uint32_t m) { return (m >> 5) & 1
 struct f2 {
     float x, y;
 };
-__device__ __forceinline__ unsigned long long f2_bits(f2 v) {
-    return (unsigned long long)__float_as_uint(v.x) | ((unsigned long long)__float_as_uint(v.y) << 32);
-}
-__device__ __forceinline__ f2 f2_from(unsigned long long b) {
-    return f2{__uint_as_float((uint32_t)b), __uint_as_float((uint32_t)(b >> 32))};
-}
 __device__ __forceinline__ f2 f2_splat(float v) { return f2{v, v}; }
-#ifndef FORMA_SCALAR_PAIRS
-__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) {
-    unsigned long long r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(f2_bits(a)), "l"(f2_bits(b)), "l"(f2_bits(c)));
-    return f2_from(r);
-}
-__device__ __forceinline__ f2 mul2(f2 a, f2 b) {
-    unsigned long long r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(f2_bits(a)), "l"(f2_bits(b)));
-    return f2_from(r);
-}
-#else
-__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { return f2{fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)}; }
-__device__ __forceinline__ f2 mul2(f2 a, f2 b) { return f2{a.x * b.x, a.y * b.y}; }
-#endif
+__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { return f2{__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)}; }
+__device__ __forceinline__ f2 mul2(f2 a, f2 b) { return f2{__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)}; }
 // a + b and a - b as one fused operation each (exact product, one rounding: the IEEE sum).
 __device__ __forceinline__ f2 add2(f2 a, f2 b) { return fma2(a, f2_splat(1.0f), b); }
 __device__ __forceinline__ f2 sub2(f2 a, f2 b) { return fma2(b, f2_splat(-1.0f), a); }
@@ -965,8 +946,8 @@ void launch_grad_setup(const StyleRec* styles, const StopRec* stops, uint32_t n_
     if (n_styles) grad_setup_kernel<<<(n_styles + 127) / 128, 128, 0, st>>>(styles, stops, n_styles, grads);
 }
 
-// Self-test of the packed fp32 arithmetic (forma_debug_selftest): every packed helper against
-// the scalar IEEE operation it stands for, on `n` operand triples. Returns mismatches in out[0].
+// Self-test of the pair arithmetic (forma_debug_selftest): every pair helper against the
+// scalar IEEE operation it stands for, on `n` operand triples. Returns mismatches in out[0].
 __global__ void f32x2_selftest_kernel(const float* __restrict__ a, const float* __restrict__ b, const float* __restrict__ c,
                                       uint32_t n, uint32_t* __restrict__ out) {
     const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) * 2u;

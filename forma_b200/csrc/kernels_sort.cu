@@ -19,8 +19,7 @@
 //   one upfront histogram kernel for all passes (every pass CTA scans its 256 counts itself), then one single-sweep
 //   ("onesweep") kernel per pass with decoupled look-back (16 B/key per pass;
 //   latency-bound at these sizes). A persistent single-sweep kernel for the large sorts
-//   was measured in round 1 (look-back-bound, 34 % of the HBM peak, profiles/r1_v2_*) and
-//   removed in favour of the reduce-then-scan passes.
+//   was measured look-back-bound and removed in favour of the reduce-then-scan passes.
 #include <mutex>
 #include "cuda_common.cuh"
 #include "kernels.h"
@@ -311,8 +310,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 // ---------------------------------------------------------------------------
 // Reduce-then-scan passes for large key-only sorts (the main pixel-segment
 // sort). The look-back of the single-sweep kernels above serialises the tiles
-// of a pass (measured: ~29 ns per 4096-key tile whatever the bandwidth, 34 % of
-// the HBM peak); here no CTA ever waits for another one:
+// of a pass whatever the bandwidth; here no CTA ever waits for another one:
 //   1. upsweep   — one CTA per tile counts the tile's digits     (reads  8 B/key)
 //   2. tile scan — counts -> exclusive global offsets per (tile, digit)
 //   3. downsweep — one CTA per tile ranks, stages in shared memory in digit
@@ -407,7 +405,7 @@ __global__ void __launch_bounds__(kRadix) radix_tile_scan_kernel(uint32_t* __res
 constexpr int kDsStages = 3;
 // 512 threads x 8 keys per 4096-key tile: the ranking chain per warp is short and an SM
 // holds 32 warps (2 CTAs, <= 64 registers) — a 256-thread x 16-key version measured
-// short-scoreboard / fixed-latency bound at 24 % occupancy (profiles/README.md, round 1).
+// short-scoreboard / fixed-latency bound at low occupancy.
 // Per-warp digit counters are u16 (a tile has 4096 keys) so that the shared memory still
 // fits twice per SM.
 constexpr int kWideThreads = 512;
@@ -541,8 +539,7 @@ __global__ void __launch_bounds__(kWideThreads, 2)
 static uint32_t tiles_for(uint32_t n, int items) { return (n + kSortThreads * items - 1) / (kSortThreads * items); }
 // Keys per thread: 4096-key tiles from 2^19 keys on (fewer tiles = a shorter look-back chain for
 // the single-sweep pair sorts, and the reduce-then-scan path for key-only sorts), 1024-key tiles
-// below that so that small sorts still spread over the SMs (option sort_big_log2, default 19:
-// 2^17 measured 4 % slower on paris@4K's 230 k-cell tables).
+// below that so that small sorts still spread over the SMs (option sort_big_log2, default 19).
 static int items_for(uint32_t n) { return n >= (1u << options().sort_big_log2) ? 16 : 4; }
 
 // scratch layout (u32 words): hist[6][256] | tile_counter[8] | lookback[6][tiles][256]
@@ -634,7 +631,7 @@ SortResult launch_radix_sort(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals,
     uint32_t* lookback = counters + 8;
     size_t total_words = (size_t)kMaxSortPasses * kRadix + 8 + (size_t)plan.n_passes * tiles * kRadix;
     cudaMemsetAsync(scratch, 0, total_words * sizeof(uint32_t), stream);
-    uint32_t hist_blocks = min(tiles_for(n, 16) * 4u, 148u * 8u);
+    uint32_t hist_blocks = min(tiles_for(n, 16) * 4u, (uint32_t)device_sm_count() * 8u);
     radix_hist_kernel<<<hist_blocks, kSortThreads, 0, stream>>>(keys, n, plan, hist, n_dev);
     res.launches = 1;
     if (vals) {

@@ -3,7 +3,7 @@
 //
 // Renderer::render follows forma/src/cpu/renderer.rs:75-224 stage by stage;
 // every stage is a CUDA kernel sequence on one stream, and there is no CPU
-// fallback: without a usable sm_100 device forma_renderer_new() fails.
+// fallback: without a usable sm_90 device forma_renderer_new() fails.
 #include <algorithm>
 #include <cctype>
 #include <condition_variable>
@@ -1703,8 +1703,8 @@ static forma_renderer* renderer_new_impl(int device_ordinal) {
         return nullptr;
     }
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device_ordinal) != cudaSuccess || prop.major != 10) {
-        set_error("device %d is sm_%d%d; this library is built for sm_100a only", device_ordinal, prop.major, prop.minor);
+    if (cudaGetDeviceProperties(&prop, device_ordinal) != cudaSuccess || prop.major != 9 || prop.minor != 0) {
+        set_error("device %d is sm_%d%d; this library is built for sm_90a only", device_ordinal, prop.major, prop.minor);
         return nullptr;
     }
     if (cudaSetDevice(device_ordinal) != cudaSuccess) {
@@ -2325,8 +2325,8 @@ int forma_get_option(const char* name, int* value) {
     return FORMA_ERR_INVALID_ARGUMENT;
 }
 
-// Packed-fp32 self-test (see kernels_painter.cu): random and special operands (zeros,
-// denormals, infinities, NaN, cancellation cases) through every packed helper of the painter.
+// Pixel-pair fp32 self-test (see kernels_painter.cu): random and special operands (zeros,
+// denormals, infinities, NaN, cancellation cases) through every pair helper of the painter.
 static int selftest_impl(int device, uint64_t* mismatches) {
     if (!mismatches) return FORMA_ERR_INVALID_ARGUMENT;
     FORMA_CUDA_TRY(cudaSetDevice(device));

@@ -1,5 +1,5 @@
 /*
- * forma_b200 — C ABI of the B200-native replacement for google/forma's
+ * forma_b200 — C ABI of the H100-native replacement for google/forma's
  * rendering hot path (flatten -> pixel-grid intersection -> 64-bit
  * pixel-segment sort -> per-tile paint).
  *
@@ -35,7 +35,7 @@ enum {
     FORMA_ERR_INVALID_ARGUMENT = 1, /* assert!/panic in the reference                     */
     FORMA_ERR_ORDER_LIMIT = 2,      /* OrderError::ExceededLayerLimit, utils/order.rs:56-65 */
     FORMA_ERR_CUDA = 3,             /* a CUDA call failed; see forma_last_error()          */
-    FORMA_ERR_NO_DEVICE = 4,        /* no usable sm_100 device: there is NO CPU fallback   */
+    FORMA_ERR_NO_DEVICE = 4,        /* no usable sm_90 device: there is NO CPU fallback    */
     FORMA_ERR_CAPACITY = 5          /* an internal device buffer could not be grown        */
 };
 
@@ -174,7 +174,7 @@ typedef struct forma_renderer forma_renderer;
 typedef struct forma_layer_cache forma_layer_cache;
 
 /* Renderer::new (:62). Binds to CUDA device `device_ordinal`. Returns NULL and
- * sets forma_last_error() when no sm_100 device is usable. */
+ * sets forma_last_error() when no sm_90 device is usable. */
 forma_renderer* forma_renderer_new(int device_ordinal);
 void forma_renderer_free(forma_renderer*);
 
@@ -214,7 +214,7 @@ void forma_renderer_set_stream(forma_renderer*, void* cuda_stream);
  * devices store their rows into it over NVLink; needs peer access). The frame is split into
  * bands of tile rows, one per device, rebalanced every frame on the previous frame's row
  * costs; each device keeps only its band's geometry resident. Layer caches are not
- * supported here (cache = NULL semantics). Every listed device must be an sm_100 GPU. */
+ * supported here (cache = NULL semantics). Every listed device must be an sm_90 GPU. */
 typedef struct forma_renderer_multi forma_renderer_multi;
 forma_renderer_multi* forma_renderer_multi_new(const int* device_ordinals, int n);
 void forma_renderer_multi_free(forma_renderer_multi*);
@@ -295,7 +295,7 @@ uint64_t forma_renderer_row_costs(forma_renderer*, uint64_t cap, uint64_t* out);
 int forma_set_option(const char* name, int value);
 int forma_get_option(const char* name, int* value);
 
-/* Device self-test of the painter's packed-fp32 (f32x2) arithmetic against the scalar IEEE
+/* Device self-test of the painter's pixel-pair fp32 arithmetic against the scalar IEEE
  * operations it stands for (2^20 operand triples incl. zeros, denormals, infinities, NaN);
  * *mismatches must come back 0. */
 int forma_debug_selftest(int device, uint64_t* mismatches);

@@ -1,5 +1,5 @@
-"""Model of the slab walk of paint_kernel<_, true> (forma_b200/csrc/kernels_painter.cu,
-profiles/r1_paint_kernel_analysis.md): walking a tile in eight two-column slabs with one
+"""Model of the slab walk of paint_kernel<_, true> (forma_b200/csrc/kernels_painter.cu
+of an earlier round): walking a tile in eight two-column slabs with one
 running cover per row — flat coverage left and right of the entry's segment columns — gives
 the coverage of every pixel that the reference's column sweep gives
 (cpu/painter/mod.rs:388-404: area(x, y) = 32 * sum of covers left of x + areas[x][y], covers

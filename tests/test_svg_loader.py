@@ -132,13 +132,18 @@ def test_picture_through_the_oracle(parsed, oracle_api):
 
 
 def test_committed_fixture_matches_the_source_file():
-    src = "/root/reference/assets/svgs/paris-30k.svg"
-    if not os.path.exists(src):
-        pytest.skip("the reference checkout is not present (GPU box)")
-    fresh = svg.parse_svg(src)
+    """tests/golden/paris30k_excerpt.svg is the source file with only every 1250th of its <path>
+    elements and the last one, each in its group (tests/golden/make_paris_fixture.py); parsed,
+    they are the same paths as in the fixture."""
     fixture = svg.PathList.load(os.path.join(ROOT, "tests", "data", "paris30k_paths.npz"))
-    for k in ("cmd", "pts", "cmd_off", "pt_off", "color", "fill_rule"):
-        assert np.array_equal(getattr(fresh, k), getattr(fixture, k)), k
+    fresh = svg.parse_svg(os.path.join(ROOT, "tests", "golden", "paris30k_excerpt.svg"))
+    picked = list(range(0, len(fixture) - 1, 1250)) + [len(fixture) - 1]
+    assert len(fixture) == 50620 and len(fresh) == len(picked)
+    for k, i in enumerate(picked):
+        for a, off in (("cmd", "cmd_off"), ("pts", "pt_off")):
+            f_off, x_off = getattr(fresh, off), getattr(fixture, off)
+            assert np.array_equal(getattr(fresh, a)[f_off[k]:f_off[k + 1]], getattr(fixture, a)[x_off[i]:x_off[i + 1]]), (a, i)
+        assert np.array_equal(fresh.color[k], fixture.color[i]) and fresh.fill_rule[k] == fixture.fill_rule[i], i
     assert len(fresh.weights) == 0 and not fresh.gradients
 
 

@@ -3,7 +3,7 @@
 #   GPU tests, smoke, the default bench line (with CPU baseline, frame check and the config-5 extra),
 #   the reference arm, the other workloads, ncu launch lists of the same commands and one
 #   `--set full` capture of the top kernels per workload.
-# Everything lands in gpurun_out/; tools/collect_profiles.py <tag> turns it into profiles/.
+# Everything lands in the scratch output directory made below.
 mkdir -p gpurun_out
 R=${1:-r2}
 python -m pytest tests -m gpu -q --timeout 600 2>&1 | tail -3 > gpurun_out/${R}_gpu_tests.txt
