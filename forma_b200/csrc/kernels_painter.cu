@@ -165,8 +165,8 @@ __device__ __forceinline__ void to_byte2(f2 v, uint32_t& b0, uint32_t& b1) {
     sc.x = d_clamp(sc.x, 0.0f, 255.0f);
     sc.y = d_clamp(sc.y, 0.0f, 255.0f);
     const f2 val = add2(sc, f2_splat(__uint_as_float(0x4B000000u)));
-    b0 = __float_as_uint(val.x) & 0xFFu;
-    b1 = __float_as_uint(val.y) & 0xFFu;
+    b0 = val.x != val.x ? 0u : __float_as_uint(val.x) & 0xFFu;  // NaN: see to_byte (paint_math.cuh)
+    b1 = val.y != val.y ? 0u : __float_as_uint(val.y) & 0xFFu;
 }
 
 __device__ __forceinline__ void store_tile_solid(const PaintScene& S, uint8_t* fb, uint32_t tx, uint32_t ty, uint32_t lane,

@@ -31,11 +31,15 @@ __device__ __forceinline__ float linear_to_srgb(float l) {
     return l <= 0.0031308f ? m : n;
 }
 
-// cpu/painter/mod.rs:135-143 (to_u32x8 + low byte)
+// cpu/painter/mod.rs:135-143 (to_u32x8 + low byte). A NaN channel (e.g. clip_color! dividing by
+// x - l = 0 for a colour outside [0, 1]) passes the clamp, and its byte is the low byte of the
+// NaN's bits. On the CPUs the reference runs on, arithmetic produces the default NaN (x86
+// 0xFFC00000, Arm 0x7FC00000) and propagates its payload, so the byte is 0; the GPU's canonical
+// NaN 0x7FFFFFFF would give 255.
 __device__ __forceinline__ uint32_t to_byte(float v) {
     float scaled = d_clamp(v * 255.0f, 0.0f, 255.0f);
     float val = scaled + __uint_as_float(0x4B000000u);
-    return __float_as_uint(val) & 0xFFu;
+    return val != val ? 0u : __float_as_uint(val) & 0xFFu;
 }
 
 __device__ __forceinline__ float channel_of(const Rgba& c, uint32_t ch) {  // cpu/painter/styling.rs:46-55
