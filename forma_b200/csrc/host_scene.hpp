@@ -154,6 +154,7 @@ class Composition {
     // (stable) sort only needs the tile_x / tile_y digits.
     bool layers_in_order = false;
     int64_t tables_cache_id = -2;     // cache id the `unchanged` bits were uploaded for
+    int rebuild_tables(int64_t cache_id);  // FORMA_STATUS_*
 
    private:
     void set_order(Layer* l, int64_t order);

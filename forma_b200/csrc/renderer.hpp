@@ -1,0 +1,284 @@
+// forma_b200 — the per-device Renderer (renderer.cu) and the C ABI objects that c_abi.cu and
+// multi_renderer.cu share.
+#pragma once
+
+#include <algorithm>
+#include <exception>
+
+#include "../../include/forma_b200.h"
+#include "host_scene.hpp"
+#include "kernels.h"
+
+namespace forma {
+
+// ---------------------------------------------------------------------------
+// Renderer
+// ---------------------------------------------------------------------------
+// BufferLayerCache (cpu/buffer/mod.rs:114-197). The per-tile records live on the
+// device (the painter reads and updates them); the host only keeps the size and
+// clear colour of the last frame.
+struct LayerCache {
+    uint8_t id = 0;
+    DeviceBuffer<uint2> tiles;  // CachedTile per tile, see PaintScene::cache_tiles
+    bool has_size = false;
+    uint64_t width = 0, height = 0;
+    bool has_clear = false;
+    float clear_color[4] = {0, 0, 0, 0};
+    bool needs_reset = true;  // the tile records must be zeroed before their next use
+    void clear() {            // BufferLayerCache::clear, mod.rs:189-196
+        has_clear = false;
+        needs_reset = true;
+    }
+};
+
+struct Timer {
+    cudaEvent_t ev[8];
+    cudaEvent_t sort_ev[3 * kMaxSortPasses];  // main sort, per pass: before upsweep, before / after downsweep
+    bool ok = false;
+};
+
+class Renderer {
+   public:
+    int device = 0;
+    int res_key = 0;  // key of this renderer's residency record in a Composition: the device ordinal, or
+                      // device + 4096 * (k + 1) for the k-th slice renderer of a host-frame pipeline
+    int copy_bands_override = 0;  // slice renderers: copy bands inside the slice (0 = option copy_bands)
+    cudaStream_t stream = 0;
+    bool owns_stream = false;
+    uint64_t launches = 0;
+    uint32_t caches_in_use = 0;
+    Timer timer;
+
+    // Per-frame device scratch (high-water-mark allocations).
+    DeviceBuffer<uint32_t> block_sums, totals;
+    DeviceBuffer<unsigned long long> scan_state;
+    SortPlan segment_plan{};  // digits of the main sort, from the bounds seen by the line-setup pass
+
+    template <class T>
+    static void swap_buffers(DeviceBuffer<T>& a, DeviceBuffer<T>& b) {
+        std::swap(a.ptr, b.ptr);
+        std::swap(a.capacity, b.capacity);
+    }
+    // launch_radix_sort of keys (+ vals, may be null) with sort_scratch; the sorted data ends up
+    // in keys / vals: the buffers trade places with their twins when it landed there.
+    SortResult sort(DeviceBuffer<uint64_t>& keys, DeviceBuffer<uint64_t>& keys_tmp, DeviceBuffer<uint32_t>* vals,
+                    DeviceBuffer<uint32_t>* vals_tmp, uint32_t n, const SortPlan& plan, cudaEvent_t* pass_events = nullptr,
+                    const uint32_t* n_dev = nullptr);
+    DeviceBuffer<uint64_t> segs, segs_tmp;
+    DeviceBuffer<uint8_t> sort_scratch;
+    DeviceBuffer<uint32_t> cell_start, perm, perm_tmp, gap_count, eid, eid_tmp, gid_tmp, heavy_tiles;
+    DeviceBuffer<uint2> tile_range;
+    DeviceBuffer<uint64_t> cell_key, key2, key2_tmp, ekey, ekey_tmp, gkey_tmp;
+    DeviceBuffer<uint4> cell_cover, carry_in, carry_after, gap_carry;
+    DeviceBuffer<uint8_t> eflags, framebuffer;
+    DeviceBuffer<EntryRec> recs;
+    // The painter-table scratch by the count that sizes it (see build_tables): per cell, per
+    // carry-only entry, per entry. n + 1 per cell and per carry-only entry: the cells pass writes
+    // its outputs below cap - 1, and the pair sorts need a slack slot.
+    template <class... B>
+    static cudaError_t reserve_all(size_t n, B&... bufs) {
+        cudaError_t e = cudaSuccess;
+        ((e = e != cudaSuccess ? e : bufs.reserve(n)), ...);
+        return e;
+    }
+    cudaError_t reserve_cell_tables(size_t n_cells) {
+        return reserve_all(n_cells + 1, cell_start, cell_key, cell_cover, carry_in, carry_after, key2, key2_tmp, perm, perm_tmp,
+                           gap_count);
+    }
+    cudaError_t reserve_gap_tables(size_t n_gaps) { return reserve_all(n_gaps + 1, ekey_tmp, eid_tmp, gkey_tmp, gid_tmp, gap_carry); }
+    cudaError_t reserve_entry_tables(size_t n_entries) { return reserve_all(n_entries, ekey, eid, eflags, recs); }
+    // Band-wise copy-back of host frames (see render()).
+    static constexpr uint32_t kMaxCopyBands = 16;
+    uint32_t copy_bands() const {
+        return (uint32_t)std::min(std::max(copy_bands_override ? copy_bands_override : options().copy_bands, 1), (int)kMaxCopyBands);
+    }
+    cudaStream_t aux_stream = nullptr;  // side stream of the geometry upload (see flush_geometry)
+    cudaEvent_t aux_ev[2];
+    cudaStream_t band_stream[kMaxCopyBands];
+    uint32_t band_streams_made = 0;  // created as needed: streams beyond the device's hardware queues alias onto them
+    bool band_streams_ok = false;    // the band events exist
+    cudaEvent_t band_ev[kMaxCopyBands + 1];
+    cudaEvent_t count_ev = nullptr;  // completion of a count read-back (waited on instead of the whole stream)
+    cudaError_t ensure_count_event() {
+        return count_ev ? cudaSuccess : cudaEventCreateWithFlags(&count_ev, cudaEventDisableTiming);
+    }
+    static bool speculation_enabled() { return options().speculate != 0; }
+    static size_t test_gap_cap_override() { return (size_t)std::max(options().test_gap_cap, 0); }
+    static bool band_copies_enabled() { return options().band_copy != 0; }
+    // Layer-cache frames: per-slot `is_unchanged` flags, the list of written
+    // tiles and their packed pixels (only these travel back to a host buffer).
+    DeviceBuffer<uint8_t> d_unchanged;
+    PinnedBuffer<uint8_t> h_unchanged;
+    DeviceBuffer<uint32_t> written_list, packed_tiles;
+    PinnedBuffer<uint32_t> h_written_list, h_packed_tiles;
+    uint32_t last_written_tiles = 0;
+    // Upload staging.
+    DeviceBuffer<QuadUp> up_quads_raw;  // as uploaded; expanded into up_quads on the device
+    DeviceBuffer<SplineRec> up_splines;
+    DeviceBuffer<PointRec> up_points;
+    DeviceBuffer<uint8_t> up_kinds;
+    DeviceBuffer<QuadRec> up_quads;
+    DeviceBuffer<FlattenJob> up_jobs;
+    DeviceBuffer<JobXf> up_xfs;
+
+    uint32_t last_segments = 0, last_cells = 0, last_entries = 0, last_gaps = 0;
+    bool last_tables_sync_free = false, last_tables_redone = false;  // how the last frame's painter tables were built
+    uint32_t last_tiles_x = 0, last_tiles_y = 0;  // tile grid of the last render (forma_renderer_row_costs)
+    RasterArgs last_raster{};        // line-setup arguments of the last render (device pointers owned by its composition)
+    bool last_raster_valid = false;
+    uint64_t h2d_bytes = 0, d2h_bytes = 0;  // bytes copied over PCIe since creation
+    double stage_ms[8] = {0};               // see forma_renderer_stage_times (valid after resolve_times)
+    double kernel_ms[4] = {0};              // see forma_renderer_kernel_times
+    uint32_t kernel_launches[4] = {0};
+    bool times_pending = false;             // the last render's events have not been turned into stage_ms / kernel_ms yet
+    int pending_sort_passes = 0;
+    uint32_t pending_paint_launches = 0;
+    void resolve_times() {
+        if (!times_pending || !timer.ok) return;
+        times_pending = false;
+        cudaSetDevice(device);
+        auto el = [&](int a, int b) {
+            float ms = 0;
+            cudaEventElapsedTime(&ms, timer.ev[a], timer.ev[b]);
+            return (double)ms;
+        };
+        stage_ms[0] = el(0, 7);  // uploads (geometry programs + flatten eval + tables)
+        stage_ms[1] = el(7, 1);  // line setup: count pass + scan (+ count read-back)
+        stage_ms[2] = el(1, 2);  // pixel-grid intersection (emit)
+        stage_ms[3] = el(2, 3);  // sort (upsweep / tile scan / downsweep per digit), no host sync inside
+        stage_ms[4] = el(3, 4);  // painter tables: cells, carries, entries (2 pair sorts)
+        stage_ms[5] = el(4, 5);  // paint kernel alone (host frames: its band launches)
+        stage_ms[6] = el(5, 6);  // device -> host copy of the framebuffer
+        stage_ms[7] = el(0, 6);  // whole call on the device timeline
+        kernel_ms[0] = kernel_ms[1] = 0;
+        for (int p = 0; p < pending_sort_passes; ++p) {
+            float a = 0, b = 0;
+            cudaEventElapsedTime(&a, timer.sort_ev[3 * p], timer.sort_ev[3 * p + 1]);
+            cudaEventElapsedTime(&b, timer.sort_ev[3 * p + 1], timer.sort_ev[3 * p + 2]);
+            kernel_ms[1] += a;  // upsweep + tile scan
+            kernel_ms[0] += b;  // downsweep
+        }
+        kernel_launches[0] = kernel_launches[1] = (uint32_t)pending_sort_passes;
+        kernel_ms[2] = stage_ms[5];
+        kernel_launches[2] = pending_paint_launches;
+    }
+    uint32_t* pinned_totals = nullptr;  // 4 x u32 pinned host words for count read-backs
+    // Renderers of a multi-device / sliced frame: the per-row costs of the frame (see
+    // row_cost_kernel) travel back behind the frame itself, without a synchronisation of their own.
+    bool track_row_costs = false;
+    DeviceBuffer<unsigned long long> d_row_costs;
+    PinnedBuffer<unsigned long long> h_row_costs;
+    uint32_t row_costs_rows = 0;  // rows of h_row_costs that belong to the last render (0 = none)
+    uint32_t last_slices = 0;     // slices of the last host frame (0 = rendered as one piece)
+    // Slice renderers of a host-frame pipeline: the uploads of the slices are issued by one thread,
+    // slice after slice, and chained (a slice's copies wait for the previous slice's), so that slice k
+    // has its geometry - and starts computing - while slices k + 1 ... are still crossing PCIe.
+    cudaEvent_t upload_done_ev = nullptr;  // recorded behind this renderer's last host -> device copy
+    cudaEvent_t upload_after = nullptr;    // this renderer's copies wait for it (the previous slice's upload_done_ev)
+    bool prefetched = false;               // prefetch() ran for the coming render: timer.ev[0] is already recorded
+    int prefetch(Composition& comp, uint64_t width, uint64_t height, const forma_rect* crop);
+    int ensure_timer() {
+        if (!timer.ok) {
+            for (auto& e : timer.ev) FORMA_CUDA_TRY(cudaEventCreate(&e));
+            for (auto& e : timer.sort_ev) FORMA_CUDA_TRY(cudaEventCreate(&e));
+            timer.ok = true;
+        }
+        return FORMA_STATUS_OK;
+    }
+
+    ~Renderer() {
+        if (pinned_totals) cudaFreeHost(pinned_totals);
+        if (count_ev) cudaEventDestroy(count_ev);
+        if (upload_done_ev) cudaEventDestroy(upload_done_ev);
+        if (band_streams_ok)
+            for (auto& e : band_ev) cudaEventDestroy(e);
+        for (uint32_t k = 0; k < band_streams_made; ++k) cudaStreamDestroy(band_stream[k]);
+        if (timer.ok) {
+            for (auto& e : timer.ev) cudaEventDestroy(e);
+            for (auto& e : timer.sort_ev) cudaEventDestroy(e);
+        }
+        if (aux_stream) {
+            cudaEventDestroy(aux_ev[0]);
+            cudaEventDestroy(aux_ev[1]);
+            cudaStreamDestroy(aux_stream);
+        }
+        if (owns_stream && stream) cudaStreamDestroy(stream);
+    }
+
+    int flush_geometry(Composition& comp, float band_lo = 0.0f, float band_hi = 0.0f, bool band_is_partial = false);
+    int upload_tables(Composition& comp, int64_t cache_id);
+    int upload_tables_device(Composition& comp, CompDevice& cd);
+    int rasterize(Composition& comp, uint32_t width, uint32_t height, float band_lo, float band_hi, uint32_t* n_out);
+    int render(Composition& comp, uint8_t* buffer, bool buffer_on_device, uint64_t width, uint64_t stride,
+               uint64_t height, const uint32_t channels[4], const float clear[4], const forma_rect* crop,
+               LayerCache* cache, forma_timings* timings);
+    // The stages of render(), in the order it runs them.
+    int begin_frame(PaintScene& S, const uint8_t* buffer, uint64_t width, uint64_t stride, uint64_t height,
+                    const uint32_t channels[4], const float clear[4], const forma_rect* crop);
+    int bind_frame(Composition& comp, PaintScene& S, LayerCache* cache, const float clear[4], bool pack_written);
+    int build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint32_t prev_cells, uint32_t prev_gaps, uint32_t* n_entries,
+                     DevCounts& dc);
+    int index_tiles(const PaintScene& S, uint32_t n, uint32_t n_entries, const DevCounts& dc, uint32_t* heavy_lists);
+    int paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t stride, bool in_bands, const uint32_t* heavy_lists,
+              uint32_t* paint_launches);
+    int copy_to_host(const PaintScene& S, uint8_t* buffer, const uint8_t* fb, uint64_t stride, cudaStream_t s);
+    int scatter_written_tiles(const PaintScene& S, const uint8_t* fb, uint8_t* buffer, uint64_t stride);
+};
+
+// Rect::new (renderer.rs:43-52): the tile columns and rows [lo, hi) a crop covers (the whole
+// frame without one).
+struct TileRect {
+    uint32_t tx_lo, tx_hi, ty_lo, ty_hi;
+};
+inline TileRect tile_rect(uint64_t width, uint64_t height, const forma_rect* crop) {
+    const uint32_t tiles_x = (uint32_t)((width + 15u) / 16u), tiles_y = (uint32_t)((height + 15u) / 16u);
+    TileRect t{0, tiles_x, 0, tiles_y};
+    if (crop) {
+        t.tx_lo = (uint32_t)std::min<uint64_t>(crop->hor_start / 16u, tiles_x);
+        t.tx_hi = (uint32_t)std::min<uint64_t>((crop->hor_end + 15u) / 16u, tiles_x);
+        t.ty_lo = (uint32_t)std::min<uint64_t>(crop->vert_start / 16u, tiles_y);
+        t.ty_hi = (uint32_t)std::min<uint64_t>((crop->vert_end + 15u) / 16u, tiles_y);
+        if (t.tx_hi < t.tx_lo) t.tx_hi = t.tx_lo;
+        if (t.ty_hi < t.ty_lo) t.ty_hi = t.ty_lo;
+    }
+    return t;
+}
+
+QuadUp quad_upload(const QuadRec& q);
+
+
+// No C++ exception crosses the C ABI: a failed host allocation (std::bad_alloc
+// from the containers behind these calls) is reported through the call's error
+// value and forma_last_error() like any other failure.
+template <class R, class F>
+static R guarded(R on_error, F&& f) noexcept {
+    try {
+        return f();
+    } catch (const std::exception& e) {
+        set_error("host error: %s", e.what());
+    } catch (...) {
+        set_error("host error: unknown exception");
+    }
+    return on_error;
+}
+template <class F>
+static void guarded_void(F&& f) noexcept {
+    guarded(0, [&] { f(); return 0; });
+}
+
+}  // namespace forma
+
+struct forma_composition { forma::Composition c; };
+struct forma_renderer {
+    forma::Renderer r;
+    // Host-frame pipeline (forma_renderer_render): slice renderers on this renderer's device,
+    // created at the first frame that is sliced.
+    forma_renderer_multi* slicer = nullptr;
+    ~forma_renderer() { forma_renderer_multi_free(slicer); }
+};
+
+// Host-frame pipeline (multi_renderer.cu): returns -1 when the frame is
+// not sliced and the plain path has to render it.
+int sliced_host_render(forma_renderer* r, forma_composition* c, uint8_t* buffer, uint64_t width, uint64_t stride,
+                       uint64_t height, const uint32_t channels[4], const float clear[4], const forma_rect* crop,
+                       forma_timings* timings);
