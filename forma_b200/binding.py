@@ -250,6 +250,8 @@ SIGNATURES = {
     "path_free": (None, [_vp]),
     "path_segments": (C.c_int, [_vp, C.POINTER(_fp), C.POINTER(_fp), C.POINTER(_u8p), _u64p]),
     "path_program_stats": (None, [_vp, _u64p]),
+    "path_program_records": (None, [_vp, C.POINTER(_vp), _u64p, C.POINTER(_vp), C.POINTER(_u8p), _u64p, C.POINTER(_vp),
+                                    _u64p, C.POINTER(C.c_int), _fp]),
     "composition_new": (_vp, []),
     "composition_free": (None, [_vp]),
     "composition_create_layer": (_vp, [_vp]),
@@ -379,6 +381,16 @@ class SharedFrame:
             self.ptr = 0
 
 
+# Flatten-program records (forma_b200/csrc/device_types.h), as Path.program() returns them.
+SPLINE_REC = np.dtype([("p0x", "<f4"), ("p0y", "<f4"), ("p2x", "<f4"), ("p2y", "<f4"), ("step", "<f4"),
+                       ("first_quad", "<u4"), ("n_quads", "<u4"), ("first_point", "<u4"), ("info", "<u4")])
+POINT_REC = np.dtype([("a", "<f4"), ("b", "<f4")])  # kind 2 / 3: a holds the quad index's bits
+QUAD_REC = np.dtype([("px", "<f4", 3), ("py", "<f4", 3), ("pw", "<f4", 3), ("x0", "<f4"), ("dx_recip", "<f4"),
+                     ("k0", "<f4"), ("dk", "<f4"), ("curv_recip", "<f4"), ("prev_curv", "<f4"), ("total", "<f4"),
+                     ("step", "<f4")])
+assert (SPLINE_REC.itemsize, POINT_REC.itemsize, QUAD_REC.itemsize) == (36, 8, 68)
+
+
 def _np_f32(ptr, n):
     return np.ctypeslib.as_array(ptr, shape=(n,)).copy() if n else np.zeros(0, np.float32)
 
@@ -398,6 +410,32 @@ class Path:
         out = (C.c_uint64 * 6)()
         self._api.path_program_stats(self._h, out)
         return dict(zip(("points", "quads", "splines", "point_records", "rational", "contour_ends"), [int(v) for v in out]))
+
+    def program(self) -> dict:
+        """The flatten program's records as the host built them (CUDA library only; needs no
+        GPU; inspection only): structured arrays "splines" (SPLINE_REC), "points" (POINT_REC),
+        "kinds" (uint8 per point record), "quads" (QUAD_REC), plus "bounded" and "bounds"
+        (min x, min y, max x, max y) and the program_stats() facts under "stats"."""
+        a = self._api
+        sp, pp, qp, kp = _vp(), _vp(), _vp(), _u8p()
+        ns, nr, nq, bounded = C.c_uint64(), C.c_uint64(), C.c_uint64(), C.c_int()
+        bounds = (C.c_float * 4)()
+        a.path_program_records(self._h, C.byref(sp), C.byref(ns), C.byref(pp), C.byref(kp), C.byref(nr), C.byref(qp),
+                               C.byref(nq), C.byref(bounded), bounds)
+
+        def records(ptr, n, dtype):
+            if n == 0:
+                return np.zeros(0, dtype)
+            return np.frombuffer(C.string_at(ptr.value, n * dtype.itemsize), dtype).copy()
+        return {
+            "splines": records(sp, ns.value, SPLINE_REC),
+            "points": records(pp, nr.value, POINT_REC),
+            "kinds": np.ctypeslib.as_array(kp, shape=(nr.value,)).copy() if nr.value else np.zeros(0, np.uint8),
+            "quads": records(qp, nq.value, QUAD_REC),
+            "bounded": bool(bounded.value),
+            "bounds": np.array(list(bounds), np.float32),
+            "stats": self.program_stats(),
+        }
 
     def segments(self):
         """Flattened points: (x, y, start_new_contour) numpy arrays."""

@@ -65,6 +65,24 @@ void forma_path_program_stats(forma_path* p, uint64_t out[6]) {
     out[5] = prog.n_contour_ends;
 }
 
+void forma_path_program_records(forma_path* p, const void** splines, uint64_t* n_splines, const void** points,
+                                const uint8_t** kinds, uint64_t* n_records, const void** quads, uint64_t* n_quads,
+                                int* bounded, float bounds[4]) {
+    const FlattenProgram& prog = p->p.data->program();
+    *splines = prog.splines.data();
+    *n_splines = prog.splines.size();
+    *points = prog.points.data();
+    *kinds = prog.kinds.data();
+    *n_records = prog.points.size();
+    *quads = prog.quads.data();
+    *n_quads = prog.quads.size();
+    *bounded = prog.bounded ? 1 : 0;
+    bounds[0] = prog.min_x;
+    bounds[1] = prog.min_y;
+    bounds[2] = prog.max_x;
+    bounds[3] = prog.max_y;
+}
+
 // Evaluates the path's flatten program on the current device and copies the
 // points back (inspection only; rendering never copies points to the host).
 static int path_segments_impl(forma_path* p, const float** x, const float** y, const uint8_t** contour, uint64_t* n) {

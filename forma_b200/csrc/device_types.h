@@ -41,6 +41,9 @@ struct QuadUpPoly {
 //   kind 0: literal point (a, b)                  (Start / End of a spline)
 //   kind 1: literal point (a, b), ends a contour  (End with new_contour)
 //   kind 2: a = quad index (u32 bits), b = pi; evaluated at quad.step * pi
+//   kind 3: a = quad index (u32 bits), b = fma(step, pi, -quad.prev_curv) with the step of the
+//           spline being walked, which need not be the quad's own (programs whose quad walk
+//           falls behind, see host_path.cpp)
 struct PointRec {
     float a, b;
 };

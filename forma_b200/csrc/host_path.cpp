@@ -61,6 +61,15 @@ uint64_t to_count(float v) {  // Rust `as usize`: saturating, NaN -> 0
     return (uint64_t)v;
 }
 
+// The first evaluated point pi in 1..last whose (float)pi exceeds the running curvature t
+// (where the reference's walk leaves the quad of total t behind); last + 1 if none does.
+uint64_t first_point_above(float t, uint64_t last) {
+    if (!(t < (float)last)) return last + 1;
+    uint64_t m = to_count(t) + 1;
+    while (!((float)m > t)) ++m;  // at most half an ulp of t (t < 2^30) steps
+    return m;
+}
+
 // Serial spline builder (path.rs:190-445). Splines are kept only as long as
 // needed to emit their point commands at the end.
 class SplineBuilder {
@@ -139,14 +148,20 @@ class SplineBuilder {
         out.quads = std::move(quads_);
         for (const QuadRec& q : out.quads)
             if (q.pw[0] != 1.0f || q.pw[1] != 1.0f || q.pw[2] != 1.0f) out.rational = true;
-        // The quads of a spline are contiguous; the reference walks them with
-        // `if pi > total[qi] { qi += 1 }` per evaluated point (path.rs:424-431), which
-        // — every quad adding more than 1 to the running curvature (path.rs:322-332) —
-        // is "the first quad whose running curvature reaches pi": the kernel
-        // (flatten_eval_kernel) finds it by bisection, no per-point command needed.
+        // The quads of a spline are contiguous; the reference walks them with one index for the
+        // whole path: `if pi > total[qi] { qi += 1 }` per evaluated point, and `qi += 1` after
+        // every spline with subdivisions (path.rs:424-445). While every quad raises the running
+        // curvature by more than 1 (path.rs:322-332), that is "the first quad of the spline whose
+        // running curvature reaches pi": the kernel (flatten_eval_kernel) finds it by bisection,
+        // no per-point command needed. In f32 it is not always so: past 2^25 a quad can add
+        // nothing (less than half an ulp, or a tie rounded to even), and from 2^23 on a quad can
+        // add exactly 1. The walk then lags behind the bisection, or ends a spline before its
+        // last quad and evaluates the next spline's points on this spline's quads. A program
+        // where that happens records the walk point by point (`walk_lags`, kind 3 below).
         std::vector<uint32_t> quads_of(splines_.size(), 0u);
         for (uint32_t si : quad_spline_) quads_of[si] += 1;
         out.splines.reserve(splines_.size());
+        bool walk_lags = false;
         uint64_t qi = 0, pt = 0;
         for (size_t si = 0; si < splines_.size(); ++si) {
             const Spline& s = splines_[si];
@@ -165,6 +180,15 @@ class SplineBuilder {
             r.info = (uint32_t)evaluated | (start ? 1u << 30 : 0u) | (s.ends_contour ? 1u << 31 : 0u);
             out.splines.push_back(r);
             for (uint32_t q = 0; q < quads_of[si]; ++q) out.quads[qi + q].step = step;
+            // The walk keeps up with the bisection iff the evaluated points cross the quads' running
+            // curvatures one quad at a time and reach the last quad: each quad but the last is left
+            // behind at its own point.
+            uint64_t crossed = 0;
+            for (uint32_t q = 0; q + 1 < quads_of[si] && !walk_lags; ++q) {
+                uint64_t p = first_point_above(out.quads[qi + q].total, evaluated);
+                walk_lags = p > evaluated || p <= crossed;
+                crossed = p;
+            }
             pt += (start ? 1u : 0u) + evaluated + 1u;
             qi += quads_of[si];
             if (s.ends_contour && si + 1 < splines_.size()) out.n_contour_ends += 1;
@@ -191,9 +215,11 @@ class SplineBuilder {
         }
         // Paths made of short line splines are smaller point by point (9 B / point
         // against 36 B / spline): expand the records on the host in that case.
-        if (sizeof(SplineRec) * out.splines.size() > (sizeof(PointRec) + 1) * (size_t)out.n_points && pt < (1ull << 31)) {
+        if ((walk_lags || sizeof(SplineRec) * out.splines.size() > (sizeof(PointRec) + 1) * (size_t)out.n_points) &&
+            pt < (1ull << 31)) {
             out.points.reserve(out.n_points);
             out.kinds.reserve(out.n_points);
+            uint32_t wq = 0;  // the reference's walk; it stays within the quads of the spline being walked
             for (const SplineRec& r : out.splines) {
                 if ((r.info >> 30) & 1u) {
                     out.points.push_back({r.p0x, r.p0y});
@@ -202,13 +228,21 @@ class SplineBuilder {
                 const uint32_t evaluated = r.info & kSplineEvalMask;
                 uint32_t q = r.first_quad;
                 for (uint32_t pi = 1; pi <= evaluated; ++pi) {
-                    while (q + 1 < r.first_quad + r.n_quads && (float)pi > out.quads[q].total) ++q;
                     PointRec p;
-                    std::memcpy(&p.a, &q, sizeof(uint32_t));
-                    p.b = (float)pi;
+                    if (walk_lags) {
+                        if ((float)pi > out.quads[wq].total) ++wq;
+                        std::memcpy(&p.a, &wq, sizeof(uint32_t));
+                        p.b = fmaf(r.step, (float)pi, -out.quads[wq].prev_curv);
+                        out.kinds.push_back(3);
+                    } else {
+                        while (q + 1 < r.first_quad + r.n_quads && (float)pi > out.quads[q].total) ++q;
+                        std::memcpy(&p.a, &q, sizeof(uint32_t));
+                        p.b = (float)pi;
+                        out.kinds.push_back(2);
+                    }
                     out.points.push_back(p);
-                    out.kinds.push_back(2);
                 }
+                if (r.n_quads) ++wq;  // a spline with quads has subdivisions
                 out.points.push_back({r.p2x, r.p2y});
                 out.kinds.push_back((r.info >> 31) ? 1 : 0);
             }

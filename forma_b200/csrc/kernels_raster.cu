@@ -104,13 +104,13 @@ __global__ void flatten_eval_kernel(const SplineRec* __restrict__ splines, const
     const FlattenJob job = jobs[lo];
     const uint32_t local = i - job.first_point;
     const uint32_t count = (lo + 1u < n_jobs ? jobs[lo + 1u].first_point : n_points) - job.first_point;
-    uint32_t kind;  // 0 literal, 1 literal + contour end, 2 evaluated
+    uint32_t kind;  // 0 literal, 1 literal + contour end, 2 evaluated, 3 evaluated, pi holds fma(step, pi, -prev_curv)
     float px = 0.0f, py = 0.0f, pi = 0.0f;
     const QuadRec* qp = nullptr;
     if (job.n_splines == 0u) {  // point encoding
         const PointRec p = points[job.spline_base + local];
         kind = kinds[job.spline_base + local];
-        if (kind == 2u) {
+        if (kind >= 2u) {
             qp = quads + job.quad_base + __float_as_uint(p.a);
             pi = p.b;
         } else {
@@ -150,10 +150,10 @@ __global__ void flatten_eval_kernel(const SplineRec* __restrict__ splines, const
             qp = qs + a;
         }
     }
-    if (kind == 2u) {
+    if (kind >= 2u) {
         const QuadRec q = *qp;
         // path.rs:515-522
-        float ratio = fmaf(q.step, pi, -q.prev_curv) * q.curv_recip;
+        float ratio = (kind == 2u ? fmaf(q.step, pi, -q.prev_curv) : pi) * q.curv_recip;
         float xx = inv_curvature(fmaf(ratio, q.dk, q.k0));
         float t = d_clamp((xx - q.x0) * q.dx_recip, 0.0f, 1.0f);
         // eval_quad, path.rs:447-471

@@ -135,6 +135,15 @@ int forma_path_segments(forma_path*, const float** x, const float** y,
  * is 0: the smaller encoding is kept), [4] 1 if some quadratic is rational,
  * [5] contour ends before the last point. */
 void forma_path_program_stats(forma_path*, uint64_t out[6]);
+/* Inspection only (tests): the records of the path's flatten program as the host built
+ * them, with the layouts of csrc/device_types.h: SplineRec (36 B), PointRec (8 B) with one
+ * kind byte per record, QuadRec (68 B). One of n_splines / n_records is 0. bounds = min x,
+ * min y, max x, max y of every point the program can emit; *bounded is 0 when no such bound
+ * exists (a weight that is not positive). Host only: no device, no upload. The pointers stay
+ * valid while the path (or a path transformed from it that shares its data) lives. */
+void forma_path_program_records(forma_path*, const void** splines, uint64_t* n_splines, const void** points,
+                                const uint8_t** kinds, uint64_t* n_records, const void** quads, uint64_t* n_quads,
+                                int* bounded, float bounds[4]);
 
 /* ------------------------------------------------------------------------ */
 /* Composition / Layer (forma/src/composition/{mod,layer}.rs)               */

@@ -27,7 +27,7 @@ def build(force: bool = False) -> str:
 def load() -> binding.Api:
     lib = C.CDLL(build())
     api = binding.Api(lib, "fo_", optional=("renderer_render_device", "renderer_stage_times", "renderer_counters", "renderer_host_slices", "renderer_kernel_times", "renderer_set_stream", "path_program_stats",
-                                        "shared_frame_create", "shared_frame_open", "shared_frame_close", "shared_frame_free",
+                                        "path_program_records", "shared_frame_create", "shared_frame_open", "shared_frame_close", "shared_frame_free",
                                         "composition_evict", "composition_point_count", "set_option", "get_option", "debug_selftest", "renderer_row_costs", "renderer_multi_new", "renderer_multi_free", "renderer_multi_device_count",
                                         "renderer_multi_render", "renderer_multi_render_device", "renderer_multi_bands"))
     _declare_hooks(lib)

@@ -19,7 +19,7 @@ from forma_b200.binding import RGBA, Color
 import oracle.oracle as O
 import synth, scenes
 OPT = ("renderer_render_device", "renderer_stage_times", "renderer_counters", "renderer_kernel_times", "renderer_set_stream", "path_program_stats",
-       "shared_frame_create", "shared_frame_open", "shared_frame_close", "shared_frame_free", "composition_evict", "composition_point_count")
+       "path_program_records", "shared_frame_create", "shared_frame_open", "shared_frame_close", "shared_frame_free", "composition_evict", "composition_point_count")
 new = O.load()
 rev = sys.argv[1]
 tmp = tempfile.mkdtemp()
