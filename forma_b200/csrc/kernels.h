@@ -66,12 +66,6 @@ void launch_raster_emit(const RasterArgs& args, const uint32_t* block_offsets, u
 // f = {x0, y0, dx, dy, a, b, c, d}, then the per-line segment counts.
 void launch_line_records(const RasterArgs& args, uint32_t n, uint32_t* orders, float* const f[8], uint32_t* lengths,
                          cudaStream_t stream);
-// In-place exclusive scan of n u32 values; total[0] = sum. `state` (scan_state_words(n)
-// u64 words) enables the multi-CTA look-back scan for large n; nullptr = one CTA.
-size_t scan_state_words(uint32_t n);
-// `n_dev` (optional): the element count in device memory, `n` then being its upper bound.
-void launch_scan_u32(uint32_t* data, uint32_t n, uint32_t* total, unsigned long long* state, cudaStream_t stream,
-                     const uint32_t* n_dev = nullptr);
 
 // ---- kernels_sort.cu --------------------------------------------------------
 // LSD radix sort of u64 keys on bits [kSortShift, 64) (+ optional u32 payload).
@@ -102,17 +96,34 @@ struct SortPlan {
 };
 // bound[f] = largest value field f (least significant first) takes in any key.
 SortPlan make_sort_plan(const KeyLayout& layout, const uint64_t bound[3]);
+#ifdef __CUDACC__
+__device__ __forceinline__ uint32_t digit_of(uint64_t key, const DigitSpec& d) {
+    uint32_t v = (uint32_t)(key >> d.shift[0]) & ((1u << d.width[0]) - 1u);  // lsh[0] == 0
+    if (d.width[1] != 0u) {  // uniform: most digits are a single bit run
+        v |= ((uint32_t)(key >> d.shift[1]) & ((1u << d.width[1]) - 1u)) << d.lsh[1];
+        v |= ((uint32_t)(key >> d.shift[2]) & ((1u << d.width[2]) - 1u)) << d.lsh[2];
+    }
+    return v;
+}
+#endif
 struct SortResult {
     int launches;
     bool in_tmp;  // the sorted data is in keys_tmp / vals_tmp (odd number of passes)
     int timed_passes = 0;  // passes whose kernels were bracketed by pass_events
 };
 size_t radix_scratch_bytes(uint32_t n);
+// Scratch of a sort whose digit histogram comes from the kernel that wrote its keys (see
+// launch_radix_sort's `hist`): tile counters and look-back tables of the single-sweep passes.
+size_t sort_lookback_bytes(uint32_t n, const SortPlan& plan);
 SortResult launch_radix_sort(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals, uint32_t* vals_tmp, uint32_t n,
                              const SortPlan& plan, void* scratch, cudaStream_t stream,
                              cudaEvent_t* pass_events = nullptr /* 3 per pass: before upsweep, before / after downsweep */,
                              const uint32_t* n_dev = nullptr /* the key count in device memory; `n` is then its upper bound
-                                                                (single-sweep passes only) */);
+                                                                and a larger count sorts nothing (single-sweep passes only) */,
+                             const uint32_t* hist = nullptr /* [kMaxSortPasses][256] digit counts of every planned pass,
+                                                               counted by the keys' producer: the sort then launches its
+                                                               passes only, and `scratch` holds sort_lookback_bytes(n, plan)
+                                                               bytes zeroed by the caller */);
 
 // ---- kernels_paint.cu -------------------------------------------------------
 struct PaintScene {
@@ -138,19 +149,34 @@ struct PaintScene {
 };
 
 uint32_t cell_num_blocks(uint32_t n);
+// Plans of the painter's two pair sorts (their key bounds are host-known).
+SortPlan carry_sort_plan(const PaintScene& S);
+SortPlan gap_sort_plan(const PaintScene& S);
+// The painter tables' scratch: one block that is zeroed before the tables of a frame are built
+// (byte offsets; every region starts 256-byte aligned). n = segments; n_cells / n_gaps: the
+// counts (or bounds) that size the carry sort / carry pass and the gap sort.
+struct TableScratch {
+    size_t heavy_count;  // kHeavyListClasses u32: lengths of the heavy-tile lists (read by the painter)
+    size_t carry_hist;   // [kMaxSortPasses][256] u32: digit counts of the carry sort (cells pass)
+    size_t gap_hist;     // [kMaxSortPasses][256] u32: digit counts of the gap sort (carry pass)
+    size_t cells_state;  // cells pass look-back
+    size_t carry_sort;   // carry sort tile counters + look-back tables
+    size_t carry_pass;   // carry pass look-back (carries, gap offsets) + ticket
+    size_t gap_sort;     // gap sort tile counters + look-back tables
+    size_t end;
+};
+TableScratch table_scratch_layout(uint32_t n, uint32_t n_cells, uint32_t n_gaps, const SortPlan& carry_plan,
+                                  const SortPlan& gap_plan);
 // Cells in one pass over the sorted segments (+ a small kernel for the cells that cross a
 // CTA tile): cell_start[c] = first segment of cell c (cell_start[#cells] = n), the cell's
 // cover (16 x i8 by local_y), its key, the (tile_y, layer, tile_x) key of the carry pass and
 // perm[c] = c, for every c < cap - 1; n_cells_out[0] = #cells. All five arrays need `cap`
-// entries. `state`: cells_state_words(n) u64 words. May be launched before the host knows the
-// count; the caller repeats it if #cells >= cap.
-size_t cells_state_words(uint32_t n);
-void launch_cells(const PaintScene& S, const uint64_t* segs, uint32_t n, unsigned long long* state, uint32_t* cell_start,
-                  uint32_t cap, uint32_t* n_cells_out, uint64_t* cell_key, uint4* cell_cover, uint64_t* key2, uint32_t* perm,
-                  cudaStream_t st);
-// Plans of the painter's two pair sorts (their key bounds are host-known).
-SortPlan carry_sort_plan(const PaintScene& S);
-SortPlan gap_sort_plan(const PaintScene& S);
+// entries. The digits of every written carry-pass key are added to `carry_hist` ([passes][256]
+// of `carry_plan`). `scratch`: the zeroed table scratch (cells_state). May be launched before the
+// host knows the count; the caller repeats it if #cells >= cap.
+void launch_cells(const PaintScene& S, const uint64_t* segs, uint32_t n, uint8_t* scratch, const TableScratch& L,
+                  const SortPlan& carry_plan, uint32_t* cell_start, uint32_t cap, uint32_t* n_cells_out, uint64_t* cell_key,
+                  uint4* cell_cover, uint64_t* key2, uint32_t* perm, cudaStream_t st);
 // Cell / carry-only-entry counts that stay on the device (frames whose tables are built without a
 // host read-back, Options::sync_free): with `cells` set, the n_cells / n_gaps arguments of the
 // launchers below are upper bounds (grid sizes) and the kernels read the counts here; a count
@@ -160,15 +186,15 @@ struct DevCounts {
     const uint32_t* gaps = nullptr;
     uint32_t cell_bound = 0, gap_bound = 0;
 };
-void launch_carry_scan(const PaintScene& S, const uint64_t* key2, const uint32_t* perm, const uint4* cell_cover,
-                       uint32_t n_cells, uint4* carry_in, uint4* carry_after, uint32_t* gap_count, cudaStream_t st,
+// One pass over the carry-sorted cells: the carry-in of every cell (carry_in, by cell id) and the
+// carry-only entries in (layer, tile_y, tile_x) order: key, payload n_cells + entry id, carried
+// cover. Entries at positions >= cap are not written; n_gaps_out[0] = their exact count. The
+// digits of every written key are added to `gap_hist` ([passes][256] of `gap_plan`). `scratch`:
+// the zeroed table scratch (carry_pass).
+void launch_carry_pass(const PaintScene& S, const uint64_t* key2, const uint32_t* perm, const uint4* cell_cover,
+                       uint32_t n_cells, uint8_t* scratch, const TableScratch& L, const SortPlan& gap_plan, uint4* carry_in,
+                       uint64_t* gkey, uint32_t* gid, uint4* gap_carry, uint32_t cap, uint32_t* n_gaps_out, cudaStream_t st,
                        const DevCounts& dc = DevCounts());
-// Carry-only entries in (layer, tile_y, tile_x) order; payload = n_cells + gap id.
-void launch_gap_fill(const PaintScene& S, const uint64_t* key2, const uint32_t* perm, const uint64_t* cell_key,
-                     const uint4* carry_after, const uint32_t* gap_offset /* scanned gap counts */, uint32_t n_cells,
-                     uint64_t* gkey, uint32_t* gid, uint4* gap_carry, const uint32_t* n_gaps_ptr, uint32_t cap,
-                     uint32_t grid_gaps /* threads to launch: >= the entry count */, cudaStream_t st,
-                     const DevCounts& dc = DevCounts());
 // One painter entry = one (tile, layer) pair with segments and / or a carried cover.
 struct EntryRec {  // 64 B
     uint32_t layer, seg0, seg1;  // layer order; [seg0, seg1) in the sorted segments (empty for carry-only entries)
@@ -181,17 +207,16 @@ struct EntryRec {  // 64 B
     uint32_t pad;
 };
 // Merges the cells with the sorted carry-only entries: ekey, entry records and
-// initial flags of the n_cells + n_gaps entries, ordered by (tile_y, tile_x, layer).
+// initial flags of the n_cells + n_gaps entries, ordered by (tile_y, tile_x, layer), and
+// the per-tile entry ranges (tile_range: zeroed by the caller, left zero for tiles without
+// entries) and, when `heavy` is not null, the lists of tiles with many entries:
+// kHeavyListClasses arrays of tiles_x * tiles_y ids each, their lengths in
+// heavy_count[kHeavyListClasses] (zeroed by the caller).
+constexpr int kHeavyListClasses = 4;
 void launch_merge_entries(const PaintScene& S, const uint64_t* cell_key, uint32_t n_cells, const uint64_t* gkey,
                           const uint32_t* gid, uint32_t n_gaps, const uint32_t* cell_start, const uint4* carry_in,
-                          const uint4* gap_carry, uint64_t* ekey, EntryRec* recs, uint8_t* eflags, cudaStream_t st,
-                          const DevCounts& dc = DevCounts());
-// Per-tile entry ranges (zero for tiles without entries) and, when `heavy` is not null, the
-// lists of tiles with many entries: kHeavyListClasses arrays of tiles_x * tiles_y ids each,
-// their lengths in heavy_count[kHeavyListClasses] (both written here).
-constexpr int kHeavyListClasses = 4;
-void launch_tile_index(const PaintScene& S, const uint64_t* ekey, uint32_t n_entries, uint2* tile_range, uint32_t* heavy,
-                       uint32_t* heavy_count, cudaStream_t st, const DevCounts& dc = DevCounts());
+                          const uint4* gap_carry, uint64_t* ekey, EntryRec* recs, uint8_t* eflags, uint2* tile_range,
+                          uint32_t* heavy, uint32_t* heavy_count, cudaStream_t st, const DevCounts& dc = DevCounts());
 void launch_paint(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range, const uint32_t* heavy,
                   const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st);
 // GradRec of every style slot (see device_types.h).

@@ -301,9 +301,7 @@ __global__ void __launch_bounds__(kRasterThreads) line_count_kernel(RasterArgs A
 // of the producing kernel, a few thousand); writes the grand total to
 // total[0]. 1024 threads, each owning a contiguous chunk.
 __global__ void __launch_bounds__(1024) scan_block_sums_kernel(uint32_t* __restrict__ data, uint32_t n,
-                                                              uint32_t* __restrict__ total,
-                                                              const uint32_t* __restrict__ n_dev = nullptr) {
-    if (n_dev) n = min(n, *n_dev);
+                                                              uint32_t* __restrict__ total) {
     __shared__ uint32_t warp_tot[32];
     __shared__ uint32_t carry, round_total;
     if (threadIdx.x == 0) carry = 0;
@@ -493,98 +491,6 @@ void launch_raster_emit(const RasterArgs& args, const uint32_t* block_offsets, u
     uint32_t nb = raster_num_blocks(args.n_points);
     if (!nb) return;
     raster_emit_kernel<<<nb, kRasterThreads, 0, stream>>>(args, block_offsets, out, cap);
-}
-
-// Multi-CTA exclusive scan (single pass, decoupled look-back): CTA = 2048
-// values; state[t] = flag (2 bits) | running value (62 bits); state[tiles] is the
-// ticket counter. `state` must hold scan_state_words(n) zeroed u64 words.
-constexpr int kScanThreads = 256, kScanItems = 8, kScanTile = kScanThreads * kScanItems;
-constexpr unsigned long long kScanAggregate = 1ull << 62, kScanInclusive = 2ull << 62, kScanFlags = 3ull << 62;
-
-__global__ void __launch_bounds__(kScanThreads) chained_scan_kernel(uint32_t* __restrict__ data, uint32_t n,
-                                                                  unsigned long long* __restrict__ state, uint32_t tiles,
-                                                                  uint32_t* __restrict__ total,
-                                                                  const uint32_t* __restrict__ n_dev) {
-    if (n_dev) n = min(n, *n_dev);  // elements past the device-side count read as 0; every tile still takes part
-    __shared__ uint32_t warp_tot[kScanThreads / 32];
-    __shared__ uint32_t s_tile;
-    __shared__ unsigned long long s_prefix;
-    const uint32_t t = threadIdx.x, lane = t & 31u, warp = t >> 5;
-    if (t == 0) s_tile = (uint32_t)atomicAdd(&state[tiles], 1ull);
-    __syncthreads();
-    const uint32_t tile = s_tile;
-    const uint32_t base = tile * kScanTile + warp * (32u * kScanItems);
-    // Warp-striped: item i of lane l is element base + i*32 + l.
-    uint32_t v[kScanItems], excl[kScanItems];
-    uint32_t running = 0;
-#pragma unroll
-    for (int i = 0; i < kScanItems; ++i) {
-        uint32_t idx = base + i * 32u + lane;
-        v[i] = idx < n ? data[idx] : 0u;
-        uint32_t incl = warp_inclusive_scan(v[i]);
-        excl[i] = running + incl - v[i];
-        running += __shfl_sync(kFullMask, incl, 31);
-    }
-    if (lane == 0) warp_tot[warp] = running;
-    __syncthreads();
-    uint32_t warp_off = 0, tile_sum = 0;
-#pragma unroll
-    for (int w = 0; w < kScanThreads / 32; ++w) {
-        if ((uint32_t)w < warp) warp_off += warp_tot[w];
-        tile_sum += warp_tot[w];
-    }
-    if (warp == 0) {  // decoupled look-back, 32 predecessors per round
-        volatile unsigned long long* st = state;
-        unsigned long long prefix = 0;
-        if (tile == 0) {
-            if (lane == 0) st[0] = kScanInclusive | tile_sum;
-        } else {
-            if (lane == 0) st[tile] = kScanAggregate | tile_sum;
-            int32_t p = (int32_t)tile - 1;
-            while (true) {
-                const int32_t idx = p - (int32_t)lane;
-                unsigned long long v = kScanInclusive;
-                if (idx >= 0) {
-                    do {
-                        v = st[idx];
-                    } while ((v & kScanFlags) == 0);
-                }
-                const uint32_t incl = __ballot_sync(kFullMask, (v & kScanFlags) == kScanInclusive);
-                const uint32_t upto = incl ? (uint32_t)__ffs((int)incl) : 32u;
-                unsigned long long part = lane < upto ? (v & ~kScanFlags) : 0ull;
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(kFullMask, part, o);
-                prefix += part;
-                if (incl) break;
-                p -= 32;
-            }
-            if (lane == 0) st[tile] = kScanInclusive | (prefix + tile_sum);
-        }
-        if (lane == 0) {
-            s_prefix = prefix;
-            if (tile + 1 == tiles) total[0] = (uint32_t)(prefix + tile_sum);
-        }
-    }
-    __syncthreads();
-    const uint32_t add = (uint32_t)s_prefix + warp_off;
-#pragma unroll
-    for (int i = 0; i < kScanItems; ++i) {
-        uint32_t idx = base + i * 32u + lane;
-        if (idx < n) data[idx] = add + excl[i];
-    }
-}
-
-size_t scan_state_words(uint32_t n) { return (size_t)(n + kScanTile - 1) / kScanTile + 2; }
-
-void launch_scan_u32(uint32_t* data, uint32_t n, uint32_t* total, unsigned long long* state, cudaStream_t stream,
-                     const uint32_t* n_dev) {
-    if (n <= 16384u || !state) {
-        scan_block_sums_kernel<<<1, 1024, 0, stream>>>(data, n, total, n_dev);
-        return;
-    }
-    uint32_t tiles = (n + kScanTile - 1) / kScanTile;
-    cudaMemsetAsync(state, 0, (tiles + 1) * sizeof(unsigned long long), stream);
-    chained_scan_kernel<<<tiles, kScanThreads, 0, stream>>>(data, n, state, tiles, total, n_dev);
 }
 
 }  // namespace forma

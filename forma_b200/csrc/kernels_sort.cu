@@ -16,7 +16,8 @@
 //   staging in shared memory, coalesced scatter): 24 B/key per pass, and no CTA
 //   ever waits for another one (see the comment above those kernels).
 // * Small sorts and (key, u32 payload) pairs (the painter's cell / gap tables):
-//   one upfront histogram kernel for all passes (every pass CTA scans its 256 counts itself), then one single-sweep
+//   one upfront histogram kernel for all passes, or none when the kernel that wrote the keys
+//   counted their digits (every pass CTA scans its 256 counts itself), then one single-sweep
 //   ("onesweep") kernel per pass with decoupled look-back (16 B/key per pass;
 //   latency-bound at these sizes). A persistent single-sweep kernel for the large sorts
 //   was measured look-back-bound and removed in favour of the reduce-then-scan passes.
@@ -38,15 +39,6 @@ constexpr uint32_t kFlagAggregate = 1u << 30;
 constexpr uint32_t kFlagInclusive = 2u << 30;
 constexpr uint32_t kFlagMask = 3u << 30;
 constexpr uint32_t kValueMask = ~kFlagMask;
-
-__device__ __forceinline__ uint32_t digit_of(uint64_t key, const DigitSpec& d) {
-    uint32_t v = (uint32_t)(key >> d.shift[0]) & ((1u << d.width[0]) - 1u);  // lsh[0] == 0
-    if (d.width[1] != 0u) {  // uniform: most digits are a single bit run
-        v |= ((uint32_t)(key >> d.shift[1]) & ((1u << d.width[1]) - 1u)) << d.lsh[1];
-        v |= ((uint32_t)(key >> d.shift[2]) & ((1u << d.width[2]) - 1u)) << d.lsh[2];
-    }
-    return v;
-}
 
 __device__ __forceinline__ uint32_t ld_relaxed(const uint32_t* p) {
     uint32_t v;
@@ -102,13 +94,20 @@ SortPlan make_sort_plan(const KeyLayout& layout, const uint64_t bound[3]) {
     return plan;
 }
 
-// Counts every digit of every planned pass in one read of the keys.
 // `n_dev` (optional): the key count in device memory; `n` is then only its upper bound (the
-// count may not be known on the host when the sort is launched, see Renderer::render).
+// count may not be known on the host when the sort is launched, see Renderer::build_tables). A
+// count above the bound means that the producer overflowed its buffers: nothing is sorted.
+__device__ __forceinline__ uint32_t resolve_key_count(uint32_t n, const uint32_t* __restrict__ n_dev) {
+    if (!n_dev) return n;
+    const uint32_t c = *n_dev;
+    return c > n ? 0u : c;
+}
+
+// Counts every digit of every planned pass in one read of the keys.
 __global__ void __launch_bounds__(kSortThreads) radix_hist_kernel(const uint64_t* __restrict__ keys, uint32_t n, SortPlan plan,
                                                                 uint32_t* __restrict__ hist /*[passes][256]*/,
                                                                 const uint32_t* __restrict__ n_dev) {
-    if (n_dev) n = min(n, *n_dev);
+    n = resolve_key_count(n, n_dev);
     __shared__ uint32_t s_hist[kMaxSortPasses][kRadix];
     for (int i = threadIdx.x; i < kMaxSortPasses * kRadix; i += kSortThreads) (&s_hist[0][0])[i] = 0;
     __syncthreads();
@@ -134,7 +133,7 @@ __global__ void __launch_bounds__(kSortThreads, kItems == 16 ? 3 : 6)
                          const uint32_t* __restrict__ digit_counts /*[256]: keys per digit (radix_hist_kernel)*/,
                          uint32_t* __restrict__ lb /*[tiles][256], zeroed*/, uint32_t* __restrict__ tile_counter,
                          const uint32_t* __restrict__ n_dev) {
-    if (n_dev) n = min(n, *n_dev);
+    n = resolve_key_count(n, n_dev);
     constexpr int kTileKeys = kSortThreads * kItems;
     __shared__ uint64_t s_keys[kTileKeys];
     __shared__ uint32_t s_warp_hist[kSortWarps][kRadix];
@@ -549,6 +548,10 @@ size_t radix_scratch_bytes(uint32_t n) {
     size_t scan_words = (size_t)kMaxSortPasses * kTotalsRows * kRadix + (size_t)tiles_for(n, kDsItems) * kRadix;
     return (words > scan_words ? words : scan_words) * sizeof(uint32_t) + 256;
 }
+// With the histogram counted elsewhere: tile_counter[8] | lookback[passes][tiles][256].
+size_t sort_lookback_bytes(uint32_t n, const SortPlan& plan) {
+    return (8 + (size_t)plan.n_passes * tiles_for(n, items_for(n)) * kRadix) * sizeof(uint32_t);
+}
 
 template <bool kPairs, int kItems>
 static void launch_passes(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals, uint32_t* vals_tmp, uint32_t n,
@@ -575,12 +578,12 @@ static void launch_passes(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals, ui
 
 SortResult launch_radix_sort(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals, uint32_t* vals_tmp, uint32_t n,
                              const SortPlan& plan, void* scratch, cudaStream_t stream, cudaEvent_t* pass_events,
-                             const uint32_t* n_dev) {
+                             const uint32_t* n_dev, const uint32_t* hist_ready) {
     SortResult res{0, false};
     if (n < 2 || plan.n_passes == 0) return res;
     const int items = items_for(n);
     const uint32_t tiles = tiles_for(n, items);
-    if (!vals && items == 16 && n >= (1u << options().sort_scan_log2) && !n_dev) {
+    if (!vals && items == 16 && n >= (1u << options().sort_scan_log2) && !n_dev && !hist_ready) {
         // Persistent TMA-staged downsweep: 2 CTAs per SM (per-device attribute + grid).
         static int wide_grids[kMaxDevices];
         static bool ds_configured[kMaxDevices] = {false};
@@ -626,14 +629,19 @@ SortResult launch_radix_sort(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals,
         }
         // (occupancy query failed: fall through to the single-sweep passes)
     }
-    uint32_t* hist = static_cast<uint32_t*>(scratch);
-    uint32_t* counters = hist + kMaxSortPasses * kRadix;
+    const uint32_t* hist = hist_ready;
+    uint32_t* counters = static_cast<uint32_t*>(scratch);
+    if (!hist_ready) {
+        uint32_t* h = static_cast<uint32_t*>(scratch);
+        counters = h + kMaxSortPasses * kRadix;
+        size_t total_words = (size_t)kMaxSortPasses * kRadix + 8 + (size_t)plan.n_passes * tiles * kRadix;
+        cudaMemsetAsync(scratch, 0, total_words * sizeof(uint32_t), stream);
+        uint32_t hist_blocks = min(tiles_for(n, 16) * 4u, (uint32_t)device_sm_count() * 8u);
+        radix_hist_kernel<<<hist_blocks, kSortThreads, 0, stream>>>(keys, n, plan, h, n_dev);
+        res.launches = 1;
+        hist = h;
+    }
     uint32_t* lookback = counters + 8;
-    size_t total_words = (size_t)kMaxSortPasses * kRadix + 8 + (size_t)plan.n_passes * tiles * kRadix;
-    cudaMemsetAsync(scratch, 0, total_words * sizeof(uint32_t), stream);
-    uint32_t hist_blocks = min(tiles_for(n, 16) * 4u, (uint32_t)device_sm_count() * 8u);
-    radix_hist_kernel<<<hist_blocks, kSortThreads, 0, stream>>>(keys, n, plan, hist, n_dev);
-    res.launches = 1;
     if (vals) {
         if (items == 16) launch_passes<true, 16>(keys, keys_tmp, vals, vals_tmp, n, plan, hist, lookback, counters, tiles, stream, n_dev);
         else launch_passes<true, 4>(keys, keys_tmp, vals, vals_tmp, n, plan, hist, lookback, counters, tiles, stream, n_dev);

@@ -10,12 +10,14 @@
 //             (cells_scan: one pass, head bits -> cell_start by decoupled look-back)
 //   covers    per cell: sum of segment covers by local_y (wrapping i8), its key (same pass)
 //   re-sort   cell ids stably by the layer bits only -> (layer, tile_y, tile_x)
+//             (digit counts from the cells pass)
 //   carries   per (tile_y, layer) group a running sum -> carry-in of every cell
 //             and "carry-only" entries for the tiles a layer spans without
 //             segments (layer_workbench/mod.rs:213-234,328-336), generated in
-//             that order and stably sorted by the tile digits only
+//             that order (carry_pass: segmented scan, decoupled look-back) and
+//             stably sorted by the tile digits only (digit counts from the carry pass)
 //   entries   cells merged with the carry-only entries by rank into 64-byte
-//             records ordered by (tile_y, tile_x, layer), + per-tile ranges
+//             records ordered by (tile_y, tile_x, layer), + per-tile ranges (same pass)
 //   paint     kernels_painter.cu: one warp per tile
 //
 // Integer semantics: areas wrap at i16 and covers at i8 in the reference;
@@ -55,9 +57,10 @@ constexpr int kCellTile = kCellThreads * kCellItems;
 constexpr unsigned long long kCellAggregate = 1ull << 62, kCellInclusive = 2ull << 62, kCellFlags = 3ull << 62;
 constexpr uint32_t kCellSlots = 512;  // cells accumulated per round (a tile with more takes several rounds)
 
-__device__ __forceinline__ void write_cell_records(const PaintScene& S, uint32_t c, uint64_t first_seg, const int32_t* acc16,
-                                                   uint64_t* __restrict__ cell_key, uint4* __restrict__ cell_cover,
-                                                   uint64_t* __restrict__ key2, uint32_t* __restrict__ perm) {
+// Returns the carry-pass key written.
+__device__ __forceinline__ uint64_t write_cell_records(const PaintScene& S, uint32_t c, uint64_t first_seg, const int32_t* acc16,
+                                                       uint64_t* __restrict__ cell_key, uint4* __restrict__ cell_cover,
+                                                       uint64_t* __restrict__ key2, uint32_t* __restrict__ perm) {
     uint32_t w[4];
 #pragma unroll
     for (int q = 0; q < 4; ++q)
@@ -69,21 +72,43 @@ __device__ __forceinline__ void write_cell_records(const PaintScene& S, uint32_t
     const bool relevant = !(ty < (int32_t)S.ty_lo || ty >= (int32_t)S.ty_hi || tx >= (int32_t)S.tx_hi);
     perm[c] = c;
     cell_cover[c] = make_uint4(w[0], w[1], w[2], w[3]);
-    key2[c] = relevant ? make_key2(ck) : sentinel_key(S.tiles_y);
+    const uint64_t k2 = relevant ? make_key2(ck) : sentinel_key(S.tiles_y);
+    key2[c] = k2;
+    return k2;
+}
+
+// Digit counts of a pair sort, gathered by the kernel that writes its keys: per CTA in shared
+// memory, added to the global histogram once at the end.
+__device__ __forceinline__ void hist_clear(uint32_t (*s_hist)[256], uint32_t passes) {
+    for (uint32_t i = threadIdx.x; i < passes * 256u; i += blockDim.x) (&s_hist[0][0])[i] = 0;
+}
+__device__ __forceinline__ void hist_count(uint32_t* hist /* [passes][256], shared or global */, const SortPlan& plan,
+                                           uint64_t key) {
+#pragma unroll
+    for (uint32_t p = 0; p < (uint32_t)kMaxSortPasses; ++p)  // unrolled: the plan stays in registers
+        if (p < plan.n_passes) atomicAdd(&hist[p * 256u + digit_of(key, plan.pass[p])], 1u);
+}
+__device__ __forceinline__ void hist_flush(const uint32_t (*s_hist)[256], uint32_t passes, uint32_t* __restrict__ hist) {
+    for (uint32_t i = threadIdx.x; i < passes * 256u; i += blockDim.x) {
+        const uint32_t v = (&s_hist[0][0])[i];
+        if (v) atomicAdd(&hist[i], v);
+    }
 }
 
 __global__ void __launch_bounds__(kCellThreads)
     cells_kernel(PaintScene S, const uint64_t* __restrict__ segs, uint32_t n, unsigned long long* __restrict__ state,
                  uint32_t tiles, uint32_t* __restrict__ cell_start, uint32_t cap, uint32_t* __restrict__ n_cells_out,
                  uint64_t* __restrict__ cell_key, uint4* __restrict__ cell_cover, uint64_t* __restrict__ key2,
-                 uint32_t* __restrict__ perm) {
+                 uint32_t* __restrict__ perm, SortPlan plan, uint32_t* __restrict__ hist) {
     __shared__ uint32_t warp_cnt[kCellThreads / 32];
     __shared__ uint32_t s_tile;
     __shared__ unsigned long long s_prefix;
     __shared__ int32_t s_acc[kCellSlots][16];
     __shared__ uint64_t s_first[kCellSlots];  // first segment of the cell in each slot
+    __shared__ uint32_t s_hist[kMaxSortPasses][256];
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
     if (threadIdx.x == 0) s_tile = (uint32_t)atomicAdd(&state[tiles], 1ull);
+    hist_clear(s_hist, plan.n_passes);
     __syncthreads();
     const uint32_t tile = s_tile;
     const uint32_t tile_base = tile * kCellTile;
@@ -206,10 +231,11 @@ __global__ void __launch_bounds__(kCellThreads)
         if (r0) accumulate(r0, nr);  // a tile with more than kCellSlots cells: further rounds
         for (uint32_t sl = threadIdx.x; sl < nr; sl += kCellThreads) {
             const uint32_t c = cells_before + r0 + sl;
-            if (c < cap) write_cell_records(S, c, s_first[sl], s_acc[sl], cell_key, cell_cover, key2, perm);
+            if (c < cap) hist_count(&s_hist[0][0], plan, write_cell_records(S, c, s_first[sl], s_acc[sl], cell_key, cell_cover, key2, perm));
         }
         __syncthreads();
     }
+    hist_flush(s_hist, plan.n_passes, hist);
 }
 
 // The cells that cross a tile boundary of cells_kernel: one warp per boundary b (between
@@ -220,7 +246,7 @@ __global__ void __launch_bounds__(kCellThreads)
     cells_boundary_kernel(PaintScene S, const uint64_t* __restrict__ segs, uint32_t n, const unsigned long long* __restrict__ state,
                           uint32_t tiles, const uint32_t* __restrict__ cell_start, uint32_t cap,
                           const uint32_t* __restrict__ n_cells_ptr, uint64_t* __restrict__ cell_key, uint4* __restrict__ cell_cover,
-                          uint64_t* __restrict__ key2, uint32_t* __restrict__ perm) {
+                          uint64_t* __restrict__ key2, uint32_t* __restrict__ perm, SortPlan plan, uint32_t* __restrict__ hist) {
     const uint32_t b = blockIdx.x * (kCellThreads / 32) + (threadIdx.x >> 5) + 1u, lane = threadIdx.x & 31u;
     if (b >= tiles) return;
     const uint32_t n_cells = *n_cells_ptr;
@@ -247,7 +273,8 @@ __global__ void __launch_bounds__(kCellThreads)
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) acc[r] += __shfl_xor_sync(kFullMask, acc[r], o);
     }
-    if (lane == 0) write_cell_records(S, c, segs[s0], acc, cell_key, cell_cover, key2, perm);
+    if (lane == 0)  // at most one cell per boundary: straight into the global histogram
+        hist_count(hist, plan, write_cell_records(S, c, segs[s0], acc, cell_key, cell_cover, key2, perm));
 }
 
 // ---------------------------------------------------------------------------
@@ -270,39 +297,217 @@ __device__ __forceinline__ void resolve_counts(const DevCounts& dc, uint32_t& n_
     n_gaps = ok ? g : 0u;
 }
 
-// One thread per (tile_y, layer) group head walks its group (cells sorted by
-// tile_x), producing each cell's carry-in, the running carry after it and the
-// number of carry-only entries to create before the next cell.
-__global__ void carry_scan_kernel(PaintScene S, const uint64_t* __restrict__ key2, const uint32_t* __restrict__ perm,
-                                  const uint4* __restrict__ cell_cover, uint32_t n_cells, uint4* __restrict__ carry_in,
-                                  uint4* __restrict__ carry_after, uint32_t* __restrict__ gap_count, DevCounts dc) {
+// The carry pass: one thread per cell in carry order ((layer, tile_y, tile_x) after the carry
+// sort; a (tile_y, layer) group is a run of equal key2 >> 32), CTA tiles of kCarryThreads cells
+// taken by ticket. Per cell:
+//   1. its carry-in: the wrapping 16 x i8 sum of the covers of the cells before it in its group
+//      (a segmented scan: inside the CTA by shuffles, across CTAs by decoupled look-back),
+//   2. the number of carry-only entries between it and the next cell of the group: the tiles
+//      a layer spans without segments while its running cover is not empty
+//      (layer_workbench/mod.rs:213-234,328-336),
+//   3. their exclusive offset (a second look-back over the counts), and the entries themselves,
+//      written by the cell's warp together: key, payload n_cells + entry id and carried cover.
+// The entries come out in (layer, tile_y, tile_x) order: a stable sort on the tile digits alone
+// then orders them by (tile_y, tile_x, layer).
+// 1024-cell tiles: the CTAs of a frame's carry pass look back at about the same time, so the
+// last tile's look-back walks up to tiles / 32 windows of predecessors; a quarter as many tiles
+// as with 256-cell tiles (paris@4K: 225).
+constexpr int kCarryThreads = 1024;
+constexpr int kCarryWarps = kCarryThreads / 32;
+constexpr uint32_t kCarryAggregate = 1u, kCarryInclusive = 2u;  // carry flag words (0: not published yet)
+constexpr unsigned long long kGapAggregate = 1ull << 62, kGapInclusive = 2ull << 62, kGapFlags = 3ull << 62;
+
+// State per CTA tile: the published cover and its flag word (a 128-bit cover cannot be published
+// with the flag in one atomic store: payload first, then the flag with release semantics) and the
+// gap-count word (flag | running count, one 64-bit word); then the ticket counter.
+struct CarryPassState {
+    uint4* aggregate;   // segmented sum of the tile: its cells after its last group head (all of them without a head)
+    uint4* inclusive;   // running cover after the tile's last cell
+    uint32_t* flag;     // kCarryAggregate / kCarryInclusive
+    unsigned long long* gaps;
+    uint32_t* ticket;
+};
+__host__ __device__ inline size_t carry_pass_state_bytes(uint32_t tiles) { return (size_t)tiles * (16 + 16 + 8 + 4) + 16; }
+__host__ __device__ inline CarryPassState carry_pass_state(uint8_t* base, uint32_t tiles) {
+    CarryPassState s;
+    s.aggregate = reinterpret_cast<uint4*>(base);
+    s.inclusive = s.aggregate + tiles;
+    s.gaps = reinterpret_cast<unsigned long long*>(s.inclusive + tiles);
+    s.flag = reinterpret_cast<uint32_t*>(s.gaps + tiles);
+    s.ticket = s.flag + tiles;
+    return s;
+}
+inline uint32_t carry_pass_tiles(uint32_t n_cells) { return (n_cells + kCarryThreads - 1) / kCarryThreads; }
+
+__device__ __forceinline__ uint32_t ld_acquire(const uint32_t* p) {
+    uint32_t v;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_release(uint32_t* p, uint32_t v) {
+    asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint4 ld_relaxed_v4(const uint4* p) {
+    uint4 v;
+    asm volatile("ld.relaxed.gpu.global.v4.u32 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
+                 : "l"(p)
+                 : "memory");
+    return v;
+}
+__device__ __forceinline__ uint4 shfl_cover(uint4 v, int src) {
+    return make_uint4(__shfl_sync(kFullMask, v.x, src), __shfl_sync(kFullMask, v.y, src), __shfl_sync(kFullMask, v.z, src),
+                      __shfl_sync(kFullMask, v.w, src));
+}
+__device__ __forceinline__ uint4 shfl_up_cover(uint4 v, unsigned d) {
+    return make_uint4(__shfl_up_sync(kFullMask, v.x, d), __shfl_up_sync(kFullMask, v.y, d), __shfl_up_sync(kFullMask, v.z, d),
+                      __shfl_up_sync(kFullMask, v.w, d));
+}
+__device__ __forceinline__ uint4 shfl_xor_cover(uint4 v, int m) {
+    return make_uint4(__shfl_xor_sync(kFullMask, v.x, m), __shfl_xor_sync(kFullMask, v.y, m), __shfl_xor_sync(kFullMask, v.z, m),
+                      __shfl_xor_sync(kFullMask, v.w, m));
+}
+
+__global__ void __launch_bounds__(kCarryThreads)
+    carry_pass_kernel(PaintScene S, const uint64_t* __restrict__ key2, const uint32_t* __restrict__ perm,
+                      const uint4* __restrict__ cell_cover, uint32_t n_cells, uint8_t* __restrict__ state_base, uint32_t tiles,
+                      uint4* __restrict__ carry_in, uint64_t* __restrict__ gkey, uint32_t* __restrict__ gid,
+                      uint4* __restrict__ gap_carry, uint32_t cap, uint32_t* __restrict__ n_gaps_out, SortPlan plan,
+                      uint32_t* __restrict__ hist, DevCounts dc) {
+    __shared__ uint32_t s_tile;
+    __shared__ uint4 s_warp_cover[kCarryWarps];
+    __shared__ uint32_t s_warp_head[kCarryWarps];
+    __shared__ uint32_t s_warp_gaps[kCarryWarps];
+    __shared__ uint4 s_carry;  // running cover into the tile's first cell
+    __shared__ unsigned long long s_gap_prefix;
+    __shared__ uint32_t s_hist[kMaxSortPasses][256];
+    const CarryPassState st = carry_pass_state(state_base, tiles);
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
     resolve_cells(dc, n_cells);
-    uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= n_cells) return;
-    uint64_t k = key2[j];
-    if (k == sentinel_key(S.tiles_y)) {  // irrelevant cell: no carries, no entries
-        gap_count[j] = 0;
+    if (threadIdx.x == 0) s_tile = atomicAdd(st.ticket, 1u);
+    hist_clear(s_hist, plan.n_passes);
+    __syncthreads();
+    const uint32_t tile = s_tile;
+    const uint32_t base = tile * (uint32_t)kCarryThreads;
+    if (base >= n_cells) {  // tiles are taken in order: nobody looks back at this one
+        if (tile == 0 && threadIdx.x == 0) n_gaps_out[0] = 0;
         return;
     }
-    if (j > 0 && (key2[j - 1] >> 32) == (k >> 32)) return;  // not a group head
-    const uint32_t layer = key2_layer(k);
-    const uint32_t fill_rule = fill_rule_of(S, layer);
-    const int32_t ty = (int32_t)key_ty(k) - 1;
-    const bool row_painted = ty >= (int32_t)S.ty_lo && ty < (int32_t)S.ty_hi;
-    uint4 run = make_uint4(0u, 0u, 0u, 0u);
-    while (true) {
-        uint32_t c = perm[j];
-        carry_in[c] = run;
-        run = cover_add(run, cell_cover[c]);
-        carry_after[j] = run;
-        int32_t t = (int32_t)key2_tx(k) - 1;
-        bool has_next = j + 1 < n_cells && (key2[j + 1] >> 32) == (k >> 32);
-        int32_t next_t = has_next ? (int32_t)key2_tx(key2[j + 1]) - 1 : (int32_t)S.tx_hi;
-        uint32_t gaps = 0;
-        if (row_painted) {
-            int32_t lo = max(t + 1, (int32_t)S.tx_lo), hi = min(next_t, (int32_t)S.tx_hi);
-            if (!cover_is_empty(run, fill_rule)) {
-                gaps = hi > lo ? (uint32_t)(hi - lo) : 0u;
+    const uint32_t last_tile = (n_cells - 1u) / kCarryThreads;
+    const uint64_t sentinel = sentinel_key(S.tiles_y);
+    const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
+
+    // 1. the cell, its group head bit and its cover (zero for cells that reach no painted tile)
+    const uint32_t j = base + threadIdx.x;
+    const bool valid = j < n_cells;
+    const uint64_t k = valid ? key2[j] : sentinel;
+    const bool relevant = valid && k != sentinel;
+    const uint32_t c = valid ? perm[j] : 0u;
+    const uint4 cover = relevant ? cell_cover[c] : zero;
+    const bool head = !valid || j == 0 || (key2[j - 1] >> 32) != (k >> 32);
+
+    // 2. segmented inclusive scan inside the warp: (head seen, sum since the last head)
+    uint4 incl = cover;
+    bool seen = head;
+#pragma unroll
+    for (unsigned o = 1; o < 32; o <<= 1) {
+        const uint4 pv = shfl_up_cover(incl, o);
+        const bool ps = __shfl_up_sync(kFullMask, seen, o);
+        if (lane >= o) {
+            if (!seen) incl = cover_add(pv, incl);
+            seen = seen || ps;
+        }
+    }
+    if (lane == 31) {
+        s_warp_cover[warp] = incl;
+        s_warp_head[warp] = seen;
+    }
+    __syncthreads();
+    uint4 warp_prefix = zero;  // segmented sum of the warps before this one
+    bool warp_prefix_seen = false;
+    for (int w = (int)warp - 1; w >= 0 && !warp_prefix_seen; --w) {
+        warp_prefix = cover_add(warp_prefix, s_warp_cover[w]);
+        warp_prefix_seen = s_warp_head[w] != 0u;
+    }
+
+    // 3. carry look-back (first warp). A tile that holds a group head knows the running cover
+    //    after its last cell by itself and publishes it at once; a tile without one publishes its
+    //    sum and, after the look-back, the running cover.
+    if (warp == 0) {
+        uint4 agg = zero;
+        bool agg_seen = false;
+        for (int w = kCarryWarps - 1; w >= 0 && !agg_seen; --w) {
+            agg = cover_add(agg, s_warp_cover[w]);
+            agg_seen = s_warp_head[w] != 0u;
+        }
+        if (lane == 0) {
+            if (agg_seen || tile == 0) {
+                st.inclusive[tile] = agg;
+                st_release(&st.flag[tile], kCarryInclusive);
+            } else {
+                st.aggregate[tile] = agg;
+                st_release(&st.flag[tile], kCarryAggregate);
+            }
+        }
+        uint4 prefix = zero;
+        if (tile != 0 && !__shfl_sync(kFullMask, head, 0)) {  // the first cell continues a group
+            int32_t p = (int32_t)tile - 1;
+            while (true) {
+                const int32_t idx = p - (int32_t)lane;
+                uint32_t f = kCarryInclusive;  // before the first tile: a running cover of 0
+                uint4 v = zero;
+                if (idx >= 0) {
+                    do {
+                        f = ld_acquire(&st.flag[idx]);
+                    } while (f == 0u);
+                    v = ld_relaxed_v4(f == kCarryInclusive ? &st.inclusive[idx] : &st.aggregate[idx]);
+                }
+                const uint32_t done = __ballot_sync(kFullMask, f == kCarryInclusive);
+                const uint32_t upto = done ? (uint32_t)__ffs((int)done) : 32u;  // lanes [0, upto) count
+                uint4 part = lane < upto ? v : zero;
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) part = cover_add(part, shfl_xor_cover(part, o));
+                prefix = cover_add(prefix, part);
+                if (done) break;
+                p -= 32;
+            }
+            if (lane == 0 && !agg_seen) {
+                st.inclusive[tile] = cover_add(prefix, agg);
+                st_release(&st.flag[tile], kCarryInclusive);
+            }
+        }
+        if (lane == 0) s_carry = prefix;
+    }
+    __syncthreads();
+
+    // 4. carry-in and running cover after the cell
+    uint4 before = shfl_up_cover(incl, 1);
+    bool before_seen = __shfl_up_sync(kFullMask, seen, 1);
+    if (lane == 0) {
+        before = zero;
+        before_seen = false;
+    }
+    if (!before_seen) {
+        before = cover_add(warp_prefix, before);
+        if (!warp_prefix_seen) before = cover_add(s_carry, before);
+    }
+    const uint4 cin = head ? zero : before;
+    const uint4 run = cover_add(cin, cover);
+    if (valid) carry_in[c] = cin;
+
+    // 5. carry-only entries after the cell: tiles [first, first + gaps) of its row
+    uint32_t gaps = 0;
+    int32_t first = 0;
+    if (relevant) {
+        const int32_t ty = (int32_t)key_ty(k) - 1;
+        if (ty >= (int32_t)S.ty_lo && ty < (int32_t)S.ty_hi) {
+            const int32_t t = (int32_t)key2_tx(k) - 1;
+            const bool has_next = j + 1u < n_cells && (key2[j + 1u] >> 32) == (k >> 32);
+            const int32_t next_t = has_next ? (int32_t)key2_tx(key2[j + 1u]) - 1 : (int32_t)S.tx_hi;
+            first = max(t + 1, (int32_t)S.tx_lo);
+            const int32_t hi = min(next_t, (int32_t)S.tx_hi);
+            if (!cover_is_empty(run, fill_rule_of(S, key2_layer(k)))) {
+                gaps = hi > first ? (uint32_t)(hi - first) : 0u;
             } else if (t < (int32_t)S.tx_lo && next_t > (int32_t)S.tx_lo && S.tx_lo < S.tx_hi) {
                 // covers_left_of_row: a layer with segments left of the first
                 // painted tile is queued for it even when its cover sums to zero
@@ -310,44 +515,80 @@ __global__ void carry_scan_kernel(PaintScene S, const uint64_t* __restrict__ key
                 gaps = 1;
             }
         }
-        gap_count[j] = gaps;
-        if (!has_next) break;
-        ++j;
-        k = key2[j];
     }
-}
 
-// Carry-only entries (payload = n_cells + gap id), generated in (layer, tile_y,
-// tile_x) order: a stable sort on the tile digits alone then orders them by
-// (tile_y, tile_x, layer).
-__global__ void gap_fill_kernel(PaintScene S, const uint64_t* __restrict__ key2, const uint32_t* __restrict__ perm,
-                                const uint64_t* __restrict__ cell_key, const uint4* __restrict__ carry_after,
-                                const uint32_t* __restrict__ gap_offset /* exclusive scan of the gap counts */,
-                                uint32_t n_cells, uint64_t* __restrict__ gkey, uint32_t* __restrict__ gid,
-                                uint4* __restrict__ gap_carry, const uint32_t* __restrict__ n_gaps_ptr, uint32_t cap,
-                                DevCounts dc) {
-    // One thread per carry-only entry q: its source cell is the last one (in carry
-    // order) whose exclusive offset is <= q — cells without entries share their
-    // offset with the next cell and sort before it.
-    const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
-    const uint32_t n_gaps = *n_gaps_ptr;
-    if (n_gaps > cap || q >= n_gaps) return;  // cap: launched before the host knows the count
-    resolve_cells(dc, n_cells);
-    if (n_cells == 0u) return;
-    uint32_t lo = 0, hi = n_cells;  // first j with gap_offset[j] > q
-    while (lo < hi) {
-        uint32_t mid = (lo + hi) >> 1;
-        if (gap_offset[mid] <= q) lo = mid + 1u;
-        else hi = mid;
+    // 6. exclusive offset of the cell's entries: inside the tile, then by look-back
+    const uint32_t gaps_incl = warp_inclusive_scan(gaps);
+    if (lane == 31) s_warp_gaps[warp] = gaps_incl;
+    __syncthreads();
+    uint32_t warp_off = 0, tile_gaps = 0;
+#pragma unroll
+    for (int w = 0; w < kCarryWarps; ++w) {
+        if ((uint32_t)w < warp) warp_off += s_warp_gaps[w];
+        tile_gaps += s_warp_gaps[w];
     }
-    const uint32_t j = lo - 1u;
-    const uint32_t r = q - gap_offset[j];
-    const uint64_t ck = cell_key[perm[j]];
-    const int32_t tx = (int32_t)key_tx(ck) - 1;
-    const int32_t first = max(tx + 1, (int32_t)S.tx_lo);
-    gkey[q] = (ck & ~(0xFFFull << 41)) | ((uint64_t)(uint32_t)(first + (int32_t)r + 1) << 41);
-    gid[q] = n_cells + q;
-    gap_carry[q] = carry_after[j];
+    if (warp == 0) {
+        volatile unsigned long long* gs = st.gaps;
+        unsigned long long prefix = 0;
+        if (tile == 0) {
+            if (lane == 0) gs[0] = kGapInclusive | tile_gaps;
+        } else {
+            if (lane == 0) gs[tile] = kGapAggregate | tile_gaps;
+            int32_t p = (int32_t)tile - 1;
+            while (true) {
+                const int32_t idx = p - (int32_t)lane;
+                unsigned long long v = kGapInclusive;
+                if (idx >= 0) {
+                    do {
+                        v = gs[idx];
+                    } while ((v & kGapFlags) == 0);
+                }
+                const uint32_t done = __ballot_sync(kFullMask, (v & kGapFlags) == kGapInclusive);
+                const uint32_t upto = done ? (uint32_t)__ffs((int)done) : 32u;
+                unsigned long long part = lane < upto ? (v & ~kGapFlags) : 0ull;
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(kFullMask, part, o);
+                prefix += part;
+                if (done) break;
+                p -= 32;
+            }
+            if (lane == 0) gs[tile] = kGapInclusive | (prefix + tile_gaps);
+        }
+        if (lane == 0) {
+            s_gap_prefix = prefix;
+            if (tile == last_tile) n_gaps_out[0] = (uint32_t)(prefix + tile_gaps);
+        }
+    }
+    __syncthreads();
+
+    // 7. the entries, written by the warp together (entry i of the warp by lane i % 32): lane l's
+    //    cell owns entries [off_l, off_l + gaps_l) of the warp, found by bisection over the lanes
+    const uint32_t warp_gaps = __shfl_sync(kFullMask, gaps_incl, 31);
+    const uint32_t off = gaps_incl - gaps;                                     // inside the warp
+    const uint64_t q0 = s_gap_prefix + warp_off;                               // the warp's first entry
+    const uint64_t bk = ((uint64_t)key_ty(k) << 53) | ((uint64_t)key2_layer(k) << 20);  // key without its tile_x
+    for (uint32_t i0 = 0; i0 < warp_gaps; i0 += 32u) {
+        const uint32_t i = i0 + lane;
+        int src = 0;
+#pragma unroll
+        for (int step = 16; step > 0; step >>= 1)
+            if (__shfl_sync(kFullMask, off, src + step) <= i) src += step;
+        const uint32_t r = i - __shfl_sync(kFullMask, off, src);
+        const int32_t f = __shfl_sync(kFullMask, first, src);
+        const uint64_t kb = ((uint64_t)__shfl_sync(kFullMask, (uint32_t)(bk >> 32), src) << 32) |
+                            (uint64_t)__shfl_sync(kFullMask, (uint32_t)bk, src);
+        const uint4 cv = shfl_cover(run, src);
+        const uint64_t q = q0 + i;
+        if (i < warp_gaps && q < cap) {
+            const uint64_t gk = kb | ((uint64_t)(uint32_t)(f + (int32_t)r + 1) << 41);
+            gkey[q] = gk;
+            gid[q] = n_cells + (uint32_t)q;
+            gap_carry[q] = cv;
+            hist_count(&s_hist[0][0], plan, gk);
+        }
+    }
+    __syncthreads();
+    hist_flush(s_hist, plan.n_passes, hist);
 }
 
 // Entries = cells (sorted by construction) merged with the sorted carry-only
@@ -362,6 +603,33 @@ __device__ __forceinline__ uint32_t lower_bound_key(const uint64_t* __restrict__
     }
     return lo;
 }
+// lower_bound_key over the whole list by one warp: 32 pivots per round cut the range 33-fold,
+// so a list of a million keys takes 4 dependent loads instead of 20.
+__device__ __forceinline__ uint32_t warp_lower_bound_key(const uint64_t* __restrict__ a, uint32_t n, uint64_t k) {
+    const uint32_t lane = threadIdx.x & 31u;
+    uint32_t lo = 0, hi = n;  // the answer lies in [lo, hi]
+    while (hi - lo > 32u) {
+        const uint64_t len = hi - lo;
+        const uint32_t below = __popc(__ballot_sync(kFullMask, a[lo + (uint32_t)(len * (lane + 1u) / 33u)] < k));
+        const uint32_t nlo = below ? lo + (uint32_t)(len * below / 33u) + 1u : lo;  // past the last pivot < k
+        hi = below < 32u ? lo + (uint32_t)(len * (below + 1u) / 33u) : hi;        // at the first pivot >= k
+        lo = nlo;
+    }
+    return lo + __popc(__ballot_sync(kFullMask, lo + lane < hi && a[lo + lane] < k));
+}
+// lower_bound_key in a[0, i] when every key from a[i] on is >= k (a[i] itself is not read):
+// galloping back from i, then bisection — a tile's entries are few and close together.
+__device__ __forceinline__ uint32_t lower_bound_back(const uint64_t* __restrict__ a, uint32_t i, uint64_t k) {
+    uint32_t hi = i, lo = 0;  // the answer lies in [lo, hi]
+    for (uint32_t step = 1; step <= hi; step <<= 1) {
+        if (a[hi - step] < k) {
+            lo = hi - step + 1u;
+            break;
+        }
+        hi -= step;
+    }
+    return lo + lower_bound_key(a + lo, hi - lo, k);
+}
 // Besides the sorted key, every entry gets a self-contained 64-byte record (its
 // segment range, carry, style bits and colour) and its initial optimizer flags,
 // so that the painter reaches everything it needs with one round of loads per
@@ -370,32 +638,39 @@ __global__ void merge_entries_kernel(PaintScene S, const uint64_t* __restrict__ 
                                      const uint64_t* __restrict__ gkey, const uint32_t* __restrict__ gid, uint32_t n_gaps,
                                      const uint32_t* __restrict__ cell_start, const uint4* __restrict__ carry_in,
                                      const uint4* __restrict__ gap_carry, uint64_t* __restrict__ ekey,
-                                     EntryRec* __restrict__ recs, uint8_t* __restrict__ eflags, DevCounts dc) {
+                                     EntryRec* __restrict__ recs, uint8_t* __restrict__ eflags, uint2* __restrict__ tile_range,
+                                     uint32_t* __restrict__ heavy, uint32_t* __restrict__ heavy_count, DevCounts dc) {
     resolve_counts(dc, n_cells, n_gaps);
     // Merge-path style partition: the keys of a CTA's 256 consecutive elements of
     // one list bracket a short range of the other list, found once per CTA (two
-    // full bisections by threads 0 and 1); every thread then bisects that range only.
+    // whole-list searches by warps 0 and 1); every thread then bisects that range only.
     __shared__ uint32_t s_bound[2];
     const uint32_t i0 = blockIdx.x * blockDim.x, i = i0 + threadIdx.x;
     const uint32_t n_all = n_cells + n_gaps;
     if (i0 >= n_all) return;  // (whole CTA; only with device-side counts)
     const bool cell_block = i0 + blockDim.x <= n_cells, gap_block = i0 >= n_cells;  // else: the one mixed CTA
-    if (threadIdx.x < 2u) {
+    if (threadIdx.x < 64u) {
+        const uint32_t w = threadIdx.x >> 5;
         const uint32_t last = min(i0 + blockDim.x, n_all) - 1u;
-        uint32_t b = threadIdx.x == 0u ? 0u : (cell_block ? n_gaps : n_cells);
-        if (cell_block) b = lower_bound_key(gkey, n_gaps, cell_key[threadIdx.x == 0u ? i0 : last]);
-        else if (gap_block) b = lower_bound_key(cell_key, n_cells, gkey[(threadIdx.x == 0u ? i0 : last) - n_cells]);
-        s_bound[threadIdx.x] = b;
+        uint32_t b = w == 0u ? 0u : (cell_block ? n_gaps : n_cells);
+        if (cell_block) b = warp_lower_bound_key(gkey, n_gaps, cell_key[w == 0u ? i0 : last]);
+        else if (gap_block) b = warp_lower_bound_key(cell_key, n_cells, gkey[(w == 0u ? i0 : last) - n_cells]);
+        if ((threadIdx.x & 31u) == 0u) s_bound[w] = b;
     }
     __syncthreads();
     if (i >= n_all) return;
     uint64_t k;
     uint32_t pos;
     EntryRec r;
+    // The entry's own list (a) from index ia on, the other list (b) from rank rb on: the next
+    // entry in tile order is the smaller of a[ia + 1] and b[rb].
+    const uint64_t *a, *b;
+    uint32_t na, nb, ia, rb;
     if (i < n_cells) {
         k = cell_key[i];
         const uint32_t lo = cell_block ? s_bound[0] : 0u, hi = cell_block ? s_bound[1] : n_gaps;
-        pos = i + lo + lower_bound_key(gkey + lo, hi - lo, k);
+        rb = lo + lower_bound_key(gkey + lo, hi - lo, k);
+        a = cell_key, na = n_cells, ia = i, b = gkey, nb = n_gaps;
         r.seg0 = cell_start[i];
         r.seg1 = cell_start[i + 1];
         r.carry = carry_in[i];
@@ -403,9 +678,30 @@ __global__ void merge_entries_kernel(PaintScene S, const uint64_t* __restrict__ 
         uint32_t g = i - n_cells;
         k = gkey[g];
         const uint32_t lo = gap_block ? s_bound[0] : 0u, hi = gap_block ? s_bound[1] : n_cells;
-        pos = g + lo + lower_bound_key(cell_key + lo, hi - lo, k);
+        rb = lo + lower_bound_key(cell_key + lo, hi - lo, k);
+        a = gkey, na = n_gaps, ia = g, b = cell_key, nb = n_cells;
         r.seg0 = r.seg1 = 0;
         r.carry = gap_carry[gid[g] - n_cells];
+    }
+    pos = ia + rb;
+    // Per painted tile: [begin, end) of its entries, written by the thread of the tile's last
+    // entry (it finds the first one in both lists, searching back from its own place in them:
+    // every key from a[ia] and from b[rb] on is >= the tile's first key); the same thread files a tile
+    // with many entries in its class list (see paint_common.cuh: kHeavyMin). Entries outside the
+    // render target (biased tile coordinate 0 = tile -1, or beyond the last tile) belong to no
+    // painted tile.
+    const uint64_t tile_bits = k >> 41;
+    const bool in_frame = key_ty(k) != 0u && key_ty(k) <= S.tiles_y && key_tx(k) != 0u && key_tx(k) <= S.tiles_x;
+    if (in_frame && (ia + 1u >= na || (a[ia + 1u] >> 41) != tile_bits) && (rb >= nb || (b[rb] >> 41) != tile_bits)) {
+        const uint64_t tile_key = tile_bits << 41;
+        const uint32_t begin = lower_bound_back(a, ia, tile_key) + lower_bound_back(b, rb, tile_key);
+        const uint32_t tid = (key_ty(k) - 1u) * S.tiles_x + (key_tx(k) - 1u);
+        tile_range[tid] = make_uint2(begin, pos + 1u);
+        const uint32_t count = pos + 1u - begin;
+        if (heavy && count >= kHeavyMin) {
+            const int hc = heavy_class(count);
+            heavy[(size_t)hc * S.tiles_x * S.tiles_y + atomicAdd(&heavy_count[hc], 1u)] = tid;
+        }
     }
     r.layer = key_layer(k);
     r.slot = r.layer < S.n_orders ? S.order_to_style[r.layer] : -1;
@@ -436,40 +732,6 @@ __global__ void merge_entries_kernel(PaintScene S, const uint64_t* __restrict__ 
     ekey[pos] = k;
     recs[pos] = r;
     eflags[pos] = (uint8_t)flags;
-}
-
-// Per painted tile: [begin, end) of its entries in the sorted entry list, written by the
-// thread of the tile's last entry (which bisects for the first one); the same thread files
-// a tile with many entries in its class list (see paint_common.cuh: kHeavyMin).
-__global__ void tile_index_kernel(PaintScene S, const uint64_t* __restrict__ ekey, uint32_t n_entries,
-                                  uint2* __restrict__ tile_range, uint32_t* __restrict__ heavy /* [classes][tiles] or null */,
-                                  uint32_t* __restrict__ heavy_count, DevCounts dc) {
-    if (dc.cells) {
-        uint32_t c = 0, g = 0;
-        resolve_counts(dc, c, g);
-        n_entries = c + g;
-    }
-    uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= n_entries) return;
-    const uint64_t k = ekey[p];
-    // Entries outside the render target (biased tile coordinate 0 = tile -1, or
-    // beyond the last tile) belong to no painted tile.
-    if (key_ty(k) == 0u || key_ty(k) > S.tiles_y || key_tx(k) == 0u || key_tx(k) > S.tiles_x) return;
-    const uint64_t tile_bits = k >> 41;
-    if (p + 1 != n_entries && (ekey[p + 1] >> 41) == tile_bits) return;  // not the tile's last entry
-    uint32_t lo = 0, hi = p;  // first entry of the tile: the first q with ekey[q] >> 41 >= tile_bits
-    while (lo < hi) {
-        const uint32_t mid = (lo + hi) >> 1;
-        if ((ekey[mid] >> 41) < tile_bits) lo = mid + 1u;
-        else hi = mid;
-    }
-    const uint32_t tid = (key_ty(k) - 1u) * S.tiles_x + (key_tx(k) - 1u);
-    tile_range[tid] = make_uint2(lo, p + 1u);
-    const uint32_t count = p + 1u - lo;
-    if (heavy && count >= kHeavyMin) {
-        const int c = heavy_class(count);
-        heavy[(size_t)c * S.tiles_x * S.tiles_y + atomicAdd(&heavy_count[c], 1u)] = tid;
-    }
 }
 
 // Cost of every tile row of the frame just rendered: 32 x its (tile, layer) entries + its
@@ -519,67 +781,70 @@ void launch_row_costs(const uint2* tile_range, uint32_t tiles_x, uint32_t tiles_
 // ---------------------------------------------------------------------------
 uint32_t cell_num_blocks(uint32_t n) { return (n + kCellTile - 1) / kCellTile; }
 
-size_t cells_state_words(uint32_t n) { return (size_t)cell_num_blocks(n) + 2; }
+static size_t align256(size_t b) { return (b + 255u) & ~(size_t)255u; }
 
-void launch_cells(const PaintScene& S, const uint64_t* segs, uint32_t n, unsigned long long* state, uint32_t* cell_start,
-                  uint32_t cap, uint32_t* n_cells_out, uint64_t* cell_key, uint4* cell_cover, uint64_t* key2, uint32_t* perm,
-                  cudaStream_t st) {
+TableScratch table_scratch_layout(uint32_t n, uint32_t n_cells, uint32_t n_gaps, const SortPlan& carry_plan,
+                                  const SortPlan& gap_plan) {
+    TableScratch L;
+    const size_t hist_bytes = align256((size_t)kMaxSortPasses * 256u * sizeof(uint32_t));
+    L.heavy_count = 0;
+    L.carry_hist = align256(kHeavyListClasses * sizeof(uint32_t));
+    L.gap_hist = L.carry_hist + hist_bytes;
+    L.cells_state = L.gap_hist + hist_bytes;
+    L.carry_sort = L.cells_state + align256(((size_t)cell_num_blocks(n) + 1u) * sizeof(unsigned long long));
+    L.carry_pass = L.carry_sort + align256(sort_lookback_bytes(n_cells, carry_plan));
+    L.gap_sort = L.carry_pass + align256(carry_pass_state_bytes(carry_pass_tiles(n_cells)));
+    L.end = L.gap_sort + align256(sort_lookback_bytes(n_gaps, gap_plan));
+    return L;
+}
+
+void launch_cells(const PaintScene& S, const uint64_t* segs, uint32_t n, uint8_t* scratch, const TableScratch& L,
+                  const SortPlan& carry_plan, uint32_t* cell_start, uint32_t cap, uint32_t* n_cells_out, uint64_t* cell_key,
+                  uint4* cell_cover, uint64_t* key2, uint32_t* perm, cudaStream_t st) {
     const uint32_t tiles = cell_num_blocks(n);
-    cudaMemsetAsync(state, 0, (tiles + 1) * sizeof(unsigned long long), st);
+    auto* state = reinterpret_cast<unsigned long long*>(scratch + L.cells_state);  // [tiles] look-back | ticket
+    auto* hist = reinterpret_cast<uint32_t*>(scratch + L.carry_hist);
     cells_kernel<<<tiles, kCellThreads, 0, st>>>(S, segs, n, state, tiles, cell_start, cap, n_cells_out, cell_key, cell_cover, key2,
-                                                 perm);
+                                                 perm, carry_plan, hist);
     if (tiles > 1)
         cells_boundary_kernel<<<(tiles - 1 + kCellThreads / 32 - 1) / (kCellThreads / 32), kCellThreads, 0, st>>>(
-            S, segs, n, state, tiles, cell_start, cap, n_cells_out, cell_key, cell_cover, key2, perm);
+            S, segs, n, state, tiles, cell_start, cap, n_cells_out, cell_key, cell_cover, key2, perm, carry_plan, hist);
 }
 
 // Largest values the three key fields can take in the pair sorts (sentinel
 // included); the sort plan only spends passes on bits below these bounds.
 // The cells arrive sorted by (tile_y, tile_x, layer); a stable sort on the layer
 // bits alone leaves them ordered by (layer, tile_y, tile_x), which is all the
-// carry scan needs: every (tile_y, layer) group contiguous, tile_x ascending.
+// carry pass needs: every (tile_y, layer) group contiguous, tile_x ascending.
 SortPlan carry_sort_plan(const PaintScene& S) {  // fields, least significant first: tile_x, layer, tile_y
     const uint64_t bound[3] = {0u, S.n_orders ? S.n_orders - 1u : 0u, 0u};
     return make_sort_plan(carry_key_layout(), bound);
 }
-// Carry-only entries: tile digits only (see gap_fill_kernel).
+// Carry-only entries: tile digits only (see carry_pass_kernel).
 SortPlan gap_sort_plan(const PaintScene& S) {  // layer, tile_x, tile_y
     const uint64_t bound[3] = {0u, S.tx_hi, S.ty_hi};
     return make_sort_plan(segment_key_layout(), bound);
 }
 
-void launch_carry_scan(const PaintScene& S, const uint64_t* key2, const uint32_t* perm, const uint4* cell_cover,
-                       uint32_t n_cells, uint4* carry_in, uint4* carry_after, uint32_t* gap_count, cudaStream_t st,
+void launch_carry_pass(const PaintScene& S, const uint64_t* key2, const uint32_t* perm, const uint4* cell_cover,
+                       uint32_t n_cells, uint8_t* scratch, const TableScratch& L, const SortPlan& gap_plan, uint4* carry_in,
+                       uint64_t* gkey, uint32_t* gid, uint4* gap_carry, uint32_t cap, uint32_t* n_gaps_out, cudaStream_t st,
                        const DevCounts& dc) {
-    carry_scan_kernel<<<(n_cells + 127) / 128, 128, 0, st>>>(S, key2, perm, cell_cover, n_cells, carry_in, carry_after,
-                                                              gap_count, dc);
-}
-
-void launch_gap_fill(const PaintScene& S, const uint64_t* key2, const uint32_t* perm, const uint64_t* cell_key,
-                     const uint4* carry_after, const uint32_t* gap_offset, uint32_t n_cells,
-                     uint64_t* gkey, uint32_t* gid, uint4* gap_carry, const uint32_t* n_gaps_ptr, uint32_t cap,
-                     uint32_t grid_gaps, cudaStream_t st, const DevCounts& dc) {
-    if (!grid_gaps || !n_cells) return;
-    gap_fill_kernel<<<(grid_gaps + 127) / 128, 128, 0, st>>>(S, key2, perm, cell_key, carry_after, gap_offset, n_cells,
-                                                              gkey, gid, gap_carry, n_gaps_ptr, cap, dc);
+    const uint32_t tiles = carry_pass_tiles(n_cells);
+    if (!tiles) return;
+    carry_pass_kernel<<<tiles, kCarryThreads, 0, st>>>(S, key2, perm, cell_cover, n_cells, scratch + L.carry_pass, tiles, carry_in,
+                                                       gkey, gid, gap_carry, cap, n_gaps_out, gap_plan,
+                                                       reinterpret_cast<uint32_t*>(scratch + L.gap_hist), dc);
 }
 
 void launch_merge_entries(const PaintScene& S, const uint64_t* cell_key, uint32_t n_cells, const uint64_t* gkey,
                           const uint32_t* gid, uint32_t n_gaps, const uint32_t* cell_start, const uint4* carry_in,
-                          const uint4* gap_carry, uint64_t* ekey, EntryRec* recs, uint8_t* eflags, cudaStream_t st,
-                          const DevCounts& dc) {
+                          const uint4* gap_carry, uint64_t* ekey, EntryRec* recs, uint8_t* eflags, uint2* tile_range,
+                          uint32_t* heavy, uint32_t* heavy_count, cudaStream_t st, const DevCounts& dc) {
     uint32_t n = n_cells + n_gaps;
     if (n)
         merge_entries_kernel<<<(n + 255) / 256, 256, 0, st>>>(S, cell_key, n_cells, gkey, gid, n_gaps, cell_start, carry_in,
-                                                               gap_carry, ekey, recs, eflags, dc);
-}
-
-void launch_tile_index(const PaintScene& S, const uint64_t* ekey, uint32_t n_entries, uint2* tile_range, uint32_t* heavy,
-                       uint32_t* heavy_count, cudaStream_t st, const DevCounts& dc) {
-    cudaMemsetAsync(tile_range, 0, (size_t)S.tiles_x * S.tiles_y * sizeof(uint2), st);
-    cudaMemsetAsync(heavy_count, 0, kHeavyClasses * sizeof(uint32_t), st);
-    if (n_entries)
-        tile_index_kernel<<<(n_entries + 255) / 256, 256, 0, st>>>(S, ekey, n_entries, tile_range, heavy, heavy_count, dc);
+                                                               gap_carry, ekey, recs, eflags, tile_range, heavy, heavy_count, dc);
 }
 
 

@@ -364,7 +364,7 @@ int Renderer::render(Composition& comp, uint8_t* buffer, bool buffer_on_device, 
     last_tiles_y = S.tiles_y;
     FORMA_CUDA_TRY(tile_range.reserve(n_tiles_total));
     FORMA_CUDA_TRY(heavy_tiles.reserve(n_tiles_total * kHeavyListClasses));
-    // Heavy tiles first (longest-processing-time order): their lists + counts (totals[8..11]).
+    // Heavy tiles first (longest-processing-time order): their lists + counts (heavy_count()).
     uint32_t* const heavy_lists = options().paint_lpt ? heavy_tiles.ptr : nullptr;
     uint8_t* fb = buffer;
     if (!buffer_on_device) {
@@ -388,13 +388,10 @@ int Renderer::render(Composition& comp, uint8_t* buffer, bool buffer_on_device, 
     last_tables_redone = false;
     uint32_t paint_launches = 1;
     for (bool sync_free = fast;; sync_free = false) {
-        uint32_t n_entries = 0;
         DevCounts dc;
-        if (n > 0) {
-            st = build_tables(S, n, sync_free, prev_cells, prev_gaps, &n_entries, dc);
-            if (st) return st;
-        }
-        st = index_tiles(S, n, n_entries, dc, heavy_lists);
+        st = build_tables(S, n, sync_free, prev_cells, prev_gaps, heavy_lists, dc);
+        if (st) return st;
+        st = queue_row_costs(S, n);
         if (st) return st;
         FORMA_CUDA_TRY(cudaEventRecord(timer.ev[4], stream));
         st = paint(S, fb, buffer, stride, in_bands, heavy_lists, &paint_launches);
@@ -525,9 +522,9 @@ int Renderer::bind_frame(Composition& comp, PaintScene& S, LayerCache* cache, co
 
 SortResult Renderer::sort(DeviceBuffer<uint64_t>& keys, DeviceBuffer<uint64_t>& keys_tmp, DeviceBuffer<uint32_t>* vals,
                           DeviceBuffer<uint32_t>* vals_tmp, uint32_t n, const SortPlan& plan, cudaEvent_t* pass_events,
-                          const uint32_t* n_dev) {
+                          const uint32_t* n_dev, const uint32_t* hist, void* scratch) {
     SortResult sr = launch_radix_sort(keys.ptr, keys_tmp.ptr, vals ? vals->ptr : nullptr, vals ? vals_tmp->ptr : nullptr, n, plan,
-                                      sort_scratch.ptr, stream, pass_events, n_dev);
+                                      scratch ? scratch : sort_scratch.ptr, stream, pass_events, n_dev, hist);
     launches += sr.launches;
     if (sr.in_tmp) {
         swap_buffers(keys, keys_tmp);
@@ -536,36 +533,52 @@ SortResult Renderer::sort(DeviceBuffer<uint64_t>& keys, DeviceBuffer<uint64_t>& 
     return sr;
 }
 
-// The painter tables of the n > 0 sorted segments: cells -> carry pair sort -> carries -> gap
-// offsets -> carry-only entries ("gaps") -> gap pair sort -> entries. The modes differ only in
-// how they get the cell and gap counts:
+// The painter tables of the n sorted segments: cells (+ the carry sort's digit counts) -> carry
+// pair sort -> carry pass: carries, carry-only entries ("gaps") (+ the gap sort's digit counts)
+// -> gap pair sort -> entries, tile ranges and heavy-tile lists. The modes differ only in how
+// they get the cell and gap counts:
 // - sync_free: a count is a bound (the previous frame's + 25 % + 4096), everything is reserved
-//   for the bounds up front, and the kernels read the real counts from device memory (dc).
+//   for the bounds up front, and the kernels read the real counts from device memory (dc). Two
+//   memsets (tile ranges, table scratch) and the kernels, nothing else.
 // - counted: a count is read back; the kernel that produces it runs ahead of the read-back into
 //   the buffers of the previous frames and is launched again when they turn out too small.
-// *n_entries: the entry count (sync_free: its bound, the grid of the tile index pass).
 int Renderer::build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint32_t prev_cells, uint32_t prev_gaps,
-                           uint32_t* n_entries, DevCounts& dc) {
-    uint32_t n_cells = 0, n_gaps = 0;  // sync_free: their bounds
-    auto cells_pass = [&](uint32_t cap) {
-        launch_cells(S, segs.ptr, n, scan_state.ptr, cell_start.ptr, cap, totals.ptr + 1, cell_key.ptr, cell_cover.ptr,
-                     key2.ptr, perm.ptr, stream);
-        launches += 2;
+                           uint32_t* heavy_lists, DevCounts& dc) {
+    // Tiles without entries keep an empty range: a frame whose tables are redone paints only the
+    // clear colour in its first attempt.
+    FORMA_CUDA_TRY(cudaMemsetAsync(tile_range.ptr, 0, (size_t)S.tiles_x * S.tiles_y * sizeof(uint2), stream));
+    const SortPlan carry_plan = carry_sort_plan(S), gap_plan = gap_sort_plan(S);
+    auto zero_scratch = [&](size_t from, size_t to) -> cudaError_t {
+        return to > from ? cudaMemsetAsync(table_scratch.ptr + from, 0, to - from, stream) : cudaSuccess;
     };
-    auto gap_fill = [&](uint32_t cap) {
-        launch_gap_fill(S, key2.ptr, perm.ptr, cell_key.ptr, carry_after.ptr, gap_count.ptr, n_cells, ekey_tmp.ptr, eid_tmp.ptr,
-                        gap_carry.ptr, totals.ptr + 2, cap, cap, stream, dc);
+    if (n == 0) {  // nothing to index; the painter still reads the heavy-list lengths
+        const TableScratch L = table_scratch_layout(0, 0, 0, carry_plan, gap_plan);
+        FORMA_CUDA_TRY(table_scratch.reserve(L.carry_hist));
+        FORMA_CUDA_TRY(zero_scratch(0, L.carry_hist));
+        return FORMA_STATUS_OK;
+    }
+    uint32_t n_cells = 0, n_gaps = 0;  // sync_free: their bounds
+    TableScratch L{};
+    auto cells_pass = [&](uint32_t cap) {
+        launch_cells(S, segs.ptr, n, table_scratch.ptr, L, carry_plan, cell_start.ptr, cap, totals.ptr + 1, cell_key.ptr,
+                     cell_cover.ptr, key2.ptr, perm.ptr, stream);
+        launches += cell_num_blocks(n) > 1 ? 2 : 1;
+    };
+    auto carry_pass = [&](uint32_t cap) {
+        launch_carry_pass(S, key2.ptr, perm.ptr, cell_cover.ptr, n_cells, table_scratch.ptr, L, gap_plan, carry_in.ptr,
+                          ekey_tmp.ptr, eid_tmp.ptr, gap_carry.ptr, cap, totals.ptr + 2, stream, dc);
         ++launches;
     };
     if (sync_free) {
         const uint64_t shrink = options().test_fast_shrink ? 2u : 1u;
         n_cells = (uint32_t)std::min<uint64_t>(((uint64_t)prev_cells + prev_cells / 4u + 4096u) / shrink, n);
         n_gaps = (uint32_t)std::min<uint64_t>(((uint64_t)prev_gaps + prev_gaps / 4u + 4096u) / shrink, 0x7FFFFFFFu);
-        FORMA_CUDA_TRY(scan_state.reserve(std::max({cells_state_words(n), scan_state_words(n), scan_state_words(n_cells)})));
         FORMA_CUDA_TRY(reserve_cell_tables(n_cells));
         FORMA_CUDA_TRY(reserve_gap_tables(n_gaps));
         FORMA_CUDA_TRY(reserve_entry_tables((size_t)n_cells + n_gaps));
-        FORMA_CUDA_TRY(sort_scratch.reserve(std::max(radix_scratch_bytes(n_cells), radix_scratch_bytes(n_gaps))));
+        L = table_scratch_layout(n, n_cells, n_gaps, carry_plan, gap_plan);
+        FORMA_CUDA_TRY(table_scratch.reserve(L.end));
+        FORMA_CUDA_TRY(zero_scratch(0, L.end));
         dc = DevCounts{totals.ptr + 1, totals.ptr + 2, n_cells, n_gaps};
         // Cells beyond cell_bound + 1 are dropped by the pass; the count it leaves in totals[1] is the real one.
         cells_pass(n_cells + 1u);
@@ -574,7 +587,9 @@ int Renderer::build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint
         // read back, but nothing waits for it: the pass runs into the buffers of the previous
         // frames (writes beyond their capacity are dropped) and is repeated below only if
         // those turn out too small.
-        FORMA_CUDA_TRY(scan_state.reserve(std::max(cells_state_words(n), scan_state_words(n))));
+        L = table_scratch_layout(n, 0, 0, carry_plan, gap_plan);
+        FORMA_CUDA_TRY(table_scratch.reserve(L.carry_sort));
+        FORMA_CUDA_TRY(zero_scratch(0, L.carry_sort));
         if (!cell_start.capacity)  // first frame: a guess that usually holds (cells ~ segments / 20)
             FORMA_CUDA_TRY(reserve_all((size_t)n / 8u + 4096u, cell_start, cell_key, cell_cover, key2, perm));
         auto cells_capacity = [&] {
@@ -588,29 +603,36 @@ int Renderer::build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint
         FORMA_CUDA_TRY(cudaEventSynchronize(count_ev));
         n_cells = pinned_totals[1];
         FORMA_CUDA_TRY(reserve_cell_tables(n_cells));
-        if ((size_t)n_cells + 1 > cell_cap) cells_pass(cells_capacity());  // the buffers were too small: the pass dropped the overflow
-        FORMA_CUDA_TRY(sort_scratch.reserve(radix_scratch_bytes(n_cells)));
+        L = table_scratch_layout(n, n_cells, 0, carry_plan, gap_plan);
+        const uint8_t* held = table_scratch.ptr;
+        FORMA_CUDA_TRY(table_scratch.reserve(L.gap_sort));
+        // The buffers were too small (the pass dropped the overflow), or the scratch moved (the
+        // digit counts went with it): once more.
+        if ((size_t)n_cells + 1 > cell_cap || table_scratch.ptr != held) {
+            FORMA_CUDA_TRY(zero_scratch(0, L.carry_sort));
+            cells_pass(cells_capacity());
+        }
+        FORMA_CUDA_TRY(zero_scratch(L.carry_sort, L.gap_sort));
     }
-    sort(key2, key2_tmp, &perm, &perm_tmp, n_cells, carry_sort_plan(S), nullptr, dc.cells);
-    launch_carry_scan(S, key2.ptr, perm.ptr, cell_cover.ptr, n_cells, carry_in.ptr, carry_after.ptr, gap_count.ptr, stream, dc);
-    // gap_count -> exclusive offsets, in place (gap_fill only needs the offsets).
-    launch_scan_u32(gap_count.ptr, n_cells, totals.ptr + 2, scan_state.ptr, stream, dc.cells);
-    launches += 2;
+    sort(key2, key2_tmp, &perm, &perm_tmp, n_cells, carry_plan, nullptr, dc.cells,
+         reinterpret_cast<const uint32_t*>(table_scratch.ptr + L.carry_hist), table_scratch.ptr + L.carry_sort);
     if (sync_free) {
-        gap_fill(n_gaps);
+        carry_pass(n_gaps);
     } else {
-        // Same scheme for the number of carry-only entries: gap_fill runs ahead of the read-back.
-        FORMA_CUDA_TRY(cudaMemcpyAsync(pinned_totals + 2, totals.ptr + 2, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
-        FORMA_CUDA_TRY(cudaEventRecord(count_ev, stream));
-        // The speculative output survives only if the reserve(n_gaps + 1) calls below do not
-        // reallocate: one element of every buffer is kept back (the sort's slack slot).
+        // Same scheme for the number of carry-only entries: the carry pass counts them and writes
+        // them ahead of the read-back, into the buffers of the previous frames (at most gap_cap;
+        // 0: the carries and the count only, the entries follow the read-back). The speculative
+        // output survives only if the reserve(n_gaps + 1) calls below do not reallocate: one
+        // element of every buffer is kept back (the sort's slack slot).
         size_t gap_cap = 0;
         if (speculation_enabled()) {
             const size_t room = std::min({ekey_tmp.capacity, eid_tmp.capacity, gap_carry.capacity});
-            gap_cap = std::min<size_t>(room ? room - 1u : 0u, (size_t)last_gaps * 2u + 4096u /* also the number of threads launched */);
+            gap_cap = std::min<size_t>(room ? room - 1u : 0u, (size_t)last_gaps * 2u + 4096u);
             if (test_gap_cap_override() && gap_cap) gap_cap = std::min<size_t>(gap_cap, test_gap_cap_override());
         }
-        if (gap_cap) gap_fill((uint32_t)gap_cap);
+        carry_pass((uint32_t)gap_cap);
+        FORMA_CUDA_TRY(cudaMemcpyAsync(pinned_totals + 2, totals.ptr + 2, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+        FORMA_CUDA_TRY(cudaEventRecord(count_ev, stream));
         FORMA_CUDA_TRY(cudaEventSynchronize(count_ev));
         n_gaps = pinned_totals[2];
         last_gaps = n_gaps;
@@ -618,25 +640,33 @@ int Renderer::build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint
         last_entries = n_cells + n_gaps;
         FORMA_CUDA_TRY(reserve_gap_tables(n_gaps));
         FORMA_CUDA_TRY(reserve_entry_tables((size_t)n_cells + n_gaps));
-        if (n_gaps) FORMA_CUDA_TRY(sort_scratch.reserve(radix_scratch_bytes(n_gaps)));
-        if (n_gaps && (!gap_cap || n_gaps > gap_cap)) gap_fill(n_gaps);
+        L = table_scratch_layout(n, n_cells, n_gaps, carry_plan, gap_plan);
+        const uint8_t* held = table_scratch.ptr;
+        FORMA_CUDA_TRY(table_scratch.reserve(L.end));
+        const bool moved = table_scratch.ptr != held;
+        const bool again = n_gaps && (n_gaps > gap_cap || moved);  // entries dropped, or their digit counts lost
+        if (again || moved) {
+            FORMA_CUDA_TRY(zero_scratch(0, L.end));
+        } else {
+            FORMA_CUDA_TRY(zero_scratch(L.gap_sort, L.end));
+        }
+        if (again) carry_pass(n_gaps);
     }
-    if (n_gaps) sort(ekey_tmp, gkey_tmp, &eid_tmp, &gid_tmp, n_gaps, gap_sort_plan(S), nullptr, dc.gaps);
+    if (n_gaps)
+        sort(ekey_tmp, gkey_tmp, &eid_tmp, &gid_tmp, n_gaps, gap_plan, nullptr, dc.gaps,
+             reinterpret_cast<const uint32_t*>(table_scratch.ptr + L.gap_hist), table_scratch.ptr + L.gap_sort);
     launch_merge_entries(S, cell_key.ptr, n_cells, ekey_tmp.ptr, eid_tmp.ptr, n_gaps, cell_start.ptr, carry_in.ptr, gap_carry.ptr,
-                         ekey.ptr, recs.ptr, eflags.ptr, stream, dc);
+                         ekey.ptr, recs.ptr, eflags.ptr, tile_range.ptr, heavy_lists, heavy_count(), stream, dc);
     ++launches;
-    *n_entries = n_cells + n_gaps;
     // sync_free: the counts travel to the host behind everything else of the frame.
     if (sync_free)
         FORMA_CUDA_TRY(cudaMemcpyAsync(pinned_totals + 1, totals.ptr + 1, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
     return FORMA_STATUS_OK;
 }
 
-// Per-tile entry ranges and the heavy-tile lists; renderers of a multi-device / sliced frame
-// also queue the per-row costs and their copy to the host.
-int Renderer::index_tiles(const PaintScene& S, uint32_t n, uint32_t n_entries, const DevCounts& dc, uint32_t* heavy_lists) {
-    launch_tile_index(S, ekey.ptr, n_entries, tile_range.ptr, heavy_lists, totals.ptr + 8, stream, dc);
-    launches += n_entries ? 1 : 0;
+// Renderers of a multi-device / sliced frame queue the per-row costs of the frame and their copy
+// to the host.
+int Renderer::queue_row_costs(const PaintScene& S, uint32_t n) {
     row_costs_rows = 0;
     if (track_row_costs && n > 0) {
         FORMA_CUDA_TRY(d_row_costs.reserve(3u * S.tiles_y));  // per row: cost, pixel segments, entries
@@ -677,7 +707,7 @@ int Renderer::paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t 
             Sb.ty_hi = S.ty_lo + paint_rows * (k + 1u) / kCopyBands;
             cudaStream_t bs = kCopyBands > 1u ? band_stream[k] : stream;
             if (kCopyBands > 1u) FORMA_CUDA_TRY(cudaStreamWaitEvent(bs, band_ev[kMaxCopyBands], 0));
-            launch_paint(Sb, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, totals.ptr + 8, eflags.ptr, fb, totals.ptr + 16 + k, bs);
+            launch_paint(Sb, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), eflags.ptr, fb, totals.ptr + 16 + k, bs);
             ++launches;
             const int st = copy_to_host(Sb, buffer, fb, stride, bs);
             if (st) return st;
@@ -686,7 +716,7 @@ int Renderer::paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t 
         for (uint32_t k = 0; kCopyBands > 1u && k < kCopyBands; ++k) FORMA_CUDA_TRY(cudaStreamWaitEvent(stream, band_ev[k], 0));
         *paint_launches = kCopyBands;
     } else {
-        launch_paint(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, totals.ptr + 8, eflags.ptr, fb, totals.ptr + 3, stream);
+        launch_paint(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), eflags.ptr, fb, totals.ptr + 3, stream);
         ++launches;
     }
     FORMA_CUDA_TRY(cudaGetLastError());

@@ -51,7 +51,6 @@ class Renderer {
 
     // Per-frame device scratch (high-water-mark allocations).
     DeviceBuffer<uint32_t> block_sums, totals;
-    DeviceBuffer<unsigned long long> scan_state;
     SortPlan segment_plan{};  // digits of the main sort, from the bounds seen by the line-setup pass
 
     template <class T>
@@ -59,17 +58,20 @@ class Renderer {
         std::swap(a.ptr, b.ptr);
         std::swap(a.capacity, b.capacity);
     }
-    // launch_radix_sort of keys (+ vals, may be null) with sort_scratch; the sorted data ends up
-    // in keys / vals: the buffers trade places with their twins when it landed there.
+    // launch_radix_sort of keys (+ vals, may be null) with sort_scratch, or with `scratch` and the
+    // digit histogram `hist` counted by the keys' producer; the sorted data ends up in keys /
+    // vals: the buffers trade places with their twins when it landed there.
     SortResult sort(DeviceBuffer<uint64_t>& keys, DeviceBuffer<uint64_t>& keys_tmp, DeviceBuffer<uint32_t>* vals,
                     DeviceBuffer<uint32_t>* vals_tmp, uint32_t n, const SortPlan& plan, cudaEvent_t* pass_events = nullptr,
-                    const uint32_t* n_dev = nullptr);
+                    const uint32_t* n_dev = nullptr, const uint32_t* hist = nullptr, void* scratch = nullptr);
     DeviceBuffer<uint64_t> segs, segs_tmp;
     DeviceBuffer<uint8_t> sort_scratch;
-    DeviceBuffer<uint32_t> cell_start, perm, perm_tmp, gap_count, eid, eid_tmp, gid_tmp, heavy_tiles;
+    DeviceBuffer<uint8_t> table_scratch;  // see TableScratch (kernels.h); zeroed per frame by build_tables
+    uint32_t* heavy_count() const { return reinterpret_cast<uint32_t*>(table_scratch.ptr); }  // TableScratch::heavy_count == 0
+    DeviceBuffer<uint32_t> cell_start, perm, perm_tmp, eid, eid_tmp, gid_tmp, heavy_tiles;
     DeviceBuffer<uint2> tile_range;
     DeviceBuffer<uint64_t> cell_key, key2, key2_tmp, ekey, ekey_tmp, gkey_tmp;
-    DeviceBuffer<uint4> cell_cover, carry_in, carry_after, gap_carry;
+    DeviceBuffer<uint4> cell_cover, carry_in, gap_carry;
     DeviceBuffer<uint8_t> eflags, framebuffer;
     DeviceBuffer<EntryRec> recs;
     // The painter-table scratch by the count that sizes it (see build_tables): per cell, per
@@ -82,8 +84,7 @@ class Renderer {
         return e;
     }
     cudaError_t reserve_cell_tables(size_t n_cells) {
-        return reserve_all(n_cells + 1, cell_start, cell_key, cell_cover, carry_in, carry_after, key2, key2_tmp, perm, perm_tmp,
-                           gap_count);
+        return reserve_all(n_cells + 1, cell_start, cell_key, cell_cover, carry_in, key2, key2_tmp, perm, perm_tmp);
     }
     cudaError_t reserve_gap_tables(size_t n_gaps) { return reserve_all(n_gaps + 1, ekey_tmp, eid_tmp, gkey_tmp, gid_tmp, gap_carry); }
     cudaError_t reserve_entry_tables(size_t n_entries) { return reserve_all(n_entries, ekey, eid, eflags, recs); }
@@ -216,9 +217,9 @@ class Renderer {
     int begin_frame(PaintScene& S, const uint8_t* buffer, uint64_t width, uint64_t stride, uint64_t height,
                     const uint32_t channels[4], const float clear[4], const forma_rect* crop);
     int bind_frame(Composition& comp, PaintScene& S, LayerCache* cache, const float clear[4], bool pack_written);
-    int build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint32_t prev_cells, uint32_t prev_gaps, uint32_t* n_entries,
+    int build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint32_t prev_cells, uint32_t prev_gaps, uint32_t* heavy_lists,
                      DevCounts& dc);
-    int index_tiles(const PaintScene& S, uint32_t n, uint32_t n_entries, const DevCounts& dc, uint32_t* heavy_lists);
+    int queue_row_costs(const PaintScene& S, uint32_t n);
     int paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t stride, bool in_bands, const uint32_t* heavy_lists,
               uint32_t* paint_launches);
     int copy_to_host(const PaintScene& S, uint8_t* buffer, const uint8_t* fb, uint64_t stride, cudaStream_t s);
