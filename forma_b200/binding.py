@@ -72,6 +72,7 @@ RGB1 = (Channel.Red, Channel.Green, Channel.Blue, Channel.One)
 BGR1 = (Channel.Blue, Channel.Green, Channel.Red, Channel.One)
 
 LAYER_LIMIT = (1 << 21) - 1
+ID_NONE = 0xFFFFFFFF  # FORMA_ID_NONE: no layer hits the pixel (see Renderer.render_ids)
 
 
 class OrderError(ValueError):
@@ -275,6 +276,11 @@ SIGNATURES = {
     "layer_cache_clear": (None, [_vp]),
     "renderer_render": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CRect), _vp, C.POINTER(_CTimings)]),
     "renderer_render_device": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CRect), _vp, C.POINTER(_CTimings)]),
+    "renderer_render_ids": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_uint64, C.c_uint64, C.POINTER(_CRect), _f, C.POINTER(_CTimings)]),
+    "renderer_render_ids_device": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_uint64, C.c_uint64, C.POINTER(_CRect), _f,
+                                             C.POINTER(_CTimings)]),
+    "renderer_render_device_with_ids": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CRect),
+                                                  _vp, C.c_uint64, _f, C.POINTER(_CTimings)]),
     "renderer_launch_count": (C.c_uint64, [_vp]),
     "renderer_stage_times": (None, [_vp, C.POINTER(C.c_double)]),
     "renderer_counters": (None, [_vp, _u64p]),
@@ -304,6 +310,11 @@ SIGNATURES = {
 }
 
 
+# The ID-frame entry points. A library may be built without them (it then loads, and the ID
+# methods of Renderer fail); `Api.attach` can take them from a companion library.
+ID_FRAME_SYMBOLS = ("renderer_render_ids", "renderer_render_ids_device", "renderer_render_device_with_ids")
+
+
 class Api:
     """Typed access to one shared library exporting `<prefix><name>` symbols."""
 
@@ -313,11 +324,20 @@ class Api:
             try:
                 fn = getattr(lib, prefix + name)
             except AttributeError:
-                if name in optional:
+                if name in optional or name in ID_FRAME_SYMBOLS:
                     continue
                 raise
             fn.restype, fn.argtypes = res, args
             setattr(self, name + "_fn" if name in ("set_option", "get_option") else name, fn)
+
+    def attach(self, lib: C.CDLL, names: Sequence[str]) -> "Api":
+        """Binds `names` (keys of SIGNATURES) from `lib`, a library with the same symbol prefix
+        that works on this library's objects."""
+        for name in names:
+            fn = getattr(lib, self.prefix + name)
+            fn.restype, fn.argtypes = SIGNATURES[name]
+            setattr(self, name, fn)
+        return self
 
     def check(self, status: int, what: str) -> None:
         if status == 0:
@@ -719,6 +739,56 @@ class Renderer:
             C.byref(t) if t is not None else None)
         self._api.check(st, "Renderer::render_device")
         return Timings(t.line_setup_ms, t.rasterize_ms, t.sort_ms, t.paint_ms, t.n_lines, t.n_segments) if t is not None else None
+
+    @staticmethod
+    def _timings(t):
+        return Timings(t.line_setup_ms, t.rasterize_ms, t.sort_ms, t.paint_ms, t.n_lines, t.n_segments) if t is not None else None
+
+    def render_ids(self, composition: Composition, ids: np.ndarray, width: int, height: int, crop: Optional[Rect] = None,
+                   stride: Optional[int] = None, min_coverage: float = 0.0, timings: bool = True) -> Optional[Timings]:
+        """ID frame into a host array: per pixel the order of the top-most Draw layer whose coverage
+        (x clip mask) exceeds `min_coverage`, or ID_NONE. `ids`: writable contiguous uint32 array
+        of >= height * stride / 4 elements; `stride` in bytes (default 4 * width). Only the crop's
+        tile rectangle is written."""
+        stride = width * 4 if stride is None else stride
+        assert ids.dtype == np.uint32 and ids.flags["C_CONTIGUOUS"] and ids.size * 4 >= height * stride
+        _, _, rect = self._common(RGBA, Color(), crop)
+        t = _CTimings() if timings else None
+        st = self._api.renderer_render_ids(self._h, composition._h, ids.ctypes.data_as(C.c_void_p), width, stride, height,
+                                           C.byref(rect) if rect is not None else None, float(min_coverage),
+                                           C.byref(t) if t is not None else None)
+        self._api.check(st, "Renderer::render_ids")
+        return self._timings(t)
+
+    def render_ids_device(self, composition: Composition, device_ptr: int, width: int, height: int,
+                          crop: Optional[Rect] = None, stride: Optional[int] = None, min_coverage: float = 0.0,
+                          timings: bool = True) -> Optional[Timings]:
+        """render_ids into device memory (e.g. a torch int32 / uint32 tensor's data_ptr())."""
+        stride = width * 4 if stride is None else stride
+        _, _, rect = self._common(RGBA, Color(), crop)
+        t = _CTimings() if timings else None
+        st = self._api.renderer_render_ids_device(self._h, composition._h, C.c_void_p(device_ptr), width, stride, height,
+                                                  C.byref(rect) if rect is not None else None, float(min_coverage),
+                                                  C.byref(t) if t is not None else None)
+        self._api.check(st, "Renderer::render_ids_device")
+        return self._timings(t)
+
+    def render_device_with_ids(self, composition: Composition, device_ptr: int, ids_device_ptr: int, width: int, height: int,
+                               channels=RGBA, clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), crop: Optional[Rect] = None,
+                               stride: Optional[int] = None, ids_stride: Optional[int] = None, min_coverage: float = 0.0,
+                               timings: bool = True) -> Optional[Timings]:
+        """render_device (without a layer cache) and render_ids_device of the same frame from one
+        pass through the stages; both pointers are device memory."""
+        stride = width * 4 if stride is None else stride
+        ids_stride = width * 4 if ids_stride is None else ids_stride
+        ch, cc, rect = self._common(channels, clear_color, crop)
+        t = _CTimings() if timings else None
+        st = self._api.renderer_render_device_with_ids(
+            self._h, composition._h, C.c_void_p(device_ptr), width, stride, height, ch, cc,
+            C.byref(rect) if rect is not None else None, C.c_void_p(ids_device_ptr), ids_stride, float(min_coverage),
+            C.byref(t) if t is not None else None)
+        self._api.check(st, "Renderer::render_device_with_ids")
+        return self._timings(t)
 
     def launch_count(self) -> int:
         return int(self._api.renderer_launch_count(self._h))

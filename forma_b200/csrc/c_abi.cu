@@ -389,6 +389,34 @@ int forma_renderer_render_device(forma_renderer* r, forma_composition* c, uint8_
                            cache ? &cache->c : nullptr, timings);
     });
 }
+int forma_renderer_render_ids(forma_renderer* r, forma_composition* c, uint32_t* ids, uint64_t width, uint64_t ids_stride,
+                              uint64_t height, const forma_rect* crop, float min_coverage, forma_timings* timings) {
+    return guarded((int)FORMA_ERR_CAPACITY, [&] {
+        return r->r.render_ids(c->c, nullptr, 0, nullptr, nullptr, ids, false, width, ids_stride, height, crop, min_coverage,
+                               timings);
+    });
+}
+int forma_renderer_render_ids_device(forma_renderer* r, forma_composition* c, uint32_t* device_ids, uint64_t width,
+                                     uint64_t ids_stride, uint64_t height, const forma_rect* crop, float min_coverage,
+                                     forma_timings* timings) {
+    return guarded((int)FORMA_ERR_CAPACITY, [&] {
+        return r->r.render_ids(c->c, nullptr, 0, nullptr, nullptr, device_ids, true, width, ids_stride, height, crop,
+                               min_coverage, timings);
+    });
+}
+int forma_renderer_render_device_with_ids(forma_renderer* r, forma_composition* c, uint8_t* device_buffer, uint64_t width,
+                                          uint64_t width_stride, uint64_t height, const uint32_t channels[4],
+                                          const float clear_color[4], const forma_rect* crop, uint32_t* device_ids,
+                                          uint64_t ids_stride, float min_coverage, forma_timings* timings) {
+    return guarded((int)FORMA_ERR_CAPACITY, [&] {
+        if (!device_buffer) {
+            set_error("forma_renderer_render_device_with_ids: no RGBA buffer");
+            return (int)FORMA_STATUS_INVALID;
+        }
+        return r->r.render_ids(c->c, device_buffer, width_stride, channels, clear_color, device_ids, true, width, ids_stride,
+                               height, crop, min_coverage, timings);
+    });
+}
 // --- shared frames (multi-GPU, see include/forma_b200.h) -----------------------
 static_assert(sizeof(cudaIpcMemHandle_t) == sizeof(forma_ipc_handle), "CUDA IPC handles are 64 bytes");
 int forma_shared_frame_create(int device, uint64_t bytes, void** device_ptr, forma_ipc_handle* handle) {

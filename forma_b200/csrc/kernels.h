@@ -219,6 +219,13 @@ void launch_merge_entries(const PaintScene& S, const uint64_t* cell_key, uint32_
                           uint32_t* heavy, uint32_t* heavy_count, cudaStream_t st, const DevCounts& dc = DevCounts());
 void launch_paint(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range, const uint32_t* heavy,
                   const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st);
+// ID frame (kernels_ids.cu): per pixel of the tile rectangle of S (clipped to the frame), the
+// order of the top-most Draw layer whose coverage x clip mask exceeds min_coverage, or
+// FORMA_ID_NONE. Reads the tables like launch_paint (never `eflags`); id_flags: one byte per
+// entry of scratch. ids_stride in bytes.
+void launch_paint_ids(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range,
+                      const uint32_t* heavy, const uint32_t* heavy_count, uint8_t* id_flags, uint32_t* ids, size_t ids_stride,
+                      float min_coverage, uint32_t* tile_counter, cudaStream_t st);
 // GradRec of every style slot (see device_types.h).
 void launch_grad_setup(const StyleRec* styles, const StopRec* stops, uint32_t n_styles, GradRec* grads, cudaStream_t st);
 // Pixel-pair fp32 arithmetic of the painter against scalar IEEE operations; mismatches are added to out[0].

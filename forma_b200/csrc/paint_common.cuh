@@ -1,5 +1,6 @@
-// Helpers shared by the painter-table kernels (kernels_tables.cu) and the
-// painter itself (kernels_painter.cu): key field access, packed 16 x i8 covers.
+// Helpers shared by the painter-table kernels (kernels_tables.cu), the painter itself
+// (kernels_painter.cu) and the ID kernel (kernels_ids.cu): key field access, packed 16 x i8
+// covers, the per-entry accumulation of segments into packed cells and the coverage rules.
 #pragma once
 
 #include "cuda_common.cuh"
@@ -65,6 +66,68 @@ __device__ __forceinline__ uint32_t fill_rule_of(const PaintScene& S, uint32_t l
     return slot >= 0 ? S.styles[slot].fill_rule : 0u;
 }
 
+
+// --- per-entry accumulation of the painter and the ID kernel -------------------------
+// Shared-memory word of pixel (local_x, local_y): row-major, ly * 16 + lx, i.e. the segment's
+// (local_x, local_y) byte with its nibbles swapped. Lane l = 2 ly + lx / 8 owns the eight
+// consecutive words l * 8 .. + 8 (two 16-byte accesses, two-way bank conflict: negligible
+// next to the index arithmetic a swizzle would cost per segment).
+__device__ __forceinline__ uint32_t cell_index_of(uint64_t s) {
+    const uint32_t t = (uint32_t)(s >> 12);  // bits 7..4 local_x, 3..0 local_y
+    return ((t & 15u) << 4) | ((t >> 4) & 15u);
+}
+
+// doubled_area_to_coverage (cpu/painter/mod.rs:76-94) by fill rule. The clamp of the
+// non-zero rule only ever sees a non-negative, non-NaN value: min(v, 1) is the same result.
+__device__ __forceinline__ float coverage_non_zero(int32_t doubled_area) {
+    return fminf(fabsf((float)doubled_area * (1.0f / 512.0f)), 1.0f);
+}
+__device__ __forceinline__ float coverage_even_odd(int32_t doubled_area) {
+    return (float)(512 - abs((doubled_area & 1023) - 512)) * (1.0f / 512.0f);
+}
+
+constexpr uint32_t kPackedSegLimit = 2016u;  // segments per normalisation round of the packed cells (< 2048)
+
+// acc_segment (cpu/painter/mod.rs:257-271) for one segment: area and cover into the packed cell.
+__device__ __forceinline__ void scatter_one(uint32_t* cells, uint64_t s) {
+    const int32_t cv = (int32_t)(((uint32_t)s & 0x3Fu) ^ 0x20u) - 0x20;
+    const int32_t dam = (int32_t)((uint32_t)(s >> 6) & 0x3Fu);
+    atomicAdd(&cells[cell_index_of(s)], (uint32_t)((dam * cv) * 65536 + cv));
+}
+
+// Segments 64.. of a long entry (about one entry in ten has more than 64). Every
+// kPackedSegLimit segments the low halves are folded back to i8 so that they cannot overflow
+// 16 bits (areas wrap at i16, covers at i8, exactly like the reference's lanes).
+__device__ __noinline__ inline void scatter_rest(const uint64_t* __restrict__ segs, uint32_t from, uint32_t s1, uint32_t* cells,
+                                                 uint32_t lane) {
+    uint32_t done = 64u;
+    for (uint32_t i0 = from; i0 < s1; i0 += 32u) {
+        if (i0 + lane < s1) scatter_one(cells, segs[i0 + lane]);
+        done += 32u;
+        if (done >= kPackedSegLimit && i0 + 32u < s1) {
+            __syncwarp();
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+                const uint32_t w = cells[k * 32 + lane];
+                const int32_t lo = (int32_t)(int16_t)(w & 0xFFFFu);
+                const uint32_t area = (w - (uint32_t)lo) & 0xFFFF0000u;
+                cells[k * 32 + lane] = area + (uint32_t)(int32_t)(int8_t)lo;
+            }
+            __syncwarp();
+            done = 0;
+        }
+    }
+}
+
+// Scatter-adds the segments [s0, s1) of one entry into `cells`. `pre0` / `pre1` hold the
+// first two 32-segment chunks (requested one entry earlier).
+__device__ __forceinline__ void scatter_entry(const uint64_t* __restrict__ segs, uint32_t s0, uint32_t s1, uint64_t pre0,
+                                              uint64_t pre1, uint32_t* cells, uint32_t lane) {
+    const uint32_t n = s1 - s0;
+    if (lane < n) scatter_one(cells, pre0);
+    if (lane + 32u < n) scatter_one(cells, pre1);
+    if (n > 64u) scatter_rest(segs, s0 + 64u, s1, cells, lane);
+}
 
 // Cells that cannot influence a painted tile (rows outside the painted band,
 // columns right of it) get this key in both pair sorts: it sorts last and keeps

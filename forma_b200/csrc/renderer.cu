@@ -4,6 +4,7 @@
 // every stage is a CUDA kernel sequence on one stream, and there is no CPU
 // fallback: without a usable sm_90 device forma_renderer_new() fails.
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <vector>
 
@@ -434,6 +435,115 @@ int Renderer::render(Composition& comp, uint8_t* buffer, bool buffer_on_device, 
             if (kv.second->enabled) kv.second->unchanged_bits |= 1u << cache->id;
             else kv.second->unchanged_bits &= ~(1u << cache->id);
         }
+    }
+    return FORMA_STATUS_OK;
+}
+
+// An ID frame, alone (rgba == nullptr) or after the RGBA frame of the same tables in device
+// memory (render_device's frame without a cache). The stages of render() run once; the
+// sync-free redo repeats the kernels. The ID frame never touches a layer cache.
+int Renderer::render_ids(Composition& comp, uint8_t* rgba, uint64_t rgba_stride, const uint32_t channels[4], const float clear[4],
+                         uint32_t* ids, bool ids_on_device, uint64_t width, uint64_t ids_stride, uint64_t height,
+                         const forma_rect* crop, float min_coverage, forma_timings* timings) {
+    if (!ids || ids_stride % 4u != 0u || !std::isfinite(min_coverage) || min_coverage < 0.0f || min_coverage >= 1.0f) {
+        set_error("invalid ID frame: stride %llu (a multiple of 4 bytes), min_coverage %g (finite, in [0, 1))",
+                  (unsigned long long)ids_stride, (double)min_coverage);
+        return FORMA_STATUS_INVALID;
+    }
+    PaintScene S{};
+    static const uint32_t kIdChannels[4] = {0, 1, 2, 3};
+    static const float kIdClear[4] = {0, 0, 0, 0};
+    int st = rgba ? begin_frame(S, rgba, width, rgba_stride, height, channels, clear, crop)
+                  : begin_frame(S, reinterpret_cast<const uint8_t*>(ids), width, ids_stride, height, kIdChannels, kIdClear, crop);
+    if (st) return st;
+    if (rgba && width * 4u > ids_stride) {
+        set_error("invalid ID frame stride %llu for width %llu", (unsigned long long)ids_stride, (unsigned long long)width);
+        return FORMA_STATUS_INVALID;
+    }
+
+    if (!prefetched) FORMA_CUDA_TRY(cudaEventRecord(timer.ev[0], stream));
+    prefetched = false;
+    const float band_lo = (float)(S.ty_lo * 16u), band_hi = (float)std::min<uint64_t>((uint64_t)S.ty_hi * 16u, height);
+    st = upload_tables(comp, -1);
+    if (st) return st;
+    st = flush_geometry(comp, band_lo, band_hi, S.ty_lo > 0u || S.ty_hi < S.tiles_y);
+    if (st) return st;
+    st = bind_frame(comp, S, nullptr, clear, false);
+    if (st) return st;
+
+    FORMA_CUDA_TRY(cudaEventRecord(timer.ev[7], stream));
+    uint32_t n = 0;
+    st = rasterize(comp, S.width, S.height, band_lo, band_hi, &n);
+    if (st) return st;
+    FORMA_CUDA_TRY(cudaEventRecord(timer.ev[2], stream));
+    int timed_sort_passes = 0;
+    if (n > 1) {
+        FORMA_CUDA_TRY(sort_scratch.reserve(radix_scratch_bytes(n)));
+        timed_sort_passes = sort(segs, segs_tmp, nullptr, nullptr, n, segment_plan, timer.sort_ev).timed_passes;
+        FORMA_CUDA_TRY(cudaGetLastError());
+    }
+    FORMA_CUDA_TRY(cudaEventRecord(timer.ev[3], stream));
+
+    const size_t n_tiles_total = (size_t)S.tiles_x * S.tiles_y;
+    last_tiles_x = S.tiles_x;
+    last_tiles_y = S.tiles_y;
+    FORMA_CUDA_TRY(tile_range.reserve(n_tiles_total));
+    FORMA_CUDA_TRY(heavy_tiles.reserve(n_tiles_total * kHeavyListClasses));
+    uint32_t* const heavy_lists = options().paint_lpt ? heavy_tiles.ptr : nullptr;
+    uint32_t* id_out = ids;
+    if (!ids_on_device) {
+        FORMA_CUDA_TRY(id_frame.reserve((size_t)(ids_stride / 4u) * height));
+        id_out = id_frame.ptr;
+    }
+    // Tables + kernels, once or (when the sync-free bounds were too small) twice, as in render().
+    const uint32_t prev_cells = last_cells, prev_gaps = last_gaps;
+    const bool fast = options().sync_free && n > 0 && prev_cells > 0;
+    last_cells = last_entries = 0;
+    last_written_tiles = 0;
+    last_tables_redone = false;
+    uint32_t kernel_launches = 1;
+    for (bool sync_free = fast;; sync_free = false) {
+        DevCounts dc;
+        st = build_tables(S, n, sync_free, prev_cells, prev_gaps, heavy_lists, dc);
+        if (st) return st;
+        FORMA_CUDA_TRY(id_flags.reserve(std::max<size_t>(recs.capacity, 1)));
+        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[4], stream));
+        if (rgba) {
+            st = paint(S, rgba, rgba, rgba_stride, false, heavy_lists, &kernel_launches);
+            if (st) return st;
+            ++kernel_launches;
+        }
+        launch_paint_ids(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), id_flags.ptr, id_out, ids_stride,
+                         min_coverage, totals.ptr + 8, stream);
+        ++launches;
+        FORMA_CUDA_TRY(cudaGetLastError());
+        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[5], stream));
+        if (!ids_on_device) {
+            st = copy_to_host(S, reinterpret_cast<uint8_t*>(ids), reinterpret_cast<const uint8_t*>(id_out), ids_stride, stream);
+            if (st) return st;
+        }
+        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[6], stream));
+        FORMA_CUDA_TRY(cudaStreamSynchronize(stream));
+        if (!sync_free) break;
+        last_cells = pinned_totals[1];
+        last_gaps = pinned_totals[2];
+        last_entries = last_cells + last_gaps;
+        if (last_cells <= dc.cell_bound && last_gaps <= dc.gap_bound) break;
+        last_tables_redone = true;
+    }
+    last_tables_sync_free = fast && !last_tables_redone;
+    times_pending = true;
+    pending_sort_passes = timed_sort_passes;
+    pending_paint_launches = kernel_launches;
+    if (timings) {
+        resolve_times();
+        const CompDevice& cd = comp.on(res_key);
+        timings->line_setup_ms = stage_ms[1];
+        timings->rasterize_ms = stage_ms[2];
+        timings->sort_ms = stage_ms[3];
+        timings->paint_ms = stage_ms[4] + stage_ms[5];
+        timings->n_lines = cd.n_resident ? cd.n_resident - 1 : 0;
+        timings->n_segments = n;
     }
     return FORMA_STATUS_OK;
 }

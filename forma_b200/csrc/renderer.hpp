@@ -213,6 +213,13 @@ class Renderer {
     int render(Composition& comp, uint8_t* buffer, bool buffer_on_device, uint64_t width, uint64_t stride,
                uint64_t height, const uint32_t channels[4], const float clear[4], const forma_rect* crop,
                LayerCache* cache, forma_timings* timings);
+    // ID frames (see forma_renderer_render_ids): the stages of render() without a layer cache, with
+    // the ID kernel in place of paint() or, when `rgba` (a device frame) is given, after it.
+    DeviceBuffer<uint8_t> id_flags;   // per entry: the ID kernel's optimizer flags (clip tiles)
+    DeviceBuffer<uint32_t> id_frame;  // host ID frames: the frame on the device
+    int render_ids(Composition& comp, uint8_t* rgba, uint64_t rgba_stride, const uint32_t channels[4], const float clear[4],
+                   uint32_t* ids, bool ids_on_device, uint64_t width, uint64_t ids_stride, uint64_t height,
+                   const forma_rect* crop, float min_coverage, forma_timings* timings);
     // The stages of render(), in the order it runs them.
     int begin_frame(PaintScene& S, const uint8_t* buffer, uint64_t width, uint64_t stride, uint64_t height,
                     const uint32_t channels[4], const float clear[4], const forma_rect* crop);

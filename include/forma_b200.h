@@ -213,6 +213,37 @@ int forma_renderer_render_device(forma_renderer*, forma_composition*, uint8_t* d
                                  const forma_rect* crop, forma_layer_cache* cache,
                                  forma_timings* timings);
 
+/* ID frames (no reference counterpart): which layer made each pixel. One uint32 per pixel,
+ * row-major, `ids_stride` BYTES between rows (a multiple of 4, at least 4 * width). The value
+ * at pixel p is the order of the top-most Func::Draw layer that hits p, or FORMA_ID_NONE.
+ * A layer hits p where the painter would blend it at p with coverage x clip mask >
+ * min_coverage (the clip mask only where a clip applies to the layer): the painter's own tile
+ * walk and optimiser passes decide, fill colour, alpha, gradient, texture and blend mode do not.
+ * Clip layers, clipped layers without an active clip and disabled layers never hit; in a tile
+ * the optimiser folds into one solid colour every pixel gets the top-most Draw layer of the
+ * fold. Coverages are multiples of 1/512, so IDs are exact.
+ * Only the crop's tile rectangle (clipped to width x height) is written, as with RGBA frames.
+ * min_coverage must be finite and in [0, 1): otherwise INVALID_ARGUMENT and nothing is
+ * written. An ID frame takes no layer cache and leaves every cache as it was.
+ * render_ids copies the rectangle back into a HOST buffer; render_ids_device writes a device
+ * buffer on the renderer's device. */
+#define FORMA_ID_NONE 0xFFFFFFFFu
+int forma_renderer_render_ids(forma_renderer*, forma_composition*, uint32_t* ids, uint64_t width,
+                              uint64_t ids_stride, uint64_t height, const forma_rect* crop /* nullable */,
+                              float min_coverage, forma_timings* timings /* nullable */);
+int forma_renderer_render_ids_device(forma_renderer*, forma_composition*, uint32_t* device_ids, uint64_t width,
+                                     uint64_t ids_stride, uint64_t height, const forma_rect* crop /* nullable */,
+                                     float min_coverage, forma_timings* timings /* nullable */);
+/* An RGBA frame (forma_renderer_render_device without a cache: the same bytes) and its ID frame
+ * (forma_renderer_render_ids_device: the same IDs) from one pass through the stages: one
+ * upload, rasterization, sort and set of painter tables, then the paint and the ID kernel.
+ * Both buffers are in the renderer's device memory. */
+int forma_renderer_render_device_with_ids(forma_renderer*, forma_composition*, uint8_t* device_buffer,
+                                          uint64_t width, uint64_t width_stride, uint64_t height,
+                                          const uint32_t channels[4], const float clear_color[4],
+                                          const forma_rect* crop /* nullable */, uint32_t* device_ids,
+                                          uint64_t ids_stride, float min_coverage, forma_timings* timings /* nullable */);
+
 /* Launch on `cuda_stream` (a cudaStream_t, e.g. torch.cuda.current_stream().cuda_stream)
  * instead of the default stream. */
 void forma_renderer_set_stream(forma_renderer*, void* cuda_stream);
@@ -264,7 +295,8 @@ void forma_composition_evict(forma_composition*);
 uint64_t forma_composition_point_count(forma_composition*);
 /* Device-timeline milliseconds of the last render: [0] uploads, [1] line-setup
  * count pass, [2] pixel-grid intersection, [3] sort, [4] painter tables,
- * [5] paint kernel, [6] device->host copy, [7] whole call. */
+ * [5] paint kernel (ID frames: the ID kernel, after the paint kernel in the combined call),
+ * [6] device->host copy, [7] whole call. */
 void forma_renderer_stage_times(const forma_renderer*, double out_ms[8]);
 /* CUDA-event time of single kernels inside the last render, summed over their
  * launches: [0] radix downsweep (main sort, one launch per pass), [1] radix
