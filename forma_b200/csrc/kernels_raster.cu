@@ -193,6 +193,21 @@ __device__ __forceinline__ uint32_t integers_between(float u, float v) {  // seg
     return d_sat_u32(ceilf(mx) - floorf(mn) - 1.0f);
 }
 
+// Line lengths and their sums saturate at 0xFFFFFFFF instead of wrapping (the reference wraps
+// in release builds and panics in debug builds): a frame whose true total reaches 2^30 is then
+// refused by Renderer::rasterize instead of being rendered from a wrapped count. Below the
+// limit nothing saturates and every count is the reference's.
+__device__ __forceinline__ uint32_t sat_add(uint32_t a, uint32_t b) { return min(a, ~b) + b; }
+
+__device__ __forceinline__ uint32_t warp_inclusive_scan_sat(uint32_t v) {
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        uint32_t n = __shfl_up_sync(kFullMask, v, o);
+        if (lane_id() >= (unsigned)o) v = sat_add(v, n);
+    }
+    return v;
+}
+
 // segment.rs:298-383 for the point pair (i, i+1).
 __device__ __forceinline__ LineParams line_setup(const RasterArgs& A, uint32_t i) {
     LineParams L;
@@ -244,7 +259,7 @@ __device__ __forceinline__ LineParams line_setup(const RasterArgs& A, uint32_t i
     L.y0 = p0y * 16.0f;
     L.dx = dx * 16.0f;
     L.dy = dy * 16.0f;
-    L.length = integers_between(p0x, p1x) + integers_between(p0y, p1y) + 1u;
+    L.length = sat_add(sat_add(integers_between(p0x, p1x), integers_between(p0y, p1y)), 1u);
     return L;
 }
 
@@ -280,13 +295,13 @@ __global__ void __launch_bounds__(kRasterThreads) line_count_kernel(RasterArgs A
             warp_max[1][threadIdx.x >> 5] = by;
         }
     }
-    uint32_t incl = warp_inclusive_scan(len);
+    uint32_t incl = warp_inclusive_scan_sat(len);
     if (lane_id() == 31) warp_sums[threadIdx.x >> 5] = incl;
     __syncthreads();
     if (threadIdx.x == 0) {
         uint32_t s = 0, bx = 0, by = 0;
         for (int w = 0; w < kRasterThreads / 32; ++w) {
-            s += warp_sums[w];
+            s = sat_add(s, warp_sums[w]);
             bx = max(bx, warp_max[0][w]);
             by = max(by, warp_max[1][w]);
         }
@@ -299,7 +314,8 @@ __global__ void __launch_bounds__(kRasterThreads) line_count_kernel(RasterArgs A
 
 // Device-wide exclusive scan of `n` u32 values by ONE CTA (n = number of CTAs
 // of the producing kernel, a few thousand); writes the grand total to
-// total[0]. 1024 threads, each owning a contiguous chunk.
+// total[0]. 1024 threads, each owning a contiguous chunk. Saturating: every
+// offset and the total are min(true value, 0xFFFFFFFF).
 __global__ void __launch_bounds__(1024) scan_block_sums_kernel(uint32_t* __restrict__ data, uint32_t n,
                                                               uint32_t* __restrict__ total) {
     __shared__ uint32_t warp_tot[32];
@@ -312,25 +328,28 @@ __global__ void __launch_bounds__(1024) scan_block_sums_kernel(uint32_t* __restr
         uint32_t v[4];
 #pragma unroll
         for (int k = 0; k < 4; ++k) v[k] = (idx + k < n) ? data[idx + k] : 0u;
-        uint32_t sum = v[0] + v[1] + v[2] + v[3];
-        uint32_t incl = warp_inclusive_scan(sum);
+        uint32_t sum = sat_add(sat_add(v[0], v[1]), sat_add(v[2], v[3]));
+        uint32_t incl = warp_inclusive_scan_sat(sum);
+        uint32_t lane_excl = __shfl_up_sync(kFullMask, incl, 1);  // (a saturated sum cannot be subtracted from)
+        if (lane_id() == 0) lane_excl = 0;
         if (lane_id() == 31) warp_tot[threadIdx.x >> 5] = incl;
         __syncthreads();
         if (threadIdx.x < 32) {
             uint32_t w = warp_tot[threadIdx.x];
-            uint32_t wi = warp_inclusive_scan(w);
-            warp_tot[threadIdx.x] = wi - w;  // exclusive over warps
+            uint32_t wi = warp_inclusive_scan_sat(w);
+            uint32_t we = __shfl_up_sync(kFullMask, wi, 1);
+            warp_tot[threadIdx.x] = threadIdx.x ? we : 0u;  // exclusive over warps
             if (threadIdx.x == 31) round_total = wi;
         }
         __syncthreads();
-        uint32_t excl = carry + warp_tot[threadIdx.x >> 5] + (incl - sum);
+        uint32_t excl = sat_add(sat_add(carry, warp_tot[threadIdx.x >> 5]), lane_excl);
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
             if (idx + k < n) data[idx + k] = excl;
-            excl += v[k];
+            excl = sat_add(excl, v[k]);
         }
         __syncthreads();
-        if (threadIdx.x == 0) carry += round_total;
+        if (threadIdx.x == 0) carry = sat_add(carry, round_total);
         __syncthreads();
     }
     if (threadIdx.x == 0) total[0] = carry;
@@ -351,7 +370,14 @@ __device__ __forceinline__ float find_param(int32_t ii, double a_over, double b_
     return fminf(guess_a, guess_b);  // NaN-ignoring, like f32::min (SURVEY.md A.3)
 }
 
-__device__ __forceinline__ int32_t round_sub(float v) { return (int32_t)floorf(v + 0.5f); }  // rasterizer.rs:78-80
+// rasterizer.rs:78-80: `(v + 0.5).floor().to_int_unchecked()`. Rust leaves NaN and values outside
+// i32 undefined there; the reference's x86 build (cvttss2si) gives i32::MIN for them, and so does
+// the CPU restatement the tests compare with. A plain cast would compile to cvt.rzi.s32.f32, which saturates
+// to INT_MAX instead. Sub-pixel positions reach 2^31 at 2^27 px.
+__device__ __forceinline__ int32_t round_sub(float v) {
+    const float f = floorf(v + 0.5f);
+    return (f >= -2147483648.0f && f < 2147483648.0f) ? (int32_t)f : INT32_MIN;
+}
 
 struct SharedLines {
     float x0[kRasterThreads], y0[kRasterThreads], dx[kRasterThreads], dy[kRasterThreads];
@@ -375,7 +401,7 @@ __global__ void __launch_bounds__(kRasterThreads)
     const uint32_t warp = t >> 5, lane = t & 31u;
     uint32_t i = blockIdx.x * kRasterThreads + t;
     LineParams L = line_setup(A, i);
-    uint32_t incl = warp_inclusive_scan(L.length);
+    uint32_t incl = warp_inclusive_scan_sat(L.length);
     if (lane == 31) warp_sums[warp] = incl;
     if (L.length) {
         S.x0[t] = L.x0; S.y0[t] = L.y0; S.dx[t] = L.dx; S.dy[t] = L.dy;
@@ -391,14 +417,20 @@ __global__ void __launch_bounds__(kRasterThreads)
     uint32_t before = 0, block_total = 0;  // segments of the warps before this one / of the whole block
 #pragma unroll
     for (uint32_t w = 0; w < (uint32_t)(kRasterThreads / 32); ++w) {
-        if (w < warp) before += warp_sums[w];
-        block_total += warp_sums[w];
+        if (w < warp) before = sat_add(before, warp_sums[w]);
+        block_total = sat_add(block_total, warp_sums[w]);
     }
+    // Exact unless the block's total saturated (a frame Renderer::rasterize refuses; the offsets
+    // then only steer the bisection, which stays inside S.excl).
     S.excl[t] = before + incl - L.length;  // exclusive prefix over the block's 256 lines
     __syncthreads();
     const uint32_t block_base = block_offsets[blockIdx.x];
+    // `cap` bounds a speculative launch made before the segment count is known on the host: the
+    // loop never runs past it, whatever the (saturated) counts of an over-limit frame. The last
+    // clamp keeps `s += kRasterThreads` from wrapping.
+    const uint32_t limit = min(min(block_total, block_base < cap ? cap - block_base : 0u), 0xFFFFFF00u);
 
-    for (uint32_t s = t; s < block_total; s += kRasterThreads) {
+    for (uint32_t s = t; s < limit; s += kRasterThreads) {
         // Largest j in [0, 256) with excl[j] <= s (zero-length lines share their
         // successor's offset and are skipped by taking the largest such j).
         uint32_t j = 0;
@@ -435,8 +467,7 @@ __global__ void __launch_bounds__(kRasterThreads)
         uint64_t tx = (uint64_t)max((int32_t)(int16_t)(tile_x + 1), 0) & 0xFFFull;
         uint64_t v = (ty << 53) | (tx << 41) | ((uint64_t)(S.order[li] & 0x1FFFFFu) << 20) | ((uint64_t)local_x << 16) |
                      ((uint64_t)local_y << 12) | ((uint64_t)(dam & 0x3Fu) << 6) | ((uint64_t)((uint32_t)cover & 0x3Fu));
-        // `cap` guards a speculative launch made before the segment count is known on the host.
-        if (block_base + s < cap) out[(uint64_t)block_base + s] = v;
+        out[(uint64_t)block_base + s] = v;
     }
 }
 

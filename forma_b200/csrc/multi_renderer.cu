@@ -341,7 +341,13 @@ int sliced_host_render(forma_renderer* r, forma_composition* c, uint8_t* buffer,
     }
     const int st = multi_render_impl(m, c, buffer, false, width, stride, height, channels, clear, crop, timings, n,
                                      options().slice_chain != 0);
-    if (st) return st;
+    if (st) {  // a failed frame describes nothing: no segments, cells, row costs or slices to inspect
+        P.last_segments = P.last_cells = P.last_entries = 0;
+        P.last_tiles_x = P.last_tiles_y = 0;
+        P.last_slices = 0;
+        P.last_raster_valid = false;
+        return st;
+    }
     // What the caller reads from this renderer after a frame: sums over the slices; stage times:
     // the slowest slice (the slices overlap, so their sum means nothing).
     P.last_segments = P.last_cells = P.last_entries = 0;

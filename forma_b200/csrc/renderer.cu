@@ -290,12 +290,23 @@ int Renderer::rasterize(Composition& comp, uint32_t width, uint32_t height, floa
         const uint64_t bound[3] = {layer_bound, pinned_totals[4], pinned_totals[5]};
         segment_plan = make_sort_plan(segment_key_layout(), bound);  // layer, tile_x, tile_y
     }
-    *n_out = n;
-    last_segments = n;
+    *n_out = 0;
+    last_segments = 0;  // (forma_renderer_segments / _row_costs read segs[0, last_segments))
+    // n saturates at 0xFFFFFFFF (line_count_kernel, scan_block_sums_kernel): a frame at or above
+    // the limit is refused, never rendered from a wrapped count. Nothing of it stays behind: the
+    // speculative emit wrote only inside `segs`, and the layer cache, its unchanged bits and the
+    // sync-free bounds (last_cells / last_gaps) are updated only by a frame that gets past here,
+    // and the segment count and tile rows of the last frame read 0.
     if (n >= (1u << 30)) {
-        set_error("%u pixel segments exceed the 2^30 limit of the sort's look-back counters", n);
+        if (n == 0xFFFFFFFFu)
+            set_error("at least 2^32 - 1 pixel segments exceed the 2^30 limit of the sort's look-back counters");
+        else
+            set_error("%u pixel segments exceed the 2^30 limit of the sort's look-back counters", n);
+        last_tiles_x = last_tiles_y = 0;  // no row costs either
         return FORMA_STATUS_CAPACITY;
     }
+    *n_out = n;
+    last_segments = n;
     FORMA_CUDA_TRY(reserve_all(n + 1, segs, segs_tmp));
     if (!speculated || (size_t)n + 1 > spec_cap) {
         if (!speculated && timer.ok) FORMA_CUDA_TRY(cudaEventRecord(timer.ev[1], stream));  // end of line setup (count pass)

@@ -36,7 +36,9 @@ enum {
     FORMA_ERR_ORDER_LIMIT = 2,      /* OrderError::ExceededLayerLimit, utils/order.rs:56-65 */
     FORMA_ERR_CUDA = 3,             /* a CUDA call failed; see forma_last_error()          */
     FORMA_ERR_NO_DEVICE = 4,        /* no usable sm_90 device: there is NO CPU fallback    */
-    FORMA_ERR_CAPACITY = 5          /* an internal device buffer could not be grown        */
+    FORMA_ERR_CAPACITY = 5          /* an internal device buffer could not be grown, or a
+                                       frame needs 2^30 or more pixel segments (refused
+                                       before anything is painted; no count wraps)         */
 };
 
 /* Human-readable description of the last failure on the calling thread. */

@@ -11,6 +11,7 @@
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
+#include <string>
 
 #ifdef _OPENMP
 #include <omp.h>
@@ -104,7 +105,16 @@ static double now_ms() {
 }
 
 // cpu/renderer.rs:75-224
-static void render(Renderer& r, Composition& comp, const RenderTarget& rt, const uint32_t channels_in[4],
+// The reason the last call failed (fo_last_error).
+static thread_local std::string g_error;
+
+static void refuse_segments(const Lines& L) {
+    g_error = std::to_string(L.total) + " pixel segments exceed the " + std::to_string(kSegmentLimit) +
+              " that u32 prefix sums can index";
+}
+
+// Returns false, with nothing painted, when rasterize() refuses the frame.
+static bool render(Renderer& r, Composition& comp, const RenderTarget& rt, const uint32_t channels_in[4],
                    const Color& clear_color, const Rect* crop, LayerCache* cache) {
     Channel ch[4];
     for (int k = 0; k < 4; ++k) {
@@ -126,7 +136,10 @@ static void render(Renderer& r, Composition& comp, const RenderTarget& rt, const
     double t0 = now_ms();
     comp.fill_cpu_view(rt.width, rt.height, r.lines);
     double t1 = now_ms();
-    rasterize(r.lines, r.segments);
+    if (!rasterize(r.lines, r.segments)) {
+        refuse_segments(r.lines);
+        return false;
+    }
     double t2 = now_ms();
     sort_segments(r.segments);
     double t3 = now_ms();
@@ -173,6 +186,7 @@ static void render(Renderer& r, Composition& comp, const RenderTarget& rt, const
     r.last.paint_ms = t4 - t3;
     r.last.n_lines = r.lines.size();
     r.last.n_segments = r.segments.size();
+    return true;
 }
 
 }  // namespace fo
@@ -439,7 +453,8 @@ int fo_renderer_render(void* rv, void* cv, uint8_t* buffer, uint64_t width, uint
         rect.vert1 = (crop->vert_end + kTile - 1) / kTile;
     }
     Color cc{clear[0], clear[1], clear[2], clear[3]};
-    render(*r, *(Composition*)cv, rt, channels, cc, crop ? &rect : nullptr, (LayerCache*)cache);
+    if (!render(*r, *(Composition*)cv, rt, channels, cc, crop ? &rect : nullptr, (LayerCache*)cache))
+        return 5;  // FORMA_ERR_CAPACITY
     if (timings) {
         timings->line_setup_ms = r->last.line_setup_ms;
         timings->rasterize_ms = r->last.rasterize_ms;
@@ -480,7 +495,10 @@ uint64_t fo_renderer_segments(void* rv, uint64_t cap, uint64_t* segs) {
 uint64_t fo_renderer_rasterize_only(void* rv, void* cv, uint64_t width, uint64_t height, uint64_t cap, uint64_t* segs) {
     Renderer* r = (Renderer*)rv;
     ((Composition*)cv)->fill_cpu_view(width, height, r->lines);
-    rasterize(r->lines, r->segments);
+    if (!rasterize(r->lines, r->segments)) {
+        refuse_segments(r->lines);
+        return 0;
+    }
     std::memcpy(segs, r->segments.data(), std::min<size_t>(cap, r->segments.size()) * 8);
     return r->segments.size();
 }
@@ -491,7 +509,7 @@ int fo_renderer_sort_u64(void*, uint64_t* keys, uint64_t n) {
     return 0;
 }
 uint64_t fo_renderer_launch_count(const void*) { return 0; }
-const char* fo_last_error() { return ""; }
+const char* fo_last_error() { return g_error.c_str(); }
 
 // --- small known-answer hooks (reference unit tests) ------------------------
 float fo_find(int32_t i, float a, float b, float c, float d) {

@@ -13,14 +13,14 @@
 
 namespace fo {
 
-static void render_ids(Composition& comp, uint32_t* ids, size_t width, size_t stride, size_t height, const Rect* crop,
+static bool render_ids(Composition& comp, uint32_t* ids, size_t width, size_t stride, size_t height, const Rect* crop,
                        float min_coverage, size_t* n_lines, size_t* n_segments) {
     size_t ht = (height + kTile - 1) / kTile;
     comp.compact_geom();
     Lines lines;
     std::vector<uint64_t> segments;
     comp.fill_cpu_view(width, height, lines);
-    rasterize(lines, segments);
+    if (!rasterize(lines, segments)) return false;  // more pixel segments than u32 sums can index
     // By key only, like the reference's sort: the order inside a key does not change the painter's
     // wrapping sums.
     std::sort(segments.begin(), segments.end(), [](uint64_t a, uint64_t b) { return (a >> kSortShift) < (b >> kSortShift); });
@@ -46,6 +46,7 @@ static void render_ids(Composition& comp, uint32_t* ids, size_t width, size_t st
     }
     *n_lines = lines.size();
     *n_segments = segments.size();
+    return true;
 }
 
 }  // namespace fo
@@ -76,8 +77,9 @@ int fo_renderer_render_ids(void*, void* cv, uint32_t* ids, uint64_t width, uint6
         rect.vert1 = (crop->vert_end + kTile - 1) / kTile;
     }
     size_t n_lines = 0, n_segments = 0;
-    render_ids(*(Composition*)cv, ids, (size_t)width, (size_t)stride, (size_t)height, crop ? &rect : nullptr, min_coverage,
-               &n_lines, &n_segments);
+    if (!render_ids(*(Composition*)cv, ids, (size_t)width, (size_t)stride, (size_t)height, crop ? &rect : nullptr, min_coverage,
+                    &n_lines, &n_segments))
+        return 5;  // FORMA_ERR_CAPACITY
     if (timings) {
         *timings = fo_ids_timings{};
         timings->n_lines = n_lines;

@@ -75,8 +75,13 @@ inline void ith_params(uint32_t i_in, float a, float b, float c, float d, float*
     *t1 = rmin(f1, 1.0f);
 }
 
-// cpu/rasterizer.rs:78-80
-inline int32_t round_sub(float v) { return (int32_t)std::floor(v + 0.5f); }
+// cpu/rasterizer.rs:78-80: `(v + 0.5).floor().to_int_unchecked()`, undefined in Rust for NaN and
+// values outside i32. The reference's x86 build (cvttss2si) gives i32::MIN for them; so does this,
+// explicitly rather than by the same undefined cast in C++.
+inline int32_t round_sub(float v) {
+    const float f = std::floor(v + 0.5f);
+    return (f >= -2147483648.0f && f < 2147483648.0f) ? (int32_t)f : INT32_MIN;
+}
 
 // cpu/rasterizer.rs:100-157 — the k-th pixel segment of line `li`.
 inline uint64_t pixel_segment(const Lines& L, size_t li, uint32_t k) {
@@ -100,11 +105,18 @@ inline uint64_t pixel_segment(const Lines& L, size_t li, uint32_t k) {
     return pack_segment(L.orders[li], tile_x, tile_y, local_x, local_y, dam, cover);
 }
 
+constexpr uint64_t kSegmentLimit = 0xFFFFFFFFull;  // what u32 prefix sums can index
+
 // cpu/rasterizer.rs:93-159 with utils/prefix_scan.rs:30-63 enumerating
-// (line, k) pairs from the inclusive prefix sums.
-inline void rasterize(const Lines& L, std::vector<uint64_t>& out) {
+// (line, k) pairs from the inclusive prefix sums. Returns false, with no segments, when the
+// true count exceeds kSegmentLimit: the wrapped sums would index past `out`.
+inline bool rasterize(const Lines& L, std::vector<uint64_t>& out) {
     size_t n_lines = L.size();
-    size_t total = n_lines ? L.lengths[n_lines - 1] : 0;
+    if (L.total > kSegmentLimit) {
+        out.clear();
+        return false;
+    }
+    size_t total = L.total;
     out.resize(total);
 #pragma omp parallel for schedule(dynamic, 1024)
     for (size_t li = 0; li < n_lines; ++li) {
@@ -112,6 +124,7 @@ inline void rasterize(const Lines& L, std::vector<uint64_t>& out) {
         uint32_t incl = L.lengths[li];
         for (uint32_t s = excl; s < incl; ++s) out[s] = pixel_segment(L, li, s - excl);
     }
+    return true;
 }
 
 // cpu/rasterizer.rs:162-164 — crumsort is an unstable comparison sort on the

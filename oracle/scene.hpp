@@ -84,8 +84,9 @@ struct Layer {
 
 // segment.rs:530-545 (the x/y/ids part) and the per-frame line arrays.
 struct Lines {
-    std::vector<uint32_t> orders, lengths;  // lengths: inclusive prefix sums
+    std::vector<uint32_t> orders, lengths;  // lengths: inclusive prefix sums, wrapping in u32 like the reference's
     std::vector<float> x0, y0, dx, dy, a, b, c, d;
+    uint64_t total = 0;  // the true pixel-segment count (a saturated integers_between counts as 2^32 - 1)
     size_t size() const { return orders.size(); }
     void resize(size_t n) {
         orders.resize(n);
@@ -257,6 +258,7 @@ struct Composition {
         size_t n = ids.empty() ? 0 : ids.size() - 1;
         if (x.size() < 2) n = 0;
         out.resize(n);
+        uint64_t wrapped = 0;  // lines whose own length wraps u32
 #pragma omp parallel
         {
         // id -> order -> layer (segment.rs:141-149: two FxHashMap look-ups per point). `layers` is an
@@ -265,7 +267,7 @@ struct Composition {
         uint64_t memo_id = 0;
         const Layer* memo_layer = nullptr;
         uint32_t memo_order = 0;
-#pragma omp for schedule(static)
+#pragma omp for schedule(static) reduction(+ : wrapped)
         for (size_t i = 0; i < n; ++i) {
             auto empty = [&] {
                 out.orders[i] = 0;
@@ -315,14 +317,20 @@ struct Composition {
             out.b[i] = std::fabs(dy_recip);
             out.c[i] = tox;
             out.d[i] = toy;
-            out.lengths[i] = integers_between(p0.x, p1.x) + integers_between(p0.y, p1.y) + 1;
+            const uint64_t len = (uint64_t)integers_between(p0.x, p1.x) + integers_between(p0.y, p1.y) + 1u;
+            out.lengths[i] = (uint32_t)len;
+            wrapped += len >> 32;
         }
         }
-        uint32_t sum = 0;
+        // prefix_sum, segment.rs:90-98: the reference's u32 sums wrap (release builds) or panic
+        // (debug builds). Here they are kept in u64 and stored wrapped, so that rasterize() can
+        // refuse a frame whose true count does not fit instead of indexing past its output.
+        uint64_t sum = 0;
         for (size_t i = 0; i < n; ++i) {
             sum += out.lengths[i];
-            out.lengths[i] = sum;
+            out.lengths[i] = (uint32_t)sum;
         }
+        out.total = sum + (wrapped << 32);
     }
 };
 
