@@ -281,6 +281,11 @@ SIGNATURES = {
                                              C.POINTER(_CTimings)]),
     "renderer_render_device_with_ids": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CRect),
                                                   _vp, C.c_uint64, _f, C.POINTER(_CTimings)]),
+    "renderer_max_views": (C.c_uint32, [C.c_uint64]),
+    "renderer_render_views": (C.c_int, [_vp, _vp, _fp, C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, _u32p, _fp,
+                                        C.POINTER(_CTimings)]),
+    "renderer_render_views_device": (C.c_int, [_vp, _vp, _fp, C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, _u32p,
+                                               _fp, C.POINTER(_CTimings)]),
     "renderer_launch_count": (C.c_uint64, [_vp]),
     "renderer_stage_times": (None, [_vp, C.POINTER(C.c_double)]),
     "renderer_counters": (None, [_vp, _u64p]),
@@ -313,6 +318,9 @@ SIGNATURES = {
 # The ID-frame entry points. A library may be built without them (it then loads, and the ID
 # methods of Renderer fail); `Api.attach` can take them from a companion library.
 ID_FRAME_SYMBOLS = ("renderer_render_ids", "renderer_render_ids_device", "renderer_render_device_with_ids")
+# The entry points of views (Renderer.render_views): the CUDA library has them, other libraries
+# with this binding's symbols may not (the view methods of Renderer then fail).
+VIEW_SYMBOLS = ("renderer_max_views", "renderer_render_views", "renderer_render_views_device")
 
 
 class Api:
@@ -324,7 +332,7 @@ class Api:
             try:
                 fn = getattr(lib, prefix + name)
             except AttributeError:
-                if name in optional or name in ID_FRAME_SYMBOLS:
+                if name in optional or name in ID_FRAME_SYMBOLS or name in VIEW_SYMBOLS:
                     continue
                 raise
             fn.restype, fn.argtypes = res, args
@@ -789,6 +797,51 @@ class Renderer:
             C.byref(t) if t is not None else None)
         self._api.check(st, "Renderer::render_device_with_ids")
         return self._timings(t)
+
+    def max_views(self, height: int) -> int:
+        """The most views of `height` rows one render_views call of the library takes (0: none)."""
+        return int(self._api.renderer_max_views(height))
+
+    def _views(self, fn, what, composition, views, ptr, width, height, channels, clear_color, stride, view_stride, timings):
+        """Calls `fn` on chunks of at most max_views(height) views, view b at ptr + b * view_stride."""
+        v = np.ascontiguousarray(np.asarray(views, dtype=np.float32).reshape(-1, 6))
+        ch, cc, _ = self._common(channels, clear_color, None)
+        chunk = max(self.max_views(height), 1)
+        t = None
+        for first in range(0, max(len(v), 1), chunk):
+            part = v[first:first + chunk]
+            t = _CTimings() if timings else None
+            st = fn(self._h, composition._h, part.ctypes.data_as(_fp), len(part), C.c_void_p(ptr + first * view_stride), width, stride,
+                    height, view_stride, ch, cc, C.byref(t) if t is not None else None)
+            self._api.check(st, what)
+        return self._timings(t)
+
+    def render_views(self, composition: Composition, views, buffer: np.ndarray, width: int, height: int, channels=RGBA,
+                     clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
+                     view_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """One frame per row of `views`, an (N, 6) array-like of transforms in set_transform order
+        [ux, vx, uy, vy, tx, ty], each a frame of the composition with every layer's transform T
+        replaced by view ∘ T. Frame b starts at byte b * view_stride (default height * stride) of
+        `buffer`, a writable contiguous uint8 host array; `stride` (default 4 * width) is the row
+        stride. N may exceed max_views(height): the views are then rendered in chunks. Returns the
+        timings of the last chunk."""
+        stride = width * 4 if stride is None else stride
+        view_stride = height * stride if view_stride is None else view_stride
+        n = len(np.asarray(views, dtype=np.float32).reshape(-1, 6))
+        assert buffer.dtype == np.uint8 and buffer.flags["C_CONTIGUOUS"]
+        assert n == 0 or buffer.size >= (n - 1) * view_stride + (height - 1) * stride + 4 * width
+        return self._views(self._api.renderer_render_views, "Renderer::render_views", composition, views, buffer.ctypes.data,
+                           width, height, channels, clear_color, stride, view_stride, timings)
+
+    def render_views_device(self, composition: Composition, views, device_ptr: int, width: int, height: int, channels=RGBA,
+                            clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
+                            view_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """render_views into device memory on the renderer's device: with the defaults, the
+        data_ptr() of a contiguous [N, height, width, 4] uint8 CUDA tensor."""
+        stride = width * 4 if stride is None else stride
+        view_stride = height * stride if view_stride is None else view_stride
+        return self._views(self._api.renderer_render_views_device, "Renderer::render_views_device", composition, views,
+                           int(device_ptr), width, height, channels, clear_color, stride, view_stride, timings)
 
     def launch_count(self) -> int:
         return int(self._api.renderer_launch_count(self._h))

@@ -417,6 +417,23 @@ int forma_renderer_render_device_with_ids(forma_renderer* r, forma_composition* 
                                height, crop, min_coverage, timings);
     });
 }
+uint32_t forma_renderer_max_views(uint64_t height) { return max_views(height); }
+int forma_renderer_render_views_device(forma_renderer* r, forma_composition* c, const float* views, uint32_t n, uint8_t* device_buffer,
+                                       uint64_t width, uint64_t width_stride, uint64_t height, uint64_t view_stride,
+                                       const uint32_t channels[4], const float clear_color[4], forma_timings* timings) {
+    return guarded((int)FORMA_ERR_CAPACITY, [&] {
+        return r->r.render_views(c->c, views, n, device_buffer, true, width, width_stride, height, view_stride, channels, clear_color,
+                                 timings);
+    });
+}
+int forma_renderer_render_views(forma_renderer* r, forma_composition* c, const float* views, uint32_t n, uint8_t* host_buffer,
+                                uint64_t width, uint64_t width_stride, uint64_t height, uint64_t view_stride,
+                                const uint32_t channels[4], const float clear_color[4], forma_timings* timings) {
+    return guarded((int)FORMA_ERR_CAPACITY, [&] {
+        return r->r.render_views(c->c, views, n, host_buffer, false, width, width_stride, height, view_stride, channels, clear_color,
+                                 timings);
+    });
+}
 // --- shared frames (multi-GPU, see include/forma_b200.h) -----------------------
 static_assert(sizeof(cudaIpcMemHandle_t) == sizeof(forma_ipc_handle), "CUDA IPC handles are 64 bytes");
 int forma_shared_frame_create(int device, uint64_t bytes, void** device_ptr, forma_ipc_handle* handle) {

@@ -62,6 +62,24 @@ void launch_line_count(const RasterArgs& args, uint32_t* block_sums, uint32_t* t
                        cudaStream_t stream);
 // Segments at positions >= cap are dropped (speculative launches, see Renderer::rasterize).
 void launch_raster_emit(const RasterArgs& args, const uint32_t* block_offsets, uint64_t* out, uint32_t cap, cudaStream_t stream);
+// Views (see forma_renderer_render_views_device): the same line setup for n_views transforms of
+// the composition, stacked top to bottom in one frame of n_views * rows tile rows. View b's line
+// of layer transform T is transformed by C = V_b ∘ T in f32, `*` rounded on its own:
+//   C.ux = fmaf(V.ux, T.ux, V.vx * T.uy)   C.vx = fmaf(V.ux, T.vx, V.vx * T.vy)
+//   C.uy = fmaf(V.uy, T.ux, V.vy * T.uy)   C.vy = fmaf(V.uy, T.vx, V.vy * T.vy)
+//   C.tx = fmaf(V.ux, T.tx, fmaf(V.vx, T.ty, V.tx))   C.ty = fmaf(V.uy, T.tx, fmaf(V.vy, T.ty, V.ty))
+// (by V alone without T), and rasterized in its own frame's coordinates; only the tile row of
+// the sort key moves: row t of view b becomes biased b * rows + t + 1, rows outside the view 0.
+struct ViewArgs {
+    const float* xf;  // n_views x 6 floats, [ux, vx, uy, vy, tx, ty] (forma_layer_set_transform order)
+    uint32_t rows;    // tile rows per view: ceil(height / 16)
+};
+// As launch_line_count / launch_raster_emit: raster_num_blocks(n_points) * n_views block sums,
+// view-major; max_tile[1] is the stacked bound.
+void launch_line_count_views(const RasterArgs& args, const ViewArgs& views, uint32_t n_views, uint32_t* block_sums, uint32_t* total,
+                             uint32_t* max_tile, cudaStream_t stream);
+void launch_raster_emit_views(const RasterArgs& args, const ViewArgs& views, uint32_t n_views, const uint32_t* block_offsets,
+                              uint64_t* out, uint32_t cap, cudaStream_t stream);
 // Line records of the n = n_points - 1 point pairs (inspection only): orders, then
 // f = {x0, y0, dx, dy, a, b, c, d}, then the per-line segment counts.
 void launch_line_records(const RasterArgs& args, uint32_t n, uint32_t* orders, float* const f[8], uint32_t* lengths,
@@ -217,8 +235,15 @@ void launch_merge_entries(const PaintScene& S, const uint64_t* cell_key, uint32_
                           const uint32_t* gid, uint32_t n_gaps, const uint32_t* cell_start, const uint4* carry_in,
                           const uint4* gap_carry, uint64_t* ekey, EntryRec* recs, uint8_t* eflags, uint2* tile_range,
                           uint32_t* heavy, uint32_t* heavy_count, cudaStream_t st, const DevCounts& dc = DevCounts());
+// view_rows != 0: S stacks views of view_rows tile rows each (ViewArgs); gradients and textures are
+// then sampled in each view's own coordinates.
 void launch_paint(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range, const uint32_t* heavy,
-                  const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st);
+                  const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st,
+                  uint32_t view_rows = 0);
+// Copies rows [0, height) of the n_views views of a stacked frame (view b's first row at
+// src + b * view_rows_px * src_stride) to dst + b * view_stride, row r at + r * stride.
+void launch_repack_views(const uint8_t* src, uint64_t src_stride, uint32_t view_rows_px, uint8_t* dst, uint64_t stride,
+                         uint64_t view_stride, uint32_t width, uint32_t height, uint32_t n_views, cudaStream_t st);
 // ID frame (kernels_ids.cu): per pixel of the tile rectangle of S (clipped to the frame), the
 // order of the top-most Draw layer whose coverage x clip mask exceeds min_coverage, or
 // FORMA_ID_NONE. Reads the tables like launch_paint (never `eflags`); id_flags: one byte per

@@ -208,8 +208,11 @@ __device__ __forceinline__ uint32_t warp_inclusive_scan_sat(uint32_t v) {
     return v;
 }
 
-// segment.rs:298-383 for the point pair (i, i+1).
-__device__ __forceinline__ LineParams line_setup(const RasterArgs& A, uint32_t i) {
+// segment.rs:298-383 for the point pair (i, i+1). kViews: the line as view `V` (6 floats in
+// forma_layer_set_transform order) sees it: the layer's transform T becomes V ∘ T (V alone for a
+// layer without one), composed exactly as ViewArgs documents; a composed identity is no transform.
+template <bool kViews = false>
+__device__ __forceinline__ LineParams line_setup(const RasterArgs& A, uint32_t i, const float* V = nullptr) {
     LineParams L;
     L.length = 0;
     L.order = 0;
@@ -229,6 +232,20 @@ __device__ __forceinline__ LineParams line_setup(const RasterArgs& A, uint32_t i
         lay.has_xf = 0u;
     }
     if (!lay.enabled) return L;
+    if constexpr (kViews) {
+        const float vux = V[0], vvx = V[1], vuy = V[2], vvy = V[3], vtx = V[4], vty = V[5];
+        float ux = vux, vx = vvx, uy = vuy, vy = vvy, tx = vtx, ty = vty;
+        if (lay.has_xf) {
+            ux = fmaf(vux, lay.ux, vvx * lay.uy);
+            vx = fmaf(vux, lay.vx, vvx * lay.vy);
+            uy = fmaf(vuy, lay.ux, vvy * lay.uy);
+            vy = fmaf(vuy, lay.vx, vvy * lay.vy);
+            tx = fmaf(vux, lay.tx, fmaf(vvx, lay.ty, vtx));
+            ty = fmaf(vuy, lay.tx, fmaf(vvy, lay.ty, vty));
+        }
+        lay.has_xf = !(ux == 1.0f && uy == 0.0f && vx == 0.0f && vy == 1.0f && tx == 0.0f && ty == 0.0f) ? 1u : 0u;
+        lay.ux = ux; lay.uy = uy; lay.vx = vx; lay.vy = vy; lay.tx = tx; lay.ty = ty;
+    }
     float p0x = A.x[i], p0y = A.y[i], p1x = A.x[i + 1], p1y = A.y[i + 1];
     if (lay.has_xf) {  // transform_point, segment.rs:30-39
         float ax = fmaf(lay.ux, p0x, fmaf(lay.vx, p0y, lay.tx));
@@ -268,12 +285,14 @@ constexpr int kRasterThreads = 256;
 // Pass 1: per-CTA sum of line lengths.
 // Also tracks the largest (biased) tile coordinates any pixel segment can take,
 // so that the sort only spends passes on key bits that can be set.
-__global__ void __launch_bounds__(kRasterThreads) line_count_kernel(RasterArgs A, uint32_t* __restrict__ block_sums,
-                                                                  uint32_t* __restrict__ max_tile /*[2]: x, y*/) {
+// kViews: CTA (x, y) = the point pairs of CTA x under view y; its sum is block y * gridDim.x + x.
+template <bool kViews>
+__device__ __forceinline__ void line_count_body(const RasterArgs& A, const ViewArgs& V, uint32_t* __restrict__ block_sums,
+                                                uint32_t* __restrict__ max_tile) {
     __shared__ uint32_t warp_sums[kRasterThreads / 32];
     __shared__ uint32_t warp_max[2][kRasterThreads / 32];
     uint32_t i = blockIdx.x * kRasterThreads + threadIdx.x;
-    const LineParams L = line_setup(A, i);
+    const LineParams L = line_setup<kViews>(A, i, kViews ? V.xf + 6u * blockIdx.y : nullptr);
     uint32_t len = L.length;
     {
         uint32_t bx = 0, by = 0;
@@ -284,6 +303,13 @@ __global__ void __launch_bounds__(kRasterThreads) line_count_kernel(RasterArgs A
             int32_t ty = ((int32_t)floorf(fminf(ey, 3.0e7f) + 0.5f) >> 8) + 2;
             bx = (uint32_t)min(max(tx, 0), 4095);
             by = (uint32_t)min(max(ty, 0), 2047);
+            if constexpr (kViews) {
+                // The emit pass maps view y's segments to the stacked rows [y * rows + 1, (y + 1) * rows].
+                by = (blockIdx.y + 1u) * V.rows;
+                // Tile columns left of -32767 wrap (int16, as in the reference) into the frame's
+                // columns: such a line can set any tile_x bit.
+                if (!(fminf(L.x0, L.x0 + L.dx) >= -8388352.0f)) bx = 4095;
+            }
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
@@ -305,11 +331,19 @@ __global__ void __launch_bounds__(kRasterThreads) line_count_kernel(RasterArgs A
             bx = max(bx, warp_max[0][w]);
             by = max(by, warp_max[1][w]);
         }
-        block_sums[blockIdx.x] = s;
+        block_sums[kViews ? blockIdx.y * gridDim.x + blockIdx.x : blockIdx.x] = s;
         // Same-address atomics serialise in L2: only raise the maximum when needed.
         if (bx > *(volatile uint32_t*)&max_tile[0]) atomicMax(&max_tile[0], bx);
         if (by > *(volatile uint32_t*)&max_tile[1]) atomicMax(&max_tile[1], by);
     }
+}
+__global__ void __launch_bounds__(kRasterThreads) line_count_kernel(RasterArgs A, uint32_t* __restrict__ block_sums,
+                                                                  uint32_t* __restrict__ max_tile /*[2]: x, y*/) {
+    line_count_body<false>(A, ViewArgs{}, block_sums, max_tile);
+}
+__global__ void __launch_bounds__(kRasterThreads) line_count_views_kernel(RasterArgs A, ViewArgs V, uint32_t* __restrict__ block_sums,
+                                                                        uint32_t* __restrict__ max_tile) {
+    line_count_body<true>(A, V, block_sums, max_tile);
 }
 
 // Device-wide exclusive scan of `n` u32 values by ONE CTA (n = number of CTAs
@@ -393,14 +427,16 @@ struct SharedLines {
 // segments (a long diagonal) is thus spread over the whole CTA instead of keeping one warp busy
 // for its whole length (measured on paris@4K: the kernel's time was one warp's tail — it did
 // not shrink when seven eighths of the lines were culled).
-__global__ void __launch_bounds__(kRasterThreads)
-    raster_emit_kernel(RasterArgs A, const uint32_t* __restrict__ block_offsets, uint64_t* __restrict__ out, uint32_t cap) {
+// kViews: CTA (x, y) emits view y's segments of the CTA x lines (see line_count_body).
+template <bool kViews>
+__device__ __forceinline__ void raster_emit_body(const RasterArgs& A, const ViewArgs& V, const uint32_t* __restrict__ block_offsets,
+                                                 uint64_t* __restrict__ out, uint32_t cap) {
     __shared__ SharedLines S;
     __shared__ uint32_t warp_sums[kRasterThreads / 32];
     const uint32_t t = threadIdx.x;
     const uint32_t warp = t >> 5, lane = t & 31u;
     uint32_t i = blockIdx.x * kRasterThreads + t;
-    LineParams L = line_setup(A, i);
+    LineParams L = line_setup<kViews>(A, i, kViews ? V.xf + 6u * blockIdx.y : nullptr);
     uint32_t incl = warp_inclusive_scan_sat(L.length);
     if (lane == 31) warp_sums[warp] = incl;
     if (L.length) {
@@ -424,7 +460,7 @@ __global__ void __launch_bounds__(kRasterThreads)
     // then only steer the bisection, which stays inside S.excl).
     S.excl[t] = before + incl - L.length;  // exclusive prefix over the block's 256 lines
     __syncthreads();
-    const uint32_t block_base = block_offsets[blockIdx.x];
+    const uint32_t block_base = block_offsets[kViews ? blockIdx.y * gridDim.x + blockIdx.x : blockIdx.x];
     // `cap` bounds a speculative launch made before the segment count is known on the host: the
     // loop never runs past it, whatever the (saturated) counts of an over-limit frame. The last
     // clamp keeps `s += kRasterThreads` from wrapping.
@@ -464,11 +500,23 @@ __global__ void __launch_bounds__(kRasterThreads)
         int32_t cover = (int32_t)(int8_t)(y1s - y0s);
         // PixelSegment::new, pixel_segment.rs:36-71
         uint64_t ty = (uint64_t)max((int32_t)(int16_t)(tile_y + 1), 0) & 0x7FFull;
+        // A view's painted rows (biased 1 ... rows) move to its place in the stacked frame; every
+        // other row becomes tile row -1 (biased 0), which no painted tile reads, so that nothing
+        // bleeds into the neighbouring views. The single frame's own wrap of the field is kept.
+        if constexpr (kViews) ty = ty - 1u < V.rows ? ty + (uint64_t)blockIdx.y * V.rows : 0u;
         uint64_t tx = (uint64_t)max((int32_t)(int16_t)(tile_x + 1), 0) & 0xFFFull;
         uint64_t v = (ty << 53) | (tx << 41) | ((uint64_t)(S.order[li] & 0x1FFFFFu) << 20) | ((uint64_t)local_x << 16) |
                      ((uint64_t)local_y << 12) | ((uint64_t)(dam & 0x3Fu) << 6) | ((uint64_t)((uint32_t)cover & 0x3Fu));
         out[(uint64_t)block_base + s] = v;
     }
+}
+__global__ void __launch_bounds__(kRasterThreads)
+    raster_emit_kernel(RasterArgs A, const uint32_t* __restrict__ block_offsets, uint64_t* __restrict__ out, uint32_t cap) {
+    raster_emit_body<false>(A, ViewArgs{}, block_offsets, out, cap);
+}
+__global__ void __launch_bounds__(kRasterThreads) raster_emit_views_kernel(RasterArgs A, ViewArgs V, const uint32_t* __restrict__ block_offsets,
+                                                                         uint64_t* __restrict__ out, uint32_t cap) {
+    raster_emit_body<true>(A, V, block_offsets, out, cap);
 }
 
 // Inspection only (forma_renderer_lines): the line records of segment.rs:298-383 as the
@@ -522,6 +570,25 @@ void launch_raster_emit(const RasterArgs& args, const uint32_t* block_offsets, u
     uint32_t nb = raster_num_blocks(args.n_points);
     if (!nb) return;
     raster_emit_kernel<<<nb, kRasterThreads, 0, stream>>>(args, block_offsets, out, cap);
+}
+
+void launch_line_count_views(const RasterArgs& args, const ViewArgs& views, uint32_t n_views, uint32_t* block_sums, uint32_t* total,
+                             uint32_t* max_tile, cudaStream_t stream) {
+    uint32_t nb = raster_num_blocks(args.n_points);
+    cudaMemsetAsync(max_tile, 0, 2 * sizeof(uint32_t), stream);
+    if (!nb || !n_views) {
+        cudaMemsetAsync(total, 0, sizeof(uint32_t), stream);
+        return;
+    }
+    line_count_views_kernel<<<dim3(nb, n_views), kRasterThreads, 0, stream>>>(args, views, block_sums, max_tile);
+    scan_block_sums_kernel<<<1, 1024, 0, stream>>>(block_sums, nb * n_views, total);
+}
+
+void launch_raster_emit_views(const RasterArgs& args, const ViewArgs& views, uint32_t n_views, const uint32_t* block_offsets,
+                              uint64_t* out, uint32_t cap, cudaStream_t stream) {
+    uint32_t nb = raster_num_blocks(args.n_points);
+    if (!nb || !n_views) return;
+    raster_emit_views_kernel<<<dim3(nb, n_views), kRasterThreads, 0, stream>>>(args, views, block_offsets, out, cap);
 }
 
 }  // namespace forma

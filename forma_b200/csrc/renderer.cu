@@ -245,9 +245,9 @@ int Renderer::upload_tables_device(Composition& comp, CompDevice& cd) {
 
 // Stages 1½ + 2: fills `segs` with the unsorted pixel segments.
 int Renderer::rasterize(Composition& comp, uint32_t width, uint32_t height, float band_lo, float band_hi,
-                        uint32_t* n_out) {
-    RasterArgs& ra = last_raster;  // kept for forma_renderer_lines
-    last_raster_valid = true;
+                        uint32_t* n_out, const ViewArgs* views, uint32_t n_views) {
+    RasterArgs& ra = last_raster;  // kept for forma_renderer_lines (a stacked frame of views has no line records)
+    last_raster_valid = !views;
     CompDevice& cd = comp.on(res_key);
     ra.x = cd.d_x.ptr;
     ra.y = cd.d_y.ptr;
@@ -262,9 +262,21 @@ int Renderer::rasterize(Composition& comp, uint32_t width, uint32_t height, floa
     ra.band_lo = band_lo;
     ra.band_hi = band_hi;
     uint32_t nb = raster_num_blocks(ra.n_points);
+    if (views) {
+        if ((uint64_t)nb * n_views >= (1ull << 32)) {
+            set_error("%u views of %u points exceed the line-setup grid", n_views, ra.n_points);
+            return FORMA_STATUS_CAPACITY;
+        }
+        nb *= n_views;  // one CTA sum per (view, CTA of points)
+    }
     FORMA_CUDA_TRY(block_sums.reserve(nb + 1));
-    launch_line_count(ra, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
+    if (views) launch_line_count_views(ra, *views, n_views, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
+    else launch_line_count(ra, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
     launches += nb ? 2 : 0;
+    auto emit = [&](uint32_t cap) {
+        if (views) launch_raster_emit_views(ra, *views, n_views, block_sums.ptr, segs.ptr, cap, stream);
+        else launch_raster_emit(ra, block_sums.ptr, segs.ptr, cap, stream);
+    };
     uint32_t n = 0;
     // One read-back: segment count + the largest tile coordinates (totals[4..5]).
     FORMA_CUDA_TRY(cudaMemcpyAsync(pinned_totals, totals.ptr, 6 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
@@ -278,7 +290,7 @@ int Renderer::rasterize(Composition& comp, uint32_t width, uint32_t height, floa
     FORMA_CUDA_TRY(cudaEventRecord(count_ev, stream));
     if (speculated) {
         if (timer.ok) FORMA_CUDA_TRY(cudaEventRecord(timer.ev[1], stream));  // end of line setup (count pass)
-        launch_raster_emit(ra, block_sums.ptr, segs.ptr, (uint32_t)(spec_cap - 1), stream);
+        emit((uint32_t)(spec_cap - 1));
         ++launches;
     }
     FORMA_CUDA_TRY(cudaEventSynchronize(count_ev));  // the read-back only, not the speculative launch
@@ -310,7 +322,7 @@ int Renderer::rasterize(Composition& comp, uint32_t width, uint32_t height, floa
     FORMA_CUDA_TRY(reserve_all(n + 1, segs, segs_tmp));
     if (!speculated || (size_t)n + 1 > spec_cap) {
         if (!speculated && timer.ok) FORMA_CUDA_TRY(cudaEventRecord(timer.ev[1], stream));  // end of line setup (count pass)
-        launch_raster_emit(ra, block_sums.ptr, segs.ptr, n, stream);
+        emit(n);
         launches += nb ? 1 : 0;
     }
     FORMA_CUDA_TRY(cudaGetLastError());
@@ -555,6 +567,144 @@ int Renderer::render_ids(Composition& comp, uint8_t* rgba, uint64_t rgba_stride,
         timings->paint_ms = stage_ms[4] + stage_ms[5];
         timings->n_lines = cd.n_resident ? cd.n_resident - 1 : 0;
         timings->n_segments = n;
+    }
+    return FORMA_STATUS_OK;
+}
+
+// n views of one composition in one pass: the stages of render() once, over a frame that stacks
+// the views top to bottom, n * rows tile rows of `width` pixels (rows = ceil(height / 16)). Line
+// setup rasterizes every view in its own coordinates and moves its segments' tile rows to the
+// view's place in the stack (ViewArgs); the tables, the sort and the painter see one frame. No
+// layer cache and no band filter: the whole composition is resident.
+int Renderer::render_views(Composition& comp, const float* views, uint32_t n, uint8_t* buffer, bool buffer_on_device, uint64_t width,
+                           uint64_t stride, uint64_t height, uint64_t view_stride, const uint32_t channels[4], const float clear[4],
+                           forma_timings* timings) {
+    if (!buffer || !views || width == 0 || height == 0 || width * 4 > stride || width > FORMA_MAX_WIDTH || height > FORMA_MAX_HEIGHT) {
+        set_error("invalid render target %llux%llu stride %llu", (unsigned long long)width, (unsigned long long)height,
+                  (unsigned long long)stride);
+        return FORMA_STATUS_INVALID;
+    }
+    const uint32_t rows = (uint32_t)((height + 15u) / 16u);
+    if (n == 0 || n > max_views(height)) {
+        set_error("%u views of height %llu: between 1 and %u views of this height fit in one call", n, (unsigned long long)height,
+                  max_views(height));
+        return FORMA_STATUS_INVALID;
+    }
+    if (view_stride < (height - 1u) * stride + 4u * width) {
+        set_error("view stride %llu is smaller than one view (%llu bytes)", (unsigned long long)view_stride,
+                  (unsigned long long)((height - 1u) * stride + 4u * width));
+        return FORMA_STATUS_INVALID;
+    }
+    for (uint32_t b = 0; b < n; ++b) {  // [ux, vx, uy, vy, tx, ty], as forma_layer_set_transform checks them
+        const float* v = views + 6u * b;
+        bool finite = true;
+        for (int k = 0; k < 6; ++k) finite = finite && std::isfinite(v[k]);
+        if (!finite || !geom_pres_ok(v[0], v[2], v[1], v[3])) {
+            set_error("view %u is not a finite transform that does not scale up", b);
+            return FORMA_STATUS_INVALID;
+        }
+    }
+    // Views whose rows are whole tile rows, laid out as the stacked frame's rows, are painted in place.
+    const bool direct = buffer_on_device && height % 16u == 0u && view_stride == height * stride;
+    const uint64_t fb_stride = direct ? stride : 4u * width;
+    PaintScene S{};
+    int st = begin_frame(S, buffer, width, fb_stride, (uint64_t)n * rows * 16u, channels, clear, nullptr);
+    if (st) return st;
+    uint8_t* fb = buffer;
+    if (!direct) {
+        FORMA_CUDA_TRY(framebuffer.reserve((size_t)fb_stride * S.height));
+        fb = framebuffer.ptr;
+    }
+
+    if (!prefetched) FORMA_CUDA_TRY(cudaEventRecord(timer.ev[0], stream));
+    prefetched = false;
+    st = upload_tables(comp, -1);
+    if (st) return st;
+    st = flush_geometry(comp);
+    if (st) return st;
+    st = bind_frame(comp, S, nullptr, clear, false);
+    if (st) return st;
+    FORMA_CUDA_TRY(h_views.reserve(6u * n));
+    FORMA_CUDA_TRY(d_views.reserve(6u * n));
+    std::memcpy(h_views.ptr, views, 6u * n * sizeof(float));  // (the previous call's copy is complete: rasterize waited for it)
+    FORMA_CUDA_TRY(cudaMemcpyAsync(d_views.ptr, h_views.ptr, 6u * n * sizeof(float), cudaMemcpyHostToDevice, stream));
+    h2d_bytes += 6u * n * sizeof(float);
+    const ViewArgs va{d_views.ptr, rows};
+
+    FORMA_CUDA_TRY(cudaEventRecord(timer.ev[7], stream));
+    uint32_t n_segs = 0;
+    st = rasterize(comp, S.width, (uint32_t)height, 0.0f, (float)height, &n_segs, &va, n);
+    if (st) return st;
+    FORMA_CUDA_TRY(cudaEventRecord(timer.ev[2], stream));
+    int timed_sort_passes = 0;
+    if (n_segs > 1) {
+        FORMA_CUDA_TRY(sort_scratch.reserve(radix_scratch_bytes(n_segs)));
+        timed_sort_passes = sort(segs, segs_tmp, nullptr, nullptr, n_segs, segment_plan, timer.sort_ev).timed_passes;
+        FORMA_CUDA_TRY(cudaGetLastError());
+    }
+    FORMA_CUDA_TRY(cudaEventRecord(timer.ev[3], stream));
+
+    const size_t n_tiles_total = (size_t)S.tiles_x * S.tiles_y;
+    last_tiles_x = S.tiles_x;
+    last_tiles_y = S.tiles_y;
+    FORMA_CUDA_TRY(tile_range.reserve(n_tiles_total));
+    FORMA_CUDA_TRY(heavy_tiles.reserve(n_tiles_total * kHeavyListClasses));
+    uint32_t* const heavy_lists = options().paint_lpt ? heavy_tiles.ptr : nullptr;
+    // Tables + paint + copy-out, once or (when the sync-free bounds were too small) twice, as in render().
+    const uint32_t prev_cells = last_cells, prev_gaps = last_gaps;
+    const bool fast = options().sync_free && n_segs > 0 && prev_cells > 0;
+    last_cells = last_entries = 0;
+    last_written_tiles = 0;
+    last_tables_redone = false;
+    uint32_t paint_launches = 1;
+    for (bool sync_free = fast;; sync_free = false) {
+        DevCounts dc;
+        st = build_tables(S, n_segs, sync_free, prev_cells, prev_gaps, heavy_lists, dc);
+        if (st) return st;
+        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[4], stream));
+        st = paint(S, fb, fb, fb_stride, false, heavy_lists, &paint_launches, rows);
+        if (st) return st;
+        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[5], stream));
+        if (buffer_on_device && !direct) {
+            launch_repack_views(fb, fb_stride, rows * 16u, buffer, stride, view_stride, S.width, (uint32_t)height, n, stream);
+            ++launches;
+            FORMA_CUDA_TRY(cudaGetLastError());
+        } else if (!buffer_on_device) {
+            // Rows [0, height) of every view, one copy per view with the pitches copy_to_host uses
+            // for a single frame (a copy over all views would have a view as its pitch, which can
+            // exceed the device's largest pitch).
+            for (uint32_t b = 0; b < n; ++b) {
+                uint8_t* dst = buffer + (size_t)b * view_stride;
+                const uint8_t* src = fb + (size_t)b * rows * 16u * fb_stride;
+                if (stride == fb_stride)
+                    FORMA_CUDA_TRY(cudaMemcpyAsync(dst, src, (height - 1u) * stride + 4u * width, cudaMemcpyDeviceToHost, stream));
+                else
+                    FORMA_CUDA_TRY(cudaMemcpy2DAsync(dst, stride, src, fb_stride, 4u * width, height, cudaMemcpyDeviceToHost, stream));
+            }
+            d2h_bytes += (uint64_t)n * height * width * 4u;
+        }
+        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[6], stream));
+        FORMA_CUDA_TRY(cudaStreamSynchronize(stream));
+        if (!sync_free) break;
+        last_cells = pinned_totals[1];
+        last_gaps = pinned_totals[2];
+        last_entries = last_cells + last_gaps;
+        if (last_cells <= dc.cell_bound && last_gaps <= dc.gap_bound) break;
+        last_tables_redone = true;
+    }
+    last_tables_sync_free = fast && !last_tables_redone;
+    times_pending = true;
+    pending_sort_passes = timed_sort_passes;
+    pending_paint_launches = paint_launches;
+    if (timings) {
+        resolve_times();
+        const CompDevice& cd = comp.on(res_key);
+        timings->line_setup_ms = stage_ms[1];
+        timings->rasterize_ms = stage_ms[2];
+        timings->sort_ms = stage_ms[3];
+        timings->paint_ms = stage_ms[4] + stage_ms[5];
+        timings->n_lines = cd.n_resident ? cd.n_resident - 1 : 0;
+        timings->n_segments = n_segs;
     }
     return FORMA_STATUS_OK;
 }
@@ -807,7 +957,7 @@ int Renderer::queue_row_costs(const PaintScene& S, uint32_t n) {
 // of band k run dry: the kernels overlap at their tails, and the PCIe transfer of a band overlaps
 // the painting of the following ones.
 int Renderer::paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t stride, bool in_bands, const uint32_t* heavy_lists,
-                    uint32_t* paint_launches) {
+                    uint32_t* paint_launches, uint32_t view_rows) {
     *paint_launches = 1;
     if (in_bands) {
         if (!band_streams_ok) {
@@ -837,7 +987,7 @@ int Renderer::paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t 
         for (uint32_t k = 0; kCopyBands > 1u && k < kCopyBands; ++k) FORMA_CUDA_TRY(cudaStreamWaitEvent(stream, band_ev[k], 0));
         *paint_launches = kCopyBands;
     } else {
-        launch_paint(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), eflags.ptr, fb, totals.ptr + 3, stream);
+        launch_paint(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), eflags.ptr, fb, totals.ptr + 3, stream, view_rows);
         ++launches;
     }
     FORMA_CUDA_TRY(cudaGetLastError());

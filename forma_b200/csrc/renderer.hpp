@@ -209,7 +209,9 @@ class Renderer {
     int flush_geometry(Composition& comp, float band_lo = 0.0f, float band_hi = 0.0f, bool band_is_partial = false);
     int upload_tables(Composition& comp, int64_t cache_id);
     int upload_tables_device(Composition& comp, CompDevice& cd);
-    int rasterize(Composition& comp, uint32_t width, uint32_t height, float band_lo, float band_hi, uint32_t* n_out);
+    // views / n_views: the line setup of render_views (a stacked frame of n_views views).
+    int rasterize(Composition& comp, uint32_t width, uint32_t height, float band_lo, float band_hi, uint32_t* n_out,
+                  const ViewArgs* views = nullptr, uint32_t n_views = 0);
     int render(Composition& comp, uint8_t* buffer, bool buffer_on_device, uint64_t width, uint64_t stride,
                uint64_t height, const uint32_t channels[4], const float clear[4], const forma_rect* crop,
                LayerCache* cache, forma_timings* timings);
@@ -220,6 +222,14 @@ class Renderer {
     int render_ids(Composition& comp, uint8_t* rgba, uint64_t rgba_stride, const uint32_t channels[4], const float clear[4],
                    uint32_t* ids, bool ids_on_device, uint64_t width, uint64_t ids_stride, uint64_t height,
                    const forma_rect* crop, float min_coverage, forma_timings* timings);
+    // n views of one composition in one pass (see forma_renderer_render_views_device): a frame of
+    // n * ceil(height / 16) tile rows, painted straight into a device buffer whose views are its
+    // rows, or into `framebuffer` and copied out view by view.
+    PinnedBuffer<float> h_views;
+    DeviceBuffer<float> d_views;
+    int render_views(Composition& comp, const float* views, uint32_t n, uint8_t* buffer, bool buffer_on_device, uint64_t width,
+                     uint64_t stride, uint64_t height, uint64_t view_stride, const uint32_t channels[4], const float clear[4],
+                     forma_timings* timings);
     // The stages of render(), in the order it runs them.
     int begin_frame(PaintScene& S, const uint8_t* buffer, uint64_t width, uint64_t stride, uint64_t height,
                     const uint32_t channels[4], const float clear[4], const forma_rect* crop);
@@ -228,7 +238,7 @@ class Renderer {
                      DevCounts& dc);
     int queue_row_costs(const PaintScene& S, uint32_t n);
     int paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t stride, bool in_bands, const uint32_t* heavy_lists,
-              uint32_t* paint_launches);
+              uint32_t* paint_launches, uint32_t view_rows = 0);
     int copy_to_host(const PaintScene& S, uint8_t* buffer, const uint8_t* fb, uint64_t stride, cudaStream_t s);
     int scatter_written_tiles(const PaintScene& S, const uint8_t* fb, uint8_t* buffer, uint64_t stride);
 };
@@ -238,6 +248,14 @@ class Renderer {
 struct TileRect {
     uint32_t tx_lo, tx_hi, ty_lo, ty_hi;
 };
+// The most views of `height` rows one render_views call takes: the stacked frame's tile rows
+// are the biased rows 1 ... n * rows of the 11-bit tile_y field, and the painter tables' sentinel
+// row (tiles_y + 1, see sentinel_key) must fit in it too: n * rows <= 2046.
+inline uint32_t max_views(uint64_t height) {
+    if (height == 0 || height > FORMA_MAX_HEIGHT) return 0;
+    return (uint32_t)(2046u / ((height + 15u) / 16u));
+}
+
 inline TileRect tile_rect(uint64_t width, uint64_t height, const forma_rect* crop) {
     const uint32_t tiles_x = (uint32_t)((width + 15u) / 16u), tiles_y = (uint32_t)((height + 15u) / 16u);
     TileRect t{0, tiles_x, 0, tiles_y};

@@ -246,6 +246,41 @@ int forma_renderer_render_device_with_ids(forma_renderer*, forma_composition*, u
                                           const forma_rect* crop /* nullable */, uint32_t* device_ids,
                                           uint64_t ids_stride, float min_coverage, forma_timings* timings /* nullable */);
 
+/* Views (no reference counterpart): `n` frames of one composition, each seen through its own
+ * transform, from one pass through the stages. `views` holds n x 6 floats, each view in
+ * forma_layer_set_transform order [ux, vx, uy, vy, tx, ty]. All frames share width x height,
+ * width_stride, channels and clear colour; frame b starts at b * view_stride bytes, and
+ * view_stride >= (height - 1) * width_stride + 4 * width, so frames never overlap. Only the
+ * frames' width x height pixels are written: row padding and the bytes between frames stay.
+ * Frame b is the bytes forma_renderer_render_device makes with every layer's transform
+ * replaced by C = V_b ∘ T (V_b for a layer without a transform T), composed in f32 as
+ *   C.ux = fmaf(V.ux, T.ux, V.vx * T.uy)   C.vx = fmaf(V.ux, T.vx, V.vx * T.vy)
+ *   C.uy = fmaf(V.uy, T.ux, V.vy * T.uy)   C.vy = fmaf(V.uy, T.vx, V.vy * T.vy)
+ *   C.tx = fmaf(V.ux, T.tx, fmaf(V.vx, T.ty, V.tx))   C.ty = fmaf(V.uy, T.tx, fmaf(V.vy, T.ty, V.ty))
+ * with every product rounded on its own; a C equal to the identity is no transform. (Frames whose
+ * lines all lie more than 2^19 px left of the frame are the exception: forma_renderer_render_device
+ * mis-sorts their wrapped tile columns, the views do not.) Path
+ * transforms apply first; gradients and textures stay in frame coordinates.
+ * Every V_b must be finite and pass forma_layer_set_transform's check (no scaling up); the
+ * composed C is not checked again, so two transforms that each pass may render with a C one
+ * rounding past the limit. 1 <= n <= forma_renderer_max_views(height). A call that breaks one
+ * of these rules returns FORMA_ERR_INVALID_ARGUMENT and writes nothing. FORMA_ERR_CAPACITY
+ * applies to the pixel segments of all views together.
+ * No layer cache is taken and every cache is left as it was. Afterwards counters, segments,
+ * stage times and row costs describe the call's stacked frame (n * ceil(height / 16) tile
+ * rows, view b's rows after view b - 1's), and forma_renderer_lines returns no records.
+ * render_views_device writes a device buffer on the renderer's device (a [n, H, W, 4] uint8
+ * tensor's data_ptr() with width_stride = 4 W, view_stride = 4 W H); render_views a host buffer. */
+uint32_t forma_renderer_max_views(uint64_t height); /* floor(2046 / ceil(height / 16)); 0 when height is 0 or too tall */
+int forma_renderer_render_views_device(forma_renderer*, forma_composition*, const float* views, uint32_t n,
+                                       uint8_t* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                       uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
+                                       forma_timings* timings /* nullable */);
+int forma_renderer_render_views(forma_renderer*, forma_composition*, const float* views, uint32_t n,
+                                uint8_t* host_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
+                                forma_timings* timings /* nullable */);
+
 /* Launch on `cuda_stream` (a cudaStream_t, e.g. torch.cuda.current_stream().cuda_stream)
  * instead of the default stream. */
 void forma_renderer_set_stream(forma_renderer*, void* cuda_stream);
