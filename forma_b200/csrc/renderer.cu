@@ -1,6 +1,6 @@
-// forma_b200 — Renderer: the uploads and Renderer::render.
+// forma_b200 — Renderer: the uploads and the frames.
 //
-// Renderer::render follows forma/src/cpu/renderer.rs:75-224 stage by stage;
+// A frame (Renderer::run_frame, and render's layer-cache steps) follows forma/src/cpu/renderer.rs:75-224 stage by stage;
 // every stage is a CUDA kernel sequence on one stream, and there is no CPU
 // fallback: without a usable sm_90 device forma_renderer_new() fails.
 #include <algorithm>
@@ -329,47 +329,66 @@ int Renderer::rasterize(Composition& comp, uint32_t width, uint32_t height, floa
     return FORMA_STATUS_OK;
 }
 
-// The upload half of render() on its own: tables + the geometry that the rows of `crop` need and
-// that is not resident yet. render() then finds everything in place.
+// The pixel rows [lo, hi) a frame paints; partial: not all of its rows (flush_geometry's band filter).
+struct FrameBand {
+    float lo, hi;
+    bool partial;
+};
+// The band of the tile rows [ty_lo, ty_hi) of a frame `height` rows high.
+static FrameBand tile_band(uint32_t ty_lo, uint32_t ty_hi, uint64_t height) {
+    return {(float)(ty_lo * 16u), (float)std::min<uint64_t>((uint64_t)ty_hi * 16u, height),
+            ty_lo > 0u || ty_hi < (height + 15u) / 16u};
+}
+
+// The upload half of run_frame() on its own: tables + the geometry that the rows of `crop` need and
+// that is not resident yet. The next frame then finds everything in place.
 int Renderer::prefetch(Composition& comp, uint64_t width, uint64_t height, const forma_rect* crop) {
     FORMA_CUDA_TRY(cudaSetDevice(device));
     const int ts = ensure_timer();
     if (ts) return ts;
-    const uint32_t tiles_y = (uint32_t)((height + 15u) / 16u);
     const TileRect t = tile_rect(width, height, crop);
     FORMA_CUDA_TRY(cudaEventRecord(timer.ev[0], stream));
     prefetched = true;
     if (upload_after) FORMA_CUDA_TRY(cudaStreamWaitEvent(stream, upload_after, 0));
-    const float band_lo = (float)(t.ty_lo * 16u), band_hi = (float)std::min<uint64_t>((uint64_t)t.ty_hi * 16u, height);
+    const FrameBand band = tile_band(t.ty_lo, t.ty_hi, height);
     int st = upload_tables(comp, -1);
     if (st) return st;
-    return flush_geometry(comp, band_lo, band_hi, t.ty_lo > 0u || t.ty_hi < tiles_y);
+    return flush_geometry(comp, band.lo, band.hi, band.partial);
 }
 
-int Renderer::render(Composition& comp, uint8_t* buffer, bool buffer_on_device, uint64_t width, uint64_t stride,
-                     uint64_t height, const uint32_t channels_in[4], const float clear[4], const forma_rect* crop,
-                     LayerCache* cache, forma_timings* timings) {
-    PaintScene S{};
-    int st = begin_frame(S, buffer, width, stride, height, channels_in, clear, crop);
-    if (st) return st;
-
+// One frame of S, whatever its kind: uploads, line setup, sort, then the painter tables,
+// paint_step(heavy_lists, &paint_launches) (the frame's kernels) and output_step() (the copy to
+// where the caller wants the frame) once or, when the sync-free bounds were too small, twice.
+template <class Paint, class Output>
+int Renderer::run_frame(Composition& comp, PaintScene& S, const FrameSpec& spec, forma_timings* timings, Paint&& paint_step,
+                        Output&& output_step) {
     if (!prefetched) FORMA_CUDA_TRY(cudaEventRecord(timer.ev[0], stream));
     prefetched = false;
     // Lines entirely above / below the painted tile rows cannot reach a painted tile: they are
     // culled per line (rasterize), and whole inserts are left out of the device's segment
-    // buffer when the band is narrower than the frame (flush_geometry).
-    const float band_lo = (float)(S.ty_lo * 16u), band_hi = (float)std::min<uint64_t>((uint64_t)S.ty_hi * 16u, height);
-    st = upload_tables(comp, -1);
+    // buffer when the band is narrower than the frame (flush_geometry). Line setup sees every view
+    // as a frame of its own: all its rows are painted.
+    const uint32_t height = spec.views ? spec.view_height : S.height;
+    const FrameBand band = spec.views ? FrameBand{0.0f, (float)height, false} : tile_band(S.ty_lo, S.ty_hi, height);
+    int st = upload_tables(comp, -1);
     if (st) return st;
-    st = flush_geometry(comp, band_lo, band_hi, S.ty_lo > 0u || S.ty_hi < S.tiles_y);
+    st = flush_geometry(comp, band.lo, band.hi, band.partial);
     if (st) return st;
-    const bool pack_written = cache && !buffer_on_device;
-    st = bind_frame(comp, S, cache, clear, pack_written);
+    st = bind_frame(comp, S, spec.cache, S.clear, spec.pack_written);
     if (st) return st;
+    if (spec.views) {
+        const uint32_t nv = spec.n_views;
+        FORMA_CUDA_TRY(h_views.reserve(6u * nv));
+        FORMA_CUDA_TRY(d_views.reserve(6u * nv));
+        std::memcpy(h_views.ptr, spec.views, 6u * nv * sizeof(float));  // (the previous call's copy is complete: rasterize waited for it)
+        FORMA_CUDA_TRY(cudaMemcpyAsync(d_views.ptr, h_views.ptr, 6u * nv * sizeof(float), cudaMemcpyHostToDevice, stream));
+        h2d_bytes += 6u * nv * sizeof(float);
+    }
+    const ViewArgs va{d_views.ptr, (height + 15u) / 16u};
 
     FORMA_CUDA_TRY(cudaEventRecord(timer.ev[7], stream));
     uint32_t n = 0;
-    st = rasterize(comp, S.width, S.height, band_lo, band_hi, &n);
+    st = rasterize(comp, S.width, height, band.lo, band.hi, &n, spec.views ? &va : nullptr, spec.n_views);
     if (st) return st;
 
     // Stage 3: sort.
@@ -383,22 +402,14 @@ int Renderer::render(Composition& comp, uint8_t* buffer, bool buffer_on_device, 
     FORMA_CUDA_TRY(cudaEventRecord(timer.ev[3], stream));
 
     // Stage 4: cells -> carries -> entries -> paint.
-    size_t n_tiles_total = (size_t)S.tiles_x * S.tiles_y;
+    const size_t n_tiles_total = (size_t)S.tiles_x * S.tiles_y;
     last_tiles_x = S.tiles_x;
     last_tiles_y = S.tiles_y;
     FORMA_CUDA_TRY(tile_range.reserve(n_tiles_total));
     FORMA_CUDA_TRY(heavy_tiles.reserve(n_tiles_total * kHeavyListClasses));
     // Heavy tiles first (longest-processing-time order): their lists + counts (heavy_count()).
     uint32_t* const heavy_lists = options().paint_lpt ? heavy_tiles.ptr : nullptr;
-    uint8_t* fb = buffer;
-    if (!buffer_on_device) {
-        FORMA_CUDA_TRY(framebuffer.reserve((size_t)stride * height));
-        fb = framebuffer.ptr;
-    }
-    const uint32_t paint_rows = S.ty_hi - S.ty_lo;
-    const bool in_bands = !buffer_on_device && !cache && paint_rows >= (copy_bands_override ? 8u : 32u) && S.tx_hi > S.tx_lo &&
-                          band_copies_enabled();
-    // Tables + paint + copy-back, once or (rarely) twice. sync_free = without count read-backs: the
+    // Tables + paint + output, once or (rarely) twice. sync_free = without count read-backs: the
     // tables of a frame are normally about as large as those of the frame before, so every
     // kernel is launched over bounds derived from the previous counts and reads the real counts
     // from device memory (DevCounts); the host looks at them only after the frame's final
@@ -406,7 +417,7 @@ int Renderer::render(Composition& comp, uint8_t* buffer, bool buffer_on_device, 
     // the clear colour) sends the frame through again with counted tables.
     // (pack_written: the host scatter of the written tiles must not see a frame that is redone.)
     const uint32_t prev_cells = last_cells, prev_gaps = last_gaps;  // of this renderer's previous frame
-    const bool fast = options().sync_free && n > 0 && prev_cells > 0 && !pack_written;
+    const bool fast = options().sync_free && n > 0 && prev_cells > 0 && !spec.pack_written;
     last_cells = last_entries = 0;
     last_written_tiles = 0;
     last_tables_redone = false;
@@ -418,13 +429,10 @@ int Renderer::render(Composition& comp, uint8_t* buffer, bool buffer_on_device, 
         st = queue_row_costs(S, n);
         if (st) return st;
         FORMA_CUDA_TRY(cudaEventRecord(timer.ev[4], stream));
-        st = paint(S, fb, buffer, stride, in_bands, heavy_lists, &paint_launches);
+        st = paint_step(heavy_lists, &paint_launches);
         if (st) return st;
         FORMA_CUDA_TRY(cudaEventRecord(timer.ev[5], stream));
-        if (pack_written)
-            st = scatter_written_tiles(S, fb, buffer, stride);
-        else if (!buffer_on_device && !in_bands)
-            st = copy_to_host(S, buffer, fb, stride, stream);
+        st = output_step();
         if (st) return st;
         FORMA_CUDA_TRY(cudaEventRecord(timer.ev[6], stream));
         FORMA_CUDA_TRY(cudaStreamSynchronize(stream));
@@ -451,6 +459,35 @@ int Renderer::render(Composition& comp, uint8_t* buffer, bool buffer_on_device, 
         timings->n_lines = cd.n_resident ? cd.n_resident - 1 : 0;
         timings->n_segments = n;
     }
+    return FORMA_STATUS_OK;
+}
+
+int Renderer::render(Composition& comp, uint8_t* buffer, bool buffer_on_device, uint64_t width, uint64_t stride,
+                     uint64_t height, const uint32_t channels_in[4], const float clear[4], const forma_rect* crop,
+                     LayerCache* cache, forma_timings* timings) {
+    PaintScene S{};
+    int st = begin_frame(S, buffer, width, stride, height, channels_in, clear, crop);
+    if (st) return st;
+    uint8_t* fb = buffer;
+    if (!buffer_on_device) {
+        FORMA_CUDA_TRY(framebuffer.reserve((size_t)stride * height));
+        fb = framebuffer.ptr;
+    }
+    const uint32_t paint_rows = S.ty_hi - S.ty_lo;
+    const bool in_bands = !buffer_on_device && !cache && paint_rows >= (copy_bands_override ? 8u : 32u) && S.tx_hi > S.tx_lo &&
+                          band_copies_enabled();
+    const bool pack_written = cache && !buffer_on_device;
+    st = run_frame(
+        comp, S, FrameSpec{cache, pack_written}, timings,
+        [&](const uint32_t* heavy_lists, uint32_t* paint_launches) {
+            return paint(S, fb, buffer, stride, in_bands, heavy_lists, paint_launches);
+        },
+        [&] {
+            if (pack_written) return scatter_written_tiles(S, fb, buffer, stride);
+            if (!buffer_on_device && !in_bands) return copy_to_host(S, buffer, fb, stride, stream);
+            return FORMA_STATUS_OK;
+        });
+    if (st) return st;
     if (cache) {  // renderer.rs:217-223
         cache->has_clear = true;
         std::memcpy(cache->clear_color, clear, sizeof(cache->clear_color));
@@ -463,8 +500,8 @@ int Renderer::render(Composition& comp, uint8_t* buffer, bool buffer_on_device, 
 }
 
 // An ID frame, alone (rgba == nullptr) or after the RGBA frame of the same tables in device
-// memory (render_device's frame without a cache). The stages of render() run once; the
-// sync-free redo repeats the kernels. The ID frame never touches a layer cache.
+// memory (render_device's frame without a cache). The sync-free redo repeats the kernels. The ID
+// frame never touches a layer cache.
 int Renderer::render_ids(Composition& comp, uint8_t* rgba, uint64_t rgba_stride, const uint32_t channels[4], const float clear[4],
                          uint32_t* ids, bool ids_on_device, uint64_t width, uint64_t ids_stride, uint64_t height,
                          const forma_rect* crop, float min_coverage, forma_timings* timings) {
@@ -483,99 +520,37 @@ int Renderer::render_ids(Composition& comp, uint8_t* rgba, uint64_t rgba_stride,
         set_error("invalid ID frame stride %llu for width %llu", (unsigned long long)ids_stride, (unsigned long long)width);
         return FORMA_STATUS_INVALID;
     }
-
-    if (!prefetched) FORMA_CUDA_TRY(cudaEventRecord(timer.ev[0], stream));
-    prefetched = false;
-    const float band_lo = (float)(S.ty_lo * 16u), band_hi = (float)std::min<uint64_t>((uint64_t)S.ty_hi * 16u, height);
-    st = upload_tables(comp, -1);
-    if (st) return st;
-    st = flush_geometry(comp, band_lo, band_hi, S.ty_lo > 0u || S.ty_hi < S.tiles_y);
-    if (st) return st;
-    st = bind_frame(comp, S, nullptr, clear, false);
-    if (st) return st;
-
-    FORMA_CUDA_TRY(cudaEventRecord(timer.ev[7], stream));
-    uint32_t n = 0;
-    st = rasterize(comp, S.width, S.height, band_lo, band_hi, &n);
-    if (st) return st;
-    FORMA_CUDA_TRY(cudaEventRecord(timer.ev[2], stream));
-    int timed_sort_passes = 0;
-    if (n > 1) {
-        FORMA_CUDA_TRY(sort_scratch.reserve(radix_scratch_bytes(n)));
-        timed_sort_passes = sort(segs, segs_tmp, nullptr, nullptr, n, segment_plan, timer.sort_ev).timed_passes;
-        FORMA_CUDA_TRY(cudaGetLastError());
-    }
-    FORMA_CUDA_TRY(cudaEventRecord(timer.ev[3], stream));
-
-    const size_t n_tiles_total = (size_t)S.tiles_x * S.tiles_y;
-    last_tiles_x = S.tiles_x;
-    last_tiles_y = S.tiles_y;
-    FORMA_CUDA_TRY(tile_range.reserve(n_tiles_total));
-    FORMA_CUDA_TRY(heavy_tiles.reserve(n_tiles_total * kHeavyListClasses));
-    uint32_t* const heavy_lists = options().paint_lpt ? heavy_tiles.ptr : nullptr;
     uint32_t* id_out = ids;
     if (!ids_on_device) {
         FORMA_CUDA_TRY(id_frame.reserve((size_t)(ids_stride / 4u) * height));
         id_out = id_frame.ptr;
     }
-    // Tables + kernels, once or (when the sync-free bounds were too small) twice, as in render().
-    const uint32_t prev_cells = last_cells, prev_gaps = last_gaps;
-    const bool fast = options().sync_free && n > 0 && prev_cells > 0;
-    last_cells = last_entries = 0;
-    last_written_tiles = 0;
-    last_tables_redone = false;
-    uint32_t kernel_launches = 1;
-    for (bool sync_free = fast;; sync_free = false) {
-        DevCounts dc;
-        st = build_tables(S, n, sync_free, prev_cells, prev_gaps, heavy_lists, dc);
-        if (st) return st;
-        FORMA_CUDA_TRY(id_flags.reserve(std::max<size_t>(recs.capacity, 1)));
-        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[4], stream));
-        if (rgba) {
-            st = paint(S, rgba, rgba, rgba_stride, false, heavy_lists, &kernel_launches);
-            if (st) return st;
-            ++kernel_launches;
-        }
-        launch_paint_ids(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), id_flags.ptr, id_out, ids_stride,
-                         min_coverage, totals.ptr + 8, stream);
-        ++launches;
-        FORMA_CUDA_TRY(cudaGetLastError());
-        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[5], stream));
-        if (!ids_on_device) {
-            st = copy_to_host(S, reinterpret_cast<uint8_t*>(ids), reinterpret_cast<const uint8_t*>(id_out), ids_stride, stream);
-            if (st) return st;
-        }
-        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[6], stream));
-        FORMA_CUDA_TRY(cudaStreamSynchronize(stream));
-        if (!sync_free) break;
-        last_cells = pinned_totals[1];
-        last_gaps = pinned_totals[2];
-        last_entries = last_cells + last_gaps;
-        if (last_cells <= dc.cell_bound && last_gaps <= dc.gap_bound) break;
-        last_tables_redone = true;
-    }
-    last_tables_sync_free = fast && !last_tables_redone;
-    times_pending = true;
-    pending_sort_passes = timed_sort_passes;
-    pending_paint_launches = kernel_launches;
-    if (timings) {
-        resolve_times();
-        const CompDevice& cd = comp.on(res_key);
-        timings->line_setup_ms = stage_ms[1];
-        timings->rasterize_ms = stage_ms[2];
-        timings->sort_ms = stage_ms[3];
-        timings->paint_ms = stage_ms[4] + stage_ms[5];
-        timings->n_lines = cd.n_resident ? cd.n_resident - 1 : 0;
-        timings->n_segments = n;
-    }
-    return FORMA_STATUS_OK;
+    return run_frame(
+        comp, S, FrameSpec{}, timings,
+        [&](const uint32_t* heavy_lists, uint32_t* paint_launches) {
+            FORMA_CUDA_TRY(id_flags.reserve(std::max<size_t>(recs.capacity, 1)));
+            if (rgba) {
+                const int st = paint(S, rgba, rgba, rgba_stride, false, heavy_lists, paint_launches);
+                if (st) return st;
+                ++*paint_launches;
+            }
+            launch_paint_ids(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), id_flags.ptr, id_out, ids_stride,
+                             min_coverage, totals.ptr + 8, stream);
+            ++launches;
+            FORMA_CUDA_TRY(cudaGetLastError());
+            return FORMA_STATUS_OK;
+        },
+        [&] {
+            if (ids_on_device) return FORMA_STATUS_OK;
+            return copy_to_host(S, reinterpret_cast<uint8_t*>(ids), reinterpret_cast<const uint8_t*>(id_out), ids_stride, stream);
+        });
 }
 
-// n views of one composition in one pass: the stages of render() once, over a frame that stacks
-// the views top to bottom, n * rows tile rows of `width` pixels (rows = ceil(height / 16)). Line
-// setup rasterizes every view in its own coordinates and moves its segments' tile rows to the
-// view's place in the stack (ViewArgs); the tables, the sort and the painter see one frame. No
-// layer cache and no band filter: the whole composition is resident.
+// n views of one composition in one pass: one frame that stacks the views top to bottom, n * rows
+// tile rows of `width` pixels (rows = ceil(height / 16)). Line setup rasterizes every view in its
+// own coordinates and moves its segments' tile rows to the view's place in the stack (ViewArgs);
+// the tables, the sort and the painter see one frame. No layer cache and no band filter: the whole
+// composition is resident.
 int Renderer::render_views(Composition& comp, const float* views, uint32_t n, uint8_t* buffer, bool buffer_on_device, uint64_t width,
                            uint64_t stride, uint64_t height, uint64_t view_stride, const uint32_t channels[4], const float clear[4],
                            forma_timings* timings) {
@@ -615,98 +590,32 @@ int Renderer::render_views(Composition& comp, const float* views, uint32_t n, ui
         FORMA_CUDA_TRY(framebuffer.reserve((size_t)fb_stride * S.height));
         fb = framebuffer.ptr;
     }
-
-    if (!prefetched) FORMA_CUDA_TRY(cudaEventRecord(timer.ev[0], stream));
-    prefetched = false;
-    st = upload_tables(comp, -1);
-    if (st) return st;
-    st = flush_geometry(comp);
-    if (st) return st;
-    st = bind_frame(comp, S, nullptr, clear, false);
-    if (st) return st;
-    FORMA_CUDA_TRY(h_views.reserve(6u * n));
-    FORMA_CUDA_TRY(d_views.reserve(6u * n));
-    std::memcpy(h_views.ptr, views, 6u * n * sizeof(float));  // (the previous call's copy is complete: rasterize waited for it)
-    FORMA_CUDA_TRY(cudaMemcpyAsync(d_views.ptr, h_views.ptr, 6u * n * sizeof(float), cudaMemcpyHostToDevice, stream));
-    h2d_bytes += 6u * n * sizeof(float);
-    const ViewArgs va{d_views.ptr, rows};
-
-    FORMA_CUDA_TRY(cudaEventRecord(timer.ev[7], stream));
-    uint32_t n_segs = 0;
-    st = rasterize(comp, S.width, (uint32_t)height, 0.0f, (float)height, &n_segs, &va, n);
-    if (st) return st;
-    FORMA_CUDA_TRY(cudaEventRecord(timer.ev[2], stream));
-    int timed_sort_passes = 0;
-    if (n_segs > 1) {
-        FORMA_CUDA_TRY(sort_scratch.reserve(radix_scratch_bytes(n_segs)));
-        timed_sort_passes = sort(segs, segs_tmp, nullptr, nullptr, n_segs, segment_plan, timer.sort_ev).timed_passes;
-        FORMA_CUDA_TRY(cudaGetLastError());
-    }
-    FORMA_CUDA_TRY(cudaEventRecord(timer.ev[3], stream));
-
-    const size_t n_tiles_total = (size_t)S.tiles_x * S.tiles_y;
-    last_tiles_x = S.tiles_x;
-    last_tiles_y = S.tiles_y;
-    FORMA_CUDA_TRY(tile_range.reserve(n_tiles_total));
-    FORMA_CUDA_TRY(heavy_tiles.reserve(n_tiles_total * kHeavyListClasses));
-    uint32_t* const heavy_lists = options().paint_lpt ? heavy_tiles.ptr : nullptr;
-    // Tables + paint + copy-out, once or (when the sync-free bounds were too small) twice, as in render().
-    const uint32_t prev_cells = last_cells, prev_gaps = last_gaps;
-    const bool fast = options().sync_free && n_segs > 0 && prev_cells > 0;
-    last_cells = last_entries = 0;
-    last_written_tiles = 0;
-    last_tables_redone = false;
-    uint32_t paint_launches = 1;
-    for (bool sync_free = fast;; sync_free = false) {
-        DevCounts dc;
-        st = build_tables(S, n_segs, sync_free, prev_cells, prev_gaps, heavy_lists, dc);
-        if (st) return st;
-        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[4], stream));
-        st = paint(S, fb, fb, fb_stride, false, heavy_lists, &paint_launches, rows);
-        if (st) return st;
-        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[5], stream));
-        if (buffer_on_device && !direct) {
-            launch_repack_views(fb, fb_stride, rows * 16u, buffer, stride, view_stride, S.width, (uint32_t)height, n, stream);
-            ++launches;
-            FORMA_CUDA_TRY(cudaGetLastError());
-        } else if (!buffer_on_device) {
-            // Rows [0, height) of every view, one copy per view with the pitches copy_to_host uses
-            // for a single frame (a copy over all views would have a view as its pitch, which can
-            // exceed the device's largest pitch).
-            for (uint32_t b = 0; b < n; ++b) {
-                uint8_t* dst = buffer + (size_t)b * view_stride;
-                const uint8_t* src = fb + (size_t)b * rows * 16u * fb_stride;
-                if (stride == fb_stride)
-                    FORMA_CUDA_TRY(cudaMemcpyAsync(dst, src, (height - 1u) * stride + 4u * width, cudaMemcpyDeviceToHost, stream));
-                else
-                    FORMA_CUDA_TRY(cudaMemcpy2DAsync(dst, stride, src, fb_stride, 4u * width, height, cudaMemcpyDeviceToHost, stream));
+    return run_frame(
+        comp, S, FrameSpec{nullptr, false, views, n, (uint32_t)height}, timings,
+        [&](const uint32_t* heavy_lists, uint32_t* paint_launches) {
+            return paint(S, fb, fb, fb_stride, false, heavy_lists, paint_launches, rows);
+        },
+        [&] {
+            if (buffer_on_device && !direct) {
+                launch_repack_views(fb, fb_stride, rows * 16u, buffer, stride, view_stride, S.width, (uint32_t)height, n, stream);
+                ++launches;
+                FORMA_CUDA_TRY(cudaGetLastError());
+            } else if (!buffer_on_device) {
+                // Rows [0, height) of every view, one copy per view with the pitches copy_to_host uses
+                // for a single frame (a copy over all views would have a view as its pitch, which can
+                // exceed the device's largest pitch).
+                for (uint32_t b = 0; b < n; ++b) {
+                    uint8_t* dst = buffer + (size_t)b * view_stride;
+                    const uint8_t* src = fb + (size_t)b * rows * 16u * fb_stride;
+                    if (stride == fb_stride)
+                        FORMA_CUDA_TRY(cudaMemcpyAsync(dst, src, (height - 1u) * stride + 4u * width, cudaMemcpyDeviceToHost, stream));
+                    else
+                        FORMA_CUDA_TRY(cudaMemcpy2DAsync(dst, stride, src, fb_stride, 4u * width, height, cudaMemcpyDeviceToHost, stream));
+                }
+                d2h_bytes += (uint64_t)n * height * width * 4u;
             }
-            d2h_bytes += (uint64_t)n * height * width * 4u;
-        }
-        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[6], stream));
-        FORMA_CUDA_TRY(cudaStreamSynchronize(stream));
-        if (!sync_free) break;
-        last_cells = pinned_totals[1];
-        last_gaps = pinned_totals[2];
-        last_entries = last_cells + last_gaps;
-        if (last_cells <= dc.cell_bound && last_gaps <= dc.gap_bound) break;
-        last_tables_redone = true;
-    }
-    last_tables_sync_free = fast && !last_tables_redone;
-    times_pending = true;
-    pending_sort_passes = timed_sort_passes;
-    pending_paint_launches = paint_launches;
-    if (timings) {
-        resolve_times();
-        const CompDevice& cd = comp.on(res_key);
-        timings->line_setup_ms = stage_ms[1];
-        timings->rasterize_ms = stage_ms[2];
-        timings->sort_ms = stage_ms[3];
-        timings->paint_ms = stage_ms[4] + stage_ms[5];
-        timings->n_lines = cd.n_resident ? cd.n_resident - 1 : 0;
-        timings->n_segments = n_segs;
-    }
-    return FORMA_STATUS_OK;
+            return FORMA_STATUS_OK;
+        });
 }
 
 // LinearLayout::new asserts (layout/mod.rs:188-193) + consts.rs limits, and the frame's PaintScene

@@ -37,6 +37,14 @@ struct Timer {
     bool ok = false;
 };
 
+// What differs between the frame kinds before painting (see Renderer::run_frame).
+struct FrameSpec {
+    LayerCache* cache = nullptr;
+    bool pack_written = false;     // only the tiles the frame writes travel back (scatter_written_tiles)
+    const float* views = nullptr;  // render_views: n_views transforms, views of view_height rows; nullptr: one frame
+    uint32_t n_views = 0, view_height = 0;
+};
+
 class Renderer {
    public:
     int device = 0;
@@ -212,11 +220,16 @@ class Renderer {
     // views / n_views: the line setup of render_views (a stacked frame of n_views views).
     int rasterize(Composition& comp, uint32_t width, uint32_t height, float band_lo, float band_hi, uint32_t* n_out,
                   const ViewArgs* views = nullptr, uint32_t n_views = 0);
+    // Every frame kind runs through run_frame (renderer.cu, its only instantiations): FrameSpec says
+    // what differs before painting, paint_step and output_step what differs after the tables.
+    template <class Paint, class Output>
+    int run_frame(Composition& comp, PaintScene& S, const FrameSpec& spec, forma_timings* timings, Paint&& paint_step,
+                  Output&& output_step);
     int render(Composition& comp, uint8_t* buffer, bool buffer_on_device, uint64_t width, uint64_t stride,
                uint64_t height, const uint32_t channels[4], const float clear[4], const forma_rect* crop,
                LayerCache* cache, forma_timings* timings);
-    // ID frames (see forma_renderer_render_ids): the stages of render() without a layer cache, with
-    // the ID kernel in place of paint() or, when `rgba` (a device frame) is given, after it.
+    // ID frames (see forma_renderer_render_ids): a frame without a layer cache, with the ID kernel
+    // in place of paint() or, when `rgba` (a device frame) is given, after it.
     DeviceBuffer<uint8_t> id_flags;   // per entry: the ID kernel's optimizer flags (clip tiles)
     DeviceBuffer<uint32_t> id_frame;  // host ID frames: the frame on the device
     int render_ids(Composition& comp, uint8_t* rgba, uint64_t rgba_stride, const uint32_t channels[4], const float clear[4],
@@ -230,7 +243,7 @@ class Renderer {
     int render_views(Composition& comp, const float* views, uint32_t n, uint8_t* buffer, bool buffer_on_device, uint64_t width,
                      uint64_t stride, uint64_t height, uint64_t view_stride, const uint32_t channels[4], const float clear[4],
                      forma_timings* timings);
-    // The stages of render(), in the order it runs them.
+    // The stages of a frame, in the order they run: begin_frame in the entry points, the rest in run_frame.
     int begin_frame(PaintScene& S, const uint8_t* buffer, uint64_t width, uint64_t stride, uint64_t height,
                     const uint32_t channels[4], const float clear[4], const forma_rect* crop);
     int bind_frame(Composition& comp, PaintScene& S, LayerCache* cache, const float clear[4], bool pack_written);

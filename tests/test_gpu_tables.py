@@ -3,7 +3,8 @@ carry pass (carry-ins, carry-only entries + the gap sort's digit counts), the ga
 merge (entries, tile ranges, heavy-tile lists).
 
 - Launch pin: a sync-free frame launches exactly that chain, 2 + carry passes + 1 + gap passes
-  + 1 kernels, around the rasterizer, the segment sort and the paint kernel.
+  + 1 kernels, around the rasterizer, the segment sort and the kernels of its kind: RGBA, ID,
+  RGBA + ID and view frames (painted in place or repacked).
 - Carry groups across the carry pass's CTA tiles (1024 cells): a 32768 px wide frame whose
   (tile_y, layer) groups hold up to 2048 cells, start exactly on CTA tiles, and whose running
   cover empties and refills along the row under both fill rules; cropped inside the groups
@@ -41,23 +42,42 @@ def _passes(bits: int) -> int:
     return (bits + 7) // 8
 
 
+VIEWS = np.array([[1, 0, 0, 1, 0, 0], [1, 0, 0, 1, -40, 12], [0.5, 0, 0, 0.5, 100, 60]], np.float32)
+
+
 @pytest.mark.gpu
-def test_sync_free_frame_launches_the_table_chain(cuda_api, tables_options):
+@pytest.mark.parametrize("kind,h,after_tables", [
+    ("render_device", 360, 1),
+    ("render_ids_device", 360, 1),
+    ("render_device_with_ids", 360, 2),  # paint + ID kernel
+    ("render_views_device", 352, 1),     # whole tile rows: the views are painted in place
+    ("render_views_device", 360, 2),     # paint into the framebuffer + repack
+], ids=["rgba", "ids", "rgba_with_ids", "views_in_place", "views_repacked"])
+def test_sync_free_frame_launches_the_table_chain(cuda_api, tables_options, kind, h, after_tables):
     """Segment sort forced onto its reduce-then-scan passes (3 launches per pass, counted by
     kernel_times), so that everything but the tables is known: the resident composition's
-    frame rasterizes with 3 launches (line count, block-sum scan, emit) and paints with one."""
-    w, h, layers = 640, 360, 300
+    frame rasterizes with 3 launches (line count, block-sum scan, emit) and launches
+    `after_tables` kernels after the tables, for every frame kind."""
+    w, layers = 640, 300
     cuda_api.set_option("sort_big_log2", 10)
     cuda_api.set_option("sort_scan_log2", 10)
     comp = cuda_api.Composition()
     synth.random_mixed(cuda_api, comp, layers, w, h, 5)
     r = cuda_api.Renderer(0)
-    dev = torch.zeros(w * h * 4, dtype=torch.uint8, device="cuda:0")
+    n_views = len(VIEWS) if kind == "render_views_device" else 1
+    dev = torch.zeros(n_views * w * h * 4, dtype=torch.uint8, device="cuda:0")
+    ids = torch.zeros(w * h, dtype=torch.int32, device="cuda:0")
+    render = {
+        "render_device": lambda: r.render_device(comp, dev.data_ptr(), w, h, RGBA, CLEAR),
+        "render_ids_device": lambda: r.render_ids_device(comp, ids.data_ptr(), w, h),
+        "render_device_with_ids": lambda: r.render_device_with_ids(comp, dev.data_ptr(), ids.data_ptr(), w, h, RGBA, CLEAR),
+        "render_views_device": lambda: r.render_views_device(comp, VIEWS, dev.data_ptr(), w, h, RGBA, CLEAR),
+    }[kind]
     for _ in range(2):  # frame 1: counts read back; frame 2 has the previous counts as bounds
-        r.render_device(comp, dev.data_ptr(), w, h, RGBA, CLEAR)
+        render()
         torch.cuda.synchronize()
     before = r.counters()["launches"]
-    r.render_device(comp, dev.data_ptr(), w, h, RGBA, CLEAR)
+    render()
     torch.cuda.synchronize()
     c = r.counters()
     assert c["tables_mode"] == 1
@@ -66,12 +86,13 @@ def test_sync_free_frame_launches_the_table_chain(cuda_api, tables_options):
     assert sort_passes > 0
     raster = 3
     assert c["segments"] > 2048  # more than one CTA tile of the cells pass: both cells kernels run
-    tiles_x, tiles_y = (w + 15) // 16, (h + 15) // 16
+    tiles_x, tiles_y = (w + 15) // 16, n_views * ((h + 15) // 16)  # views: one frame of stacked views
     carry = _passes(int(layers - 1).bit_length())
     gap = _passes(int(tiles_x).bit_length() + int(tiles_y).bit_length())
     tables = 2 + carry + 1 + gap + 1
-    assert tables == 8
-    assert frame == raster + 3 * sort_passes + tables + 1, (frame, raster, sort_passes)
+    if n_views == 1:
+        assert tables == 8
+    assert frame == raster + 3 * sort_passes + tables + after_tables, (frame, raster, sort_passes, tables)
 
 
 # ---------------------------------------------------------------------------
