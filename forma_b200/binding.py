@@ -286,6 +286,10 @@ SIGNATURES = {
                                         C.POINTER(_CTimings)]),
     "renderer_render_views_device": (C.c_int, [_vp, _vp, _fp, C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, _u32p,
                                                _fp, C.POINTER(_CTimings)]),
+    "renderer_render_batch": (C.c_int, [_vp, C.POINTER(_vp), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, _u32p,
+                                        _fp, C.POINTER(_CTimings)]),
+    "renderer_render_batch_device": (C.c_int, [_vp, C.POINTER(_vp), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
+                                               _u32p, _fp, C.POINTER(_CTimings)]),
     "renderer_launch_count": (C.c_uint64, [_vp]),
     "renderer_stage_times": (None, [_vp, C.POINTER(C.c_double)]),
     "renderer_counters": (None, [_vp, _u64p]),
@@ -321,6 +325,8 @@ ID_FRAME_SYMBOLS = ("renderer_render_ids", "renderer_render_ids_device", "render
 # The entry points of views (Renderer.render_views): the CUDA library has them, other libraries
 # with this binding's symbols may not (the view methods of Renderer then fail).
 VIEW_SYMBOLS = ("renderer_max_views", "renderer_render_views", "renderer_render_views_device")
+# The same for batches (Renderer.render_batch).
+BATCH_SYMBOLS = ("renderer_render_batch", "renderer_render_batch_device")
 
 
 class Api:
@@ -332,7 +338,7 @@ class Api:
             try:
                 fn = getattr(lib, prefix + name)
             except AttributeError:
-                if name in optional or name in ID_FRAME_SYMBOLS or name in VIEW_SYMBOLS:
+                if name in optional or name in ID_FRAME_SYMBOLS or name in VIEW_SYMBOLS or name in BATCH_SYMBOLS:
                     continue
                 raise
             fn.restype, fn.argtypes = res, args
@@ -842,6 +848,48 @@ class Renderer:
         view_stride = height * stride if view_stride is None else view_stride
         return self._views(self._api.renderer_render_views_device, "Renderer::render_views_device", composition, views,
                            int(device_ptr), width, height, channels, clear_color, stride, view_stride, timings)
+
+    def _batch(self, fn, what, comps, ptr, width, height, channels, clear_color, stride, frame_stride, timings):
+        """Calls `fn` on chunks of at most max_views(height) compositions, frame c at ptr + c * frame_stride."""
+        comps = list(comps)
+        ch, cc, _ = self._common(channels, clear_color, None)
+        chunk = max(self.max_views(height), 1)
+        t = None
+        for first in range(0, max(len(comps), 1), chunk):
+            part = comps[first:first + chunk]
+            handles = (_vp * max(len(part), 1))(*[c._h for c in part])
+            t = _CTimings() if timings else None
+            st = fn(self._h, handles, len(part), C.c_void_p(ptr + first * frame_stride), width, stride, height, frame_stride, ch, cc,
+                    C.byref(t) if t is not None else None)
+            self._api.check(st, what)
+        return self._timings(t)
+
+    def render_batch(self, comps, buffer: np.ndarray, width: int, height: int, channels=RGBA,
+                     clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
+                     frame_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """One frame per composition of the sequence `comps` (repeats allowed), frame c showing
+        comps[c] alone, from one pass through the stages. Frame c starts at byte c * frame_stride
+        (default height * stride) of `buffer`, a writable contiguous uint8 host array; `stride`
+        (default 4 * width) is the row stride. N may exceed max_views(height): the compositions
+        are then rendered in chunks. A chunk whose distinct compositions need more than 2^21 layer
+        orders raises OrderError. Returns the timings of the last chunk."""
+        comps = list(comps)
+        stride = width * 4 if stride is None else stride
+        frame_stride = height * stride if frame_stride is None else frame_stride
+        assert buffer.dtype == np.uint8 and buffer.flags["C_CONTIGUOUS"]
+        assert not comps or buffer.size >= (len(comps) - 1) * frame_stride + (height - 1) * stride + 4 * width
+        return self._batch(self._api.renderer_render_batch, "Renderer::render_batch", comps, buffer.ctypes.data, width, height,
+                           channels, clear_color, stride, frame_stride, timings)
+
+    def render_batch_device(self, comps, device_ptr: int, width: int, height: int, channels=RGBA,
+                            clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
+                            frame_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """render_batch into device memory on the renderer's device: with the defaults, the
+        data_ptr() of a contiguous [N, height, width, 4] uint8 CUDA tensor."""
+        stride = width * 4 if stride is None else stride
+        frame_stride = height * stride if frame_stride is None else frame_stride
+        return self._batch(self._api.renderer_render_batch_device, "Renderer::render_batch_device", comps, int(device_ptr), width,
+                           height, channels, clear_color, stride, frame_stride, timings)
 
     def launch_count(self) -> int:
         return int(self._api.renderer_launch_count(self._h))

@@ -426,6 +426,27 @@ int forma_renderer_render_views_device(forma_renderer* r, forma_composition* c, 
                                  timings);
     });
 }
+// The Compositions behind the handles (null entries stay null for Renderer::render_batch to refuse).
+static int render_batch(forma_renderer* r, forma_composition* const* comps, uint32_t n, uint8_t* buffer, bool on_device,
+                        uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride, const uint32_t channels[4],
+                        const float clear_color[4], forma_timings* timings) {
+    return guarded((int)FORMA_ERR_CAPACITY, [&] {
+        std::vector<Composition*> cs(comps ? n : 0u);
+        for (size_t k = 0; k < cs.size(); ++k) cs[k] = comps[k] ? &comps[k]->c : nullptr;
+        return r->r.render_batch(comps ? cs.data() : nullptr, n, buffer, on_device, width, width_stride, height, frame_stride, channels,
+                                 clear_color, timings);
+    });
+}
+int forma_renderer_render_batch_device(forma_renderer* r, forma_composition* const* comps, uint32_t n, uint8_t* device_buffer,
+                                       uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride,
+                                       const uint32_t channels[4], const float clear_color[4], forma_timings* timings) {
+    return render_batch(r, comps, n, device_buffer, true, width, width_stride, height, frame_stride, channels, clear_color, timings);
+}
+int forma_renderer_render_batch(forma_renderer* r, forma_composition* const* comps, uint32_t n, uint8_t* host_buffer, uint64_t width,
+                                uint64_t width_stride, uint64_t height, uint64_t frame_stride, const uint32_t channels[4],
+                                const float clear_color[4], forma_timings* timings) {
+    return render_batch(r, comps, n, host_buffer, false, width, width_stride, height, frame_stride, channels, clear_color, timings);
+}
 int forma_renderer_render_views(forma_renderer* r, forma_composition* c, const float* views, uint32_t n, uint8_t* host_buffer,
                                 uint64_t width, uint64_t width_stride, uint64_t height, uint64_t view_stride,
                                 const uint32_t channels[4], const float clear_color[4], forma_timings* timings) {
@@ -650,7 +671,7 @@ static uint64_t rasterize_only_impl(forma_renderer* r, forma_composition* c, uin
     if (cudaSetDevice(R.device) != cudaSuccess) return 0;
     if (R.upload_tables(c->c, -1) || R.flush_geometry(c->c)) return 0;
     uint32_t n = 0;
-    if (R.rasterize(c->c, (uint32_t)std::min<uint64_t>(width, 0xFFFFFFFFu), (uint32_t)std::min<uint64_t>(height, 0xFFFFFFFFu),
+    if (R.rasterize(&c->c, (uint32_t)std::min<uint64_t>(width, 0xFFFFFFFFu), (uint32_t)std::min<uint64_t>(height, 0xFFFFFFFFu),
                     -3.0e38f, 3.0e38f, &n))
         return 0;
     if (cudaStreamSynchronize(R.stream) != cudaSuccess) return 0;

@@ -8,6 +8,7 @@
 // composition is rendered.
 #pragma once
 
+#include <atomic>
 #include <map>
 #include <memory>
 #include <unordered_map>
@@ -97,6 +98,13 @@ struct CompDevice {
 
 class Composition {
    public:
+    // Unique in the process and never reused (an address can be: a freed composition and a new
+    // one may share it): what a renderer's batch tables are keyed on, with tables_version.
+    const uint64_t serial = new_serial();
+    static uint64_t new_serial() {
+        static std::atomic<uint64_t> next{1};
+        return next++;
+    }
     std::map<uint32_t, Layer*> layers;              // attached layers by order
     std::unordered_map<Layer*, std::unique_ptr<Layer>> pool;  // every live layer (attached or not)
     std::unordered_map<uint32_t, int64_t> geom_to_order;  // dense id -> order, -1 == None

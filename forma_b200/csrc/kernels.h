@@ -80,6 +80,35 @@ void launch_line_count_views(const RasterArgs& args, const ViewArgs& views, uint
                              uint32_t* max_tile, cudaStream_t stream);
 void launch_raster_emit_views(const RasterArgs& args, const ViewArgs& views, uint32_t n_views, const uint32_t* block_offsets,
                               uint64_t* out, uint32_t cap, cudaStream_t stream);
+// Batches (see forma_renderer_render_batch_device): frame c of a stack of n_frames frames is a
+// composition of its own. Each frame's line setup reads its composition's segment buffer and
+// tables (as RasterArgs, over the whole frame), and only two key fields move: row t of frame c
+// becomes biased c * rows + t + 1 (rows outside the frame 0, as for views), and the layer field
+// gets the frame's order base.
+struct BatchFrame {  // 64 B
+    const float* x;
+    const float* y;
+    const uint32_t* gid;
+    const int32_t* geom_slot;
+    const LayerRec* layers;      // nullptr: layer_bits
+    const uint32_t* layer_bits;
+    uint32_t n_points, n_geoms;
+    uint32_t order_base;         // first order of the composition's slice of the layer field
+    uint32_t pad;
+};
+struct BatchArgs {
+    const BatchFrame* frames;
+    const uint32_t* cta_first;   // n_frames + 1: the frame's first CTA (its CTA count is the next entry minus this)
+    uint32_t n_frames;
+    uint32_t rows;               // tile rows per frame: ceil(height / 16)
+    float width, height;
+};
+// One CTA of raster_num_blocks(n_points) per frame, frame-major: cta_first[n_frames] block sums.
+// max_tile[1] is the stacked bound.
+void launch_line_count_batch(const BatchArgs& batch, uint32_t n_ctas, uint32_t* block_sums, uint32_t* total, uint32_t* max_tile,
+                             cudaStream_t stream);
+void launch_raster_emit_batch(const BatchArgs& batch, uint32_t n_ctas, const uint32_t* block_offsets, uint64_t* out, uint32_t cap,
+                              cudaStream_t stream);
 // Line records of the n = n_points - 1 point pairs (inspection only): orders, then
 // f = {x0, y0, dx, dy, a, b, c, d}, then the per-line segment counts.
 void launch_line_records(const RasterArgs& args, uint32_t n, uint32_t* orders, float* const f[8], uint32_t* lengths,
@@ -251,6 +280,21 @@ void launch_repack_views(const uint8_t* src, uint64_t src_stride, uint32_t view_
 void launch_paint_ids(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range,
                       const uint32_t* heavy, const uint32_t* heavy_count, uint8_t* id_flags, uint32_t* ids, size_t ids_stride,
                       float min_coverage, uint32_t* tile_counter, cudaStream_t st);
+// The painter tables of a batch: the device tables of its distinct compositions, concatenated.
+// Composition k's orders land at order_base + order (the slots they name shifted by style_base,
+// -1 kept), its StyleRecs at style_base with stop_first + stop_base and tex_first + texel_base;
+// stops, texels (in texels of 4 x u16) and GradRecs are copied as they are.
+struct BatchTableSrc {
+    const int32_t* order_to_style;
+    const StyleRec* styles;
+    const GradRec* grads;
+    const StopRec* stops;
+    const uint16_t* texels;
+    uint32_t n_orders, n_styles, n_stops, n_texels;  // n_texels: texels (4 x u16 each)
+    uint32_t order_base, style_base, stop_base, texel_base;
+};
+void launch_batch_tables(const BatchTableSrc* src, uint32_t n_src, uint32_t max_items, int32_t* order_to_style, StyleRec* styles,
+                         GradRec* grads, StopRec* stops, uint16_t* texels, cudaStream_t st);
 // GradRec of every style slot (see device_types.h).
 void launch_grad_setup(const StyleRec* styles, const StopRec* stops, uint32_t n_styles, GradRec* grads, cudaStream_t st);
 // Pixel-pair fp32 arithmetic of the painter against scalar IEEE operations; mismatches are added to out[0].

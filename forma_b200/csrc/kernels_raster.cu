@@ -282,16 +282,47 @@ __device__ __forceinline__ LineParams line_setup(const RasterArgs& A, uint32_t i
 
 constexpr int kRasterThreads = 256;
 
+// Where a CTA of a batch works: its frame, its CTA within the frame's points, the frame's order base.
+struct BatchPos {
+    uint32_t frame, block, order_base;
+};
+// The CTA's frame (the last one whose first CTA is at or before it: frames without points own no
+// CTA) and that frame's line-setup arguments, over the whole frame.
+__device__ __forceinline__ BatchPos batch_pos(const BatchArgs& B, RasterArgs& A) {
+    uint32_t lo = 0, hi = B.n_frames - 1u;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1u) >> 1;
+        if (B.cta_first[mid] <= blockIdx.x) lo = mid;
+        else hi = mid - 1u;
+    }
+    const BatchFrame& F = B.frames[lo];
+    A.x = F.x;
+    A.y = F.y;
+    A.gid = F.gid;
+    A.n_points = F.n_points;
+    A.geom_slot = F.geom_slot;
+    A.n_geoms = F.n_geoms;
+    A.layers = F.layers;
+    A.layer_bits = F.layer_bits;
+    A.width = B.width;
+    A.height = B.height;
+    A.band_lo = 0.0f;
+    A.band_hi = B.height;
+    return BatchPos{lo, blockIdx.x - B.cta_first[lo], F.order_base};
+}
+
 // Pass 1: per-CTA sum of line lengths.
 // Also tracks the largest (biased) tile coordinates any pixel segment can take,
 // so that the sort only spends passes on key bits that can be set.
 // kViews: CTA (x, y) = the point pairs of CTA x under view y; its sum is block y * gridDim.x + x.
-template <bool kViews>
+// kBatch: CTA x = the point pairs of CTA P.block of frame P.frame (V.rows: the frame's tile rows);
+// its sum is block x.
+template <bool kViews, bool kBatch = false>
 __device__ __forceinline__ void line_count_body(const RasterArgs& A, const ViewArgs& V, uint32_t* __restrict__ block_sums,
-                                                uint32_t* __restrict__ max_tile) {
+                                                uint32_t* __restrict__ max_tile, const BatchPos& P = BatchPos{}) {
     __shared__ uint32_t warp_sums[kRasterThreads / 32];
     __shared__ uint32_t warp_max[2][kRasterThreads / 32];
-    uint32_t i = blockIdx.x * kRasterThreads + threadIdx.x;
+    uint32_t i = (kBatch ? P.block : blockIdx.x) * kRasterThreads + threadIdx.x;
     const LineParams L = line_setup<kViews>(A, i, kViews ? V.xf + 6u * blockIdx.y : nullptr);
     uint32_t len = L.length;
     {
@@ -303,9 +334,9 @@ __device__ __forceinline__ void line_count_body(const RasterArgs& A, const ViewA
             int32_t ty = ((int32_t)floorf(fminf(ey, 3.0e7f) + 0.5f) >> 8) + 2;
             bx = (uint32_t)min(max(tx, 0), 4095);
             by = (uint32_t)min(max(ty, 0), 2047);
-            if constexpr (kViews) {
+            if constexpr (kViews || kBatch) {
                 // The emit pass maps view y's segments to the stacked rows [y * rows + 1, (y + 1) * rows].
-                by = (blockIdx.y + 1u) * V.rows;
+                by = ((kBatch ? P.frame : blockIdx.y) + 1u) * V.rows;
                 // Tile columns left of -32767 wrap (int16, as in the reference) into the frame's
                 // columns: such a line can set any tile_x bit.
                 if (!(fminf(L.x0, L.x0 + L.dx) >= -8388352.0f)) bx = 4095;
@@ -331,7 +362,7 @@ __device__ __forceinline__ void line_count_body(const RasterArgs& A, const ViewA
             bx = max(bx, warp_max[0][w]);
             by = max(by, warp_max[1][w]);
         }
-        block_sums[kViews ? blockIdx.y * gridDim.x + blockIdx.x : blockIdx.x] = s;
+        block_sums[kViews && !kBatch ? blockIdx.y * gridDim.x + blockIdx.x : blockIdx.x] = s;
         // Same-address atomics serialise in L2: only raise the maximum when needed.
         if (bx > *(volatile uint32_t*)&max_tile[0]) atomicMax(&max_tile[0], bx);
         if (by > *(volatile uint32_t*)&max_tile[1]) atomicMax(&max_tile[1], by);
@@ -344,6 +375,12 @@ __global__ void __launch_bounds__(kRasterThreads) line_count_kernel(RasterArgs A
 __global__ void __launch_bounds__(kRasterThreads) line_count_views_kernel(RasterArgs A, ViewArgs V, uint32_t* __restrict__ block_sums,
                                                                         uint32_t* __restrict__ max_tile) {
     line_count_body<true>(A, V, block_sums, max_tile);
+}
+__global__ void __launch_bounds__(kRasterThreads) line_count_batch_kernel(BatchArgs B, uint32_t* __restrict__ block_sums,
+                                                                        uint32_t* __restrict__ max_tile) {
+    RasterArgs A;
+    const BatchPos P = batch_pos(B, A);
+    line_count_body<false, true>(A, ViewArgs{nullptr, B.rows}, block_sums, max_tile, P);
 }
 
 // Device-wide exclusive scan of `n` u32 values by ONE CTA (n = number of CTAs
@@ -428,15 +465,17 @@ struct SharedLines {
 // for its whole length (measured on paris@4K: the kernel's time was one warp's tail — it did
 // not shrink when seven eighths of the lines were culled).
 // kViews: CTA (x, y) emits view y's segments of the CTA x lines (see line_count_body).
-template <bool kViews>
+// kBatch: CTA x emits frame P.frame's segments, its layers moved up by the frame's order base.
+template <bool kViews, bool kBatch = false>
 __device__ __forceinline__ void raster_emit_body(const RasterArgs& A, const ViewArgs& V, const uint32_t* __restrict__ block_offsets,
-                                                 uint64_t* __restrict__ out, uint32_t cap) {
+                                                 uint64_t* __restrict__ out, uint32_t cap, const BatchPos& P = BatchPos{}) {
     __shared__ SharedLines S;
     __shared__ uint32_t warp_sums[kRasterThreads / 32];
     const uint32_t t = threadIdx.x;
     const uint32_t warp = t >> 5, lane = t & 31u;
-    uint32_t i = blockIdx.x * kRasterThreads + t;
+    uint32_t i = (kBatch ? P.block : blockIdx.x) * kRasterThreads + t;
     LineParams L = line_setup<kViews>(A, i, kViews ? V.xf + 6u * blockIdx.y : nullptr);
+    if constexpr (kBatch) L.order += P.order_base;
     uint32_t incl = warp_inclusive_scan_sat(L.length);
     if (lane == 31) warp_sums[warp] = incl;
     if (L.length) {
@@ -460,7 +499,7 @@ __device__ __forceinline__ void raster_emit_body(const RasterArgs& A, const View
     // then only steer the bisection, which stays inside S.excl).
     S.excl[t] = before + incl - L.length;  // exclusive prefix over the block's 256 lines
     __syncthreads();
-    const uint32_t block_base = block_offsets[kViews ? blockIdx.y * gridDim.x + blockIdx.x : blockIdx.x];
+    const uint32_t block_base = block_offsets[kViews && !kBatch ? blockIdx.y * gridDim.x + blockIdx.x : blockIdx.x];
     // `cap` bounds a speculative launch made before the segment count is known on the host: the
     // loop never runs past it, whatever the (saturated) counts of an over-limit frame. The last
     // clamp keeps `s += kRasterThreads` from wrapping.
@@ -503,7 +542,7 @@ __device__ __forceinline__ void raster_emit_body(const RasterArgs& A, const View
         // A view's painted rows (biased 1 ... rows) move to its place in the stacked frame; every
         // other row becomes tile row -1 (biased 0), which no painted tile reads, so that nothing
         // bleeds into the neighbouring views. The single frame's own wrap of the field is kept.
-        if constexpr (kViews) ty = ty - 1u < V.rows ? ty + (uint64_t)blockIdx.y * V.rows : 0u;
+        if constexpr (kViews || kBatch) ty = ty - 1u < V.rows ? ty + (uint64_t)(kBatch ? P.frame : blockIdx.y) * V.rows : 0u;
         uint64_t tx = (uint64_t)max((int32_t)(int16_t)(tile_x + 1), 0) & 0xFFFull;
         uint64_t v = (ty << 53) | (tx << 41) | ((uint64_t)(S.order[li] & 0x1FFFFFu) << 20) | ((uint64_t)local_x << 16) |
                      ((uint64_t)local_y << 12) | ((uint64_t)(dam & 0x3Fu) << 6) | ((uint64_t)((uint32_t)cover & 0x3Fu));
@@ -517,6 +556,12 @@ __global__ void __launch_bounds__(kRasterThreads)
 __global__ void __launch_bounds__(kRasterThreads) raster_emit_views_kernel(RasterArgs A, ViewArgs V, const uint32_t* __restrict__ block_offsets,
                                                                          uint64_t* __restrict__ out, uint32_t cap) {
     raster_emit_body<true>(A, V, block_offsets, out, cap);
+}
+__global__ void __launch_bounds__(kRasterThreads) raster_emit_batch_kernel(BatchArgs B, const uint32_t* __restrict__ block_offsets,
+                                                                         uint64_t* __restrict__ out, uint32_t cap) {
+    RasterArgs A;
+    const BatchPos P = batch_pos(B, A);
+    raster_emit_body<false, true>(A, ViewArgs{nullptr, B.rows}, block_offsets, out, cap, P);
 }
 
 // Inspection only (forma_renderer_lines): the line records of segment.rs:298-383 as the
@@ -589,6 +634,23 @@ void launch_raster_emit_views(const RasterArgs& args, const ViewArgs& views, uin
     uint32_t nb = raster_num_blocks(args.n_points);
     if (!nb || !n_views) return;
     raster_emit_views_kernel<<<dim3(nb, n_views), kRasterThreads, 0, stream>>>(args, views, block_offsets, out, cap);
+}
+
+void launch_line_count_batch(const BatchArgs& batch, uint32_t n_ctas, uint32_t* block_sums, uint32_t* total, uint32_t* max_tile,
+                             cudaStream_t stream) {
+    cudaMemsetAsync(max_tile, 0, 2 * sizeof(uint32_t), stream);
+    if (!n_ctas) {
+        cudaMemsetAsync(total, 0, sizeof(uint32_t), stream);
+        return;
+    }
+    line_count_batch_kernel<<<n_ctas, kRasterThreads, 0, stream>>>(batch, block_sums, max_tile);
+    scan_block_sums_kernel<<<1, 1024, 0, stream>>>(block_sums, n_ctas, total);
+}
+
+void launch_raster_emit_batch(const BatchArgs& batch, uint32_t n_ctas, const uint32_t* block_offsets, uint64_t* out, uint32_t cap,
+                              cudaStream_t stream) {
+    if (!n_ctas) return;
+    raster_emit_batch_kernel<<<n_ctas, kRasterThreads, 0, stream>>>(batch, block_offsets, out, cap);
 }
 
 }  // namespace forma

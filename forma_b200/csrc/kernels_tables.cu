@@ -847,5 +847,40 @@ void launch_merge_entries(const PaintScene& S, const uint64_t* cell_key, uint32_
                                                                gap_carry, ekey, recs, eflags, tile_range, heavy, heavy_count, dc);
 }
 
+// ---------------------------------------------------------------------------
+// Batch tables
+// ---------------------------------------------------------------------------
+// CTA (x, k) copies every gridDim.x-th run of 256 records of composition k's tables into the
+// batch's, moving the indices into the shared arrays by the composition's bases.
+__global__ void __launch_bounds__(256) batch_tables_kernel(const BatchTableSrc* __restrict__ src, int32_t* __restrict__ order_to_style,
+                                                           StyleRec* __restrict__ styles, GradRec* __restrict__ grads,
+                                                           StopRec* __restrict__ stops, uint2* __restrict__ texels) {
+    const BatchTableSrc s = src[blockIdx.y];
+    const uint32_t step = gridDim.x * blockDim.x;
+    const uint32_t first = blockIdx.x * blockDim.x + threadIdx.x;
+    for (uint32_t i = first; i < s.n_orders; i += step) {
+        const int32_t slot = s.order_to_style[i];
+        order_to_style[s.order_base + i] = slot < 0 ? -1 : slot + (int32_t)s.style_base;
+    }
+    for (uint32_t i = first; i < s.n_styles; i += step) {
+        StyleRec r = s.styles[i];
+        r.stop_first += s.stop_base;
+        r.tex_first += s.texel_base;
+        styles[s.style_base + i] = r;
+        grads[s.style_base + i] = s.grads[i];
+    }
+    for (uint32_t i = first; i < s.n_stops; i += step) stops[s.stop_base + i] = s.stops[i];
+    const uint2* tex = reinterpret_cast<const uint2*>(s.texels);  // one texel = 4 x u16 = 8 B
+    for (uint32_t i = first; i < s.n_texels; i += step) texels[s.texel_base + i] = tex[i];
+}
+
+void launch_batch_tables(const BatchTableSrc* src, uint32_t n_src, uint32_t max_items, int32_t* order_to_style, StyleRec* styles,
+                         GradRec* grads, StopRec* stops, uint16_t* texels, cudaStream_t st) {
+    if (!n_src || !max_items) return;
+    const uint32_t per_comp = std::min<uint32_t>((max_items + 255u) / 256u, 256u);
+    batch_tables_kernel<<<dim3(per_comp, n_src), 256, 0, st>>>(src, order_to_style, styles, grads, stops,
+                                                               reinterpret_cast<uint2*>(texels));
+}
+
 
 }  // namespace forma

@@ -244,24 +244,26 @@ int Renderer::upload_tables_device(Composition& comp, CompDevice& cd) {
 }
 
 // Stages 1½ + 2: fills `segs` with the unsorted pixel segments.
-int Renderer::rasterize(Composition& comp, uint32_t width, uint32_t height, float band_lo, float band_hi,
-                        uint32_t* n_out, const ViewArgs* views, uint32_t n_views) {
-    RasterArgs& ra = last_raster;  // kept for forma_renderer_lines (a stacked frame of views has no line records)
-    last_raster_valid = !views;
-    CompDevice& cd = comp.on(res_key);
-    ra.x = cd.d_x.ptr;
-    ra.y = cd.d_y.ptr;
-    ra.gid = cd.d_gid.ptr;
-    ra.n_points = cd.n_resident;
-    ra.geom_slot = cd.d_geom_slot.ptr;
-    ra.n_geoms = comp.n_geoms;
-    ra.layers = comp.layers_have_xf ? cd.d_layers.ptr : nullptr;
-    ra.layer_bits = cd.d_layer_bits.ptr;
-    ra.width = (float)width;
-    ra.height = (float)height;
-    ra.band_lo = band_lo;
-    ra.band_hi = band_hi;
-    uint32_t nb = raster_num_blocks(ra.n_points);
+int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, float band_lo, float band_hi,
+                        uint32_t* n_out, const ViewArgs* views, uint32_t n_views, const BatchLines* batch) {
+    RasterArgs& ra = last_raster;  // kept for forma_renderer_lines (a stacked frame has no line records)
+    last_raster_valid = !views && !batch;
+    if (comp) {
+        CompDevice& cd = comp->on(res_key);
+        ra.x = cd.d_x.ptr;
+        ra.y = cd.d_y.ptr;
+        ra.gid = cd.d_gid.ptr;
+        ra.n_points = cd.n_resident;
+        ra.geom_slot = cd.d_geom_slot.ptr;
+        ra.n_geoms = comp->n_geoms;
+        ra.layers = comp->layers_have_xf ? cd.d_layers.ptr : nullptr;
+        ra.layer_bits = cd.d_layer_bits.ptr;
+        ra.width = (float)width;
+        ra.height = (float)height;
+        ra.band_lo = band_lo;
+        ra.band_hi = band_hi;
+    }
+    uint32_t nb = batch ? batch->n_ctas : raster_num_blocks(ra.n_points);
     if (views) {
         if ((uint64_t)nb * n_views >= (1ull << 32)) {
             set_error("%u views of %u points exceed the line-setup grid", n_views, ra.n_points);
@@ -270,11 +272,13 @@ int Renderer::rasterize(Composition& comp, uint32_t width, uint32_t height, floa
         nb *= n_views;  // one CTA sum per (view, CTA of points)
     }
     FORMA_CUDA_TRY(block_sums.reserve(nb + 1));
-    if (views) launch_line_count_views(ra, *views, n_views, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
+    if (batch) launch_line_count_batch(batch->args, nb, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
+    else if (views) launch_line_count_views(ra, *views, n_views, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
     else launch_line_count(ra, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
     launches += nb ? 2 : 0;
     auto emit = [&](uint32_t cap) {
-        if (views) launch_raster_emit_views(ra, *views, n_views, block_sums.ptr, segs.ptr, cap, stream);
+        if (batch) launch_raster_emit_batch(batch->args, nb, block_sums.ptr, segs.ptr, cap, stream);
+        else if (views) launch_raster_emit_views(ra, *views, n_views, block_sums.ptr, segs.ptr, cap, stream);
         else launch_raster_emit(ra, block_sums.ptr, segs.ptr, cap, stream);
     };
     uint32_t n = 0;
@@ -298,7 +302,9 @@ int Renderer::rasterize(Composition& comp, uint32_t width, uint32_t height, floa
     {
         // Already ordered by layer: no layer digits (see Composition::layers_in_order).
         const bool skip_layer_digits = options().sort_full_key == 0;
-        const uint64_t layer_bound = (comp.layers_in_order && skip_layer_digits) ? 0u : (comp.n_orders ? comp.n_orders - 1u : 0u);
+        const uint64_t layer_bound = batch ? batch->layer_bound
+                                     : (comp->layers_in_order && skip_layer_digits) ? 0u
+                                                                                    : (comp->n_orders ? comp->n_orders - 1u : 0u);
         const uint64_t bound[3] = {layer_bound, pinned_totals[4], pinned_totals[5]};
         segment_plan = make_sort_plan(segment_key_layout(), bound);  // layer, tile_x, tile_y
     }
@@ -360,24 +366,31 @@ int Renderer::prefetch(Composition& comp, uint64_t width, uint64_t height, const
 // paint_step(heavy_lists, &paint_launches) (the frame's kernels) and output_step() (the copy to
 // where the caller wants the frame) once or, when the sync-free bounds were too small, twice.
 template <class Paint, class Output>
-int Renderer::run_frame(Composition& comp, PaintScene& S, const FrameSpec& spec, forma_timings* timings, Paint&& paint_step,
+int Renderer::run_frame(Composition* comp, PaintScene& S, const FrameSpec& spec, forma_timings* timings, Paint&& paint_step,
                         Output&& output_step) {
     if (!prefetched) FORMA_CUDA_TRY(cudaEventRecord(timer.ev[0], stream));
     prefetched = false;
     // Lines entirely above / below the painted tile rows cannot reach a painted tile: they are
     // culled per line (rasterize), and whole inserts are left out of the device's segment
-    // buffer when the band is narrower than the frame (flush_geometry). Line setup sees every view
-    // as a frame of its own: all its rows are painted.
-    const uint32_t height = spec.views ? spec.view_height : S.height;
-    const FrameBand band = spec.views ? FrameBand{0.0f, (float)height, false} : tile_band(S.ty_lo, S.ty_hi, height);
-    int st = upload_tables(comp, -1);
-    if (st) return st;
-    st = flush_geometry(comp, band.lo, band.hi, band.partial);
-    if (st) return st;
-    st = bind_frame(comp, S, spec.cache, S.clear, spec.pack_written);
-    if (st) return st;
+    // buffer when the band is narrower than the frame (flush_geometry). Line setup sees every
+    // frame of a stack as a frame of its own: all its rows are painted.
+    const uint32_t height = spec.n_frames ? spec.frame_height : S.height;
+    const FrameBand band = spec.n_frames ? FrameBand{0.0f, (float)height, false} : tile_band(S.ty_lo, S.ty_hi, height);
+    int st = FORMA_STATUS_OK;
+    BatchLines batch{};
+    if (spec.batch) {  // every composition's uploads, then the batch tables
+        st = bind_batch(spec.batch, spec.n_frames, S, height, batch);
+        if (st) return st;
+    } else {
+        st = upload_tables(*comp, -1);
+        if (st) return st;
+        st = flush_geometry(*comp, band.lo, band.hi, band.partial);
+        if (st) return st;
+        st = bind_frame(*comp, S, spec.cache, S.clear, spec.pack_written);
+        if (st) return st;
+    }
     if (spec.views) {
-        const uint32_t nv = spec.n_views;
+        const uint32_t nv = spec.n_frames;
         FORMA_CUDA_TRY(h_views.reserve(6u * nv));
         FORMA_CUDA_TRY(d_views.reserve(6u * nv));
         std::memcpy(h_views.ptr, spec.views, 6u * nv * sizeof(float));  // (the previous call's copy is complete: rasterize waited for it)
@@ -388,7 +401,8 @@ int Renderer::run_frame(Composition& comp, PaintScene& S, const FrameSpec& spec,
 
     FORMA_CUDA_TRY(cudaEventRecord(timer.ev[7], stream));
     uint32_t n = 0;
-    st = rasterize(comp, S.width, height, band.lo, band.hi, &n, spec.views ? &va : nullptr, spec.n_views);
+    st = rasterize(comp, S.width, height, band.lo, band.hi, &n, spec.views ? &va : nullptr, spec.n_frames,
+                   spec.batch ? &batch : nullptr);
     if (st) return st;
 
     // Stage 3: sort.
@@ -451,12 +465,16 @@ int Renderer::run_frame(Composition& comp, PaintScene& S, const FrameSpec& spec,
     pending_paint_launches = paint_launches;
     if (timings) {
         resolve_times();
-        const CompDevice& cd = comp.on(res_key);
         timings->line_setup_ms = stage_ms[1];
         timings->rasterize_ms = stage_ms[2];
         timings->sort_ms = stage_ms[3];
         timings->paint_ms = stage_ms[4] + stage_ms[5];
-        timings->n_lines = cd.n_resident ? cd.n_resident - 1 : 0;
+        if (comp) {
+            const CompDevice& cd = comp->on(res_key);
+            timings->n_lines = cd.n_resident ? cd.n_resident - 1 : 0;
+        } else {
+            timings->n_lines = batch.n_lines;
+        }
         timings->n_segments = n;
     }
     return FORMA_STATUS_OK;
@@ -478,7 +496,7 @@ int Renderer::render(Composition& comp, uint8_t* buffer, bool buffer_on_device, 
                           band_copies_enabled();
     const bool pack_written = cache && !buffer_on_device;
     st = run_frame(
-        comp, S, FrameSpec{cache, pack_written}, timings,
+        &comp, S, FrameSpec{cache, pack_written}, timings,
         [&](const uint32_t* heavy_lists, uint32_t* paint_launches) {
             return paint(S, fb, buffer, stride, in_bands, heavy_lists, paint_launches);
         },
@@ -526,7 +544,7 @@ int Renderer::render_ids(Composition& comp, uint8_t* rgba, uint64_t rgba_stride,
         id_out = id_frame.ptr;
     }
     return run_frame(
-        comp, S, FrameSpec{}, timings,
+        &comp, S, FrameSpec{}, timings,
         [&](const uint32_t* heavy_lists, uint32_t* paint_launches) {
             FORMA_CUDA_TRY(id_flags.reserve(std::max<size_t>(recs.capacity, 1)));
             if (rgba) {
@@ -554,22 +572,8 @@ int Renderer::render_ids(Composition& comp, uint8_t* rgba, uint64_t rgba_stride,
 int Renderer::render_views(Composition& comp, const float* views, uint32_t n, uint8_t* buffer, bool buffer_on_device, uint64_t width,
                            uint64_t stride, uint64_t height, uint64_t view_stride, const uint32_t channels[4], const float clear[4],
                            forma_timings* timings) {
-    if (!buffer || !views || width == 0 || height == 0 || width * 4 > stride || width > FORMA_MAX_WIDTH || height > FORMA_MAX_HEIGHT) {
-        set_error("invalid render target %llux%llu stride %llu", (unsigned long long)width, (unsigned long long)height,
-                  (unsigned long long)stride);
-        return FORMA_STATUS_INVALID;
-    }
-    const uint32_t rows = (uint32_t)((height + 15u) / 16u);
-    if (n == 0 || n > max_views(height)) {
-        set_error("%u views of height %llu: between 1 and %u views of this height fit in one call", n, (unsigned long long)height,
-                  max_views(height));
-        return FORMA_STATUS_INVALID;
-    }
-    if (view_stride < (height - 1u) * stride + 4u * width) {
-        set_error("view stride %llu is smaller than one view (%llu bytes)", (unsigned long long)view_stride,
-                  (unsigned long long)((height - 1u) * stride + 4u * width));
-        return FORMA_STATUS_INVALID;
-    }
+    int st = check_stack("view", n, width, stride, height, view_stride, views ? buffer : nullptr);
+    if (st) return st;
     for (uint32_t b = 0; b < n; ++b) {  // [ux, vx, uy, vy, tx, ty], as forma_layer_set_transform checks them
         const float* v = views + 6u * b;
         bool finite = true;
@@ -579,43 +583,217 @@ int Renderer::render_views(Composition& comp, const float* views, uint32_t n, ui
             return FORMA_STATUS_INVALID;
         }
     }
-    // Views whose rows are whole tile rows, laid out as the stacked frame's rows, are painted in place.
-    const bool direct = buffer_on_device && height % 16u == 0u && view_stride == height * stride;
-    const uint64_t fb_stride = direct ? stride : 4u * width;
+    FrameStack K{buffer, buffer_on_device, width, stride, height, view_stride, n};
     PaintScene S{};
-    int st = begin_frame(S, buffer, width, fb_stride, (uint64_t)n * rows * 16u, channels, clear, nullptr);
+    st = begin_stack(K, S, channels, clear);
     if (st) return st;
-    uint8_t* fb = buffer;
-    if (!direct) {
-        FORMA_CUDA_TRY(framebuffer.reserve((size_t)fb_stride * S.height));
-        fb = framebuffer.ptr;
-    }
     return run_frame(
-        comp, S, FrameSpec{nullptr, false, views, n, (uint32_t)height}, timings,
+        &comp, S, FrameSpec{nullptr, false, views, n, (uint32_t)height}, timings,
         [&](const uint32_t* heavy_lists, uint32_t* paint_launches) {
-            return paint(S, fb, fb, fb_stride, false, heavy_lists, paint_launches, rows);
+            return paint(S, K.fb, K.fb, K.fb_stride, false, heavy_lists, paint_launches, K.rows);
         },
-        [&] {
-            if (buffer_on_device && !direct) {
-                launch_repack_views(fb, fb_stride, rows * 16u, buffer, stride, view_stride, S.width, (uint32_t)height, n, stream);
-                ++launches;
-                FORMA_CUDA_TRY(cudaGetLastError());
-            } else if (!buffer_on_device) {
-                // Rows [0, height) of every view, one copy per view with the pitches copy_to_host uses
-                // for a single frame (a copy over all views would have a view as its pitch, which can
-                // exceed the device's largest pitch).
-                for (uint32_t b = 0; b < n; ++b) {
-                    uint8_t* dst = buffer + (size_t)b * view_stride;
-                    const uint8_t* src = fb + (size_t)b * rows * 16u * fb_stride;
-                    if (stride == fb_stride)
-                        FORMA_CUDA_TRY(cudaMemcpyAsync(dst, src, (height - 1u) * stride + 4u * width, cudaMemcpyDeviceToHost, stream));
-                    else
-                        FORMA_CUDA_TRY(cudaMemcpy2DAsync(dst, stride, src, fb_stride, 4u * width, height, cudaMemcpyDeviceToHost, stream));
-                }
-                d2h_bytes += (uint64_t)n * height * width * 4u;
-            }
-            return FORMA_STATUS_OK;
-        });
+        [&] { return output_stack(K, S); });
+}
+
+// n compositions, one frame each, in one pass: the stacked frame of render_views, but frame c's
+// line setup reads comps[c]'s segment buffer and moves its segments' layers to the composition's
+// slice of the layer field (bind_batch), so that the batch tables serve every frame. No layer
+// cache and no band filter: every composition is resident.
+int Renderer::render_batch(Composition* const* comps, uint32_t n, uint8_t* buffer, bool buffer_on_device, uint64_t width,
+                           uint64_t stride, uint64_t height, uint64_t frame_stride, const uint32_t channels[4], const float clear[4],
+                           forma_timings* timings) {
+    int st = check_stack("frame", n, width, stride, height, frame_stride, comps ? buffer : nullptr);
+    if (st) return st;
+    // The distinct compositions in order of first appearance, and the slices of the layer field
+    // they need: n_orders each, as rebuild_tables counts them.
+    batch_distinct.clear();
+    batch_slot.resize(n);
+    std::unordered_map<const Composition*, uint32_t> index;
+    uint64_t order_sum = 0;
+    for (uint32_t c = 0; c < n; ++c) {
+        if (!comps[c]) {
+            set_error("batch entry %u is null", c);
+            return FORMA_STATUS_INVALID;
+        }
+        auto it = index.emplace(comps[c], (uint32_t)batch_distinct.size()).first;
+        batch_slot[c] = it->second;
+        if (it->second < batch_distinct.size()) continue;
+        batch_distinct.push_back(comps[c]);
+        const auto& layers = comps[c]->layers;
+        order_sum += layers.empty() ? 0u : (uint64_t)layers.rbegin()->first + 1u;
+    }
+    if (order_sum > (1ull << 21)) {
+        set_error("the batch's compositions need %llu layer orders; the layer field holds %u",
+                  (unsigned long long)order_sum, 1u << 21);
+        return FORMA_STATUS_ORDER;
+    }
+    FrameStack K{buffer, buffer_on_device, width, stride, height, frame_stride, n};
+    PaintScene S{};
+    st = begin_stack(K, S, channels, clear);
+    if (st) return st;
+    return run_frame(
+        nullptr, S, FrameSpec{nullptr, false, nullptr, n, (uint32_t)height, comps}, timings,
+        [&](const uint32_t* heavy_lists, uint32_t* paint_launches) {
+            return paint(S, K.fb, K.fb, K.fb_stride, false, heavy_lists, paint_launches, K.rows);
+        },
+        [&] { return output_stack(K, S); });
+}
+
+// Every distinct composition of the batch (batch_distinct, as render_batch found them) is uploaded
+// (tables, then all of its geometry), in the order of first appearance, and gets its slices:
+// orders from order_base, style slots, stops and texels from their bases, each the sum of the
+// counts of the compositions before it. The batch tables are gathered from the compositions'
+// device tables when their list of (serial, version) changed; the per-frame line-setup records
+// are uploaded every call (the segment buffers move as they grow).
+int Renderer::bind_batch(Composition* const* comps, uint32_t n, PaintScene& S, uint32_t height, BatchLines& lines) {
+    const uint32_t nd = (uint32_t)batch_distinct.size();
+    FORMA_CUDA_TRY(h_batch_src.reserve(nd));
+    batch_key_next.clear();
+    uint64_t orders = 0, styles = 0, stops = 0, texels = 0, max_items = 0;
+    bool in_order = options().sort_full_key == 0;
+    for (uint32_t k = 0; k < nd; ++k) {
+        Composition& comp = *batch_distinct[k];
+        int st = upload_tables(comp, -1);
+        if (st) return st;
+        st = flush_geometry(comp, 0.0f, (float)height, false);
+        if (st) return st;
+        const CompDevice& cd = comp.on(res_key);
+        const uint64_t n_texels = comp.n_texels / 4u;
+        h_batch_src.ptr[k] = BatchTableSrc{cd.d_order_to_style.ptr, cd.d_styles.ptr, cd.d_grads.ptr, cd.d_stops.ptr, cd.d_texels.ptr,
+                                           comp.n_orders, (uint32_t)comp.n_style_recs, (uint32_t)comp.n_stops, (uint32_t)n_texels,
+                                           (uint32_t)orders, (uint32_t)styles, (uint32_t)stops, (uint32_t)texels};
+        max_items = std::max<uint64_t>({max_items, comp.n_orders, comp.n_style_recs, comp.n_stops, n_texels});
+        orders += comp.n_orders;
+        styles += comp.n_style_recs;
+        stops += comp.n_stops;
+        texels += n_texels;
+        in_order = in_order && comp.layers_in_order;
+        batch_key_next.emplace_back(comp.serial, comp.tables_version);
+    }
+    if (stops > 0xFFFFFFFFu || texels > 0xFFFFFFFFu || styles > 0x7FFFFFFFu) {
+        set_error("the batch's %llu gradient stops / %llu texels / %llu styles exceed the 32-bit indices of its tables",
+                  (unsigned long long)stops, (unsigned long long)texels, (unsigned long long)styles);
+        return FORMA_STATUS_CAPACITY;
+    }
+    if (batch_key_next != batch_key) {
+        batch_key.clear();  // (until the gather below is queued)
+        FORMA_CUDA_TRY(batch_order_to_style.reserve(orders + 1));
+        FORMA_CUDA_TRY(batch_styles.reserve(styles + 1));
+        FORMA_CUDA_TRY(batch_grads.reserve(styles + 1));
+        FORMA_CUDA_TRY(batch_stops.reserve(stops + 1));
+        FORMA_CUDA_TRY(batch_texels.reserve(4u * texels + 4u));
+        FORMA_CUDA_TRY(d_batch_src.reserve(nd));
+        FORMA_CUDA_TRY(cudaMemcpyAsync(d_batch_src.ptr, h_batch_src.ptr, nd * sizeof(BatchTableSrc), cudaMemcpyHostToDevice, stream));
+        h2d_bytes += nd * sizeof(BatchTableSrc);
+        launch_batch_tables(d_batch_src.ptr, nd, (uint32_t)max_items, batch_order_to_style.ptr, batch_styles.ptr, batch_grads.ptr,
+                            batch_stops.ptr, batch_texels.ptr, stream);
+        launches += max_items ? 1 : 0;
+        FORMA_CUDA_TRY(cudaGetLastError());
+        batch_key.swap(batch_key_next);
+    }
+    S.styles = batch_styles.ptr;
+    S.order_to_style = batch_order_to_style.ptr;
+    S.n_orders = (uint32_t)orders;
+    S.stops = batch_stops.ptr;
+    S.grads = batch_grads.ptr;
+    S.texels = batch_texels.ptr;
+
+    // Line setup: one record per frame, then the frames' first CTAs.
+    const size_t frames_bytes = (size_t)n * sizeof(BatchFrame), bytes = frames_bytes + (n + 1u) * sizeof(uint32_t);
+    FORMA_CUDA_TRY(h_batch_lines.reserve(bytes));
+    FORMA_CUDA_TRY(d_batch_lines.reserve(bytes));
+    BatchFrame* frames = reinterpret_cast<BatchFrame*>(h_batch_lines.ptr);
+    uint32_t* cta_first = reinterpret_cast<uint32_t*>(h_batch_lines.ptr + frames_bytes);
+    uint64_t ctas = 0, n_lines = 0;
+    for (uint32_t c = 0; c < n; ++c) {
+        const Composition& comp = *comps[c];
+        const CompDevice& cd = *comp.devices.at(res_key);
+        frames[c] = BatchFrame{cd.d_x.ptr, cd.d_y.ptr, cd.d_gid.ptr, cd.d_geom_slot.ptr, comp.layers_have_xf ? cd.d_layers.ptr : nullptr,
+                               cd.d_layer_bits.ptr, cd.n_resident, comp.n_geoms, h_batch_src.ptr[batch_slot[c]].order_base, 0u};
+        cta_first[c] = (uint32_t)std::min<uint64_t>(ctas, 0xFFFFFFFFu);
+        ctas += raster_num_blocks(cd.n_resident);
+        n_lines += cd.n_resident ? cd.n_resident - 1u : 0u;
+    }
+    if (ctas >= (1ull << 31)) {  // the launch's largest grid
+        set_error("the batch's %llu line-setup CTAs exceed the largest grid", (unsigned long long)ctas);
+        return FORMA_STATUS_CAPACITY;
+    }
+    cta_first[n] = (uint32_t)ctas;
+    FORMA_CUDA_TRY(cudaMemcpyAsync(d_batch_lines.ptr, h_batch_lines.ptr, bytes, cudaMemcpyHostToDevice, stream));
+    h2d_bytes += bytes;
+    lines.args = BatchArgs{reinterpret_cast<const BatchFrame*>(d_batch_lines.ptr),
+                           reinterpret_cast<const uint32_t*>(d_batch_lines.ptr + frames_bytes), n, (height + 15u) / 16u,
+                           (float)S.width, (float)height};
+    lines.n_ctas = (uint32_t)ctas;
+    // Layer digits can be skipped when every composition emits its segments in layer order: a
+    // painted tile holds one frame's segments, in emission order (stacked row 0 mixes frames, and
+    // no painted tile reads it).
+    lines.layer_bound = in_order ? 0u : (orders ? orders - 1u : 0u);
+    lines.n_lines = n_lines;
+    return FORMA_STATUS_OK;
+}
+
+// The checks of a stack of n frames of width x height pixels, frame_stride bytes apart.
+int Renderer::check_stack(const char* what, uint32_t n, uint64_t width, uint64_t stride, uint64_t height, uint64_t frame_stride,
+                          const uint8_t* buffer) {
+    if (!buffer || width == 0 || height == 0 || width * 4 > stride || width > FORMA_MAX_WIDTH || height > FORMA_MAX_HEIGHT) {
+        set_error("invalid render target %llux%llu stride %llu", (unsigned long long)width, (unsigned long long)height,
+                  (unsigned long long)stride);
+        return FORMA_STATUS_INVALID;
+    }
+    if (n == 0 || n > max_views(height)) {
+        set_error("%u %ss of height %llu: between 1 and %u %ss of this height fit in one call", n, what, (unsigned long long)height,
+                  max_views(height), what);
+        return FORMA_STATUS_INVALID;
+    }
+    if (frame_stride < (height - 1u) * stride + 4u * width) {
+        set_error("%s stride %llu is smaller than one %s (%llu bytes)", what, (unsigned long long)frame_stride, what,
+                  (unsigned long long)((height - 1u) * stride + 4u * width));
+        return FORMA_STATUS_INVALID;
+    }
+    return FORMA_STATUS_OK;
+}
+
+// The stacked frame's PaintScene and device frame. Frames whose rows are whole tile rows, laid out
+// as the stacked frame's rows, are painted in place.
+int Renderer::begin_stack(FrameStack& K, PaintScene& S, const uint32_t channels[4], const float clear[4]) {
+    K.rows = (uint32_t)((K.height + 15u) / 16u);
+    K.direct = K.on_device && K.height % 16u == 0u && K.frame_stride == K.height * K.stride;
+    K.fb_stride = K.direct ? K.stride : 4u * K.width;
+    const int st = begin_frame(S, K.buffer, K.width, K.fb_stride, (uint64_t)K.n * K.rows * 16u, channels, clear, nullptr);
+    if (st) return st;
+    K.fb = K.buffer;
+    if (!K.direct) {
+        FORMA_CUDA_TRY(framebuffer.reserve((size_t)K.fb_stride * S.height));
+        K.fb = framebuffer.ptr;
+    }
+    return FORMA_STATUS_OK;
+}
+
+// Moves the frames of a stack painted into K.fb to the caller's buffer: nothing to do in place,
+// repack_views_kernel into another device layout, or one copy per frame to a host buffer.
+int Renderer::output_stack(const FrameStack& K, const PaintScene& S) {
+    if (K.on_device && !K.direct) {
+        launch_repack_views(K.fb, K.fb_stride, K.rows * 16u, K.buffer, K.stride, K.frame_stride, S.width, (uint32_t)K.height, K.n,
+                            stream);
+        ++launches;
+        FORMA_CUDA_TRY(cudaGetLastError());
+    } else if (!K.on_device) {
+        // Rows [0, height) of every frame, one copy per frame with the pitches copy_to_host uses
+        // for a single frame (a copy over all frames would have a frame as its pitch, which can
+        // exceed the device's largest pitch).
+        for (uint32_t b = 0; b < K.n; ++b) {
+            uint8_t* dst = K.buffer + (size_t)b * K.frame_stride;
+            const uint8_t* src = K.fb + (size_t)b * K.rows * 16u * K.fb_stride;
+            if (K.stride == K.fb_stride)
+                FORMA_CUDA_TRY(cudaMemcpyAsync(dst, src, (K.height - 1u) * K.stride + 4u * K.width, cudaMemcpyDeviceToHost, stream));
+            else
+                FORMA_CUDA_TRY(
+                    cudaMemcpy2DAsync(dst, K.stride, src, K.fb_stride, 4u * K.width, K.height, cudaMemcpyDeviceToHost, stream));
+        }
+        d2h_bytes += (uint64_t)K.n * K.height * K.width * 4u;
+    }
+    return FORMA_STATUS_OK;
 }
 
 // LinearLayout::new asserts (layout/mod.rs:188-193) + consts.rs limits, and the frame's PaintScene

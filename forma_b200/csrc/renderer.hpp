@@ -41,8 +41,31 @@ struct Timer {
 struct FrameSpec {
     LayerCache* cache = nullptr;
     bool pack_written = false;     // only the tiles the frame writes travel back (scatter_written_tiles)
-    const float* views = nullptr;  // render_views: n_views transforms, views of view_height rows; nullptr: one frame
-    uint32_t n_views = 0, view_height = 0;
+    const float* views = nullptr;  // render_views: n_frames transforms of the composition
+    uint32_t n_frames = 0, frame_height = 0;  // stacked frames (views or a batch) of frame_height rows; 0: one frame
+    Composition* const* batch = nullptr;      // render_batch: n_frames compositions, one per frame
+};
+
+// A stack of n frames of width x height pixels (views, batches) in `buffer`: frame b at
+// b * frame_stride, row r of it at + r * stride. The device frame stacks them by tile rows
+// (rows = ceil(height / 16) each) in `fb`, rows fb_stride bytes apart: `buffer` itself when the
+// layouts agree (direct), the renderer's framebuffer otherwise.
+struct FrameStack {
+    uint8_t* buffer;
+    bool on_device;
+    uint64_t width, stride, height, frame_stride;
+    uint32_t n, rows;
+    bool direct;
+    uint8_t* fb;
+    uint64_t fb_stride;
+};
+
+// The line setup of a batch (see Renderer::bind_batch).
+struct BatchLines {
+    BatchArgs args;
+    uint32_t n_ctas;
+    uint64_t layer_bound;  // the sort plan's bound of the layer field
+    uint64_t n_lines;      // point pairs of all frames (forma_timings)
 };
 
 class Renderer {
@@ -217,13 +240,15 @@ class Renderer {
     int flush_geometry(Composition& comp, float band_lo = 0.0f, float band_hi = 0.0f, bool band_is_partial = false);
     int upload_tables(Composition& comp, int64_t cache_id);
     int upload_tables_device(Composition& comp, CompDevice& cd);
-    // views / n_views: the line setup of render_views (a stacked frame of n_views views).
-    int rasterize(Composition& comp, uint32_t width, uint32_t height, float band_lo, float band_hi, uint32_t* n_out,
-                  const ViewArgs* views = nullptr, uint32_t n_views = 0);
+    // views / n_views: the line setup of render_views (a stacked frame of n_views views); batch:
+    // that of render_batch (comp is then null).
+    int rasterize(Composition* comp, uint32_t width, uint32_t height, float band_lo, float band_hi, uint32_t* n_out,
+                  const ViewArgs* views = nullptr, uint32_t n_views = 0, const BatchLines* batch = nullptr);
     // Every frame kind runs through run_frame (renderer.cu, its only instantiations): FrameSpec says
     // what differs before painting, paint_step and output_step what differs after the tables.
+    // comp is null for a batch (spec.batch).
     template <class Paint, class Output>
-    int run_frame(Composition& comp, PaintScene& S, const FrameSpec& spec, forma_timings* timings, Paint&& paint_step,
+    int run_frame(Composition* comp, PaintScene& S, const FrameSpec& spec, forma_timings* timings, Paint&& paint_step,
                   Output&& output_step);
     int render(Composition& comp, uint8_t* buffer, bool buffer_on_device, uint64_t width, uint64_t stride,
                uint64_t height, const uint32_t channels[4], const float clear[4], const forma_rect* crop,
@@ -243,6 +268,32 @@ class Renderer {
     int render_views(Composition& comp, const float* views, uint32_t n, uint8_t* buffer, bool buffer_on_device, uint64_t width,
                      uint64_t stride, uint64_t height, uint64_t view_stride, const uint32_t channels[4], const float clear[4],
                      forma_timings* timings);
+    // A batch of n compositions, one frame each, in one pass (see forma_renderer_render_batch_device):
+    // the stacked frame of the views, every frame with its own composition. The distinct
+    // compositions' tables are gathered into the batch tables below, which are kept until a batch
+    // of other compositions or other table versions comes (batch_key).
+    std::vector<std::pair<uint64_t, uint64_t>> batch_key;  // (Composition::serial, tables_version) of the distinct compositions
+    std::vector<std::pair<uint64_t, uint64_t>> batch_key_next;
+    std::vector<Composition*> batch_distinct;  // of the current call, in order of first appearance (render_batch)
+    std::vector<uint32_t> batch_slot;          // per frame: its composition's index in batch_distinct
+    PinnedBuffer<uint8_t> h_batch_lines;  // BatchFrame per frame, then cta_first
+    DeviceBuffer<uint8_t> d_batch_lines;
+    PinnedBuffer<BatchTableSrc> h_batch_src;
+    DeviceBuffer<BatchTableSrc> d_batch_src;
+    DeviceBuffer<int32_t> batch_order_to_style;
+    DeviceBuffer<StyleRec> batch_styles;
+    DeviceBuffer<GradRec> batch_grads;
+    DeviceBuffer<StopRec> batch_stops;
+    DeviceBuffer<uint16_t> batch_texels;
+    int render_batch(Composition* const* comps, uint32_t n, uint8_t* buffer, bool buffer_on_device, uint64_t width, uint64_t stride,
+                     uint64_t height, uint64_t frame_stride, const uint32_t channels[4], const float clear[4], forma_timings* timings);
+    int bind_batch(Composition* const* comps, uint32_t n, PaintScene& S, uint32_t height, BatchLines& lines);
+    // Stacked frames (views, batches): the checks of the target and the stack, then its PaintScene
+    // and device frame, and the output step that moves the frames to where the caller wants them.
+    int check_stack(const char* what, uint32_t n, uint64_t width, uint64_t stride, uint64_t height, uint64_t frame_stride,
+                    const uint8_t* buffer);
+    int begin_stack(FrameStack& K, PaintScene& S, const uint32_t channels[4], const float clear[4]);
+    int output_stack(const FrameStack& K, const PaintScene& S);
     // The stages of a frame, in the order they run: begin_frame in the entry points, the rest in run_frame.
     int begin_frame(PaintScene& S, const uint8_t* buffer, uint64_t width, uint64_t stride, uint64_t height,
                     const uint32_t channels[4], const float clear[4], const forma_rect* crop);

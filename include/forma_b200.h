@@ -271,7 +271,8 @@ int forma_renderer_render_device_with_ids(forma_renderer*, forma_composition*, u
  * rows, view b's rows after view b - 1's), and forma_renderer_lines returns no records.
  * render_views_device writes a device buffer on the renderer's device (a [n, H, W, 4] uint8
  * tensor's data_ptr() with width_stride = 4 W, view_stride = 4 W H); render_views a host buffer. */
-uint32_t forma_renderer_max_views(uint64_t height); /* floor(2046 / ceil(height / 16)); 0 when height is 0 or too tall */
+uint32_t forma_renderer_max_views(uint64_t height); /* floor(2046 / ceil(height / 16)); 0 when height is 0 or too tall;
+                                                       also the most frames of one render_batch call */
 int forma_renderer_render_views_device(forma_renderer*, forma_composition*, const float* views, uint32_t n,
                                        uint8_t* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
                                        uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
@@ -280,6 +281,38 @@ int forma_renderer_render_views(forma_renderer*, forma_composition*, const float
                                 uint8_t* host_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
                                 uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
                                 forma_timings* timings /* nullable */);
+
+/* Batches (no reference counterpart): `n` frames of `n` compositions from one pass through the
+ * stages, frame c showing comps[c] alone. The layout is that of the views: all frames share
+ * width x height, width_stride, channels and clear colour; frame c starts at c * frame_stride
+ * bytes, frame_stride >= (height - 1) * width_stride + 4 * width, and only the frames'
+ * width x height pixels are written. Frame c is the bytes forma_renderer_render_device makes of
+ * comps[c] without crop or cache (frames whose lines all lie more than 2^19 px left of the frame
+ * excepted, as for the views). A composition may appear more than once; every occurrence is a
+ * frame of its own.
+ * Layer orders: the distinct compositions, in order of first appearance, get consecutive slices
+ * of the 21-bit layer field. Composition k's slice starts at base_k, the sum of n_orders (its
+ * largest attached order + 1, or 0 without layers) of the distinct compositions before it, and
+ * its segments carry base_k + order. The sum over all distinct compositions must not exceed
+ * 2^21: otherwise FORMA_ERR_ORDER_LIMIT. Null comps or a null entry, n outside
+ * 1 ... forma_renderer_max_views(height), a short frame_stride, or an invalid target or channel
+ * return FORMA_ERR_INVALID_ARGUMENT. All of these are refused before anything is written.
+ * FORMA_ERR_CAPACITY: more gradient stops or texels than the tables' 32-bit indices hold, or 2^30
+ * pixel segments or more in all frames together.
+ * Every composition is made resident whole (no band filter). No layer cache is taken and every
+ * cache is left as it was. Afterwards counters, segments, stage times and row costs describe the
+ * stacked frame (n * ceil(height / 16) tile rows), and forma_renderer_lines returns no records.
+ * The renderer keeps the gathered tables of the last batch and gathers them again only when the
+ * list of compositions or one of their tables changed.
+ * render_batch_device writes a device buffer on the renderer's device (a [n, H, W, 4] uint8
+ * tensor's data_ptr() with width_stride = 4 W, frame_stride = 4 W H); render_batch a host buffer. */
+int forma_renderer_render_batch_device(forma_renderer*, forma_composition* const* comps, uint32_t n,
+                                       uint8_t* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                       uint64_t frame_stride, const uint32_t channels[4], const float clear_color[4],
+                                       forma_timings* timings /* nullable */);
+int forma_renderer_render_batch(forma_renderer*, forma_composition* const* comps, uint32_t n, uint8_t* host_buffer,
+                                uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride,
+                                const uint32_t channels[4], const float clear_color[4], forma_timings* timings /* nullable */);
 
 /* Launch on `cuda_stream` (a cudaStream_t, e.g. torch.cuda.current_stream().cuda_stream)
  * instead of the default stream. */
