@@ -290,6 +290,14 @@ SIGNATURES = {
                                         _fp, C.POINTER(_CTimings)]),
     "renderer_render_batch_device": (C.c_int, [_vp, C.POINTER(_vp), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
                                                _u32p, _fp, C.POINTER(_CTimings)]),
+    "renderer_render_views_ids": (C.c_int, [_vp, _vp, _fp, C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, _f,
+                                            C.POINTER(_CTimings)]),
+    "renderer_render_views_ids_device": (C.c_int, [_vp, _vp, _fp, C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
+                                                   _u32p, _fp, _vp, C.c_uint64, C.c_uint64, _f, C.POINTER(_CTimings)]),
+    "renderer_render_batch_ids": (C.c_int, [_vp, C.POINTER(_vp), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, _f,
+                                            C.POINTER(_CTimings)]),
+    "renderer_render_batch_ids_device": (C.c_int, [_vp, C.POINTER(_vp), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64,
+                                                   C.c_uint64, _u32p, _fp, _vp, C.c_uint64, C.c_uint64, _f, C.POINTER(_CTimings)]),
     "renderer_launch_count": (C.c_uint64, [_vp]),
     "renderer_stage_times": (None, [_vp, C.POINTER(C.c_double)]),
     "renderer_counters": (None, [_vp, _u64p]),
@@ -327,6 +335,9 @@ ID_FRAME_SYMBOLS = ("renderer_render_ids", "renderer_render_ids_device", "render
 VIEW_SYMBOLS = ("renderer_max_views", "renderer_render_views", "renderer_render_views_device")
 # The same for batches (Renderer.render_batch).
 BATCH_SYMBOLS = ("renderer_render_batch", "renderer_render_batch_device")
+# The same for the ID frames of views and batches (Renderer.render_views_ids, render_batch_ids).
+STACK_ID_SYMBOLS = ("renderer_render_views_ids", "renderer_render_views_ids_device", "renderer_render_batch_ids",
+                    "renderer_render_batch_ids_device")
 
 
 class Api:
@@ -338,7 +349,8 @@ class Api:
             try:
                 fn = getattr(lib, prefix + name)
             except AttributeError:
-                if name in optional or name in ID_FRAME_SYMBOLS or name in VIEW_SYMBOLS or name in BATCH_SYMBOLS:
+                if (name in optional or name in ID_FRAME_SYMBOLS or name in VIEW_SYMBOLS or name in BATCH_SYMBOLS
+                        or name in STACK_ID_SYMBOLS):
                     continue
                 raise
             fn.restype, fn.argtypes = res, args
@@ -890,6 +902,109 @@ class Renderer:
         frame_stride = height * stride if frame_stride is None else frame_stride
         return self._batch(self._api.renderer_render_batch_device, "Renderer::render_batch_device", comps, int(device_ptr), width,
                            height, channels, clear_color, stride, frame_stride, timings)
+
+    def _stack_ids(self, fn, what, first_args, n, ids_ptr, host, rgba_ptr, width, height, channels, clear_color, stride, frame_stride,
+                   ids_stride, ids_frame_stride, min_coverage, timings):
+        """Calls `fn` (an ID entry point of views or batches) on chunks of at most max_views(height)
+        frames, as _views / _batch chunk: first_args(first, count) gives the chunk's leading
+        arguments (views or handles, count). host: a host entry point (IDs only); a device one
+        takes rgba_ptr, None or the device pointer of the RGBA frames."""
+        ids_stride = width * 4 if ids_stride is None else ids_stride
+        ids_frame_stride = height * ids_stride if ids_frame_stride is None else ids_frame_stride
+        stride = width * 4 if stride is None else stride
+        frame_stride = height * stride if frame_stride is None else frame_stride
+        ch, cc, _ = self._common(channels, clear_color, None)
+        chunk = max(self.max_views(height), 1)
+        t = None
+        for first in range(0, max(n, 1), chunk):
+            count = min(chunk, n - first)
+            t = _CTimings() if timings else None
+            tp = C.byref(t) if t is not None else None
+            ids = C.c_void_p(ids_ptr + first * ids_frame_stride)
+            if host:
+                st = fn(self._h, *first_args(first, count), ids, width, ids_stride, height, ids_frame_stride, float(min_coverage), tp)
+            else:
+                rgba = C.c_void_p(rgba_ptr + first * frame_stride) if rgba_ptr is not None else None
+                st = fn(self._h, *first_args(first, count), rgba, width, stride, height, frame_stride, ch, cc, ids, ids_stride,
+                        ids_frame_stride, float(min_coverage), tp)
+            self._api.check(st, what)
+        return self._timings(t)
+
+    @staticmethod
+    def _view_args(composition, views):
+        v = np.ascontiguousarray(np.asarray(views, dtype=np.float32).reshape(-1, 6))
+        keep = []  # the chunk handed to the library stays alive until the next one
+
+        def args(first, count):
+            keep[:] = [np.ascontiguousarray(v[first:first + count])]
+            return composition._h, keep[0].ctypes.data_as(_fp), count
+        return len(v), args
+
+    @staticmethod
+    def _batch_args(comps):
+        comps = list(comps)
+
+        def args(first, count):
+            part = comps[first:first + count]
+            return (_vp * max(len(part), 1))(*[c._h for c in part]), count
+        return len(comps), args
+
+    def render_views_ids(self, composition: Composition, views, ids: np.ndarray, width: int, height: int,
+                         ids_stride: Optional[int] = None, ids_view_stride: Optional[int] = None, min_coverage: float = 0.0,
+                         timings: bool = True) -> Optional[Timings]:
+        """The ID frame (see render_ids) of every view of render_views, in one pass. ID frame b
+        starts at byte b * ids_view_stride (default height * ids_stride) of `ids`, a writable
+        contiguous uint32 host array; `ids_stride` (default 4 * width) is the row stride in bytes.
+        Chunked like render_views."""
+        n, args = self._view_args(composition, views)
+        s = width * 4 if ids_stride is None else ids_stride
+        fs = height * s if ids_view_stride is None else ids_view_stride
+        assert ids.dtype == np.uint32 and ids.flags["C_CONTIGUOUS"]
+        assert n == 0 or ids.size * 4 >= (n - 1) * fs + (height - 1) * s + 4 * width
+        return self._stack_ids(self._api.renderer_render_views_ids, "Renderer::render_views_ids", args, n, ids.ctypes.data, True,
+                               None, width, height, RGBA, Color(), None, None, ids_stride, ids_view_stride, min_coverage, timings)
+
+    def render_views_ids_device(self, composition: Composition, views, ids_device_ptr: int, width: int, height: int,
+                                rgba_ptr: Optional[int] = None, channels=RGBA, clear_color: Color = Color(1.0, 1.0, 1.0, 1.0),
+                                stride: Optional[int] = None, view_stride: Optional[int] = None, ids_stride: Optional[int] = None,
+                                ids_view_stride: Optional[int] = None, min_coverage: float = 0.0,
+                                timings: bool = True) -> Optional[Timings]:
+        """render_views_ids into device memory: with the defaults, the data_ptr() of a contiguous
+        [N, height, width] int32 / uint32 CUDA tensor. With `rgba_ptr` (a [N, height, width, 4]
+        uint8 tensor's data_ptr() with the default strides) the frames of render_views_device are
+        written as well, from the same pass; rgba_ptr=None renders the IDs only."""
+        n, args = self._view_args(composition, views)
+        return self._stack_ids(self._api.renderer_render_views_ids_device, "Renderer::render_views_ids_device", args, n,
+                               int(ids_device_ptr), False, None if rgba_ptr is None else int(rgba_ptr), width, height, channels, clear_color,
+                               stride, view_stride, ids_stride, ids_view_stride, min_coverage, timings)
+
+    def render_batch_ids(self, comps, ids: np.ndarray, width: int, height: int, ids_stride: Optional[int] = None,
+                         ids_frame_stride: Optional[int] = None, min_coverage: float = 0.0,
+                         timings: bool = True) -> Optional[Timings]:
+        """The ID frame (see render_ids) of every frame of render_batch, in one pass: frame c holds
+        comps[c]'s own layer orders (or ID_NONE). Layout as for render_views_ids; chunked like
+        render_batch."""
+        n, args = self._batch_args(comps)
+        s = width * 4 if ids_stride is None else ids_stride
+        fs = height * s if ids_frame_stride is None else ids_frame_stride
+        assert ids.dtype == np.uint32 and ids.flags["C_CONTIGUOUS"]
+        assert n == 0 or ids.size * 4 >= (n - 1) * fs + (height - 1) * s + 4 * width
+        return self._stack_ids(self._api.renderer_render_batch_ids, "Renderer::render_batch_ids", args, n, ids.ctypes.data, True,
+                               None, width, height, RGBA, Color(), None, None, ids_stride, ids_frame_stride, min_coverage, timings)
+
+    def render_batch_ids_device(self, comps, ids_device_ptr: int, width: int, height: int, rgba_ptr: Optional[int] = None,
+                                channels=RGBA, clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
+                                frame_stride: Optional[int] = None, ids_stride: Optional[int] = None,
+                                ids_frame_stride: Optional[int] = None, min_coverage: float = 0.0,
+                                timings: bool = True) -> Optional[Timings]:
+        """render_batch_ids into device memory (a contiguous [N, height, width] int32 / uint32 CUDA
+        tensor's data_ptr() with the defaults): the labels of a batch of scenes. With `rgba_ptr`
+        the frames of render_batch_device are written as well, from the same pass; rgba_ptr=None
+        renders the IDs only."""
+        n, args = self._batch_args(comps)
+        return self._stack_ids(self._api.renderer_render_batch_ids_device, "Renderer::render_batch_ids_device", args, n,
+                               int(ids_device_ptr), False, None if rgba_ptr is None else int(rgba_ptr), width, height, channels, clear_color,
+                               stride, frame_stride, ids_stride, ids_frame_stride, min_coverage, timings)
 
     def launch_count(self) -> int:
         return int(self._api.renderer_launch_count(self._h))

@@ -429,12 +429,12 @@ int forma_renderer_render_views_device(forma_renderer* r, forma_composition* c, 
 // The Compositions behind the handles (null entries stay null for Renderer::render_batch to refuse).
 static int render_batch(forma_renderer* r, forma_composition* const* comps, uint32_t n, uint8_t* buffer, bool on_device,
                         uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride, const uint32_t channels[4],
-                        const float clear_color[4], forma_timings* timings) {
+                        const float clear_color[4], forma_timings* timings, const IdStack* ids = nullptr) {
     return guarded((int)FORMA_ERR_CAPACITY, [&] {
         std::vector<Composition*> cs(comps ? n : 0u);
         for (size_t k = 0; k < cs.size(); ++k) cs[k] = comps[k] ? &comps[k]->c : nullptr;
         return r->r.render_batch(comps ? cs.data() : nullptr, n, buffer, on_device, width, width_stride, height, frame_stride, channels,
-                                 clear_color, timings);
+                                 clear_color, timings, ids);
     });
 }
 int forma_renderer_render_batch_device(forma_renderer* r, forma_composition* const* comps, uint32_t n, uint8_t* device_buffer,
@@ -454,6 +454,50 @@ int forma_renderer_render_views(forma_renderer* r, forma_composition* c, const f
         return r->r.render_views(c->c, views, n, host_buffer, false, width, width_stride, height, view_stride, channels, clear_color,
                                  timings);
     });
+}
+// ID frames of views and batches. A call without ID frames at all is refused here: the Renderer
+// would take it for the RGBA call.
+static int no_id_frames(const char* fn) {
+    set_error("%s: no ID buffer", fn);
+    return FORMA_STATUS_INVALID;
+}
+int forma_renderer_render_views_ids_device(forma_renderer* r, forma_composition* c, const float* views, uint32_t n,
+                                           uint8_t* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                           uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
+                                           uint32_t* device_ids, uint64_t ids_stride, uint64_t ids_view_stride, float min_coverage,
+                                           forma_timings* timings) {
+    return guarded((int)FORMA_ERR_CAPACITY, [&] {
+        if (!device_ids) return no_id_frames("forma_renderer_render_views_ids_device");
+        const IdStack ids{device_ids, true, ids_stride, ids_view_stride, min_coverage};
+        return r->r.render_views(c->c, views, n, device_buffer, true, width, width_stride, height, view_stride, channels, clear_color,
+                                 timings, &ids);
+    });
+}
+int forma_renderer_render_views_ids(forma_renderer* r, forma_composition* c, const float* views, uint32_t n, uint32_t* host_ids,
+                                    uint64_t width, uint64_t ids_stride, uint64_t height, uint64_t ids_view_stride,
+                                    float min_coverage, forma_timings* timings) {
+    return guarded((int)FORMA_ERR_CAPACITY, [&] {
+        if (!host_ids) return no_id_frames("forma_renderer_render_views_ids");
+        const IdStack ids{host_ids, false, ids_stride, ids_view_stride, min_coverage};
+        return r->r.render_views(c->c, views, n, nullptr, false, width, 0, height, 0, nullptr, nullptr, timings, &ids);
+    });
+}
+int forma_renderer_render_batch_ids_device(forma_renderer* r, forma_composition* const* comps, uint32_t n, uint8_t* device_buffer,
+                                           uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride,
+                                           const uint32_t channels[4], const float clear_color[4], uint32_t* device_ids,
+                                           uint64_t ids_stride, uint64_t ids_frame_stride, float min_coverage,
+                                           forma_timings* timings) {
+    if (!device_ids) return no_id_frames("forma_renderer_render_batch_ids_device");
+    const IdStack ids{device_ids, true, ids_stride, ids_frame_stride, min_coverage};
+    return render_batch(r, comps, n, device_buffer, true, width, width_stride, height, frame_stride, channels, clear_color, timings,
+                        &ids);
+}
+int forma_renderer_render_batch_ids(forma_renderer* r, forma_composition* const* comps, uint32_t n, uint32_t* host_ids, uint64_t width,
+                                    uint64_t ids_stride, uint64_t height, uint64_t ids_frame_stride, float min_coverage,
+                                    forma_timings* timings) {
+    if (!host_ids) return no_id_frames("forma_renderer_render_batch_ids");
+    const IdStack ids{host_ids, false, ids_stride, ids_frame_stride, min_coverage};
+    return render_batch(r, comps, n, nullptr, false, width, 0, height, 0, nullptr, nullptr, timings, &ids);
 }
 // --- shared frames (multi-GPU, see include/forma_b200.h) -----------------------
 static_assert(sizeof(cudaIpcMemHandle_t) == sizeof(forma_ipc_handle), "CUDA IPC handles are 64 bytes");

@@ -277,9 +277,13 @@ void launch_repack_views(const uint8_t* src, uint64_t src_stride, uint32_t view_
 // order of the top-most Draw layer whose coverage x clip mask exceeds min_coverage, or
 // FORMA_ID_NONE. Reads the tables like launch_paint (never `eflags`); id_flags: one byte per
 // entry of scratch. ids_stride in bytes.
+// frames != nullptr: S stacks the frames of a batch, `rows` tile rows each, whose entries carry
+// frames[c].order_base + order (BatchArgs); every ID stored is the frame's own order
+// (paint_ids_stacked_kernel). The stacked views of one composition need neither.
 void launch_paint_ids(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range,
                       const uint32_t* heavy, const uint32_t* heavy_count, uint8_t* id_flags, uint32_t* ids, size_t ids_stride,
-                      float min_coverage, uint32_t* tile_counter, cudaStream_t st);
+                      float min_coverage, uint32_t* tile_counter, cudaStream_t st, uint32_t rows = 0,
+                      const BatchFrame* frames = nullptr);
 // The painter tables of a batch: the device tables of its distinct compositions, concatenated.
 // Composition k's orders land at order_base + order (the slots they name shifted by style_base,
 // -1 kept), its StyleRecs at style_base with stop_first + stop_base and tex_first + texel_base;

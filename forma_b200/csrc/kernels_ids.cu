@@ -19,6 +19,12 @@
 // in place, and the combined call runs this kernel after it): skip_trivial_clips runs again
 // from flags0 into `id_flags`, and the walk starts at the same top-most full opaque layer
 // as the painter (a clipped layer above it whose clip lies below it is never painted).
+//
+// Stacked frames: a tile row belongs to one frame and the walk never looks at another tile, so
+// the views of one composition need nothing else. The frames of a batch carry base + order in
+// their entries (BatchFrame::order_base), and the walk compares layers and clip ranges in that
+// shifted space; paint_ids_stacked_kernel, the same body, takes the frame's base off every ID it
+// stores (one look-up per tile).
 #include <mutex>
 
 #include "../../include/forma_b200.h"
@@ -147,199 +153,57 @@ __device__ __forceinline__ void skip_trivial_clips_ids(const EntryRec* __restric
     if (has_clip && !clip_used) out[clip_i] |= (uint8_t)kFlagMaskedOut;
 }
 
+// The lane's eight IDs of a batch frame's tile (base + order) as the frame's own orders.
+__device__ __forceinline__ void rebase_ids(uint32_t* out, uint32_t base) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+        if (out[j] != FORMA_ID_NONE) out[j] -= base;
+}
+
 __global__ void __launch_bounds__(kIdWarpsPerBlock * 32) paint_ids_kernel(PaintScene S, IdInputs in, uint32_t n_tiles) {
-    __shared__ __align__(16) IdWarpSmem s_warp[kIdWarpsPerBlock];
-    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
-    IdWarpSmem& W = s_warp[warp];
-    const uint32_t ntx = S.tx_hi - S.tx_lo;
-    const uint32_t row = lane >> 1, hx = lane & 1u;
-    const bool vec_ok = ((reinterpret_cast<uintptr_t>(in.ids) | (uintptr_t)in.ids_stride) & 15u) == 0u;
-    const float min_cov = in.min_coverage;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) W.cells[k * 32 + lane] = 0u;
-    __syncwarp();
+#define FORMA_IDS_REBASE(out, ty)
+#include "paint_ids_body.cuh"
+#undef FORMA_IDS_REBASE
+}
+// S stacks the frames of a batch, `rows` tile rows each; frame c's entries carry
+// frames[c].order_base + order, and the IDs stored are the frame's own orders.
+__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) paint_ids_stacked_kernel(PaintScene S, IdInputs in, uint32_t n_tiles,
+                                                                                  uint32_t rows, const BatchFrame* __restrict__ frames) {
+#define FORMA_IDS_REBASE(out, ty) rebase_ids(out, frames[(ty) / rows].order_base)
+#include "paint_ids_body.cuh"
+#undef FORMA_IDS_REBASE
+}
 
-    uint32_t hcount[kHeavyClasses], H = 0;
-#pragma unroll
-    for (int c = 0; c < kHeavyClasses; ++c) {
-        hcount[c] = in.heavy ? in.heavy_count[c] : 0u;
-        H += hcount[c];
+// CTAs of `kernel` that fill the device (one occupancy query per device and kernel).
+template <class Kernel>
+static uint32_t id_grid_limit(Kernel kernel, int (&blocks_per_sm)[kMaxDevices]) {
+    static std::mutex config_mu;
+    std::lock_guard<std::mutex> lk(config_mu);
+    int& slot = blocks_per_sm[current_device_index()];
+    if (!slot) {
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&slot, kernel, kIdWarpsPerBlock * 32, 0);
+        if (slot < 1) slot = 1;
     }
-    const uint32_t n_tickets = H + n_tiles;
-    for (;;) {
-        // Ticket -> tile, as in paint_kernel: tickets [0, H) walk the heavy lists (largest class
-        // first), the rest the tile rectangle row-major, skipping the listed tiles.
-        uint32_t ticket = 0;
-        if (lane == 0) ticket = atomicAdd(in.tile_counter, 1u);
-        ticket = __shfl_sync(kFullMask, ticket, 0);
-        if (ticket >= n_tickets) break;
-        uint32_t tid;
-        if (ticket < H) {
-            uint32_t t = ticket;
-            int c = kHeavyClasses - 1;
-#pragma unroll
-            for (int q = kHeavyClasses - 1; q > 0; --q)
-                if (c == q && t >= hcount[q]) {
-                    t -= hcount[q];
-                    c = q - 1;
-                }
-            tid = in.heavy[(size_t)c * in.n_tiles_total + t];
-            const uint32_t ty = tid / S.tiles_x, tx = tid - ty * S.tiles_x;
-            if (ty < S.ty_lo || ty >= S.ty_hi || tx < S.tx_lo || tx >= S.tx_hi) continue;
-        } else {
-            const uint32_t lin = ticket - H;
-            tid = (S.ty_lo + lin / ntx) * S.tiles_x + S.tx_lo + lin % ntx;
-        }
-        const uint2 range = in.tile_range[tid];
-        const uint32_t b = range.x, e = range.y;
-        if (ticket >= H && in.heavy && e - b >= kHeavyMin) continue;  // done from its list
-        const uint32_t ty = tid / S.tiles_x, tx = tid - ty * S.tiles_x;
-
-        bool clip_tile = false;
-        for (uint32_t p0 = b; p0 < e && !clip_tile; p0 += 32u) {
-            const uint32_t p = p0 + lane;
-            clip_tile = __any_sync(kFullMask, p < e && (in.recs[p].flags0 & kFlagClipish) != 0u);
-        }
-
-        uint32_t* out = W.ids + 8u * lane;  // this lane's eight pixels
-#pragma unroll
-        for (int j = 0; j < 8; ++j) out[j] = FORMA_ID_NONE;
-        float cov[8];
-        if (!clip_tile) {
-            uint32_t open = 0xFFu;  // this lane's pixels without a hit yet
-            bool done = e == b;
-            for (uint32_t hi = e; hi > b && !done;) {
-                const uint32_t lo = hi - b >= 32u ? hi - 32u : b;
-                stage_group(W, in, lo, hi - lo, false, lane);
-                for (uint32_t k = hi - lo; k-- > 0u;) {
-                    const EntryRec& h = W.hdr[k];
-                    const uint32_t flags = h.pad;
-                    if (flags & kFlagMaskedOut) continue;
-                    if (flags & kFlagFull) {  // an unclipped Draw entry of coverage 1 everywhere
-#pragma unroll
-                        for (int j = 0; j < 8; ++j)
-                            if ((open >> j) & 1u) out[j] = h.layer;
-                        done = true;
-                        break;
-                    }
-                    entry_coverage(W, h, in.segs, lane, cov);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j)
-                        if (((open >> j) & 1u) && cov[j] > min_cov) {
-                            out[j] = h.layer;
-                            open &= ~(1u << j);
-                        }
-                    if (__all_sync(kFullMask, open == 0u)) {
-                        done = true;
-                        break;
-                    }
-                }
-                hi = lo;
-            }
-        } else {
-            if (lane == 0) skip_trivial_clips_ids(in.recs, in.id_flags, b, e);
-            __syncwarp();
-            // The painter's first layer (skip_fully_covered_layers): the top-most visible full,
-            // unclipped, opaque entry.
-            uint32_t first = b;
-            for (uint32_t hi = e; hi > b;) {
-                const uint32_t lo = hi - b >= 32u ? hi - 32u : b;
-                bool cand = false;
-                if (lo + lane < hi) {
-                    const uint32_t f = in.id_flags[lo + lane];
-                    const bool clipped = (f & kFlagClippedDraw) && !(f & kFlagSkipClip);
-                    cand = !(f & kFlagMaskedOut) && !clipped && (f & kFlagFull) && (f & kFlagOpaque);
-                }
-                const uint32_t m = __ballot_sync(kFullMask, cand);
-                if (m) {
-                    first = lo + 31u - (uint32_t)__clz((int)m);
-                    break;
-                }
-                hi = lo;
-            }
-            bool clip_active = false;
-            uint32_t clip_last = 0;
-            for (uint32_t p0 = first; p0 < e; p0 += 32u) {
-                const uint32_t cnt = min(32u, e - p0);
-                stage_group(W, in, p0, cnt, true, lane);
-                for (uint32_t k = 0; k < cnt; ++k) {
-                    const EntryRec& h = W.hdr[k];
-                    const uint32_t flags = h.pad;
-                    if (flags & kFlagMaskedOut) continue;
-                    const uint32_t layer = h.layer, meta = h.meta;
-                    if (clip_active && clip_last < layer) clip_active = false;  // mod.rs:302-306
-                    const bool is_clip = ((meta >> 1) & 1u) != 0u;
-                    const bool apply_clip = !is_clip && ((meta >> 2) & 1u) && !(flags & kFlagSkipClip);
-                    if (!is_clip && !apply_clip && (flags & kFlagFull)) {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) out[j] = layer;
-                        continue;
-                    }
-                    if (apply_clip && !clip_active) continue;  // mod.rs:317-323
-                    entry_coverage(W, h, in.segs, lane, cov);
-                    if (is_clip) {  // clip_at, mod.rs:449-464
-                        if (!clip_active) {
-                            clip_active = true;
-                            clip_last = layer + h.clip_layers;
-                        }
-                        float4* m4 = reinterpret_cast<float4*>(W.clip);
-                        m4[2u * lane] = make_float4(cov[0], cov[1], cov[2], cov[3]);
-                        m4[2u * lane + 1u] = make_float4(cov[4], cov[5], cov[6], cov[7]);
-                        __syncwarp();
-                        continue;
-                    }
-                    if (apply_clip) {
-                        const float4* m4 = reinterpret_cast<const float4*>(W.clip);
-                        const float4 m0 = m4[2u * lane], m1 = m4[2u * lane + 1u];
-                        const float m[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) cov[j] = __fmul_rn(cov[j], m[j]);
-                    }
-#pragma unroll
-                    for (int j = 0; j < 8; ++j)
-                        if (cov[j] > min_cov) out[j] = layer;
-                }
-            }
-        }
-
-        const uint32_t py = ty * 16u + row, x0 = tx * 16u + hx * 8u;
-        if (py < S.height && x0 < S.width) {
-            uint32_t* rowp = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(in.ids) + (size_t)py * in.ids_stride) + x0;
-            if (vec_ok && x0 + 8u <= S.width) {
-                reinterpret_cast<uint4*>(rowp)[0] = reinterpret_cast<const uint4*>(out)[0];
-                reinterpret_cast<uint4*>(rowp)[1] = reinterpret_cast<const uint4*>(out)[1];
-            } else {
-#pragma unroll
-                for (int j = 0; j < 8; ++j)
-                    if (x0 + (uint32_t)j < S.width) rowp[j] = out[j];
-            }
-        }
-    }
+    return (uint32_t)(slot * device_sm_count());
 }
 
 void launch_paint_ids(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range,
                       const uint32_t* heavy, const uint32_t* heavy_count, uint8_t* id_flags, uint32_t* ids, size_t ids_stride,
-                      float min_coverage, uint32_t* tile_counter, cudaStream_t st) {
+                      float min_coverage, uint32_t* tile_counter, cudaStream_t st, uint32_t rows, const BatchFrame* frames) {
     if (S.tx_hi <= S.tx_lo || S.ty_hi <= S.ty_lo) return;
     const uint32_t n_tiles = (S.tx_hi - S.tx_lo) * (S.ty_hi - S.ty_lo);
     cudaMemsetAsync(tile_counter, 0, sizeof(uint32_t), st);
     IdInputs in{segs, recs, tile_range, heavy, heavy_count, S.tiles_x * S.tiles_y, id_flags, ids, ids_stride, min_coverage,
                 tile_counter};
-    static int blocks_per_sm[kMaxDevices] = {0};
-    static std::mutex config_mu;
-    int per_sm = 0;
-    {
-        std::lock_guard<std::mutex> lk(config_mu);
-        int& slot = blocks_per_sm[current_device_index()];
-        if (!slot) {
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&slot, paint_ids_kernel, kIdWarpsPerBlock * 32, 0);
-            if (slot < 1) slot = 1;
-        }
-        per_sm = slot;
-    }
-    const uint32_t want = (uint32_t)(per_sm * device_sm_count());
+    static int blocks_per_sm[2][kMaxDevices] = {{0}};
     const uint32_t need = (n_tiles + kIdWarpsPerBlock - 1) / kIdWarpsPerBlock;
-    paint_ids_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles);
+    if (frames) {
+        const uint32_t want = id_grid_limit(paint_ids_stacked_kernel, blocks_per_sm[1]);
+        paint_ids_stacked_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles, rows, frames);
+    } else {
+        const uint32_t want = id_grid_limit(paint_ids_kernel, blocks_per_sm[0]);
+        paint_ids_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles);
+    }
 }
 
 }  // namespace forma

@@ -571,8 +571,8 @@ int Renderer::render_ids(Composition& comp, uint8_t* rgba, uint64_t rgba_stride,
 // composition is resident.
 int Renderer::render_views(Composition& comp, const float* views, uint32_t n, uint8_t* buffer, bool buffer_on_device, uint64_t width,
                            uint64_t stride, uint64_t height, uint64_t view_stride, const uint32_t channels[4], const float clear[4],
-                           forma_timings* timings) {
-    int st = check_stack("view", n, width, stride, height, view_stride, views ? buffer : nullptr);
+                           forma_timings* timings, const IdStack* ids) {
+    const int st = check_stacks("view", views != nullptr, n, width, height, buffer, stride, view_stride, ids);
     if (st) return st;
     for (uint32_t b = 0; b < n; ++b) {  // [ux, vx, uy, vy, tx, ty], as forma_layer_set_transform checks them
         const float* v = views + 6u * b;
@@ -584,15 +584,7 @@ int Renderer::render_views(Composition& comp, const float* views, uint32_t n, ui
         }
     }
     FrameStack K{buffer, buffer_on_device, width, stride, height, view_stride, n};
-    PaintScene S{};
-    st = begin_stack(K, S, channels, clear);
-    if (st) return st;
-    return run_frame(
-        &comp, S, FrameSpec{nullptr, false, views, n, (uint32_t)height}, timings,
-        [&](const uint32_t* heavy_lists, uint32_t* paint_launches) {
-            return paint(S, K.fb, K.fb, K.fb_stride, false, heavy_lists, paint_launches, K.rows);
-        },
-        [&] { return output_stack(K, S); });
+    return run_stack(&comp, FrameSpec{nullptr, false, views, n, (uint32_t)height}, K, ids, channels, clear, timings);
 }
 
 // n compositions, one frame each, in one pass: the stacked frame of render_views, but frame c's
@@ -601,8 +593,8 @@ int Renderer::render_views(Composition& comp, const float* views, uint32_t n, ui
 // cache and no band filter: every composition is resident.
 int Renderer::render_batch(Composition* const* comps, uint32_t n, uint8_t* buffer, bool buffer_on_device, uint64_t width,
                            uint64_t stride, uint64_t height, uint64_t frame_stride, const uint32_t channels[4], const float clear[4],
-                           forma_timings* timings) {
-    int st = check_stack("frame", n, width, stride, height, frame_stride, comps ? buffer : nullptr);
+                           forma_timings* timings, const IdStack* ids) {
+    const int st = check_stacks("frame", comps != nullptr, n, width, height, buffer, stride, frame_stride, ids);
     if (st) return st;
     // The distinct compositions in order of first appearance, and the slices of the layer field
     // they need: n_orders each, as rebuild_tables counts them.
@@ -628,15 +620,7 @@ int Renderer::render_batch(Composition* const* comps, uint32_t n, uint8_t* buffe
         return FORMA_STATUS_ORDER;
     }
     FrameStack K{buffer, buffer_on_device, width, stride, height, frame_stride, n};
-    PaintScene S{};
-    st = begin_stack(K, S, channels, clear);
-    if (st) return st;
-    return run_frame(
-        nullptr, S, FrameSpec{nullptr, false, nullptr, n, (uint32_t)height, comps}, timings,
-        [&](const uint32_t* heavy_lists, uint32_t* paint_launches) {
-            return paint(S, K.fb, K.fb, K.fb_stride, false, heavy_lists, paint_launches, K.rows);
-        },
-        [&] { return output_stack(K, S); });
+    return run_stack(nullptr, FrameSpec{nullptr, false, nullptr, n, (uint32_t)height, comps}, K, ids, channels, clear, timings);
 }
 
 // Every distinct composition of the batch (batch_distinct, as render_batch found them) is uploaded
@@ -754,20 +738,84 @@ int Renderer::check_stack(const char* what, uint32_t n, uint64_t width, uint64_t
     return FORMA_STATUS_OK;
 }
 
-// The stacked frame's PaintScene and device frame. Frames whose rows are whole tile rows, laid out
-// as the stacked frame's rows, are painted in place.
-int Renderer::begin_stack(FrameStack& K, PaintScene& S, const uint32_t channels[4], const float clear[4]) {
-    K.rows = (uint32_t)((K.height + 15u) / 16u);
-    K.direct = K.on_device && K.height % 16u == 0u && K.frame_stride == K.height * K.stride;
-    K.fb_stride = K.direct ? K.stride : 4u * K.width;
-    const int st = begin_frame(S, K.buffer, K.width, K.fb_stride, (uint64_t)K.n * K.rows * 16u, channels, clear, nullptr);
+// The checks of a stacked call's targets: the RGBA stack (absent when there is an ID stack and no
+// buffer), then the ID stack. args: the call's views / compositions are there.
+int Renderer::check_stacks(const char* what, bool args, uint32_t n, uint64_t width, uint64_t height, const uint8_t* buffer,
+                           uint64_t stride, uint64_t frame_stride, const IdStack* ids) {
+    if (buffer || !ids) {
+        const int st = check_stack(what, n, width, stride, height, frame_stride, args ? buffer : nullptr);
+        if (st) return st;
+    }
+    if (!ids) return FORMA_STATUS_OK;
+    if (ids->stride % 4u != 0u || ids->frame_stride % 4u != 0u || !std::isfinite(ids->min_coverage) || ids->min_coverage < 0.0f ||
+        ids->min_coverage >= 1.0f) {
+        set_error("invalid ID frames: stride %llu, %s stride %llu (multiples of 4 bytes), min_coverage %g (finite, in [0, 1))",
+                  (unsigned long long)ids->stride, what, (unsigned long long)ids->frame_stride, (double)ids->min_coverage);
+        return FORMA_STATUS_INVALID;
+    }
+    return check_stack(what, n, width, ids->stride, height, ids->frame_stride, args ? reinterpret_cast<const uint8_t*>(ids->ids) : nullptr);
+}
+
+// The stacked frame's PaintScene (that of the RGBA stack K, or of the ID stack I when there is no
+// K) and the device frame of each stack. Frames whose rows are whole tile rows, laid out as the
+// stacked frame's rows, are painted in place; each stack decides for itself.
+int Renderer::begin_stack(FrameStack* K, FrameStack* I, PaintScene& S, const uint32_t channels[4], const float clear[4]) {
+    static const uint32_t kIdChannels[4] = {0, 1, 2, 3};
+    static const float kIdClear[4] = {0, 0, 0, 0};
+    for (FrameStack* k : {K, I}) {
+        if (!k) continue;
+        k->rows = (uint32_t)((k->height + 15u) / 16u);
+        k->direct = k->on_device && k->height % 16u == 0u && k->frame_stride == k->height * k->stride;
+        k->fb_stride = k->direct ? k->stride : 4u * k->width;
+        k->fb = k->buffer;
+    }
+    const FrameStack& M = K ? *K : *I;
+    const int st = begin_frame(S, M.buffer, M.width, M.fb_stride, (uint64_t)M.n * M.rows * 16u, K ? channels : kIdChannels,
+                               K ? clear : kIdClear, nullptr);
     if (st) return st;
-    K.fb = K.buffer;
-    if (!K.direct) {
-        FORMA_CUDA_TRY(framebuffer.reserve((size_t)K.fb_stride * S.height));
-        K.fb = framebuffer.ptr;
+    if (K && !K->direct) {
+        FORMA_CUDA_TRY(framebuffer.reserve((size_t)K->fb_stride * S.height));
+        K->fb = framebuffer.ptr;
+    }
+    if (I && !I->direct) {
+        FORMA_CUDA_TRY(id_frame.reserve((size_t)(I->fb_stride / 4u) * S.height));
+        I->fb = reinterpret_cast<uint8_t*>(id_frame.ptr);
     }
     return FORMA_STATUS_OK;
+}
+
+// A stacked frame through run_frame: the RGBA stack K (K.buffer null: none), the ID stack `ids`
+// (null: none), or both from one set of tables, the paint kernel and then the ID kernel. The
+// sync-free redo repeats the kernels and the output of both stacks.
+int Renderer::run_stack(Composition* comp, const FrameSpec& spec, FrameStack& K, const IdStack* ids, const uint32_t channels[4],
+                        const float clear[4], forma_timings* timings) {
+    const bool rgba = K.buffer != nullptr;
+    FrameStack I{};
+    if (ids) I = FrameStack{reinterpret_cast<uint8_t*>(ids->ids), ids->on_device, K.width, ids->stride, K.height, ids->frame_stride, K.n};
+    PaintScene S{};
+    const int st = begin_stack(rgba ? &K : nullptr, ids ? &I : nullptr, S, channels, clear);
+    if (st) return st;
+    return run_frame(
+        comp, S, spec, timings,
+        [&](const uint32_t* heavy_lists, uint32_t* paint_launches) {
+            if (rgba) {
+                const int st = paint(S, K.fb, K.fb, K.fb_stride, false, heavy_lists, paint_launches, K.rows);
+                if (st || !ids) return st;
+                ++*paint_launches;
+            }
+            // A batch's entries carry each frame's order base (bind_batch): the kernel takes it off.
+            FORMA_CUDA_TRY(id_flags.reserve(std::max<size_t>(recs.capacity, 1)));
+            launch_paint_ids(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), id_flags.ptr,
+                             reinterpret_cast<uint32_t*>(I.fb), I.fb_stride, ids->min_coverage, totals.ptr + 8, stream, I.rows,
+                             spec.batch ? reinterpret_cast<const BatchFrame*>(d_batch_lines.ptr) : nullptr);
+            ++launches;
+            FORMA_CUDA_TRY(cudaGetLastError());
+            return (int)FORMA_STATUS_OK;
+        },
+        [&] {
+            const int st = rgba ? output_stack(K, S) : FORMA_STATUS_OK;
+            return st || !ids ? st : output_stack(I, S);
+        });
 }
 
 // Moves the frames of a stack painted into K.fb to the caller's buffer: nothing to do in place,

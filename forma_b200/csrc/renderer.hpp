@@ -60,6 +60,15 @@ struct FrameStack {
     uint64_t fb_stride;
 };
 
+// The ID frames of a stacked call (render_views / render_batch): frame b's words at
+// b * frame_stride bytes of `ids`, rows `stride` bytes apart.
+struct IdStack {
+    uint32_t* ids;
+    bool on_device;
+    uint64_t stride, frame_stride;
+    float min_coverage;
+};
+
 // The line setup of a batch (see Renderer::bind_batch).
 struct BatchLines {
     BatchArgs args;
@@ -262,12 +271,14 @@ class Renderer {
                    const forma_rect* crop, float min_coverage, forma_timings* timings);
     // n views of one composition in one pass (see forma_renderer_render_views_device): a frame of
     // n * ceil(height / 16) tile rows, painted straight into a device buffer whose views are its
-    // rows, or into `framebuffer` and copied out view by view.
+    // rows, or into `framebuffer` and copied out view by view. With `ids`, the views' ID frames
+    // from the same tables (forma_renderer_render_views_ids_device); `buffer` may then be null
+    // (no RGBA frames; stride, view_stride, channels and clear are not read).
     PinnedBuffer<float> h_views;
     DeviceBuffer<float> d_views;
     int render_views(Composition& comp, const float* views, uint32_t n, uint8_t* buffer, bool buffer_on_device, uint64_t width,
                      uint64_t stride, uint64_t height, uint64_t view_stride, const uint32_t channels[4], const float clear[4],
-                     forma_timings* timings);
+                     forma_timings* timings, const IdStack* ids = nullptr);
     // A batch of n compositions, one frame each, in one pass (see forma_renderer_render_batch_device):
     // the stacked frame of the views, every frame with its own composition. The distinct
     // compositions' tables are gathered into the batch tables below, which are kept until a batch
@@ -285,14 +296,23 @@ class Renderer {
     DeviceBuffer<GradRec> batch_grads;
     DeviceBuffer<StopRec> batch_stops;
     DeviceBuffer<uint16_t> batch_texels;
+    // `ids`: as for render_views; the IDs of frame c are comps[c]'s own orders.
     int render_batch(Composition* const* comps, uint32_t n, uint8_t* buffer, bool buffer_on_device, uint64_t width, uint64_t stride,
-                     uint64_t height, uint64_t frame_stride, const uint32_t channels[4], const float clear[4], forma_timings* timings);
+                     uint64_t height, uint64_t frame_stride, const uint32_t channels[4], const float clear[4], forma_timings* timings,
+                     const IdStack* ids = nullptr);
     int bind_batch(Composition* const* comps, uint32_t n, PaintScene& S, uint32_t height, BatchLines& lines);
-    // Stacked frames (views, batches): the checks of the target and the stack, then its PaintScene
-    // and device frame, and the output step that moves the frames to where the caller wants them.
+    // Stacked frames (views, batches): the checks of the targets (the RGBA stack, the ID stack or
+    // both), then the PaintScene and the device frames, the frame itself (run_stack: run_frame with
+    // the paint and / or ID kernel) and the output step that moves a stack's frames to where the
+    // caller wants them. A stack is 4-byte pixels either way: RGBA8 with `framebuffer` as its
+    // scratch, ID words with `id_frame`.
     int check_stack(const char* what, uint32_t n, uint64_t width, uint64_t stride, uint64_t height, uint64_t frame_stride,
                     const uint8_t* buffer);
-    int begin_stack(FrameStack& K, PaintScene& S, const uint32_t channels[4], const float clear[4]);
+    int check_stacks(const char* what, bool args, uint32_t n, uint64_t width, uint64_t height, const uint8_t* buffer, uint64_t stride,
+                     uint64_t frame_stride, const IdStack* ids);
+    int begin_stack(FrameStack* K, FrameStack* I, PaintScene& S, const uint32_t channels[4], const float clear[4]);
+    int run_stack(Composition* comp, const FrameSpec& spec, FrameStack& K, const IdStack* ids, const uint32_t channels[4],
+                  const float clear[4], forma_timings* timings);
     int output_stack(const FrameStack& K, const PaintScene& S);
     // The stages of a frame, in the order they run: begin_frame in the entry points, the rest in run_frame.
     int begin_frame(PaintScene& S, const uint8_t* buffer, uint64_t width, uint64_t stride, uint64_t height,

@@ -314,6 +314,51 @@ int forma_renderer_render_batch(forma_renderer*, forma_composition* const* comps
                                 uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride,
                                 const uint32_t channels[4], const float clear_color[4], forma_timings* timings /* nullable */);
 
+/* ID frames of views and batches: the ID frame (see forma_renderer_render_ids) of every frame of a
+ * views or batch call, alone or together with the RGBA frames, from one pass through the stages.
+ * The ID stack is laid out like the RGBA stack: ID frame b starts at b * ids_view_stride
+ * (ids_frame_stride) bytes, its rows are ids_stride bytes apart. Both are multiples of 4,
+ * ids_stride >= 4 * width and ids_view_stride >= (height - 1) * ids_stride + 4 * width. Only the
+ * frames' width x height words are written: row padding and the bytes between frames stay.
+ * The _device calls write the ID stack and, when device_buffer is not null, the RGBA stack as
+ * well: one upload, line setup, sort and set of painter tables, then the paint kernel and the ID
+ * kernel. The RGBA bytes are those of forma_renderer_render_views_device /
+ * forma_renderer_render_batch_device with the same arguments. With a null device_buffer,
+ * width_stride, view_stride / frame_stride, channels and clear_color are not read. The host
+ * calls (render_views_ids, render_batch_ids) make ID frames only.
+ * Views: ID frame b holds what forma_renderer_render_ids_device gives, without a crop, for the
+ * composition with every layer's transform replaced by C = V_b ∘ T (the formula above); the
+ * values are layer orders of the composition.
+ * Batches: ID frame c holds what forma_renderer_render_ids_device gives for comps[c] alone: the
+ * values are comps[c]'s own orders, not base_k + order (which slice of the layer field a
+ * composition gets stays inside the call), and FORMA_ID_NONE where no layer hits.
+ * (Frames whose lines all lie more than 2^19 px left of the frame are the exception of views and
+ * batches again: the stacked calls are right, forma_renderer_render_ids_device is not.)
+ * min_coverage must be finite and in [0, 1); 1 <= n <= forma_renderer_max_views(height); the
+ * order-sum, stop / texel and 2^30-segment limits of the RGBA calls apply. Every refusal
+ * (FORMA_ERR_INVALID_ARGUMENT, also for a null ID buffer; FORMA_ERR_ORDER_LIMIT;
+ * FORMA_ERR_CAPACITY) comes before anything is written to either buffer.
+ * No layer cache is taken and every cache is left as it was. Afterwards counters, segments,
+ * stage times and row costs describe the stacked frame; stage time [5] is the paint kernel
+ * followed by the ID kernel, as after forma_renderer_render_device_with_ids.
+ * With the defaults of a [n, H, W] int32 / uint32 tensor: ids_stride = 4 W, ids_view_stride = 4 W H. */
+int forma_renderer_render_views_ids_device(forma_renderer*, forma_composition*, const float* views, uint32_t n,
+                                           uint8_t* device_buffer /* nullable */, uint64_t width, uint64_t width_stride,
+                                           uint64_t height, uint64_t view_stride, const uint32_t channels[4],
+                                           const float clear_color[4], uint32_t* device_ids, uint64_t ids_stride,
+                                           uint64_t ids_view_stride, float min_coverage, forma_timings* timings /* nullable */);
+int forma_renderer_render_views_ids(forma_renderer*, forma_composition*, const float* views, uint32_t n, uint32_t* host_ids,
+                                    uint64_t width, uint64_t ids_stride, uint64_t height, uint64_t ids_view_stride,
+                                    float min_coverage, forma_timings* timings /* nullable */);
+int forma_renderer_render_batch_ids_device(forma_renderer*, forma_composition* const* comps, uint32_t n,
+                                           uint8_t* device_buffer /* nullable */, uint64_t width, uint64_t width_stride,
+                                           uint64_t height, uint64_t frame_stride, const uint32_t channels[4],
+                                           const float clear_color[4], uint32_t* device_ids, uint64_t ids_stride,
+                                           uint64_t ids_frame_stride, float min_coverage, forma_timings* timings /* nullable */);
+int forma_renderer_render_batch_ids(forma_renderer*, forma_composition* const* comps, uint32_t n, uint32_t* host_ids,
+                                    uint64_t width, uint64_t ids_stride, uint64_t height, uint64_t ids_frame_stride,
+                                    float min_coverage, forma_timings* timings /* nullable */);
+
 /* Launch on `cuda_stream` (a cudaStream_t, e.g. torch.cuda.current_stream().cuda_stream)
  * instead of the default stream. */
 void forma_renderer_set_stream(forma_renderer*, void* cuda_stream);
