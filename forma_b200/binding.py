@@ -224,6 +224,10 @@ class Timings:
     n_segments: int
 
 
+def _timings(t: Optional[_CTimings]) -> Optional[Timings]:
+    return Timings(t.line_setup_ms, t.rasterize_ms, t.sort_ms, t.paint_ms, t.n_lines, t.n_segments) if t is not None else None
+
+
 @dataclass
 class Rect:
     """cpu::Rect::new(horizontal, vertical), pixel ranges (cpu/renderer.rs:38-53)."""
@@ -340,6 +344,9 @@ STACK_ID_SYMBOLS = ("renderer_render_views_ids", "renderer_render_views_ids_devi
                     "renderer_render_batch_ids_device")
 
 
+_OPTIONAL_SYMBOLS = frozenset(ID_FRAME_SYMBOLS + VIEW_SYMBOLS + BATCH_SYMBOLS + STACK_ID_SYMBOLS)
+
+
 class Api:
     """Typed access to one shared library exporting `<prefix><name>` symbols."""
 
@@ -349,8 +356,7 @@ class Api:
             try:
                 fn = getattr(lib, prefix + name)
             except AttributeError:
-                if (name in optional or name in ID_FRAME_SYMBOLS or name in VIEW_SYMBOLS or name in BATCH_SYMBOLS
-                        or name in STACK_ID_SYMBOLS):
+                if name in optional or name in _OPTIONAL_SYMBOLS:
                     continue
                 raise
             fn.restype, fn.argtypes = res, args
@@ -735,6 +741,18 @@ class Renderer:
             rect = _CRect(crop.horizontal[0], crop.horizontal[1], crop.vertical[0], crop.vertical[1])
         return ch, cc, rect
 
+    def _frame(self, fn, what, composition, ptr, width, height, stride, colors, crop, tail, timings):
+        """Calls `fn`, a single-frame entry point: fn(renderer, composition, ptr, width, stride, height,
+        [channels, clear colour,] crop, *tail, timings), with channels and clear colour when
+        `colors` = (channels, clear_color) is given."""
+        stride = width * 4 if stride is None else stride
+        ch, cc, rect = self._common(*(colors or (RGBA, Color())), crop)
+        t = _CTimings() if timings else None
+        st = fn(self._h, composition._h, ptr, width, stride, height, *((ch, cc) if colors else ()),
+                C.byref(rect) if rect is not None else None, *tail, C.byref(t) if t is not None else None)
+        self._api.check(st, what)
+        return _timings(t)
+
     def render(self, composition: Composition, buffer: np.ndarray, width: int, height: int,
                channels=RGBA, clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), crop: Optional[Rect] = None,
                layer_cache: Optional[LayerCache] = None, stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
@@ -743,32 +761,15 @@ class Renderer:
         (stage_times() still can, afterwards)."""
         stride = width * 4 if stride is None else stride
         assert buffer.dtype == np.uint8 and buffer.flags["C_CONTIGUOUS"] and buffer.size >= height * stride
-        ch, cc, rect = self._common(channels, clear_color, crop)
-        t = _CTimings() if timings else None
-        st = self._api.renderer_render(
-            self._h, composition._h, buffer.ctypes.data_as(C.c_void_p), width, stride, height, ch, cc,
-            C.byref(rect) if rect is not None else None, layer_cache._h if layer_cache else None,
-            C.byref(t) if t is not None else None)
-        self._api.check(st, "Renderer::render")
-        return Timings(t.line_setup_ms, t.rasterize_ms, t.sort_ms, t.paint_ms, t.n_lines, t.n_segments) if t is not None else None
+        return self._frame(self._api.renderer_render, "Renderer::render", composition, buffer.ctypes.data_as(C.c_void_p), width,
+                           height, stride, (channels, clear_color), crop, (layer_cache._h if layer_cache else None,), timings)
 
     def render_device(self, composition: Composition, device_ptr: int, width: int, height: int,
                       channels=RGBA, clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), crop: Optional[Rect] = None,
                       layer_cache: Optional[LayerCache] = None, stride: Optional[int] = None,
                       timings: bool = True) -> Optional[Timings]:
-        stride = width * 4 if stride is None else stride
-        ch, cc, rect = self._common(channels, clear_color, crop)
-        t = _CTimings() if timings else None
-        st = self._api.renderer_render_device(
-            self._h, composition._h, C.c_void_p(device_ptr), width, stride, height, ch, cc,
-            C.byref(rect) if rect is not None else None, layer_cache._h if layer_cache else None,
-            C.byref(t) if t is not None else None)
-        self._api.check(st, "Renderer::render_device")
-        return Timings(t.line_setup_ms, t.rasterize_ms, t.sort_ms, t.paint_ms, t.n_lines, t.n_segments) if t is not None else None
-
-    @staticmethod
-    def _timings(t):
-        return Timings(t.line_setup_ms, t.rasterize_ms, t.sort_ms, t.paint_ms, t.n_lines, t.n_segments) if t is not None else None
+        return self._frame(self._api.renderer_render_device, "Renderer::render_device", composition, C.c_void_p(device_ptr), width,
+                           height, stride, (channels, clear_color), crop, (layer_cache._h if layer_cache else None,), timings)
 
     def render_ids(self, composition: Composition, ids: np.ndarray, width: int, height: int, crop: Optional[Rect] = None,
                    stride: Optional[int] = None, min_coverage: float = 0.0, timings: bool = True) -> Optional[Timings]:
@@ -778,26 +779,15 @@ class Renderer:
         tile rectangle is written."""
         stride = width * 4 if stride is None else stride
         assert ids.dtype == np.uint32 and ids.flags["C_CONTIGUOUS"] and ids.size * 4 >= height * stride
-        _, _, rect = self._common(RGBA, Color(), crop)
-        t = _CTimings() if timings else None
-        st = self._api.renderer_render_ids(self._h, composition._h, ids.ctypes.data_as(C.c_void_p), width, stride, height,
-                                           C.byref(rect) if rect is not None else None, float(min_coverage),
-                                           C.byref(t) if t is not None else None)
-        self._api.check(st, "Renderer::render_ids")
-        return self._timings(t)
+        return self._frame(self._api.renderer_render_ids, "Renderer::render_ids", composition, ids.ctypes.data_as(C.c_void_p), width,
+                           height, stride, None, crop, (float(min_coverage),), timings)
 
     def render_ids_device(self, composition: Composition, device_ptr: int, width: int, height: int,
                           crop: Optional[Rect] = None, stride: Optional[int] = None, min_coverage: float = 0.0,
                           timings: bool = True) -> Optional[Timings]:
         """render_ids into device memory (e.g. a torch int32 / uint32 tensor's data_ptr())."""
-        stride = width * 4 if stride is None else stride
-        _, _, rect = self._common(RGBA, Color(), crop)
-        t = _CTimings() if timings else None
-        st = self._api.renderer_render_ids_device(self._h, composition._h, C.c_void_p(device_ptr), width, stride, height,
-                                                  C.byref(rect) if rect is not None else None, float(min_coverage),
-                                                  C.byref(t) if t is not None else None)
-        self._api.check(st, "Renderer::render_ids_device")
-        return self._timings(t)
+        return self._frame(self._api.renderer_render_ids_device, "Renderer::render_ids_device", composition, C.c_void_p(device_ptr),
+                           width, height, stride, None, crop, (float(min_coverage),), timings)
 
     def render_device_with_ids(self, composition: Composition, device_ptr: int, ids_device_ptr: int, width: int, height: int,
                                channels=RGBA, clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), crop: Optional[Rect] = None,
@@ -805,130 +795,48 @@ class Renderer:
                                timings: bool = True) -> Optional[Timings]:
         """render_device (without a layer cache) and render_ids_device of the same frame from one
         pass through the stages; both pointers are device memory."""
-        stride = width * 4 if stride is None else stride
         ids_stride = width * 4 if ids_stride is None else ids_stride
-        ch, cc, rect = self._common(channels, clear_color, crop)
-        t = _CTimings() if timings else None
-        st = self._api.renderer_render_device_with_ids(
-            self._h, composition._h, C.c_void_p(device_ptr), width, stride, height, ch, cc,
-            C.byref(rect) if rect is not None else None, C.c_void_p(ids_device_ptr), ids_stride, float(min_coverage),
-            C.byref(t) if t is not None else None)
-        self._api.check(st, "Renderer::render_device_with_ids")
-        return self._timings(t)
+        return self._frame(self._api.renderer_render_device_with_ids, "Renderer::render_device_with_ids", composition,
+                           C.c_void_p(device_ptr), width, height, stride, (channels, clear_color), crop,
+                           (C.c_void_p(ids_device_ptr), ids_stride, float(min_coverage)), timings)
 
     def max_views(self, height: int) -> int:
         """The most views of `height` rows one render_views call of the library takes (0: none)."""
         return int(self._api.renderer_max_views(height))
 
-    def _views(self, fn, what, composition, views, ptr, width, height, channels, clear_color, stride, view_stride, timings):
-        """Calls `fn` on chunks of at most max_views(height) views, view b at ptr + b * view_stride."""
-        v = np.ascontiguousarray(np.asarray(views, dtype=np.float32).reshape(-1, 6))
-        ch, cc, _ = self._common(channels, clear_color, None)
+    def _stack(self, fn, what, first_args, n, width, height, rgba, ids, timings):
+        """Calls `fn`, an entry point of views or batches, on chunks of at most max_views(height)
+        frames: first_args(first, count) gives a chunk's leading arguments (views or handles,
+        count), then come its targets. rgba = (ptr or None, stride, frame_stride, channels,
+        clear_color) and ids = (ptr, stride, frame_stride, min_coverage), either may be None; a
+        stride of None takes its default (4 * width, height * stride). An entry point with both
+        takes the ID target's arguments without width and height."""
         chunk = max(self.max_views(height), 1)
-        t = None
-        for first in range(0, max(len(v), 1), chunk):
-            part = v[first:first + chunk]
-            t = _CTimings() if timings else None
-            st = fn(self._h, composition._h, part.ctypes.data_as(_fp), len(part), C.c_void_p(ptr + first * view_stride), width, stride,
-                    height, view_stride, ch, cc, C.byref(t) if t is not None else None)
-            self._api.check(st, what)
-        return self._timings(t)
-
-    def render_views(self, composition: Composition, views, buffer: np.ndarray, width: int, height: int, channels=RGBA,
-                     clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
-                     view_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
-        """One frame per row of `views`, an (N, 6) array-like of transforms in set_transform order
-        [ux, vx, uy, vy, tx, ty], each a frame of the composition with every layer's transform T
-        replaced by view ∘ T. Frame b starts at byte b * view_stride (default height * stride) of
-        `buffer`, a writable contiguous uint8 host array; `stride` (default 4 * width) is the row
-        stride. N may exceed max_views(height): the views are then rendered in chunks. Returns the
-        timings of the last chunk."""
-        stride = width * 4 if stride is None else stride
-        view_stride = height * stride if view_stride is None else view_stride
-        n = len(np.asarray(views, dtype=np.float32).reshape(-1, 6))
-        assert buffer.dtype == np.uint8 and buffer.flags["C_CONTIGUOUS"]
-        assert n == 0 or buffer.size >= (n - 1) * view_stride + (height - 1) * stride + 4 * width
-        return self._views(self._api.renderer_render_views, "Renderer::render_views", composition, views, buffer.ctypes.data,
-                           width, height, channels, clear_color, stride, view_stride, timings)
-
-    def render_views_device(self, composition: Composition, views, device_ptr: int, width: int, height: int, channels=RGBA,
-                            clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
-                            view_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
-        """render_views into device memory on the renderer's device: with the defaults, the
-        data_ptr() of a contiguous [N, height, width, 4] uint8 CUDA tensor."""
-        stride = width * 4 if stride is None else stride
-        view_stride = height * stride if view_stride is None else view_stride
-        return self._views(self._api.renderer_render_views_device, "Renderer::render_views_device", composition, views,
-                           int(device_ptr), width, height, channels, clear_color, stride, view_stride, timings)
-
-    def _batch(self, fn, what, comps, ptr, width, height, channels, clear_color, stride, frame_stride, timings):
-        """Calls `fn` on chunks of at most max_views(height) compositions, frame c at ptr + c * frame_stride."""
-        comps = list(comps)
-        ch, cc, _ = self._common(channels, clear_color, None)
-        chunk = max(self.max_views(height), 1)
-        t = None
-        for first in range(0, max(len(comps), 1), chunk):
-            part = comps[first:first + chunk]
-            handles = (_vp * max(len(part), 1))(*[c._h for c in part])
-            t = _CTimings() if timings else None
-            st = fn(self._h, handles, len(part), C.c_void_p(ptr + first * frame_stride), width, stride, height, frame_stride, ch, cc,
-                    C.byref(t) if t is not None else None)
-            self._api.check(st, what)
-        return self._timings(t)
-
-    def render_batch(self, comps, buffer: np.ndarray, width: int, height: int, channels=RGBA,
-                     clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
-                     frame_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
-        """One frame per composition of the sequence `comps` (repeats allowed), frame c showing
-        comps[c] alone, from one pass through the stages. Frame c starts at byte c * frame_stride
-        (default height * stride) of `buffer`, a writable contiguous uint8 host array; `stride`
-        (default 4 * width) is the row stride. N may exceed max_views(height): the compositions
-        are then rendered in chunks. A chunk whose distinct compositions need more than 2^21 layer
-        orders raises OrderError. Returns the timings of the last chunk."""
-        comps = list(comps)
-        stride = width * 4 if stride is None else stride
-        frame_stride = height * stride if frame_stride is None else frame_stride
-        assert buffer.dtype == np.uint8 and buffer.flags["C_CONTIGUOUS"]
-        assert not comps or buffer.size >= (len(comps) - 1) * frame_stride + (height - 1) * stride + 4 * width
-        return self._batch(self._api.renderer_render_batch, "Renderer::render_batch", comps, buffer.ctypes.data, width, height,
-                           channels, clear_color, stride, frame_stride, timings)
-
-    def render_batch_device(self, comps, device_ptr: int, width: int, height: int, channels=RGBA,
-                            clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
-                            frame_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
-        """render_batch into device memory on the renderer's device: with the defaults, the
-        data_ptr() of a contiguous [N, height, width, 4] uint8 CUDA tensor."""
-        stride = width * 4 if stride is None else stride
-        frame_stride = height * stride if frame_stride is None else frame_stride
-        return self._batch(self._api.renderer_render_batch_device, "Renderer::render_batch_device", comps, int(device_ptr), width,
-                           height, channels, clear_color, stride, frame_stride, timings)
-
-    def _stack_ids(self, fn, what, first_args, n, ids_ptr, host, rgba_ptr, width, height, channels, clear_color, stride, frame_stride,
-                   ids_stride, ids_frame_stride, min_coverage, timings):
-        """Calls `fn` (an ID entry point of views or batches) on chunks of at most max_views(height)
-        frames, as _views / _batch chunk: first_args(first, count) gives the chunk's leading
-        arguments (views or handles, count). host: a host entry point (IDs only); a device one
-        takes rgba_ptr, None or the device pointer of the RGBA frames."""
-        ids_stride = width * 4 if ids_stride is None else ids_stride
-        ids_frame_stride = height * ids_stride if ids_frame_stride is None else ids_frame_stride
-        stride = width * 4 if stride is None else stride
-        frame_stride = height * stride if frame_stride is None else frame_stride
-        ch, cc, _ = self._common(channels, clear_color, None)
-        chunk = max(self.max_views(height), 1)
+        if rgba is not None:
+            rgba_ptr, stride, frame_stride = rgba[0], *self._strides(width, height, rgba[1], rgba[2])
+            ch, cc, _ = self._common(rgba[3], rgba[4], None)
+        if ids is not None:
+            ids_ptr, ids_stride, ids_frame_stride = ids[0], *self._strides(width, height, ids[1], ids[2])
         t = None
         for first in range(0, max(n, 1), chunk):
-            count = min(chunk, n - first)
+            args = list(first_args(first, min(chunk, n - first)))
+            if rgba is not None:
+                ptr = C.c_void_p(rgba_ptr + first * frame_stride) if rgba_ptr is not None else None
+                args += [ptr, width, stride, height, frame_stride, ch, cc]
+            if ids is not None:
+                ptr = C.c_void_p(ids_ptr + first * ids_frame_stride)
+                layout = [ids_stride, ids_frame_stride] if rgba is not None else [width, ids_stride, height, ids_frame_stride]
+                args += [ptr, *layout, float(ids[3])]
             t = _CTimings() if timings else None
-            tp = C.byref(t) if t is not None else None
-            ids = C.c_void_p(ids_ptr + first * ids_frame_stride)
-            if host:
-                st = fn(self._h, *first_args(first, count), ids, width, ids_stride, height, ids_frame_stride, float(min_coverage), tp)
-            else:
-                rgba = C.c_void_p(rgba_ptr + first * frame_stride) if rgba_ptr is not None else None
-                st = fn(self._h, *first_args(first, count), rgba, width, stride, height, frame_stride, ch, cc, ids, ids_stride,
-                        ids_frame_stride, float(min_coverage), tp)
+            st = fn(self._h, *args, C.byref(t) if t is not None else None)
             self._api.check(st, what)
-        return self._timings(t)
+        return _timings(t)
+
+    @staticmethod
+    def _strides(width, height, stride, frame_stride):
+        """Row and frame strides in bytes, by default 4 * width and height * stride."""
+        stride = width * 4 if stride is None else stride
+        return stride, height * stride if frame_stride is None else frame_stride
 
     @staticmethod
     def _view_args(composition, views):
@@ -949,6 +857,56 @@ class Renderer:
             return (_vp * max(len(part), 1))(*[c._h for c in part]), count
         return len(comps), args
 
+    def render_views(self, composition: Composition, views, buffer: np.ndarray, width: int, height: int, channels=RGBA,
+                     clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
+                     view_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """One frame per row of `views`, an (N, 6) array-like of transforms in set_transform order
+        [ux, vx, uy, vy, tx, ty], each a frame of the composition with every layer's transform T
+        replaced by view ∘ T. Frame b starts at byte b * view_stride (default height * stride) of
+        `buffer`, a writable contiguous uint8 host array; `stride` (default 4 * width) is the row
+        stride. N may exceed max_views(height): the views are then rendered in chunks. Returns the
+        timings of the last chunk."""
+        n, args = self._view_args(composition, views)
+        stride, view_stride = self._strides(width, height, stride, view_stride)
+        assert buffer.dtype == np.uint8 and buffer.flags["C_CONTIGUOUS"]
+        assert n == 0 or buffer.size >= (n - 1) * view_stride + (height - 1) * stride + 4 * width
+        return self._stack(self._api.renderer_render_views, "Renderer::render_views", args, n, width, height,
+                           (buffer.ctypes.data, stride, view_stride, channels, clear_color), None, timings)
+
+    def render_views_device(self, composition: Composition, views, device_ptr: int, width: int, height: int, channels=RGBA,
+                            clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
+                            view_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """render_views into device memory on the renderer's device: with the defaults, the
+        data_ptr() of a contiguous [N, height, width, 4] uint8 CUDA tensor."""
+        n, args = self._view_args(composition, views)
+        return self._stack(self._api.renderer_render_views_device, "Renderer::render_views_device", args, n, width, height,
+                           (int(device_ptr), stride, view_stride, channels, clear_color), None, timings)
+
+    def render_batch(self, comps, buffer: np.ndarray, width: int, height: int, channels=RGBA,
+                     clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
+                     frame_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """One frame per composition of the sequence `comps` (repeats allowed), frame c showing
+        comps[c] alone, from one pass through the stages. Frame c starts at byte c * frame_stride
+        (default height * stride) of `buffer`, a writable contiguous uint8 host array; `stride`
+        (default 4 * width) is the row stride. N may exceed max_views(height): the compositions
+        are then rendered in chunks. A chunk whose distinct compositions need more than 2^21 layer
+        orders raises OrderError. Returns the timings of the last chunk."""
+        n, args = self._batch_args(comps)
+        stride, frame_stride = self._strides(width, height, stride, frame_stride)
+        assert buffer.dtype == np.uint8 and buffer.flags["C_CONTIGUOUS"]
+        assert n == 0 or buffer.size >= (n - 1) * frame_stride + (height - 1) * stride + 4 * width
+        return self._stack(self._api.renderer_render_batch, "Renderer::render_batch", args, n, width, height,
+                           (buffer.ctypes.data, stride, frame_stride, channels, clear_color), None, timings)
+
+    def render_batch_device(self, comps, device_ptr: int, width: int, height: int, channels=RGBA,
+                            clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
+                            frame_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """render_batch into device memory on the renderer's device: with the defaults, the
+        data_ptr() of a contiguous [N, height, width, 4] uint8 CUDA tensor."""
+        n, args = self._batch_args(comps)
+        return self._stack(self._api.renderer_render_batch_device, "Renderer::render_batch_device", args, n, width, height,
+                           (int(device_ptr), stride, frame_stride, channels, clear_color), None, timings)
+
     def render_views_ids(self, composition: Composition, views, ids: np.ndarray, width: int, height: int,
                          ids_stride: Optional[int] = None, ids_view_stride: Optional[int] = None, min_coverage: float = 0.0,
                          timings: bool = True) -> Optional[Timings]:
@@ -957,12 +915,11 @@ class Renderer:
         contiguous uint32 host array; `ids_stride` (default 4 * width) is the row stride in bytes.
         Chunked like render_views."""
         n, args = self._view_args(composition, views)
-        s = width * 4 if ids_stride is None else ids_stride
-        fs = height * s if ids_view_stride is None else ids_view_stride
+        s, fs = self._strides(width, height, ids_stride, ids_view_stride)
         assert ids.dtype == np.uint32 and ids.flags["C_CONTIGUOUS"]
         assert n == 0 or ids.size * 4 >= (n - 1) * fs + (height - 1) * s + 4 * width
-        return self._stack_ids(self._api.renderer_render_views_ids, "Renderer::render_views_ids", args, n, ids.ctypes.data, True,
-                               None, width, height, RGBA, Color(), None, None, ids_stride, ids_view_stride, min_coverage, timings)
+        return self._stack(self._api.renderer_render_views_ids, "Renderer::render_views_ids", args, n, width, height, None,
+                           (ids.ctypes.data, s, fs, min_coverage), timings)
 
     def render_views_ids_device(self, composition: Composition, views, ids_device_ptr: int, width: int, height: int,
                                 rgba_ptr: Optional[int] = None, channels=RGBA, clear_color: Color = Color(1.0, 1.0, 1.0, 1.0),
@@ -974,9 +931,9 @@ class Renderer:
         uint8 tensor's data_ptr() with the default strides) the frames of render_views_device are
         written as well, from the same pass; rgba_ptr=None renders the IDs only."""
         n, args = self._view_args(composition, views)
-        return self._stack_ids(self._api.renderer_render_views_ids_device, "Renderer::render_views_ids_device", args, n,
-                               int(ids_device_ptr), False, None if rgba_ptr is None else int(rgba_ptr), width, height, channels, clear_color,
-                               stride, view_stride, ids_stride, ids_view_stride, min_coverage, timings)
+        return self._stack(self._api.renderer_render_views_ids_device, "Renderer::render_views_ids_device", args, n, width, height,
+                           (None if rgba_ptr is None else int(rgba_ptr), stride, view_stride, channels, clear_color),
+                           (int(ids_device_ptr), ids_stride, ids_view_stride, min_coverage), timings)
 
     def render_batch_ids(self, comps, ids: np.ndarray, width: int, height: int, ids_stride: Optional[int] = None,
                          ids_frame_stride: Optional[int] = None, min_coverage: float = 0.0,
@@ -985,12 +942,11 @@ class Renderer:
         comps[c]'s own layer orders (or ID_NONE). Layout as for render_views_ids; chunked like
         render_batch."""
         n, args = self._batch_args(comps)
-        s = width * 4 if ids_stride is None else ids_stride
-        fs = height * s if ids_frame_stride is None else ids_frame_stride
+        s, fs = self._strides(width, height, ids_stride, ids_frame_stride)
         assert ids.dtype == np.uint32 and ids.flags["C_CONTIGUOUS"]
         assert n == 0 or ids.size * 4 >= (n - 1) * fs + (height - 1) * s + 4 * width
-        return self._stack_ids(self._api.renderer_render_batch_ids, "Renderer::render_batch_ids", args, n, ids.ctypes.data, True,
-                               None, width, height, RGBA, Color(), None, None, ids_stride, ids_frame_stride, min_coverage, timings)
+        return self._stack(self._api.renderer_render_batch_ids, "Renderer::render_batch_ids", args, n, width, height, None,
+                           (ids.ctypes.data, s, fs, min_coverage), timings)
 
     def render_batch_ids_device(self, comps, ids_device_ptr: int, width: int, height: int, rgba_ptr: Optional[int] = None,
                                 channels=RGBA, clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
@@ -1002,9 +958,9 @@ class Renderer:
         the frames of render_batch_device are written as well, from the same pass; rgba_ptr=None
         renders the IDs only."""
         n, args = self._batch_args(comps)
-        return self._stack_ids(self._api.renderer_render_batch_ids_device, "Renderer::render_batch_ids_device", args, n,
-                               int(ids_device_ptr), False, None if rgba_ptr is None else int(rgba_ptr), width, height, channels, clear_color,
-                               stride, frame_stride, ids_stride, ids_frame_stride, min_coverage, timings)
+        return self._stack(self._api.renderer_render_batch_ids_device, "Renderer::render_batch_ids_device", args, n, width, height,
+                           (None if rgba_ptr is None else int(rgba_ptr), stride, frame_stride, channels, clear_color),
+                           (int(ids_device_ptr), ids_stride, ids_frame_stride, min_coverage), timings)
 
     def launch_count(self) -> int:
         return int(self._api.renderer_launch_count(self._h))
@@ -1112,7 +1068,7 @@ class MultiRenderer:
         t = _CTimings()
         st = fn(self._h, composition._h, ptr, width, stride, height, ch, cc, C.byref(rect) if rect is not None else None, C.byref(t))
         self._api.check(st, what)
-        return Timings(t.line_setup_ms, t.rasterize_ms, t.sort_ms, t.paint_ms, t.n_lines, t.n_segments)
+        return _timings(t)
 
     def render(self, composition: "Composition", buffer: np.ndarray, width: int, height: int, channels=RGBA,
                clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), crop: Optional[Rect] = None, stride: Optional[int] = None) -> Timings:

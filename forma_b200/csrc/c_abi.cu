@@ -369,135 +369,135 @@ void forma_layer_cache_clear(forma_layer_cache* c) {
     if (c) c->c.clear();
 }
 
+// Every render entry point fills a FrameRequest and calls render_request(): the Compositions behind the
+// handles (null batch entries stay null for Renderer::render to refuse), the sliced host-frame
+// pipeline first for a host RGBA frame without a layer cache, and no C++ exception across the ABI.
+// ids_fn: the name of an ID entry point, which is refused without an ID buffer (the Renderer would
+// take the call for an RGBA-only request).
+static int render_request(forma_renderer* r, FrameRequest q, forma_composition* c, forma_composition* const* comps = nullptr,
+                          const char* ids_fn = nullptr) {
+    return guarded((int)FORMA_ERR_CAPACITY, [&] {
+        if (ids_fn && !q.ids.ptr) {
+            set_error("%s: no ID buffer", ids_fn);
+            return (int)FORMA_STATUS_INVALID;
+        }
+        std::vector<Composition*> cs(comps ? q.n : 0u);
+        for (size_t k = 0; k < cs.size(); ++k) cs[k] = comps[k] ? &comps[k]->c : nullptr;
+        q.comp = c ? &c->c : nullptr;
+        q.batch = comps ? cs.data() : nullptr;
+        if (q.kind == FrameKind::single && q.rgba.ptr && !q.rgba.on_device && !q.cache) {
+            const int st = sliced_host_render(r, q);
+            if (st >= 0) return st;
+        }
+        return r->r.render(q);
+    });
+}
 int forma_renderer_render(forma_renderer* r, forma_composition* c, uint8_t* buffer, uint64_t width, uint64_t stride,
                           uint64_t height, const uint32_t channels[4], const float clear[4], const forma_rect* crop,
                           forma_layer_cache* cache, forma_timings* timings) {
-    return guarded((int)FORMA_ERR_CAPACITY, [&] {
-        if (!cache) {
-            const int st = sliced_host_render(r, c, buffer, width, stride, height, channels, clear, crop, timings);
-            if (st >= 0) return st;
-        }
-        return r->r.render(c->c, buffer, false, width, stride, height, channels, clear, crop, cache ? &cache->c : nullptr,
-                           timings);
-    });
+    FrameRequest q{FrameKind::single, 0, width, height, channels, clear, timings, crop, cache ? &cache->c : nullptr};
+    q.rgba = {buffer, false, stride};
+    return render_request(r, q, c);
 }
 int forma_renderer_render_device(forma_renderer* r, forma_composition* c, uint8_t* device_buffer, uint64_t width,
                                  uint64_t stride, uint64_t height, const uint32_t channels[4], const float clear[4],
                                  const forma_rect* crop, forma_layer_cache* cache, forma_timings* timings) {
-    return guarded((int)FORMA_ERR_CAPACITY, [&] {
-        return r->r.render(c->c, device_buffer, true, width, stride, height, channels, clear, crop,
-                           cache ? &cache->c : nullptr, timings);
-    });
+    FrameRequest q{FrameKind::single, 0, width, height, channels, clear, timings, crop, cache ? &cache->c : nullptr};
+    q.rgba = {device_buffer, true, stride};
+    return render_request(r, q, c);
 }
 int forma_renderer_render_ids(forma_renderer* r, forma_composition* c, uint32_t* ids, uint64_t width, uint64_t ids_stride,
                               uint64_t height, const forma_rect* crop, float min_coverage, forma_timings* timings) {
-    return guarded((int)FORMA_ERR_CAPACITY, [&] {
-        return r->r.render_ids(c->c, nullptr, 0, nullptr, nullptr, ids, false, width, ids_stride, height, crop, min_coverage,
-                               timings);
-    });
+    FrameRequest q{FrameKind::single, 0, width, height, nullptr, nullptr, timings, crop};
+    q.ids = {reinterpret_cast<uint8_t*>(ids), false, ids_stride, 0, min_coverage};
+    return render_request(r, q, c, nullptr, __func__);
 }
 int forma_renderer_render_ids_device(forma_renderer* r, forma_composition* c, uint32_t* device_ids, uint64_t width,
                                      uint64_t ids_stride, uint64_t height, const forma_rect* crop, float min_coverage,
                                      forma_timings* timings) {
-    return guarded((int)FORMA_ERR_CAPACITY, [&] {
-        return r->r.render_ids(c->c, nullptr, 0, nullptr, nullptr, device_ids, true, width, ids_stride, height, crop,
-                               min_coverage, timings);
-    });
+    FrameRequest q{FrameKind::single, 0, width, height, nullptr, nullptr, timings, crop};
+    q.ids = {reinterpret_cast<uint8_t*>(device_ids), true, ids_stride, 0, min_coverage};
+    return render_request(r, q, c, nullptr, __func__);
 }
 int forma_renderer_render_device_with_ids(forma_renderer* r, forma_composition* c, uint8_t* device_buffer, uint64_t width,
                                           uint64_t width_stride, uint64_t height, const uint32_t channels[4],
                                           const float clear_color[4], const forma_rect* crop, uint32_t* device_ids,
                                           uint64_t ids_stride, float min_coverage, forma_timings* timings) {
-    return guarded((int)FORMA_ERR_CAPACITY, [&] {
-        if (!device_buffer) {
-            set_error("forma_renderer_render_device_with_ids: no RGBA buffer");
-            return (int)FORMA_STATUS_INVALID;
-        }
-        return r->r.render_ids(c->c, device_buffer, width_stride, channels, clear_color, device_ids, true, width, ids_stride,
-                               height, crop, min_coverage, timings);
-    });
+    if (!device_buffer) {  // (without one, the call would be forma_renderer_render_ids_device)
+        set_error("forma_renderer_render_device_with_ids: no RGBA buffer");
+        return FORMA_STATUS_INVALID;
+    }
+    FrameRequest q{FrameKind::single, 0, width, height, channels, clear_color, timings, crop};
+    q.rgba = {device_buffer, true, width_stride};
+    q.ids = {reinterpret_cast<uint8_t*>(device_ids), true, ids_stride, 0, min_coverage};
+    return render_request(r, q, c, nullptr, __func__);
 }
 uint32_t forma_renderer_max_views(uint64_t height) { return max_views(height); }
 int forma_renderer_render_views_device(forma_renderer* r, forma_composition* c, const float* views, uint32_t n, uint8_t* device_buffer,
                                        uint64_t width, uint64_t width_stride, uint64_t height, uint64_t view_stride,
                                        const uint32_t channels[4], const float clear_color[4], forma_timings* timings) {
-    return guarded((int)FORMA_ERR_CAPACITY, [&] {
-        return r->r.render_views(c->c, views, n, device_buffer, true, width, width_stride, height, view_stride, channels, clear_color,
-                                 timings);
-    });
-}
-// The Compositions behind the handles (null entries stay null for Renderer::render_batch to refuse).
-static int render_batch(forma_renderer* r, forma_composition* const* comps, uint32_t n, uint8_t* buffer, bool on_device,
-                        uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride, const uint32_t channels[4],
-                        const float clear_color[4], forma_timings* timings, const IdStack* ids = nullptr) {
-    return guarded((int)FORMA_ERR_CAPACITY, [&] {
-        std::vector<Composition*> cs(comps ? n : 0u);
-        for (size_t k = 0; k < cs.size(); ++k) cs[k] = comps[k] ? &comps[k]->c : nullptr;
-        return r->r.render_batch(comps ? cs.data() : nullptr, n, buffer, on_device, width, width_stride, height, frame_stride, channels,
-                                 clear_color, timings, ids);
-    });
-}
-int forma_renderer_render_batch_device(forma_renderer* r, forma_composition* const* comps, uint32_t n, uint8_t* device_buffer,
-                                       uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride,
-                                       const uint32_t channels[4], const float clear_color[4], forma_timings* timings) {
-    return render_batch(r, comps, n, device_buffer, true, width, width_stride, height, frame_stride, channels, clear_color, timings);
-}
-int forma_renderer_render_batch(forma_renderer* r, forma_composition* const* comps, uint32_t n, uint8_t* host_buffer, uint64_t width,
-                                uint64_t width_stride, uint64_t height, uint64_t frame_stride, const uint32_t channels[4],
-                                const float clear_color[4], forma_timings* timings) {
-    return render_batch(r, comps, n, host_buffer, false, width, width_stride, height, frame_stride, channels, clear_color, timings);
+    FrameRequest q{FrameKind::views, n, width, height, channels, clear_color, timings};
+    q.views = views;
+    q.rgba = {device_buffer, true, width_stride, view_stride};
+    return render_request(r, q, c);
 }
 int forma_renderer_render_views(forma_renderer* r, forma_composition* c, const float* views, uint32_t n, uint8_t* host_buffer,
                                 uint64_t width, uint64_t width_stride, uint64_t height, uint64_t view_stride,
                                 const uint32_t channels[4], const float clear_color[4], forma_timings* timings) {
-    return guarded((int)FORMA_ERR_CAPACITY, [&] {
-        return r->r.render_views(c->c, views, n, host_buffer, false, width, width_stride, height, view_stride, channels, clear_color,
-                                 timings);
-    });
+    FrameRequest q{FrameKind::views, n, width, height, channels, clear_color, timings};
+    q.views = views;
+    q.rgba = {host_buffer, false, width_stride, view_stride};
+    return render_request(r, q, c);
 }
-// ID frames of views and batches. A call without ID frames at all is refused here: the Renderer
-// would take it for the RGBA call.
-static int no_id_frames(const char* fn) {
-    set_error("%s: no ID buffer", fn);
-    return FORMA_STATUS_INVALID;
+int forma_renderer_render_batch_device(forma_renderer* r, forma_composition* const* comps, uint32_t n, uint8_t* device_buffer,
+                                       uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride,
+                                       const uint32_t channels[4], const float clear_color[4], forma_timings* timings) {
+    FrameRequest q{FrameKind::batch, n, width, height, channels, clear_color, timings};
+    q.rgba = {device_buffer, true, width_stride, frame_stride};
+    return render_request(r, q, nullptr, comps);
+}
+int forma_renderer_render_batch(forma_renderer* r, forma_composition* const* comps, uint32_t n, uint8_t* host_buffer, uint64_t width,
+                                uint64_t width_stride, uint64_t height, uint64_t frame_stride, const uint32_t channels[4],
+                                const float clear_color[4], forma_timings* timings) {
+    FrameRequest q{FrameKind::batch, n, width, height, channels, clear_color, timings};
+    q.rgba = {host_buffer, false, width_stride, frame_stride};
+    return render_request(r, q, nullptr, comps);
 }
 int forma_renderer_render_views_ids_device(forma_renderer* r, forma_composition* c, const float* views, uint32_t n,
                                            uint8_t* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
                                            uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
                                            uint32_t* device_ids, uint64_t ids_stride, uint64_t ids_view_stride, float min_coverage,
                                            forma_timings* timings) {
-    return guarded((int)FORMA_ERR_CAPACITY, [&] {
-        if (!device_ids) return no_id_frames("forma_renderer_render_views_ids_device");
-        const IdStack ids{device_ids, true, ids_stride, ids_view_stride, min_coverage};
-        return r->r.render_views(c->c, views, n, device_buffer, true, width, width_stride, height, view_stride, channels, clear_color,
-                                 timings, &ids);
-    });
+    FrameRequest q{FrameKind::views, n, width, height, channels, clear_color, timings};
+    q.views = views;
+    q.rgba = {device_buffer, true, width_stride, view_stride};
+    q.ids = {reinterpret_cast<uint8_t*>(device_ids), true, ids_stride, ids_view_stride, min_coverage};
+    return render_request(r, q, c, nullptr, __func__);
 }
 int forma_renderer_render_views_ids(forma_renderer* r, forma_composition* c, const float* views, uint32_t n, uint32_t* host_ids,
                                     uint64_t width, uint64_t ids_stride, uint64_t height, uint64_t ids_view_stride,
                                     float min_coverage, forma_timings* timings) {
-    return guarded((int)FORMA_ERR_CAPACITY, [&] {
-        if (!host_ids) return no_id_frames("forma_renderer_render_views_ids");
-        const IdStack ids{host_ids, false, ids_stride, ids_view_stride, min_coverage};
-        return r->r.render_views(c->c, views, n, nullptr, false, width, 0, height, 0, nullptr, nullptr, timings, &ids);
-    });
+    FrameRequest q{FrameKind::views, n, width, height, nullptr, nullptr, timings};
+    q.views = views;
+    q.ids = {reinterpret_cast<uint8_t*>(host_ids), false, ids_stride, ids_view_stride, min_coverage};
+    return render_request(r, q, c, nullptr, __func__);
 }
 int forma_renderer_render_batch_ids_device(forma_renderer* r, forma_composition* const* comps, uint32_t n, uint8_t* device_buffer,
                                            uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride,
                                            const uint32_t channels[4], const float clear_color[4], uint32_t* device_ids,
                                            uint64_t ids_stride, uint64_t ids_frame_stride, float min_coverage,
                                            forma_timings* timings) {
-    if (!device_ids) return no_id_frames("forma_renderer_render_batch_ids_device");
-    const IdStack ids{device_ids, true, ids_stride, ids_frame_stride, min_coverage};
-    return render_batch(r, comps, n, device_buffer, true, width, width_stride, height, frame_stride, channels, clear_color, timings,
-                        &ids);
+    FrameRequest q{FrameKind::batch, n, width, height, channels, clear_color, timings};
+    q.rgba = {device_buffer, true, width_stride, frame_stride};
+    q.ids = {reinterpret_cast<uint8_t*>(device_ids), true, ids_stride, ids_frame_stride, min_coverage};
+    return render_request(r, q, nullptr, comps, __func__);
 }
 int forma_renderer_render_batch_ids(forma_renderer* r, forma_composition* const* comps, uint32_t n, uint32_t* host_ids, uint64_t width,
                                     uint64_t ids_stride, uint64_t height, uint64_t ids_frame_stride, float min_coverage,
                                     forma_timings* timings) {
-    if (!host_ids) return no_id_frames("forma_renderer_render_batch_ids");
-    const IdStack ids{host_ids, false, ids_stride, ids_frame_stride, min_coverage};
-    return render_batch(r, comps, n, nullptr, false, width, 0, height, 0, nullptr, nullptr, timings, &ids);
+    FrameRequest q{FrameKind::batch, n, width, height, nullptr, nullptr, timings};
+    q.ids = {reinterpret_cast<uint8_t*>(host_ids), false, ids_stride, ids_frame_stride, min_coverage};
+    return render_request(r, q, nullptr, comps, __func__);
 }
 // --- shared frames (multi-GPU, see include/forma_b200.h) -----------------------
 static_assert(sizeof(cudaIpcMemHandle_t) == sizeof(forma_ipc_handle), "CUDA IPC handles are 64 bytes");

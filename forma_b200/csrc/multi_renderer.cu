@@ -104,7 +104,7 @@ struct forma_renderer_multi {
     }
 };
 
-static int multi_render_impl(forma_renderer_multi* m, forma_composition* c, uint8_t* buffer, bool on_device, uint64_t width,
+static int multi_render_impl(forma_renderer_multi* m, Composition* c, uint8_t* buffer, bool on_device, uint64_t width,
                              uint64_t stride, uint64_t height, const uint32_t channels[4], const float clear[4],
                              const forma_rect* crop, forma_timings* timings, size_t n_use = 0, bool chained_uploads = false) {
     const size_t n = n_use ? std::min(n_use, m->dev.size()) : m->dev.size();
@@ -117,7 +117,7 @@ static int multi_render_impl(forma_renderer_multi* m, forma_composition* c, uint
         set_error("forma_renderer_multi_render_device: peer access to the first device is not available");
         return FORMA_STATUS_INVALID;
     }
-    Composition& comp = c->c;
+    Composition& comp = *c;
     // Tile rows to paint (crop is tile-granular like cpu/renderer.rs:43-52).
     const uint32_t tiles_y = (uint32_t)((height + 15u) / 16u);
     const TileRect tiles = tile_rect(width, height, crop);
@@ -174,9 +174,10 @@ static int multi_render_impl(forma_renderer_multi* m, forma_composition* c, uint
         forma_rect band;
         if (!band_of(i, &band)) return;
         Renderer& R = m->dev[i]->r;
-        status[i] = guarded((int)FORMA_ERR_CAPACITY, [&] {
-            return R.render(comp, buffer, on_device, width, stride, height, channels, clear, &band, nullptr, &tms[i]);
-        });
+        FrameRequest q{FrameKind::single, 0, width, height, channels, clear, &tms[i], &band};
+        q.rgba = {buffer, on_device, stride};
+        q.comp = &comp;
+        status[i] = guarded((int)FORMA_ERR_CAPACITY, [&] { return R.render(q); });
         if (status[i]) {
             errors[i] = forma_last_error();
             return;
@@ -276,16 +277,18 @@ static int multi_render_impl(forma_renderer_multi* m, forma_composition* c, uint
 // those of a band render (tests/test_gpu_bench_scale.py: bands == whole frame).
 // Not sliced: frames with a layer cache (the cache records belong to one renderer), layers with
 // transforms (no band filter: every slice would upload everything), small compositions, short frames.
-int sliced_host_render(forma_renderer* r, forma_composition* c, uint8_t* buffer, uint64_t width, uint64_t stride,
-                       uint64_t height, const uint32_t channels[4], const float clear[4], const forma_rect* crop,
-                       forma_timings* timings) {
+int sliced_host_render(forma_renderer* r, const FrameRequest& q) {
     Renderer& P = r->r;
+    uint8_t* buffer = q.rgba.ptr;
+    const uint64_t width = q.width, stride = q.rgba.stride, height = q.height;
+    const uint32_t* channels = q.channels;
+    const forma_rect* crop = q.crop;
     const int want = options().host_slices;
     if (want < 2 || !buffer || !width || !height || width > FORMA_MAX_WIDTH || height > FORMA_MAX_HEIGHT || width * 4 > stride)
         return -1;  // (invalid targets are reported by the plain path)
     for (int k = 0; k < 4; ++k)
         if (channels[k] > 5u) return -1;
-    Composition& comp = c->c;
+    Composition& comp = *q.comp;
     if ((uint64_t)comp.n_points < (uint64_t)std::max(options().slice_min_points, 0)) return -1;
     if (crop && crop->hor_end <= crop->hor_start) return -1;
     const TileRect tiles = tile_rect(width, height, crop);
@@ -339,7 +342,7 @@ int sliced_host_render(forma_renderer* r, forma_composition* c, uint8_t* buffer,
         FORMA_CUDA_TRY(cudaStreamWaitEvent(Q.stream, P.count_ev, 0));
         before[i] = {Q.launches, Q.h2d_bytes, Q.d2h_bytes};
     }
-    const int st = multi_render_impl(m, c, buffer, false, width, stride, height, channels, clear, crop, timings, n,
+    const int st = multi_render_impl(m, q.comp, buffer, false, width, stride, height, channels, q.clear, crop, q.timings, n,
                                      options().slice_chain != 0);
     if (st) {  // a failed frame describes nothing: no segments, cells, row costs or slices to inspect
         P.last_segments = P.last_cells = P.last_entries = 0;
@@ -439,14 +442,16 @@ int forma_renderer_multi_device_count(const forma_renderer_multi* m) { return m 
 int forma_renderer_multi_render(forma_renderer_multi* m, forma_composition* c, uint8_t* buffer, uint64_t width, uint64_t stride,
                                 uint64_t height, const uint32_t channels[4], const float clear[4], const forma_rect* crop,
                                 forma_timings* timings) {
-    return guarded((int)FORMA_ERR_CAPACITY,
-                   [&] { return multi_render_impl(m, c, buffer, false, width, stride, height, channels, clear, crop, timings); });
+    return guarded((int)FORMA_ERR_CAPACITY, [&] {
+        return multi_render_impl(m, c ? &c->c : nullptr, buffer, false, width, stride, height, channels, clear, crop, timings);
+    });
 }
 int forma_renderer_multi_render_device(forma_renderer_multi* m, forma_composition* c, uint8_t* buffer_on_first_device,
                                        uint64_t width, uint64_t stride, uint64_t height, const uint32_t channels[4],
                                        const float clear[4], const forma_rect* crop, forma_timings* timings) {
     return guarded((int)FORMA_ERR_CAPACITY, [&] {
-        return multi_render_impl(m, c, buffer_on_first_device, true, width, stride, height, channels, clear, crop, timings);
+        return multi_render_impl(m, c ? &c->c : nullptr, buffer_on_first_device, true, width, stride, height, channels, clear, crop,
+                                 timings);
     });
 }
 /* Tile-row boundaries of the bands the next frame will use (n + 1 values) and the

@@ -363,37 +363,36 @@ int Renderer::prefetch(Composition& comp, uint64_t width, uint64_t height, const
 }
 
 // One frame of S, whatever its kind: uploads, line setup, sort, then the painter tables,
-// paint_step(heavy_lists, &paint_launches) (the frame's kernels) and output_step() (the copy to
-// where the caller wants the frame) once or, when the sync-free bounds were too small, twice.
-template <class Paint, class Output>
-int Renderer::run_frame(Composition* comp, PaintScene& S, const FrameSpec& spec, forma_timings* timings, Paint&& paint_step,
-                        Output&& output_step) {
+// paint_step (the frame's kernels) and output_step (the copy to where the caller wants the frame)
+// once or, when the sync-free bounds were too small, twice.
+int Renderer::run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p) {
     if (!prefetched) FORMA_CUDA_TRY(cudaEventRecord(timer.ev[0], stream));
     prefetched = false;
     // Lines entirely above / below the painted tile rows cannot reach a painted tile: they are
     // culled per line (rasterize), and whole inserts are left out of the device's segment
     // buffer when the band is narrower than the frame (flush_geometry). Line setup sees every
     // frame of a stack as a frame of its own: all its rows are painted.
-    const uint32_t height = spec.n_frames ? spec.frame_height : S.height;
-    const FrameBand band = spec.n_frames ? FrameBand{0.0f, (float)height, false} : tile_band(S.ty_lo, S.ty_hi, height);
+    const uint32_t height = (uint32_t)q.height;
+    const FrameBand band = p.rows ? FrameBand{0.0f, (float)height, false} : tile_band(S.ty_lo, S.ty_hi, height);
+    const bool views = q.kind == FrameKind::views, batched = q.kind == FrameKind::batch;
     int st = FORMA_STATUS_OK;
     BatchLines batch{};
-    if (spec.batch) {  // every composition's uploads, then the batch tables
-        st = bind_batch(spec.batch, spec.n_frames, S, height, batch);
+    if (batched) {  // every composition's uploads, then the batch tables
+        st = bind_batch(q.batch, q.n, S, height, batch);
         if (st) return st;
     } else {
-        st = upload_tables(*comp, -1);
+        st = upload_tables(*q.comp, -1);
         if (st) return st;
-        st = flush_geometry(*comp, band.lo, band.hi, band.partial);
+        st = flush_geometry(*q.comp, band.lo, band.hi, band.partial);
         if (st) return st;
-        st = bind_frame(*comp, S, spec.cache, S.clear, spec.pack_written);
+        st = bind_frame(*q.comp, S, q.cache, S.clear, p.pack_written);
         if (st) return st;
     }
-    if (spec.views) {
-        const uint32_t nv = spec.n_frames;
+    if (views) {
+        const uint32_t nv = q.n;
         FORMA_CUDA_TRY(h_views.reserve(6u * nv));
         FORMA_CUDA_TRY(d_views.reserve(6u * nv));
-        std::memcpy(h_views.ptr, spec.views, 6u * nv * sizeof(float));  // (the previous call's copy is complete: rasterize waited for it)
+        std::memcpy(h_views.ptr, q.views, 6u * nv * sizeof(float));  // (the previous call's copy is complete: rasterize waited for it)
         FORMA_CUDA_TRY(cudaMemcpyAsync(d_views.ptr, h_views.ptr, 6u * nv * sizeof(float), cudaMemcpyHostToDevice, stream));
         h2d_bytes += 6u * nv * sizeof(float);
     }
@@ -401,8 +400,7 @@ int Renderer::run_frame(Composition* comp, PaintScene& S, const FrameSpec& spec,
 
     FORMA_CUDA_TRY(cudaEventRecord(timer.ev[7], stream));
     uint32_t n = 0;
-    st = rasterize(comp, S.width, height, band.lo, band.hi, &n, spec.views ? &va : nullptr, spec.n_frames,
-                   spec.batch ? &batch : nullptr);
+    st = rasterize(q.comp, S.width, height, band.lo, band.hi, &n, views ? &va : nullptr, q.n, batched ? &batch : nullptr);
     if (st) return st;
 
     // Stage 3: sort.
@@ -431,7 +429,7 @@ int Renderer::run_frame(Composition* comp, PaintScene& S, const FrameSpec& spec,
     // the clear colour) sends the frame through again with counted tables.
     // (pack_written: the host scatter of the written tiles must not see a frame that is redone.)
     const uint32_t prev_cells = last_cells, prev_gaps = last_gaps;  // of this renderer's previous frame
-    const bool fast = options().sync_free && n > 0 && prev_cells > 0 && !spec.pack_written;
+    const bool fast = options().sync_free && n > 0 && prev_cells > 0 && !p.pack_written;
     last_cells = last_entries = 0;
     last_written_tiles = 0;
     last_tables_redone = false;
@@ -443,10 +441,10 @@ int Renderer::run_frame(Composition* comp, PaintScene& S, const FrameSpec& spec,
         st = queue_row_costs(S, n);
         if (st) return st;
         FORMA_CUDA_TRY(cudaEventRecord(timer.ev[4], stream));
-        st = paint_step(heavy_lists, &paint_launches);
+        st = paint_step(q, S, p, heavy_lists, &paint_launches);
         if (st) return st;
         FORMA_CUDA_TRY(cudaEventRecord(timer.ev[5], stream));
-        st = output_step();
+        st = output_step(q, S, p);
         if (st) return st;
         FORMA_CUDA_TRY(cudaEventRecord(timer.ev[6], stream));
         FORMA_CUDA_TRY(cudaStreamSynchronize(stream));
@@ -463,14 +461,14 @@ int Renderer::run_frame(Composition* comp, PaintScene& S, const FrameSpec& spec,
     times_pending = true;
     pending_sort_passes = timed_sort_passes;
     pending_paint_launches = paint_launches;
-    if (timings) {
+    if (forma_timings* timings = q.timings) {
         resolve_times();
         timings->line_setup_ms = stage_ms[1];
         timings->rasterize_ms = stage_ms[2];
         timings->sort_ms = stage_ms[3];
         timings->paint_ms = stage_ms[4] + stage_ms[5];
-        if (comp) {
-            const CompDevice& cd = comp->on(res_key);
+        if (q.comp) {
+            const CompDevice& cd = q.comp->on(res_key);
             timings->n_lines = cd.n_resident ? cd.n_resident - 1 : 0;
         } else {
             timings->n_lines = batch.n_lines;
@@ -480,102 +478,95 @@ int Renderer::run_frame(Composition* comp, PaintScene& S, const FrameSpec& spec,
     return FORMA_STATUS_OK;
 }
 
-int Renderer::render(Composition& comp, uint8_t* buffer, bool buffer_on_device, uint64_t width, uint64_t stride,
-                     uint64_t height, const uint32_t channels_in[4], const float clear[4], const forma_rect* crop,
-                     LayerCache* cache, forma_timings* timings) {
+int Renderer::render(const FrameRequest& q) {
+    int st = check_request(q);
+    if (st) return st;
+    const bool stack = q.kind != FrameKind::single, rgba = q.rgba.ptr != nullptr;
+    // Each target's frame on the device. A single frame keeps the caller's stride and is painted in
+    // place when it is on the device. A stack is painted in place when its frames are whole tile
+    // rows laid out as the stacked frame's rows; each target decides for itself.
+    auto device_frame = [&](const FrameTarget& t) {
+        const bool direct = t.on_device && (!stack || (q.height % 16u == 0u && t.frame_stride == q.height * t.stride));
+        return DeviceFrame{t.ptr, direct || !stack ? t.stride : 4u * q.width, direct};
+    };
+    FramePlan p{device_frame(q.rgba), device_frame(q.ids), stack ? (uint32_t)((q.height + 15u) / 16u) : 0u, false, false};
+    // The PaintScene of the RGBA target, or of the ID target when it is alone.
+    static const uint32_t kIdChannels[4] = {0, 1, 2, 3};
+    static const float kIdClear[4] = {0, 0, 0, 0};
     PaintScene S{};
-    int st = begin_frame(S, buffer, width, stride, height, channels_in, clear, crop);
+    st = begin_frame(S, q.width, rgba ? p.rgba.stride : p.ids.stride, stack ? (uint64_t)q.n * p.rows * 16u : q.height,
+                     rgba ? q.channels : kIdChannels, rgba ? q.clear : kIdClear, q.crop);
     if (st) return st;
-    uint8_t* fb = buffer;
-    if (!buffer_on_device) {
-        FORMA_CUDA_TRY(framebuffer.reserve((size_t)stride * height));
-        fb = framebuffer.ptr;
+    if (rgba && !p.rgba.direct) {
+        FORMA_CUDA_TRY(framebuffer.reserve((size_t)p.rgba.stride * S.height));
+        p.rgba.ptr = framebuffer.ptr;
     }
-    const uint32_t paint_rows = S.ty_hi - S.ty_lo;
-    const bool in_bands = !buffer_on_device && !cache && paint_rows >= (copy_bands_override ? 8u : 32u) && S.tx_hi > S.tx_lo &&
-                          band_copies_enabled();
-    const bool pack_written = cache && !buffer_on_device;
-    st = run_frame(
-        &comp, S, FrameSpec{cache, pack_written}, timings,
-        [&](const uint32_t* heavy_lists, uint32_t* paint_launches) {
-            return paint(S, fb, buffer, stride, in_bands, heavy_lists, paint_launches);
-        },
-        [&] {
-            if (pack_written) return scatter_written_tiles(S, fb, buffer, stride);
-            if (!buffer_on_device && !in_bands) return copy_to_host(S, buffer, fb, stride, stream);
-            return FORMA_STATUS_OK;
-        });
+    if (q.ids.ptr && !p.ids.direct) {
+        FORMA_CUDA_TRY(id_frame.reserve((size_t)(p.ids.stride / 4u) * S.height));
+        p.ids.ptr = reinterpret_cast<uint8_t*>(id_frame.ptr);
+    }
+    p.in_bands = rgba && !stack && !q.rgba.on_device && !q.cache && S.ty_hi - S.ty_lo >= (copy_bands_override ? 8u : 32u) &&
+                 S.tx_hi > S.tx_lo && band_copies_enabled();
+    p.pack_written = q.cache && !q.rgba.on_device;
+    st = run_frame(q, S, p);
     if (st) return st;
-    if (cache) {  // renderer.rs:217-223
-        cache->has_clear = true;
-        std::memcpy(cache->clear_color, clear, sizeof(cache->clear_color));
-        for (auto& kv : comp.layers) {
-            if (kv.second->enabled) kv.second->unchanged_bits |= 1u << cache->id;
-            else kv.second->unchanged_bits &= ~(1u << cache->id);
+    if (q.cache) {  // renderer.rs:217-223
+        q.cache->has_clear = true;
+        std::memcpy(q.cache->clear_color, q.clear, sizeof(q.cache->clear_color));
+        for (auto& kv : q.comp->layers) {
+            if (kv.second->enabled) kv.second->unchanged_bits |= 1u << q.cache->id;
+            else kv.second->unchanged_bits &= ~(1u << q.cache->id);
         }
     }
     return FORMA_STATUS_OK;
 }
 
-// An ID frame, alone (rgba == nullptr) or after the RGBA frame of the same tables in device
-// memory (render_device's frame without a cache). The sync-free redo repeats the kernels. The ID
-// frame never touches a layer cache.
-int Renderer::render_ids(Composition& comp, uint8_t* rgba, uint64_t rgba_stride, const uint32_t channels[4], const float clear[4],
-                         uint32_t* ids, bool ids_on_device, uint64_t width, uint64_t ids_stride, uint64_t height,
-                         const forma_rect* crop, float min_coverage, forma_timings* timings) {
-    if (!ids || ids_stride % 4u != 0u || !std::isfinite(min_coverage) || min_coverage < 0.0f || min_coverage >= 1.0f) {
-        set_error("invalid ID frame: stride %llu (a multiple of 4 bytes), min_coverage %g (finite, in [0, 1))",
-                  (unsigned long long)ids_stride, (double)min_coverage);
+// The checks of a request, before anything is written: each target (LinearLayout::new asserts,
+// layout/mod.rs:188-193, consts.rs limits, and for a stack the frame count and frame stride), the
+// ID target's own, then the views or the compositions of a batch. An ID-only request has no RGBA
+// target to check.
+int Renderer::check_request(const FrameRequest& q) {
+    const bool stack = q.kind != FrameKind::single;
+    const char* what = q.kind == FrameKind::views ? "view" : "frame";
+    const uint64_t width = q.width, height = q.height;
+    auto check_target = [&](const FrameTarget& t) {
+        if (!t.ptr || width == 0 || height == 0 || width * 4 > t.stride || width > FORMA_MAX_WIDTH || height > FORMA_MAX_HEIGHT) {
+            set_error("invalid render target %llux%llu stride %llu", (unsigned long long)width, (unsigned long long)height,
+                      (unsigned long long)t.stride);
+            return (int)FORMA_STATUS_INVALID;
+        }
+        if (!stack) return (int)FORMA_STATUS_OK;
+        if (q.n == 0 || q.n > max_views(height)) {
+            set_error("%u %ss of height %llu: between 1 and %u %ss of this height fit in one call", q.n, what,
+                      (unsigned long long)height, max_views(height), what);
+            return (int)FORMA_STATUS_INVALID;
+        }
+        if (t.frame_stride < (height - 1u) * t.stride + 4u * width) {
+            set_error("%s stride %llu is smaller than one %s (%llu bytes)", what, (unsigned long long)t.frame_stride, what,
+                      (unsigned long long)((height - 1u) * t.stride + 4u * width));
+            return (int)FORMA_STATUS_INVALID;
+        }
+        return (int)FORMA_STATUS_OK;
+    };
+    int st = q.rgba.ptr || !q.ids.ptr ? check_target(q.rgba) : FORMA_STATUS_OK;
+    if (st) return st;
+    if (q.ids.ptr) {
+        const FrameTarget& t = q.ids;
+        if (t.stride % 4u != 0u || t.frame_stride % 4u != 0u || !std::isfinite(t.min_coverage) || t.min_coverage < 0.0f ||
+            t.min_coverage >= 1.0f) {
+            set_error("invalid ID frame: stride %llu, %s stride %llu (multiples of 4 bytes), min_coverage %g (finite, in [0, 1))",
+                      (unsigned long long)t.stride, what, (unsigned long long)t.frame_stride, (double)t.min_coverage);
+            return FORMA_STATUS_INVALID;
+        }
+        st = check_target(t);
+        if (st) return st;
+    }
+    if ((q.kind == FrameKind::views && !q.views) || (q.kind == FrameKind::batch && !q.batch)) {
+        set_error("no %s", q.kind == FrameKind::views ? "views" : "compositions");
         return FORMA_STATUS_INVALID;
     }
-    PaintScene S{};
-    static const uint32_t kIdChannels[4] = {0, 1, 2, 3};
-    static const float kIdClear[4] = {0, 0, 0, 0};
-    int st = rgba ? begin_frame(S, rgba, width, rgba_stride, height, channels, clear, crop)
-                  : begin_frame(S, reinterpret_cast<const uint8_t*>(ids), width, ids_stride, height, kIdChannels, kIdClear, crop);
-    if (st) return st;
-    if (rgba && width * 4u > ids_stride) {
-        set_error("invalid ID frame stride %llu for width %llu", (unsigned long long)ids_stride, (unsigned long long)width);
-        return FORMA_STATUS_INVALID;
-    }
-    uint32_t* id_out = ids;
-    if (!ids_on_device) {
-        FORMA_CUDA_TRY(id_frame.reserve((size_t)(ids_stride / 4u) * height));
-        id_out = id_frame.ptr;
-    }
-    return run_frame(
-        &comp, S, FrameSpec{}, timings,
-        [&](const uint32_t* heavy_lists, uint32_t* paint_launches) {
-            FORMA_CUDA_TRY(id_flags.reserve(std::max<size_t>(recs.capacity, 1)));
-            if (rgba) {
-                const int st = paint(S, rgba, rgba, rgba_stride, false, heavy_lists, paint_launches);
-                if (st) return st;
-                ++*paint_launches;
-            }
-            launch_paint_ids(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), id_flags.ptr, id_out, ids_stride,
-                             min_coverage, totals.ptr + 8, stream);
-            ++launches;
-            FORMA_CUDA_TRY(cudaGetLastError());
-            return FORMA_STATUS_OK;
-        },
-        [&] {
-            if (ids_on_device) return FORMA_STATUS_OK;
-            return copy_to_host(S, reinterpret_cast<uint8_t*>(ids), reinterpret_cast<const uint8_t*>(id_out), ids_stride, stream);
-        });
-}
-
-// n views of one composition in one pass: one frame that stacks the views top to bottom, n * rows
-// tile rows of `width` pixels (rows = ceil(height / 16)). Line setup rasterizes every view in its
-// own coordinates and moves its segments' tile rows to the view's place in the stack (ViewArgs);
-// the tables, the sort and the painter see one frame. No layer cache and no band filter: the whole
-// composition is resident.
-int Renderer::render_views(Composition& comp, const float* views, uint32_t n, uint8_t* buffer, bool buffer_on_device, uint64_t width,
-                           uint64_t stride, uint64_t height, uint64_t view_stride, const uint32_t channels[4], const float clear[4],
-                           forma_timings* timings, const IdStack* ids) {
-    const int st = check_stacks("view", views != nullptr, n, width, height, buffer, stride, view_stride, ids);
-    if (st) return st;
-    for (uint32_t b = 0; b < n; ++b) {  // [ux, vx, uy, vy, tx, ty], as forma_layer_set_transform checks them
-        const float* v = views + 6u * b;
+    for (uint32_t b = 0; q.kind == FrameKind::views && b < q.n; ++b) {  // [ux, vx, uy, vy, tx, ty], as forma_layer_set_transform checks them
+        const float* v = q.views + 6u * b;
         bool finite = true;
         for (int k = 0; k < 6; ++k) finite = finite && std::isfinite(v[k]);
         if (!finite || !geom_pres_ok(v[0], v[2], v[1], v[3])) {
@@ -583,35 +574,23 @@ int Renderer::render_views(Composition& comp, const float* views, uint32_t n, ui
             return FORMA_STATUS_INVALID;
         }
     }
-    FrameStack K{buffer, buffer_on_device, width, stride, height, view_stride, n};
-    return run_stack(&comp, FrameSpec{nullptr, false, views, n, (uint32_t)height}, K, ids, channels, clear, timings);
-}
-
-// n compositions, one frame each, in one pass: the stacked frame of render_views, but frame c's
-// line setup reads comps[c]'s segment buffer and moves its segments' layers to the composition's
-// slice of the layer field (bind_batch), so that the batch tables serve every frame. No layer
-// cache and no band filter: every composition is resident.
-int Renderer::render_batch(Composition* const* comps, uint32_t n, uint8_t* buffer, bool buffer_on_device, uint64_t width,
-                           uint64_t stride, uint64_t height, uint64_t frame_stride, const uint32_t channels[4], const float clear[4],
-                           forma_timings* timings, const IdStack* ids) {
-    const int st = check_stacks("frame", comps != nullptr, n, width, height, buffer, stride, frame_stride, ids);
-    if (st) return st;
+    if (q.kind != FrameKind::batch) return FORMA_STATUS_OK;
     // The distinct compositions in order of first appearance, and the slices of the layer field
     // they need: n_orders each, as rebuild_tables counts them.
     batch_distinct.clear();
-    batch_slot.resize(n);
+    batch_slot.resize(q.n);
     std::unordered_map<const Composition*, uint32_t> index;
     uint64_t order_sum = 0;
-    for (uint32_t c = 0; c < n; ++c) {
-        if (!comps[c]) {
+    for (uint32_t c = 0; c < q.n; ++c) {
+        if (!q.batch[c]) {
             set_error("batch entry %u is null", c);
             return FORMA_STATUS_INVALID;
         }
-        auto it = index.emplace(comps[c], (uint32_t)batch_distinct.size()).first;
+        auto it = index.emplace(q.batch[c], (uint32_t)batch_distinct.size()).first;
         batch_slot[c] = it->second;
         if (it->second < batch_distinct.size()) continue;
-        batch_distinct.push_back(comps[c]);
-        const auto& layers = comps[c]->layers;
+        batch_distinct.push_back(q.batch[c]);
+        const auto& layers = q.batch[c]->layers;
         order_sum += layers.empty() ? 0u : (uint64_t)layers.rbegin()->first + 1u;
     }
     if (order_sum > (1ull << 21)) {
@@ -619,11 +598,10 @@ int Renderer::render_batch(Composition* const* comps, uint32_t n, uint8_t* buffe
                   (unsigned long long)order_sum, 1u << 21);
         return FORMA_STATUS_ORDER;
     }
-    FrameStack K{buffer, buffer_on_device, width, stride, height, frame_stride, n};
-    return run_stack(nullptr, FrameSpec{nullptr, false, nullptr, n, (uint32_t)height, comps}, K, ids, channels, clear, timings);
+    return FORMA_STATUS_OK;
 }
 
-// Every distinct composition of the batch (batch_distinct, as render_batch found them) is uploaded
+// Every distinct composition of the batch (batch_distinct, as check_request found them) is uploaded
 // (tables, then all of its geometry), in the order of first appearance, and gets its slices:
 // orders from order_base, style slots, stops and texels from their bases, each the sum of the
 // counts of the compositions before it. The batch tables are gathered from the compositions'
@@ -717,142 +695,63 @@ int Renderer::bind_batch(Composition* const* comps, uint32_t n, PaintScene& S, u
     return FORMA_STATUS_OK;
 }
 
-// The checks of a stack of n frames of width x height pixels, frame_stride bytes apart.
-int Renderer::check_stack(const char* what, uint32_t n, uint64_t width, uint64_t stride, uint64_t height, uint64_t frame_stride,
-                          const uint8_t* buffer) {
-    if (!buffer || width == 0 || height == 0 || width * 4 > stride || width > FORMA_MAX_WIDTH || height > FORMA_MAX_HEIGHT) {
-        set_error("invalid render target %llux%llu stride %llu", (unsigned long long)width, (unsigned long long)height,
-                  (unsigned long long)stride);
-        return FORMA_STATUS_INVALID;
+// The frame's kernels: paint() for the RGBA target (in copy bands, or with the rows of a stack's
+// frames), then the ID kernel for the ID target. The sync-free redo repeats both.
+int Renderer::paint_step(const FrameRequest& q, const PaintScene& S, const FramePlan& p, const uint32_t* heavy_lists,
+                         uint32_t* paint_launches) {
+    if (q.rgba.ptr) {
+        const int st = paint(S, p.rgba.ptr, q.rgba.ptr, q.rgba.stride, p.in_bands, heavy_lists, paint_launches, p.rows);
+        if (st || !q.ids.ptr) return st;
+        ++*paint_launches;
     }
-    if (n == 0 || n > max_views(height)) {
-        set_error("%u %ss of height %llu: between 1 and %u %ss of this height fit in one call", n, what, (unsigned long long)height,
-                  max_views(height), what);
-        return FORMA_STATUS_INVALID;
-    }
-    if (frame_stride < (height - 1u) * stride + 4u * width) {
-        set_error("%s stride %llu is smaller than one %s (%llu bytes)", what, (unsigned long long)frame_stride, what,
-                  (unsigned long long)((height - 1u) * stride + 4u * width));
-        return FORMA_STATUS_INVALID;
-    }
+    // A batch's entries carry each frame's order base (bind_batch): the kernel takes it off.
+    FORMA_CUDA_TRY(id_flags.reserve(std::max<size_t>(recs.capacity, 1)));
+    launch_paint_ids(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), id_flags.ptr, reinterpret_cast<uint32_t*>(p.ids.ptr),
+                     p.ids.stride, q.ids.min_coverage, totals.ptr + 8, stream, p.rows,
+                     q.kind == FrameKind::batch ? reinterpret_cast<const BatchFrame*>(d_batch_lines.ptr) : nullptr);
+    ++launches;
+    FORMA_CUDA_TRY(cudaGetLastError());
     return FORMA_STATUS_OK;
 }
 
-// The checks of a stacked call's targets: the RGBA stack (absent when there is an ID stack and no
-// buffer), then the ID stack. args: the call's views / compositions are there.
-int Renderer::check_stacks(const char* what, bool args, uint32_t n, uint64_t width, uint64_t height, const uint8_t* buffer,
-                           uint64_t stride, uint64_t frame_stride, const IdStack* ids) {
-    if (buffer || !ids) {
-        const int st = check_stack(what, n, width, stride, height, frame_stride, args ? buffer : nullptr);
-        if (st) return st;
-    }
-    if (!ids) return FORMA_STATUS_OK;
-    if (ids->stride % 4u != 0u || ids->frame_stride % 4u != 0u || !std::isfinite(ids->min_coverage) || ids->min_coverage < 0.0f ||
-        ids->min_coverage >= 1.0f) {
-        set_error("invalid ID frames: stride %llu, %s stride %llu (multiples of 4 bytes), min_coverage %g (finite, in [0, 1))",
-                  (unsigned long long)ids->stride, what, (unsigned long long)ids->frame_stride, (double)ids->min_coverage);
-        return FORMA_STATUS_INVALID;
-    }
-    return check_stack(what, n, width, ids->stride, height, ids->frame_stride, args ? reinterpret_cast<const uint8_t*>(ids->ids) : nullptr);
-}
-
-// The stacked frame's PaintScene (that of the RGBA stack K, or of the ID stack I when there is no
-// K) and the device frame of each stack. Frames whose rows are whole tile rows, laid out as the
-// stacked frame's rows, are painted in place; each stack decides for itself.
-int Renderer::begin_stack(FrameStack* K, FrameStack* I, PaintScene& S, const uint32_t channels[4], const float clear[4]) {
-    static const uint32_t kIdChannels[4] = {0, 1, 2, 3};
-    static const float kIdClear[4] = {0, 0, 0, 0};
-    for (FrameStack* k : {K, I}) {
-        if (!k) continue;
-        k->rows = (uint32_t)((k->height + 15u) / 16u);
-        k->direct = k->on_device && k->height % 16u == 0u && k->frame_stride == k->height * k->stride;
-        k->fb_stride = k->direct ? k->stride : 4u * k->width;
-        k->fb = k->buffer;
-    }
-    const FrameStack& M = K ? *K : *I;
-    const int st = begin_frame(S, M.buffer, M.width, M.fb_stride, (uint64_t)M.n * M.rows * 16u, K ? channels : kIdChannels,
-                               K ? clear : kIdClear, nullptr);
-    if (st) return st;
-    if (K && !K->direct) {
-        FORMA_CUDA_TRY(framebuffer.reserve((size_t)K->fb_stride * S.height));
-        K->fb = framebuffer.ptr;
-    }
-    if (I && !I->direct) {
-        FORMA_CUDA_TRY(id_frame.reserve((size_t)(I->fb_stride / 4u) * S.height));
-        I->fb = reinterpret_cast<uint8_t*>(id_frame.ptr);
-    }
-    return FORMA_STATUS_OK;
-}
-
-// A stacked frame through run_frame: the RGBA stack K (K.buffer null: none), the ID stack `ids`
-// (null: none), or both from one set of tables, the paint kernel and then the ID kernel. The
-// sync-free redo repeats the kernels and the output of both stacks.
-int Renderer::run_stack(Composition* comp, const FrameSpec& spec, FrameStack& K, const IdStack* ids, const uint32_t channels[4],
-                        const float clear[4], forma_timings* timings) {
-    const bool rgba = K.buffer != nullptr;
-    FrameStack I{};
-    if (ids) I = FrameStack{reinterpret_cast<uint8_t*>(ids->ids), ids->on_device, K.width, ids->stride, K.height, ids->frame_stride, K.n};
-    PaintScene S{};
-    const int st = begin_stack(rgba ? &K : nullptr, ids ? &I : nullptr, S, channels, clear);
-    if (st) return st;
-    return run_frame(
-        comp, S, spec, timings,
-        [&](const uint32_t* heavy_lists, uint32_t* paint_launches) {
-            if (rgba) {
-                const int st = paint(S, K.fb, K.fb, K.fb_stride, false, heavy_lists, paint_launches, K.rows);
-                if (st || !ids) return st;
-                ++*paint_launches;
-            }
-            // A batch's entries carry each frame's order base (bind_batch): the kernel takes it off.
-            FORMA_CUDA_TRY(id_flags.reserve(std::max<size_t>(recs.capacity, 1)));
-            launch_paint_ids(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), id_flags.ptr,
-                             reinterpret_cast<uint32_t*>(I.fb), I.fb_stride, ids->min_coverage, totals.ptr + 8, stream, I.rows,
-                             spec.batch ? reinterpret_cast<const BatchFrame*>(d_batch_lines.ptr) : nullptr);
+// Moves every target's frames from the device frame to the caller's buffer: only the written
+// tiles of a cached host frame, the crop's tile rectangle of a single host frame, and for a stack
+// repack_views_kernel into another device layout or one copy per frame to a host buffer. Nothing
+// for a frame painted in place or copied back band by band.
+int Renderer::output_step(const FrameRequest& q, const PaintScene& S, const FramePlan& p) {
+    if (p.pack_written) return scatter_written_tiles(S, p.rgba.ptr, q.rgba.ptr, q.rgba.stride);
+    auto output = [&](const FrameTarget& t, const DeviceFrame& f) {
+        if (!t.ptr || f.direct) return (int)FORMA_STATUS_OK;
+        if (!p.rows) return copy_to_host(S, t.ptr, f.ptr, t.stride, stream);
+        const uint32_t height = (uint32_t)q.height;
+        if (t.on_device) {
+            launch_repack_views(f.ptr, f.stride, p.rows * 16u, t.ptr, t.stride, t.frame_stride, S.width, height, q.n, stream);
             ++launches;
             FORMA_CUDA_TRY(cudaGetLastError());
             return (int)FORMA_STATUS_OK;
-        },
-        [&] {
-            const int st = rgba ? output_stack(K, S) : FORMA_STATUS_OK;
-            return st || !ids ? st : output_stack(I, S);
-        });
-}
-
-// Moves the frames of a stack painted into K.fb to the caller's buffer: nothing to do in place,
-// repack_views_kernel into another device layout, or one copy per frame to a host buffer.
-int Renderer::output_stack(const FrameStack& K, const PaintScene& S) {
-    if (K.on_device && !K.direct) {
-        launch_repack_views(K.fb, K.fb_stride, K.rows * 16u, K.buffer, K.stride, K.frame_stride, S.width, (uint32_t)K.height, K.n,
-                            stream);
-        ++launches;
-        FORMA_CUDA_TRY(cudaGetLastError());
-    } else if (!K.on_device) {
+        }
         // Rows [0, height) of every frame, one copy per frame with the pitches copy_to_host uses
         // for a single frame (a copy over all frames would have a frame as its pitch, which can
         // exceed the device's largest pitch).
-        for (uint32_t b = 0; b < K.n; ++b) {
-            uint8_t* dst = K.buffer + (size_t)b * K.frame_stride;
-            const uint8_t* src = K.fb + (size_t)b * K.rows * 16u * K.fb_stride;
-            if (K.stride == K.fb_stride)
-                FORMA_CUDA_TRY(cudaMemcpyAsync(dst, src, (K.height - 1u) * K.stride + 4u * K.width, cudaMemcpyDeviceToHost, stream));
+        for (uint32_t b = 0; b < q.n; ++b) {
+            uint8_t* dst = t.ptr + (size_t)b * t.frame_stride;
+            const uint8_t* src = f.ptr + (size_t)b * p.rows * 16u * f.stride;
+            if (t.stride == f.stride)
+                FORMA_CUDA_TRY(cudaMemcpyAsync(dst, src, (height - 1u) * t.stride + 4u * q.width, cudaMemcpyDeviceToHost, stream));
             else
-                FORMA_CUDA_TRY(
-                    cudaMemcpy2DAsync(dst, K.stride, src, K.fb_stride, 4u * K.width, K.height, cudaMemcpyDeviceToHost, stream));
+                FORMA_CUDA_TRY(cudaMemcpy2DAsync(dst, t.stride, src, f.stride, 4u * q.width, height, cudaMemcpyDeviceToHost, stream));
         }
-        d2h_bytes += (uint64_t)K.n * K.height * K.width * 4u;
-    }
-    return FORMA_STATUS_OK;
+        d2h_bytes += (uint64_t)q.n * height * q.width * 4u;
+        return (int)FORMA_STATUS_OK;
+    };
+    const int st = p.in_bands ? FORMA_STATUS_OK : output(q.rgba, p.rgba);
+    return st ? st : output(q.ids, p.ids);
 }
 
-// LinearLayout::new asserts (layout/mod.rs:188-193) + consts.rs limits, and the frame's PaintScene
-// without its composition tables: target, channels, clear colour and the tile rectangle of the crop.
-int Renderer::begin_frame(PaintScene& S, const uint8_t* buffer, uint64_t width, uint64_t stride, uint64_t height,
-                          const uint32_t channels_in[4], const float clear[4], const forma_rect* crop) {
-    if (!buffer || width == 0 || height == 0 || width * 4 > stride || width > FORMA_MAX_WIDTH || height > FORMA_MAX_HEIGHT) {
-        set_error("invalid render target %llux%llu stride %llu", (unsigned long long)width, (unsigned long long)height,
-                  (unsigned long long)stride);
-        return FORMA_STATUS_INVALID;
-    }
+// The frame's PaintScene without its composition tables, for a target that check_request
+// accepted: size, channels, clear colour and the tile rectangle of the crop.
+int Renderer::begin_frame(PaintScene& S, uint64_t width, uint64_t stride, uint64_t height, const uint32_t channels_in[4],
+                          const float clear[4], const forma_rect* crop) {
     FORMA_CUDA_TRY(cudaSetDevice(device));
     last_slices = 0;
     const int ts = ensure_timer();

@@ -37,36 +37,56 @@ struct Timer {
     bool ok = false;
 };
 
-// What differs between the frame kinds before painting (see Renderer::run_frame).
-struct FrameSpec {
-    LayerCache* cache = nullptr;
-    bool pack_written = false;     // only the tiles the frame writes travel back (scatter_written_tiles)
-    const float* views = nullptr;  // render_views: n_frames transforms of the composition
-    uint32_t n_frames = 0, frame_height = 0;  // stacked frames (views or a batch) of frame_height rows; 0: one frame
-    Composition* const* batch = nullptr;      // render_batch: n_frames compositions, one per frame
+// A target of a FrameRequest: 4-byte pixels, RGBA8 or the layer IDs of ID frames (see
+// forma_renderer_render_ids). Row r of frame b at ptr + b * frame_stride + r * stride
+// (frame_stride: stacks only).
+struct FrameTarget {
+    uint8_t* ptr = nullptr;  // null: the request has no such target
+    bool on_device = false;
+    uint64_t stride = 0, frame_stride = 0;
+    float min_coverage = 0.0f;  // the ID target
 };
 
-// A stack of n frames of width x height pixels (views, batches) in `buffer`: frame b at
-// b * frame_stride, row r of it at + r * stride. The device frame stacks them by tile rows
-// (rows = ceil(height / 16) each) in `fb`, rows fb_stride bytes apart: `buffer` itself when the
-// layouts agree (direct), the renderer's framebuffer otherwise.
-struct FrameStack {
-    uint8_t* buffer;
-    bool on_device;
-    uint64_t width, stride, height, frame_stride;
-    uint32_t n, rows;
+// What a FrameRequest renders. single: one frame of a composition. views: n views of one
+// composition in one pass, stacked top to bottom as one frame of n * ceil(height / 16) tile rows;
+// line setup rasterizes every view in its own coordinates and moves its segments' tile rows to the
+// view's place in the stack (ViewArgs), and the tables, the sort and the painter see one frame.
+// batch: n compositions, one frame each, stacked as views are; frame c's line setup reads
+// comps[c]'s segment buffer and moves its segments' layers to the composition's slice of the
+// layer field (bind_batch), so that the batch tables serve every frame, and frame c's IDs are
+// comps[c]'s own orders. A stack takes no layer cache and no band filter: every composition is
+// resident whole.
+enum class FrameKind { single, views, batch };
+
+// One call of Renderer::render: what is rendered, the size of one frame, and its targets: an
+// RGBA target, an ID target (channels {0, 1, 2, 3}, clear colour 0 when it is alone) or both.
+struct FrameRequest {
+    FrameKind kind = FrameKind::single;
+    uint32_t n = 0;  // stacks: the frames
+    uint64_t width = 0, height = 0;
+    const uint32_t* channels = nullptr;  // of the RGBA target
+    const float* clear = nullptr;
+    forma_timings* timings = nullptr;
+    const forma_rect* crop = nullptr;  // single frames only
+    LayerCache* cache = nullptr;       // single RGBA frames only
+    FrameTarget rgba, ids;
+    Composition* comp = nullptr;          // single, views
+    const float* views = nullptr;         // views: n transforms [ux, vx, uy, vy, tx, ty]
+    Composition* const* batch = nullptr;  // batch: n compositions (null entries are refused)
+};
+
+// Where Renderer::render paints a request's targets: per target the frame on the device (the
+// caller's buffer when `direct`, the renderer's scratch otherwise) and its row stride.
+struct DeviceFrame {
+    uint8_t* ptr;
+    uint64_t stride;
     bool direct;
-    uint8_t* fb;
-    uint64_t fb_stride;
 };
-
-// The ID frames of a stacked call (render_views / render_batch): frame b's words at
-// b * frame_stride bytes of `ids`, rows `stride` bytes apart.
-struct IdStack {
-    uint32_t* ids;
-    bool on_device;
-    uint64_t stride, frame_stride;
-    float min_coverage;
+struct FramePlan {
+    DeviceFrame rgba, ids;
+    uint32_t rows;      // stacks: tile rows of each frame; 0: a single frame
+    bool in_bands;      // a single host RGBA frame painted and copied back band by band (see paint)
+    bool pack_written;  // a cached host frame: only the tiles it writes travel back (scatter_written_tiles)
 };
 
 // The line setup of a batch (see Renderer::bind_batch).
@@ -249,43 +269,29 @@ class Renderer {
     int flush_geometry(Composition& comp, float band_lo = 0.0f, float band_hi = 0.0f, bool band_is_partial = false);
     int upload_tables(Composition& comp, int64_t cache_id);
     int upload_tables_device(Composition& comp, CompDevice& cd);
-    // views / n_views: the line setup of render_views (a stacked frame of n_views views); batch:
-    // that of render_batch (comp is then null).
+    // views / n_views: the line setup of a views request (a stacked frame of n_views views); batch:
+    // that of a batch request (comp is then null).
     int rasterize(Composition* comp, uint32_t width, uint32_t height, float band_lo, float band_hi, uint32_t* n_out,
                   const ViewArgs* views = nullptr, uint32_t n_views = 0, const BatchLines* batch = nullptr);
-    // Every frame kind runs through run_frame (renderer.cu, its only instantiations): FrameSpec says
-    // what differs before painting, paint_step and output_step what differs after the tables.
-    // comp is null for a batch (spec.batch).
-    template <class Paint, class Output>
-    int run_frame(Composition* comp, PaintScene& S, const FrameSpec& spec, forma_timings* timings, Paint&& paint_step,
-                  Output&& output_step);
-    int render(Composition& comp, uint8_t* buffer, bool buffer_on_device, uint64_t width, uint64_t stride,
-               uint64_t height, const uint32_t channels[4], const float clear[4], const forma_rect* crop,
-               LayerCache* cache, forma_timings* timings);
-    // ID frames (see forma_renderer_render_ids): a frame without a layer cache, with the ID kernel
-    // in place of paint() or, when `rgba` (a device frame) is given, after it.
+    // Every frame, whatever its kind and targets: check_request, the PaintScene (begin_frame), each
+    // target's device frame, run_frame and, for a layer cache, its bookkeeping.
+    int render(const FrameRequest& q);
+    int check_request(const FrameRequest& q);
+    // One frame of S: uploads, line setup, sort, then the painter tables, paint_step and
+    // output_step once or, when the sync-free bounds were too small, twice.
+    int run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p);
+    int paint_step(const FrameRequest& q, const PaintScene& S, const FramePlan& p, const uint32_t* heavy_lists,
+                   uint32_t* paint_launches);
+    int output_step(const FrameRequest& q, const PaintScene& S, const FramePlan& p);
     DeviceBuffer<uint8_t> id_flags;   // per entry: the ID kernel's optimizer flags (clip tiles)
-    DeviceBuffer<uint32_t> id_frame;  // host ID frames: the frame on the device
-    int render_ids(Composition& comp, uint8_t* rgba, uint64_t rgba_stride, const uint32_t channels[4], const float clear[4],
-                   uint32_t* ids, bool ids_on_device, uint64_t width, uint64_t ids_stride, uint64_t height,
-                   const forma_rect* crop, float min_coverage, forma_timings* timings);
-    // n views of one composition in one pass (see forma_renderer_render_views_device): a frame of
-    // n * ceil(height / 16) tile rows, painted straight into a device buffer whose views are its
-    // rows, or into `framebuffer` and copied out view by view. With `ids`, the views' ID frames
-    // from the same tables (forma_renderer_render_views_ids_device); `buffer` may then be null
-    // (no RGBA frames; stride, view_stride, channels and clear are not read).
+    DeviceBuffer<uint32_t> id_frame;  // the ID target's scratch frame
     PinnedBuffer<float> h_views;
     DeviceBuffer<float> d_views;
-    int render_views(Composition& comp, const float* views, uint32_t n, uint8_t* buffer, bool buffer_on_device, uint64_t width,
-                     uint64_t stride, uint64_t height, uint64_t view_stride, const uint32_t channels[4], const float clear[4],
-                     forma_timings* timings, const IdStack* ids = nullptr);
-    // A batch of n compositions, one frame each, in one pass (see forma_renderer_render_batch_device):
-    // the stacked frame of the views, every frame with its own composition. The distinct
-    // compositions' tables are gathered into the batch tables below, which are kept until a batch
-    // of other compositions or other table versions comes (batch_key).
+    // A batch's distinct compositions' tables are gathered into the batch tables below, which are
+    // kept until a batch of other compositions or other table versions comes (batch_key).
     std::vector<std::pair<uint64_t, uint64_t>> batch_key;  // (Composition::serial, tables_version) of the distinct compositions
     std::vector<std::pair<uint64_t, uint64_t>> batch_key_next;
-    std::vector<Composition*> batch_distinct;  // of the current call, in order of first appearance (render_batch)
+    std::vector<Composition*> batch_distinct;  // of the current call, in order of first appearance (check_request)
     std::vector<uint32_t> batch_slot;          // per frame: its composition's index in batch_distinct
     PinnedBuffer<uint8_t> h_batch_lines;  // BatchFrame per frame, then cta_first
     DeviceBuffer<uint8_t> d_batch_lines;
@@ -296,27 +302,10 @@ class Renderer {
     DeviceBuffer<GradRec> batch_grads;
     DeviceBuffer<StopRec> batch_stops;
     DeviceBuffer<uint16_t> batch_texels;
-    // `ids`: as for render_views; the IDs of frame c are comps[c]'s own orders.
-    int render_batch(Composition* const* comps, uint32_t n, uint8_t* buffer, bool buffer_on_device, uint64_t width, uint64_t stride,
-                     uint64_t height, uint64_t frame_stride, const uint32_t channels[4], const float clear[4], forma_timings* timings,
-                     const IdStack* ids = nullptr);
     int bind_batch(Composition* const* comps, uint32_t n, PaintScene& S, uint32_t height, BatchLines& lines);
-    // Stacked frames (views, batches): the checks of the targets (the RGBA stack, the ID stack or
-    // both), then the PaintScene and the device frames, the frame itself (run_stack: run_frame with
-    // the paint and / or ID kernel) and the output step that moves a stack's frames to where the
-    // caller wants them. A stack is 4-byte pixels either way: RGBA8 with `framebuffer` as its
-    // scratch, ID words with `id_frame`.
-    int check_stack(const char* what, uint32_t n, uint64_t width, uint64_t stride, uint64_t height, uint64_t frame_stride,
-                    const uint8_t* buffer);
-    int check_stacks(const char* what, bool args, uint32_t n, uint64_t width, uint64_t height, const uint8_t* buffer, uint64_t stride,
-                     uint64_t frame_stride, const IdStack* ids);
-    int begin_stack(FrameStack* K, FrameStack* I, PaintScene& S, const uint32_t channels[4], const float clear[4]);
-    int run_stack(Composition* comp, const FrameSpec& spec, FrameStack& K, const IdStack* ids, const uint32_t channels[4],
-                  const float clear[4], forma_timings* timings);
-    int output_stack(const FrameStack& K, const PaintScene& S);
-    // The stages of a frame, in the order they run: begin_frame in the entry points, the rest in run_frame.
-    int begin_frame(PaintScene& S, const uint8_t* buffer, uint64_t width, uint64_t stride, uint64_t height,
-                    const uint32_t channels[4], const float clear[4], const forma_rect* crop);
+    // The stages of a frame, in the order they run: begin_frame in render, the rest in run_frame.
+    int begin_frame(PaintScene& S, uint64_t width, uint64_t stride, uint64_t height, const uint32_t channels[4],
+                    const float clear[4], const forma_rect* crop);
     int bind_frame(Composition& comp, PaintScene& S, LayerCache* cache, const float clear[4], bool pack_written);
     int build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint32_t prev_cells, uint32_t prev_gaps, uint32_t* heavy_lists,
                      DevCounts& dc);
@@ -332,7 +321,7 @@ class Renderer {
 struct TileRect {
     uint32_t tx_lo, tx_hi, ty_lo, ty_hi;
 };
-// The most views of `height` rows one render_views call takes: the stacked frame's tile rows
+// The most views of `height` rows one views request takes: the stacked frame's tile rows
 // are the biased rows 1 ... n * rows of the 11-bit tile_y field, and the painter tables' sentinel
 // row (tiles_y + 1, see sentinel_key) must fit in it too: n * rows <= 2046.
 inline uint32_t max_views(uint64_t height) {
@@ -387,8 +376,6 @@ struct forma_renderer {
     ~forma_renderer() { forma_renderer_multi_free(slicer); }
 };
 
-// Host-frame pipeline (multi_renderer.cu): returns -1 when the frame is
-// not sliced and the plain path has to render it.
-int sliced_host_render(forma_renderer* r, forma_composition* c, uint8_t* buffer, uint64_t width, uint64_t stride,
-                       uint64_t height, const uint32_t channels[4], const float clear[4], const forma_rect* crop,
-                       forma_timings* timings);
+// Host-frame pipeline (multi_renderer.cu) of a single host RGBA frame without a layer cache:
+// returns -1 when the frame is not sliced and the plain path has to render it.
+int sliced_host_render(forma_renderer* r, const forma::FrameRequest& q);
