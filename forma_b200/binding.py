@@ -318,6 +318,9 @@ SIGNATURES = {
     "renderer_segments": (C.c_uint64, [_vp, C.c_uint64, _u64p]),
     "renderer_rasterize_only": (C.c_uint64, [_vp, _vp, C.c_uint64, C.c_uint64, C.c_uint64, _u64p]),
     "renderer_sort_u64": (C.c_int, [_vp, _u64p, C.c_uint64]),
+    "debug_sort_plan": (C.c_int, [C.c_int, _u64p, _u8p]),
+    "renderer_sort_pairs": (C.c_int, [_vp, C.c_int, C.c_int, _u64p, _u32p, C.c_uint64, C.c_uint64]),
+    "renderer_sort_bounds": (None, [_vp, _u64p]),
     "debug_selftest": (C.c_int, [C.c_int, _u64p]),
     "renderer_multi_new": (_vp, [C.POINTER(C.c_int), C.c_int]),
     "renderer_multi_free": (None, [_vp]),
@@ -344,7 +347,11 @@ STACK_ID_SYMBOLS = ("renderer_render_views_ids", "renderer_render_views_ids_devi
                     "renderer_render_batch_ids_device")
 
 
-_OPTIONAL_SYMBOLS = frozenset(ID_FRAME_SYMBOLS + VIEW_SYMBOLS + BATCH_SYMBOLS + STACK_ID_SYMBOLS)
+# The same for the inspection entry points of the sort (sort_plan, Renderer.sort_pairs, sort_bounds).
+SORT_DEBUG_SYMBOLS = ("debug_sort_plan", "renderer_sort_pairs", "renderer_sort_bounds")
+
+
+_OPTIONAL_SYMBOLS = frozenset(ID_FRAME_SYMBOLS + VIEW_SYMBOLS + BATCH_SYMBOLS + STACK_ID_SYMBOLS + SORT_DEBUG_SYMBOLS)
 
 
 class Api:
@@ -387,6 +394,15 @@ class Api:
         v = C.c_int(0)
         self.check(self.__dict__["get_option_fn"](name.encode(), C.byref(v)), f"get_option({name})")
         return int(v.value)
+
+    def sort_plan(self, layout: int, bound: Sequence[int]) -> bytes:
+        """The library's sort plan for the field bounds `bound` (least significant field first)
+        under layout 0 (segments) or 1 (carry keys): n_passes, total_bits, then 10 bytes per pass
+        (shift[3], width[3], lsh[3], bits). No device is touched."""
+        b = (C.c_uint64 * 3)(*[int(v) for v in bound])
+        out = (C.c_uint8 * 62)()
+        self.check(self.debug_sort_plan(layout, b, out), "sort_plan")
+        return bytes(out)
 
     # Constructors bound to this library -----------------------------------
     def PathBuilder(self) -> "PathBuilder":
@@ -1039,6 +1055,27 @@ class Renderer:
         out = np.ascontiguousarray(keys, dtype=np.uint64).copy()
         self._api.check(self._api.renderer_sort_u64(self._h, out.ctypes.data_as(_u64p), out.size), "sort_u64")
         return out
+
+    def sort_pairs(self, keys: np.ndarray, vals: np.ndarray, layout: int = 0, mode: int = 0, count: Optional[int] = None,
+                   cap: int = 0):
+        """(keys, vals) sorted by the single-sweep pair passes (forma_renderer_sort_pairs).
+        mode bit 0: `count` (default: len(keys)) goes to the kernels in device memory with `cap`
+        as its bound; bit 1: the digit histogram is counted before the sort and passed in."""
+        k = np.ascontiguousarray(keys, dtype=np.uint64).copy()
+        v = np.ascontiguousarray(vals, dtype=np.uint32).copy()
+        count = k.size if count is None else int(count)
+        held = min(count, cap) if mode & 1 else count
+        if k.size != held or v.size != held:
+            raise ValueError(f"sort_pairs: {k.size} keys and {v.size} values for {held} elements")
+        self._api.check(self._api.renderer_sort_pairs(self._h, layout, mode, k.ctypes.data_as(_u64p), v.ctypes.data_as(_u32p),
+                                                      count, cap), "sort_pairs")
+        return k, v
+
+    def sort_bounds(self) -> dict:
+        """The field bounds and bit count of the last frame's segment sort plan."""
+        out = (C.c_uint64 * 4)()
+        self._api.renderer_sort_bounds(self._h, out)
+        return dict(zip(("layer", "tile_x", "tile_y", "total_bits"), [int(x) for x in out]))
 
     def __del__(self):
         try:

@@ -749,5 +749,72 @@ int forma_renderer_sort_u64(forma_renderer* r, uint64_t* keys, uint64_t n) {
     FORMA_CUDA_TRY(cudaStreamSynchronize(R.stream));
     return FORMA_OK;
 }
+int forma_debug_sort_plan(int layout, const uint64_t bound[3], uint8_t out[2 + 10 * kMaxSortPasses]) {
+    if (layout != 0 && layout != 1) {
+        set_error("sort_plan: layout %d is neither 0 (segments) nor 1 (carry)", layout);
+        return FORMA_ERR_INVALID_ARGUMENT;
+    }
+    const SortPlan plan = make_sort_plan(layout ? carry_key_layout() : segment_key_layout(), bound);
+    out[0] = (uint8_t)plan.n_passes;
+    out[1] = (uint8_t)plan.total_bits;
+    static_assert(sizeof(DigitSpec) == 10, "shift[3], width[3], lsh[3], bits");
+    std::memcpy(out + 2, plan.pass, sizeof(plan.pass));
+    return FORMA_OK;
+}
+void forma_renderer_sort_bounds(const forma_renderer* r, uint64_t out[4]) {
+    for (int f = 0; f < 3; ++f) out[f] = r->r.segment_bound[f];
+    out[3] = r->r.segment_plan.total_bits;
+}
+int forma_renderer_sort_pairs(forma_renderer* r, int layout, int mode, uint64_t* keys, uint32_t* vals, uint64_t count,
+                              uint64_t cap) {
+    Renderer& R = r->r;
+    const bool dev_count = (mode & 1) != 0, hist_ready = (mode & 2) != 0;
+    if ((layout != 0 && layout != 1) || (mode & ~3)) {
+        set_error("sort_pairs: layout %d / mode %d", layout, mode);
+        return FORMA_ERR_INVALID_ARGUMENT;
+    }
+    if (count >= (1ull << 30) || (dev_count && cap >= (1ull << 30))) {
+        set_error("sort_pairs: n too large");
+        return FORMA_ERR_CAPACITY;
+    }
+    const uint32_t n = (uint32_t)(dev_count ? cap : count);    // what the launches are sized by
+    const uint64_t held = dev_count ? std::min(count, cap) : count;  // elements of keys / vals
+    if (n < 2 || held == 0) return FORMA_OK;
+    FORMA_CUDA_TRY(cudaSetDevice(R.device));
+    const KeyLayout lay = layout ? carry_key_layout() : segment_key_layout();
+    uint64_t all = 0, bound[3];
+    for (uint64_t i = 0; i < held; ++i) all |= keys[i];
+    for (int f = 0; f < 3; ++f) bound[f] = (all >> lay.pos[f]) & ((1ull << lay.maxw[f]) - 1u);
+    const SortPlan plan = make_sort_plan(lay, bound);
+    // Scratch: the count | (hist_ready) hist[kMaxSortPasses][256], then the zeroed look-back block |
+    // (otherwise) the sort's own scratch, which it zeroes itself.
+    const size_t hist_bytes = (size_t)kMaxSortPasses * 256 * sizeof(uint32_t);
+    const size_t work = hist_ready ? hist_bytes + sort_lookback_bytes(n, plan) : radix_scratch_bytes(n);
+    FORMA_CUDA_TRY(R.sort_scratch.reserve(256 + work));
+    FORMA_CUDA_TRY(Renderer::reserve_all((size_t)n + 1, R.key2, R.key2_tmp, R.perm, R.perm_tmp));
+    uint32_t* d_count = reinterpret_cast<uint32_t*>(R.sort_scratch.ptr);
+    uint8_t* d_work = R.sort_scratch.ptr + 256;
+    const uint32_t count32 = (uint32_t)count;
+    FORMA_CUDA_TRY(cudaMemcpyAsync(d_count, &count32, sizeof(uint32_t), cudaMemcpyHostToDevice, R.stream));
+    FORMA_CUDA_TRY(cudaMemcpyAsync(R.key2.ptr, keys, held * sizeof(uint64_t), cudaMemcpyHostToDevice, R.stream));
+    FORMA_CUDA_TRY(cudaMemcpyAsync(R.perm.ptr, vals, held * sizeof(uint32_t), cudaMemcpyHostToDevice, R.stream));
+    const uint32_t* n_dev = dev_count ? d_count : nullptr;
+    const uint32_t* hist = nullptr;
+    if (hist_ready) {
+        FORMA_CUDA_TRY(cudaMemsetAsync(d_work, 0, work, R.stream));
+        launch_radix_hist(R.key2.ptr, n, plan, reinterpret_cast<uint32_t*>(d_work), n_dev, R.stream);
+        hist = reinterpret_cast<const uint32_t*>(d_work);
+    }
+    // A refused sort (count > cap) leaves its input where it was, whichever buffer the passes end in.
+    const bool refused = dev_count && count > cap;
+    const uint64_t* in_keys = R.key2.ptr;
+    const uint32_t* in_vals = R.perm.ptr;
+    R.sort(R.key2, R.key2_tmp, &R.perm, &R.perm_tmp, n, plan, nullptr, n_dev, hist, hist_ready ? d_work + hist_bytes : d_work);
+    FORMA_CUDA_TRY(cudaGetLastError());
+    FORMA_CUDA_TRY(cudaMemcpyAsync(keys, refused ? in_keys : R.key2.ptr, held * sizeof(uint64_t), cudaMemcpyDeviceToHost, R.stream));
+    FORMA_CUDA_TRY(cudaMemcpyAsync(vals, refused ? in_vals : R.perm.ptr, held * sizeof(uint32_t), cudaMemcpyDeviceToHost, R.stream));
+    FORMA_CUDA_TRY(cudaStreamSynchronize(R.stream));
+    return FORMA_OK;
+}
 
 }  // extern "C"

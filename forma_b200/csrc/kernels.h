@@ -162,6 +162,9 @@ size_t radix_scratch_bytes(uint32_t n);
 // Scratch of a sort whose digit histogram comes from the kernel that wrote its keys (see
 // launch_radix_sort's `hist`): tile counters and look-back tables of the single-sweep passes.
 size_t sort_lookback_bytes(uint32_t n, const SortPlan& plan);
+// Adds the digit counts of every planned pass of keys[0, n) (n_dev: as below) to hist[kMaxSortPasses][256].
+void launch_radix_hist(const uint64_t* keys, uint32_t n, const SortPlan& plan, uint32_t* hist, const uint32_t* n_dev,
+                       cudaStream_t stream);
 SortResult launch_radix_sort(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals, uint32_t* vals_tmp, uint32_t n,
                              const SortPlan& plan, void* scratch, cudaStream_t stream,
                              cudaEvent_t* pass_events = nullptr /* 3 per pass: before upsweep, before / after downsweep */,

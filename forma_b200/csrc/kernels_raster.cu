@@ -340,6 +340,14 @@ __device__ __forceinline__ void line_count_body(const RasterArgs& A, const ViewA
                 // Tile columns left of -32767 wrap (int16, as in the reference) into the frame's
                 // columns: such a line can set any tile_x bit.
                 if (!(fminf(L.x0, L.x0 + L.dx) >= -8388352.0f)) bx = 4095;
+            } else {
+                // The same for the single frame, and for its rows: the skip rules drop a line only
+                // when both ends are above the frame, so a line with one end in the frame and the
+                // other above tile row -32767 survives, and its rows wrap into every value of the
+                // 11-bit field. (A stacked frame maps every row outside the view to 0 instead. Rows
+                // below the frame need no rule: from row 2045 on the clamp already gives 2047.)
+                if (!(fminf(L.x0, L.x0 + L.dx) >= -8388352.0f)) bx = 4095;
+                if (!(fminf(L.y0, L.y0 + L.dy) >= -8388352.0f)) by = 2047;
             }
         }
 #pragma unroll

@@ -553,6 +553,12 @@ size_t sort_lookback_bytes(uint32_t n, const SortPlan& plan) {
     return (8 + (size_t)plan.n_passes * tiles_for(n, items_for(n)) * kRadix) * sizeof(uint32_t);
 }
 
+void launch_radix_hist(const uint64_t* keys, uint32_t n, const SortPlan& plan, uint32_t* hist, const uint32_t* n_dev,
+                       cudaStream_t stream) {
+    uint32_t hist_blocks = min(tiles_for(n, 16) * 4u, (uint32_t)device_sm_count() * 8u);
+    radix_hist_kernel<<<hist_blocks, kSortThreads, 0, stream>>>(keys, n, plan, hist, n_dev);
+}
+
 template <bool kPairs, int kItems>
 static void launch_passes(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals, uint32_t* vals_tmp, uint32_t n,
                           const SortPlan& plan, const uint32_t* hist, uint32_t* lookback, uint32_t* counters, uint32_t tiles,
@@ -636,8 +642,7 @@ SortResult launch_radix_sort(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals,
         counters = h + kMaxSortPasses * kRadix;
         size_t total_words = (size_t)kMaxSortPasses * kRadix + 8 + (size_t)plan.n_passes * tiles * kRadix;
         cudaMemsetAsync(scratch, 0, total_words * sizeof(uint32_t), stream);
-        uint32_t hist_blocks = min(tiles_for(n, 16) * 4u, (uint32_t)device_sm_count() * 8u);
-        radix_hist_kernel<<<hist_blocks, kSortThreads, 0, stream>>>(keys, n, plan, h, n_dev);
+        launch_radix_hist(keys, n, plan, h, n_dev, stream);
         res.launches = 1;
         hist = h;
     }

@@ -307,6 +307,7 @@ int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, floa
                                                                                     : (comp->n_orders ? comp->n_orders - 1u : 0u);
         const uint64_t bound[3] = {layer_bound, pinned_totals[4], pinned_totals[5]};
         segment_plan = make_sort_plan(segment_key_layout(), bound);  // layer, tile_x, tile_y
+        std::copy(bound, bound + 3, segment_bound);
     }
     *n_out = 0;
     last_segments = 0;  // (forma_renderer_segments / _row_costs read segs[0, last_segments))

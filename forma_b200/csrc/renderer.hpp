@@ -112,6 +112,7 @@ class Renderer {
     // Per-frame device scratch (high-water-mark allocations).
     DeviceBuffer<uint32_t> block_sums, totals;
     SortPlan segment_plan{};  // digits of the main sort, from the bounds seen by the line-setup pass
+    uint64_t segment_bound[3] = {0, 0, 0};  // ... those bounds: layer, tile_x, tile_y (forma_renderer_sort_bounds)
 
     template <class T>
     static void swap_buffers(DeviceBuffer<T>& a, DeviceBuffer<T>& b) {

@@ -479,6 +479,24 @@ uint64_t forma_renderer_rasterize_only(forma_renderer*, forma_composition*, uint
 /* Stage 3 alone: sort `n` host keys on bits [20, 64) on the device
  * (replaces crumsort at cpu/rasterizer.rs:162-164). */
 int forma_renderer_sort_u64(forma_renderer*, uint64_t* keys, uint64_t n);
+/* The sort plan for `bound` (the largest value of each key field, least significant field first)
+ * under layout 0 (segments: layer | tile_x | tile_y) or 1 (the painter's carry keys: tile_x |
+ * layer | tile_y): out[0] = n_passes, out[1] = total_bits, then 10 bytes per pass (shift[3],
+ * width[3], lsh[3], bits); the bytes of unused passes are 0. Host only: no device. */
+int forma_debug_sort_plan(int layout, const uint64_t bound[3], uint8_t out[2 + 10 * 6]);
+/* Sorts (key, value) pairs with the single-sweep pair passes of the painter tables. layout: as
+ * above; the plan's bounds are taken from the OR of the keys.
+ * mode bit 0: the count is passed to the kernels in device memory and `cap` as its bound; keys /
+ *             vals then hold min(count, cap) elements. Without it `count` elements are sorted and
+ *             `cap` is ignored.
+ * mode bit 1: the digit histogram is counted before the sort and passed in, as a kernel that
+ *             writes the keys would.
+ * With bit 0 and count > cap nothing is sorted and keys / vals come back unchanged. */
+int forma_renderer_sort_pairs(forma_renderer*, int layout, int mode, uint64_t* keys, uint32_t* vals, uint64_t count,
+                              uint64_t cap);
+/* The bounds the last frame's segment sort was planned from: out[0..2] = layer, tile_x, tile_y
+ * (the largest value each field was taken to have), out[3] = the key bits the plan sorts. */
+void forma_renderer_sort_bounds(const forma_renderer*, uint64_t out[4]);
 
 #ifdef __cplusplus
 }

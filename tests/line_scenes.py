@@ -255,6 +255,20 @@ def _scenes() -> List[Scene]:
         LayerSpec(0, None, [[(10, 10), (20, 10), (20, 2 ** 20)]]),
         LayerSpec(1, None, [[(10, 20), (2 ** 20, 20), (2 ** 20, 40)]]),
     ], lambda rec: int(rec["counts"].total) > 2 ** 20))
+    # The same to the other side: one end in the frame, the other 2^20 px above or left of it. The
+    # skip rules keep such a line (only a line with both ends outside is dropped), and its tiles
+    # wrap through i16 into every value of the tile_y / tile_x field: the sort's plan must keep
+    # all of that field's bits although the frame itself needs two or three.
+    out.append(Scene("far_up", "a line from inside the frame to y ~ -2^20 px: tile rows wrap into all 11 bits", [
+        LayerSpec(0, None, [[(10, 20), (2 ** 20, 20), (10, -2 ** 20)]]),
+        LayerSpec(1, None, blob),
+    ], lambda rec: bool(np.any(rec["keep"] & (np.minimum(rec["y0"], rec["y0"] + rec["dy"]) < -32770 * 256.0)
+                               & (np.maximum(rec["y0"], rec["y0"] + rec["dy"]) > 0)))))
+    out.append(Scene("far_left_line", "a line from inside the frame to x ~ -2^20 px: tile columns wrap into all 12 bits", [
+        LayerSpec(0, None, [[(20, 10), (20, 2 ** 20), (-2 ** 20, 10)]]),
+        LayerSpec(1, None, blob),
+    ], lambda rec: bool(np.any(rec["keep"] & (np.minimum(rec["x0"], rec["x0"] + rec["dx"]) < -32770 * 256.0)
+                               & (np.maximum(rec["x0"], rec["x0"] + rec["dx"]) > 0)))))
     # Long lines: one line of ~6e6 segments has every segment of its CTA, the other 255 lines
     # (zig-zags above the frame or right of it) have none, at CTA positions 0 and 255 too.
     zig = [(1 + 0.01 * i, -1.0 - (i % 2)) for i in range(100)] + [(3.0e6, 3.0e6)]

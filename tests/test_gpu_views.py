@@ -129,7 +129,7 @@ def test_identity_view_equals_render_device(cuda_api, name):
 def test_composition_formula_device_against_device(cuda_api):
     """A view over layers with transforms T equals render_device with each layer's transform set
     to the model's C (device against device)."""
-    for name in ("straddle", "far_compose", "far_compose_neg", "far_points"):
+    for name in ("straddle", "far_compose", "far_compose_neg", "far_points", "far_left"):
         _device_against_device(cuda_api, vs.SCENES[name])
 
 
@@ -148,7 +148,7 @@ def _device_against_device(cuda_api, sc):
         assert np.array_equal(frames[b].reshape(-1), t.cpu().numpy()), f"{sc.name}: view {b}"
 
 
-@pytest.mark.parametrize("name", ["straddle", "straddle_h100", "far_compose", "far_points", "inf_points", "e2e_covers",
+@pytest.mark.parametrize("name", ["straddle", "straddle_h100", "far_compose", "far_points", "far_left", "inf_points", "e2e_covers",
                                   "extreme_crowd_64"])
 def test_view_segments_are_the_single_frames_moved(cuda_api, unsliced, name):
     import torch
