@@ -302,6 +302,18 @@ SIGNATURES = {
                                             C.POINTER(_CTimings)]),
     "renderer_render_batch_ids_device": (C.c_int, [_vp, C.POINTER(_vp), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64,
                                                    C.c_uint64, _u32p, _fp, _vp, C.c_uint64, C.c_uint64, _f, C.POINTER(_CTimings)]),
+    "renderer_render_linear": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CRect), C.c_uint32,
+                                         C.POINTER(_CTimings)]),
+    "renderer_render_linear_device": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CRect),
+                                                C.c_uint32, C.POINTER(_CTimings)]),
+    "renderer_render_views_linear": (C.c_int, [_vp, _vp, _fp, C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, _u32p,
+                                               _fp, C.c_uint32, C.POINTER(_CTimings)]),
+    "renderer_render_views_linear_device": (C.c_int, [_vp, _vp, _fp, C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
+                                                      _u32p, _fp, C.c_uint32, C.POINTER(_CTimings)]),
+    "renderer_render_batch_linear": (C.c_int, [_vp, C.POINTER(_vp), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
+                                               _u32p, _fp, C.c_uint32, C.POINTER(_CTimings)]),
+    "renderer_render_batch_linear_device": (C.c_int, [_vp, C.POINTER(_vp), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64,
+                                                      C.c_uint64, _u32p, _fp, C.c_uint32, C.POINTER(_CTimings)]),
     "renderer_launch_count": (C.c_uint64, [_vp]),
     "renderer_stage_times": (None, [_vp, C.POINTER(C.c_double)]),
     "renderer_counters": (None, [_vp, _u64p]),
@@ -349,9 +361,23 @@ STACK_ID_SYMBOLS = ("renderer_render_views_ids", "renderer_render_views_ids_devi
 
 # The same for the inspection entry points of the sort (sort_plan, Renderer.sort_pairs, sort_bounds).
 SORT_DEBUG_SYMBOLS = ("debug_sort_plan", "renderer_sort_pairs", "renderer_sort_bounds")
+# The same for linear float frames (Renderer.render_linear, render_views_linear, render_batch_linear).
+LINEAR_SYMBOLS = ("renderer_render_linear", "renderer_render_linear_device", "renderer_render_views_linear",
+                  "renderer_render_views_linear_device", "renderer_render_batch_linear", "renderer_render_batch_linear_device")
+
+# Pixel formats of linear frames: name -> (FORMA_PIXEL_*, bytes per pixel, element dtype).
+PIXEL_FORMATS = {"f16": (1, 8, np.float16), "f32": (2, 16, np.float32)}
 
 
-_OPTIONAL_SYMBOLS = frozenset(ID_FRAME_SYMBOLS + VIEW_SYMBOLS + BATCH_SYMBOLS + STACK_ID_SYMBOLS + SORT_DEBUG_SYMBOLS)
+def pixel_format(fmt: str):
+    """(FORMA_PIXEL_* code, bytes per pixel, numpy dtype) of "f16" or "f32"."""
+    if fmt not in PIXEL_FORMATS:
+        raise ValueError(f"pixel format {fmt!r}: 'f16' or 'f32'")
+    return PIXEL_FORMATS[fmt]
+
+
+_OPTIONAL_SYMBOLS = frozenset(ID_FRAME_SYMBOLS + VIEW_SYMBOLS + BATCH_SYMBOLS + STACK_ID_SYMBOLS + SORT_DEBUG_SYMBOLS +
+                              LINEAR_SYMBOLS)
 
 
 class Api:
@@ -820,16 +846,17 @@ class Renderer:
         """The most views of `height` rows one render_views call of the library takes (0: none)."""
         return int(self._api.renderer_max_views(height))
 
-    def _stack(self, fn, what, first_args, n, width, height, rgba, ids, timings):
+    def _stack(self, fn, what, first_args, n, width, height, rgba, ids, timings, bpp=4, tail=()):
         """Calls `fn`, an entry point of views or batches, on chunks of at most max_views(height)
         frames: first_args(first, count) gives a chunk's leading arguments (views or handles,
         count), then come its targets. rgba = (ptr or None, stride, frame_stride, channels,
         clear_color) and ids = (ptr, stride, frame_stride, min_coverage), either may be None; a
-        stride of None takes its default (4 * width, height * stride). An entry point with both
-        takes the ID target's arguments without width and height."""
+        stride of None takes its default (bpp * width, height * stride; IDs: bpp 4). An entry point
+        with both takes the ID target's arguments without width and height. `tail` follows the
+        targets."""
         chunk = max(self.max_views(height), 1)
         if rgba is not None:
-            rgba_ptr, stride, frame_stride = rgba[0], *self._strides(width, height, rgba[1], rgba[2])
+            rgba_ptr, stride, frame_stride = rgba[0], *self._strides(width, height, rgba[1], rgba[2], bpp)
             ch, cc, _ = self._common(rgba[3], rgba[4], None)
         if ids is not None:
             ids_ptr, ids_stride, ids_frame_stride = ids[0], *self._strides(width, height, ids[1], ids[2])
@@ -844,14 +871,14 @@ class Renderer:
                 layout = [ids_stride, ids_frame_stride] if rgba is not None else [width, ids_stride, height, ids_frame_stride]
                 args += [ptr, *layout, float(ids[3])]
             t = _CTimings() if timings else None
-            st = fn(self._h, *args, C.byref(t) if t is not None else None)
+            st = fn(self._h, *args, *tail, C.byref(t) if t is not None else None)
             self._api.check(st, what)
         return _timings(t)
 
     @staticmethod
-    def _strides(width, height, stride, frame_stride):
-        """Row and frame strides in bytes, by default 4 * width and height * stride."""
-        stride = width * 4 if stride is None else stride
+    def _strides(width, height, stride, frame_stride, bpp=4):
+        """Row and frame strides in bytes, by default bpp * width and height * stride."""
+        stride = width * bpp if stride is None else stride
         return stride, height * stride if frame_stride is None else frame_stride
 
     @staticmethod
@@ -977,6 +1004,84 @@ class Renderer:
         return self._stack(self._api.renderer_render_batch_ids_device, "Renderer::render_batch_ids_device", args, n, width, height,
                            (None if rgba_ptr is None else int(rgba_ptr), stride, frame_stride, channels, clear_color),
                            (int(ids_device_ptr), ids_stride, ids_frame_stride, min_coverage), timings)
+
+    @staticmethod
+    def _linear_host(buffer: np.ndarray, dtype, nbytes: int) -> None:
+        assert buffer.dtype == dtype and buffer.flags["C_CONTIGUOUS"] and buffer.nbytes >= nbytes, \
+            f"a contiguous {np.dtype(dtype).name} array of at least {nbytes} bytes"
+
+    def render_linear(self, composition: Composition, buffer: np.ndarray, width: int, height: int, channels=RGBA,
+                      clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), crop: Optional[Rect] = None, format: str = "f32",
+                      stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """The frame's linear colour (see include/forma_b200.h: forma_renderer_render_linear): per
+        pixel the painter's four values in channel order, before the sRGB encode, as float32
+        (format "f32") or float16 ("f16"). `buffer`: a writable contiguous host array of that dtype,
+        e.g. [height, width, 4]; `stride` in bytes (default bpp * width, bpp = 16 or 8). Only the
+        crop's tile rectangle is written."""
+        code, bpp, dtype = pixel_format(format)
+        stride = width * bpp if stride is None else stride
+        self._linear_host(buffer, dtype, height * stride)
+        return self._frame(self._api.renderer_render_linear, "Renderer::render_linear", composition, buffer.ctypes.data_as(C.c_void_p),
+                           width, height, stride, (channels, clear_color), crop, (code,), timings)
+
+    def render_linear_device(self, composition: Composition, device_ptr: int, width: int, height: int, channels=RGBA,
+                             clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), crop: Optional[Rect] = None, format: str = "f32",
+                             stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """render_linear into device memory on the renderer's device: with the defaults, the
+        data_ptr() of a contiguous [height, width, 4] float32 / float16 CUDA tensor."""
+        code, bpp, _ = pixel_format(format)
+        return self._frame(self._api.renderer_render_linear_device, "Renderer::render_linear_device", composition,
+                           C.c_void_p(device_ptr), width, height, width * bpp if stride is None else stride, (channels, clear_color),
+                           crop, (code,), timings)
+
+    def render_views_linear(self, composition: Composition, views, buffer: np.ndarray, width: int, height: int, channels=RGBA,
+                            clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), format: str = "f32", stride: Optional[int] = None,
+                            view_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """render_views as linear float frames (see render_linear): frame b at byte b * view_stride
+        (default height * stride) of `buffer`, a writable contiguous host array of the format's
+        dtype, e.g. [N, height, width, 4]. Chunked like render_views."""
+        code, bpp, dtype = pixel_format(format)
+        n, args = self._view_args(composition, views)
+        stride, view_stride = self._strides(width, height, stride, view_stride, bpp)
+        if n:
+            self._linear_host(buffer, dtype, (n - 1) * view_stride + (height - 1) * stride + bpp * width)
+        return self._stack(self._api.renderer_render_views_linear, "Renderer::render_views_linear", args, n, width, height,
+                           (buffer.ctypes.data, stride, view_stride, channels, clear_color), None, timings, bpp, (code,))
+
+    def render_views_linear_device(self, composition: Composition, views, device_ptr: int, width: int, height: int,
+                                   channels=RGBA, clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), format: str = "f32",
+                                   stride: Optional[int] = None, view_stride: Optional[int] = None,
+                                   timings: bool = True) -> Optional[Timings]:
+        """render_views_linear into device memory: with the defaults, the data_ptr() of a
+        contiguous [N, height, width, 4] float32 / float16 CUDA tensor."""
+        code, bpp, _ = pixel_format(format)
+        n, args = self._view_args(composition, views)
+        return self._stack(self._api.renderer_render_views_linear_device, "Renderer::render_views_linear_device", args, n, width,
+                           height, (int(device_ptr), stride, view_stride, channels, clear_color), None, timings, bpp, (code,))
+
+    def render_batch_linear(self, comps, buffer: np.ndarray, width: int, height: int, channels=RGBA,
+                            clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), format: str = "f32", stride: Optional[int] = None,
+                            frame_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """render_batch as linear float frames (see render_linear); layout as for
+        render_views_linear, chunked like render_batch."""
+        code, bpp, dtype = pixel_format(format)
+        n, args = self._batch_args(comps)
+        stride, frame_stride = self._strides(width, height, stride, frame_stride, bpp)
+        if n:
+            self._linear_host(buffer, dtype, (n - 1) * frame_stride + (height - 1) * stride + bpp * width)
+        return self._stack(self._api.renderer_render_batch_linear, "Renderer::render_batch_linear", args, n, width, height,
+                           (buffer.ctypes.data, stride, frame_stride, channels, clear_color), None, timings, bpp, (code,))
+
+    def render_batch_linear_device(self, comps, device_ptr: int, width: int, height: int, channels=RGBA,
+                                   clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), format: str = "f32",
+                                   stride: Optional[int] = None, frame_stride: Optional[int] = None,
+                                   timings: bool = True) -> Optional[Timings]:
+        """render_batch_linear into device memory: with the defaults, the data_ptr() of a
+        contiguous [N, height, width, 4] float32 / float16 CUDA tensor."""
+        code, bpp, _ = pixel_format(format)
+        n, args = self._batch_args(comps)
+        return self._stack(self._api.renderer_render_batch_linear_device, "Renderer::render_batch_linear_device", args, n, width,
+                           height, (int(device_ptr), stride, frame_stride, channels, clear_color), None, timings, bpp, (code,))
 
     def launch_count(self) -> int:
         return int(self._api.renderer_launch_count(self._h))

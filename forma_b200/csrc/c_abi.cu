@@ -385,7 +385,7 @@ static int render_request(forma_renderer* r, FrameRequest q, forma_composition* 
         for (size_t k = 0; k < cs.size(); ++k) cs[k] = comps[k] ? &comps[k]->c : nullptr;
         q.comp = c ? &c->c : nullptr;
         q.batch = comps ? cs.data() : nullptr;
-        if (q.kind == FrameKind::single && q.rgba.ptr && !q.rgba.on_device && !q.cache) {
+        if (q.kind == FrameKind::single && q.rgba.ptr && q.rgba.bpp == 4u && !q.rgba.on_device && !q.cache) {
             const int st = sliced_host_render(r, q);
             if (st >= 0) return st;
         }
@@ -498,6 +498,62 @@ int forma_renderer_render_batch_ids(forma_renderer* r, forma_composition* const*
     FrameRequest q{FrameKind::batch, n, width, height, nullptr, nullptr, timings};
     q.ids = {reinterpret_cast<uint8_t*>(host_ids), false, ids_stride, ids_frame_stride, min_coverage};
     return render_request(r, q, nullptr, comps, __func__);
+}
+// Linear float frames: the RGBA target with 8- or 16-byte pixels (a null buffer is refused by
+// Renderer::check_request like any missing target).
+static int render_linear(forma_renderer* r, FrameRequest q, uint32_t format, forma_composition* c, forma_composition* const* comps) {
+    q.rgba.bpp = format == FORMA_PIXEL_RGBA16F ? 8u : format == FORMA_PIXEL_RGBA32F ? 16u : 0u;
+    if (!q.rgba.bpp) {
+        set_error("invalid pixel format %u", format);
+        return FORMA_STATUS_INVALID;
+    }
+    return render_request(r, q, c, comps);
+}
+int forma_renderer_render_linear(forma_renderer* r, forma_composition* c, void* buffer, uint64_t width, uint64_t width_stride,
+                                 uint64_t height, const uint32_t channels[4], const float clear_color[4], const forma_rect* crop,
+                                 uint32_t format, forma_timings* timings) {
+    FrameRequest q{FrameKind::single, 0, width, height, channels, clear_color, timings, crop};
+    q.rgba = {static_cast<uint8_t*>(buffer), false, width_stride};
+    return render_linear(r, q, format, c, nullptr);
+}
+int forma_renderer_render_linear_device(forma_renderer* r, forma_composition* c, void* device_buffer, uint64_t width,
+                                        uint64_t width_stride, uint64_t height, const uint32_t channels[4], const float clear_color[4],
+                                        const forma_rect* crop, uint32_t format, forma_timings* timings) {
+    FrameRequest q{FrameKind::single, 0, width, height, channels, clear_color, timings, crop};
+    q.rgba = {static_cast<uint8_t*>(device_buffer), true, width_stride};
+    return render_linear(r, q, format, c, nullptr);
+}
+int forma_renderer_render_views_linear(forma_renderer* r, forma_composition* c, const float* views, uint32_t n, void* host_buffer,
+                                       uint64_t width, uint64_t width_stride, uint64_t height, uint64_t view_stride,
+                                       const uint32_t channels[4], const float clear_color[4], uint32_t format, forma_timings* timings) {
+    FrameRequest q{FrameKind::views, n, width, height, channels, clear_color, timings};
+    q.views = views;
+    q.rgba = {static_cast<uint8_t*>(host_buffer), false, width_stride, view_stride};
+    return render_linear(r, q, format, c, nullptr);
+}
+int forma_renderer_render_views_linear_device(forma_renderer* r, forma_composition* c, const float* views, uint32_t n,
+                                              void* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                              uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
+                                              uint32_t format, forma_timings* timings) {
+    FrameRequest q{FrameKind::views, n, width, height, channels, clear_color, timings};
+    q.views = views;
+    q.rgba = {static_cast<uint8_t*>(device_buffer), true, width_stride, view_stride};
+    return render_linear(r, q, format, c, nullptr);
+}
+int forma_renderer_render_batch_linear(forma_renderer* r, forma_composition* const* comps, uint32_t n, void* host_buffer, uint64_t width,
+                                       uint64_t width_stride, uint64_t height, uint64_t frame_stride, const uint32_t channels[4],
+                                       const float clear_color[4], uint32_t format, forma_timings* timings) {
+    FrameRequest q{FrameKind::batch, n, width, height, channels, clear_color, timings};
+    q.rgba = {static_cast<uint8_t*>(host_buffer), false, width_stride, frame_stride};
+    return render_linear(r, q, format, nullptr, comps);
+}
+int forma_renderer_render_batch_linear_device(forma_renderer* r, forma_composition* const* comps, uint32_t n, void* device_buffer,
+                                              uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride,
+                                              const uint32_t channels[4], const float clear_color[4], uint32_t format,
+                                              forma_timings* timings) {
+    FrameRequest q{FrameKind::batch, n, width, height, channels, clear_color, timings};
+    q.rgba = {static_cast<uint8_t*>(device_buffer), true, width_stride, frame_stride};
+    return render_linear(r, q, format, nullptr, comps);
 }
 // --- shared frames (multi-GPU, see include/forma_b200.h) -----------------------
 static_assert(sizeof(cudaIpcMemHandle_t) == sizeof(forma_ipc_handle), "CUDA IPC handles are 64 bytes");

@@ -21,7 +21,7 @@ struct Options {
     int sort_scan_log2 = 22; // key-only sorts: key count from which the reduce-then-scan passes replace the single-sweep ones
     int test_gap_cap = 0;    // test hook: cap of the speculative carry-only-entry launch (0 = none)
     int paint_lpt = 1;       // heavy tiles first (longest-processing-time order) in the paint kernel
-    int paint_wide = 0;      // 1: the paint kernel built for 6 CTAs / SM (up to 168 registers) instead of 8 (128)
+    int paint_wide = 0;      // 1: the paint kernel built for 6 CTAs / SM (up to 168 registers) instead of 8 (128); sRGB8 frames only (float frames always use the 8-CTA build)
     int band_filter = 1;     // a render cropped to a band of rows only makes the band's geometry resident
     int sync_free = 1;       // painter tables without count read-backs when the previous frame's counts bound this one's (redone the slow way if they do not)
     int test_fast_shrink = 0;  // test hook: halve the bounds of the sync-free tables (forces the redo)
@@ -272,6 +272,12 @@ void launch_merge_entries(const PaintScene& S, const uint64_t* cell_key, uint32_
 void launch_paint(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range, const uint32_t* heavy,
                   const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st,
                   uint32_t view_rows = 0);
+// launch_paint for a linear float frame of `bpp` bytes per pixel: 8 (RGBA16F) or 16 (RGBA32F), the
+// painter's planes in channel order where launch_paint stores their sRGB bytes (see
+// forma_renderer_render_linear). `framebuffer` and S.stride: multiples of 4 bytes.
+void launch_paint_linear(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range, const uint32_t* heavy,
+                         const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st,
+                         uint32_t view_rows, uint32_t bpp);
 // Copies rows [0, height) of the n_views views of a stacked frame (view b's first row at
 // src + b * view_rows_px * src_stride) to dst + b * view_stride, row r at + r * stride.
 void launch_repack_views(const uint8_t* src, uint64_t src_stride, uint32_t view_rows_px, uint8_t* dst, uint64_t stride,

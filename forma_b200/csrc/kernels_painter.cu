@@ -32,6 +32,8 @@
 // (tile_index_kernel sorts them into four classes by entry count): a tile is painted by
 // one warp from its first to its last layer, so the heaviest tile bounds the kernel's
 // tail unless it starts early (longest-processing-time order).
+#include <cuda_fp16.h>
+
 #include <mutex>
 #include "paint_common.cuh"
 #include "paint_math.cuh"
@@ -317,6 +319,92 @@ __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, kMinBlocks)
 #undef FORMA_PAINT_FRAME_TY
 }
 
+// ---------------------------------------------------------------------------
+// Linear float frames: the painter's planes as they are, RGBA16F (8-byte pixels, each value
+// __float2half_rn) or RGBA32F (16-byte pixels), in channel order
+// ---------------------------------------------------------------------------
+// The four values of a pixel in channel order: what compute_srgb encodes, not encoded.
+__device__ __forceinline__ float4 linear_pixel(float r, float g, float b, float a, const uint32_t ch[4]) {
+    const Rgba c{r, g, b, a};
+    return make_float4(channel_of(c, ch[0]), channel_of(c, ch[1]), channel_of(c, ch[2]), channel_of(c, ch[3]));
+}
+__device__ __forceinline__ uint32_t half2_bits(float lo, float hi) {
+    return (uint32_t)__half_as_ushort(__float2half_rn(lo)) | ((uint32_t)__half_as_ushort(__float2half_rn(hi)) << 16);
+}
+// Stores the pixel pair (p0, p1) whose first pixel is at `dst`; `both`: p1 lies inside the frame.
+// vec: the frame and its stride are 16-byte aligned (a pair is 16 or 32 bytes at a 16-byte
+// offset); otherwise 4-byte stores, which the 4-byte alignment of float frames allows.
+__device__ __forceinline__ void store_linear_pair(uint8_t* dst, float4 p0, float4 p1, bool both, bool vec, uint32_t bpp) {
+    if (bpp == 8u) {
+        const uint4 h = make_uint4(half2_bits(p0.x, p0.y), half2_bits(p0.z, p0.w), half2_bits(p1.x, p1.y), half2_bits(p1.z, p1.w));
+        uint32_t* w = reinterpret_cast<uint32_t*>(dst);
+        if (vec && both) {
+            *reinterpret_cast<uint4*>(dst) = h;
+        } else {
+            w[0] = h.x;
+            w[1] = h.y;
+            if (both) {
+                w[2] = h.z;
+                w[3] = h.w;
+            }
+        }
+    } else if (vec) {
+        float4* v = reinterpret_cast<float4*>(dst);
+        v[0] = p0;
+        if (both) v[1] = p1;
+    } else {
+        float* f = reinterpret_cast<float*>(dst);
+        f[0] = p0.x; f[1] = p0.y; f[2] = p0.z; f[3] = p0.w;
+        if (both) {
+            f[4] = p1.x; f[5] = p1.y; f[6] = p1.z; f[7] = p1.w;
+        }
+    }
+}
+// The lane's eight pixels of row py from column x0 (planes in pixel pairs, as the painter holds them).
+__device__ __forceinline__ void store_linear_run(const PaintScene& S, uint8_t* fb, uint32_t py, uint32_t x0, const f2 (&r)[4],
+                                                 const f2 (&g)[4], const f2 (&b)[4], const f2 (&a)[4], bool vec, uint32_t bpp) {
+    if (py >= S.height || x0 >= S.width) return;
+    uint8_t* row = fb + (size_t)py * S.stride + (size_t)x0 * bpp;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        const uint32_t x = x0 + 2u * (uint32_t)q;
+        if (x < S.width)
+            store_linear_pair(row + (size_t)(2 * q) * bpp, linear_pixel(r[q].x, g[q].x, b[q].x, a[q].x, S.channels),
+                              linear_pixel(r[q].y, g[q].y, b[q].y, a[q].y, S.channels), x + 1u < S.width, vec, bpp);
+    }
+}
+// store_tile_solid for a linear frame: the folded colour (BlendMode::blend's result) in every pixel.
+__device__ __forceinline__ void store_tile_solid_linear(const PaintScene& S, uint8_t* fb, uint32_t tx, uint32_t ty, uint32_t lane,
+                                                        const Rgba& c, bool vec, uint32_t bpp) {
+    const f2 r[4] = {f2_splat(c.r), f2_splat(c.r), f2_splat(c.r), f2_splat(c.r)};
+    const f2 g[4] = {f2_splat(c.g), f2_splat(c.g), f2_splat(c.g), f2_splat(c.g)};
+    const f2 b[4] = {f2_splat(c.b), f2_splat(c.b), f2_splat(c.b), f2_splat(c.b)};
+    const f2 a[4] = {f2_splat(c.a), f2_splat(c.a), f2_splat(c.a), f2_splat(c.a)};
+    store_linear_run(S, fb, ty * 16u + (lane >> 1), tx * 16u + (lane & 1u) * 8u, r, g, b, a, vec, bpp);
+}
+
+// paint_kernel / paint_views_kernel storing a linear frame of `bpp` (8: RGBA16F, 16: RGBA32F)
+// bytes per pixel. Built for 8 CTAs / SM only. A float frame takes no layer cache, so the
+// solid-tile hook has no cached colour to compare with.
+#define FORMA_PAINT_STORE_SOLID(c) store_tile_solid_linear(S, in.framebuffer, tx, ty, lane, c, vec_ok, bpp)
+#define FORMA_PAINT_STORE_PIXELS() \
+    (void)rgba_order;              \
+    store_linear_run(S, in.framebuffer, ty * 16u + row, x0, dr, dg, db, da, vec_ok, bpp)
+__global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, 8)
+    paint_linear_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles, uint32_t bpp) {
+#define FORMA_PAINT_FRAME_TY(ty) (ty)
+#include "paint_kernel_body.cuh"
+#undef FORMA_PAINT_FRAME_TY
+}
+__global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, 8)
+    paint_views_linear_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles, uint32_t view_rows, uint32_t bpp) {
+#define FORMA_PAINT_FRAME_TY(ty) ((ty) % view_rows)
+#include "paint_kernel_body.cuh"
+#undef FORMA_PAINT_FRAME_TY
+}
+#undef FORMA_PAINT_STORE_SOLID
+#undef FORMA_PAINT_STORE_PIXELS
+
 // Rows [0, height) of every view of a stacked frame (view b at src + b * view_rows_px * src_stride)
 // to dst + b * view_stride + row * stride: padding rows and the bytes between views stay untouched.
 // One thread per pixel, 4 bytes apart in every row.
@@ -477,6 +565,33 @@ void launch_paint(const PaintScene& S, const uint64_t* segs, const EntryRec* rec
     } else {
         paint_kernel<8><<<min(want, need), kPaintWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles);
     }
+}
+
+void launch_paint_linear(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range, const uint32_t* heavy,
+                         const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st,
+                         uint32_t view_rows, uint32_t bpp) {
+    if (S.tx_hi <= S.tx_lo || S.ty_hi <= S.ty_lo) return;
+    const uint32_t n_tiles = (S.tx_hi - S.tx_lo) * (S.ty_hi - S.ty_lo);
+    cudaMemsetAsync(tile_counter, 0, sizeof(uint32_t), st);
+    PaintInputs in{segs, recs, tile_range, heavy, heavy_count, S.tiles_x * S.tiles_y, eflags, framebuffer, tile_counter};
+    // Persistent warps, as in launch_paint.
+    static int blocks_per_sm[2][kMaxDevices] = {{0}};
+    static std::mutex config_mu;
+    const int views = view_rows ? 1 : 0;
+    int per_sm = 0;
+    {
+        std::lock_guard<std::mutex> lk(config_mu);
+        int& slot = blocks_per_sm[views][current_device_index()];
+        if (!slot) {
+            const void* k = views ? (const void*)paint_views_linear_kernel : (const void*)paint_linear_kernel;
+            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&slot, k, kPaintWarpsPerBlock * 32, 0);
+            if (slot < 1) slot = 1;
+        }
+        per_sm = slot;
+    }
+    const uint32_t grid = min((uint32_t)(per_sm * device_sm_count()), (n_tiles + kPaintWarpsPerBlock - 1) / kPaintWarpsPerBlock);
+    if (views) paint_views_linear_kernel<<<grid, kPaintWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles, view_rows, bpp);
+    else paint_linear_kernel<<<grid, kPaintWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles, bpp);
 }
 
 }  // namespace forma

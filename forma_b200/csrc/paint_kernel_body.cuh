@@ -1,7 +1,10 @@
-// The body of paint_kernel and paint_views_kernel (kernels_painter.cu), included into both so that
+// The body of paint_kernel, paint_views_kernel and their linear twins (kernels_painter.cu), included into each so that
 // each kernel is compiled from the same text as a function of its own. Expects S, in and n_tiles,
 // and FORMA_PAINT_FRAME_TY(ty): the tile row in frame coordinates at which gradients and textures
 // are sampled (ty itself for a single frame, the row inside its view for a stack of views).
+// A kernel that stores something other than sRGB8 defines both store hooks:
+//   FORMA_PAINT_STORE_SOLID(dst): the tile folded to the one colour dst (Rgba, no layer cache);
+//   FORMA_PAINT_STORE_PIXELS():   the lane's painted pixels, planes dr / dg / db / da at (x0, ty * 16 + row).
     __shared__ __align__(16) WarpSmem s_warp[kPaintWarpsPerBlock];
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
     WarpSmem& W = s_warp[warp];
@@ -218,6 +221,10 @@
                 }
             }
             if (solid) {
+#ifdef FORMA_PAINT_STORE_SOLID
+                FORMA_PAINT_STORE_SOLID(dst);
+                continue;
+#else
                 const uint32_t bytes = solid_to_srgb_bytes(dst, S.channels);
                 // CachedTile::convert_optimizer_op (cpu/painter/mod.rs:686-704): the same
                 // solid colour as last frame is not written again.
@@ -228,6 +235,7 @@
                     if (!same && S.written_list) S.written_list[atomicAdd(S.written_count, 1u)] = tid;
                 }
                 continue;
+#endif
             }
         }
         if (lane == 0) {
@@ -472,6 +480,9 @@
             }
         }
 
+#ifdef FORMA_PAINT_STORE_PIXELS
+        FORMA_PAINT_STORE_PIXELS();
+#else
         // compute_srgb + LinearLayout::write (mod.rs:466-483, layout/mod.rs:265-282).
         const uint32_t py = ty * 16u + row;
         if (py < S.height && x0 < S.width) {
@@ -504,4 +515,5 @@
                     if (x0 + (uint32_t)j < S.width) reinterpret_cast<uint32_t*>(rowp)[j] = out[j];
             }
         }
+#endif
     }

@@ -488,7 +488,7 @@ int Renderer::render(const FrameRequest& q) {
     // rows laid out as the stacked frame's rows; each target decides for itself.
     auto device_frame = [&](const FrameTarget& t) {
         const bool direct = t.on_device && (!stack || (q.height % 16u == 0u && t.frame_stride == q.height * t.stride));
-        return DeviceFrame{t.ptr, direct || !stack ? t.stride : 4u * q.width, direct};
+        return DeviceFrame{t.ptr, direct || !stack ? t.stride : t.bpp * q.width, direct};
     };
     FramePlan p{device_frame(q.rgba), device_frame(q.ids), stack ? (uint32_t)((q.height + 15u) / 16u) : 0u, false, false};
     // The PaintScene of the RGBA target, or of the ID target when it is alone.
@@ -506,7 +506,8 @@ int Renderer::render(const FrameRequest& q) {
         FORMA_CUDA_TRY(id_frame.reserve((size_t)(p.ids.stride / 4u) * S.height));
         p.ids.ptr = reinterpret_cast<uint8_t*>(id_frame.ptr);
     }
-    p.in_bands = rgba && !stack && !q.rgba.on_device && !q.cache && S.ty_hi - S.ty_lo >= (copy_bands_override ? 8u : 32u) &&
+    // (A host float frame is painted whole and copied back once.)
+    p.in_bands = rgba && q.rgba.bpp == 4u && !stack && !q.rgba.on_device && !q.cache && S.ty_hi - S.ty_lo >= (copy_bands_override ? 8u : 32u) &&
                  S.tx_hi > S.tx_lo && band_copies_enabled();
     p.pack_written = q.cache && !q.rgba.on_device;
     st = run_frame(q, S, p);
@@ -531,7 +532,7 @@ int Renderer::check_request(const FrameRequest& q) {
     const char* what = q.kind == FrameKind::views ? "view" : "frame";
     const uint64_t width = q.width, height = q.height;
     auto check_target = [&](const FrameTarget& t) {
-        if (!t.ptr || width == 0 || height == 0 || width * 4 > t.stride || width > FORMA_MAX_WIDTH || height > FORMA_MAX_HEIGHT) {
+        if (!t.ptr || width == 0 || height == 0 || width * t.bpp > t.stride || width > FORMA_MAX_WIDTH || height > FORMA_MAX_HEIGHT) {
             set_error("invalid render target %llux%llu stride %llu", (unsigned long long)width, (unsigned long long)height,
                       (unsigned long long)t.stride);
             return (int)FORMA_STATUS_INVALID;
@@ -542,15 +543,20 @@ int Renderer::check_request(const FrameRequest& q) {
                       (unsigned long long)height, max_views(height), what);
             return (int)FORMA_STATUS_INVALID;
         }
-        if (t.frame_stride < (height - 1u) * t.stride + 4u * width) {
+        if (t.frame_stride < (height - 1u) * t.stride + t.bpp * width) {
             set_error("%s stride %llu is smaller than one %s (%llu bytes)", what, (unsigned long long)t.frame_stride, what,
-                      (unsigned long long)((height - 1u) * t.stride + 4u * width));
+                      (unsigned long long)((height - 1u) * t.stride + t.bpp * width));
             return (int)FORMA_STATUS_INVALID;
         }
         return (int)FORMA_STATUS_OK;
     };
     int st = q.rgba.ptr || !q.ids.ptr ? check_target(q.rgba) : FORMA_STATUS_OK;
     if (st) return st;
+    if (q.rgba.bpp != 4u && (((uintptr_t)q.rgba.ptr | q.rgba.stride | q.rgba.frame_stride) & 3u) != 0u) {
+        set_error("invalid float frame: buffer, stride %llu and %s stride %llu must be multiples of 4 bytes",
+                  (unsigned long long)q.rgba.stride, what, (unsigned long long)q.rgba.frame_stride);
+        return FORMA_STATUS_INVALID;
+    }
     if (q.ids.ptr) {
         const FrameTarget& t = q.ids;
         if (t.stride % 4u != 0u || t.frame_stride % 4u != 0u || !std::isfinite(t.min_coverage) || t.min_coverage < 0.0f ||
@@ -701,7 +707,7 @@ int Renderer::bind_batch(Composition* const* comps, uint32_t n, PaintScene& S, u
 int Renderer::paint_step(const FrameRequest& q, const PaintScene& S, const FramePlan& p, const uint32_t* heavy_lists,
                          uint32_t* paint_launches) {
     if (q.rgba.ptr) {
-        const int st = paint(S, p.rgba.ptr, q.rgba.ptr, q.rgba.stride, p.in_bands, heavy_lists, paint_launches, p.rows);
+        const int st = paint(S, p.rgba.ptr, q.rgba.ptr, q.rgba.stride, p.in_bands, heavy_lists, paint_launches, p.rows, q.rgba.bpp);
         if (st || !q.ids.ptr) return st;
         ++*paint_launches;
     }
@@ -723,10 +729,11 @@ int Renderer::output_step(const FrameRequest& q, const PaintScene& S, const Fram
     if (p.pack_written) return scatter_written_tiles(S, p.rgba.ptr, q.rgba.ptr, q.rgba.stride);
     auto output = [&](const FrameTarget& t, const DeviceFrame& f) {
         if (!t.ptr || f.direct) return (int)FORMA_STATUS_OK;
-        if (!p.rows) return copy_to_host(S, t.ptr, f.ptr, t.stride, stream);
+        if (!p.rows) return copy_to_host(S, t.ptr, f.ptr, t.stride, stream, t.bpp);
         const uint32_t height = (uint32_t)q.height;
-        if (t.on_device) {
-            launch_repack_views(f.ptr, f.stride, p.rows * 16u, t.ptr, t.stride, t.frame_stride, S.width, height, q.n, stream);
+        if (t.on_device) {  // (a frame of 8- or 16-byte pixels is a frame of 4-byte words bpp / 4 times as wide)
+            launch_repack_views(f.ptr, f.stride, p.rows * 16u, t.ptr, t.stride, t.frame_stride, S.width * (t.bpp / 4u), height, q.n,
+                                stream);
             ++launches;
             FORMA_CUDA_TRY(cudaGetLastError());
             return (int)FORMA_STATUS_OK;
@@ -738,11 +745,11 @@ int Renderer::output_step(const FrameRequest& q, const PaintScene& S, const Fram
             uint8_t* dst = t.ptr + (size_t)b * t.frame_stride;
             const uint8_t* src = f.ptr + (size_t)b * p.rows * 16u * f.stride;
             if (t.stride == f.stride)
-                FORMA_CUDA_TRY(cudaMemcpyAsync(dst, src, (height - 1u) * t.stride + 4u * q.width, cudaMemcpyDeviceToHost, stream));
+                FORMA_CUDA_TRY(cudaMemcpyAsync(dst, src, (height - 1u) * t.stride + t.bpp * q.width, cudaMemcpyDeviceToHost, stream));
             else
-                FORMA_CUDA_TRY(cudaMemcpy2DAsync(dst, t.stride, src, f.stride, 4u * q.width, height, cudaMemcpyDeviceToHost, stream));
+                FORMA_CUDA_TRY(cudaMemcpy2DAsync(dst, t.stride, src, f.stride, t.bpp * q.width, height, cudaMemcpyDeviceToHost, stream));
         }
-        d2h_bytes += (uint64_t)q.n * height * q.width * 4u;
+        d2h_bytes += (uint64_t)q.n * height * q.width * t.bpp;
         return (int)FORMA_STATUS_OK;
     };
     const int st = p.in_bands ? FORMA_STATUS_OK : output(q.rgba, p.rgba);
@@ -991,8 +998,9 @@ int Renderer::queue_row_costs(const PaintScene& S, uint32_t n) {
 // kernels are persistent (one CTA per resident slot), so the CTAs of band k + 1 start as the warps
 // of band k run dry: the kernels overlap at their tails, and the PCIe transfer of a band overlaps
 // the painting of the following ones.
+// bpp: bytes per pixel of fb, 4 (sRGB8), or 8 / 16 for a linear float frame (never in bands).
 int Renderer::paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t stride, bool in_bands, const uint32_t* heavy_lists,
-                    uint32_t* paint_launches, uint32_t view_rows) {
+                    uint32_t* paint_launches, uint32_t view_rows, uint32_t bpp) {
     *paint_launches = 1;
     if (in_bands) {
         if (!band_streams_ok) {
@@ -1021,8 +1029,12 @@ int Renderer::paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t 
         }
         for (uint32_t k = 0; kCopyBands > 1u && k < kCopyBands; ++k) FORMA_CUDA_TRY(cudaStreamWaitEvent(stream, band_ev[k], 0));
         *paint_launches = kCopyBands;
-    } else {
+    } else if (bpp == 4u) {
         launch_paint(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), eflags.ptr, fb, totals.ptr + 3, stream, view_rows);
+        ++launches;
+    } else {
+        launch_paint_linear(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), eflags.ptr, fb, totals.ptr + 3, stream,
+                            view_rows, bpp);
         ++launches;
     }
     FORMA_CUDA_TRY(cudaGetLastError());
@@ -1031,17 +1043,17 @@ int Renderer::paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t 
 
 // Copies the painted tile rectangle of S from the frame on the device to the host buffer. Only the
 // cropped tile rectangle is written by the reference (cpu/painter/mod.rs:524-529,589-593); padding
-// bytes beyond width*4 stay untouched.
-int Renderer::copy_to_host(const PaintScene& S, uint8_t* buffer, const uint8_t* fb, uint64_t stride, cudaStream_t s) {
+// bytes beyond width * bpp stay untouched.
+int Renderer::copy_to_host(const PaintScene& S, uint8_t* buffer, const uint8_t* fb, uint64_t stride, cudaStream_t s, uint32_t bpp) {
     const uint64_t x0 = (uint64_t)S.tx_lo * 16u, x1 = std::min<uint64_t>((uint64_t)S.tx_hi * 16u, S.width);
     const uint64_t y0 = (uint64_t)S.ty_lo * 16u, y1 = std::min<uint64_t>((uint64_t)S.ty_hi * 16u, S.height);
     if (x1 > x0 && y1 > y0) {
-        if (x0 == 0 && x1 * 4 == stride)  // whole rows without padding: one contiguous copy
+        if (x0 == 0 && x1 * bpp == stride)  // whole rows without padding: one contiguous copy
             FORMA_CUDA_TRY(cudaMemcpyAsync(buffer + y0 * stride, fb + y0 * stride, (y1 - y0) * stride, cudaMemcpyDeviceToHost, s));
         else
-            FORMA_CUDA_TRY(cudaMemcpy2DAsync(buffer + y0 * stride + x0 * 4, stride, fb + y0 * stride + x0 * 4, stride,
-                                             (x1 - x0) * 4, y1 - y0, cudaMemcpyDeviceToHost, s));
-        d2h_bytes += (x1 - x0) * 4 * (y1 - y0);
+            FORMA_CUDA_TRY(cudaMemcpy2DAsync(buffer + y0 * stride + x0 * bpp, stride, fb + y0 * stride + x0 * bpp, stride,
+                                             (x1 - x0) * bpp, y1 - y0, cudaMemcpyDeviceToHost, s));
+        d2h_bytes += (x1 - x0) * bpp * (y1 - y0);
     }
     return FORMA_STATUS_OK;
 }

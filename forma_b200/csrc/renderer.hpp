@@ -37,7 +37,8 @@ struct Timer {
     bool ok = false;
 };
 
-// A target of a FrameRequest: 4-byte pixels, RGBA8 or the layer IDs of ID frames (see
+// A target of a FrameRequest: pixels of `bpp` bytes, RGBA8 (4), RGBA16F (8) or RGBA32F (16) for the
+// RGBA target (see forma_renderer_render_linear), the 4-byte layer IDs of ID frames (see
 // forma_renderer_render_ids). Row r of frame b at ptr + b * frame_stride + r * stride
 // (frame_stride: stacks only).
 struct FrameTarget {
@@ -45,6 +46,7 @@ struct FrameTarget {
     bool on_device = false;
     uint64_t stride = 0, frame_stride = 0;
     float min_coverage = 0.0f;  // the ID target
+    uint32_t bpp = 4;
 };
 
 // What a FrameRequest renders. single: one frame of a composition. views: n views of one
@@ -85,7 +87,7 @@ struct DeviceFrame {
 struct FramePlan {
     DeviceFrame rgba, ids;
     uint32_t rows;      // stacks: tile rows of each frame; 0: a single frame
-    bool in_bands;      // a single host RGBA frame painted and copied back band by band (see paint)
+    bool in_bands;      // a single host sRGB8 frame painted and copied back band by band (see paint)
     bool pack_written;  // a cached host frame: only the tiles it writes travel back (scatter_written_tiles)
 };
 
@@ -312,8 +314,8 @@ class Renderer {
                      DevCounts& dc);
     int queue_row_costs(const PaintScene& S, uint32_t n);
     int paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t stride, bool in_bands, const uint32_t* heavy_lists,
-              uint32_t* paint_launches, uint32_t view_rows = 0);
-    int copy_to_host(const PaintScene& S, uint8_t* buffer, const uint8_t* fb, uint64_t stride, cudaStream_t s);
+              uint32_t* paint_launches, uint32_t view_rows = 0, uint32_t bpp = 4);
+    int copy_to_host(const PaintScene& S, uint8_t* buffer, const uint8_t* fb, uint64_t stride, cudaStream_t s, uint32_t bpp = 4);
     int scatter_written_tiles(const PaintScene& S, const uint8_t* fb, uint8_t* buffer, uint64_t stride);
 };
 

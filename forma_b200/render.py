@@ -1,6 +1,6 @@
 """Headless front end: render an SVG file to PPM / PNG on the GPU.
 
-    python -m forma_b200.render in.svg out.ppm [--width W --height H --scale S --device 0] [--ids ids.npy]
+    python -m forma_b200.render in.svg out.ppm [--width W --height H --scale S --device 0] [--ids ids.npy] [--linear out.npy]
 
 The equivalent of the reference's `demo svg --file in.svg --scale S` + the `S` key's
 capture.ppm (demo/src/main.rs, demo/src/runner.rs:193-219: a binary P6 file with the
@@ -8,6 +8,8 @@ frame's RGB bytes), without a window. The output format follows the extension (.
 .png when Pillow is available). There is no CPU fallback: without a CUDA device the
 renderer cannot be created and the command fails. `--ids` also writes the frame's ID frame (per pixel
 the order of the top-most layer drawn there, 0xFFFFFFFF for none) as an H x W uint32 .npy.
+`--linear` also writes the frame's linear colour before the sRGB encode (RGBA, float32) as an
+H x W x 4 .npy.
 """
 from __future__ import annotations
 
@@ -36,6 +38,7 @@ def main(argv=None) -> int:
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--frames", type=int, default=1, help="render this many times and report the last frame's timings")
     ap.add_argument("--ids", help="also write the ID frame (H x W uint32, Renderer.render_ids) to this .npy file")
+    ap.add_argument("--linear", help="also write the linear float frame (H x W x 4 float32, Renderer.render_linear) to this .npy file")
     args = ap.parse_args(argv)
 
     import forma_b200
@@ -63,6 +66,10 @@ def main(argv=None) -> int:
         ids = np.zeros(args.width * args.height, np.uint32)
         renderer.render_ids(comp, ids, args.width, args.height)
         np.save(args.ids, ids.reshape(args.height, args.width))
+    if args.linear:
+        linear = np.zeros((args.height, args.width, 4), np.float32)
+        renderer.render_linear(comp, linear, args.width, args.height, RGBA, Color(1.0, 1.0, 1.0, 1.0), format="f32")
+        np.save(args.linear, linear)
     print(f"{len(paths)} paths parsed in {t1 - t0:.2f} s, composed in {t2 - t1:.2f} s; {t.n_segments} pixel segments; "
           f"last frame: line setup {t.line_setup_ms:.3f} ms, rasterize {t.rasterize_ms:.3f} ms, sort {t.sort_ms:.3f} ms, "
           f"paint {t.paint_ms:.3f} ms ({(t3 - t2) / max(args.frames, 1) * 1e3:.2f} ms per call) -> {args.out}", file=sys.stderr)

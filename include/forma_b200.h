@@ -359,6 +359,57 @@ int forma_renderer_render_batch_ids(forma_renderer*, forma_composition* const* c
                                     uint64_t width, uint64_t ids_stride, uint64_t height, uint64_t ids_frame_stride,
                                     float min_coverage, forma_timings* timings /* nullable */);
 
+/* Linear float frames (the reference's gpu::Renderer::render_to_texture writes an Rgba16Float
+ * texture; see INTEGRATION.md): the painter's linear colour before the sRGB encode. Per pixel of
+ * the written rectangle four values in the order of `channels`:
+ *   - a painted tile: the planes (r, g, b, a) the painter holds after the tile's last blend, the
+ *     values compute_srgb receives; no sRGB encode, no clamp, no rounding to bytes;
+ *   - a tile the optimiser folds into one colour: that colour (BlendMode::blend's result);
+ *   - a tile without layers: the clear colour;
+ *   - FORMA_CHANNEL_ZERO gives 0.0, FORMA_CHANNEL_ONE 1.0, and ALPHA becomes ONE when
+ *     clear_color[3] == 1, as for sRGB8 frames.
+ * FORMA_PIXEL_RGBA32F stores the f32 values as they are (16 bytes per pixel); FORMA_PIXEL_RGBA16F
+ * stores each rounded to the nearest half, ties to even (8 bytes per pixel): beyond the half range
+ * a value becomes +-inf, a NaN stays a NaN. Encoding an RGBA32F frame with compute_srgb gives the
+ * bytes forma_renderer_render_device writes for the same call.
+ * Each call has the arguments of its sRGB8 twin (forma_renderer_render{,_device},
+ * forma_renderer_render_views{,_device}, forma_renderer_render_batch{,_device}) without the layer
+ * cache and with `format`; `buffer` may hold any type, and every stride is in BYTES:
+ * width_stride >= bpp * width and view_stride / frame_stride >= (height - 1) * width_stride +
+ * bpp * width, bpp = 8 or 16. The buffer and every stride must be multiples of 4 bytes; 16 lets
+ * the paint kernel store 16-byte vectors. Refused with FORMA_ERR_INVALID_ARGUMENT before anything
+ * is written: a null buffer, a format other than the two below, a stride or alignment that breaks
+ * these rules, and everything the sRGB8 twin refuses (n, views, null batch entries, ...); the
+ * order-sum, stop / texel and 2^30-segment limits of the twins apply as well. Only the crop's
+ * tile rectangle (single frames) or the frames' width x height pixels (stacks) are written.
+ * A float frame takes no layer cache and leaves every cache as it was. With the defaults of a
+ * [H, W, 4] / [n, H, W, 4] float32 or float16 tensor: width_stride = bpp * W, view_stride /
+ * frame_stride = bpp * W * H. */
+enum { FORMA_PIXEL_RGBA16F = 1, FORMA_PIXEL_RGBA32F = 2 };
+int forma_renderer_render_linear(forma_renderer*, forma_composition*, void* buffer, uint64_t width, uint64_t width_stride,
+                                 uint64_t height, const uint32_t channels[4], const float clear_color[4],
+                                 const forma_rect* crop /* nullable */, uint32_t format, forma_timings* timings /* nullable */);
+int forma_renderer_render_linear_device(forma_renderer*, forma_composition*, void* device_buffer, uint64_t width,
+                                        uint64_t width_stride, uint64_t height, const uint32_t channels[4],
+                                        const float clear_color[4], const forma_rect* crop /* nullable */, uint32_t format,
+                                        forma_timings* timings /* nullable */);
+int forma_renderer_render_views_linear(forma_renderer*, forma_composition*, const float* views, uint32_t n, void* host_buffer,
+                                       uint64_t width, uint64_t width_stride, uint64_t height, uint64_t view_stride,
+                                       const uint32_t channels[4], const float clear_color[4], uint32_t format,
+                                       forma_timings* timings /* nullable */);
+int forma_renderer_render_views_linear_device(forma_renderer*, forma_composition*, const float* views, uint32_t n,
+                                              void* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                              uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
+                                              uint32_t format, forma_timings* timings /* nullable */);
+int forma_renderer_render_batch_linear(forma_renderer*, forma_composition* const* comps, uint32_t n, void* host_buffer,
+                                       uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride,
+                                       const uint32_t channels[4], const float clear_color[4], uint32_t format,
+                                       forma_timings* timings /* nullable */);
+int forma_renderer_render_batch_linear_device(forma_renderer*, forma_composition* const* comps, uint32_t n, void* device_buffer,
+                                              uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride,
+                                              const uint32_t channels[4], const float clear_color[4], uint32_t format,
+                                              forma_timings* timings /* nullable */);
+
 /* Launch on `cuda_stream` (a cudaStream_t, e.g. torch.cuda.current_stream().cuda_stream)
  * instead of the default stream. */
 void forma_renderer_set_stream(forma_renderer*, void* cuda_stream);
