@@ -14,9 +14,10 @@
 //     pixels one 32-byte run of the frame buffer;
 //   * an entry without segments has one coverage value per lane.
 // The reference's f32x8 is eight rows of one column; its "skip when all eight coverages
-// are zero" (mod.rs:317-319) is reproduced from eight ballots where it can matter (any
-// fill / blend other than a solid `Over`, for which blending with zero coverage is the
-// identity on finite values).
+// are zero" (mod.rs:317-319) is kept on every path: from eight ballots for the pair and
+// generic paths, and from three shuffles of a per-lane 8-bit mask for a solid `Over` layer.
+// Blending at zero coverage is not the identity there either: a non-finite colour or alpha
+// makes the pixel NaN, and a -0 plane becomes +0.
 //
 // Per (tile, layer) entry the segments are scatter-added into packed cells — area in the
 // high and cover in the low 16 bits of one word, one shared-memory atomic per segment —
@@ -73,6 +74,8 @@ __device__ __forceinline__ f2 sub2(f2 a, f2 b) { return fma2(b, f2_splat(-1.0f),
 __device__ __forceinline__ f2 neg2(f2 a) { return f2{-a.x, -a.y}; }
 __device__ __forceinline__ f2 min2(f2 a, f2 b) { return f2{fminf(a.x, b.x), fminf(a.y, b.y)}; }
 __device__ __forceinline__ f2 max2(f2 a, f2 b) { return f2{fmaxf(a.x, b.x), fmaxf(a.y, b.y)}; }
+// The blended pair where bit 0 (x) / bit 1 (y) of `act` is set, the old pair elsewhere.
+__device__ __forceinline__ f2 keep2(uint32_t act, f2 blended, f2 old) { return f2{act & 1u ? blended.x : old.x, act & 2u ? blended.y : old.y}; }
 
 // The 12 separable blend modes of the vector macro blend_function! (styling.rs:438-592) on a
 // pixel pair, same operation order as vblend::blend (paint_math.cuh). `mode` is uniform.

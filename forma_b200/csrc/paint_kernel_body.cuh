@@ -399,8 +399,18 @@
                 const uint32_t fill_type = meta_fill_type(meta);
                 const uint4 h2 = hdr4[k * 4u + 2u];  // the solid colour
                 if (fill_type == 0u && mode == 0u) {
-                    // blend_at (mod.rs:406-447) for a solid `Over` layer: blended == src, and zero
-                    // coverage leaves the pixel as it is, so no f32x8 bookkeeping is needed.
+                    // blend_at (mod.rs:406-447) for a solid `Over` layer: blended == src. Zero
+                    // coverage is not the identity (a non-finite colour gives NaN, a -0 plane
+                    // becomes +0), so the f32x8 rule holds here too: bit j of `act` is set iff
+                    // pixel j of the lane's f32x8 group (the 8 lanes that differ in lane bits 1-3)
+                    // has non-zero coverage somewhere.
+                    uint32_t act = 0;
+#pragma unroll
+                    for (int q = 0; q < 4; ++q)
+                        act |= (cov[q].x != 0.0f ? 1u : 0u) << (2 * q) | (cov[q].y != 0.0f ? 2u : 0u) << (2 * q);
+                    act |= __shfl_xor_sync(kFullMask, act, 2);
+                    act |= __shfl_xor_sync(kFullMask, act, 4);
+                    act |= __shfl_xor_sync(kFullMask, act, 8);
                     const f2 cr = f2_splat(__uint_as_float(h2.x)), cg = f2_splat(__uint_as_float(h2.y));
                     const f2 cb = f2_splat(__uint_as_float(h2.z)), ca = f2_splat(__uint_as_float(h2.w));
                     if (apply_clip) {  // src_a = fill.a * coverage * mask (mod.rs:425-429)
@@ -417,10 +427,11 @@
                         const f2 inv_dst_a_src_a = mul2(inv_dst_a, sa);
                         const f2 inv_src_a = sub2(f2_splat(1.0f), sa);
                         const f2 dst_a_src_a = mul2(da[q], sa);
-                        dr[q] = compose2(dr[q], cr, cr, inv_dst_a_src_a, dst_a_src_a, inv_src_a);
-                        dg[q] = compose2(dg[q], cg, cg, inv_dst_a_src_a, dst_a_src_a, inv_src_a);
-                        db[q] = compose2(db[q], cb, cb, inv_dst_a_src_a, dst_a_src_a, inv_src_a);
-                        da[q] = fma2(da[q], inv_src_a, sa);
+                        const uint32_t a2 = act >> (2 * q);
+                        dr[q] = keep2(a2, compose2(dr[q], cr, cr, inv_dst_a_src_a, dst_a_src_a, inv_src_a), dr[q]);
+                        dg[q] = keep2(a2, compose2(dg[q], cg, cg, inv_dst_a_src_a, dst_a_src_a, inv_src_a), dg[q]);
+                        db[q] = keep2(a2, compose2(db[q], cb, cb, inv_dst_a_src_a, dst_a_src_a, inv_src_a), db[q]);
+                        da[q] = keep2(a2, fma2(da[q], inv_src_a, sa), da[q]);
                     }
                     __syncwarp();
                     continue;
