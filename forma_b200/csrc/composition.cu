@@ -43,6 +43,7 @@ static const OptionName kOptionNames[] = {
     {"sort_big_log2", &Options::sort_big_log2, 10, 30}, {"test_gap_cap", &Options::test_gap_cap, 0, 1 << 30},
     {"paint_lpt", &Options::paint_lpt, 0, 1},         {"band_filter", &Options::band_filter, 0, 1},
     {"paint_wide", &Options::paint_wide, 0, 1},       {"sort_scan_log2", &Options::sort_scan_log2, 10, 31},
+    {"paint_solid", &Options::paint_solid, 0, 1},
     {"sync_free", &Options::sync_free, 0, 1},         {"test_fast_shrink", &Options::test_fast_shrink, 0, 1},
     {"host_slices", &Options::host_slices, 1, 16},    {"slice_bands", &Options::slice_bands, 1, 16},
     {"slice_min_points", &Options::slice_min_points, 0, 1 << 30}, {"slice_chain", &Options::slice_chain, 0, 1},
@@ -291,7 +292,7 @@ int Composition::rebuild_tables(int64_t cache_id) {
     std::fill(h_order_to_style.ptr, h_order_to_style.ptr + n_orders, -1);
     std::fill(h_geom_slot.ptr, h_geom_slot.ptr + n_geoms, -1);
     uint32_t slot = 0, n_styles = 0;
-    bool any_xf = false;
+    bool any_xf = false, solid_over = true;
     FORMA_CUDA_TRY(h_layer_bits.reserve(layers.size() + 1));
     std::unordered_map<std::string, uint32_t> interned;
     std::vector<int32_t> order_to_slot(n_orders, -1);
@@ -305,6 +306,7 @@ int Composition::rebuild_tables(int64_t cache_id) {
         h_layer_bits.ptr[slot] = (kv.first & 0x1FFFFFu) | (r.enabled << 21);
         any_xf = any_xf || l.has_xf;
         StyleRec s = l.props.rec;
+        solid_over = solid_over && s.func == 0u && !s.is_clipped && s.fill_type == 0u && s.blend_mode == 0u;
         s.stop_first = (uint32_t)stops.size();
         s.stop_count = (uint32_t)l.props.stops.size();
         stops.insert(stops.end(), l.props.stops.begin(), l.props.stops.end());
@@ -358,6 +360,7 @@ int Composition::rebuild_tables(int64_t cache_id) {
     if (!texels.empty()) std::memcpy(h_texels.ptr, texels.data(), texels.size() * sizeof(uint16_t));
     n_layer_recs = slot;
     layers_have_xf = any_xf;
+    solid_over_only = solid_over;
     n_style_recs = n_styles;
     n_stops = stops.size();
     n_texels = texels.size();

@@ -161,6 +161,9 @@ class Composition {
     // rasterizer emits the pixel segments already ordered by layer and the
     // (stable) sort only needs the tile_x / tile_y digits.
     bool layers_in_order = false;
+    // Every layer is a Draw layer with a solid fill, BlendMode::Over and no clip: its frames are
+    // painted by the lean build of the paint kernel (launch_paint).
+    bool solid_over_only = false;
     int64_t tables_cache_id = -2;     // cache id the `unchanged` bits were uploaded for
     int rebuild_tables(int64_t cache_id);  // FORMA_STATUS_*
 

@@ -21,7 +21,8 @@ struct Options {
     int sort_scan_log2 = 22; // key-only sorts: key count from which the reduce-then-scan passes replace the single-sweep ones
     int test_gap_cap = 0;    // test hook: cap of the speculative carry-only-entry launch (0 = none)
     int paint_lpt = 1;       // heavy tiles first (longest-processing-time order) in the paint kernel
-    int paint_wide = 0;      // 1: the paint kernel built for 6 CTAs / SM (up to 168 registers) instead of 8 (128); sRGB8 frames only (float frames always use the 8-CTA build)
+    int paint_wide = 0;      // 1: the general paint kernel built for 6 CTAs / SM (up to 168 registers) instead of 8 (128); sRGB8 frames only (float frames always use the 8-CTA build)
+    int paint_solid = 1;     // sRGB8 frames whose layers are all solid `Over` fills without clips are painted by the paint kernel's lean build (0: by the general one)
     int band_filter = 1;     // a render cropped to a band of rows only makes the band's geometry resident
     int sync_free = 1;       // painter tables without count read-backs when the previous frame's counts bound this one's (redone the slow way if they do not)
     int test_fast_shrink = 0;  // test hook: halve the bounds of the sync-free tables (forces the redo)
@@ -268,10 +269,11 @@ void launch_merge_entries(const PaintScene& S, const uint64_t* cell_key, uint32_
                           const uint4* gap_carry, uint64_t* ekey, EntryRec* recs, uint8_t* eflags, uint2* tile_range,
                           uint32_t* heavy, uint32_t* heavy_count, cudaStream_t st, const DevCounts& dc = DevCounts());
 // view_rows != 0: S stacks views of view_rows tile rows each (ViewArgs); gradients and textures are
-// then sampled in each view's own coordinates.
+// then sampled in each view's own coordinates. solid_over: every layer of the frame is a solid `Over`
+// fill without clips (Composition::solid_over_only); the lean build of the kernel paints it.
 void launch_paint(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range, const uint32_t* heavy,
                   const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st,
-                  uint32_t view_rows = 0);
+                  uint32_t view_rows = 0, bool solid_over = false);
 // launch_paint for a linear float frame of `bpp` bytes per pixel: 8 (RGBA16F) or 16 (RGBA32F), the
 // painter's planes in channel order where launch_paint stores their sRGB bytes (see
 // forma_renderer_render_linear). `framebuffer` and S.stride: multiples of 4 bytes.

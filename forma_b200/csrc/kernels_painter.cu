@@ -321,6 +321,25 @@ __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, kMinBlocks)
 #include "paint_kernel_body.cuh"
 #undef FORMA_PAINT_FRAME_TY
 }
+// paint_kernel / paint_views_kernel for a frame whose layers are all solid `Over` fills without clips
+// (Composition::solid_over_only): the same body without the code of other styles and clips. Built
+// for 8 CTAs / SM it needs 96 registers and no spills, so 10 CTAs fit an SM; the bounds 10 and 12
+// (95 registers; 80 with 74 B of spills) were no faster on paris4k and slower on cubics100k.
+#define FORMA_PAINT_SOLID_OVER
+template <int kMinBlocks>
+__global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, kMinBlocks) paint_solid_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles) {
+#define FORMA_PAINT_FRAME_TY(ty) (ty)
+#include "paint_kernel_body.cuh"
+#undef FORMA_PAINT_FRAME_TY
+}
+template <int kMinBlocks>
+__global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, kMinBlocks)
+    paint_views_solid_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles, uint32_t view_rows) {
+#define FORMA_PAINT_FRAME_TY(ty) ((ty) % view_rows)
+#include "paint_kernel_body.cuh"
+#undef FORMA_PAINT_FRAME_TY
+}
+#undef FORMA_PAINT_SOLID_OVER
 
 // ---------------------------------------------------------------------------
 // Linear float frames: the painter's planes as they are, RGBA16F (8-byte pixels, each value
@@ -536,37 +555,45 @@ void launch_f32x2_selftest(const float* a, const float* b, const float* c, uint3
 
 void launch_paint(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range, const uint32_t* heavy,
                   const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st,
-                  uint32_t view_rows) {
+                  uint32_t view_rows, bool solid_over) {
     if (S.tx_hi <= S.tx_lo || S.ty_hi <= S.ty_lo) return;
     uint32_t n_tiles = (S.tx_hi - S.tx_lo) * (S.ty_hi - S.ty_lo);
     cudaMemsetAsync(tile_counter, 0, sizeof(uint32_t), st);
     PaintInputs in{segs, recs, tile_range, heavy, heavy_count, S.tiles_x * S.tiles_y, eflags, framebuffer, tile_counter};
     // Persistent warps: enough CTAs to fill every SM at the kernel's occupancy (per device).
-    // Option paint_wide = 1 selects the build with up to 168 registers (6 CTAs / SM) instead of 128 (8 CTAs / SM).
-    static int blocks_per_sm[2][2][kMaxDevices] = {{{0}}};
+    // Build 0: the general kernel at 128 registers (8 CTAs / SM); 1: option paint_wide = 1, up to 168
+    // registers (6 CTAs / SM); 2: a solid `Over` frame (option paint_solid = 1), the lean build at 96
+    // registers (10 CTAs / SM).
+    static int blocks_per_sm[2][3][kMaxDevices] = {{{0}}};
     static std::mutex config_mu;  // several host threads may render on one device
-    const int wide = options().paint_wide ? 1 : 0, views = view_rows ? 1 : 0;
+    const int build = solid_over && options().paint_solid ? 2 : options().paint_wide ? 1 : 0, views = view_rows ? 1 : 0;
+    const void* kernels[2][3] = {{(const void*)paint_kernel<8>, (const void*)paint_kernel<6>, (const void*)paint_solid_kernel<8>},
+                                 {(const void*)paint_views_kernel<8>, (const void*)paint_views_kernel<6>, (const void*)paint_views_solid_kernel<8>}};
     int per_sm = 0;
     {
         std::lock_guard<std::mutex> lk(config_mu);
-        int& slot = blocks_per_sm[views][wide][current_device_index()];
+        int& slot = blocks_per_sm[views][build][current_device_index()];
         if (!slot) {
-            const void* k = views ? (wide ? (const void*)paint_views_kernel<6> : (const void*)paint_views_kernel<8>)
-                                  : (wide ? (const void*)paint_kernel<6> : (const void*)paint_kernel<8>);
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&slot, k, kPaintWarpsPerBlock * 32, 0);
+            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&slot, kernels[views][build], kPaintWarpsPerBlock * 32, 0);
             if (slot < 1) slot = 1;
         }
         per_sm = slot;
     }
     const uint32_t want = (uint32_t)(per_sm * device_sm_count());
     const uint32_t need = (n_tiles + kPaintWarpsPerBlock - 1) / kPaintWarpsPerBlock;
+    const dim3 grid(min(want, need)), block(kPaintWarpsPerBlock * 32);
     if (views) {
-        if (wide) paint_views_kernel<6><<<min(want, need), kPaintWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles, view_rows);
-        else paint_views_kernel<8><<<min(want, need), kPaintWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles, view_rows);
-    } else if (wide) {
-        paint_kernel<6><<<min(want, need), kPaintWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles);
+        switch (build) {
+            case 0: paint_views_kernel<8><<<grid, block, 0, st>>>(S, in, n_tiles, view_rows); break;
+            case 1: paint_views_kernel<6><<<grid, block, 0, st>>>(S, in, n_tiles, view_rows); break;
+            default: paint_views_solid_kernel<8><<<grid, block, 0, st>>>(S, in, n_tiles, view_rows); break;
+        }
     } else {
-        paint_kernel<8><<<min(want, need), kPaintWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles);
+        switch (build) {
+            case 0: paint_kernel<8><<<grid, block, 0, st>>>(S, in, n_tiles); break;
+            case 1: paint_kernel<6><<<grid, block, 0, st>>>(S, in, n_tiles); break;
+            default: paint_solid_kernel<8><<<grid, block, 0, st>>>(S, in, n_tiles); break;
+        }
     }
 }
 

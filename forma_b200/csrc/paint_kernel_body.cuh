@@ -5,6 +5,14 @@
 // A kernel that stores something other than sRGB8 defines both store hooks:
 //   FORMA_PAINT_STORE_SOLID(dst): the tile folded to the one colour dst (Rgba, no layer cache);
 //   FORMA_PAINT_STORE_PIXELS():   the lane's painted pixels, planes dr / dg / db / da at (x0, ty * 16 + row).
+// A kernel for frames whose layers are all solid `Over` fills without clips (Composition::solid_over_only)
+// defines FORMA_PAINT_SOLID_OVER: clip state, pass B, gradient prefetch and the blend paths of every
+// other style fold away, and what remains is the same code as for such layers in the general build.
+#ifdef FORMA_PAINT_SOLID_OVER
+    constexpr bool kSolidOver = true;
+#else
+    constexpr bool kSolidOver = false;
+#endif
     __shared__ __align__(16) WarpSmem s_warp[kPaintWarpsPerBlock];
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
     WarpSmem& W = s_warp[warp];
@@ -91,7 +99,7 @@
         for (uint32_t p0 = b; p0 < e; p0 += 32u) {
             uint32_t p = p0 + lane;
             uint32_t f = p < e ? (uint32_t)in.eflags[p] : kFlagUnchanged;
-            any_clip |= __any_sync(kFullMask, (f & kFlagClipish) != 0u);
+            if (!kSolidOver) any_clip |= __any_sync(kFullMask, (f & kFlagClipish) != 0u);
             all_unchanged = all_unchanged && !__any_sync(kFullMask, (f & kFlagUnchanged) == 0u);
         }
 
@@ -118,7 +126,7 @@
         }
 
         // Pass B: skip_trivial_clips (sequential; only tiles that contain clips).
-        if (any_clip) {
+        if (!kSolidOver && any_clip) {
             if (lane == 0) {
                 bool has_clip = false, clip_full = false, clip_used = false;
                 uint32_t clip_last = 0, clip_i = 0;
@@ -281,7 +289,7 @@
             uint32_t grad_word = 0, grad_next = 0;
             {
                 const uint4 h = hdr4[0];
-                if (h.w & kMetaSmallGradient) grad_next = reinterpret_cast<const uint32_t*>(&S.grads[hdr4[3].x])[lane];
+                if (!kSolidOver && (h.w & kMetaSmallGradient)) grad_next = reinterpret_cast<const uint32_t*>(&S.grads[hdr4[3].x])[lane];
                 const uint32_t s0 = h.y, s1 = h.z;
                 uint64_t a0 = 0, a1 = 0;
                 if (s0 + lane < s1) a0 = in.segs[s0 + lane];
@@ -308,7 +316,7 @@
                     grad_word = grad_next;  // word `lane` of this entry's gradient record (if it has one)
                     if (k + 1u < cnt) {
                         const uint4 g = hdr4[(k + 1u) * 4u];
-                        if (g.w & kMetaSmallGradient)
+                        if (!kSolidOver && (g.w & kMetaSmallGradient))
                             grad_next = reinterpret_cast<const uint32_t*>(&S.grads[hdr4[(k + 1u) * 4u + 3u].x])[lane];
                         if (g.z > g.y) scatter_entry(in.segs, g.y, g.z, c0, c1, W.cells[(k + 1u) & 1u], lane);
                     }
@@ -367,7 +375,7 @@
 
                 if (clip_active && clip_last < layer) clip_active = false;  // mod.rs:302-306
 
-                if (meta_func(meta) == 1u) {  // clip_at, mod.rs:449-464
+                if (!kSolidOver && meta_func(meta) == 1u) {  // clip_at, mod.rs:449-464
                     if (!clip_active) {
                         clip_active = true;
                         clip_last = layer + h3.y;
@@ -378,7 +386,7 @@
                     __syncwarp();
                     continue;
                 }
-                const bool apply_clip = meta_is_clipped(meta) && !(flags & kFlagSkipClip);
+                const bool apply_clip = !kSolidOver && meta_is_clipped(meta) && !(flags & kFlagSkipClip);
                 bool nonzero = false;
 #pragma unroll
                 for (int q = 0; q < 4; ++q) nonzero = nonzero || cov[q].x != 0.0f || cov[q].y != 0.0f;
@@ -433,6 +441,10 @@
                         db[q] = keep2(a2, compose2(db[q], cb, cb, inv_dst_a_src_a, dst_a_src_a, inv_src_a), db[q]);
                         da[q] = keep2(a2, fma2(da[q], inv_src_a, sa), da[q]);
                     }
+                    __syncwarp();
+                    continue;
+                }
+                if (kSolidOver) {  // (no other layer in such a frame)
                     __syncwarp();
                     continue;
                 }

@@ -707,7 +707,13 @@ int Renderer::bind_batch(Composition* const* comps, uint32_t n, PaintScene& S, u
 int Renderer::paint_step(const FrameRequest& q, const PaintScene& S, const FramePlan& p, const uint32_t* heavy_lists,
                          uint32_t* paint_launches) {
     if (q.rgba.ptr) {
-        const int st = paint(S, p.rgba.ptr, q.rgba.ptr, q.rgba.stride, p.in_bands, heavy_lists, paint_launches, p.rows, q.rgba.bpp);
+        bool solid_over = true;
+        if (q.kind == FrameKind::batch)
+            for (const Composition* c : batch_distinct) solid_over = solid_over && c->solid_over_only;
+        else
+            solid_over = solid_over && q.comp->solid_over_only;
+        const int st =
+            paint(S, p.rgba.ptr, q.rgba.ptr, q.rgba.stride, p.in_bands, heavy_lists, paint_launches, p.rows, q.rgba.bpp, solid_over);
         if (st || !q.ids.ptr) return st;
         ++*paint_launches;
     }
@@ -999,8 +1005,9 @@ int Renderer::queue_row_costs(const PaintScene& S, uint32_t n) {
 // of band k run dry: the kernels overlap at their tails, and the PCIe transfer of a band overlaps
 // the painting of the following ones.
 // bpp: bytes per pixel of fb, 4 (sRGB8), or 8 / 16 for a linear float frame (never in bands).
+// solid_over: see launch_paint (sRGB8 frames; a float frame is painted by the general build).
 int Renderer::paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t stride, bool in_bands, const uint32_t* heavy_lists,
-                    uint32_t* paint_launches, uint32_t view_rows, uint32_t bpp) {
+                    uint32_t* paint_launches, uint32_t view_rows, uint32_t bpp, bool solid_over) {
     *paint_launches = 1;
     if (in_bands) {
         if (!band_streams_ok) {
@@ -1021,7 +1028,8 @@ int Renderer::paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t 
             Sb.ty_hi = S.ty_lo + paint_rows * (k + 1u) / kCopyBands;
             cudaStream_t bs = kCopyBands > 1u ? band_stream[k] : stream;
             if (kCopyBands > 1u) FORMA_CUDA_TRY(cudaStreamWaitEvent(bs, band_ev[kMaxCopyBands], 0));
-            launch_paint(Sb, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), eflags.ptr, fb, totals.ptr + 16 + k, bs);
+            launch_paint(Sb, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), eflags.ptr, fb, totals.ptr + 16 + k, bs, 0,
+                         solid_over);
             ++launches;
             const int st = copy_to_host(Sb, buffer, fb, stride, bs);
             if (st) return st;
@@ -1030,7 +1038,8 @@ int Renderer::paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t 
         for (uint32_t k = 0; kCopyBands > 1u && k < kCopyBands; ++k) FORMA_CUDA_TRY(cudaStreamWaitEvent(stream, band_ev[k], 0));
         *paint_launches = kCopyBands;
     } else if (bpp == 4u) {
-        launch_paint(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), eflags.ptr, fb, totals.ptr + 3, stream, view_rows);
+        launch_paint(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), eflags.ptr, fb, totals.ptr + 3, stream, view_rows,
+                     solid_over);
         ++launches;
     } else {
         launch_paint_linear(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), eflags.ptr, fb, totals.ptr + 3, stream,

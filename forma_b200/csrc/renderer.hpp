@@ -314,7 +314,7 @@ class Renderer {
                      DevCounts& dc);
     int queue_row_costs(const PaintScene& S, uint32_t n);
     int paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t stride, bool in_bands, const uint32_t* heavy_lists,
-              uint32_t* paint_launches, uint32_t view_rows = 0, uint32_t bpp = 4);
+              uint32_t* paint_launches, uint32_t view_rows = 0, uint32_t bpp = 4, bool solid_over = false);
     int copy_to_host(const PaintScene& S, uint8_t* buffer, const uint8_t* fb, uint64_t stride, cudaStream_t s, uint32_t bpp = 4);
     int scatter_written_tiles(const PaintScene& S, const uint8_t* fb, uint8_t* buffer, uint64_t stride);
 };
