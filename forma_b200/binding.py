@@ -314,6 +314,12 @@ SIGNATURES = {
                                                _u32p, _fp, C.c_uint32, C.POINTER(_CTimings)]),
     "renderer_render_batch_linear_device": (C.c_int, [_vp, C.POINTER(_vp), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64,
                                                       C.c_uint64, _u32p, _fp, C.c_uint32, C.POINTER(_CTimings)]),
+    "renderer_render_over_device": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_uint64, C.c_uint64, _u32p, C.POINTER(_CRect), C.c_uint32,
+                                              C.POINTER(_CTimings)]),
+    "renderer_render_views_over_device": (C.c_int, [_vp, _vp, _fp, C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
+                                                    _u32p, C.c_uint32, C.POINTER(_CTimings)]),
+    "renderer_render_batch_over_device": (C.c_int, [_vp, C.POINTER(_vp), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64,
+                                                    C.c_uint64, _u32p, C.c_uint32, C.POINTER(_CTimings)]),
     "renderer_launch_count": (C.c_uint64, [_vp]),
     "renderer_stage_times": (None, [_vp, C.POINTER(C.c_double)]),
     "renderer_counters": (None, [_vp, _u64p]),
@@ -365,8 +371,14 @@ SORT_DEBUG_SYMBOLS = ("debug_sort_plan", "renderer_sort_pairs", "renderer_sort_b
 LINEAR_SYMBOLS = ("renderer_render_linear", "renderer_render_linear_device", "renderer_render_views_linear",
                   "renderer_render_views_linear_device", "renderer_render_batch_linear", "renderer_render_batch_linear_device")
 
+# The same for frames over a background (Renderer.render_over_device, render_views_over_device,
+# render_batch_over_device).
+OVER_SYMBOLS = ("renderer_render_over_device", "renderer_render_views_over_device", "renderer_render_batch_over_device")
+
 # Pixel formats of linear frames: name -> (FORMA_PIXEL_*, bytes per pixel, element dtype).
 PIXEL_FORMATS = {"f16": (1, 8, np.float16), "f32": (2, 16, np.float32)}
+# ... and of frames over a background, which may be sRGB8 as well.
+OVER_FORMATS = {"srgb8": (0, 4, np.uint8), **PIXEL_FORMATS}
 
 
 def pixel_format(fmt: str):
@@ -376,8 +388,15 @@ def pixel_format(fmt: str):
     return PIXEL_FORMATS[fmt]
 
 
+def over_format(fmt: str):
+    """(FORMA_PIXEL_* code, bytes per pixel, numpy dtype) of "srgb8", "f16" or "f32"."""
+    if fmt not in OVER_FORMATS:
+        raise ValueError(f"pixel format {fmt!r}: 'srgb8', 'f16' or 'f32'")
+    return OVER_FORMATS[fmt]
+
+
 _OPTIONAL_SYMBOLS = frozenset(ID_FRAME_SYMBOLS + VIEW_SYMBOLS + BATCH_SYMBOLS + STACK_ID_SYMBOLS + SORT_DEBUG_SYMBOLS +
-                              LINEAR_SYMBOLS)
+                              LINEAR_SYMBOLS + OVER_SYMBOLS)
 
 
 class Api:
@@ -785,12 +804,14 @@ class Renderer:
 
     def _frame(self, fn, what, composition, ptr, width, height, stride, colors, crop, tail, timings):
         """Calls `fn`, a single-frame entry point: fn(renderer, composition, ptr, width, stride, height,
-        [channels, clear colour,] crop, *tail, timings), with channels and clear colour when
-        `colors` = (channels, clear_color) is given."""
+        [channels, [clear colour,]] crop, *tail, timings), with channels and clear colour when
+        `colors` = (channels, clear_color) is given, channels alone when clear_color is None."""
         stride = width * 4 if stride is None else stride
-        ch, cc, rect = self._common(*(colors or (RGBA, Color())), crop)
+        channels, clear = colors or (RGBA, Color())
+        ch, cc, rect = self._common(channels, Color() if clear is None else clear, crop)
+        colour_args = () if not colors else (ch,) if clear is None else (ch, cc)
         t = _CTimings() if timings else None
-        st = fn(self._h, composition._h, ptr, width, stride, height, *((ch, cc) if colors else ()),
+        st = fn(self._h, composition._h, ptr, width, stride, height, *colour_args,
                 C.byref(rect) if rect is not None else None, *tail, C.byref(t) if t is not None else None)
         self._api.check(st, what)
         return _timings(t)
@@ -851,13 +872,14 @@ class Renderer:
         frames: first_args(first, count) gives a chunk's leading arguments (views or handles,
         count), then come its targets. rgba = (ptr or None, stride, frame_stride, channels,
         clear_color) and ids = (ptr, stride, frame_stride, min_coverage), either may be None; a
-        stride of None takes its default (bpp * width, height * stride; IDs: bpp 4). An entry point
-        with both takes the ID target's arguments without width and height. `tail` follows the
-        targets."""
+        stride of None takes its default (bpp * width, height * stride; IDs: bpp 4); a clear colour
+        of None is not passed (frames over a background). An entry point with both takes the ID
+        target's arguments without width and height. `tail` follows the targets."""
         chunk = max(self.max_views(height), 1)
         if rgba is not None:
             rgba_ptr, stride, frame_stride = rgba[0], *self._strides(width, height, rgba[1], rgba[2], bpp)
-            ch, cc, _ = self._common(rgba[3], rgba[4], None)
+            ch, cc, _ = self._common(rgba[3], Color() if rgba[4] is None else rgba[4], None)
+            colour_args = [ch] if rgba[4] is None else [ch, cc]
         if ids is not None:
             ids_ptr, ids_stride, ids_frame_stride = ids[0], *self._strides(width, height, ids[1], ids[2])
         t = None
@@ -865,7 +887,7 @@ class Renderer:
             args = list(first_args(first, min(chunk, n - first)))
             if rgba is not None:
                 ptr = C.c_void_p(rgba_ptr + first * frame_stride) if rgba_ptr is not None else None
-                args += [ptr, width, stride, height, frame_stride, ch, cc]
+                args += [ptr, width, stride, height, frame_stride, *colour_args]
             if ids is not None:
                 ptr = C.c_void_p(ids_ptr + first * ids_frame_stride)
                 layout = [ids_stride, ids_frame_stride] if rgba is not None else [width, ids_stride, height, ids_frame_stride]
@@ -1082,6 +1104,41 @@ class Renderer:
         n, args = self._batch_args(comps)
         return self._stack(self._api.renderer_render_batch_linear_device, "Renderer::render_batch_linear_device", args, n, width,
                            height, (int(device_ptr), stride, frame_stride, channels, clear_color), None, timings, bpp, (code,))
+
+    def render_over_device(self, composition: Composition, device_ptr: int, width: int, height: int, channels=RGBA,
+                           crop: Optional[Rect] = None, format: str = "srgb8", stride: Optional[int] = None,
+                           timings: bool = True) -> Optional[Timings]:
+        """Draws the composition over the pixels already in device memory (see
+        include/forma_b200.h: forma_renderer_render_over_device): each pixel's own value, decoded,
+        is its clear colour, so the result is render_device's (format "srgb8") or
+        render_linear_device's ("f16", "f32") with that clear colour, pixel by pixel. With the
+        defaults, the data_ptr() of a contiguous [height, width, 4] uint8 / float16 / float32 CUDA
+        tensor. `channels`: a permutation of R, G, B, A (for "srgb8" with A last). Only the crop's
+        tile rectangle is read and written."""
+        code, bpp, _ = over_format(format)
+        return self._frame(self._api.renderer_render_over_device, "Renderer::render_over_device", composition, C.c_void_p(device_ptr),
+                           width, height, width * bpp if stride is None else stride, (channels, None), crop, (code,), timings)
+
+    def render_views_over_device(self, composition: Composition, views, device_ptr: int, width: int, height: int, channels=RGBA,
+                                 format: str = "srgb8", stride: Optional[int] = None, view_stride: Optional[int] = None,
+                                 timings: bool = True) -> Optional[Timings]:
+        """render_views over the frames already in device memory (see render_over_device): with the
+        defaults, the data_ptr() of a contiguous [N, height, width, 4] uint8 / float16 / float32 CUDA
+        tensor. Chunked like render_views."""
+        code, bpp, _ = over_format(format)
+        n, args = self._view_args(composition, views)
+        return self._stack(self._api.renderer_render_views_over_device, "Renderer::render_views_over_device", args, n, width, height,
+                           (int(device_ptr), stride, view_stride, channels, None), None, timings, bpp, (code,))
+
+    def render_batch_over_device(self, comps, device_ptr: int, width: int, height: int, channels=RGBA, format: str = "srgb8",
+                                 stride: Optional[int] = None, frame_stride: Optional[int] = None,
+                                 timings: bool = True) -> Optional[Timings]:
+        """render_batch over the frames already in device memory (see render_over_device): frame c
+        of comps over frame c of the [N, height, width, 4] tensor. Chunked like render_batch."""
+        code, bpp, _ = over_format(format)
+        n, args = self._batch_args(comps)
+        return self._stack(self._api.renderer_render_batch_over_device, "Renderer::render_batch_over_device", args, n, width, height,
+                           (int(device_ptr), stride, frame_stride, channels, None), None, timings, bpp, (code,))
 
     def launch_count(self) -> int:
         return int(self._api.renderer_launch_count(self._h))

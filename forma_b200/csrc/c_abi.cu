@@ -555,6 +555,38 @@ int forma_renderer_render_batch_linear_device(forma_renderer* r, forma_compositi
     q.rgba = {static_cast<uint8_t*>(device_buffer), true, width_stride, frame_stride};
     return render_linear(r, q, format, nullptr, comps);
 }
+// Frames over a background: the RGBA target in device memory, painted over its own pixels in any
+// of the three formats (render_linear's checks and refusals, and check_request's over rules).
+static int render_over(forma_renderer* r, FrameRequest q, uint32_t format, forma_composition* c, forma_composition* const* comps) {
+    q.rgba.over = true;
+    if (format == FORMA_PIXEL_SRGB8) {
+        q.rgba.bpp = 4u;
+        return render_request(r, q, c, comps);
+    }
+    return render_linear(r, q, format, c, comps);
+}
+int forma_renderer_render_over_device(forma_renderer* r, forma_composition* c, void* device_buffer, uint64_t width, uint64_t width_stride,
+                                      uint64_t height, const uint32_t channels[4], const forma_rect* crop, uint32_t format,
+                                      forma_timings* timings) {
+    FrameRequest q{FrameKind::single, 0, width, height, channels, nullptr, timings, crop};
+    q.rgba = {static_cast<uint8_t*>(device_buffer), true, width_stride};
+    return render_over(r, q, format, c, nullptr);
+}
+int forma_renderer_render_views_over_device(forma_renderer* r, forma_composition* c, const float* views, uint32_t n, void* device_buffer,
+                                            uint64_t width, uint64_t width_stride, uint64_t height, uint64_t view_stride,
+                                            const uint32_t channels[4], uint32_t format, forma_timings* timings) {
+    FrameRequest q{FrameKind::views, n, width, height, channels, nullptr, timings};
+    q.views = views;
+    q.rgba = {static_cast<uint8_t*>(device_buffer), true, width_stride, view_stride};
+    return render_over(r, q, format, c, nullptr);
+}
+int forma_renderer_render_batch_over_device(forma_renderer* r, forma_composition* const* comps, uint32_t n, void* device_buffer,
+                                            uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride,
+                                            const uint32_t channels[4], uint32_t format, forma_timings* timings) {
+    FrameRequest q{FrameKind::batch, n, width, height, channels, nullptr, timings};
+    q.rgba = {static_cast<uint8_t*>(device_buffer), true, width_stride, frame_stride};
+    return render_over(r, q, format, nullptr, comps);
+}
 // --- shared frames (multi-GPU, see include/forma_b200.h) -----------------------
 static_assert(sizeof(cudaIpcMemHandle_t) == sizeof(forma_ipc_handle), "CUDA IPC handles are 64 bytes");
 int forma_shared_frame_create(int device, uint64_t bytes, void** device_ptr, forma_ipc_handle* handle) {

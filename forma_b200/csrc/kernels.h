@@ -280,6 +280,19 @@ void launch_paint(const PaintScene& S, const uint64_t* segs, const EntryRec* rec
 void launch_paint_linear(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range, const uint32_t* heavy,
                          const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st,
                          uint32_t view_rows, uint32_t bpp);
+// launch_paint over the pixels already in `framebuffer` (see forma_renderer_render_over_device):
+// each pixel's own value, decoded, is its clear colour; tiles without entries are not written.
+// bpp 4 (sRGB8, channels a permutation with A last), 8 (RGBA16F) or 16 (RGBA32F, both: any
+// permutation); S.channels are not upgraded (the kernels upgrade Alpha -> One per pixel).
+// `framebuffer` and S.stride: multiples of 4 bytes.
+void launch_paint_over(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range, const uint32_t* heavy,
+                       const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st,
+                       uint32_t view_rows, uint32_t bpp);
+// The inverse of launch_repack_views: rows [0, height) of the n_views frames at src + b * view_stride
+// (row r at + r * stride) to the stacked frame at dst, frame b's first row at
+// dst + b * view_rows_px * dst_stride. `width` in 4-byte words; every pointer and stride a multiple of 4.
+void launch_unpack_views(const uint8_t* src, uint64_t stride, uint64_t view_stride, uint8_t* dst, uint64_t dst_stride,
+                         uint32_t view_rows_px, uint32_t width, uint32_t height, uint32_t n_views, cudaStream_t st);
 // Copies rows [0, height) of the n_views views of a stacked frame (view b's first row at
 // src + b * view_rows_px * src_stride) to dst + b * view_stride, row r at + r * stride.
 void launch_repack_views(const uint8_t* src, uint64_t src_stride, uint32_t view_rows_px, uint8_t* dst, uint64_t stride,

@@ -38,6 +38,7 @@
 #include <mutex>
 #include "paint_common.cuh"
 #include "paint_math.cuh"
+#include "srgb_decode.h"
 
 namespace forma {
 
@@ -427,6 +428,216 @@ __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, 8)
 #undef FORMA_PAINT_STORE_SOLID
 #undef FORMA_PAINT_STORE_PIXELS
 
+// ---------------------------------------------------------------------------
+// Frames over a background (forma_renderer_render_over_device): the frame's own pixels are each
+// pixel's clear colour. sRGB8 bytes decode through the table D (srgb_decode.h: every byte
+// round-trips through compute_srgb's encode) and alpha as byte / 255; RGBA16F through
+// __half2float; RGBA32F as stored. The channel order is a permutation of R, G, B, A (for sRGB8
+// with A last, see check_request).
+// ---------------------------------------------------------------------------
+__device__ const float kSrgbDecode[256] = FORMA_SRGB_DECODE_TABLE;
+
+// The byte (sRGB8) or value (float) position of each of R, G, B, A in a pixel: 2 bits each.
+__device__ __forceinline__ uint32_t channel_positions(const uint32_t ch[4]) {
+    uint32_t pos = 0;
+#pragma unroll
+    for (uint32_t k = 0; k < 4u; ++k) pos |= k << (2u * (ch[k] & 3u));
+    return pos;
+}
+__device__ __forceinline__ uint32_t pos_of(uint32_t pos, uint32_t c) { return (pos >> (2u * c)) & 3u; }
+
+// One background pixel into element `h` (0: x, 1: y) of the pair planes; its opaque bit at `bit`.
+__device__ __forceinline__ void put_pixel(f2& r, f2& g, f2& b, f2& a, uint32_t h, float vr, float vg, float vb, float va,
+                                          uint32_t& opaque, uint32_t bit) {
+    if (h == 0u) {
+        r.x = vr; g.x = vg; b.x = vb; a.x = va;
+    } else {
+        r.y = vr; g.y = vg; b.y = vb; a.y = va;
+    }
+    if (va == 1.0f) opaque |= 1u << bit;
+}
+
+// The lane's eight sRGB8 pixels of row py from column x0 (pixels outside the frame read as 0).
+__device__ __forceinline__ void load_srgb_run(const PaintScene& S, const uint8_t* fb, uint32_t py, uint32_t x0, bool vec,
+                                              const float* dec, uint32_t pos, f2 (&r)[4], f2 (&g)[4], f2 (&b)[4], f2 (&a)[4],
+                                              uint32_t& opaque) {
+    uint32_t w[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
+    if (py < S.height && x0 < S.width) {
+        const uint8_t* rowp = fb + (size_t)py * S.stride + (size_t)x0 * 4u;
+        if (vec && x0 + 8u <= S.width) {
+            const uint4 v0 = reinterpret_cast<const uint4*>(rowp)[0], v1 = reinterpret_cast<const uint4*>(rowp)[1];
+            w[0] = v0.x; w[1] = v0.y; w[2] = v0.z; w[3] = v0.w; w[4] = v1.x; w[5] = v1.y; w[6] = v1.z; w[7] = v1.w;
+        } else {
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+                if (x0 + (uint32_t)j < S.width) w[j] = reinterpret_cast<const uint32_t*>(rowp)[j];
+        }
+    }
+    const uint32_t sr = 8u * pos_of(pos, 0), sg = 8u * pos_of(pos, 1), sb = 8u * pos_of(pos, 2), sa = 8u * pos_of(pos, 3);
+    opaque = 0u;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const uint32_t v = w[j];
+        put_pixel(r[j >> 1], g[j >> 1], b[j >> 1], a[j >> 1], (uint32_t)j & 1u, dec[(v >> sr) & 0xFFu], dec[(v >> sg) & 0xFFu],
+                  dec[(v >> sb) & 0xFFu], (float)((v >> sa) & 0xFFu) / 255.0f, opaque, (uint32_t)j);
+    }
+}
+
+// The same for a float frame of `bpp` bytes per pixel (8: RGBA16F, 16: RGBA32F).
+__device__ __forceinline__ void load_linear_run(const PaintScene& S, const uint8_t* fb, uint32_t py, uint32_t x0, bool vec, uint32_t bpp,
+                                                uint32_t pos, f2 (&r)[4], f2 (&g)[4], f2 (&b)[4], f2 (&a)[4], uint32_t& opaque) {
+    opaque = 0u;
+    const bool row_in = py < S.height;
+    const uint8_t* rowp = fb + (size_t)py * S.stride + (size_t)x0 * bpp;
+    const uint32_t pr = pos_of(pos, 0), pg = pos_of(pos, 1), pb = pos_of(pos, 2), pa = pos_of(pos, 3);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        float v[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+        if (row_in && x0 + (uint32_t)j < S.width) {
+            const uint8_t* px = rowp + (size_t)j * bpp;
+            if (bpp == 8u) {
+                uint2 h;
+                if (vec) {
+                    h = *reinterpret_cast<const uint2*>(px);
+                } else {
+                    h.x = reinterpret_cast<const uint32_t*>(px)[0];
+                    h.y = reinterpret_cast<const uint32_t*>(px)[1];
+                }
+                v[0] = __half2float(__ushort_as_half((unsigned short)(h.x & 0xFFFFu)));
+                v[1] = __half2float(__ushort_as_half((unsigned short)(h.x >> 16)));
+                v[2] = __half2float(__ushort_as_half((unsigned short)(h.y & 0xFFFFu)));
+                v[3] = __half2float(__ushort_as_half((unsigned short)(h.y >> 16)));
+            } else if (vec) {
+                const float4 f = *reinterpret_cast<const float4*>(px);
+                v[0] = f.x; v[1] = f.y; v[2] = f.z; v[3] = f.w;
+            } else {
+                const float* f = reinterpret_cast<const float*>(px);
+                v[0] = f[0]; v[1] = f[1]; v[2] = f[2]; v[3] = f[3];
+            }
+        }
+        put_pixel(r[j >> 1], g[j >> 1], b[j >> 1], a[j >> 1], (uint32_t)j & 1u, v[pr], v[pg], v[pb], v[pa], opaque, (uint32_t)j);
+    }
+}
+
+// The per-pixel Alpha -> One upgrade (renderer.rs:87-92 with the pixel's background as clear colour):
+// an opaque background gives alpha 1 whatever was painted. The channel order is a permutation, so
+// storing alpha 1 is storing ONE.
+__device__ __forceinline__ void upgrade_alpha(f2 (&a)[4], uint32_t opaque) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        if ((opaque >> (2 * q)) & 1u) a[q].x = 1.0f;
+        if ((opaque >> (2 * q + 1)) & 1u) a[q].y = 1.0f;
+    }
+}
+
+// compute_srgb + LinearLayout::write of the lane's eight pixels, as the body stores them. With A the
+// last channel, a solid tile's to_srgb_bytes (position 3 unencoded) is this encode of its colour.
+__device__ __forceinline__ void store_srgb_run(const PaintScene& S, uint8_t* fb, uint32_t py, uint32_t x0, const f2 (&dr)[4],
+                                               const f2 (&dg)[4], const f2 (&db)[4], const f2 (&da)[4], bool vec, bool rgba_order) {
+    if (py >= S.height || x0 >= S.width) return;
+    uint32_t out[8];
+    if (rgba_order) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            uint32_t r0, r1, g0, g1, b0, b1, a0, a1;
+            to_byte2(srgb2(dr[q]), r0, r1);
+            to_byte2(srgb2(dg[q]), g0, g1);
+            to_byte2(srgb2(db[q]), b0, b1);
+            to_byte2(da[q], a0, a1);
+            out[2 * q] = r0 | (g0 << 8) | (b0 << 16) | (a0 << 24);
+            out[2 * q + 1] = r1 | (g1 << 8) | (b1 << 16) | (a1 << 24);
+        }
+    } else {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            out[2 * q] = srgb_bytes_any_order(dr[q].x, dg[q].x, db[q].x, da[q].x, S.channels);
+            out[2 * q + 1] = srgb_bytes_any_order(dr[q].y, dg[q].y, db[q].y, da[q].y, S.channels);
+        }
+    }
+    uint8_t* rowp = fb + (size_t)py * S.stride + (size_t)x0 * 4u;
+    if (vec && x0 + 8u <= S.width) {
+        reinterpret_cast<uint4*>(rowp)[0] = make_uint4(out[0], out[1], out[2], out[3]);
+        reinterpret_cast<uint4*>(rowp)[1] = make_uint4(out[4], out[5], out[6], out[7]);
+    } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+            if (x0 + (uint32_t)j < S.width) reinterpret_cast<uint32_t*>(rowp)[j] = out[j];
+    }
+}
+
+// paint_kernel / paint_views_kernel over the frame's own sRGB8 pixels, and their linear twins over
+// float pixels. The general build at 8 CTAs / SM whatever paint_wide and paint_solid say. D is
+// copied to shared memory once per CTA: the eight bytes of a lane index it at random, which the
+// constant cache would serialise.
+#define FORMA_PAINT_OVER_SRGB_PROLOGUE                                          \
+    __shared__ float s_decode[256];                                             \
+    for (uint32_t i = threadIdx.x; i < 256u; i += blockDim.x) s_decode[i] = kSrgbDecode[i]; \
+    __syncthreads();                                                            \
+    const uint32_t over_pos = channel_positions(S.channels);
+#define FORMA_PAINT_LOAD_PIXELS() load_srgb_run(S, in.framebuffer, ty * 16u + row, x0, vec_ok, s_decode, over_pos, dr, dg, db, da, bg_opaque)
+#define FORMA_PAINT_STORE_PIXELS()   \
+    upgrade_alpha(da, bg_opaque); \
+    store_srgb_run(S, in.framebuffer, ty * 16u + row, x0, dr, dg, db, da, vec_ok, rgba_order)
+__global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, 8) paint_over_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles) {
+    FORMA_PAINT_OVER_SRGB_PROLOGUE
+#define FORMA_PAINT_FRAME_TY(ty) (ty)
+#include "paint_kernel_body.cuh"
+#undef FORMA_PAINT_FRAME_TY
+}
+__global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, 8)
+    paint_views_over_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles, uint32_t view_rows) {
+    FORMA_PAINT_OVER_SRGB_PROLOGUE
+#define FORMA_PAINT_FRAME_TY(ty) ((ty) % view_rows)
+#include "paint_kernel_body.cuh"
+#undef FORMA_PAINT_FRAME_TY
+}
+#undef FORMA_PAINT_LOAD_PIXELS
+#undef FORMA_PAINT_STORE_PIXELS
+#undef FORMA_PAINT_OVER_SRGB_PROLOGUE
+
+#define FORMA_PAINT_LOAD_PIXELS() load_linear_run(S, in.framebuffer, ty * 16u + row, x0, vec_ok, bpp, over_pos, dr, dg, db, da, bg_opaque)
+#define FORMA_PAINT_STORE_PIXELS()   \
+    (void)rgba_order;                \
+    upgrade_alpha(da, bg_opaque); \
+    store_linear_run(S, in.framebuffer, ty * 16u + row, x0, dr, dg, db, da, vec_ok, bpp)
+__global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, 8)
+    paint_over_linear_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles, uint32_t bpp) {
+    const uint32_t over_pos = channel_positions(S.channels);
+#define FORMA_PAINT_FRAME_TY(ty) (ty)
+#include "paint_kernel_body.cuh"
+#undef FORMA_PAINT_FRAME_TY
+}
+__global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, 8)
+    paint_views_over_linear_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles, uint32_t view_rows, uint32_t bpp) {
+    const uint32_t over_pos = channel_positions(S.channels);
+#define FORMA_PAINT_FRAME_TY(ty) ((ty) % view_rows)
+#include "paint_kernel_body.cuh"
+#undef FORMA_PAINT_FRAME_TY
+}
+#undef FORMA_PAINT_LOAD_PIXELS
+#undef FORMA_PAINT_STORE_PIXELS
+
+// The inverse of repack_views_kernel: rows [0, height) of every frame of the caller's stack (frame b
+// at src + b * view_stride, row r at + r * stride) to the stacked frame (frame b's first row at
+// dst + b * view_rows_px * dst_stride), so that a stack painted in scratch starts from its
+// background. One thread per 4-byte word, `width` words per row.
+__global__ void __launch_bounds__(256) unpack_views_kernel(const uint8_t* __restrict__ src, uint64_t stride, uint64_t view_stride,
+                                                           uint8_t* __restrict__ dst, uint64_t dst_stride, uint32_t view_rows_px,
+                                                           uint32_t width, uint32_t height) {
+    const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t r = blockIdx.y, b = blockIdx.z;
+    if (x >= width) return;
+    const uint8_t* s = src + (uint64_t)b * view_stride + (uint64_t)r * stride + (uint64_t)x * 4u;
+    uint8_t* d = dst + ((uint64_t)b * view_rows_px + r) * dst_stride + (uint64_t)x * 4u;
+    *reinterpret_cast<uint32_t*>(d) = *reinterpret_cast<const uint32_t*>(s);
+}
+void launch_unpack_views(const uint8_t* src, uint64_t stride, uint64_t view_stride, uint8_t* dst, uint64_t dst_stride,
+                         uint32_t view_rows_px, uint32_t width, uint32_t height, uint32_t n_views, cudaStream_t st) {
+    if (!width || !height || !n_views) return;
+    unpack_views_kernel<<<dim3((width + 255u) / 256u, height, n_views), 256, 0, st>>>(src, stride, view_stride, dst, dst_stride,
+                                                                                      view_rows_px, width, height);
+}
+
 // Rows [0, height) of every view of a stacked frame (view b at src + b * view_rows_px * src_stride)
 // to dst + b * view_stride + row * stride: padding rows and the bytes between views stay untouched.
 // One thread per pixel, 4 bytes apart in every row.
@@ -622,6 +833,40 @@ void launch_paint_linear(const PaintScene& S, const uint64_t* segs, const EntryR
     const uint32_t grid = min((uint32_t)(per_sm * device_sm_count()), (n_tiles + kPaintWarpsPerBlock - 1) / kPaintWarpsPerBlock);
     if (views) paint_views_linear_kernel<<<grid, kPaintWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles, view_rows, bpp);
     else paint_linear_kernel<<<grid, kPaintWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles, bpp);
+}
+
+void launch_paint_over(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range, const uint32_t* heavy,
+                       const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st,
+                       uint32_t view_rows, uint32_t bpp) {
+    if (S.tx_hi <= S.tx_lo || S.ty_hi <= S.ty_lo) return;
+    const uint32_t n_tiles = (S.tx_hi - S.tx_lo) * (S.ty_hi - S.ty_lo);
+    cudaMemsetAsync(tile_counter, 0, sizeof(uint32_t), st);
+    PaintInputs in{segs, recs, tile_range, heavy, heavy_count, S.tiles_x * S.tiles_y, eflags, framebuffer, tile_counter};
+    // Persistent warps, as in launch_paint.
+    static int blocks_per_sm[2][2][kMaxDevices] = {{{0}}};
+    static std::mutex config_mu;
+    const int views = view_rows ? 1 : 0, linear = bpp == 4u ? 0 : 1;
+    const void* kernels[2][2] = {{(const void*)paint_over_kernel, (const void*)paint_over_linear_kernel},
+                                 {(const void*)paint_views_over_kernel, (const void*)paint_views_over_linear_kernel}};
+    int per_sm = 0;
+    {
+        std::lock_guard<std::mutex> lk(config_mu);
+        int& slot = blocks_per_sm[views][linear][current_device_index()];
+        if (!slot) {
+            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&slot, kernels[views][linear], kPaintWarpsPerBlock * 32, 0);
+            if (slot < 1) slot = 1;
+        }
+        per_sm = slot;
+    }
+    const uint32_t grid = min((uint32_t)(per_sm * device_sm_count()), (n_tiles + kPaintWarpsPerBlock - 1) / kPaintWarpsPerBlock);
+    const uint32_t block = kPaintWarpsPerBlock * 32;
+    if (views) {
+        if (linear) paint_views_over_linear_kernel<<<grid, block, 0, st>>>(S, in, n_tiles, view_rows, bpp);
+        else paint_views_over_kernel<<<grid, block, 0, st>>>(S, in, n_tiles, view_rows);
+    } else {
+        if (linear) paint_over_linear_kernel<<<grid, block, 0, st>>>(S, in, n_tiles, bpp);
+        else paint_over_kernel<<<grid, block, 0, st>>>(S, in, n_tiles);
+    }
 }
 
 }  // namespace forma

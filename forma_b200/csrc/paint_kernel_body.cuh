@@ -8,6 +8,14 @@
 // A kernel for frames whose layers are all solid `Over` fills without clips (Composition::solid_over_only)
 // defines FORMA_PAINT_SOLID_OVER: clip state, pass B, gradient prefetch and the blend paths of every
 // other style fold away, and what remains is the same code as for such layers in the general build.
+// A kernel that paints over the pixels already in the frame (forma_renderer_render_over_device)
+// defines FORMA_PAINT_LOAD_PIXELS() as well as FORMA_PAINT_STORE_PIXELS():
+//   FORMA_PAINT_LOAD_PIXELS(): the lane's eight pixels at (x0, ty * 16 + row), decoded into the
+//   planes dr / dg / db / da, and bit j of bg_opaque set where pixel j's alpha is 1.
+// The background is then each pixel's clear colour: a tile without entries is not written (its
+// pixels are what the clear colour would give them back), the solid fold runs per pixel from the
+// background unless an opaque layer is its bottom, and every tile is stored through
+// FORMA_PAINT_STORE_PIXELS(), which applies the Alpha -> One upgrade per pixel (bg_opaque).
 #ifdef FORMA_PAINT_SOLID_OVER
     constexpr bool kSolidOver = true;
 #else
@@ -91,6 +99,11 @@
         }
         if (tid == 0xFFFFFFFFu) continue;
         const uint32_t ty = tid / S.tiles_x, tx = tid - ty * S.tiles_x;
+#ifdef FORMA_PAINT_LOAD_PIXELS
+        // No entries: the background stays. This also keeps the first attempt of a sync-free frame
+        // whose tables are redone from writing: its tile ranges are all empty (build_tables).
+        if (b == e) continue;
+#endif
 
         // ---- optimizer passes (layer_workbench/passes/*.rs) ------------------
         // Pass A: per-entry facts, 32 entries at a time.
@@ -207,6 +220,59 @@
             continue;
         }
 
+#ifdef FORMA_PAINT_LOAD_PIXELS
+        (void)clear;
+        f2 dr[4], dg[4], db[4], da[4];
+        uint32_t bg_opaque = 0;
+        const uint32_t x0 = tx * 16u + hx * 8u;  // first pixel column of the lane
+        FORMA_PAINT_LOAD_PIXELS();
+        if (!incomplete) {
+            // The fold of skip_fully_covered_layers (rs:81-118) with each pixel's background as its
+            // clear colour: from an opaque bottom layer once, as the other kernels fold, or else per
+            // pixel from the background. The planes then hold the solid tile's colour.
+            const uint32_t p_first = first_paint + (have_opaque ? 1u : 0u);
+            bool solid = true;
+            for (uint32_t p = p_first; p < e; ++p) {
+                if (in.eflags[p] & kFlagMaskedOut) continue;
+                const uint32_t m = in.recs[p].meta;
+                if (meta_func(m) != 0u || meta_fill_type(m) != 0u) {
+                    solid = false;
+                    break;
+                }
+            }
+            if (solid) {
+                if (have_opaque) {
+                    const EntryRec& r0 = in.recs[first_paint];
+                    Rgba dst{r0.color[0], r0.color[1], r0.color[2], r0.color[3]};
+                    for (uint32_t p = p_first; p < e; ++p) {
+                        if (in.eflags[p] & kFlagMaskedOut) continue;
+                        const EntryRec& r = in.recs[p];
+                        dst = blend_solid(meta_blend(r.meta), dst, Rgba{r.color[0], r.color[1], r.color[2], r.color[3]});
+                    }
+#pragma unroll
+                    for (int q = 0; q < 4; ++q) {
+                        dr[q] = f2_splat(dst.r); dg[q] = f2_splat(dst.g); db[q] = f2_splat(dst.b); da[q] = f2_splat(dst.a);
+                    }
+                } else {
+                    for (uint32_t p = p_first; p < e; ++p) {
+                        if (in.eflags[p] & kFlagMaskedOut) continue;
+                        const EntryRec& r = in.recs[p];
+                        const Rgba src{r.color[0], r.color[1], r.color[2], r.color[3]};
+                        const uint32_t mode = meta_blend(r.meta);
+#pragma unroll
+                        for (int q = 0; q < 4; ++q) {
+                            const Rgba d0 = blend_solid(mode, Rgba{dr[q].x, dg[q].x, db[q].x, da[q].x}, src);
+                            const Rgba d1 = blend_solid(mode, Rgba{dr[q].y, dg[q].y, db[q].y, da[q].y}, src);
+                            dr[q] = f2{d0.r, d1.r}; dg[q] = f2{d0.g, d1.g}; db[q] = f2{d0.b, d1.b}; da[q] = f2{d0.a, d1.a};
+                        }
+                    }
+                }
+                first_paint = e;  // nothing to paint: straight to the store
+            }
+        }
+        bool clip_active = false;
+        uint32_t clip_last = 0;
+#else
         if (!incomplete) {
             // Every visible layer is full: fold with the scalar blend and emit a
             // solid tile (skip_fully_covered_layers.rs:81-118, mod.rs:686-704).
@@ -262,6 +328,7 @@
         bool clip_active = false;
         uint32_t clip_last = 0;
         const uint32_t x0 = tx * 16u + hx * 8u;            // first pixel column of the lane
+#endif
         const float fy8 = (float)(FORMA_PAINT_FRAME_TY(ty) * 16u + (row & 8u));  // y of lane 0 of the reference's f32x8 holding this row
         const int ly8 = (int)(row & 7u);                   // the row inside it
         const uint32_t grp_shift = (lane & 16u) + hx;      // ballot bits of this lane's f32x8 group: grp_shift + 2 i

@@ -492,11 +492,13 @@ int Renderer::render(const FrameRequest& q) {
     };
     FramePlan p{device_frame(q.rgba), device_frame(q.ids), stack ? (uint32_t)((q.height + 15u) / 16u) : 0u, false, false};
     // The PaintScene of the RGBA target, or of the ID target when it is alone.
+    // An over frame has no clear colour: its kernels read each pixel's, and upgrade Alpha -> One per
+    // pixel, so the scene's channels stay as given.
     static const uint32_t kIdChannels[4] = {0, 1, 2, 3};
     static const float kIdClear[4] = {0, 0, 0, 0};
     PaintScene S{};
     st = begin_frame(S, q.width, rgba ? p.rgba.stride : p.ids.stride, stack ? (uint64_t)q.n * p.rows * 16u : q.height,
-                     rgba ? q.channels : kIdChannels, rgba ? q.clear : kIdClear, q.crop);
+                     rgba ? q.channels : kIdChannels, rgba && !q.rgba.over ? q.clear : kIdClear, q.crop);
     if (st) return st;
     if (rgba && !p.rgba.direct) {
         FORMA_CUDA_TRY(framebuffer.reserve((size_t)p.rgba.stride * S.height));
@@ -556,6 +558,25 @@ int Renderer::check_request(const FrameRequest& q) {
         set_error("invalid float frame: buffer, stride %llu and %s stride %llu must be multiples of 4 bytes",
                   (unsigned long long)q.rgba.stride, what, (unsigned long long)q.rgba.frame_stride);
         return FORMA_STATUS_INVALID;
+    }
+    if (q.rgba.over) {
+        // Over frames: device memory, 4-byte aligned in every format, no ID target or layer cache, and
+        // a channel order that can be decoded: a permutation of R, G, B, A, for sRGB8 with A last (a
+        // solid tile's bytes encode by position, so only then do they decode to its colour).
+        bool seen[4] = {false, false, false, false}, perm = q.channels != nullptr;
+        for (int k = 0; perm && k < 4; ++k) {
+            const uint32_t c = q.channels[k];
+            perm = perm && c < 4u && !seen[c];
+            if (c < 4u) seen[c] = true;
+        }
+        if (!q.rgba.on_device || q.ids.ptr || q.cache || !perm || (q.rgba.bpp == 4u && q.channels[3] != FORMA_CHANNEL_ALPHA) ||
+            (((uintptr_t)q.rgba.ptr | q.rgba.stride | q.rgba.frame_stride) & 3u) != 0u) {
+            set_error("invalid over frame: a device buffer without IDs or layer cache, channels a permutation of R, G, B, A%s, "
+                      "and buffer, stride %llu and %s stride %llu multiples of 4 bytes",
+                      q.rgba.bpp == 4u ? " with A last" : "", (unsigned long long)q.rgba.stride, what,
+                      (unsigned long long)q.rgba.frame_stride);
+            return FORMA_STATUS_INVALID;
+        }
     }
     if (q.ids.ptr) {
         const FrameTarget& t = q.ids;
@@ -712,8 +733,16 @@ int Renderer::paint_step(const FrameRequest& q, const PaintScene& S, const Frame
             for (const Composition* c : batch_distinct) solid_over = solid_over && c->solid_over_only;
         else
             solid_over = solid_over && q.comp->solid_over_only;
-        const int st =
-            paint(S, p.rgba.ptr, q.rgba.ptr, q.rgba.stride, p.in_bands, heavy_lists, paint_launches, p.rows, q.rgba.bpp, solid_over);
+        if (q.rgba.over && p.rows && !p.rgba.direct) {
+            // A stack painted in scratch starts from its background (the redo of a sync-free frame
+            // copies it again: the first attempt wrote nothing, and its repack gave the buffer back as it was).
+            launch_unpack_views(q.rgba.ptr, q.rgba.stride, q.rgba.frame_stride, p.rgba.ptr, p.rgba.stride, p.rows * 16u,
+                                S.width * (q.rgba.bpp / 4u), (uint32_t)q.height, q.n, stream);
+            ++launches;
+            FORMA_CUDA_TRY(cudaGetLastError());
+        }
+        const int st = paint(S, p.rgba.ptr, q.rgba.ptr, q.rgba.stride, p.in_bands, heavy_lists, paint_launches, p.rows, q.rgba.bpp,
+                             solid_over, q.rgba.over);
         if (st || !q.ids.ptr) return st;
         ++*paint_launches;
     }
@@ -864,7 +893,8 @@ SortResult Renderer::sort(DeviceBuffer<uint64_t>& keys, DeviceBuffer<uint64_t>& 
 int Renderer::build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint32_t prev_cells, uint32_t prev_gaps,
                            uint32_t* heavy_lists, DevCounts& dc) {
     // Tiles without entries keep an empty range: a frame whose tables are redone paints only the
-    // clear colour in its first attempt.
+    // clear colour in its first attempt. A count above its bound leaves every range empty (the
+    // merge kernel then writes none), so that attempt of an over frame writes nothing at all.
     FORMA_CUDA_TRY(cudaMemsetAsync(tile_range.ptr, 0, (size_t)S.tiles_x * S.tiles_y * sizeof(uint2), stream));
     const SortPlan carry_plan = carry_sort_plan(S), gap_plan = gap_sort_plan(S);
     auto zero_scratch = [&](size_t from, size_t to) -> cudaError_t {
@@ -1006,10 +1036,15 @@ int Renderer::queue_row_costs(const PaintScene& S, uint32_t n) {
 // the painting of the following ones.
 // bpp: bytes per pixel of fb, 4 (sRGB8), or 8 / 16 for a linear float frame (never in bands).
 // solid_over: see launch_paint (sRGB8 frames; a float frame is painted by the general build).
+// over: paint over fb's own pixels (launch_paint_over), in any of the three formats.
 int Renderer::paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t stride, bool in_bands, const uint32_t* heavy_lists,
-                    uint32_t* paint_launches, uint32_t view_rows, uint32_t bpp, bool solid_over) {
+                    uint32_t* paint_launches, uint32_t view_rows, uint32_t bpp, bool solid_over, bool over) {
     *paint_launches = 1;
-    if (in_bands) {
+    if (over) {  // (never in bands: an over frame is on the device)
+        launch_paint_over(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), eflags.ptr, fb, totals.ptr + 3, stream,
+                          view_rows, bpp);
+        ++launches;
+    } else if (in_bands) {
         if (!band_streams_ok) {
             for (auto& e : band_ev) FORMA_CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
             band_streams_ok = true;

@@ -47,6 +47,7 @@ struct FrameTarget {
     uint64_t stride = 0, frame_stride = 0;
     float min_coverage = 0.0f;  // the ID target
     uint32_t bpp = 4;
+    bool over = false;  // the RGBA target: painted over its own pixels, each its clear colour (see forma_renderer_render_over_device)
 };
 
 // What a FrameRequest renders. single: one frame of a composition. views: n views of one
@@ -314,7 +315,7 @@ class Renderer {
                      DevCounts& dc);
     int queue_row_costs(const PaintScene& S, uint32_t n);
     int paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t stride, bool in_bands, const uint32_t* heavy_lists,
-              uint32_t* paint_launches, uint32_t view_rows = 0, uint32_t bpp = 4, bool solid_over = false);
+              uint32_t* paint_launches, uint32_t view_rows = 0, uint32_t bpp = 4, bool solid_over = false, bool over = false);
     int copy_to_host(const PaintScene& S, uint8_t* buffer, const uint8_t* fb, uint64_t stride, cudaStream_t s, uint32_t bpp = 4);
     int scatter_written_tiles(const PaintScene& S, const uint8_t* fb, uint8_t* buffer, uint64_t stride);
 };

@@ -1,6 +1,7 @@
 """Headless front end: render an SVG file to PPM / PNG on the GPU.
 
     python -m forma_b200.render in.svg out.ppm [--width W --height H --scale S --device 0] [--ids ids.npy] [--linear out.npy]
+                                               [--over image.{ppm,png}]
 
 The equivalent of the reference's `demo svg --file in.svg --scale S` + the `S` key's
 capture.ppm (demo/src/main.rs, demo/src/runner.rs:193-219: a binary P6 file with the
@@ -10,6 +11,9 @@ renderer cannot be created and the command fails. `--ids` also writes the frame'
 the order of the top-most layer drawn there, 0xFFFFFFFF for none) as an H x W uint32 .npy.
 `--linear` also writes the frame's linear colour before the sRGB encode (RGBA, float32) as an
 H x W x 4 .npy.
+`--over` draws the SVG over an image instead of a white frame: the image (binary PPM, or PNG with
+Pillow) goes to the GPU as an H x W x 4 uint8 tensor, Renderer.render_over_device draws over it, and
+its size replaces --width / --height.
 """
 from __future__ import annotations
 
@@ -28,6 +32,34 @@ def write_ppm(path: str, rgba: np.ndarray, width: int, height: int) -> None:
         f.write(rgb.tobytes())
 
 
+def read_image(path: str) -> np.ndarray:
+    """An H x W x 4 uint8 RGBA array of a binary PPM (alpha 255) or, with Pillow, a PNG."""
+    if path.lower().endswith(".png"):
+        from PIL import Image
+        return np.asarray(Image.open(path).convert("RGBA"), np.uint8).copy()
+    with open(path, "rb") as f:
+        data = f.read()
+    fields, pos = [], 0
+    while len(fields) < 4:  # magic, width, height, maxval; '#' comments between them
+        while data[pos:pos + 1].isspace():
+            pos += 1
+        if data[pos:pos + 1] == b"#":
+            pos = data.index(b"\n", pos)
+            continue
+        end = pos
+        while not data[end:end + 1].isspace():
+            end += 1
+        fields.append(data[pos:end])
+        pos = end
+    if fields[0] != b"P6" or int(fields[3]) != 255:
+        raise ValueError(f"{path}: not a binary 8-bit PPM")
+    w, h = int(fields[1]), int(fields[2])
+    rgb = np.frombuffer(data, np.uint8, 3 * w * h, pos + 1).reshape(h, w, 3)
+    out = np.full((h, w, 4), 255, np.uint8)
+    out[..., :3] = rgb
+    return out
+
+
 def main(argv=None) -> int:
     ap = argparse.ArgumentParser(prog="python -m forma_b200.render", description=__doc__.split("\n\n")[0])
     ap.add_argument("svg")
@@ -39,12 +71,18 @@ def main(argv=None) -> int:
     ap.add_argument("--frames", type=int, default=1, help="render this many times and report the last frame's timings")
     ap.add_argument("--ids", help="also write the ID frame (H x W uint32, Renderer.render_ids) to this .npy file")
     ap.add_argument("--linear", help="also write the linear float frame (H x W x 4 float32, Renderer.render_linear) to this .npy file")
+    ap.add_argument("--over", help="draw over this image (.ppm or .png, Renderer.render_over_device) instead of a white frame; its size "
+                                   "replaces --width / --height")
     args = ap.parse_args(argv)
 
     import forma_b200
     from forma_b200 import svg
     from forma_b200.binding import RGBA, Color
 
+    image = None
+    if args.over:
+        image = read_image(args.over)
+        args.height, args.width = image.shape[:2]
     t0 = time.perf_counter()
     paths = svg.parse_svg(args.svg)
     t1 = time.perf_counter()
@@ -54,8 +92,18 @@ def main(argv=None) -> int:
     svg.compose(api, comp, paths, scale=args.scale)
     buf = np.zeros(args.width * args.height * 4, np.uint8)
     t2 = time.perf_counter()
-    for _ in range(max(args.frames, 1)):
-        t = renderer.render(comp, buf, args.width, args.height, RGBA, Color(1.0, 1.0, 1.0, 1.0))  # the demo clears to white
+    if image is None:
+        for _ in range(max(args.frames, 1)):
+            t = renderer.render(comp, buf, args.width, args.height, RGBA, Color(1.0, 1.0, 1.0, 1.0))  # the demo clears to white
+    else:
+        import torch
+        frame = torch.empty((args.height, args.width, 4), dtype=torch.uint8, device=f"cuda:{args.device}")
+        src = torch.from_numpy(image).to(frame.device)
+        for _ in range(max(args.frames, 1)):
+            frame.copy_(src)
+            torch.cuda.synchronize(frame.device)
+            t = renderer.render_over_device(comp, frame.data_ptr(), args.width, args.height, RGBA)
+        buf = frame.cpu().numpy().reshape(-1)
     t3 = time.perf_counter()
     if args.out.lower().endswith(".png"):
         from PIL import Image

@@ -410,6 +410,54 @@ int forma_renderer_render_batch_linear_device(forma_renderer*, forma_composition
                                               const uint32_t channels[4], const float clear_color[4], uint32_t format,
                                               forma_timings* timings /* nullable */);
 
+/* Frames over a background: draw onto pixels a device buffer already holds (video frames, photos,
+ * a batch of training images). The calls take no clear colour: the buffer's current contents are
+ * the background. The value written at pixel p is exactly the value the twin call writes at p when
+ * its clear colour is decode(background[p]): byte for byte in FORMA_PIXEL_SRGB8, bit for bit in
+ * the float formats. That includes the optimiser's fold of full layers (per pixel from the pixel's
+ * background, unless an opaque layer is the bottom) and the Alpha -> One upgrade (per pixel, where
+ * the decoded alpha is exactly 1). The twins: forma_renderer_render_device /
+ * forma_renderer_render_linear_device, forma_renderer_render_views{,_linear}_device and
+ * forma_renderer_render_batch{,_linear}_device; each call has its twin's arguments without the clear
+ * colour and the layer cache, and with `format`.
+ * decode, per channel:
+ *   - FORMA_PIXEL_RGBA32F: the stored value; FORMA_PIXEL_RGBA16F: __half2float (exact);
+ *   - FORMA_PIXEL_SRGB8: alpha = (float)byte / 255.0f; r, g, b = D[byte], a table of 256 f32
+ *     (forma_b200/csrc/srgb_decode.h): the f32 nearest the standard sRGB EOTF of byte / 255 when
+ *     compute_srgb's encode turns it back into the byte, else the nearest f32 that it does (byte 11:
+ *     the EOTF gives 0.0033465, which encodes to 12; D[11] = 0.0033159761). Every byte round-trips,
+ *     so a pixel that nothing covers comes back unchanged.
+ * Rules:
+ *   - `channels` is a permutation of R, G, B, A (ZERO and ONE cannot be decoded); for
+ *     FORMA_PIXEL_SRGB8 with A last (RGBA, BGRA, ...): the twin writes a solid tile's bytes by
+ *     position, alpha unencoded at position 3, and only then does such a tile decode to its colour;
+ *   - the buffer and every stride are multiples of 4 bytes, strides as for the twin of the same
+ *     format (bpp = 4, 8 or 16);
+ *   - only the crop's tile rectangle (single frames) or the frames' width x height pixels (stacks)
+ *     are read or written; row padding and the bytes between frames stay as they were. A tile no
+ *     layer reaches is not written at all (its pixels are what the twin would write there);
+ *   - no layer cache is taken, and every cache is left as it was;
+ *   - every refusal returns FORMA_ERR_INVALID_ARGUMENT before anything is read or written: a null
+ *     buffer, an unknown format, bad strides or alignment, a channel order that is not one of the
+ *     above, and everything the twin refuses; the twin's order-sum, stop / texel and 2^30-segment
+ *     limits apply as well;
+ *   - counters, segments, stage times and row costs afterwards are those of the twin; a stack that is
+ *     not painted in place (frames not whole tile rows laid out as the stacked frame's rows) has one
+ *     more launch: its background is copied into the renderer's scratch before painting.
+ * With the defaults of a [H, W, 4] / [n, H, W, 4] uint8, float16 or float32 tensor: width_stride =
+ * bpp * W, view_stride / frame_stride = bpp * W * H. */
+enum { FORMA_PIXEL_SRGB8 = 0 };
+int forma_renderer_render_over_device(forma_renderer*, forma_composition*, void* device_buffer, uint64_t width,
+                                      uint64_t width_stride, uint64_t height, const uint32_t channels[4],
+                                      const forma_rect* crop /* nullable */, uint32_t format, forma_timings* timings /* nullable */);
+int forma_renderer_render_views_over_device(forma_renderer*, forma_composition*, const float* views, uint32_t n,
+                                            void* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                            uint64_t view_stride, const uint32_t channels[4], uint32_t format,
+                                            forma_timings* timings /* nullable */);
+int forma_renderer_render_batch_over_device(forma_renderer*, forma_composition* const* comps, uint32_t n, void* device_buffer,
+                                            uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride,
+                                            const uint32_t channels[4], uint32_t format, forma_timings* timings /* nullable */);
+
 /* Launch on `cuda_stream` (a cudaStream_t, e.g. torch.cuda.current_stream().cuda_stream)
  * instead of the default stream. */
 void forma_renderer_set_stream(forma_renderer*, void* cuda_stream);
