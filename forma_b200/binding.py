@@ -339,6 +339,7 @@ SIGNATURES = {
     "debug_sort_plan": (C.c_int, [C.c_int, _u64p, _u8p]),
     "renderer_sort_pairs": (C.c_int, [_vp, C.c_int, C.c_int, _u64p, _u32p, C.c_uint64, C.c_uint64]),
     "renderer_sort_bounds": (None, [_vp, _u64p]),
+    "renderer_sort_counts": (C.c_uint64, [_vp, C.c_int, _u32p, _u32p, C.c_uint64]),
     "debug_selftest": (C.c_int, [C.c_int, _u64p]),
     "renderer_multi_new": (_vp, [C.POINTER(C.c_int), C.c_int]),
     "renderer_multi_free": (None, [_vp]),
@@ -366,7 +367,7 @@ STACK_ID_SYMBOLS = ("renderer_render_views_ids", "renderer_render_views_ids_devi
 
 
 # The same for the inspection entry points of the sort (sort_plan, Renderer.sort_pairs, sort_bounds).
-SORT_DEBUG_SYMBOLS = ("debug_sort_plan", "renderer_sort_pairs", "renderer_sort_bounds")
+SORT_DEBUG_SYMBOLS = ("debug_sort_plan", "renderer_sort_pairs", "renderer_sort_bounds", "renderer_sort_counts")
 # The same for linear float frames (Renderer.render_linear, render_views_linear, render_batch_linear).
 LINEAR_SYMBOLS = ("renderer_render_linear", "renderer_render_linear_device", "renderer_render_views_linear",
                   "renderer_render_views_linear_device", "renderer_render_batch_linear", "renderer_render_batch_linear_device")
@@ -1238,6 +1239,21 @@ class Renderer:
         out = (C.c_uint64 * 4)()
         self._api.renderer_sort_bounds(self._h, out)
         return dict(zip(("layer", "tile_x", "tile_y", "total_bits"), [int(x) for x in out]))
+
+    SORT_COUNT_SOURCES = ("none", "speculative_emit", "emit", "upsweep")
+
+    def sort_counts(self, keep: int = -1) -> dict:
+        """The last frame's segment-sort tile counts (forma_renderer_sort_counts): where pass 0's
+        came from, and the kept counts as a [passes, tiles, 256] array (empty unless keep was on
+        for that frame). keep: 1 / 0 turns keeping on / off for the following frames."""
+        info = (C.c_uint32 * 3)()
+        words = int(self._api.renderer_sort_counts(self._h, keep, info, None, 0))
+        out = np.zeros(words, np.uint32)
+        if words:
+            got = int(self._api.renderer_sort_counts(self._h, -1, info, out.ctypes.data_as(_u32p), words))
+            self._api.check(0 if got == words else -1, "sort_counts")
+        return {"source": self.SORT_COUNT_SOURCES[info[0]], "passes": int(info[1]), "tiles": int(info[2]),
+                "counts": out.reshape(int(info[1]), int(info[2]), 256)}
 
     def __del__(self):
         try:

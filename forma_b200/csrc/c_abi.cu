@@ -849,6 +849,25 @@ int forma_debug_sort_plan(int layout, const uint64_t bound[3], uint8_t out[2 + 1
     std::memcpy(out + 2, plan.pass, sizeof(plan.pass));
     return FORMA_OK;
 }
+uint64_t forma_renderer_sort_counts(forma_renderer* r, int keep, uint32_t info[3], uint32_t* out, uint64_t cap) {
+    Renderer& R = r->r;
+    if (keep >= 0) R.keep_sort_counts = keep != 0;
+    info[0] = (uint32_t)R.last_count_source;
+    info[1] = R.kept_passes;
+    info[2] = R.kept_tiles;
+    const uint64_t words = (uint64_t)R.kept_passes * R.kept_tiles * 256u;
+    if (out && cap && words) {
+        cudaError_t e = cudaSetDevice(R.device);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(R.stream);
+        if (e == cudaSuccess)
+            e = cudaMemcpy(out, R.kept_counts.ptr, std::min<uint64_t>(cap, words) * sizeof(uint32_t), cudaMemcpyDeviceToHost);
+        if (e != cudaSuccess) {
+            set_error("forma_renderer_sort_counts: %s", cudaGetErrorString(e));
+            return 0;
+        }
+    }
+    return words;
+}
 void forma_renderer_sort_bounds(const forma_renderer* r, uint64_t out[4]) {
     for (int f = 0; f < 3; ++f) out[f] = r->r.segment_bound[f];
     out[3] = r->r.segment_plan.total_bits;

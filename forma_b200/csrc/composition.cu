@@ -43,7 +43,7 @@ static const OptionName kOptionNames[] = {
     {"sort_big_log2", &Options::sort_big_log2, 10, 30}, {"test_gap_cap", &Options::test_gap_cap, 0, 1 << 30},
     {"paint_lpt", &Options::paint_lpt, 0, 1},         {"band_filter", &Options::band_filter, 0, 1},
     {"paint_wide", &Options::paint_wide, 0, 1},       {"sort_scan_log2", &Options::sort_scan_log2, 10, 31},
-    {"paint_solid", &Options::paint_solid, 0, 1},
+    {"paint_solid", &Options::paint_solid, 0, 1},     {"sort_counts", &Options::sort_counts, 0, 1},
     {"sync_free", &Options::sync_free, 0, 1},         {"test_fast_shrink", &Options::test_fast_shrink, 0, 1},
     {"host_slices", &Options::host_slices, 1, 16},    {"slice_bands", &Options::slice_bands, 1, 16},
     {"slice_min_points", &Options::slice_min_points, 0, 1 << 30}, {"slice_chain", &Options::slice_chain, 0, 1},

@@ -19,6 +19,7 @@ struct Options {
     int sort_full_key = 0;   // 1: sort the layer digits even when the inserts are in layer order
     int sort_big_log2 = 19;  // key count from which the 4096-key tiles / reduce-then-scan passes are used
     int sort_scan_log2 = 22; // key-only sorts: key count from which the reduce-then-scan passes replace the single-sweep ones
+    int sort_counts = 1;     // reduce-then-scan segment sorts: per-tile digit counts from the kernels that write the keys (0: an upsweep pass per digit)
     int test_gap_cap = 0;    // test hook: cap of the speculative carry-only-entry launch (0 = none)
     int paint_lpt = 1;       // heavy tiles first (longest-processing-time order) in the paint kernel
     int paint_wide = 0;      // 1: the general paint kernel built for 6 CTAs / SM (up to 168 registers) instead of 8 (128); sRGB8 frames only (float frames always use the 8-CTA build)
@@ -62,7 +63,11 @@ uint32_t raster_num_blocks(uint32_t n_points);
 void launch_line_count(const RasterArgs& args, uint32_t* block_sums, uint32_t* total, uint32_t* max_tile,
                        cudaStream_t stream);
 // Segments at positions >= cap are dropped (speculative launches, see Renderer::rasterize).
-void launch_raster_emit(const RasterArgs& args, const uint32_t* block_offsets, uint64_t* out, uint32_t cap, cudaStream_t stream);
+// `counts` (optional): the digit of every stored segment is added to the counts of its 4096-key
+// sort tile (TileCounts); dropped segments are not counted.
+struct CountArgs;
+void launch_raster_emit(const RasterArgs& args, const uint32_t* block_offsets, uint64_t* out, uint32_t cap, cudaStream_t stream,
+                        const CountArgs* counts = nullptr);
 // Views (see forma_renderer_render_views_device): the same line setup for n_views transforms of
 // the composition, stacked top to bottom in one frame of n_views * rows tile rows. View b's line
 // of layer transform T is transformed by C = V_b ∘ T in f32, `*` rounded on its own:
@@ -80,7 +85,7 @@ struct ViewArgs {
 void launch_line_count_views(const RasterArgs& args, const ViewArgs& views, uint32_t n_views, uint32_t* block_sums, uint32_t* total,
                              uint32_t* max_tile, cudaStream_t stream);
 void launch_raster_emit_views(const RasterArgs& args, const ViewArgs& views, uint32_t n_views, const uint32_t* block_offsets,
-                              uint64_t* out, uint32_t cap, cudaStream_t stream);
+                              uint64_t* out, uint32_t cap, cudaStream_t stream, const CountArgs* counts = nullptr);
 // Batches (see forma_renderer_render_batch_device): frame c of a stack of n_frames frames is a
 // composition of its own. Each frame's line setup reads its composition's segment buffer and
 // tables (as RasterArgs, over the whole frame), and only two key fields move: row t of frame c
@@ -109,7 +114,7 @@ struct BatchArgs {
 void launch_line_count_batch(const BatchArgs& batch, uint32_t n_ctas, uint32_t* block_sums, uint32_t* total, uint32_t* max_tile,
                              cudaStream_t stream);
 void launch_raster_emit_batch(const BatchArgs& batch, uint32_t n_ctas, const uint32_t* block_offsets, uint64_t* out, uint32_t cap,
-                              cudaStream_t stream);
+                              cudaStream_t stream, const CountArgs* counts = nullptr);
 // Line records of the n = n_points - 1 point pairs (inspection only): orders, then
 // f = {x0, y0, dx, dy, a, b, c, d}, then the per-line segment counts.
 void launch_line_records(const RasterArgs& args, uint32_t n, uint32_t* orders, float* const f[8], uint32_t* lengths,
@@ -154,11 +159,54 @@ __device__ __forceinline__ uint32_t digit_of(uint64_t key, const DigitSpec& d) {
     return v;
 }
 #endif
+inline bool same_digit(const DigitSpec& a, const DigitSpec& b) {
+    for (int r = 0; r < 3; ++r)
+        if (a.shift[r] != b.shift[r] || a.width[r] != b.width[r] || a.lsh[r] != b.lsh[r]) return false;
+    return a.bits == b.bits;
+}
 struct SortResult {
     int launches;
     bool in_tmp;  // the sorted data is in keys_tmp / vals_tmp (odd number of passes)
     int timed_passes = 0;  // passes whose kernels were bracketed by pass_events
 };
+
+// Per-tile digit counts of the reduce-then-scan passes of a key-only sort, counted by the kernels
+// that write the keys instead of by an upsweep pass that reads them again (option sort_counts): the
+// emit pass counts pass 0 (Renderer::rasterize), the downsweep of pass p counts pass p + 1 by the
+// keys' destinations. Two blocks of u32, pass p using block p & 1:
+//   block = totals[kTotalsRows][256] | hist[tile_cap][256]
+// hist: per 4096-key tile, the only counts the producers add to (one atomic per warp group of equal
+// (tile, digit)). totals: per chunk of tiles_per_chunk consecutive tiles, then per super-chunk of
+// kChunksPerSuper chunks (what the tile scan reads), summed from hist by radix_chunk_totals_kernel.
+// The downsweep of pass p zeroes what it consumed (hist of pass p, its super-chunk rows): after a
+// sort both blocks are zero again, and the next frame's producers count into them without a memset.
+constexpr uint32_t kSortTileKeys = 4096;
+constexpr uint32_t kChunksPerSuper = 16;
+constexpr uint32_t kMaxSupers = 32;
+constexpr uint32_t kMaxChunks = kChunksPerSuper * kMaxSupers;  // 512
+constexpr uint32_t kTotalsRows = kMaxChunks + kMaxSupers;      // chunk rows, then super-chunk rows
+inline uint32_t sort_tiles(uint32_t n) { return (n + kSortTileKeys - 1u) / kSortTileKeys; }
+struct TileCounts {
+    uint32_t* base = nullptr;
+    uint32_t tile_cap = 0;         // tiles each block is laid out for
+    uint32_t tiles_per_chunk = 1;  // ceil(tile_cap / kMaxChunks)
+    bool pass0 = false;            // block 0 holds pass 0's counts; otherwise the sort counts them itself (upsweep)
+    size_t block_words() const { return (size_t)(kTotalsRows + tile_cap) * 256u; }
+    uint32_t* totals(uint32_t p) const { return base + (p & 1u) * block_words(); }
+    uint32_t* hist(uint32_t p) const { return totals(p) + (size_t)kTotalsRows * 256u; }
+};
+// Where a producer adds its keys' digit counts: the pass's per-tile counts and digit.
+struct CountArgs {
+    uint32_t* hist;
+    DigitSpec spec;
+};
+#ifdef __CUDACC__
+__device__ __forceinline__ void add_tile_count(const CountArgs& C, uint32_t tile, uint32_t digit, uint32_t count) {
+    atomicAdd(&C.hist[(size_t)tile * 256u + digit], count);
+}
+#endif
+// Whether a key-only sort of n keys runs the reduce-then-scan passes (the only ones that take TileCounts).
+bool radix_sort_scans(uint32_t n);
 size_t radix_scratch_bytes(uint32_t n);
 // Scratch of a sort whose digit histogram comes from the kernel that wrote its keys (see
 // launch_radix_sort's `hist`): tile counters and look-back tables of the single-sweep passes.
@@ -174,7 +222,14 @@ SortResult launch_radix_sort(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals,
                              const uint32_t* hist = nullptr /* [kMaxSortPasses][256] digit counts of every planned pass,
                                                                counted by the keys' producer: the sort then launches its
                                                                passes only, and `scratch` holds sort_lookback_bytes(n, plan)
-                                                               bytes zeroed by the caller */);
+                                                               bytes zeroed by the caller */,
+                             const TileCounts* counts = nullptr /* reduce-then-scan passes: the tile counts, both blocks zero
+                                                                   except for what the emit counted into block 0 (counts->pass0;
+                                                                   without it, block 0 must be zero: pass 0 is counted by an
+                                                                   upsweep); no upsweep from pass 1 on, and both blocks are zero
+                                                                   again when the sort is done */,
+                             uint32_t* keep_counts = nullptr /* with `counts`: pass p's tile counts are copied to
+                                                                keep_counts + p * tiles * 256 before its tile scan */);
 
 // ---- kernels_paint.cu -------------------------------------------------------
 struct PaintScene {

@@ -281,6 +281,7 @@ __device__ __forceinline__ LineParams line_setup(const RasterArgs& A, uint32_t i
 }
 
 constexpr int kRasterThreads = 256;
+constexpr uint32_t kRadixDigits = 256;  // digits of a sort pass (counted by the emit pass)
 
 // Where a CTA of a batch works: its frame, its CTA within the frame's points, the frame's order base.
 struct BatchPos {
@@ -474,13 +475,23 @@ struct SharedLines {
 // not shrink when seven eighths of the lines were culled).
 // kViews: CTA (x, y) emits view y's segments of the CTA x lines (see line_count_body).
 // kBatch: CTA x emits frame P.frame's segments, its layers moved up by the frame's order base.
-template <bool kViews, bool kBatch = false>
+// kCount: the digit C.spec of every stored segment is counted for its 4096-key sort tile (TileCounts).
+// A CTA's segments are consecutive, most often within two sort tiles: their counts gather in
+// shared memory, warp-aggregated, and go out once per CTA; the tiles after those two (a CTA of long
+// lines) take warp-aggregated global atomics.
+template <bool kViews, bool kBatch = false, bool kCount = false>
 __device__ __forceinline__ void raster_emit_body(const RasterArgs& A, const ViewArgs& V, const uint32_t* __restrict__ block_offsets,
-                                                 uint64_t* __restrict__ out, uint32_t cap, const BatchPos& P = BatchPos{}) {
+                                                 uint64_t* __restrict__ out, uint32_t cap, const BatchPos& P = BatchPos{},
+                                                 const CountArgs& C = CountArgs{}) {
     __shared__ SharedLines S;
     __shared__ uint32_t warp_sums[kRasterThreads / 32];
+    __shared__ uint32_t s_count[kCount ? 2 * kRadixDigits : 1];  // [2 tiles][digit]
     const uint32_t t = threadIdx.x;
     const uint32_t warp = t >> 5, lane = t & 31u;
+    if constexpr (kCount) {
+        s_count[t] = 0;
+        s_count[t + kRasterThreads] = 0;
+    }
     uint32_t i = (kBatch ? P.block : blockIdx.x) * kRasterThreads + t;
     LineParams L = line_setup<kViews>(A, i, kViews ? V.xf + 6u * blockIdx.y : nullptr);
     if constexpr (kBatch) L.order += P.order_base;
@@ -555,21 +566,41 @@ __device__ __forceinline__ void raster_emit_body(const RasterArgs& A, const View
         uint64_t v = (ty << 53) | (tx << 41) | ((uint64_t)(S.order[li] & 0x1FFFFFu) << 20) | ((uint64_t)local_x << 16) |
                      ((uint64_t)local_y << 12) | ((uint64_t)(dam & 0x3Fu) << 6) | ((uint64_t)((uint32_t)cover & 0x3Fu));
         out[(uint64_t)block_base + s] = v;
+        if constexpr (kCount) {
+            // block_base + s < cap < 2^32. The lanes of one (tile, digit) add their count at once.
+            const uint32_t rel = ((block_base + s) / kSortTileKeys) - block_base / kSortTileKeys, d = digit_of(v, C.spec);
+            const uint32_t peers = __match_any_sync(__activemask(), (rel << 8) | d);
+            if (lane == __ffs(peers) - 1u) {
+                if (rel < 2u) atomicAdd(&s_count[rel * kRadixDigits + d], (uint32_t)__popc(peers));
+                else add_tile_count(C, block_base / kSortTileKeys + rel, d, (uint32_t)__popc(peers));
+            }
+        }
+    }
+    if constexpr (kCount) {
+        __syncthreads();
+        for (uint32_t i = t; i < 2u * kRadixDigits; i += kRasterThreads) {
+            const uint32_t c = s_count[i];
+            if (c) add_tile_count(C, block_base / kSortTileKeys + i / kRadixDigits, i % kRadixDigits, c);
+        }
     }
 }
-__global__ void __launch_bounds__(kRasterThreads)
-    raster_emit_kernel(RasterArgs A, const uint32_t* __restrict__ block_offsets, uint64_t* __restrict__ out, uint32_t cap) {
-    raster_emit_body<false>(A, ViewArgs{}, block_offsets, out, cap);
+// The counting builds keep the plain builds' 32 registers: 8 CTAs per SM.
+template <bool kCount>
+__global__ void __launch_bounds__(kRasterThreads, kCount ? 8 : 0)
+    raster_emit_kernel(RasterArgs A, const uint32_t* __restrict__ block_offsets, uint64_t* __restrict__ out, uint32_t cap, CountArgs C) {
+    raster_emit_body<false, false, kCount>(A, ViewArgs{}, block_offsets, out, cap, BatchPos{}, C);
 }
-__global__ void __launch_bounds__(kRasterThreads) raster_emit_views_kernel(RasterArgs A, ViewArgs V, const uint32_t* __restrict__ block_offsets,
-                                                                         uint64_t* __restrict__ out, uint32_t cap) {
-    raster_emit_body<true>(A, V, block_offsets, out, cap);
+template <bool kCount>
+__global__ void __launch_bounds__(kRasterThreads, kCount ? 8 : 0) raster_emit_views_kernel(RasterArgs A, ViewArgs V, const uint32_t* __restrict__ block_offsets,
+                                                                         uint64_t* __restrict__ out, uint32_t cap, CountArgs C) {
+    raster_emit_body<true, false, kCount>(A, V, block_offsets, out, cap, BatchPos{}, C);
 }
-__global__ void __launch_bounds__(kRasterThreads) raster_emit_batch_kernel(BatchArgs B, const uint32_t* __restrict__ block_offsets,
-                                                                         uint64_t* __restrict__ out, uint32_t cap) {
+template <bool kCount>
+__global__ void __launch_bounds__(kRasterThreads, kCount ? 8 : 0) raster_emit_batch_kernel(BatchArgs B, const uint32_t* __restrict__ block_offsets,
+                                                                         uint64_t* __restrict__ out, uint32_t cap, CountArgs C) {
     RasterArgs A;
     const BatchPos P = batch_pos(B, A);
-    raster_emit_body<false, true>(A, ViewArgs{nullptr, B.rows}, block_offsets, out, cap, P);
+    raster_emit_body<false, true, kCount>(A, ViewArgs{nullptr, B.rows}, block_offsets, out, cap, P, C);
 }
 
 // Inspection only (forma_renderer_lines): the line records of segment.rs:298-383 as the
@@ -619,10 +650,12 @@ void launch_line_count(const RasterArgs& args, uint32_t* block_sums, uint32_t* t
     scan_block_sums_kernel<<<1, 1024, 0, stream>>>(block_sums, nb, total);
 }
 
-void launch_raster_emit(const RasterArgs& args, const uint32_t* block_offsets, uint64_t* out, uint32_t cap, cudaStream_t stream) {
+void launch_raster_emit(const RasterArgs& args, const uint32_t* block_offsets, uint64_t* out, uint32_t cap, cudaStream_t stream,
+                        const CountArgs* counts) {
     uint32_t nb = raster_num_blocks(args.n_points);
     if (!nb) return;
-    raster_emit_kernel<<<nb, kRasterThreads, 0, stream>>>(args, block_offsets, out, cap);
+    if (counts) raster_emit_kernel<true><<<nb, kRasterThreads, 0, stream>>>(args, block_offsets, out, cap, *counts);
+    else raster_emit_kernel<false><<<nb, kRasterThreads, 0, stream>>>(args, block_offsets, out, cap, CountArgs{});
 }
 
 void launch_line_count_views(const RasterArgs& args, const ViewArgs& views, uint32_t n_views, uint32_t* block_sums, uint32_t* total,
@@ -638,10 +671,13 @@ void launch_line_count_views(const RasterArgs& args, const ViewArgs& views, uint
 }
 
 void launch_raster_emit_views(const RasterArgs& args, const ViewArgs& views, uint32_t n_views, const uint32_t* block_offsets,
-                              uint64_t* out, uint32_t cap, cudaStream_t stream) {
+                              uint64_t* out, uint32_t cap, cudaStream_t stream, const CountArgs* counts) {
     uint32_t nb = raster_num_blocks(args.n_points);
     if (!nb || !n_views) return;
-    raster_emit_views_kernel<<<dim3(nb, n_views), kRasterThreads, 0, stream>>>(args, views, block_offsets, out, cap);
+    if (counts)
+        raster_emit_views_kernel<true><<<dim3(nb, n_views), kRasterThreads, 0, stream>>>(args, views, block_offsets, out, cap, *counts);
+    else
+        raster_emit_views_kernel<false><<<dim3(nb, n_views), kRasterThreads, 0, stream>>>(args, views, block_offsets, out, cap, CountArgs{});
 }
 
 void launch_line_count_batch(const BatchArgs& batch, uint32_t n_ctas, uint32_t* block_sums, uint32_t* total, uint32_t* max_tile,
@@ -656,9 +692,10 @@ void launch_line_count_batch(const BatchArgs& batch, uint32_t n_ctas, uint32_t* 
 }
 
 void launch_raster_emit_batch(const BatchArgs& batch, uint32_t n_ctas, const uint32_t* block_offsets, uint64_t* out, uint32_t cap,
-                              cudaStream_t stream) {
+                              cudaStream_t stream, const CountArgs* counts) {
     if (!n_ctas) return;
-    raster_emit_batch_kernel<<<n_ctas, kRasterThreads, 0, stream>>>(batch, block_offsets, out, cap);
+    if (counts) raster_emit_batch_kernel<true><<<n_ctas, kRasterThreads, 0, stream>>>(batch, block_offsets, out, cap, *counts);
+    else raster_emit_batch_kernel<false><<<n_ctas, kRasterThreads, 0, stream>>>(batch, block_offsets, out, cap, CountArgs{});
 }
 
 }  // namespace forma

@@ -14,7 +14,9 @@
 //   (global offset of every (tile, digit) run) and the persistent, TMA-staged
 //   `radix_downsweep_wide_kernel` (stable warp match/popc ranking, digit-order
 //   staging in shared memory, coalesced scatter): 24 B/key per pass, and no CTA
-//   ever waits for another one (see the comment above those kernels).
+//   ever waits for another one (see the comment above those kernels). For the segment sort the
+//   kernels that write the keys count the tiles' digits instead (TileCounts, option sort_counts):
+//   `radix_chunk_totals_kernel` replaces the upsweep, 16 B/key per pass.
 // * Small sorts and (key, u32 payload) pairs (the painter's cell / gap tables):
 //   one upfront histogram kernel for all passes, or none when the kernel that wrote the keys
 //   counted their digits (every pass CTA scans its 256 counts itself), then one single-sweep
@@ -318,12 +320,10 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 // ---------------------------------------------------------------------------
 constexpr int kDsItems = 16;
 constexpr int kDsTile = kSortThreads * kDsItems;  // 4096 keys = 32 KB
-// The tile scan works on chunks of consecutive tiles (one CTA each) grouped into
-// super-chunks: a CTA needs 32 + 16 loads per digit to know what precedes it.
-constexpr uint32_t kChunksPerSuper = 16;
-constexpr uint32_t kMaxSupers = 32;
-constexpr uint32_t kMaxChunks = kChunksPerSuper * kMaxSupers;  // 512
-constexpr uint32_t kTotalsRows = kMaxChunks + kMaxSupers;      // per pass: chunk rows, then super-chunk rows
+static_assert(kDsTile == (int)kSortTileKeys, "the tiles of TileCounts");
+// The tile scan works on chunks of consecutive tiles (one CTA each) grouped into super-chunks
+// (kChunksPerSuper, kMaxSupers, kTotalsRows: kernels.h): a CTA needs 32 + 16 loads per digit to
+// know what precedes it.
 
 __global__ void __launch_bounds__(kSortThreads) radix_upsweep_kernel(const uint64_t* __restrict__ keys, uint32_t n, DigitSpec spec,
                                                                    uint32_t* __restrict__ tile_hist /*[tiles][256]*/,
@@ -353,6 +353,26 @@ __global__ void __launch_bounds__(kSortThreads) radix_upsweep_kernel(const uint6
         atomicAdd(&totals[(size_t)chunk * kRadix + t], c);
         atomicAdd(&totals[(size_t)(kMaxChunks + chunk / kChunksPerSuper) * kRadix + t], c);
     }
+}
+
+// Tile counts from the keys' producers (TileCounts): CTA c sums the counts of tiles
+// [c * tiles_per_chunk, ...) into chunk row c (stores) and its super-chunk row (atomics, on rows the
+// previous downsweep over this block left zero). Thread d owns digit d.
+__global__ void __launch_bounds__(kRadix) radix_chunk_totals_kernel(const uint32_t* __restrict__ tile_hist,
+                                                                  uint32_t* __restrict__ totals, uint32_t tiles,
+                                                                  uint32_t tiles_per_chunk) {
+    const uint32_t d = threadIdx.x, c = blockIdx.x;
+    const uint32_t t0 = c * tiles_per_chunk, t1 = min(tiles, t0 + tiles_per_chunk);
+    uint32_t sum = 0;
+    for (uint32_t tb = t0; tb < t1; tb += 8u) {
+        uint32_t v[8];
+#pragma unroll
+        for (uint32_t k = 0; k < 8u; ++k) v[k] = (tb + k < t1) ? tile_hist[(size_t)(tb + k) * kRadix + d] : 0u;
+#pragma unroll
+        for (uint32_t k = 0; k < 8u; ++k) sum += v[k];
+    }
+    totals[(size_t)c * kRadix + d] = sum;
+    if (sum) atomicAdd(&totals[(size_t)(kMaxChunks + c / kChunksPerSuper) * kRadix + d], sum);
 }
 
 // CTA c turns the digit counts of tiles [c * tiles_per_chunk, ...) into the
@@ -420,9 +440,14 @@ struct DownsweepWideSmem {
     uint64_t bar[kDsStages];
 };
 
+// kCount: every key written also counts for the next pass: digit next.spec, at the tile of its
+// destination (TileCounts), one atomic per group of lanes with the same (tile, digit).
+// kZero: what the pass consumed is left zero for the next producer (TileCounts): every tile's
+// offsets once read, and the pass's super-chunk rows `supers` (CTA 0; the tile scan read them).
+template <bool kCount, bool kZero>
 __global__ void __launch_bounds__(kWideThreads, 2)
     radix_downsweep_wide_kernel(const uint64_t* __restrict__ keys_in, uint64_t* __restrict__ keys_out, uint32_t n, DigitSpec spec,
-                                const uint32_t* __restrict__ tile_base, uint32_t tiles) {
+                                uint32_t* __restrict__ tile_base, uint32_t tiles, CountArgs next, uint32_t* __restrict__ supers) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     DownsweepWideSmem& S = *reinterpret_cast<DownsweepWideSmem*>(smem_raw);
     const uint32_t t = threadIdx.x, warp = t >> 5, lane = t & 31u;
@@ -444,6 +469,10 @@ __global__ void __launch_bounds__(kWideThreads, 2)
     };
 
     uint32_t tile = blockIdx.x;
+    if constexpr (kZero) {
+        if (tile == 0)
+            for (uint32_t i = t; i < kMaxSupers * (uint32_t)kRadix; i += kWideThreads) supers[i] = 0;
+    }
     if (tile >= tiles) return;
     if (t == 0) {
 #pragma unroll
@@ -527,9 +556,17 @@ __global__ void __launch_bounds__(kWideThreads, 2)
             uint32_t p = t + k * kWideThreads;
             if (p < valid) {
                 uint64_t kk = stage[p];
-                keys_out[S.global_base[digit_of(kk, spec)] + p] = kk;
+                const uint32_t dst = S.global_base[digit_of(kk, spec)] + p;
+                keys_out[dst] = kk;
+                if constexpr (kCount) {
+                    const uint32_t dt = dst / kSortTileKeys, d = digit_of(kk, next.spec);
+                    const uint32_t peers = __match_any_sync(__activemask(), (dt << 8) | d);
+                    if (lane == __ffs(peers) - 1u) add_tile_count(next, dt, d, (uint32_t)__popc(peers));
+                }
             }
         }
+        // (Zeroed here, long after the load: a store right behind it would wait for the load.)
+        if (kZero && t < (uint32_t)kRadix) tile_base[(size_t)tile * kRadix + t] = 0;
         __syncthreads();  // the stage is free again: the next iteration refills it by TMA
         st = (st + 1u) % kDsStages;
     }
@@ -582,35 +619,82 @@ static void launch_passes(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals, ui
     }
 }
 
+// The persistent downsweep's grid on the current device: 2 CTAs per SM (0: the occupancy query
+// failed, and the reduce-then-scan passes are not used). The attribute is set at first use.
+static int downsweep_grid() {
+    static int wide_grids[kMaxDevices];
+    static bool ds_configured[kMaxDevices] = {false};
+    const int cur_dev = current_device_index();
+    // Under a lock: a second host thread rendering on the same device (a slice of a host-frame
+    // pipeline) must not see the flag before the attributes are set and the grid is known.
+    std::lock_guard<std::mutex> lk(g_sort_config_mu);
+    if (!ds_configured[cur_dev]) {
+        // The plain build, and the builds that leave the tile counts zero (+ count the next pass).
+        int per_sm_all = 1 << 30;
+        for (auto* k : {radix_downsweep_wide_kernel<false, false>, radix_downsweep_wide_kernel<false, true>,
+                        radix_downsweep_wide_kernel<true, true>}) {
+            cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DownsweepWideSmem));
+            int per_sm = 0;
+            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, kWideThreads, sizeof(DownsweepWideSmem));
+            per_sm_all = min(per_sm_all, per_sm);  // one grid for all: a persistent CTA must never wait for a slot
+        }
+        wide_grids[cur_dev] = per_sm_all > 0 ? per_sm_all * device_sm_count() : 0;
+        ds_configured[cur_dev] = true;
+    }
+    return wide_grids[cur_dev];
+}
+
+bool radix_sort_scans(uint32_t n) {
+    return n >= 2 && items_for(n) == 16 && n >= (1u << options().sort_scan_log2) && downsweep_grid() > 0;
+}
+
 SortResult launch_radix_sort(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals, uint32_t* vals_tmp, uint32_t n,
                              const SortPlan& plan, void* scratch, cudaStream_t stream, cudaEvent_t* pass_events,
-                             const uint32_t* n_dev, const uint32_t* hist_ready) {
+                             const uint32_t* n_dev, const uint32_t* hist_ready, const TileCounts* counts, uint32_t* keep_counts) {
     SortResult res{0, false};
     if (n < 2 || plan.n_passes == 0) return res;
     const int items = items_for(n);
     const uint32_t tiles = tiles_for(n, items);
     if (!vals && items == 16 && n >= (1u << options().sort_scan_log2) && !n_dev && !hist_ready) {
-        // Persistent TMA-staged downsweep: 2 CTAs per SM (per-device attribute + grid).
-        static int wide_grids[kMaxDevices];
-        static bool ds_configured[kMaxDevices] = {false};
-        const int cur_dev = current_device_index();
-        int wide_grid = 0;
-        {
-            // Under a lock: a second host thread rendering on the same device (a slice of a host-frame
-            // pipeline) must not see the flag before the attribute is set and the grid is known.
-            std::lock_guard<std::mutex> lk(g_sort_config_mu);
-            if (!ds_configured[cur_dev]) {
-                cudaFuncSetAttribute(radix_downsweep_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)sizeof(DownsweepWideSmem));
-                int per_sm = 0;
-                cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, radix_downsweep_wide_kernel, kWideThreads,
-                                                              sizeof(DownsweepWideSmem));
-                wide_grids[cur_dev] = per_sm > 0 ? per_sm * device_sm_count() : 0;
-                ds_configured[cur_dev] = true;
-            }
-            wide_grid = wide_grids[cur_dev];
-        }
+        const int wide_grid = downsweep_grid();
         if (wide_grid > 0) {
+            const uint32_t grid = min(tiles, (uint32_t)wide_grid);
+            if (counts && tiles <= counts->tile_cap) {
+                // Pass p's tile counts are in block p & 1: counted by the emit pass (pass 0, when
+                // counts->pass0) or the upsweep (pass 0 otherwise), then by the downsweep of pass p - 1.
+                const uint32_t tpc = counts->tiles_per_chunk;
+                const uint32_t chunks = (tiles + tpc - 1) / tpc;
+                for (uint32_t p = 0; p < plan.n_passes; ++p) {
+                    const uint64_t* kin = (p & 1u) ? keys_tmp : keys;
+                    uint64_t* kout = (p & 1u) ? keys : keys_tmp;
+                    if (pass_events) cudaEventRecord(pass_events[3 * p], stream);
+                    if (p == 0 && !counts->pass0) {  // the upsweep stores the tile counts and adds to zeroed totals
+                        cudaMemsetAsync(counts->totals(0), 0, (size_t)kTotalsRows * kRadix * sizeof(uint32_t), stream);
+                        radix_upsweep_kernel<<<tiles, kSortThreads, 0, stream>>>(kin, n, plan.pass[0], counts->hist(0), counts->totals(0), tpc);
+                    } else {
+                        radix_chunk_totals_kernel<<<chunks, kRadix, 0, stream>>>(counts->hist(p), counts->totals(p), tiles, tpc);
+                    }
+                    if (keep_counts)
+                        cudaMemcpyAsync(keep_counts + (size_t)p * tiles * kRadix, counts->hist(p), (size_t)tiles * kRadix * sizeof(uint32_t),
+                                        cudaMemcpyDeviceToDevice, stream);
+                    radix_tile_scan_kernel<<<chunks, kRadix, 0, stream>>>(counts->hist(p), counts->totals(p), tiles, tpc);
+                    if (pass_events) cudaEventRecord(pass_events[3 * p + 1], stream);
+                    uint32_t* supers = counts->totals(p) + (size_t)kMaxChunks * kRadix;
+                    if (p + 1 < plan.n_passes) {
+                        const CountArgs next{counts->hist(p + 1), plan.pass[p + 1]};
+                        radix_downsweep_wide_kernel<true, true><<<grid, kWideThreads, sizeof(DownsweepWideSmem), stream>>>(
+                            kin, kout, n, plan.pass[p], counts->hist(p), tiles, next, supers);
+                    } else {
+                        radix_downsweep_wide_kernel<false, true><<<grid, kWideThreads, sizeof(DownsweepWideSmem), stream>>>(
+                            kin, kout, n, plan.pass[p], counts->hist(p), tiles, CountArgs{}, supers);
+                    }
+                    if (pass_events) cudaEventRecord(pass_events[3 * p + 2], stream);
+                }
+                res.timed_passes = pass_events ? (int)plan.n_passes : 0;
+                res.launches = 3 * (int)plan.n_passes;
+                res.in_tmp = (plan.n_passes & 1u) != 0u;
+                return res;
+            }
             const uint32_t tiles_per_chunk = (tiles + kMaxChunks - 1) / kMaxChunks;
             const uint32_t chunks = (tiles + tiles_per_chunk - 1) / tiles_per_chunk;
             uint32_t* chunk_totals = static_cast<uint32_t*>(scratch);
@@ -624,8 +708,8 @@ SortResult launch_radix_sort(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals,
                 radix_upsweep_kernel<<<tiles, kSortThreads, 0, stream>>>(kin, n, plan.pass[p], tile_hist, totals, tiles_per_chunk);
                 radix_tile_scan_kernel<<<chunks, kRadix, 0, stream>>>(tile_hist, totals, tiles, tiles_per_chunk);
                 if (pass_events) cudaEventRecord(pass_events[3 * p + 1], stream);
-                radix_downsweep_wide_kernel<<<min(tiles, (uint32_t)wide_grid), kWideThreads, sizeof(DownsweepWideSmem), stream>>>(
-                    kin, kout, n, plan.pass[p], tile_hist, tiles);
+                radix_downsweep_wide_kernel<false, false><<<grid, kWideThreads, sizeof(DownsweepWideSmem), stream>>>(
+                    kin, kout, n, plan.pass[p], tile_hist, tiles, CountArgs{}, nullptr);
                 if (pass_events) cudaEventRecord(pass_events[3 * p + 2], stream);
             }
             res.timed_passes = pass_events ? (int)plan.n_passes : 0;

@@ -276,11 +276,21 @@ int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, floa
     else if (views) launch_line_count_views(ra, *views, n_views, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
     else launch_line_count(ra, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
     launches += nb ? 2 : 0;
-    auto emit = [&](uint32_t cap) {
-        if (batch) launch_raster_emit_batch(batch->args, nb, block_sums.ptr, segs.ptr, cap, stream);
-        else if (views) launch_raster_emit_views(ra, *views, n_views, block_sums.ptr, segs.ptr, cap, stream);
-        else launch_raster_emit(ra, block_sums.ptr, segs.ptr, cap, stream);
+    auto emit = [&](uint32_t cap, const CountArgs* counts) {
+        if (batch) launch_raster_emit_batch(batch->args, nb, block_sums.ptr, segs.ptr, cap, stream, counts);
+        else if (views) launch_raster_emit_views(ra, *views, n_views, block_sums.ptr, segs.ptr, cap, stream, counts);
+        else launch_raster_emit(ra, block_sums.ptr, segs.ptr, cap, stream, counts);
     };
+    // The emit pass counts the sort's pass-0 digits (TileCounts) when the sort will take them: with
+    // the digit of the previous frame when it runs ahead of the read-back (used when this frame's
+    // plan has the same pass 0), with the plan's own when it runs after it.
+    const bool counting = options().sort_counts != 0;
+    auto pass0_counts = [&](const DigitSpec& spec) {
+        counts_clean = false;  // what the emit counts is zero again only once a sort has consumed it
+        return CountArgs{tile_counts.hist(0), spec};
+    };
+    last_count_source = 0;
+    tile_counts.pass0 = false;
     uint32_t n = 0;
     // One read-back: segment count + the largest tile coordinates (totals[4..5]).
     FORMA_CUDA_TRY(cudaMemcpyAsync(pinned_totals, totals.ptr, 6 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
@@ -292,9 +302,14 @@ int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, floa
     const bool speculated = spec_cap > 1 && nb;
     FORMA_CUDA_TRY(ensure_count_event());
     FORMA_CUDA_TRY(cudaEventRecord(count_ev, stream));
+    const bool spec_counted = speculated && counting && count_spec_valid;
+    if (spec_counted) {
+        FORMA_CUDA_TRY(prepare_tile_counts((uint32_t)(spec_cap - 1)));
+    }
     if (speculated) {
         if (timer.ok) FORMA_CUDA_TRY(cudaEventRecord(timer.ev[1], stream));  // end of line setup (count pass)
-        emit((uint32_t)(spec_cap - 1));
+        const CountArgs c = spec_counted ? pass0_counts(count_spec) : CountArgs{};
+        emit((uint32_t)(spec_cap - 1), spec_counted ? &c : nullptr);
         ++launches;
     }
     FORMA_CUDA_TRY(cudaEventSynchronize(count_ev));  // the read-back only, not the speculative launch
@@ -317,6 +332,7 @@ int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, floa
     // sync-free bounds (last_cells / last_gaps) are updated only by a frame that gets past here,
     // and the segment count and tile rows of the last frame read 0.
     if (n >= (1u << 30)) {
+        count_spec_valid = false;
         if (n == 0xFFFFFFFFu)
             set_error("at least 2^32 - 1 pixel segments exceed the 2^30 limit of the sort's look-back counters");
         else
@@ -327,13 +343,52 @@ int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, floa
     *n_out = n;
     last_segments = n;
     FORMA_CUDA_TRY(reserve_all(n + 1, segs, segs_tmp));
+    const bool sort_counted = counting && radix_sort_scans(n);
+    int source = 0;
     if (!speculated || (size_t)n + 1 > spec_cap) {
         if (!speculated && timer.ok) FORMA_CUDA_TRY(cudaEventRecord(timer.ev[1], stream));  // end of line setup (count pass)
-        emit(n);
+        if (sort_counted) {  // (re)counted from zero with the plan's own digit
+            FORMA_CUDA_TRY(prepare_tile_counts(n));
+            source = 2;
+        }
+        const CountArgs c = sort_counted ? pass0_counts(segment_plan.pass[0]) : CountArgs{};
+        emit(n, sort_counted ? &c : nullptr);
         launches += nb ? 1 : 0;
+    } else if (sort_counted) {
+        if (spec_counted && same_digit(segment_plan.pass[0], count_spec)) {
+            source = 1;
+        } else {  // the sort counts pass 0 itself (upsweep)
+            FORMA_CUDA_TRY(prepare_tile_counts(n));
+            source = 3;
+        }
     }
+    last_count_source = source;
+    tile_counts.pass0 = source == 1 || source == 2;
+    count_spec_valid = sort_counted;
+    count_spec = segment_plan.pass[0];
     FORMA_CUDA_TRY(cudaGetLastError());
     return FORMA_STATUS_OK;
+}
+
+cudaError_t Renderer::prepare_tile_counts(uint32_t max_keys) {
+    const uint32_t tiles = std::max(sort_tiles(max_keys), 1u);
+    if (tiles > tile_counts.tile_cap) {
+        TileCounts t;
+        counts_clean = false;
+        t.tile_cap = tiles;
+        cudaError_t e = sort_counts.reserve(2 * t.block_words());
+        if (e != cudaSuccess) return e;
+        t.tile_cap = (uint32_t)(sort_counts.capacity / 2u / 256u) - kTotalsRows;  // all that was reserved
+        t.base = sort_counts.ptr;
+        t.tiles_per_chunk = (t.tile_cap + kMaxChunks - 1u) / kMaxChunks;
+        tile_counts = t;
+    }
+    tile_counts.pass0 = false;
+    // A sort that took the counts leaves both blocks zero (its downsweeps clear what they read): only
+    // a new buffer, or counts that no sort consumed (a fallback, rasterize_only), need the memset.
+    if (counts_clean) return cudaSuccess;
+    counts_clean = true;
+    return cudaMemsetAsync(tile_counts.base, 0, 2 * tile_counts.block_words() * sizeof(uint32_t), stream);
 }
 
 // The pixel rows [lo, hi) a frame paints; partial: not all of its rows (flush_geometry's band filter).
@@ -409,7 +464,18 @@ int Renderer::run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p
     int timed_sort_passes = 0;
     if (n > 1) {
         FORMA_CUDA_TRY(sort_scratch.reserve(radix_scratch_bytes(n)));
-        timed_sort_passes = sort(segs, segs_tmp, nullptr, nullptr, n, segment_plan, timer.sort_ev).timed_passes;
+        uint32_t* keep = nullptr;
+        kept_passes = kept_tiles = 0;
+        if (keep_sort_counts && last_count_source) {
+            FORMA_CUDA_TRY(kept_counts.reserve((size_t)segment_plan.n_passes * sort_tiles(n) * 256u));
+            keep = kept_counts.ptr;
+            kept_passes = segment_plan.n_passes;
+            kept_tiles = sort_tiles(n);
+        }
+        timed_sort_passes = sort(segs, segs_tmp, nullptr, nullptr, n, segment_plan, timer.sort_ev, nullptr, nullptr, nullptr,
+                                 last_count_source ? &tile_counts : nullptr, keep)
+                                .timed_passes;
+        if (last_count_source) counts_clean = true;  // (rasterize reserved the counts for n keys: the sort took them)
         FORMA_CUDA_TRY(cudaGetLastError());
     }
     FORMA_CUDA_TRY(cudaEventRecord(timer.ev[3], stream));
@@ -870,9 +936,10 @@ int Renderer::bind_frame(Composition& comp, PaintScene& S, LayerCache* cache, co
 
 SortResult Renderer::sort(DeviceBuffer<uint64_t>& keys, DeviceBuffer<uint64_t>& keys_tmp, DeviceBuffer<uint32_t>* vals,
                           DeviceBuffer<uint32_t>* vals_tmp, uint32_t n, const SortPlan& plan, cudaEvent_t* pass_events,
-                          const uint32_t* n_dev, const uint32_t* hist, void* scratch) {
+                          const uint32_t* n_dev, const uint32_t* hist, void* scratch, const TileCounts* counts,
+                          uint32_t* keep_counts) {
     SortResult sr = launch_radix_sort(keys.ptr, keys_tmp.ptr, vals ? vals->ptr : nullptr, vals ? vals_tmp->ptr : nullptr, n, plan,
-                                      scratch ? scratch : sort_scratch.ptr, stream, pass_events, n_dev, hist);
+                                      scratch ? scratch : sort_scratch.ptr, stream, pass_events, n_dev, hist, counts, keep_counts);
     launches += sr.launches;
     if (sr.in_tmp) {
         swap_buffers(keys, keys_tmp);

@@ -127,9 +127,28 @@ class Renderer {
     // vals: the buffers trade places with their twins when it landed there.
     SortResult sort(DeviceBuffer<uint64_t>& keys, DeviceBuffer<uint64_t>& keys_tmp, DeviceBuffer<uint32_t>* vals,
                     DeviceBuffer<uint32_t>* vals_tmp, uint32_t n, const SortPlan& plan, cudaEvent_t* pass_events = nullptr,
-                    const uint32_t* n_dev = nullptr, const uint32_t* hist = nullptr, void* scratch = nullptr);
+                    const uint32_t* n_dev = nullptr, const uint32_t* hist = nullptr, void* scratch = nullptr,
+                    const TileCounts* counts = nullptr, uint32_t* keep_counts = nullptr);
     DeviceBuffer<uint64_t> segs, segs_tmp;
     DeviceBuffer<uint8_t> sort_scratch;
+    // The segment sort's per-tile digit counts (TileCounts, option sort_counts), counted by the emit
+    // pass and the downsweeps. Laid out for tile_counts.tile_cap tiles: reserved before the emit pass
+    // that counts into it (prepare_tile_counts), never moved between that pass and the sort.
+    DeviceBuffer<uint32_t> sort_counts;
+    TileCounts tile_counts;
+    // Pass 0 of the last frame whose sort used the tile counts: the speculative emit pass of the next
+    // frame counts that digit (the frame's own plan is only known after the count read-back).
+    DigitSpec count_spec{};
+    bool count_spec_valid = false;
+    // Where the last frame's pass-0 counts came from (see forma_renderer_sort_counts): 0 none,
+    // 1 the speculative emit, 2 the emit after the read-back, 3 an upsweep.
+    int last_count_source = 0;
+    bool keep_sort_counts = false;  // forma_renderer_sort_counts: keep every pass's counts of the next frames
+    DeviceBuffer<uint32_t> kept_counts;
+    uint32_t kept_passes = 0, kept_tiles = 0;
+    bool counts_clean = false;  // both blocks of tile_counts are zero (TileCounts)
+    // Reserves the tile counts for max_keys keys and zeroes them unless they are clean.
+    cudaError_t prepare_tile_counts(uint32_t max_keys);
     DeviceBuffer<uint8_t> table_scratch;  // see TableScratch (kernels.h); zeroed per frame by build_tables
     uint32_t* heavy_count() const { return reinterpret_cast<uint32_t*>(table_scratch.ptr); }  // TableScratch::heavy_count == 0
     DeviceBuffer<uint32_t> cell_start, perm, perm_tmp, eid, eid_tmp, gid_tmp, heavy_tiles;

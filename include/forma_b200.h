@@ -543,7 +543,7 @@ int forma_renderer_host_slices(const forma_renderer*, double* out_ms, double* ou
 uint64_t forma_renderer_row_costs(forma_renderer*, uint64_t cap, uint64_t* out);
 
 /* Schedule switches of the library (process-wide; none changes results): "speculate",
- * "band_copy", "copy_bands", "sort_full_key", "sort_big_log2", "sort_scan_log2", "paint_lpt",
+ * "band_copy", "copy_bands", "sort_full_key", "sort_big_log2", "sort_scan_log2", "sort_counts", "paint_lpt",
  * "paint_wide", "band_filter", "sync_free", "host_slices", "slice_bands", "slice_min_points", "slice_chain",
  * "test_gap_cap", "test_fast_shrink".
  * Defaults come from the environment (FORMA_SPECULATE, ...); see DESIGN.md section 6. */
@@ -596,6 +596,17 @@ int forma_renderer_sort_pairs(forma_renderer*, int layout, int mode, uint64_t* k
 /* The bounds the last frame's segment sort was planned from: out[0..2] = layer, tile_x, tile_y
  * (the largest value each field was taken to have), out[3] = the key bits the plan sorts. */
 void forma_renderer_sort_bounds(const forma_renderer*, uint64_t out[4]);
+/* The per-tile digit counts of the last frame's segment sort (option "sort_counts"): the counts
+ * its reduce-then-scan passes were given by the kernels that wrote their keys. keep: 1 = the
+ * following frames of this renderer keep a copy of every pass's counts, 0 = they do not, -1 =
+ * unchanged. info[0]: where pass 0's counts came from: 0 no tile counts (option off, or a sort
+ * without reduce-then-scan passes), 1 the emit pass launched before the count read-back, with the
+ * previous frame's pass-0 digit, 2 the emit pass launched after it (no speculation, or segments
+ * beyond the speculative capacity), 3 an upsweep pass of the sort (first frame, the digit changed,
+ * the previous frame had no tile counts); info[1] = passes and info[2] = 4096-key tiles of the
+ * kept counts (0 when none were kept). `out` (may be null) gets min(cap, passes * tiles * 256) u32:
+ * pass p's count of digit d in tile t at [(p * tiles + t) * 256 + d]. Returns passes * tiles * 256. */
+uint64_t forma_renderer_sort_counts(forma_renderer*, int keep, uint32_t info[3], uint32_t* out, uint64_t cap);
 
 #ifdef __cplusplus
 }
