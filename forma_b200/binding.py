@@ -207,6 +207,11 @@ class _CRect(C.Structure):
     _fields_ = [("hor_start", C.c_uint64), ("hor_end", C.c_uint64), ("vert_start", C.c_uint64), ("vert_end", C.c_uint64)]
 
 
+class _CMasks(C.Structure):  # forma_masks
+    _fields_ = [("ptr", C.c_void_p), ("first_order", C.c_uint32), ("n_orders", C.c_uint32), ("format", C.c_uint32),
+                ("stride", C.c_uint64), ("plane_stride", C.c_uint64)]
+
+
 class _CTimings(C.Structure):
     _fields_ = [
         ("line_setup_ms", C.c_double), ("rasterize_ms", C.c_double), ("sort_ms", C.c_double),
@@ -320,6 +325,13 @@ SIGNATURES = {
                                                     _u32p, C.c_uint32, C.POINTER(_CTimings)]),
     "renderer_render_batch_over_device": (C.c_int, [_vp, C.POINTER(_vp), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64,
                                                     C.c_uint64, _u32p, C.c_uint32, C.POINTER(_CTimings)]),
+    "renderer_render_masks": (C.c_int, [_vp, _vp, C.POINTER(_CMasks), C.c_uint64, C.c_uint64, C.POINTER(_CRect), C.POINTER(_CTimings)]),
+    "renderer_render_masks_device": (C.c_int, [_vp, _vp, C.POINTER(_CMasks), C.c_uint64, C.c_uint64, C.POINTER(_CRect), _vp,
+                                               C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
+    "renderer_render_views_masks_device": (C.c_int, [_vp, _vp, _fp, C.c_uint32, C.POINTER(_CMasks), C.c_uint64, C.c_uint64, _vp,
+                                                     C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
+    "renderer_render_batch_masks_device": (C.c_int, [_vp, C.POINTER(_vp), C.c_uint32, C.POINTER(_CMasks), C.c_uint64, C.c_uint64,
+                                                     _vp, C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
     "renderer_launch_count": (C.c_uint64, [_vp]),
     "renderer_stage_times": (None, [_vp, C.POINTER(C.c_double)]),
     "renderer_counters": (None, [_vp, _u64p]),
@@ -376,6 +388,21 @@ LINEAR_SYMBOLS = ("renderer_render_linear", "renderer_render_linear_device", "re
 # render_batch_over_device).
 OVER_SYMBOLS = ("renderer_render_over_device", "renderer_render_views_over_device", "renderer_render_batch_over_device")
 
+# The same for layer coverage masks (Renderer.render_masks, render_masks_device, render_views_masks_device,
+# render_batch_masks_device).
+MASK_SYMBOLS = ("renderer_render_masks", "renderer_render_masks_device", "renderer_render_views_masks_device",
+                "renderer_render_batch_masks_device")
+# Value formats of mask planes: name -> (FORMA_MASK_*, bytes per value, numpy dtype).
+MASK_FORMATS = {"f32": (0, 4, np.float32), "u8": (1, 1, np.uint8)}
+
+
+def mask_format(fmt: str):
+    """(FORMA_MASK_* code, bytes per value, numpy dtype) of "f32" or "u8"."""
+    if fmt not in MASK_FORMATS:
+        raise ValueError(f"mask format {fmt!r}: 'f32' or 'u8'")
+    return MASK_FORMATS[fmt]
+
+
 # Pixel formats of linear frames: name -> (FORMA_PIXEL_*, bytes per pixel, element dtype).
 PIXEL_FORMATS = {"f16": (1, 8, np.float16), "f32": (2, 16, np.float32)}
 # ... and of frames over a background, which may be sRGB8 as well.
@@ -397,7 +424,7 @@ def over_format(fmt: str):
 
 
 _OPTIONAL_SYMBOLS = frozenset(ID_FRAME_SYMBOLS + VIEW_SYMBOLS + BATCH_SYMBOLS + STACK_ID_SYMBOLS + SORT_DEBUG_SYMBOLS +
-                              LINEAR_SYMBOLS + OVER_SYMBOLS)
+                              LINEAR_SYMBOLS + OVER_SYMBOLS + MASK_SYMBOLS)
 
 
 class Api:
@@ -1140,6 +1167,102 @@ class Renderer:
         n, args = self._batch_args(comps)
         return self._stack(self._api.renderer_render_batch_over_device, "Renderer::render_batch_over_device", args, n, width, height,
                            (int(device_ptr), stride, frame_stride, channels, None), None, timings, bpp, (code,))
+
+    @staticmethod
+    def _mask_layout(width, height, n_orders, format, stride, plane_stride):
+        """(FORMA_MASK_* code, bpp, dtype, stride, plane_stride) with the defaults of a contiguous
+        [K, height, width] array: stride = bpp * width, plane_stride = height * stride."""
+        code, bpp, dtype = mask_format(format)
+        stride = width * bpp if stride is None else stride
+        return code, bpp, dtype, stride, height * stride if plane_stride is None else plane_stride
+
+    def render_masks(self, composition: Composition, masks: np.ndarray, width: int, height: int, first_order: int,
+                     n_orders: Optional[int] = None, crop: Optional[Rect] = None, stride: Optional[int] = None,
+                     plane_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """Layer coverage masks into a host array (see include/forma_b200.h: forma_renderer_render_masks):
+        plane k holds the coverage (x clip mask) of layer order first_order + k, amodal, whatever
+        the layers above it. `masks`: a writable contiguous float32 ("f32", exact) or uint8 ("u8",
+        the alpha byte of sRGB8 frames) array, by default [K, height, width] with K = n_orders
+        (default masks.shape[0]); strides in bytes. Only the crop's tile rectangle of each plane
+        is written."""
+        fmt = {np.dtype(np.float32): "f32", np.dtype(np.uint8): "u8"}.get(masks.dtype)
+        assert fmt is not None and masks.flags["C_CONTIGUOUS"], "a contiguous float32 or uint8 array"
+        k = masks.shape[0] if n_orders is None else n_orders
+        code, bpp, _, stride, plane_stride = self._mask_layout(width, height, k, fmt, stride, plane_stride)
+        assert k == 0 or masks.nbytes >= (k - 1) * plane_stride + (height - 1) * stride + bpp * width
+        m = _CMasks(masks.ctypes.data, first_order, k, code, stride, plane_stride)
+        _, _, rect = self._common(RGBA, Color(), crop)
+        t = _CTimings() if timings else None
+        st = self._api.renderer_render_masks(self._h, composition._h, C.byref(m), width, height,
+                                             C.byref(rect) if rect is not None else None, C.byref(t) if t is not None else None)
+        self._api.check(st, "Renderer::render_masks")
+        return _timings(t)
+
+    def render_masks_device(self, composition: Composition, masks_ptr: int, width: int, height: int, first_order: int,
+                            n_orders: int, format: str = "f32", crop: Optional[Rect] = None, stride: Optional[int] = None,
+                            plane_stride: Optional[int] = None, rgba_ptr: Optional[int] = None, channels=RGBA,
+                            clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), rgba_stride: Optional[int] = None,
+                            timings: bool = True) -> Optional[Timings]:
+        """render_masks into device memory: with the defaults, the data_ptr() of a contiguous
+        [n_orders, height, width] float32 ("f32") or uint8 ("u8") CUDA tensor. With `rgba_ptr` the
+        frame of render_device (no layer cache; default stride 4 * width) is written as well, from
+        the same pass."""
+        code, _, _, stride, plane_stride = self._mask_layout(width, height, n_orders, format, stride, plane_stride)
+        m = _CMasks(int(masks_ptr), first_order, n_orders, code, stride, plane_stride)
+        ch, cc, rect = self._common(channels, clear_color, crop)
+        t = _CTimings() if timings else None
+        st = self._api.renderer_render_masks_device(self._h, composition._h, C.byref(m), width, height,
+                                                    C.byref(rect) if rect is not None else None,
+                                                    None if rgba_ptr is None else C.c_void_p(int(rgba_ptr)),
+                                                    4 * width if rgba_stride is None else rgba_stride, ch, cc,
+                                                    C.byref(t) if t is not None else None)
+        self._api.check(st, "Renderer::render_masks_device")
+        return _timings(t)
+
+    def _stack_masks(self, fn, what, first_args, n, masks_ptr, width, height, first_order, n_orders, format, stride, plane_stride, rgba_ptr,
+                     channels, clear_color, rgba_stride, frame_stride, timings):
+        """Calls `fn`, the mask entry point of views or batches, on chunks of at most
+        max_views(height) frames (see _stack)."""
+        code, _, _, stride, plane_stride = self._mask_layout(width, height, n_orders, format, stride, plane_stride)
+        rgba_stride, frame_stride = self._strides(width, height, rgba_stride, frame_stride)
+        ch, cc, _ = self._common(channels, clear_color, None)
+        chunk = max(self.max_views(height), 1)
+        t = None
+        for first in range(0, max(n, 1), chunk):
+            m = _CMasks(int(masks_ptr) + first * n_orders * plane_stride, first_order, n_orders, code, stride, plane_stride)
+            rgba = None if rgba_ptr is None else C.c_void_p(int(rgba_ptr) + first * frame_stride)
+            t = _CTimings() if timings else None
+            st = fn(self._h, *first_args(first, min(chunk, n - first)), C.byref(m), width, height, rgba, rgba_stride, frame_stride, ch, cc,
+                    C.byref(t) if t is not None else None)
+            self._api.check(st, what)
+        return _timings(t)
+
+    def render_views_masks_device(self, composition: Composition, views, masks_ptr: int, width: int, height: int, first_order: int,
+                                  n_orders: int, format: str = "f32", stride: Optional[int] = None,
+                                  plane_stride: Optional[int] = None, rgba_ptr: Optional[int] = None, channels=RGBA,
+                                  clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), rgba_stride: Optional[int] = None,
+                                  view_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """The masks (see render_masks) of every view of render_views_device, in one pass: with the
+        defaults, the data_ptr() of a contiguous [N, n_orders, height, width] CUDA tensor; every
+        view holds the same orders. With `rgba_ptr` the frames of render_views_device are written
+        as well. Chunked like render_views."""
+        n, args = self._view_args(composition, views)
+        return self._stack_masks(self._api.renderer_render_views_masks_device, "Renderer::render_views_masks_device", args, n, masks_ptr, width,
+                                 height, first_order, n_orders, format, stride, plane_stride, rgba_ptr, channels, clear_color,
+                                 rgba_stride, view_stride, timings)
+
+    def render_batch_masks_device(self, comps, masks_ptr: int, width: int, height: int, first_order: int, n_orders: int,
+                                  format: str = "f32", stride: Optional[int] = None, plane_stride: Optional[int] = None,
+                                  rgba_ptr: Optional[int] = None, channels=RGBA, clear_color: Color = Color(1.0, 1.0, 1.0, 1.0),
+                                  rgba_stride: Optional[int] = None, frame_stride: Optional[int] = None,
+                                  timings: bool = True) -> Optional[Timings]:
+        """The masks (see render_masks) of every frame of render_batch_device, in one pass: frame c's
+        planes hold comps[c]'s own orders [first_order, first_order + n_orders). Layout as for
+        render_views_masks_device; chunked like render_batch."""
+        n, args = self._batch_args(comps)
+        return self._stack_masks(self._api.renderer_render_batch_masks_device, "Renderer::render_batch_masks_device", args, n, masks_ptr, width,
+                                 height, first_order, n_orders, format, stride, plane_stride, rgba_ptr, channels, clear_color,
+                                 rgba_stride, frame_stride, timings)
 
     def launch_count(self) -> int:
         return int(self._api.renderer_launch_count(self._h))

@@ -363,6 +363,23 @@ void launch_paint_ids(const PaintScene& S, const uint64_t* segs, const EntryRec*
                       const uint32_t* heavy, const uint32_t* heavy_count, uint8_t* id_flags, uint32_t* ids, size_t ids_stride,
                       float min_coverage, uint32_t* tile_counter, cudaStream_t st, uint32_t rows = 0,
                       const BatchFrame* frames = nullptr);
+// Layer coverage masks (kernels_ids.cu, see forma_renderer_render_masks): n_orders planes per frame
+// of n_frames, plane (b, k) at ptr + (b * n_orders + k) * plane_stride with rows `stride` bytes
+// apart, holding order first_order + k: f32 (format 0) or the u8 encode of alpha (format 1).
+struct MaskFrame {
+    uint8_t* ptr;
+    uint64_t stride, plane_stride;
+    uint32_t first_order, n_orders, format;
+    uint32_t height;    // rows of one frame
+    uint32_t n_frames;  // 1 for a single frame
+};
+// Zeroes the written rectangle of every plane (the crop's tile rectangle of a single frame, each
+// frame's width x height pixels of a stack), then paints the masks from the tables like
+// launch_paint_ids (id_flags: the same scratch). rows != 0: S stacks frames of `rows` tile rows;
+// frames != nullptr: a batch, whose entries carry frames[c].order_base + order. Returns the launches.
+uint32_t launch_paint_masks(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range,
+                            const uint32_t* heavy, const uint32_t* heavy_count, uint8_t* id_flags, const MaskFrame& m,
+                            uint32_t* tile_counter, cudaStream_t st, uint32_t rows = 0, const BatchFrame* frames = nullptr);
 // The painter tables of a batch: the device tables of its distinct compositions, concatenated.
 // Composition k's orders land at order_base + order (the slots they name shifted by style_base,
 // -1 kept), its StyleRecs at style_base with stop_first + stop_base and tex_first + texel_base;

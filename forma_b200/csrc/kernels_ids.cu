@@ -25,6 +25,7 @@
 // their entries (BatchFrame::order_base), and the walk compares layers and clip ranges in that
 // shifted space; paint_ids_stacked_kernel, the same body, takes the frame's base off every ID it
 // stores (one look-up per tile).
+#include <algorithm>
 #include <mutex>
 
 #include "../../include/forma_b200.h"
@@ -204,6 +205,286 @@ void launch_paint_ids(const PaintScene& S, const uint64_t* segs, const EntryRec*
         const uint32_t want = id_grid_limit(paint_ids_kernel, blocks_per_sm[0]);
         paint_ids_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles);
     }
+}
+
+// ---------------------------------------------------------------------------
+// Layer coverage masks (forma_renderer_render_masks): plane k of a frame holds, per pixel, the
+// coverage of order o = first_order + k as paint_layer computes it, times the clip mask where a
+// clip applies to o. Amodal: every layer of the tile is walked, none is skipped below an opaque
+// one. The same warp scheme as the ID kernel (tickets, heavy lists first, lane = the painter's
+// eight pixels), with entry_coverage, stage_group and skip_trivial_clips_ids reused as they are.
+//
+// Tiles without clip-ish entries: the entries are sorted by layer, so the walk bisects to the
+// window's first entry and stops at its end; nothing outside the window is read. Tiles with
+// clips walk bottom-up from their first entry with the painter's clip state after
+// skip_trivial_clips (as in the ID kernel's clip tiles, without the skip below the first opaque
+// layer). A clip below the window is only accumulated when its mask can still apply to a window
+// entry (the clip state's last layer reaches the window); other entries below the window are
+// skipped without reading their segments.
+//
+// Only tiles with window entries are stored, and each such entry stores its own plane: the zero
+// fill before the kernel (zero_masks_kernel) gives every other pixel its 0.
+// ---------------------------------------------------------------------------
+struct MaskInputs {
+    IdInputs t;  // tables, id_flags and ticket counter (t.ids, t.ids_stride and t.min_coverage unused)
+    uint8_t* out;
+    uint64_t stride, plane_stride;
+    uint32_t first_order, n_orders;
+    uint32_t height;  // rows of one frame
+    uint32_t rows;    // stacks: tile rows per frame; 0: a single frame
+    bool u8;
+};
+
+// compute_srgb's alpha encode (paint_math.cuh: to_byte) of a coverage in [0, 1].
+__device__ __forceinline__ uint32_t mask_byte(float v) {
+    const float scaled = fminf(fmaxf(v * 255.0f, 0.0f), 255.0f);
+    return __float_as_uint(scaled + __uint_as_float(0x4B000000u)) & 0xFFu;
+}
+
+// The lane's eight values at `p` (its first pixel of plane row), n <= 8 of them inside the frame.
+__device__ __forceinline__ void store_mask(uint8_t* p, const float cov[8], uint32_t n, bool u8, bool vec_ok) {
+    if (u8) {
+        uint32_t lo = 0, hi = 0;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            lo |= mask_byte(cov[j]) << (8 * j);
+            hi |= mask_byte(cov[4 + j]) << (8 * j);
+        }
+        if (vec_ok && n == 8u) {
+            *reinterpret_cast<uint2*>(p) = make_uint2(lo, hi);
+        } else {
+#pragma unroll
+            for (uint32_t j = 0; j < 8u; ++j)
+                if (j < n) p[j] = (uint8_t)((j < 4u ? lo >> (8u * j) : hi >> (8u * (j - 4u))) & 0xFFu);
+        }
+        return;
+    }
+    float* f = reinterpret_cast<float*>(p);
+    if (vec_ok && n == 8u) {
+        reinterpret_cast<float4*>(f)[0] = make_float4(cov[0], cov[1], cov[2], cov[3]);
+        reinterpret_cast<float4*>(f)[1] = make_float4(cov[4], cov[5], cov[6], cov[7]);
+    } else {
+#pragma unroll
+        for (uint32_t j = 0; j < 8u; ++j)
+            if (j < n) f[j] = cov[j];
+    }
+}
+
+template <bool kBatch>
+__device__ __forceinline__ void paint_masks_body(const PaintScene& S, const MaskInputs& in, uint32_t n_tiles,
+                                                 const BatchFrame* __restrict__ frames) {
+    __shared__ __align__(16) IdWarpSmem s_warp[kIdWarpsPerBlock];
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+    IdWarpSmem& W = s_warp[warp];
+    const IdInputs& T = in.t;
+    const uint32_t ntx = S.tx_hi - S.tx_lo;
+    const uint32_t row = lane >> 1, hx = lane & 1u;
+    const uint32_t bpp = in.u8 ? 1u : 4u;
+    const bool vec_ok = ((reinterpret_cast<uintptr_t>(in.out) | (uintptr_t)in.stride | (uintptr_t)in.plane_stride) &
+                         (in.u8 ? 7u : 15u)) == 0u;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) W.cells[k * 32 + lane] = 0u;
+    __syncwarp();
+
+    uint32_t hcount[kHeavyClasses], H = 0;
+#pragma unroll
+    for (int c = 0; c < kHeavyClasses; ++c) {
+        hcount[c] = T.heavy ? T.heavy_count[c] : 0u;
+        H += hcount[c];
+    }
+    const uint32_t n_tickets = H + n_tiles;
+    for (;;) {
+        uint32_t ticket = 0;
+        if (lane == 0) ticket = atomicAdd(T.tile_counter, 1u);
+        ticket = __shfl_sync(kFullMask, ticket, 0);
+        if (ticket >= n_tickets) break;
+        uint32_t tid;
+        if (ticket < H) {  // the heavy lists, largest class first (as in the ID kernel)
+            uint32_t t = ticket;
+            int c = kHeavyClasses - 1;
+#pragma unroll
+            for (int q = kHeavyClasses - 1; q > 0; --q)
+                if (c == q && t >= hcount[q]) {
+                    t -= hcount[q];
+                    c = q - 1;
+                }
+            tid = T.heavy[(size_t)c * T.n_tiles_total + t];
+            const uint32_t ty = tid / S.tiles_x, tx = tid - ty * S.tiles_x;
+            if (ty < S.ty_lo || ty >= S.ty_hi || tx < S.tx_lo || tx >= S.tx_hi) continue;
+        } else {
+            const uint32_t lin = ticket - H;
+            tid = (S.ty_lo + lin / ntx) * S.tiles_x + S.tx_lo + lin % ntx;
+        }
+        const uint2 range = T.tile_range[tid];
+        const uint32_t b = range.x, e = range.y;
+        if (ticket >= H && T.heavy && e - b >= kHeavyMin) continue;  // done from its list
+        if (e == b) continue;
+        const uint32_t ty = tid / S.tiles_x, tx = tid - ty * S.tiles_x;
+        const uint32_t frame = in.rows ? ty / in.rows : 0u, fty = in.rows ? ty - frame * in.rows : ty;
+        const uint32_t base = kBatch ? frames[frame].order_base : 0u;
+        const uint32_t lo_w = base + in.first_order, hi_w = lo_w + in.n_orders;  // the window in the entries' layer space
+        const uint32_t py = fty * 16u + row, x0 = tx * 16u + hx * 8u;
+        const bool inside = py < in.height && x0 < S.width;
+        const uint32_t n_px = inside ? min(8u, S.width - x0) : 0u;
+        uint8_t* const px = in.out + ((size_t)frame * in.n_orders) * in.plane_stride + (size_t)py * in.stride + (size_t)x0 * bpp;
+        float cov[8];
+        auto put = [&](uint32_t layer) {
+            if (inside) store_mask(px + (size_t)(layer - lo_w) * in.plane_stride, cov, n_px, in.u8, vec_ok);
+        };
+        auto coverage = [&](const EntryRec& h) {
+            if (h.pad & kFlagFull) {  // no segments, a full carried cover: coverage 1 without reading anything
+#pragma unroll
+                for (int j = 0; j < 8; ++j) cov[j] = 1.0f;
+            } else {
+                entry_coverage(W, h, T.segs, lane, cov);
+            }
+        };
+
+        bool clip_tile = false;
+        for (uint32_t p0 = b; p0 < e && !clip_tile; p0 += 32u) {
+            const uint32_t p = p0 + lane;
+            clip_tile = __any_sync(kFullMask, p < e && (T.recs[p].flags0 & kFlagClipish) != 0u);
+        }
+
+        if (!clip_tile) {
+            uint32_t lo = b, hi = e;  // the first entry of the window
+            while (lo < hi) {
+                const uint32_t mid = (lo + hi) >> 1;
+                if (T.recs[mid].layer < lo_w) lo = mid + 1u;
+                else hi = mid;
+            }
+            bool done = false;
+            for (uint32_t p0 = lo; p0 < e && !done; p0 += 32u) {
+                const uint32_t cnt = min(32u, e - p0);
+                stage_group(W, T, p0, cnt, false, lane);
+                for (uint32_t k = 0; k < cnt; ++k) {
+                    const EntryRec& h = W.hdr[k];
+                    if (h.layer >= hi_w) {
+                        done = true;
+                        break;
+                    }
+                    if (h.pad & kFlagMaskedOut) continue;  // a layer without props
+                    coverage(h);
+                    put(h.layer);
+                }
+            }
+        } else {
+            if (lane == 0) skip_trivial_clips_ids(T.recs, T.id_flags, b, e);
+            __syncwarp();
+            bool clip_active = false, done = false;
+            uint32_t clip_last = 0;
+            for (uint32_t p0 = b; p0 < e && !done; p0 += 32u) {
+                const uint32_t cnt = min(32u, e - p0);
+                stage_group(W, T, p0, cnt, true, lane);
+                for (uint32_t k = 0; k < cnt; ++k) {
+                    const EntryRec& h = W.hdr[k];
+                    const uint32_t flags = h.pad, layer = h.layer, meta = h.meta;
+                    if (layer >= hi_w) {
+                        done = true;
+                        break;
+                    }
+                    const bool is_clip = ((meta >> 1) & 1u) != 0u, in_window = layer >= lo_w;
+                    if (flags & kFlagMaskedOut) {
+                        // Not painted, no clip state. A clip's plane is its own coverage all the
+                        // same (a layer without props has meta 0: no clip).
+                        if (is_clip && in_window) {
+                            coverage(h);
+                            put(layer);
+                        }
+                        continue;
+                    }
+                    if (clip_active && clip_last < layer) clip_active = false;  // mod.rs:302-306
+                    if (is_clip) {  // clip_at, mod.rs:449-464
+                        if (!clip_active) {
+                            clip_active = true;
+                            clip_last = layer + h.clip_layers;
+                        }
+                        const bool mask_used = clip_last >= lo_w;
+                        if (!mask_used && !in_window) continue;
+                        coverage(h);
+                        if (mask_used) {
+                            float4* m4 = reinterpret_cast<float4*>(W.clip);
+                            m4[2u * lane] = make_float4(cov[0], cov[1], cov[2], cov[3]);
+                            m4[2u * lane + 1u] = make_float4(cov[4], cov[5], cov[6], cov[7]);
+                            __syncwarp();
+                        }
+                        if (in_window) put(layer);
+                        continue;
+                    }
+                    if (!in_window) continue;
+                    const bool apply_clip = ((meta >> 2) & 1u) && !(flags & kFlagSkipClip);
+                    if (apply_clip && !clip_active) continue;  // mod.rs:317-323: never painted, 0
+                    coverage(h);
+                    if (apply_clip) {
+                        const float4* m4 = reinterpret_cast<const float4*>(W.clip);
+                        const float4 m0 = m4[2u * lane], m1 = m4[2u * lane + 1u];
+                        const float m[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) cov[j] = __fmul_rn(cov[j], m[j]);
+                    }
+                    put(layer);
+                }
+            }
+        }
+    }
+}
+
+__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) paint_masks_kernel(PaintScene S, MaskInputs in, uint32_t n_tiles) {
+    paint_masks_body<false>(S, in, n_tiles, nullptr);
+}
+// S stacks the frames of a batch; frame c's entries carry frames[c].order_base + order, and its
+// planes hold the frame's own orders.
+__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) paint_masks_stacked_kernel(PaintScene S, MaskInputs in, uint32_t n_tiles,
+                                                                                    const BatchFrame* __restrict__ frames) {
+    paint_masks_body<true>(S, in, n_tiles, frames);
+}
+
+// Zeroes `row_bytes` bytes from byte x0 of rows [y0, y0 + n_rows) of n_planes planes: one warp per
+// row, 16-byte stores between an unaligned head and tail.
+constexpr int kZeroWarps = 8;
+__global__ void __launch_bounds__(kZeroWarps * 32) zero_masks_kernel(uint8_t* out, uint64_t stride, uint64_t plane_stride,
+                                                                     uint32_t n_planes, uint32_t y0, uint32_t n_rows, uint64_t x0,
+                                                                     uint64_t row_bytes) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint64_t total = (uint64_t)n_planes * n_rows;
+    for (uint64_t r = (uint64_t)blockIdx.x * kZeroWarps + (threadIdx.x >> 5); r < total; r += (uint64_t)gridDim.x * kZeroWarps) {
+        const uint64_t plane = r / n_rows, y = y0 + r % n_rows;
+        uint8_t* p = out + plane * plane_stride + y * stride + x0;
+        const uint64_t head = min(row_bytes, (uint64_t)((16u - (reinterpret_cast<uintptr_t>(p) & 15u)) & 15u));
+        const uint64_t n_vec = (row_bytes - head) / 16u, tail = head + 16u * n_vec;
+        if (lane < head) p[lane] = 0;
+        uint4* q = reinterpret_cast<uint4*>(p + head);
+        for (uint64_t i = lane; i < n_vec; i += 32u) q[i] = make_uint4(0u, 0u, 0u, 0u);
+        if (tail + lane < row_bytes) p[tail + lane] = 0;
+    }
+}
+
+uint32_t launch_paint_masks(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range,
+                            const uint32_t* heavy, const uint32_t* heavy_count, uint8_t* id_flags, const MaskFrame& m,
+                            uint32_t* tile_counter, cudaStream_t st, uint32_t rows, const BatchFrame* frames) {
+    if (S.tx_hi <= S.tx_lo || S.ty_hi <= S.ty_lo) return 0;
+    const uint32_t bpp = m.format == FORMA_MASK_U8 ? 1u : 4u;
+    // The written rectangle: a stack's frames whole, a single frame's tile rectangle clipped to it.
+    const uint32_t y0 = rows ? 0u : S.ty_lo * 16u, y1 = rows ? m.height : min(S.ty_hi * 16u, S.height);
+    const uint32_t x0 = rows ? 0u : S.tx_lo * 16u, x1 = rows ? S.width : min(S.tx_hi * 16u, S.width);
+    const uint64_t n_rows = (uint64_t)m.n_frames * m.n_orders * (y1 - y0);
+    const uint32_t zero_ctas = (uint32_t)std::min<uint64_t>((n_rows + kZeroWarps - 1) / kZeroWarps, 8u * (uint64_t)device_sm_count());
+    zero_masks_kernel<<<zero_ctas, kZeroWarps * 32, 0, st>>>(m.ptr, m.stride, m.plane_stride, m.n_frames * m.n_orders, y0, y1 - y0,
+                                                             (uint64_t)x0 * bpp, (uint64_t)(x1 - x0) * bpp);
+    const uint32_t n_tiles = (S.tx_hi - S.tx_lo) * (S.ty_hi - S.ty_lo);
+    cudaMemsetAsync(tile_counter, 0, sizeof(uint32_t), st);
+    MaskInputs in{IdInputs{segs, recs, tile_range, heavy, heavy_count, S.tiles_x * S.tiles_y, id_flags, nullptr, 0, 0.0f, tile_counter},
+                  m.ptr, m.stride, m.plane_stride, m.first_order, m.n_orders, m.height, rows, m.format == FORMA_MASK_U8};
+    static int blocks_per_sm[2][kMaxDevices] = {{0}};
+    const uint32_t need = (n_tiles + kIdWarpsPerBlock - 1) / kIdWarpsPerBlock;
+    if (frames) {
+        const uint32_t want = id_grid_limit(paint_masks_stacked_kernel, blocks_per_sm[1]);
+        paint_masks_stacked_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles, frames);
+    } else {
+        const uint32_t want = id_grid_limit(paint_masks_kernel, blocks_per_sm[0]);
+        paint_masks_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles);
+    }
+    return 2;
 }
 
 }  // namespace forma

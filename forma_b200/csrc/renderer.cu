@@ -557,13 +557,21 @@ int Renderer::render(const FrameRequest& q) {
         return DeviceFrame{t.ptr, direct || !stack ? t.stride : t.bpp * q.width, direct};
     };
     FramePlan p{device_frame(q.rgba), device_frame(q.ids), stack ? (uint32_t)((q.height + 15u) / 16u) : 0u, false, false};
-    // The PaintScene of the RGBA target, or of the ID target when it is alone.
+    // Masks are painted straight into the caller's planes on the device (a stack's tile rows are
+    // mapped to its frames by the kernel), host masks into scratch planes of 16-byte aligned rows.
+    p.masks = DeviceFrame{q.masks.ptr, q.masks.stride, q.masks.on_device};
+    p.mask_plane_stride = q.masks.plane_stride;
+    if (q.masks.ptr && !q.masks.on_device) {
+        p.masks.stride = (q.masks.bpp() * q.width + 15u) / 16u * 16u;
+        p.mask_plane_stride = p.masks.stride * q.height;
+    }
+    // The PaintScene of the RGBA target, or of the ID target or the masks when they are alone.
     // An over frame has no clear colour: its kernels read each pixel's, and upgrade Alpha -> One per
     // pixel, so the scene's channels stay as given.
     static const uint32_t kIdChannels[4] = {0, 1, 2, 3};
     static const float kIdClear[4] = {0, 0, 0, 0};
     PaintScene S{};
-    st = begin_frame(S, q.width, rgba ? p.rgba.stride : p.ids.stride, stack ? (uint64_t)q.n * p.rows * 16u : q.height,
+    st = begin_frame(S, q.width, rgba ? p.rgba.stride : q.ids.ptr ? p.ids.stride : p.masks.stride, stack ? (uint64_t)q.n * p.rows * 16u : q.height,
                      rgba ? q.channels : kIdChannels, rgba && !q.rgba.over ? q.clear : kIdClear, q.crop);
     if (st) return st;
     if (rgba && !p.rgba.direct) {
@@ -573,6 +581,10 @@ int Renderer::render(const FrameRequest& q) {
     if (q.ids.ptr && !p.ids.direct) {
         FORMA_CUDA_TRY(id_frame.reserve((size_t)(p.ids.stride / 4u) * S.height));
         p.ids.ptr = reinterpret_cast<uint8_t*>(id_frame.ptr);
+    }
+    if (q.masks.ptr && !p.masks.direct) {
+        FORMA_CUDA_TRY(mask_frame.reserve((size_t)p.mask_plane_stride * q.masks.n_orders));
+        p.masks.ptr = mask_frame.ptr;
     }
     // (A host float frame is painted whole and copied back once.)
     p.in_bands = rgba && q.rgba.bpp == 4u && !stack && !q.rgba.on_device && !q.cache && S.ty_hi - S.ty_lo >= (copy_bands_override ? 8u : 32u) &&
@@ -618,7 +630,7 @@ int Renderer::check_request(const FrameRequest& q) {
         }
         return (int)FORMA_STATUS_OK;
     };
-    int st = q.rgba.ptr || !q.ids.ptr ? check_target(q.rgba) : FORMA_STATUS_OK;
+    int st = q.rgba.ptr || (!q.ids.ptr && !q.masks.ptr) ? check_target(q.rgba) : FORMA_STATUS_OK;
     if (st) return st;
     if (q.rgba.bpp != 4u && (((uintptr_t)q.rgba.ptr | q.rgba.stride | q.rgba.frame_stride) & 3u) != 0u) {
         set_error("invalid float frame: buffer, stride %llu and %s stride %llu must be multiples of 4 bytes",
@@ -653,6 +665,10 @@ int Renderer::check_request(const FrameRequest& q) {
             return FORMA_STATUS_INVALID;
         }
         st = check_target(t);
+        if (st) return st;
+    }
+    if (q.masks.ptr) {
+        st = check_masks(q);
         if (st) return st;
     }
     if ((q.kind == FrameKind::views && !q.views) || (q.kind == FrameKind::batch && !q.batch)) {
@@ -691,6 +707,44 @@ int Renderer::check_request(const FrameRequest& q) {
         set_error("the batch's compositions need %llu layer orders; the layer field holds %u",
                   (unsigned long long)order_sum, 1u << 21);
         return FORMA_STATUS_ORDER;
+    }
+    return FORMA_STATUS_OK;
+}
+
+// The masks target's own checks (see forma_renderer_render_masks), then those of any target for
+// its size, the frame count and its planes: masks go alone or with an sRGB8 RGBA target that is
+// neither painted over its pixels nor cached, never with an ID target.
+int Renderer::check_masks(const FrameRequest& q) {
+    const MaskTarget& m = q.masks;
+    const uint64_t width = q.width, height = q.height, bpp = m.bpp(), frames = q.kind == FrameKind::single ? 1u : q.n;
+    if (q.ids.ptr || (q.rgba.ptr && (q.rgba.bpp != 4u || q.rgba.over || q.cache))) {
+        set_error("masks go alone or with an sRGB8 RGBA frame without a layer cache");
+        return FORMA_STATUS_INVALID;
+    }
+    if (m.n_orders == 0u || (uint64_t)m.first_order + m.n_orders > (1ull << 21) || m.format > FORMA_MASK_U8) {
+        set_error("invalid masks: orders [%u, %u + %u) (1 to 2^21 orders below 2^21), format %u", m.first_order, m.first_order,
+                  m.n_orders, m.format);
+        return FORMA_STATUS_INVALID;
+    }
+    if (width == 0 || height == 0 || width > FORMA_MAX_WIDTH || height > FORMA_MAX_HEIGHT || m.stride < bpp * width ||
+        m.plane_stride < (height - 1u) * m.stride + bpp * width ||
+        (bpp == 4u && (((uintptr_t)m.ptr | m.stride | m.plane_stride) & 3u) != 0u)) {
+        set_error("invalid masks %llux%llu: stride %llu, plane stride %llu (f32: multiples of 4 bytes)", (unsigned long long)width,
+                  (unsigned long long)height, (unsigned long long)m.stride, (unsigned long long)m.plane_stride);
+        return FORMA_STATUS_INVALID;
+    }
+    // The whole stack of planes: (frames * K - 1) * plane_stride + one plane, within 64 bits.
+    uint64_t planes = 0, span = 0, end = 0;
+    if (__builtin_mul_overflow(frames, (uint64_t)m.n_orders, &planes) || __builtin_mul_overflow(planes - 1u, m.plane_stride, &span) ||
+        __builtin_add_overflow(span, (height - 1u) * m.stride + bpp * width, &end)) {
+        set_error("the masks' planes overflow 64 bits: %llu planes of stride %llu", (unsigned long long)planes,
+                  (unsigned long long)m.plane_stride);
+        return FORMA_STATUS_INVALID;
+    }
+    if (q.kind != FrameKind::single && (q.n == 0 || q.n > max_views(height))) {
+        set_error("%u %ss of height %llu: between 1 and %u fit in one call", q.n, q.kind == FrameKind::views ? "view" : "frame",
+                  (unsigned long long)height, max_views(height));
+        return FORMA_STATUS_INVALID;
     }
     return FORMA_STATUS_OK;
 }
@@ -809,14 +863,24 @@ int Renderer::paint_step(const FrameRequest& q, const PaintScene& S, const Frame
         }
         const int st = paint(S, p.rgba.ptr, q.rgba.ptr, q.rgba.stride, p.in_bands, heavy_lists, paint_launches, p.rows, q.rgba.bpp,
                              solid_over, q.rgba.over);
-        if (st || !q.ids.ptr) return st;
-        ++*paint_launches;
+        if (st || (!q.ids.ptr && !q.masks.ptr)) return st;
+        if (q.ids.ptr) ++*paint_launches;
+    }
+    FORMA_CUDA_TRY(id_flags.reserve(std::max<size_t>(recs.capacity, 1)));
+    const BatchFrame* frames = q.kind == FrameKind::batch ? reinterpret_cast<const BatchFrame*>(d_batch_lines.ptr) : nullptr;
+    if (q.masks.ptr) {  // the zero fill of the planes, then the masks (the redo of a sync-free frame repeats both)
+        const MaskFrame m{p.masks.ptr, p.masks.stride, p.mask_plane_stride, q.masks.first_order, q.masks.n_orders, q.masks.format,
+                          (uint32_t)q.height, q.kind == FrameKind::single ? 1u : q.n};
+        const uint32_t n = launch_paint_masks(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), id_flags.ptr, m,
+                                              totals.ptr + 8, stream, p.rows, frames);
+        launches += n;
+        *paint_launches = q.rgba.ptr ? *paint_launches + n : n;
+        FORMA_CUDA_TRY(cudaGetLastError());
+        return FORMA_STATUS_OK;
     }
     // A batch's entries carry each frame's order base (bind_batch): the kernel takes it off.
-    FORMA_CUDA_TRY(id_flags.reserve(std::max<size_t>(recs.capacity, 1)));
     launch_paint_ids(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), id_flags.ptr, reinterpret_cast<uint32_t*>(p.ids.ptr),
-                     p.ids.stride, q.ids.min_coverage, totals.ptr + 8, stream, p.rows,
-                     q.kind == FrameKind::batch ? reinterpret_cast<const BatchFrame*>(d_batch_lines.ptr) : nullptr);
+                     p.ids.stride, q.ids.min_coverage, totals.ptr + 8, stream, p.rows, frames);
     ++launches;
     FORMA_CUDA_TRY(cudaGetLastError());
     return FORMA_STATUS_OK;
@@ -853,8 +917,21 @@ int Renderer::output_step(const FrameRequest& q, const PaintScene& S, const Fram
         d2h_bytes += (uint64_t)q.n * height * q.width * t.bpp;
         return (int)FORMA_STATUS_OK;
     };
-    const int st = p.in_bands ? FORMA_STATUS_OK : output(q.rgba, p.rgba);
-    return st ? st : output(q.ids, p.ids);
+    int st = p.in_bands ? FORMA_STATUS_OK : output(q.rgba, p.rgba);
+    st = st ? st : output(q.ids, p.ids);
+    if (st || !q.masks.ptr || q.masks.on_device) return st;
+    // Host masks (single frames): the crop's tile rectangle of every plane.
+    const MaskTarget& m = q.masks;
+    const uint64_t bpp = m.bpp();
+    const uint64_t x0 = (uint64_t)S.tx_lo * 16u, x1 = std::min<uint64_t>((uint64_t)S.tx_hi * 16u, S.width);
+    const uint64_t y0 = (uint64_t)S.ty_lo * 16u, y1 = std::min<uint64_t>((uint64_t)S.ty_hi * 16u, S.height);
+    if (x1 <= x0 || y1 <= y0) return FORMA_STATUS_OK;
+    for (uint32_t k = 0; k < m.n_orders; ++k)
+        FORMA_CUDA_TRY(cudaMemcpy2DAsync(m.ptr + k * m.plane_stride + y0 * m.stride + x0 * bpp, m.stride,
+                                         p.masks.ptr + k * p.mask_plane_stride + y0 * p.masks.stride + x0 * bpp, p.masks.stride,
+                                         (x1 - x0) * bpp, y1 - y0, cudaMemcpyDeviceToHost, stream));
+    d2h_bytes += (uint64_t)m.n_orders * (x1 - x0) * bpp * (y1 - y0);
+    return FORMA_STATUS_OK;
 }
 
 // The frame's PaintScene without its composition tables, for a target that check_request

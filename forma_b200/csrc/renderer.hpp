@@ -50,6 +50,17 @@ struct FrameTarget {
     bool over = false;  // the RGBA target: painted over its own pixels, each its clear colour (see forma_renderer_render_over_device)
 };
 
+// The masks target of a FrameRequest (see forma_renderer_render_masks): n_orders planes of order
+// first_order + k per frame, plane (b, k) at ptr + (b * n_orders + k) * plane_stride, rows `stride`
+// bytes apart, f32 or u8 values (format).
+struct MaskTarget {
+    uint8_t* ptr = nullptr;  // null: the request has no masks
+    bool on_device = false;
+    uint32_t first_order = 0, n_orders = 0, format = 0;
+    uint64_t stride = 0, plane_stride = 0;
+    uint32_t bpp() const { return format == FORMA_MASK_U8 ? 1u : 4u; }
+};
+
 // What a FrameRequest renders. single: one frame of a composition. views: n views of one
 // composition in one pass, stacked top to bottom as one frame of n * ceil(height / 16) tile rows;
 // line setup rasterizes every view in its own coordinates and moves its segments' tile rows to the
@@ -62,7 +73,8 @@ struct FrameTarget {
 enum class FrameKind { single, views, batch };
 
 // One call of Renderer::render: what is rendered, the size of one frame, and its targets: an
-// RGBA target, an ID target (channels {0, 1, 2, 3}, clear colour 0 when it is alone) or both.
+// RGBA target, an ID target (channels {0, 1, 2, 3}, clear colour 0 when it is alone) or both, or
+// masks, alone or with an sRGB8 RGBA target.
 struct FrameRequest {
     FrameKind kind = FrameKind::single;
     uint32_t n = 0;  // stacks: the frames
@@ -73,6 +85,7 @@ struct FrameRequest {
     const forma_rect* crop = nullptr;  // single frames only
     LayerCache* cache = nullptr;       // single RGBA frames only
     FrameTarget rgba, ids;
+    MaskTarget masks;
     Composition* comp = nullptr;          // single, views
     const float* views = nullptr;         // views: n transforms [ux, vx, uy, vy, tx, ty]
     Composition* const* batch = nullptr;  // batch: n compositions (null entries are refused)
@@ -90,6 +103,8 @@ struct FramePlan {
     uint32_t rows;      // stacks: tile rows of each frame; 0: a single frame
     bool in_bands;      // a single host sRGB8 frame painted and copied back band by band (see paint)
     bool pack_written;  // a cached host frame: only the tiles it writes travel back (scatter_written_tiles)
+    DeviceFrame masks;  // the caller's planes on the device, or (host masks) the renderer's scratch ...
+    uint64_t mask_plane_stride;  // ... with this plane stride
 };
 
 // The line setup of a batch (see Renderer::bind_batch).
@@ -300,6 +315,7 @@ class Renderer {
     // target's device frame, run_frame and, for a layer cache, its bookkeeping.
     int render(const FrameRequest& q);
     int check_request(const FrameRequest& q);
+    int check_masks(const FrameRequest& q);
     // One frame of S: uploads, line setup, sort, then the painter tables, paint_step and
     // output_step once or, when the sync-free bounds were too small, twice.
     int run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p);
@@ -308,6 +324,7 @@ class Renderer {
     int output_step(const FrameRequest& q, const PaintScene& S, const FramePlan& p);
     DeviceBuffer<uint8_t> id_flags;   // per entry: the ID kernel's optimizer flags (clip tiles)
     DeviceBuffer<uint32_t> id_frame;  // the ID target's scratch frame
+    DeviceBuffer<uint8_t> mask_frame; // the planes of host masks
     PinnedBuffer<float> h_views;
     DeviceBuffer<float> d_views;
     // A batch's distinct compositions' tables are gathered into the batch tables below, which are

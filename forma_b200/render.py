@@ -1,7 +1,7 @@
 """Headless front end: render an SVG file to PPM / PNG on the GPU.
 
     python -m forma_b200.render in.svg out.ppm [--width W --height H --scale S --device 0] [--ids ids.npy] [--linear out.npy]
-                                               [--over image.{ppm,png}]
+                                               [--over image.{ppm,png}] [--masks masks.npy --mask-orders A:B [--mask-u8]]
 
 The equivalent of the reference's `demo svg --file in.svg --scale S` + the `S` key's
 capture.ppm (demo/src/main.rs, demo/src/runner.rs:193-219: a binary P6 file with the
@@ -14,6 +14,9 @@ H x W x 4 .npy.
 `--over` draws the SVG over an image instead of a white frame: the image (binary PPM, or PNG with
 Pillow) goes to the GPU as an H x W x 4 uint8 tensor, Renderer.render_over_device draws over it, and
 its size replaces --width / --height.
+`--masks` also writes the layer coverage masks of orders [A, B) (`--mask-orders A:B`, Renderer.render_masks):
+per layer its anti-aliased coverage, whatever lies above it, as a (B - A) x H x W float32 .npy, or uint8 with
+`--mask-u8`.
 """
 from __future__ import annotations
 
@@ -73,7 +76,13 @@ def main(argv=None) -> int:
     ap.add_argument("--linear", help="also write the linear float frame (H x W x 4 float32, Renderer.render_linear) to this .npy file")
     ap.add_argument("--over", help="draw over this image (.ppm or .png, Renderer.render_over_device) instead of a white frame; its size "
                                    "replaces --width / --height")
+    ap.add_argument("--masks", help="also write the layer coverage masks (K x H x W, Renderer.render_masks) to this .npy file")
+    ap.add_argument("--mask-orders", default="0:1", help="the masks' layer orders A:B, i.e. [A, B) (default 0:1)")
+    ap.add_argument("--mask-u8", action="store_true", help="masks as uint8 (the alpha byte of sRGB8 frames) instead of float32")
     args = ap.parse_args(argv)
+    mask_lo, mask_hi = (int(v) for v in args.mask_orders.split(":"))
+    if args.masks and mask_hi <= mask_lo:
+        ap.error("--mask-orders A:B needs A < B")
 
     import forma_b200
     from forma_b200 import svg
@@ -118,6 +127,10 @@ def main(argv=None) -> int:
         linear = np.zeros((args.height, args.width, 4), np.float32)
         renderer.render_linear(comp, linear, args.width, args.height, RGBA, Color(1.0, 1.0, 1.0, 1.0), format="f32")
         np.save(args.linear, linear)
+    if args.masks:
+        masks = np.zeros((mask_hi - mask_lo, args.height, args.width), np.uint8 if args.mask_u8 else np.float32)
+        renderer.render_masks(comp, masks, args.width, args.height, mask_lo)
+        np.save(args.masks, masks)
     print(f"{len(paths)} paths parsed in {t1 - t0:.2f} s, composed in {t2 - t1:.2f} s; {t.n_segments} pixel segments; "
           f"last frame: line setup {t.line_setup_ms:.3f} ms, rasterize {t.rasterize_ms:.3f} ms, sort {t.sort_ms:.3f} ms, "
           f"paint {t.paint_ms:.3f} ms ({(t3 - t2) / max(args.frames, 1) * 1e3:.2f} ms per call) -> {args.out}", file=sys.stderr)

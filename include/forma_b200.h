@@ -458,6 +458,70 @@ int forma_renderer_render_batch_over_device(forma_renderer*, forma_composition* 
                                             uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride,
                                             const uint32_t channels[4], uint32_t format, forma_timings* timings /* nullable */);
 
+/* Layer coverage masks (no reference counterpart): each layer's anti-aliased coverage as a plane of
+ * its own, for instance mattes, amodal masks and per-shape losses. A request names a window of
+ * layer orders [first_order, first_order + n_orders), n_orders = K >= 1; plane k holds order
+ * o = first_order + k. Its value at pixel p:
+ *   - o an enabled Func::Draw layer without is_clipped: c_o(p), the coverage the painter's
+ *     paint_layer computes for o at p under its fill rule from its cells and carried cover
+ *     (doubled_area_to_coverage), a multiple of 1/512 in [0, 1];
+ *   - o a Func::Draw layer with is_clipped: c_o(p) x m(p), m the clip mask that applies to o in p's
+ *     tile under the painter's clip state (clip_at, cpu/painter/mod.rs:302-323, 449-464), the
+ *     tile's layers walked bottom-up after the skip_trivial_clips pass with every layer painted:
+ *     nothing is skipped below an opaque layer, so the mask is amodal (the parts other layers hide
+ *     are kept). Where no clip applies to o (no clip active, or the pass masks o out), 0; where the
+ *     pass finds o's clip full, the clip is 1 and the value c_o(p);
+ *   - o a Func::Clip layer: its own coverage c_o(p);
+ *   - anything else (no such layer, a disabled layer, a layer without props): 0.
+ * Colour, alpha, gradient, texture and blend mode play no part, nor does any other layer than the
+ * clips. A plane of an unclipped Draw layer is the alpha of a linear frame (clear colour 0) of the
+ * composition with every other Draw layer disabled and o solid white, opaque and Over.
+ * Formats: FORMA_MASK_F32 stores the value (exact: k / 512 or a product of two such values);
+ * FORMA_MASK_U8 stores compute_srgb's encode of alpha, the low byte of
+ * bits(clamp(255 v, 0, 255) + 2^23).
+ * Layout: plane (frame b, k) starts at ptr + (b K + k) plane_stride, its rows `stride` bytes apart
+ * (a [n, K, H, W] tensor, or [K, H, W] for a single frame: stride = bpp W, plane_stride = bpp W H,
+ * bpp = 4 or 1). Only each plane's width x height pixels are written, and for a single frame only
+ * the crop's tile rectangle; row padding and the bytes between planes stay as they were. For a
+ * batch, frame c's planes are comps[c]'s own orders; every view uses the same orders.
+ * With a non-null device_buffer the call also writes the sRGB8 RGBA frame or stack from the same
+ * pass (one upload, line setup, sort and set of painter tables): exactly the bytes of
+ * forma_renderer_render_device (without a layer cache), forma_renderer_render_views_device or
+ * forma_renderer_render_batch_device with the same arguments. With a null device_buffer,
+ * width_stride, view_stride / frame_stride, channels and clear_color are not read.
+ * Refusals return FORMA_ERR_INVALID_ARGUMENT before anything is written to either buffer: a null
+ * descriptor or pointer; K = 0 or first_order + K > 2^21; an unknown format; stride < bpp width;
+ * plane_stride < (height - 1) stride + bpp width; F32 pointers or strides that are not multiples of
+ * 4; a plane stack whose size overflows 64 bits; and everything the RGBA calls refuse for the
+ * target, views and batches. Their order-sum, stop / texel and 2^30-segment limits apply as well.
+ * A mask call takes no layer cache and leaves every cache as it was. Afterwards counters,
+ * segments, stage times and row costs describe the call's frame; stage time [5] covers the paint
+ * kernel and the mask kernels (a zero fill of the planes' written rectangles, then the masks).
+ * render_masks paints into device scratch and copies the planes' rectangles into a HOST buffer;
+ * the _device calls write device memory on the renderer's device. */
+enum { FORMA_MASK_F32 = 0, FORMA_MASK_U8 = 1 };
+typedef struct forma_masks {
+    void* ptr;
+    uint32_t first_order, n_orders, format;
+    uint64_t stride, plane_stride; /* bytes */
+} forma_masks;
+int forma_renderer_render_masks(forma_renderer*, forma_composition*, const forma_masks* masks, uint64_t width, uint64_t height,
+                                const forma_rect* crop /* nullable */, forma_timings* timings /* nullable */);
+int forma_renderer_render_masks_device(forma_renderer*, forma_composition*, const forma_masks* masks, uint64_t width,
+                                       uint64_t height, const forma_rect* crop /* nullable */,
+                                       uint8_t* device_buffer /* nullable */, uint64_t width_stride, const uint32_t channels[4],
+                                       const float clear_color[4], forma_timings* timings /* nullable */);
+int forma_renderer_render_views_masks_device(forma_renderer*, forma_composition*, const float* views, uint32_t n,
+                                             const forma_masks* masks, uint64_t width, uint64_t height,
+                                             uint8_t* device_buffer /* nullable */, uint64_t width_stride, uint64_t view_stride,
+                                             const uint32_t channels[4], const float clear_color[4],
+                                             forma_timings* timings /* nullable */);
+int forma_renderer_render_batch_masks_device(forma_renderer*, forma_composition* const* comps, uint32_t n,
+                                             const forma_masks* masks, uint64_t width, uint64_t height,
+                                             uint8_t* device_buffer /* nullable */, uint64_t width_stride, uint64_t frame_stride,
+                                             const uint32_t channels[4], const float clear_color[4],
+                                             forma_timings* timings /* nullable */);
+
 /* Launch on `cuda_stream` (a cudaStream_t, e.g. torch.cuda.current_stream().cuda_stream)
  * instead of the default stream. */
 void forma_renderer_set_stream(forma_renderer*, void* cuda_stream);
