@@ -212,6 +212,24 @@ class _CMasks(C.Structure):  # forma_masks
                 ("stride", C.c_uint64), ("plane_stride", C.c_uint64)]
 
 
+class _CStats(C.Structure):  # forma_stats
+    _fields_ = [("ptr", C.c_void_p), ("first_order", C.c_uint32), ("n_orders", C.c_uint32), ("min_coverage", C.c_float)]
+
+
+# forma_layer_stats, one 48-byte record per frame and order (see include/forma_b200.h).
+STATS_DTYPE = np.dtype([("area", np.uint64), ("pixels", np.uint32), ("visible", np.uint32), ("box", np.uint32, (4,)),
+                        ("visible_box", np.uint32, (4,))])
+
+
+def split_stats(t):
+    """The fields of device records, a [..., 12] int32 tensor (or array) of forma_layer_stats: a dict
+    of `area` (int64), `pixels`, `visible` ([...], int64) and `box`, `visible_box` ([..., 4], int64),
+    the unsigned values of the records."""
+    w = (t.astype(np.int64) if isinstance(t, np.ndarray) else t.long()) & 0xFFFFFFFF  # the words as unsigned 32-bit values
+    return {"area": w[..., 0] | (w[..., 1] << 32), "pixels": w[..., 2], "visible": w[..., 3], "box": w[..., 4:8],
+            "visible_box": w[..., 8:12]}
+
+
 class _CTimings(C.Structure):
     _fields_ = [
         ("line_setup_ms", C.c_double), ("rasterize_ms", C.c_double), ("sort_ms", C.c_double),
@@ -332,6 +350,13 @@ SIGNATURES = {
                                                      C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
     "renderer_render_batch_masks_device": (C.c_int, [_vp, C.POINTER(_vp), C.c_uint32, C.POINTER(_CMasks), C.c_uint64, C.c_uint64,
                                                      _vp, C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
+    "renderer_render_stats": (C.c_int, [_vp, _vp, C.POINTER(_CStats), C.c_uint64, C.c_uint64, C.POINTER(_CRect), C.POINTER(_CTimings)]),
+    "renderer_render_stats_device": (C.c_int, [_vp, _vp, C.POINTER(_CStats), C.c_uint64, C.c_uint64, C.POINTER(_CRect), _vp,
+                                               C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
+    "renderer_render_views_stats_device": (C.c_int, [_vp, _vp, _fp, C.c_uint32, C.POINTER(_CStats), C.c_uint64, C.c_uint64, _vp,
+                                                     C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
+    "renderer_render_batch_stats_device": (C.c_int, [_vp, C.POINTER(_vp), C.c_uint32, C.POINTER(_CStats), C.c_uint64, C.c_uint64,
+                                                     _vp, C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
     "renderer_launch_count": (C.c_uint64, [_vp]),
     "renderer_stage_times": (None, [_vp, C.POINTER(C.c_double)]),
     "renderer_counters": (None, [_vp, _u64p]),
@@ -392,6 +417,10 @@ OVER_SYMBOLS = ("renderer_render_over_device", "renderer_render_views_over_devic
 # render_batch_masks_device).
 MASK_SYMBOLS = ("renderer_render_masks", "renderer_render_masks_device", "renderer_render_views_masks_device",
                 "renderer_render_batch_masks_device")
+# The same for layer statistics (Renderer.render_stats, render_stats_device, render_views_stats_device,
+# render_batch_stats_device).
+STATS_SYMBOLS = ("renderer_render_stats", "renderer_render_stats_device", "renderer_render_views_stats_device",
+                 "renderer_render_batch_stats_device")
 # Value formats of mask planes: name -> (FORMA_MASK_*, bytes per value, numpy dtype).
 MASK_FORMATS = {"f32": (0, 4, np.float32), "u8": (1, 1, np.uint8)}
 
@@ -424,7 +453,7 @@ def over_format(fmt: str):
 
 
 _OPTIONAL_SYMBOLS = frozenset(ID_FRAME_SYMBOLS + VIEW_SYMBOLS + BATCH_SYMBOLS + STACK_ID_SYMBOLS + SORT_DEBUG_SYMBOLS +
-                              LINEAR_SYMBOLS + OVER_SYMBOLS + MASK_SYMBOLS)
+                              LINEAR_SYMBOLS + OVER_SYMBOLS + MASK_SYMBOLS + STATS_SYMBOLS)
 
 
 class Api:
@@ -1263,6 +1292,82 @@ class Renderer:
         return self._stack_masks(self._api.renderer_render_batch_masks_device, "Renderer::render_batch_masks_device", args, n, masks_ptr, width,
                                  height, first_order, n_orders, format, stride, plane_stride, rgba_ptr, channels, clear_color,
                                  rgba_stride, frame_stride, timings)
+
+    def render_stats(self, composition: Composition, width: int, height: int, first_order: int, n_orders: int,
+                     min_coverage: float = 0.0, crop: Optional[Rect] = None, out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Layer statistics into a host array (see include/forma_b200.h: forma_renderer_render_stats):
+        per order o of [first_order, first_order + n_orders) its amodal area (sum of mask values x 2^18),
+        the pixels its mask exceeds min_coverage on and their box, and the pixels its ID owns and
+        their box. Returns the [n_orders] STATS_DTYPE array (`out`, if given)."""
+        if out is None:
+            out = np.zeros(n_orders, STATS_DTYPE)
+        assert out.dtype == STATS_DTYPE and out.flags["C_CONTIGUOUS"] and out.size >= n_orders
+        s = _CStats(out.ctypes.data, first_order, n_orders, min_coverage)
+        _, _, rect = self._common(RGBA, Color(), crop)
+        st = self._api.renderer_render_stats(self._h, composition._h, C.byref(s), width, height,
+                                             C.byref(rect) if rect is not None else None, None)
+        self._api.check(st, "Renderer::render_stats")
+        return out
+
+    def render_stats_device(self, composition: Composition, stats_ptr: int, width: int, height: int, first_order: int,
+                            n_orders: int, min_coverage: float = 0.0, crop: Optional[Rect] = None, rgba_ptr: Optional[int] = None,
+                            channels=RGBA, clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), rgba_stride: Optional[int] = None,
+                            timings: bool = True) -> Optional[Timings]:
+        """render_stats into device memory: the data_ptr() of a contiguous [n_orders, 12] int32 CUDA
+        tensor (split_stats reads its fields). With `rgba_ptr` the frame of render_device (no layer
+        cache; default stride 4 * width) is written as well, from the same pass."""
+        s = _CStats(int(stats_ptr), first_order, n_orders, min_coverage)
+        ch, cc, rect = self._common(channels, clear_color, crop)
+        t = _CTimings() if timings else None
+        st = self._api.renderer_render_stats_device(self._h, composition._h, C.byref(s), width, height,
+                                                    C.byref(rect) if rect is not None else None,
+                                                    None if rgba_ptr is None else C.c_void_p(int(rgba_ptr)),
+                                                    4 * width if rgba_stride is None else rgba_stride, ch, cc,
+                                                    C.byref(t) if t is not None else None)
+        self._api.check(st, "Renderer::render_stats_device")
+        return _timings(t)
+
+    def _stack_stats(self, fn, what, first_args, n, stats_ptr, width, height, first_order, n_orders, min_coverage, rgba_ptr, channels,
+                     clear_color, rgba_stride, frame_stride, timings):
+        """Calls `fn`, the statistics entry point of views or batches, on chunks of at most
+        max_views(height) frames (see _stack)."""
+        rgba_stride, frame_stride = self._strides(width, height, rgba_stride, frame_stride)
+        ch, cc, _ = self._common(channels, clear_color, None)
+        chunk = max(self.max_views(height), 1)
+        t = None
+        for first in range(0, max(n, 1), chunk):
+            s = _CStats(int(stats_ptr) + first * n_orders * STATS_DTYPE.itemsize, first_order, n_orders, min_coverage)
+            rgba = None if rgba_ptr is None else C.c_void_p(int(rgba_ptr) + first * frame_stride)
+            t = _CTimings() if timings else None
+            st = fn(self._h, *first_args(first, min(chunk, n - first)), C.byref(s), width, height, rgba, rgba_stride, frame_stride, ch, cc,
+                    C.byref(t) if t is not None else None)
+            self._api.check(st, what)
+        return _timings(t)
+
+    def render_views_stats_device(self, composition: Composition, views, stats_ptr: int, width: int, height: int, first_order: int,
+                                  n_orders: int, min_coverage: float = 0.0, rgba_ptr: Optional[int] = None, channels=RGBA,
+                                  clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), rgba_stride: Optional[int] = None,
+                                  view_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """The statistics (see render_stats) of every view of render_views_device, in one pass: the
+        data_ptr() of a contiguous [N, n_orders, 12] int32 CUDA tensor; every view reports the same
+        orders. With `rgba_ptr` the frames of render_views_device are written as well. Chunked like
+        render_views."""
+        n, args = self._view_args(composition, views)
+        return self._stack_stats(self._api.renderer_render_views_stats_device, "Renderer::render_views_stats_device", args, n, stats_ptr,
+                                 width, height, first_order, n_orders, min_coverage, rgba_ptr, channels, clear_color, rgba_stride,
+                                 view_stride, timings)
+
+    def render_batch_stats_device(self, comps, stats_ptr: int, width: int, height: int, first_order: int, n_orders: int,
+                                  min_coverage: float = 0.0, rgba_ptr: Optional[int] = None, channels=RGBA,
+                                  clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), rgba_stride: Optional[int] = None,
+                                  frame_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """The statistics (see render_stats) of every frame of render_batch_device, in one pass: frame
+        c's records are comps[c]'s own orders [first_order, first_order + n_orders). Layout as for
+        render_views_stats_device; chunked like render_batch."""
+        n, args = self._batch_args(comps)
+        return self._stack_stats(self._api.renderer_render_batch_stats_device, "Renderer::render_batch_stats_device", args, n, stats_ptr,
+                                 width, height, first_order, n_orders, min_coverage, rgba_ptr, channels, clear_color, rgba_stride,
+                                 frame_stride, timings)
 
     def launch_count(self) -> int:
         return int(self._api.renderer_launch_count(self._h))

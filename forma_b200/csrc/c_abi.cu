@@ -540,6 +540,46 @@ int forma_renderer_render_batch_masks_device(forma_renderer* r, forma_compositio
     FrameRequest q{FrameKind::batch, n, width, height, channels, clear_color, timings};
     return render_masks(r, q, masks, true, device_buffer, width_stride, frame_stride, nullptr, comps, __func__);
 }
+// Layer statistics: the statistics target from the descriptor (a null descriptor or pointer is
+// refused here, the rest by Renderer::check_request), with or without the RGBA target.
+static int render_stats(forma_renderer* r, FrameRequest q, const forma_stats* stats, bool on_device, uint8_t* device_buffer,
+                        uint64_t width_stride, uint64_t frame_stride, forma_composition* c, forma_composition* const* comps,
+                        const char* fn) {
+    if (!stats || !stats->ptr) {
+        set_error("%s: no %s", fn, stats ? "record array" : "statistics descriptor");
+        return FORMA_STATUS_INVALID;
+    }
+    q.stats = StatsTarget{stats->ptr, on_device, stats->first_order, stats->n_orders, stats->min_coverage};
+    if (device_buffer) q.rgba = {device_buffer, true, width_stride, frame_stride};
+    else q.channels = nullptr, q.clear = nullptr;
+    return render_request(r, q, c, comps);
+}
+int forma_renderer_render_stats(forma_renderer* r, forma_composition* c, const forma_stats* stats, uint64_t width, uint64_t height,
+                                const forma_rect* crop, forma_timings* timings) {
+    FrameRequest q{FrameKind::single, 0, width, height, nullptr, nullptr, timings, crop};
+    return render_stats(r, q, stats, false, nullptr, 0, 0, c, nullptr, __func__);
+}
+int forma_renderer_render_stats_device(forma_renderer* r, forma_composition* c, const forma_stats* stats, uint64_t width,
+                                       uint64_t height, const forma_rect* crop, uint8_t* device_buffer, uint64_t width_stride,
+                                       const uint32_t channels[4], const float clear_color[4], forma_timings* timings) {
+    FrameRequest q{FrameKind::single, 0, width, height, channels, clear_color, timings, crop};
+    return render_stats(r, q, stats, true, device_buffer, width_stride, 0, c, nullptr, __func__);
+}
+int forma_renderer_render_views_stats_device(forma_renderer* r, forma_composition* c, const float* views, uint32_t n,
+                                             const forma_stats* stats, uint64_t width, uint64_t height, uint8_t* device_buffer,
+                                             uint64_t width_stride, uint64_t view_stride, const uint32_t channels[4],
+                                             const float clear_color[4], forma_timings* timings) {
+    FrameRequest q{FrameKind::views, n, width, height, channels, clear_color, timings};
+    q.views = views;
+    return render_stats(r, q, stats, true, device_buffer, width_stride, view_stride, c, nullptr, __func__);
+}
+int forma_renderer_render_batch_stats_device(forma_renderer* r, forma_composition* const* comps, uint32_t n,
+                                             const forma_stats* stats, uint64_t width, uint64_t height, uint8_t* device_buffer,
+                                             uint64_t width_stride, uint64_t frame_stride, const uint32_t channels[4],
+                                             const float clear_color[4], forma_timings* timings) {
+    FrameRequest q{FrameKind::batch, n, width, height, channels, clear_color, timings};
+    return render_stats(r, q, stats, true, device_buffer, width_stride, frame_stride, nullptr, comps, __func__);
+}
 // Linear float frames: the RGBA target with 8- or 16-byte pixels (a null buffer is refused by
 // Renderer::check_request like any missing target).
 static int render_linear(forma_renderer* r, FrameRequest q, uint32_t format, forma_composition* c, forma_composition* const* comps) {

@@ -7,6 +7,8 @@
 
 #include "device_types.h"
 
+struct forma_layer_stats;  // include/forma_b200.h
+
 namespace forma {
 
 // Schedule switches (none of them changes results). Initialised from the environment
@@ -379,6 +381,21 @@ struct MaskFrame {
 // frames != nullptr: a batch, whose entries carry frames[c].order_base + order. Returns the launches.
 uint32_t launch_paint_masks(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range,
                             const uint32_t* heavy, const uint32_t* heavy_count, uint8_t* id_flags, const MaskFrame& m,
+                            uint32_t* tile_counter, cudaStream_t st, uint32_t rows = 0, const BatchFrame* frames = nullptr);
+// Layer statistics (kernels_ids.cu, see forma_renderer_render_stats): n_orders records of order
+// first_order + k per frame of n_frames, frame b's at ptr + b * n_orders.
+struct StatsFrame {
+    forma_layer_stats* ptr;
+    uint32_t first_order, n_orders;
+    float min_coverage;
+    uint32_t height;    // rows of one frame
+    uint32_t n_frames;  // 1 for a single frame
+};
+// Initialises the records, reduces the amodal walk (the mask kernel's) and the visible walk (the
+// ID kernel's) into them, then writes the empty sets' boxes: the whole of the records, so that the
+// sync-free redo can repeat it. rows / frames as for launch_paint_masks. Returns the launches.
+uint32_t launch_paint_stats(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range,
+                            const uint32_t* heavy, const uint32_t* heavy_count, uint8_t* id_flags, const StatsFrame& f,
                             uint32_t* tile_counter, cudaStream_t st, uint32_t rows = 0, const BatchFrame* frames = nullptr);
 // The painter tables of a batch: the device tables of its distinct compositions, concatenated.
 // Composition k's orders land at order_base + order (the slots they name shifted by style_base,

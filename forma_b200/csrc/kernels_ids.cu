@@ -270,9 +270,128 @@ __device__ __forceinline__ void store_mask(uint8_t* p, const float cov[8], uint3
     }
 }
 
-template <bool kBatch>
+// ---------------------------------------------------------------------------
+// Layer statistics (forma_renderer_render_stats): per frame and window order one
+// forma_layer_stats record, reduced from the walks of the mask kernel (amodal: area, pixels, box)
+// and of the ID kernel (visible, visible_box) instead of stored planes. Each (tile, entry) of the
+// amodal walk and each distinct window ID of a tile in the visible walk is one warp reduction and
+// one set of integer atomics on its record, so the result is exact and does not depend on the
+// order of the atomics. Boxes start as {~0, ~0, 0, 0} (min / max sentinels) and
+// fix_stats_kernel turns the box of an empty set into {0, 0, 0, 0} at the end.
+// ---------------------------------------------------------------------------
+struct StatsOut {
+    forma_layer_stats* rec;  // n_frames x n_orders records
+    uint32_t first_order, n_orders;
+    uint32_t height;  // rows of one frame
+    uint32_t rows;    // stacks: tile rows per frame; 0: a single frame
+    float min_cov;
+};
+
+// Widens `box` (x0, y0, x1, y1) to hold [x0, x1) x [y0, y1). Bounds only move outwards, so a
+// relaxed read that finds one already as wide skips its atomic (a stale read only costs an atomic).
+__device__ __forceinline__ void widen_box(uint32_t* box, uint32_t x0, uint32_t y0, uint32_t x1, uint32_t y1) {
+    const uint2 lo = __ldcg(reinterpret_cast<const uint2*>(box)), hi = __ldcg(reinterpret_cast<const uint2*>(box + 2));
+    if (x0 < lo.x) atomicMin(box, x0);
+    if (y0 < lo.y) atomicMin(box + 1, y0);
+    if (x1 > hi.x) atomicMax(box + 2, x1);
+    if (y1 > hi.y) atomicMax(box + 3, y1);
+}
+
+// The amodal statistics of one (tile, entry): the lane's eight values cov (n_px of them in the
+// frame, from column x0 of frame row py) into `r`. `full`: a kFlagFull entry that no clip mask
+// scales, 1 on the tile's whole in-frame rectangle [tx0, tx0 + tw) x [ty0, ty0 + th), taken without
+// a reduction. Called by the whole warp.
+__device__ __forceinline__ void add_amodal(forma_layer_stats* r, const float cov[8], bool full, uint32_t n_px, uint32_t x0,
+                                           uint32_t py, uint32_t tx0, uint32_t tw, uint32_t ty0, uint32_t th, float min_cov,
+                                           uint32_t lane) {
+    if (full) {
+        if (lane == 0 && tw && th) {
+            atomicAdd(reinterpret_cast<unsigned long long*>(&r->area), (unsigned long long)(tw * th) << 18);
+            atomicAdd(&r->pixels, tw * th);
+            widen_box(r->box, tx0, ty0, tx0 + tw, ty0 + th);
+        }
+        return;
+    }
+    uint32_t units = 0, cnt = 0, xl = ~0u, xh = 0;
+#pragma unroll
+    for (uint32_t j = 0; j < 8u; ++j) {
+        if (j >= n_px) continue;
+        units += (uint32_t)(cov[j] * 262144.0f);  // exact: v x 2^18 is an integer <= 2^18
+        if (cov[j] > min_cov) {
+            ++cnt;
+            xl = min(xl, x0 + j);
+            xh = x0 + j + 1u;
+        }
+    }
+    units = __reduce_add_sync(kFullMask, units);  // <= 256 x 2^18
+    const uint32_t n = __reduce_add_sync(kFullMask, cnt);
+    if (n) {
+        xl = __reduce_min_sync(kFullMask, xl);
+        xh = __reduce_max_sync(kFullMask, xh);
+    }
+    const uint32_t yl = n ? __reduce_min_sync(kFullMask, cnt ? py : ~0u) : 0u;
+    const uint32_t yh = n ? __reduce_max_sync(kFullMask, cnt ? py + 1u : 0u) : 0u;
+    if (lane == 0) {
+        if (units) atomicAdd(reinterpret_cast<unsigned long long*>(&r->area), (unsigned long long)units);
+        if (n) {
+            atomicAdd(&r->pixels, n);
+            widen_box(r->box, xl, yl, xh, yh);
+        }
+    }
+}
+
+// The visible statistics of one tile (tile row ty, column tx) from the ID walk's eight IDs `out` of
+// each lane (tile row `row`, half hx): one reduction per distinct window ID of the tile. `frames`: a batch, whose IDs carry
+// the frame's order base. Called by the whole warp.
+__device__ __forceinline__ void add_visible(const PaintScene& S, const StatsOut& so, const uint32_t* out, uint32_t ty, uint32_t tx,
+                                            uint32_t row, uint32_t hx, uint32_t lane, const BatchFrame* __restrict__ frames) {
+    const uint32_t frame = so.rows ? ty / so.rows : 0u, fty = so.rows ? ty - frame * so.rows : ty;
+    const uint32_t lo_w = (frames ? frames[frame].order_base : 0u) + so.first_order;
+    const uint32_t py = fty * 16u + row, x0 = tx * 16u + hx * 8u;
+    const uint32_t n_px = py < so.height && x0 < S.width ? min(8u, S.width - x0) : 0u;
+    uint32_t k[8], pend = 0;  // window indices; the lane's pixels not reduced yet
+#pragma unroll
+    for (uint32_t j = 0; j < 8u; ++j) {
+        k[j] = out[j] - lo_w;  // (FORMA_ID_NONE and orders outside the window land at >= n_orders)
+        if (j < n_px && k[j] < so.n_orders) pend |= 1u << j;
+    }
+    forma_layer_stats* rec = so.rec + (size_t)frame * so.n_orders;
+    for (;;) {
+        const uint32_t any = __ballot_sync(kFullMask, pend != 0u);
+        if (!any) break;
+        uint32_t mine = 0, seen = 0;
+#pragma unroll
+        for (uint32_t j = 0; j < 8u; ++j)
+            if (((pend >> j) & 1u) && !seen) {
+                mine = k[j];
+                seen = 1;
+            }
+        const uint32_t id = __shfl_sync(kFullMask, mine, __ffs(any) - 1);
+        uint32_t cnt = 0, xl = ~0u, xh = 0;
+#pragma unroll
+        for (uint32_t j = 0; j < 8u; ++j)
+            if (((pend >> j) & 1u) && k[j] == id) {
+                ++cnt;
+                xl = min(xl, x0 + j);
+                xh = x0 + j + 1u;
+                pend &= ~(1u << j);
+            }
+        const uint32_t n = __reduce_add_sync(kFullMask, cnt);
+        xl = __reduce_min_sync(kFullMask, xl);
+        xh = __reduce_max_sync(kFullMask, xh);
+        const uint32_t yl = __reduce_min_sync(kFullMask, cnt ? py : ~0u), yh = __reduce_max_sync(kFullMask, cnt ? py + 1u : 0u);
+        if (lane == 0) {
+            atomicAdd(&rec[id].visible, n);
+            widen_box(rec[id].visible_box, xl, yl, xh, yh);
+        }
+    }
+}
+
+// kStats: the amodal statistics (add_amodal into so) in place of the planes; `in` then only
+// gives the tables and the window.
+template <bool kBatch, bool kStats = false>
 __device__ __forceinline__ void paint_masks_body(const PaintScene& S, const MaskInputs& in, uint32_t n_tiles,
-                                                 const BatchFrame* __restrict__ frames) {
+                                                 const BatchFrame* __restrict__ frames, const StatsOut& so = StatsOut{}) {
     __shared__ __align__(16) IdWarpSmem s_warp[kIdWarpsPerBlock];
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
     IdWarpSmem& W = s_warp[warp];
@@ -328,10 +447,19 @@ __device__ __forceinline__ void paint_masks_body(const PaintScene& S, const Mask
         const uint32_t n_px = inside ? min(8u, S.width - x0) : 0u;
         uint8_t* const px = in.out + ((size_t)frame * in.n_orders) * in.plane_stride + (size_t)py * in.stride + (size_t)x0 * bpp;
         float cov[8];
+        bool full = false;  // cov is a kFlagFull entry's 1 everywhere (kStats)
         auto put = [&](uint32_t layer) {
-            if (inside) store_mask(px + (size_t)(layer - lo_w) * in.plane_stride, cov, n_px, in.u8, vec_ok);
+            if constexpr (kStats) {
+                const uint32_t tx0 = tx * 16u, ty0 = fty * 16u;
+                const uint32_t tw = tx0 < S.width ? min(16u, S.width - tx0) : 0u, th = ty0 < in.height ? min(16u, in.height - ty0) : 0u;
+                add_amodal(so.rec + (size_t)frame * in.n_orders + (layer - lo_w), cov, full, n_px, x0, py, tx0, tw, ty0, th,
+                           so.min_cov, lane);
+            } else if (inside) {
+                store_mask(px + (size_t)(layer - lo_w) * in.plane_stride, cov, n_px, in.u8, vec_ok);
+            }
         };
         auto coverage = [&](const EntryRec& h) {
+            full = (h.pad & kFlagFull) != 0u;
             if (h.pad & kFlagFull) {  // no segments, a full carried cover: coverage 1 without reading anything
 #pragma unroll
                 for (int j = 0; j < 8; ++j) cov[j] = 1.0f;
@@ -421,6 +549,7 @@ __device__ __forceinline__ void paint_masks_body(const PaintScene& S, const Mask
                         const float m[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
 #pragma unroll
                         for (int j = 0; j < 8; ++j) cov[j] = __fmul_rn(cov[j], m[j]);
+                        full = false;
                     }
                     put(layer);
                 }
@@ -485,6 +614,89 @@ uint32_t launch_paint_masks(const PaintScene& S, const uint64_t* segs, const Ent
         paint_masks_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles);
     }
     return 2;
+}
+
+// The statistics kernels (see add_amodal / add_visible above): the amodal walk of the mask kernel
+// and the visible walk of the ID kernel, each single-frame / views and batch.
+__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_amodal_kernel(PaintScene S, MaskInputs in, uint32_t n_tiles,
+                                                                             StatsOut so) {
+    paint_masks_body<false, true>(S, in, n_tiles, nullptr, so);
+}
+__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_amodal_stacked_kernel(PaintScene S, MaskInputs in, uint32_t n_tiles,
+                                                                                     StatsOut so,
+                                                                                     const BatchFrame* __restrict__ frames) {
+    paint_masks_body<true, true>(S, in, n_tiles, frames, so);
+}
+__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_visible_kernel(PaintScene S, IdInputs in, uint32_t n_tiles,
+                                                                              StatsOut so) {
+#define FORMA_IDS_SINK(out, ty, tx, row, hx) add_visible(S, so, out, ty, tx, row, hx, lane, nullptr)
+#include "paint_ids_body.cuh"
+#undef FORMA_IDS_SINK
+}
+__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_visible_stacked_kernel(PaintScene S, IdInputs in, uint32_t n_tiles,
+                                                                                      StatsOut so,
+                                                                                      const BatchFrame* __restrict__ frames) {
+#define FORMA_IDS_SINK(out, ty, tx, row, hx) add_visible(S, so, out, ty, tx, row, hx, lane, frames)
+#include "paint_ids_body.cuh"
+#undef FORMA_IDS_SINK
+}
+
+// Every record to 0 with the boxes' min / max sentinels {~0, ~0, 0, 0}.
+__global__ void init_stats_kernel(forma_layer_stats* rec, uint64_t n) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        uint2* r = reinterpret_cast<uint2*>(rec + i);  // 8-byte aligned (check_stats)
+        r[0] = make_uint2(0u, 0u);             // area
+        r[1] = make_uint2(0u, 0u);             // pixels, visible
+        r[2] = make_uint2(~0u, ~0u);           // box x0, y0
+        r[3] = make_uint2(0u, 0u);             // box x1, y1
+        r[4] = make_uint2(~0u, ~0u);           // visible_box x0, y0
+        r[5] = make_uint2(0u, 0u);             // visible_box x1, y1
+    }
+}
+// The box of an empty set to {0, 0, 0, 0}.
+__global__ void fix_stats_kernel(forma_layer_stats* rec, uint64_t n) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        forma_layer_stats& r = rec[i];
+        if (r.pixels == 0u) r.box[0] = r.box[1] = 0u;
+        if (r.visible == 0u) r.visible_box[0] = r.visible_box[1] = 0u;
+    }
+}
+
+uint32_t launch_paint_stats(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range,
+                            const uint32_t* heavy, const uint32_t* heavy_count, uint8_t* id_flags, const StatsFrame& f,
+                            uint32_t* tile_counter, cudaStream_t st, uint32_t rows, const BatchFrame* frames) {
+    const uint64_t n_rec = (uint64_t)f.n_frames * f.n_orders;
+    const uint32_t rec_ctas = (uint32_t)std::min<uint64_t>((n_rec + 255u) / 256u, 8u * (uint64_t)device_sm_count());
+    init_stats_kernel<<<rec_ctas, 256, 0, st>>>(f.ptr, n_rec);
+    uint32_t launches = 2;
+    if (S.tx_hi > S.tx_lo && S.ty_hi > S.ty_lo) {
+        const uint32_t n_tiles = (S.tx_hi - S.tx_lo) * (S.ty_hi - S.ty_lo);
+        const IdInputs t{segs, recs, tile_range, heavy, heavy_count, S.tiles_x * S.tiles_y, id_flags, nullptr, 0, f.min_coverage,
+                         tile_counter};
+        const MaskInputs in{t, nullptr, 0, 0, f.first_order, f.n_orders, f.height, rows, false};
+        const StatsOut so{f.ptr, f.first_order, f.n_orders, f.height, rows, f.min_coverage};
+        static int blocks_per_sm[4][kMaxDevices] = {{0}};
+        const uint32_t need = (n_tiles + kIdWarpsPerBlock - 1) / kIdWarpsPerBlock;
+        cudaMemsetAsync(tile_counter, 0, sizeof(uint32_t), st);
+        if (frames) {
+            const uint32_t want = id_grid_limit(stats_amodal_stacked_kernel, blocks_per_sm[1]);
+            stats_amodal_stacked_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles, so, frames);
+        } else {
+            const uint32_t want = id_grid_limit(stats_amodal_kernel, blocks_per_sm[0]);
+            stats_amodal_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles, so);
+        }
+        cudaMemsetAsync(tile_counter, 0, sizeof(uint32_t), st);
+        if (frames) {
+            const uint32_t want = id_grid_limit(stats_visible_stacked_kernel, blocks_per_sm[3]);
+            stats_visible_stacked_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, t, n_tiles, so, frames);
+        } else {
+            const uint32_t want = id_grid_limit(stats_visible_kernel, blocks_per_sm[2]);
+            stats_visible_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, t, n_tiles, so);
+        }
+        launches += 2;
+    }
+    fix_stats_kernel<<<rec_ctas, 256, 0, st>>>(f.ptr, n_rec);
+    return launches;
 }
 
 }  // namespace forma

@@ -2,7 +2,8 @@
 // that each kernel is compiled from the same text as a function of its own. Expects S, in and
 // n_tiles, and FORMA_IDS_REBASE(out, ty): what happens to the lane's eight IDs of a tile of row ty
 // before they are stored (nothing for a single frame or views; a batch takes the frame's order
-// base off them).
+// base off them). A kernel that defines FORMA_IDS_SINK(out, ty, tx, row, hx) hands the lane's eight
+// IDs of every tile to it instead of storing them (FORMA_IDS_REBASE is then not used).
     __shared__ __align__(16) IdWarpSmem s_warp[kIdWarpsPerBlock];
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
     IdWarpSmem& W = s_warp[warp];
@@ -157,6 +158,10 @@
             }
         }
 
+#ifdef FORMA_IDS_SINK
+        (void)vec_ok;
+        FORMA_IDS_SINK(out, ty, tx, row, hx);
+#else
         FORMA_IDS_REBASE(out, ty);
         const uint32_t py = ty * 16u + row, x0 = tx * 16u + hx * 8u;
         if (py < S.height && x0 < S.width) {
@@ -170,4 +175,5 @@
                     if (x0 + (uint32_t)j < S.width) rowp[j] = out[j];
             }
         }
+#endif
     }

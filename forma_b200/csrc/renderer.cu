@@ -565,13 +565,16 @@ int Renderer::render(const FrameRequest& q) {
         p.masks.stride = (q.masks.bpp() * q.width + 15u) / 16u * 16u;
         p.mask_plane_stride = p.masks.stride * q.height;
     }
-    // The PaintScene of the RGBA target, or of the ID target or the masks when they are alone.
+    p.stats = q.stats.ptr;
+    // The PaintScene of the RGBA target, or of the ID target, the masks or the statistics when they
+    // are alone (statistics have no frame: the stride is that of an sRGB8 frame's rows).
     // An over frame has no clear colour: its kernels read each pixel's, and upgrade Alpha -> One per
     // pixel, so the scene's channels stay as given.
     static const uint32_t kIdChannels[4] = {0, 1, 2, 3};
     static const float kIdClear[4] = {0, 0, 0, 0};
     PaintScene S{};
-    st = begin_frame(S, q.width, rgba ? p.rgba.stride : q.ids.ptr ? p.ids.stride : p.masks.stride, stack ? (uint64_t)q.n * p.rows * 16u : q.height,
+    st = begin_frame(S, q.width, rgba ? p.rgba.stride : q.ids.ptr ? p.ids.stride : q.masks.ptr ? p.masks.stride : 4u * q.width,
+                     stack ? (uint64_t)q.n * p.rows * 16u : q.height,
                      rgba ? q.channels : kIdChannels, rgba && !q.rgba.over ? q.clear : kIdClear, q.crop);
     if (st) return st;
     if (rgba && !p.rgba.direct) {
@@ -585,6 +588,10 @@ int Renderer::render(const FrameRequest& q) {
     if (q.masks.ptr && !p.masks.direct) {
         FORMA_CUDA_TRY(mask_frame.reserve((size_t)p.mask_plane_stride * q.masks.n_orders));
         p.masks.ptr = mask_frame.ptr;
+    }
+    if (q.stats.ptr && !q.stats.on_device) {
+        FORMA_CUDA_TRY(stats_scratch.reserve((size_t)q.stats.n_orders));
+        p.stats = stats_scratch.ptr;
     }
     // (A host float frame is painted whole and copied back once.)
     p.in_bands = rgba && q.rgba.bpp == 4u && !stack && !q.rgba.on_device && !q.cache && S.ty_hi - S.ty_lo >= (copy_bands_override ? 8u : 32u) &&
@@ -630,7 +637,7 @@ int Renderer::check_request(const FrameRequest& q) {
         }
         return (int)FORMA_STATUS_OK;
     };
-    int st = q.rgba.ptr || (!q.ids.ptr && !q.masks.ptr) ? check_target(q.rgba) : FORMA_STATUS_OK;
+    int st = q.rgba.ptr || (!q.ids.ptr && !q.masks.ptr && !q.stats.ptr) ? check_target(q.rgba) : FORMA_STATUS_OK;
     if (st) return st;
     if (q.rgba.bpp != 4u && (((uintptr_t)q.rgba.ptr | q.rgba.stride | q.rgba.frame_stride) & 3u) != 0u) {
         set_error("invalid float frame: buffer, stride %llu and %s stride %llu must be multiples of 4 bytes",
@@ -669,6 +676,10 @@ int Renderer::check_request(const FrameRequest& q) {
     }
     if (q.masks.ptr) {
         st = check_masks(q);
+        if (st) return st;
+    }
+    if (q.stats.ptr) {
+        st = check_stats(q);
         if (st) return st;
     }
     if ((q.kind == FrameKind::views && !q.views) || (q.kind == FrameKind::batch && !q.batch)) {
@@ -739,6 +750,40 @@ int Renderer::check_masks(const FrameRequest& q) {
         __builtin_add_overflow(span, (height - 1u) * m.stride + bpp * width, &end)) {
         set_error("the masks' planes overflow 64 bits: %llu planes of stride %llu", (unsigned long long)planes,
                   (unsigned long long)m.plane_stride);
+        return FORMA_STATUS_INVALID;
+    }
+    if (q.kind != FrameKind::single && (q.n == 0 || q.n > max_views(height))) {
+        set_error("%u %ss of height %llu: between 1 and %u fit in one call", q.n, q.kind == FrameKind::views ? "view" : "frame",
+                  (unsigned long long)height, max_views(height));
+        return FORMA_STATUS_INVALID;
+    }
+    return FORMA_STATUS_OK;
+}
+
+// The statistics target's own checks (see forma_renderer_render_stats), then those of any target
+// for its size and the frame count: statistics go alone or with an sRGB8 RGBA target that is
+// neither painted over its pixels nor cached, never with IDs or masks.
+int Renderer::check_stats(const FrameRequest& q) {
+    const StatsTarget& t = q.stats;
+    const uint64_t width = q.width, height = q.height, frames = q.kind == FrameKind::single ? 1u : q.n;
+    if (q.ids.ptr || q.masks.ptr || (q.rgba.ptr && (q.rgba.bpp != 4u || q.rgba.over || q.cache))) {
+        set_error("statistics go alone or with an sRGB8 RGBA frame without a layer cache");
+        return FORMA_STATUS_INVALID;
+    }
+    if (((uintptr_t)t.ptr & 7u) != 0u || t.n_orders == 0u || (uint64_t)t.first_order + t.n_orders > (1ull << 21) ||
+        !std::isfinite(t.min_coverage) || t.min_coverage < 0.0f || t.min_coverage >= 1.0f) {
+        set_error("invalid statistics: records 8-byte aligned, orders [%u, %u + %u) (1 to 2^21 orders below 2^21), "
+                  "min_coverage %g (finite, in [0, 1))", t.first_order, t.first_order, t.n_orders, (double)t.min_coverage);
+        return FORMA_STATUS_INVALID;
+    }
+    if (width == 0 || height == 0 || width > FORMA_MAX_WIDTH || height > FORMA_MAX_HEIGHT) {
+        set_error("invalid statistics frame %llux%llu", (unsigned long long)width, (unsigned long long)height);
+        return FORMA_STATUS_INVALID;
+    }
+    uint64_t n_rec = 0, bytes = 0;
+    if (__builtin_mul_overflow(frames, (uint64_t)t.n_orders, &n_rec) ||
+        __builtin_mul_overflow(n_rec, (uint64_t)sizeof(forma_layer_stats), &bytes)) {
+        set_error("the statistics' records overflow 64 bits: %llu frames of %u records", (unsigned long long)frames, t.n_orders);
         return FORMA_STATUS_INVALID;
     }
     if (q.kind != FrameKind::single && (q.n == 0 || q.n > max_views(height))) {
@@ -844,7 +889,8 @@ int Renderer::bind_batch(Composition* const* comps, uint32_t n, PaintScene& S, u
 }
 
 // The frame's kernels: paint() for the RGBA target (in copy bands, or with the rows of a stack's
-// frames), then the ID kernel for the ID target. The sync-free redo repeats both.
+// frames), then the ID kernel for the ID target, or the mask or statistics kernels. The sync-free
+// redo repeats them all.
 int Renderer::paint_step(const FrameRequest& q, const PaintScene& S, const FramePlan& p, const uint32_t* heavy_lists,
                          uint32_t* paint_launches) {
     if (q.rgba.ptr) {
@@ -863,7 +909,7 @@ int Renderer::paint_step(const FrameRequest& q, const PaintScene& S, const Frame
         }
         const int st = paint(S, p.rgba.ptr, q.rgba.ptr, q.rgba.stride, p.in_bands, heavy_lists, paint_launches, p.rows, q.rgba.bpp,
                              solid_over, q.rgba.over);
-        if (st || (!q.ids.ptr && !q.masks.ptr)) return st;
+        if (st || (!q.ids.ptr && !q.masks.ptr && !q.stats.ptr)) return st;
         if (q.ids.ptr) ++*paint_launches;
     }
     FORMA_CUDA_TRY(id_flags.reserve(std::max<size_t>(recs.capacity, 1)));
@@ -872,6 +918,16 @@ int Renderer::paint_step(const FrameRequest& q, const PaintScene& S, const Frame
         const MaskFrame m{p.masks.ptr, p.masks.stride, p.mask_plane_stride, q.masks.first_order, q.masks.n_orders, q.masks.format,
                           (uint32_t)q.height, q.kind == FrameKind::single ? 1u : q.n};
         const uint32_t n = launch_paint_masks(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), id_flags.ptr, m,
+                                              totals.ptr + 8, stream, p.rows, frames);
+        launches += n;
+        *paint_launches = q.rgba.ptr ? *paint_launches + n : n;
+        FORMA_CUDA_TRY(cudaGetLastError());
+        return FORMA_STATUS_OK;
+    }
+    if (q.stats.ptr) {  // the records' initialisation, both walks, the empty boxes (the redo of a sync-free frame repeats all)
+        const StatsFrame f{p.stats, q.stats.first_order, q.stats.n_orders, q.stats.min_coverage, (uint32_t)q.height,
+                           q.kind == FrameKind::single ? 1u : q.n};
+        const uint32_t n = launch_paint_stats(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), id_flags.ptr, f,
                                               totals.ptr + 8, stream, p.rows, frames);
         launches += n;
         *paint_launches = q.rgba.ptr ? *paint_launches + n : n;
@@ -919,7 +975,13 @@ int Renderer::output_step(const FrameRequest& q, const PaintScene& S, const Fram
     };
     int st = p.in_bands ? FORMA_STATUS_OK : output(q.rgba, p.rgba);
     st = st ? st : output(q.ids, p.ids);
-    if (st || !q.masks.ptr || q.masks.on_device) return st;
+    if (st) return st;
+    if (q.stats.ptr && !q.stats.on_device) {  // host statistics (single frames): the records
+        const size_t bytes = (size_t)q.stats.n_orders * sizeof(forma_layer_stats);
+        FORMA_CUDA_TRY(cudaMemcpyAsync(q.stats.ptr, p.stats, bytes, cudaMemcpyDeviceToHost, stream));
+        d2h_bytes += bytes;
+    }
+    if (!q.masks.ptr || q.masks.on_device) return FORMA_STATUS_OK;
     // Host masks (single frames): the crop's tile rectangle of every plane.
     const MaskTarget& m = q.masks;
     const uint64_t bpp = m.bpp();

@@ -61,6 +61,15 @@ struct MaskTarget {
     uint32_t bpp() const { return format == FORMA_MASK_U8 ? 1u : 4u; }
 };
 
+// The statistics target of a FrameRequest (see forma_renderer_render_stats): n_orders records of
+// order first_order + k per frame, frame b's at ptr + b * n_orders.
+struct StatsTarget {
+    forma_layer_stats* ptr = nullptr;  // null: the request has no statistics
+    bool on_device = false;
+    uint32_t first_order = 0, n_orders = 0;
+    float min_coverage = 0.0f;
+};
+
 // What a FrameRequest renders. single: one frame of a composition. views: n views of one
 // composition in one pass, stacked top to bottom as one frame of n * ceil(height / 16) tile rows;
 // line setup rasterizes every view in its own coordinates and moves its segments' tile rows to the
@@ -74,7 +83,7 @@ enum class FrameKind { single, views, batch };
 
 // One call of Renderer::render: what is rendered, the size of one frame, and its targets: an
 // RGBA target, an ID target (channels {0, 1, 2, 3}, clear colour 0 when it is alone) or both, or
-// masks, alone or with an sRGB8 RGBA target.
+// masks or statistics, alone or with an sRGB8 RGBA target.
 struct FrameRequest {
     FrameKind kind = FrameKind::single;
     uint32_t n = 0;  // stacks: the frames
@@ -86,6 +95,7 @@ struct FrameRequest {
     LayerCache* cache = nullptr;       // single RGBA frames only
     FrameTarget rgba, ids;
     MaskTarget masks;
+    StatsTarget stats;
     Composition* comp = nullptr;          // single, views
     const float* views = nullptr;         // views: n transforms [ux, vx, uy, vy, tx, ty]
     Composition* const* batch = nullptr;  // batch: n compositions (null entries are refused)
@@ -105,6 +115,7 @@ struct FramePlan {
     bool pack_written;  // a cached host frame: only the tiles it writes travel back (scatter_written_tiles)
     DeviceFrame masks;  // the caller's planes on the device, or (host masks) the renderer's scratch ...
     uint64_t mask_plane_stride;  // ... with this plane stride
+    forma_layer_stats* stats;    // the caller's records on the device, or (host statistics) the renderer's scratch
 };
 
 // The line setup of a batch (see Renderer::bind_batch).
@@ -316,6 +327,7 @@ class Renderer {
     int render(const FrameRequest& q);
     int check_request(const FrameRequest& q);
     int check_masks(const FrameRequest& q);
+    int check_stats(const FrameRequest& q);
     // One frame of S: uploads, line setup, sort, then the painter tables, paint_step and
     // output_step once or, when the sync-free bounds were too small, twice.
     int run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p);
@@ -325,6 +337,7 @@ class Renderer {
     DeviceBuffer<uint8_t> id_flags;   // per entry: the ID kernel's optimizer flags (clip tiles)
     DeviceBuffer<uint32_t> id_frame;  // the ID target's scratch frame
     DeviceBuffer<uint8_t> mask_frame; // the planes of host masks
+    DeviceBuffer<forma_layer_stats> stats_scratch;  // the records of host statistics
     PinnedBuffer<float> h_views;
     DeviceBuffer<float> d_views;
     // A batch's distinct compositions' tables are gathered into the batch tables below, which are

@@ -2,6 +2,7 @@
 
     python -m forma_b200.render in.svg out.ppm [--width W --height H --scale S --device 0] [--ids ids.npy] [--linear out.npy]
                                                [--over image.{ppm,png}] [--masks masks.npy --mask-orders A:B [--mask-u8]]
+                                               [--stats stats.npz [--stats-orders A:B] [--stats-min-coverage C]]
 
 The equivalent of the reference's `demo svg --file in.svg --scale S` + the `S` key's
 capture.ppm (demo/src/main.rs, demo/src/runner.rs:193-219: a binary P6 file with the
@@ -17,6 +18,10 @@ its size replaces --width / --height.
 `--masks` also writes the layer coverage masks of orders [A, B) (`--mask-orders A:B`, Renderer.render_masks):
 per layer its anti-aliased coverage, whatever lies above it, as a (B - A) x H x W float32 .npy, or uint8 with
 `--mask-u8`.
+`--stats` also writes the layer statistics of orders [A, B) (`--stats-orders A:B`, default every order;
+Renderer.render_stats) to an .npz: per order its amodal `area` (sum of mask values x 2^18), the `pixels`
+its mask exceeds `--stats-min-coverage` on and their `box` (x0, y0, x1, y1), the `visible` pixels its
+ID owns and their `visible_box`, and the window's `first_order`.
 """
 from __future__ import annotations
 
@@ -79,6 +84,10 @@ def main(argv=None) -> int:
     ap.add_argument("--masks", help="also write the layer coverage masks (K x H x W, Renderer.render_masks) to this .npy file")
     ap.add_argument("--mask-orders", default="0:1", help="the masks' layer orders A:B, i.e. [A, B) (default 0:1)")
     ap.add_argument("--mask-u8", action="store_true", help="masks as uint8 (the alpha byte of sRGB8 frames) instead of float32")
+    ap.add_argument("--stats", help="also write the layer statistics (Renderer.render_stats) to this .npz file")
+    ap.add_argument("--stats-orders", help="the statistics' layer orders A:B, i.e. [A, B) (default: every order)")
+    ap.add_argument("--stats-min-coverage", type=float, default=0.0,
+                    help="the coverage a pixel's mask must exceed to count for pixels / box, as for ID frames (default 0)")
     args = ap.parse_args(argv)
     mask_lo, mask_hi = (int(v) for v in args.mask_orders.split(":"))
     if args.masks and mask_hi <= mask_lo:
@@ -131,6 +140,19 @@ def main(argv=None) -> int:
         masks = np.zeros((mask_hi - mask_lo, args.height, args.width), np.uint8 if args.mask_u8 else np.float32)
         renderer.render_masks(comp, masks, args.width, args.height, mask_lo)
         np.save(args.masks, masks)
+    if args.stats:
+        if args.stats_orders:
+            stats_lo, stats_hi = (int(v) for v in args.stats_orders.split(":"))
+        else:
+            stats_lo, stats_hi, found = 0, 0, 0  # every order: up to the last of the composition's layers
+            while found < len(comp):
+                found += comp.get(stats_hi) is not None
+                stats_hi += 1
+            stats_hi = max(stats_hi, 1)
+        if stats_hi <= stats_lo:
+            ap.error("--stats-orders A:B needs A < B")
+        rec = renderer.render_stats(comp, args.width, args.height, stats_lo, stats_hi - stats_lo, args.stats_min_coverage)
+        np.savez(args.stats, first_order=stats_lo, **{name: rec[name] for name in rec.dtype.names})
     print(f"{len(paths)} paths parsed in {t1 - t0:.2f} s, composed in {t2 - t1:.2f} s; {t.n_segments} pixel segments; "
           f"last frame: line setup {t.line_setup_ms:.3f} ms, rasterize {t.rasterize_ms:.3f} ms, sort {t.sort_ms:.3f} ms, "
           f"paint {t.paint_ms:.3f} ms ({(t3 - t2) / max(args.frames, 1) * 1e3:.2f} ms per call) -> {args.out}", file=sys.stderr)

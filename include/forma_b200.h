@@ -522,6 +522,71 @@ int forma_renderer_render_batch_masks_device(forma_renderer*, forma_composition*
                                              const uint32_t channels[4], const float clear_color[4],
                                              forma_timings* timings /* nullable */);
 
+/* Layer statistics (no reference counterpart): a handful of exact integers per layer instead of
+ * its planes, for the boxes, areas and occlusion ratios of instance and amodal datasets. A request
+ * names a window of layer orders [first_order, first_order + n_orders), n_orders = K >= 1, as the
+ * mask calls do, and a min_coverage in [0, 1) as the ID calls do. For every frame b and every
+ * order o of the window there is one 48-byte record, frame b's at ptr + b K:
+ *   - area:    sum over the counted pixels p of v_o(p) x 2^18, v_o(p) exactly the F32 value of
+ *              forma_renderer_render_masks for o at p (clipped and clip layers included; 0 for
+ *              orders that are absent, disabled or without props). v is k / 512 or a product of
+ *              two such values, so the sum is an exact integer;
+ *   - pixels:  the counted pixels with v_o(p) > min_coverage;
+ *   - visible: the counted pixels whose ID (forma_renderer_render_ids at min_coverage) is o;
+ *   - box, visible_box: x0, y0, x1, y1 (half-open, in frame pixels) of the `pixels` and the
+ *              `visible` set; all four 0 when the set is empty.
+ * visible / pixels is the share of a layer that no layer above it hides: the occlusion ratio.
+ * Counted pixels: for a single frame, the frame's pixels inside the crop's tile rectangle (the
+ * rectangle mask and ID calls write); for views and batches, each frame's own width x height
+ * pixels in its own coordinates (rows of the last tile row at or below `height` never count).
+ * For a batch, frame c's records are comps[c]'s own orders; every view reports the same orders.
+ * The records are integers, so the result does not depend on the order the device adds them in:
+ * two identical calls give identical bytes.
+ * With a non-null device_buffer the device calls also write the sRGB8 RGBA frame or stack from
+ * the same pass: exactly the bytes of forma_renderer_render_device (without a layer cache),
+ * forma_renderer_render_views_device or forma_renderer_render_batch_device with the same
+ * arguments. With a null device_buffer, width_stride, view_stride / frame_stride, channels and
+ * clear_color are not read.
+ * Refusals return FORMA_ERR_INVALID_ARGUMENT before anything is written to either buffer: a null
+ * descriptor or pointer; a pointer that is not 8-byte aligned; K = 0 or first_order + K > 2^21;
+ * min_coverage not finite or outside [0, 1); a record array whose size overflows 64 bits; and
+ * everything the mask calls refuse for the target, views and batches. Their order-sum, stop /
+ * texel and 2^30-segment limits apply as well. Statistics go alone or with an sRGB8 RGBA target,
+ * never with IDs or masks; they take no layer cache and leave every cache as it was. Afterwards
+ * counters, segments, stage times and row costs describe the call's frame; stage time [5] covers
+ * the paint kernel and the statistics kernels (the records' initialisation, the amodal walk, the
+ * visible walk and the empty boxes' fix-up).
+ * render_stats reduces into device scratch and copies the records into a HOST array; the _device
+ * calls write device memory on the renderer's device. */
+typedef struct forma_layer_stats {
+    uint64_t area;           /* sum over p of v_o(p) * 2^18: exact (v is k/512 or a product of two such) */
+    uint32_t pixels;         /* pixels p with v_o(p) > min_coverage                                      */
+    uint32_t visible;        /* pixels p whose ID (forma_renderer_render_ids at min_coverage) is o       */
+    uint32_t box[4];         /* x0, y0, x1, y1 (half-open, frame pixels) of the `pixels` set; 0s if empty */
+    uint32_t visible_box[4]; /* the same for the `visible` set                                           */
+} forma_layer_stats;
+typedef struct forma_stats {
+    forma_layer_stats* ptr; /* frame b's records at ptr + b * n_orders; 8-byte aligned */
+    uint32_t first_order, n_orders;
+    float min_coverage;
+} forma_stats;
+int forma_renderer_render_stats(forma_renderer*, forma_composition*, const forma_stats* stats, uint64_t width, uint64_t height,
+                                const forma_rect* crop /* nullable */, forma_timings* timings /* nullable */);
+int forma_renderer_render_stats_device(forma_renderer*, forma_composition*, const forma_stats* stats, uint64_t width,
+                                       uint64_t height, const forma_rect* crop /* nullable */,
+                                       uint8_t* device_buffer /* nullable */, uint64_t width_stride, const uint32_t channels[4],
+                                       const float clear_color[4], forma_timings* timings /* nullable */);
+int forma_renderer_render_views_stats_device(forma_renderer*, forma_composition*, const float* views, uint32_t n,
+                                             const forma_stats* stats, uint64_t width, uint64_t height,
+                                             uint8_t* device_buffer /* nullable */, uint64_t width_stride, uint64_t view_stride,
+                                             const uint32_t channels[4], const float clear_color[4],
+                                             forma_timings* timings /* nullable */);
+int forma_renderer_render_batch_stats_device(forma_renderer*, forma_composition* const* comps, uint32_t n,
+                                             const forma_stats* stats, uint64_t width, uint64_t height,
+                                             uint8_t* device_buffer /* nullable */, uint64_t width_stride, uint64_t frame_stride,
+                                             const uint32_t channels[4], const float clear_color[4],
+                                             forma_timings* timings /* nullable */);
+
 /* Launch on `cuda_stream` (a cudaStream_t, e.g. torch.cuda.current_stream().cuda_stream)
  * instead of the default stream. */
 void forma_renderer_set_stream(forma_renderer*, void* cuda_stream);
