@@ -319,12 +319,15 @@ struct EntryRec {  // 64 B
 // the per-tile entry ranges (tile_range: zeroed by the caller, left zero for tiles without
 // entries) and, when `heavy` is not null, the lists of tiles with many entries:
 // kHeavyListClasses arrays of tiles_x * tiles_y ids each, their lengths in
-// heavy_count[kHeavyListClasses] (zeroed by the caller).
+// heavy_count[kHeavyListClasses] (zeroed by the caller). frames != nullptr: S stacks the frames of
+// a batch, `rows` tile rows each (their order bases bound each entry's clip_layers to the range a
+// single frame of its composition has).
 constexpr int kHeavyListClasses = 4;
 void launch_merge_entries(const PaintScene& S, const uint64_t* cell_key, uint32_t n_cells, const uint64_t* gkey,
                           const uint32_t* gid, uint32_t n_gaps, const uint32_t* cell_start, const uint4* carry_in,
                           const uint4* gap_carry, uint64_t* ekey, EntryRec* recs, uint8_t* eflags, uint2* tile_range,
-                          uint32_t* heavy, uint32_t* heavy_count, cudaStream_t st, const DevCounts& dc = DevCounts());
+                          uint32_t* heavy, uint32_t* heavy_count, cudaStream_t st, const DevCounts& dc = DevCounts(),
+                          const BatchFrame* frames = nullptr, uint32_t rows = 0);
 // view_rows != 0: S stacks views of view_rows tile rows each (ViewArgs); gradients and textures are
 // then sampled in each view's own coordinates. solid_over: every layer of the frame is a solid `Over`
 // fill without clips (Composition::solid_over_only); the lean build of the kernel paints it.

@@ -218,7 +218,9 @@ void launch_paint_ids(const PaintScene& S, const uint64_t* segs, const EntryRec*
 // window's first entry and stops at its end; nothing outside the window is read. Tiles with
 // clips walk bottom-up from their first entry with the painter's clip state after
 // skip_trivial_clips (as in the ID kernel's clip tiles, without the skip below the first opaque
-// layer). A clip below the window is only accumulated when its mask can still apply to a window
+// layer); the clip state restarts at every entry the ID kernel could take as its first (full,
+// opaque, unclipped), so that each layer's mask is its walk in the painter's render of the
+// composition cut off above it. A clip below the window is only accumulated when its mask can still apply to a window
 // entry (the clip state's last layer reaches the window); other entries below the window are
 // skipped without reading their segments.
 //
@@ -521,6 +523,10 @@ __device__ __forceinline__ void paint_masks_body(const PaintScene& S, const Mask
                         }
                         continue;
                     }
+                    // A layer the painter could start from (the ID kernel's `cand`): the walk of
+                    // every layer from here up starts with no clip, as the painter's would.
+                    const bool clipped = (flags & kFlagClippedDraw) && !(flags & kFlagSkipClip);
+                    if (!clipped && (flags & kFlagFull) && (flags & kFlagOpaque)) clip_active = false;
                     if (clip_active && clip_last < layer) clip_active = false;  // mod.rs:302-306
                     if (is_clip) {  // clip_at, mod.rs:449-464
                         if (!clip_active) {

@@ -639,7 +639,8 @@ __global__ void merge_entries_kernel(PaintScene S, const uint64_t* __restrict__ 
                                      const uint32_t* __restrict__ cell_start, const uint4* __restrict__ carry_in,
                                      const uint4* __restrict__ gap_carry, uint64_t* __restrict__ ekey,
                                      EntryRec* __restrict__ recs, uint8_t* __restrict__ eflags, uint2* __restrict__ tile_range,
-                                     uint32_t* __restrict__ heavy, uint32_t* __restrict__ heavy_count, DevCounts dc) {
+                                     uint32_t* __restrict__ heavy, uint32_t* __restrict__ heavy_count, DevCounts dc,
+                                     const BatchFrame* __restrict__ frames, uint32_t rows) {
     resolve_counts(dc, n_cells, n_gaps);
     // Merge-path style partition: the keys of a CTA's 256 consecutive elements of
     // one list bracket a short range of the other list, found once per CTA (two
@@ -710,7 +711,12 @@ __global__ void merge_entries_kernel(PaintScene S, const uint64_t* __restrict__ 
         const StyleRec& st = S.styles[r.slot];
         const bool unchanged = S.unchanged && S.unchanged[r.layer];
         r.meta = pack_style_meta(st, unchanged);
-        r.clip_layers = st.clip_layers;
+        // The clip's range in the frame's own orders o (a batch's layers are order_base + o, see
+        // BatchFrame): o + clip_layers wraps below o in 32 bits (the clip then ends at itself), or
+        // ends at the last order there can be. Every walk adds it to the layer as it stands, and
+        // then finds the range a single frame of the composition finds.
+        const uint32_t o = frames && in_frame ? r.layer - frames[(key_ty(k) - 1u) / rows].order_base : r.layer;
+        r.clip_layers = o + st.clip_layers < o ? 0u : min(st.clip_layers, kLayerLimit - o);
         r.color[0] = st.color[0];
         r.color[1] = st.color[1];
         r.color[2] = st.color[2];
@@ -840,11 +846,13 @@ void launch_carry_pass(const PaintScene& S, const uint64_t* key2, const uint32_t
 void launch_merge_entries(const PaintScene& S, const uint64_t* cell_key, uint32_t n_cells, const uint64_t* gkey,
                           const uint32_t* gid, uint32_t n_gaps, const uint32_t* cell_start, const uint4* carry_in,
                           const uint4* gap_carry, uint64_t* ekey, EntryRec* recs, uint8_t* eflags, uint2* tile_range,
-                          uint32_t* heavy, uint32_t* heavy_count, cudaStream_t st, const DevCounts& dc) {
+                          uint32_t* heavy, uint32_t* heavy_count, cudaStream_t st, const DevCounts& dc, const BatchFrame* frames,
+                          uint32_t rows) {
     uint32_t n = n_cells + n_gaps;
     if (n)
         merge_entries_kernel<<<(n + 255) / 256, 256, 0, st>>>(S, cell_key, n_cells, gkey, gid, n_gaps, cell_start, carry_in,
-                                                               gap_carry, ekey, recs, eflags, tile_range, heavy, heavy_count, dc);
+                                                               gap_carry, ekey, recs, eflags, tile_range, heavy, heavy_count, dc,
+                                                               frames, rows);
 }
 
 // ---------------------------------------------------------------------------

@@ -503,7 +503,7 @@ int Renderer::run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p
     uint32_t paint_launches = 1;
     for (bool sync_free = fast;; sync_free = false) {
         DevCounts dc;
-        st = build_tables(S, n, sync_free, prev_cells, prev_gaps, heavy_lists, dc);
+        st = build_tables(S, n, sync_free, prev_cells, prev_gaps, heavy_lists, dc, batched ? &batch.args : nullptr);
         if (st) return st;
         st = queue_row_costs(S, n);
         if (st) return st;
@@ -1096,8 +1096,9 @@ SortResult Renderer::sort(DeviceBuffer<uint64_t>& keys, DeviceBuffer<uint64_t>& 
 //   memsets (tile ranges, table scratch) and the kernels, nothing else.
 // - counted: a count is read back; the kernel that produces it runs ahead of the read-back into
 //   the buffers of the previous frames and is launched again when they turn out too small.
+// batch: the frames of a batch (the merge bounds each entry's clip range by its frame's orders).
 int Renderer::build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint32_t prev_cells, uint32_t prev_gaps,
-                           uint32_t* heavy_lists, DevCounts& dc) {
+                           uint32_t* heavy_lists, DevCounts& dc, const BatchArgs* batch) {
     // Tiles without entries keep an empty range: a frame whose tables are redone paints only the
     // clear colour in its first attempt. A count above its bound leaves every range empty (the
     // merge kernel then writes none), so that attempt of an over frame writes nothing at all.
@@ -1211,7 +1212,8 @@ int Renderer::build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint
         sort(ekey_tmp, gkey_tmp, &eid_tmp, &gid_tmp, n_gaps, gap_plan, nullptr, dc.gaps,
              reinterpret_cast<const uint32_t*>(table_scratch.ptr + L.gap_hist), table_scratch.ptr + L.gap_sort);
     launch_merge_entries(S, cell_key.ptr, n_cells, ekey_tmp.ptr, eid_tmp.ptr, n_gaps, cell_start.ptr, carry_in.ptr, gap_carry.ptr,
-                         ekey.ptr, recs.ptr, eflags.ptr, tile_range.ptr, heavy_lists, heavy_count(), stream, dc);
+                         ekey.ptr, recs.ptr, eflags.ptr, tile_range.ptr, heavy_lists, heavy_count(), stream, dc,
+                         batch ? batch->frames : nullptr, batch ? batch->rows : 0u);
     ++launches;
     // sync_free: the counts travel to the host behind everything else of the frame.
     if (sync_free)

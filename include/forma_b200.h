@@ -293,7 +293,9 @@ int forma_renderer_render_views(forma_renderer*, forma_composition*, const float
  * Layer orders: the distinct compositions, in order of first appearance, get consecutive slices
  * of the 21-bit layer field. Composition k's slice starts at base_k, the sum of n_orders (its
  * largest attached order + 1, or 0 without layers) of the distinct compositions before it, and
- * its segments carry base_k + order. The sum over all distinct compositions must not exceed
+ * its segments carry base_k + order. Clip ranges stay in the composition's own orders: a
+ * Func::Clip(n) at order o covers o .. o + n, and only itself where o + n does not fit in 32 bits,
+ * for every n in [0, 2^32) and whatever base_k is. The sum over all distinct compositions must not exceed
  * 2^21: otherwise FORMA_ERR_ORDER_LIMIT. Null comps or a null entry, n outside
  * 1 ... forma_renderer_max_views(height), a short frame_stride, or an invalid target or channel
  * return FORMA_ERR_INVALID_ARGUMENT. All of these are refused before anything is written.
@@ -331,7 +333,9 @@ int forma_renderer_render_batch(forma_renderer*, forma_composition* const* comps
  * values are layer orders of the composition.
  * Batches: ID frame c holds what forma_renderer_render_ids_device gives for comps[c] alone: the
  * values are comps[c]'s own orders, not base_k + order (which slice of the layer field a
- * composition gets stays inside the call), and FORMA_ID_NONE where no layer hits.
+ * composition gets stays inside the call), and FORMA_ID_NONE where no layer hits. That holds for
+ * every Func::Clip(n), n in [0, 2^32): a clip at order o covers the orders o .. o + n of its own
+ * composition, and only itself when o + n does not fit in 32 bits, whatever its slice.
  * (Frames whose lines all lie more than 2^19 px left of the frame are the exception of views and
  * batches again: the stacked calls are right, forma_renderer_render_ids_device is not.)
  * min_coverage must be finite and in [0, 1); 1 <= n <= forma_renderer_max_views(height); the
@@ -466,11 +470,14 @@ int forma_renderer_render_batch_over_device(forma_renderer*, forma_composition* 
  *     paint_layer computes for o at p under its fill rule from its cells and carried cover
  *     (doubled_area_to_coverage), a multiple of 1/512 in [0, 1];
  *   - o a Func::Draw layer with is_clipped: c_o(p) x m(p), m the clip mask that applies to o in p's
- *     tile under the painter's clip state (clip_at, cpu/painter/mod.rs:302-323, 449-464), the
- *     tile's layers walked bottom-up after the skip_trivial_clips pass with every layer painted:
- *     nothing is skipped below an opaque layer, so the mask is amodal (the parts other layers hide
- *     are kept). Where no clip applies to o (no clip active, or the pass masks o out), 0; where the
- *     pass finds o's clip full, the clip is 1 and the value c_o(p);
+ *     tile in the painter's walk of the composition cut off above o (clip_at, cpu/painter/mod.rs:
+ *     302-323, 449-464): the tile's layers are walked bottom-up from its first layer after the
+ *     skip_trivial_clips pass with every layer painted, so the mask is amodal (the parts other
+ *     layers hide are kept), and the clip state restarts at every layer the painter could start
+ *     from (skip_fully_covered_layers: painted, not clipped, full in the tile, a solid opaque Over
+ *     fill). Where no clip applies to o (no clip active, or the pass masks o out), 0; where the
+ *     pass finds o's clip full, the clip is 1 and the value c_o(p). So wherever o is painted, its
+ *     value is exactly the coverage x clip mask the painter paints it with;
  *   - o a Func::Clip layer: its own coverage c_o(p);
  *   - anything else (no such layer, a disabled layer, a layer without props): 0.
  * Colour, alpha, gradient, texture and blend mode play no part, nor does any other layer than the
@@ -535,7 +542,9 @@ int forma_renderer_render_batch_masks_device(forma_renderer*, forma_composition*
  *   - visible: the counted pixels whose ID (forma_renderer_render_ids at min_coverage) is o;
  *   - box, visible_box: x0, y0, x1, y1 (half-open, in frame pixels) of the `pixels` and the
  *              `visible` set; all four 0 when the set is empty.
- * visible / pixels is the share of a layer that no layer above it hides: the occlusion ratio.
+ * A pixel's ID is o only where v_o(p) > min_coverage (the painter paints o there with v_o), so
+ * visible <= pixels and visible_box lies inside box: visible / pixels is the share of a layer that
+ * no layer above it hides, the occlusion ratio.
  * Counted pixels: for a single frame, the frame's pixels inside the crop's tile rectangle (the
  * rectangle mask and ID calls write); for views and batches, each frame's own width x height
  * pixels in its own coordinates (rows of the last tile row at or below `height` never count).

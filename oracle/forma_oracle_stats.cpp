@@ -58,6 +58,7 @@ static void drive_tile_stats(Workbench& wb, Painter& painter, const TileContext&
         const uint32_t id = wb.ids[k].id;
         const Props& props = ctx.props->get(id);
         const bool is_clip = props.func != kDraw, in_window = window.holds(id);
+        if (may_start_painting(wb, k, props)) painter.clip_active = false;
         if (wb.ids[k].mask || (is_clip && in_window)) {
             painter.clear_cells();
             if (const Workbench::SegRange* r = wb.segments_of(id))

@@ -4,7 +4,8 @@
 // state) recording each layer's coverage x clip mask instead of blending. Free functions over the
 // painter's own types, so that painter.hpp and the RGBA path built from it stay exactly as they are.
 // Every layer of a tile is painted: skip_trivial_clips decides which clips are painted and which
-// clipped layers keep their clip, as in the painter, but no layer is skipped below an opaque one.
+// clipped layers keep their clip, as in the painter, but no layer is skipped below an opaque one
+// (the clip state restarts at every layer the painter could start from instead).
 #pragma once
 
 #include "painter.hpp"
@@ -67,6 +68,17 @@ inline Cover paint_layer_masks(Painter& p, uint32_t layer_id, const Props& props
     return out;
 }
 
+// Whether entry k of the tile (after skip_trivial_clips) is a layer skip_fully_covered_layers
+// may choose as the painter's first (passes/skip_fully_covered_layers.rs:27-119): painted,
+// unclipped, full, and a solid opaque Over fill. The mask of layer o is its walk in the painter's
+// render of the composition cut off above o, which starts at the top-most such layer at or below
+// o: the mask walk restarts its clip state at every one of them.
+inline bool may_start_painting(const Workbench& wb, size_t k, const Props& props) {
+    const bool clipped = props.func == kDraw && props.is_clipped && !wb.ids[k].skip_clipping;
+    return wb.ids[k].mask && props.func == kDraw && !clipped && wb.layer_is_full(wb.ids[k].id, props.fill_rule) &&
+           props.fill_type == kSolid && props.blend_mode == kOver && props.color.a == 1.0f;
+}
+
 // Workbench::drive_tile_painting for a mask frame (no layer cache): populate_layers and
 // skip_trivial_clips, then every layer bottom-up. `planes` (window.count x 256, zeroed by the
 // caller) receives the window's layers.
@@ -78,6 +90,7 @@ inline void drive_tile_masks(Workbench& wb, Painter& painter, const TileContext&
         const uint32_t id = wb.ids[k].id;
         const Props& props = ctx.props->get(id);
         const bool is_clip = props.func != kDraw;
+        if (may_start_painting(wb, k, props)) painter.clip_active = false;
         float* plane = window.holds(id) ? planes + (size_t)(id - window.first) * (kTile * kTile) : nullptr;
         if (wb.ids[k].mask || (is_clip && plane)) {
             painter.clear_cells();
