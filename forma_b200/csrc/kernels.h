@@ -328,26 +328,35 @@ void launch_merge_entries(const PaintScene& S, const uint64_t* cell_key, uint32_
                           const uint4* gap_carry, uint64_t* ekey, EntryRec* recs, uint8_t* eflags, uint2* tile_range,
                           uint32_t* heavy, uint32_t* heavy_count, cudaStream_t st, const DevCounts& dc = DevCounts(),
                           const BatchFrame* frames = nullptr, uint32_t rows = 0);
+// The painter tables of a frame as every tile kernel (paint, ID, mask, statistics) reads them: the
+// sorted segments, the entry records, the per-tile entry ranges and, when `heavy` is not null, the
+// heavy-tile lists with their lengths (launch_merge_entries).
+struct TileTables {
+    const uint64_t* segs;
+    const EntryRec* recs;
+    const uint2* tile_range;
+    const uint32_t* heavy;
+    const uint32_t* heavy_count;
+};
+// The tile kernels below are persistent: their warps take the tiles of S's tile rectangle by ticket
+// from `tile_counter`, which the launcher resets on `st`. Nothing is launched for an empty rectangle.
 // view_rows != 0: S stacks views of view_rows tile rows each (ViewArgs); gradients and textures are
 // then sampled in each view's own coordinates. solid_over: every layer of the frame is a solid `Over`
 // fill without clips (Composition::solid_over_only); the lean build of the kernel paints it.
-void launch_paint(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range, const uint32_t* heavy,
-                  const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st,
-                  uint32_t view_rows = 0, bool solid_over = false);
+void launch_paint(const PaintScene& S, const TileTables& t, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter,
+                  cudaStream_t st, uint32_t view_rows = 0, bool solid_over = false);
 // launch_paint for a linear float frame of `bpp` bytes per pixel: 8 (RGBA16F) or 16 (RGBA32F), the
 // painter's planes in channel order where launch_paint stores their sRGB bytes (see
 // forma_renderer_render_linear). `framebuffer` and S.stride: multiples of 4 bytes.
-void launch_paint_linear(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range, const uint32_t* heavy,
-                         const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st,
-                         uint32_t view_rows, uint32_t bpp);
+void launch_paint_linear(const PaintScene& S, const TileTables& t, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter,
+                         cudaStream_t st, uint32_t view_rows, uint32_t bpp);
 // launch_paint over the pixels already in `framebuffer` (see forma_renderer_render_over_device):
 // each pixel's own value, decoded, is its clear colour; tiles without entries are not written.
 // bpp 4 (sRGB8, channels a permutation with A last), 8 (RGBA16F) or 16 (RGBA32F, both: any
 // permutation); S.channels are not upgraded (the kernels upgrade Alpha -> One per pixel).
 // `framebuffer` and S.stride: multiples of 4 bytes.
-void launch_paint_over(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range, const uint32_t* heavy,
-                       const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st,
-                       uint32_t view_rows, uint32_t bpp);
+void launch_paint_over(const PaintScene& S, const TileTables& t, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter,
+                       cudaStream_t st, uint32_t view_rows, uint32_t bpp);
 // The inverse of launch_repack_views: rows [0, height) of the n_views frames at src + b * view_stride
 // (row r at + r * stride) to the stacked frame at dst, frame b's first row at
 // dst + b * view_rows_px * dst_stride. `width` in 4-byte words; every pointer and stride a multiple of 4.
@@ -364,8 +373,7 @@ void launch_repack_views(const uint8_t* src, uint64_t src_stride, uint32_t view_
 // frames != nullptr: S stacks the frames of a batch, `rows` tile rows each, whose entries carry
 // frames[c].order_base + order (BatchArgs); every ID stored is the frame's own order
 // (paint_ids_stacked_kernel). The stacked views of one composition need neither.
-void launch_paint_ids(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range,
-                      const uint32_t* heavy, const uint32_t* heavy_count, uint8_t* id_flags, uint32_t* ids, size_t ids_stride,
+void launch_paint_ids(const PaintScene& S, const TileTables& t, uint8_t* id_flags, uint32_t* ids, size_t ids_stride,
                       float min_coverage, uint32_t* tile_counter, cudaStream_t st, uint32_t rows = 0,
                       const BatchFrame* frames = nullptr);
 // Layer coverage masks (kernels_ids.cu, see forma_renderer_render_masks): n_orders planes per frame
@@ -382,9 +390,8 @@ struct MaskFrame {
 // frame's width x height pixels of a stack), then paints the masks from the tables like
 // launch_paint_ids (id_flags: the same scratch). rows != 0: S stacks frames of `rows` tile rows;
 // frames != nullptr: a batch, whose entries carry frames[c].order_base + order. Returns the launches.
-uint32_t launch_paint_masks(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range,
-                            const uint32_t* heavy, const uint32_t* heavy_count, uint8_t* id_flags, const MaskFrame& m,
-                            uint32_t* tile_counter, cudaStream_t st, uint32_t rows = 0, const BatchFrame* frames = nullptr);
+uint32_t launch_paint_masks(const PaintScene& S, const TileTables& t, uint8_t* id_flags, const MaskFrame& m, uint32_t* tile_counter,
+                            cudaStream_t st, uint32_t rows = 0, const BatchFrame* frames = nullptr);
 // Layer statistics (kernels_ids.cu, see forma_renderer_render_stats): n_orders records of order
 // first_order + k per frame of n_frames, frame b's at ptr + b * n_orders.
 struct StatsFrame {
@@ -397,9 +404,8 @@ struct StatsFrame {
 // Initialises the records, reduces the amodal walk (the mask kernel's) and the visible walk (the
 // ID kernel's) into them, then writes the empty sets' boxes: the whole of the records, so that the
 // sync-free redo can repeat it. rows / frames as for launch_paint_masks. Returns the launches.
-uint32_t launch_paint_stats(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range,
-                            const uint32_t* heavy, const uint32_t* heavy_count, uint8_t* id_flags, const StatsFrame& f,
-                            uint32_t* tile_counter, cudaStream_t st, uint32_t rows = 0, const BatchFrame* frames = nullptr);
+uint32_t launch_paint_stats(const PaintScene& S, const TileTables& t, uint8_t* id_flags, const StatsFrame& f, uint32_t* tile_counter,
+                            cudaStream_t st, uint32_t rows = 0, const BatchFrame* frames = nullptr);
 // The painter tables of a batch: the device tables of its distinct compositions, concatenated.
 // Composition k's orders land at order_base + order (the slots they name shifted by style_base,
 // -1 kept), its StyleRecs at style_base with stop_first + stop_base and tex_first + texel_base;

@@ -23,17 +23,20 @@
 // Stacked frames: a tile row belongs to one frame and the walk never looks at another tile, so
 // the views of one composition need nothing else. The frames of a batch carry base + order in
 // their entries (BatchFrame::order_base), and the walk compares layers and clip ranges in that
-// shifted space; paint_ids_stacked_kernel, the same body, takes the frame's base off every ID it
+// shifted space; paint_ids_stacked_kernel, the same walk, takes the frame's base off every ID it
 // stores (one look-up per tile).
+//
+// The ID walk (ids_walk) and the amodal walk of the mask and statistics kernels (amodal_walk) hand
+// each tile's result to a sink: the ID frame's store or add_visible, store_mask or add_amodal.
 #include <algorithm>
-#include <mutex>
 
 #include "../../include/forma_b200.h"
 #include "paint_common.cuh"
 
 namespace forma {
 
-struct IdInputs {
+// The tables every walk reads (TileTables, with the scratch and the ticket counter of the call).
+struct IdTables {
     const uint64_t* segs;
     const EntryRec* recs;
     const uint2* tile_range;
@@ -41,10 +44,28 @@ struct IdInputs {
     const uint32_t* heavy_count;
     uint32_t n_tiles_total;
     uint8_t* id_flags;            // per sorted entry: the flags after skip_trivial_clips (clip tiles only)
-    uint32_t* ids;                // the ID frame
-    size_t ids_stride;            // bytes
-    float min_coverage;
     uint32_t* tile_counter;
+};
+// The orders [first_order, first_order + n_orders) of the mask and statistics kernels, and the
+// frames of a stack.
+struct OrderWindow {
+    uint32_t first_order, n_orders;
+    uint32_t height;  // rows of one frame
+    uint32_t rows;    // stacks: tile rows per frame; 0: a single frame
+};
+struct IdsOut {
+    uint32_t* ids;  // the ID frame
+    size_t stride;  // bytes
+    float min_coverage;
+};
+struct MaskOut {
+    uint8_t* ptr;
+    uint64_t stride, plane_stride;
+    bool u8;
+};
+struct StatsOut {
+    forma_layer_stats* rec;  // n_frames x n_orders records
+    float min_coverage;
 };
 
 constexpr int kIdWarpsPerBlock = 2;
@@ -100,14 +121,14 @@ __device__ __forceinline__ void entry_coverage(IdWarpSmem& W, const EntryRec& h,
 }
 
 // Stages the records [lo, lo + cnt) in W.hdr, with the flags the walk uses in `pad`.
-__device__ __forceinline__ void stage_group(IdWarpSmem& W, const IdInputs& in, uint32_t lo, uint32_t cnt, bool clip_tile,
+__device__ __forceinline__ void stage_group(IdWarpSmem& W, const IdTables& T, uint32_t lo, uint32_t cnt, bool clip_tile,
                                             uint32_t lane) {
     __syncwarp();  // the previous group's records are no longer read
     if (lane < cnt) {
-        const uint4* src = reinterpret_cast<const uint4*>(in.recs + lo + lane);
+        const uint4* src = reinterpret_cast<const uint4*>(T.recs + lo + lane);
         uint4* dst = reinterpret_cast<uint4*>(&W.hdr[lane]);
         uint4 q3 = src[3];
-        q3.w = clip_tile ? (uint32_t)in.id_flags[lo + lane] : q3.z;  // pad <- flags (q3.z = flags0)
+        q3.w = clip_tile ? (uint32_t)T.id_flags[lo + lane] : q3.z;  // pad <- flags (q3.z = flags0)
         dst[0] = src[0]; dst[1] = src[1]; dst[2] = src[2]; dst[3] = q3;
     }
     __syncwarp();
@@ -154,65 +175,254 @@ __device__ __forceinline__ void skip_trivial_clips_ids(const EntryRec* __restric
     if (has_clip && !clip_used) out[clip_i] |= (uint8_t)kFlagMaskedOut;
 }
 
-// The lane's eight IDs of a batch frame's tile (base + order) as the frame's own orders.
-__device__ __forceinline__ void rebase_ids(uint32_t* out, uint32_t base) {
+// The warp's tiles, as paint_kernel takes them: tickets [0, H) walk the heavy lists (largest class
+// first), the rest the tile rectangle row-major. Listed tiles outside the rectangle are skipped,
+// and so are the rectangle's tiles that a list holds. Only H and the ticket count live in registers
+// (a heavy ticket reads the list lengths again), and a skipped ticket returns to the walk's loop
+// instead of looping here: with the lengths in registers or a loop here, the walk kernels spill
+// more or keep fewer CTAs resident (-Xptxas -v).
+struct TileTickets {
+    const PaintScene& S;
+    const IdTables& T;
+    uint32_t lane, H = 0, n_tickets;
+
+    __device__ __forceinline__ TileTickets(const PaintScene& S_, const IdTables& T_, uint32_t n_tiles, uint32_t lane_)
+        : S(S_), T(T_), lane(lane_) {
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
-        if (out[j] != FORMA_ID_NONE) out[j] -= base;
+        for (int c = 0; c < kHeavyClasses; ++c) H += T.heavy ? T.heavy_count[c] : 0u;
+        n_tickets = H + n_tiles;
+    }
+    // Takes the next ticket: false once they have run out. Otherwise `tile` says whether it names a
+    // tile to walk, with its linear id and entry range [b, e).
+    __device__ __forceinline__ bool next(bool& tile, uint32_t& tid, uint32_t& b, uint32_t& e) {
+        uint32_t ticket = 0;
+        if (lane == 0) ticket = atomicAdd(T.tile_counter, 1u);
+        ticket = __shfl_sync(kFullMask, ticket, 0);
+        if (ticket >= n_tickets) return false;
+        tile = false;
+        if (ticket < H) {
+            uint32_t t = ticket;
+            int c = kHeavyClasses - 1;
+#pragma unroll
+            for (int q = kHeavyClasses - 1; q > 0; --q)
+                if (c == q && t >= T.heavy_count[q]) {
+                    t -= T.heavy_count[q];
+                    c = q - 1;
+                }
+            tid = T.heavy[(size_t)c * T.n_tiles_total + t];
+            const uint32_t ty = tid / S.tiles_x, tx = tid - ty * S.tiles_x;
+            if (ty < S.ty_lo || ty >= S.ty_hi || tx < S.tx_lo || tx >= S.tx_hi) return true;
+        } else {
+            const uint32_t lin = ticket - H, ntx = S.tx_hi - S.tx_lo;
+            tid = (S.ty_lo + lin / ntx) * S.tiles_x + S.tx_lo + lin % ntx;
+        }
+        const uint2 range = T.tile_range[tid];
+        b = range.x;
+        e = range.y;
+        tile = !(ticket >= H && T.heavy && e - b >= kHeavyMin);  // done from its list
+        return true;
+    }
+};
+
+// Tile row ty of a stack of `rows` tile rows per frame (rows 0: a single frame): its frame, its
+// row in the frame and the order base of the frame's entries (frames: a batch; otherwise 0).
+struct FrameRow {
+    uint32_t frame, fty, base;
+};
+__device__ __forceinline__ FrameRow frame_row(uint32_t ty, uint32_t rows, const BatchFrame* __restrict__ frames) {
+    const uint32_t frame = rows ? ty / rows : 0u;
+    return FrameRow{frame, ty - frame * rows, frames ? frames[frame].order_base : 0u};
 }
 
-__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) paint_ids_kernel(PaintScene S, IdInputs in, uint32_t n_tiles) {
-#define FORMA_IDS_REBASE(out, ty)
-#include "paint_ids_body.cuh"
-#undef FORMA_IDS_REBASE
+// Whether entries [b, e) hold a clip-ish one (Func::Clip, or a clipped Draw). Called by the whole warp.
+__device__ __forceinline__ bool clip_tile_of(const IdTables& T, uint32_t b, uint32_t e, uint32_t lane) {
+    bool clip_tile = false;
+    for (uint32_t p0 = b; p0 < e && !clip_tile; p0 += 32u) {
+        const uint32_t p = p0 + lane;
+        clip_tile = __any_sync(kFullMask, p < e && (T.recs[p].flags0 & kFlagClipish) != 0u);
+    }
+    return clip_tile;
+}
+
+// The ID walk of every tile: sink(ids, ty, tx, lane) gets the lane's eight IDs (shared memory) of
+// the tile in row ty, column tx. IDs are the entries' layers, FORMA_ID_NONE where no layer hits.
+template <class Sink>
+__device__ __forceinline__ void ids_walk(const PaintScene& S, const IdTables& T, uint32_t n_tiles, float min_cov, Sink sink) {
+    __shared__ __align__(16) IdWarpSmem s_warp[kIdWarpsPerBlock];
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+    IdWarpSmem& W = s_warp[warp];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) W.cells[k * 32 + lane] = 0u;
+    __syncwarp();
+
+    TileTickets tickets(S, T, n_tiles, lane);
+    uint32_t tid, b, e;
+    for (bool tile; tickets.next(tile, tid, b, e);) {
+        if (!tile) continue;
+        const uint32_t ty = tid / S.tiles_x, tx = tid - ty * S.tiles_x;
+        const bool clip_tile = clip_tile_of(T, b, e, lane);
+
+        uint32_t* out = W.ids + 8u * lane;  // this lane's eight pixels
+#pragma unroll
+        for (int j = 0; j < 8; ++j) out[j] = FORMA_ID_NONE;
+        float cov[8];
+        if (!clip_tile) {
+            uint32_t open = 0xFFu;  // this lane's pixels without a hit yet
+            bool done = e == b;
+            for (uint32_t hi = e; hi > b && !done;) {
+                const uint32_t lo = hi - b >= 32u ? hi - 32u : b;
+                stage_group(W, T, lo, hi - lo, false, lane);
+                for (uint32_t k = hi - lo; k-- > 0u;) {
+                    const EntryRec& h = W.hdr[k];
+                    const uint32_t flags = h.pad;
+                    if (flags & kFlagMaskedOut) continue;
+                    if (flags & kFlagFull) {  // an unclipped Draw entry of coverage 1 everywhere
+#pragma unroll
+                        for (int j = 0; j < 8; ++j)
+                            if ((open >> j) & 1u) out[j] = h.layer;
+                        done = true;
+                        break;
+                    }
+                    entry_coverage(W, h, T.segs, lane, cov);
+#pragma unroll
+                    for (int j = 0; j < 8; ++j)
+                        if (((open >> j) & 1u) && cov[j] > min_cov) {
+                            out[j] = h.layer;
+                            open &= ~(1u << j);
+                        }
+                    if (__all_sync(kFullMask, open == 0u)) {
+                        done = true;
+                        break;
+                    }
+                }
+                hi = lo;
+            }
+        } else {
+            if (lane == 0) skip_trivial_clips_ids(T.recs, T.id_flags, b, e);
+            __syncwarp();
+            // The painter's first layer (skip_fully_covered_layers): the top-most visible full,
+            // unclipped, opaque entry.
+            uint32_t first = b;
+            for (uint32_t hi = e; hi > b;) {
+                const uint32_t lo = hi - b >= 32u ? hi - 32u : b;
+                bool cand = false;
+                if (lo + lane < hi) {
+                    const uint32_t f = T.id_flags[lo + lane];
+                    const bool clipped = (f & kFlagClippedDraw) && !(f & kFlagSkipClip);
+                    cand = !(f & kFlagMaskedOut) && !clipped && (f & kFlagFull) && (f & kFlagOpaque);
+                }
+                const uint32_t m = __ballot_sync(kFullMask, cand);
+                if (m) {
+                    first = lo + 31u - (uint32_t)__clz((int)m);
+                    break;
+                }
+                hi = lo;
+            }
+            bool clip_active = false;
+            uint32_t clip_last = 0;
+            for (uint32_t p0 = first; p0 < e; p0 += 32u) {
+                const uint32_t cnt = min(32u, e - p0);
+                stage_group(W, T, p0, cnt, true, lane);
+                for (uint32_t k = 0; k < cnt; ++k) {
+                    const EntryRec& h = W.hdr[k];
+                    const uint32_t flags = h.pad;
+                    if (flags & kFlagMaskedOut) continue;
+                    const uint32_t layer = h.layer, meta = h.meta;
+                    if (clip_active && clip_last < layer) clip_active = false;  // mod.rs:302-306
+                    const bool is_clip = ((meta >> 1) & 1u) != 0u;
+                    const bool apply_clip = !is_clip && ((meta >> 2) & 1u) && !(flags & kFlagSkipClip);
+                    if (!is_clip && !apply_clip && (flags & kFlagFull)) {
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) out[j] = layer;
+                        continue;
+                    }
+                    if (apply_clip && !clip_active) continue;  // mod.rs:317-323
+                    entry_coverage(W, h, T.segs, lane, cov);
+                    if (is_clip) {  // clip_at, mod.rs:449-464
+                        if (!clip_active) {
+                            clip_active = true;
+                            clip_last = layer + h.clip_layers;
+                        }
+                        float4* m4 = reinterpret_cast<float4*>(W.clip);
+                        m4[2u * lane] = make_float4(cov[0], cov[1], cov[2], cov[3]);
+                        m4[2u * lane + 1u] = make_float4(cov[4], cov[5], cov[6], cov[7]);
+                        __syncwarp();
+                        continue;
+                    }
+                    if (apply_clip) {
+                        const float4* m4 = reinterpret_cast<const float4*>(W.clip);
+                        const float4 m0 = m4[2u * lane], m1 = m4[2u * lane + 1u];
+                        const float m[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) cov[j] = __fmul_rn(cov[j], m[j]);
+                    }
+#pragma unroll
+                    for (int j = 0; j < 8; ++j)
+                        if (cov[j] > min_cov) out[j] = layer;
+                }
+            }
+        }
+        sink(out, ty, tx, lane);
+    }
+}
+
+// The ID frame's sink: the lane's eight IDs of tile (tx, ty), less `base` (a batch frame's order
+// base), into the frame.
+__device__ __forceinline__ void store_ids(const PaintScene& S, const IdsOut& f, const uint32_t* out, uint32_t ty, uint32_t tx,
+                                          uint32_t lane, uint32_t base) {
+    const uint32_t py = ty * 16u + (lane >> 1), x0 = tx * 16u + (lane & 1u) * 8u;
+    if (py >= S.height || x0 >= S.width) return;
+    const uint4 a = reinterpret_cast<const uint4*>(out)[0], c = reinterpret_cast<const uint4*>(out)[1];
+    uint32_t v[8] = {a.x, a.y, a.z, a.w, c.x, c.y, c.z, c.w};
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+        if (v[j] != FORMA_ID_NONE) v[j] -= base;
+    uint32_t* rowp = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(f.ids) + (size_t)py * f.stride) + x0;
+    const bool vec_ok = ((reinterpret_cast<uintptr_t>(f.ids) | (uintptr_t)f.stride) & 15u) == 0u;
+    if (vec_ok && x0 + 8u <= S.width) {
+        reinterpret_cast<uint4*>(rowp)[0] = make_uint4(v[0], v[1], v[2], v[3]);
+        reinterpret_cast<uint4*>(rowp)[1] = make_uint4(v[4], v[5], v[6], v[7]);
+    } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+            if (x0 + (uint32_t)j < S.width) rowp[j] = v[j];
+    }
+}
+
+__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) paint_ids_kernel(PaintScene S, IdTables T, IdsOut f, uint32_t n_tiles) {
+    ids_walk(S, T, n_tiles, f.min_coverage,
+             [&](const uint32_t* ids, uint32_t ty, uint32_t tx, uint32_t lane) { store_ids(S, f, ids, ty, tx, lane, 0u); });
 }
 // S stacks the frames of a batch, `rows` tile rows each; frame c's entries carry
 // frames[c].order_base + order, and the IDs stored are the frame's own orders.
-__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) paint_ids_stacked_kernel(PaintScene S, IdInputs in, uint32_t n_tiles,
+__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) paint_ids_stacked_kernel(PaintScene S, IdTables T, IdsOut f, uint32_t n_tiles,
                                                                                   uint32_t rows, const BatchFrame* __restrict__ frames) {
-#define FORMA_IDS_REBASE(out, ty) rebase_ids(out, frames[(ty) / rows].order_base)
-#include "paint_ids_body.cuh"
-#undef FORMA_IDS_REBASE
+    ids_walk(S, T, n_tiles, f.min_coverage, [&](const uint32_t* ids, uint32_t ty, uint32_t tx, uint32_t lane) {
+        store_ids(S, f, ids, ty, tx, lane, frame_row(ty, rows, frames).base);
+    });
 }
 
-// CTAs of `kernel` that fill the device (one occupancy query per device and kernel).
-template <class Kernel>
-static uint32_t id_grid_limit(Kernel kernel, int (&blocks_per_sm)[kMaxDevices]) {
-    static std::mutex config_mu;
-    std::lock_guard<std::mutex> lk(config_mu);
-    int& slot = blocks_per_sm[current_device_index()];
-    if (!slot) {
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&slot, kernel, kIdWarpsPerBlock * 32, 0);
-        if (slot < 1) slot = 1;
-    }
-    return (uint32_t)(slot * device_sm_count());
+static IdTables id_tables(const PaintScene& S, const TileTables& t, uint8_t* id_flags, uint32_t* tile_counter) {
+    return IdTables{t.segs, t.recs, t.tile_range, t.heavy, t.heavy_count, S.tiles_x * S.tiles_y, id_flags, tile_counter};
 }
 
-void launch_paint_ids(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range,
-                      const uint32_t* heavy, const uint32_t* heavy_count, uint8_t* id_flags, uint32_t* ids, size_t ids_stride,
+void launch_paint_ids(const PaintScene& S, const TileTables& t, uint8_t* id_flags, uint32_t* ids, size_t ids_stride,
                       float min_coverage, uint32_t* tile_counter, cudaStream_t st, uint32_t rows, const BatchFrame* frames) {
-    if (S.tx_hi <= S.tx_lo || S.ty_hi <= S.ty_lo) return;
-    const uint32_t n_tiles = (S.tx_hi - S.tx_lo) * (S.ty_hi - S.ty_lo);
-    cudaMemsetAsync(tile_counter, 0, sizeof(uint32_t), st);
-    IdInputs in{segs, recs, tile_range, heavy, heavy_count, S.tiles_x * S.tiles_y, id_flags, ids, ids_stride, min_coverage,
-                tile_counter};
-    static int blocks_per_sm[2][kMaxDevices] = {{0}};
-    const uint32_t need = (n_tiles + kIdWarpsPerBlock - 1) / kIdWarpsPerBlock;
-    if (frames) {
-        const uint32_t want = id_grid_limit(paint_ids_stacked_kernel, blocks_per_sm[1]);
-        paint_ids_stacked_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles, rows, frames);
-    } else {
-        const uint32_t want = id_grid_limit(paint_ids_kernel, blocks_per_sm[0]);
-        paint_ids_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles);
-    }
+    const void* kernel = frames ? (const void*)paint_ids_stacked_kernel : (const void*)paint_ids_kernel;
+    const TileGrid g = tile_grid(S, kernel, kIdWarpsPerBlock, tile_counter, st);
+    if (!g.n_tiles) return;
+    const IdTables T = id_tables(S, t, id_flags, tile_counter);
+    const IdsOut f{ids, ids_stride, min_coverage};
+    if (frames) paint_ids_stacked_kernel<<<g.ctas, kIdWarpsPerBlock * 32, 0, st>>>(S, T, f, g.n_tiles, rows, frames);
+    else paint_ids_kernel<<<g.ctas, kIdWarpsPerBlock * 32, 0, st>>>(S, T, f, g.n_tiles);
 }
 
 // ---------------------------------------------------------------------------
 // Layer coverage masks (forma_renderer_render_masks): plane k of a frame holds, per pixel, the
 // coverage of order o = first_order + k as paint_layer computes it, times the clip mask where a
 // clip applies to o. Amodal: every layer of the tile is walked, none is skipped below an opaque
-// one. The same warp scheme as the ID kernel (tickets, heavy lists first, lane = the painter's
-// eight pixels), with entry_coverage, stage_group and skip_trivial_clips_ids reused as they are.
+// one. The same warp scheme as the ID kernel (TileTickets, lane = the painter's eight pixels), with
+// entry_coverage, stage_group and skip_trivial_clips_ids reused as they are.
 //
 // Tiles without clip-ish entries: the entries are sorted by layer, so the walk bisects to the
 // window's first entry and stops at its end; nothing outside the window is read. Tiles with
@@ -227,14 +437,11 @@ void launch_paint_ids(const PaintScene& S, const uint64_t* segs, const EntryRec*
 // Only tiles with window entries are stored, and each such entry stores its own plane: the zero
 // fill before the kernel (zero_masks_kernel) gives every other pixel its 0.
 // ---------------------------------------------------------------------------
-struct MaskInputs {
-    IdInputs t;  // tables, id_flags and ticket counter (t.ids, t.ids_stride and t.min_coverage unused)
-    uint8_t* out;
-    uint64_t stride, plane_stride;
-    uint32_t first_order, n_orders;
-    uint32_t height;  // rows of one frame
-    uint32_t rows;    // stacks: tile rows per frame; 0: a single frame
-    bool u8;
+
+// A lane's part of a tile of the amodal walk: the tile's frame, its row fty in the frame and its
+// column tx; the lane's frame row py, first column x0 and its n_px pixels inside the frame.
+struct LaneTile {
+    uint32_t frame, fty, tx, py, x0, n_px, lane;
 };
 
 // compute_srgb's alpha encode (paint_math.cuh: to_byte) of a coverage in [0, 1].
@@ -243,9 +450,13 @@ __device__ __forceinline__ uint32_t mask_byte(float v) {
     return __float_as_uint(scaled + __uint_as_float(0x4B000000u)) & 0xFFu;
 }
 
-// The lane's eight values at `p` (its first pixel of plane row), n <= 8 of them inside the frame.
-__device__ __forceinline__ void store_mask(uint8_t* p, const float cov[8], uint32_t n, bool u8, bool vec_ok) {
-    if (u8) {
+// The mask planes' sink: the lane's eight values of window order k into plane k of the tile's frame.
+__device__ __forceinline__ void store_mask(const OrderWindow& w, const MaskOut& m, const LaneTile& t, uint32_t k, const float cov[8]) {
+    const uint32_t n = t.n_px;
+    if (!n) return;
+    const bool vec_ok = ((reinterpret_cast<uintptr_t>(m.ptr) | (uintptr_t)m.stride | (uintptr_t)m.plane_stride) & (m.u8 ? 7u : 15u)) == 0u;
+    uint8_t* p = m.ptr + ((size_t)t.frame * w.n_orders + k) * m.plane_stride + (size_t)t.py * m.stride + (size_t)t.x0 * (m.u8 ? 1u : 4u);
+    if (m.u8) {
         uint32_t lo = 0, hi = 0;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
@@ -281,13 +492,6 @@ __device__ __forceinline__ void store_mask(uint8_t* p, const float cov[8], uint3
 // order of the atomics. Boxes start as {~0, ~0, 0, 0} (min / max sentinels) and
 // fix_stats_kernel turns the box of an empty set into {0, 0, 0, 0} at the end.
 // ---------------------------------------------------------------------------
-struct StatsOut {
-    forma_layer_stats* rec;  // n_frames x n_orders records
-    uint32_t first_order, n_orders;
-    uint32_t height;  // rows of one frame
-    uint32_t rows;    // stacks: tile rows per frame; 0: a single frame
-    float min_cov;
-};
 
 // Widens `box` (x0, y0, x1, y1) to hold [x0, x1) x [y0, y1). Bounds only move outwards, so a
 // relaxed read that finds one already as wide skips its atomic (a stale read only costs an atomic).
@@ -299,14 +503,16 @@ __device__ __forceinline__ void widen_box(uint32_t* box, uint32_t x0, uint32_t y
     if (y1 > hi.y) atomicMax(box + 3, y1);
 }
 
-// The amodal statistics of one (tile, entry): the lane's eight values cov (n_px of them in the
-// frame, from column x0 of frame row py) into `r`. `full`: a kFlagFull entry that no clip mask
-// scales, 1 on the tile's whole in-frame rectangle [tx0, tx0 + tw) x [ty0, ty0 + th), taken without
-// a reduction. Called by the whole warp.
-__device__ __forceinline__ void add_amodal(forma_layer_stats* r, const float cov[8], bool full, uint32_t n_px, uint32_t x0,
-                                           uint32_t py, uint32_t tx0, uint32_t tw, uint32_t ty0, uint32_t th, float min_cov,
-                                           uint32_t lane) {
+// The amodal statistics' sink: the lane's eight values cov of window order k into the record of
+// (frame, k). `full`: a kFlagFull entry that no clip mask scales, 1 on the tile's whole in-frame
+// rectangle, taken without a reduction. Called by the whole warp.
+__device__ __forceinline__ void add_amodal(const PaintScene& S, const OrderWindow& w, const StatsOut& so, const LaneTile& t,
+                                           uint32_t k, const float cov[8], bool full) {
+    const uint32_t lane = t.lane;
+    forma_layer_stats* r = so.rec + (size_t)t.frame * w.n_orders + k;
     if (full) {
+        const uint32_t tx0 = t.tx * 16u, ty0 = t.fty * 16u;
+        const uint32_t tw = tx0 < S.width ? min(16u, S.width - tx0) : 0u, th = ty0 < w.height ? min(16u, w.height - ty0) : 0u;
         if (lane == 0 && tw && th) {
             atomicAdd(reinterpret_cast<unsigned long long*>(&r->area), (unsigned long long)(tw * th) << 18);
             atomicAdd(&r->pixels, tw * th);
@@ -317,12 +523,12 @@ __device__ __forceinline__ void add_amodal(forma_layer_stats* r, const float cov
     uint32_t units = 0, cnt = 0, xl = ~0u, xh = 0;
 #pragma unroll
     for (uint32_t j = 0; j < 8u; ++j) {
-        if (j >= n_px) continue;
+        if (j >= t.n_px) continue;
         units += (uint32_t)(cov[j] * 262144.0f);  // exact: v x 2^18 is an integer <= 2^18
-        if (cov[j] > min_cov) {
+        if (cov[j] > so.min_coverage) {
             ++cnt;
-            xl = min(xl, x0 + j);
-            xh = x0 + j + 1u;
+            xl = min(xl, t.x0 + j);
+            xh = t.x0 + j + 1u;
         }
     }
     units = __reduce_add_sync(kFullMask, units);  // <= 256 x 2^18
@@ -331,8 +537,8 @@ __device__ __forceinline__ void add_amodal(forma_layer_stats* r, const float cov
         xl = __reduce_min_sync(kFullMask, xl);
         xh = __reduce_max_sync(kFullMask, xh);
     }
-    const uint32_t yl = n ? __reduce_min_sync(kFullMask, cnt ? py : ~0u) : 0u;
-    const uint32_t yh = n ? __reduce_max_sync(kFullMask, cnt ? py + 1u : 0u) : 0u;
+    const uint32_t yl = n ? __reduce_min_sync(kFullMask, cnt ? t.py : ~0u) : 0u;
+    const uint32_t yh = n ? __reduce_max_sync(kFullMask, cnt ? t.py + 1u : 0u) : 0u;
     if (lane == 0) {
         if (units) atomicAdd(reinterpret_cast<unsigned long long*>(&r->area), (unsigned long long)units);
         if (n) {
@@ -342,22 +548,22 @@ __device__ __forceinline__ void add_amodal(forma_layer_stats* r, const float cov
     }
 }
 
-// The visible statistics of one tile (tile row ty, column tx) from the ID walk's eight IDs `out` of
-// each lane (tile row `row`, half hx): one reduction per distinct window ID of the tile. `frames`: a batch, whose IDs carry
-// the frame's order base. Called by the whole warp.
-__device__ __forceinline__ void add_visible(const PaintScene& S, const StatsOut& so, const uint32_t* out, uint32_t ty, uint32_t tx,
-                                            uint32_t row, uint32_t hx, uint32_t lane, const BatchFrame* __restrict__ frames) {
-    const uint32_t frame = so.rows ? ty / so.rows : 0u, fty = so.rows ? ty - frame * so.rows : ty;
-    const uint32_t lo_w = (frames ? frames[frame].order_base : 0u) + so.first_order;
-    const uint32_t py = fty * 16u + row, x0 = tx * 16u + hx * 8u;
-    const uint32_t n_px = py < so.height && x0 < S.width ? min(8u, S.width - x0) : 0u;
+// The visible statistics' sink: the tile's (row ty, column tx) IDs `out`, eight of each lane, one
+// reduction per distinct window ID of the tile. `frames`: a batch, whose IDs carry the frame's
+// order base. Called by the whole warp.
+__device__ __forceinline__ void add_visible(const PaintScene& S, const OrderWindow& w, const StatsOut& so, const uint32_t* out,
+                                            uint32_t ty, uint32_t tx, uint32_t lane, const BatchFrame* __restrict__ frames) {
+    const FrameRow fr = frame_row(ty, w.rows, frames);
+    const uint32_t lo_w = fr.base + w.first_order;
+    const uint32_t py = fr.fty * 16u + (lane >> 1), x0 = tx * 16u + (lane & 1u) * 8u;
+    const uint32_t n_px = py < w.height && x0 < S.width ? min(8u, S.width - x0) : 0u;
     uint32_t k[8], pend = 0;  // window indices; the lane's pixels not reduced yet
 #pragma unroll
     for (uint32_t j = 0; j < 8u; ++j) {
         k[j] = out[j] - lo_w;  // (FORMA_ID_NONE and orders outside the window land at >= n_orders)
-        if (j < n_px && k[j] < so.n_orders) pend |= 1u << j;
+        if (j < n_px && k[j] < w.n_orders) pend |= 1u << j;
     }
-    forma_layer_stats* rec = so.rec + (size_t)frame * so.n_orders;
+    forma_layer_stats* rec = so.rec + (size_t)fr.frame * w.n_orders;
     for (;;) {
         const uint32_t any = __ballot_sync(kFullMask, pend != 0u);
         if (!any) break;
@@ -389,77 +595,33 @@ __device__ __forceinline__ void add_visible(const PaintScene& S, const StatsOut&
     }
 }
 
-// kStats: the amodal statistics (add_amodal into so) in place of the planes; `in` then only
-// gives the tables and the window.
-template <bool kBatch, bool kStats = false>
-__device__ __forceinline__ void paint_masks_body(const PaintScene& S, const MaskInputs& in, uint32_t n_tiles,
-                                                 const BatchFrame* __restrict__ frames, const StatsOut& so = StatsOut{}) {
+// The amodal walk of every tile with entries: sink(t, k, cov, full) gets the lane's eight values of
+// each window entry of order first_order + k; `full`: cov is a kFlagFull entry's 1 everywhere.
+// `frames`: a batch, whose entries carry the frame's order base.
+template <class Sink>
+__device__ __forceinline__ void amodal_walk(const PaintScene& S, const IdTables& T, const OrderWindow& w, uint32_t n_tiles,
+                                            const BatchFrame* __restrict__ frames, Sink sink) {
     __shared__ __align__(16) IdWarpSmem s_warp[kIdWarpsPerBlock];
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
     IdWarpSmem& W = s_warp[warp];
-    const IdInputs& T = in.t;
-    const uint32_t ntx = S.tx_hi - S.tx_lo;
     const uint32_t row = lane >> 1, hx = lane & 1u;
-    const uint32_t bpp = in.u8 ? 1u : 4u;
-    const bool vec_ok = ((reinterpret_cast<uintptr_t>(in.out) | (uintptr_t)in.stride | (uintptr_t)in.plane_stride) &
-                         (in.u8 ? 7u : 15u)) == 0u;
 #pragma unroll
     for (int k = 0; k < 8; ++k) W.cells[k * 32 + lane] = 0u;
     __syncwarp();
 
-    uint32_t hcount[kHeavyClasses], H = 0;
-#pragma unroll
-    for (int c = 0; c < kHeavyClasses; ++c) {
-        hcount[c] = T.heavy ? T.heavy_count[c] : 0u;
-        H += hcount[c];
-    }
-    const uint32_t n_tickets = H + n_tiles;
-    for (;;) {
-        uint32_t ticket = 0;
-        if (lane == 0) ticket = atomicAdd(T.tile_counter, 1u);
-        ticket = __shfl_sync(kFullMask, ticket, 0);
-        if (ticket >= n_tickets) break;
-        uint32_t tid;
-        if (ticket < H) {  // the heavy lists, largest class first (as in the ID kernel)
-            uint32_t t = ticket;
-            int c = kHeavyClasses - 1;
-#pragma unroll
-            for (int q = kHeavyClasses - 1; q > 0; --q)
-                if (c == q && t >= hcount[q]) {
-                    t -= hcount[q];
-                    c = q - 1;
-                }
-            tid = T.heavy[(size_t)c * T.n_tiles_total + t];
-            const uint32_t ty = tid / S.tiles_x, tx = tid - ty * S.tiles_x;
-            if (ty < S.ty_lo || ty >= S.ty_hi || tx < S.tx_lo || tx >= S.tx_hi) continue;
-        } else {
-            const uint32_t lin = ticket - H;
-            tid = (S.ty_lo + lin / ntx) * S.tiles_x + S.tx_lo + lin % ntx;
-        }
-        const uint2 range = T.tile_range[tid];
-        const uint32_t b = range.x, e = range.y;
-        if (ticket >= H && T.heavy && e - b >= kHeavyMin) continue;  // done from its list
+    TileTickets tickets(S, T, n_tiles, lane);
+    uint32_t tid, b, e;
+    for (bool tile; tickets.next(tile, tid, b, e);) {
+        if (!tile) continue;
         if (e == b) continue;
         const uint32_t ty = tid / S.tiles_x, tx = tid - ty * S.tiles_x;
-        const uint32_t frame = in.rows ? ty / in.rows : 0u, fty = in.rows ? ty - frame * in.rows : ty;
-        const uint32_t base = kBatch ? frames[frame].order_base : 0u;
-        const uint32_t lo_w = base + in.first_order, hi_w = lo_w + in.n_orders;  // the window in the entries' layer space
-        const uint32_t py = fty * 16u + row, x0 = tx * 16u + hx * 8u;
-        const bool inside = py < in.height && x0 < S.width;
-        const uint32_t n_px = inside ? min(8u, S.width - x0) : 0u;
-        uint8_t* const px = in.out + ((size_t)frame * in.n_orders) * in.plane_stride + (size_t)py * in.stride + (size_t)x0 * bpp;
+        const FrameRow fr = frame_row(ty, w.rows, frames);
+        const uint32_t lo_w = fr.base + w.first_order, hi_w = lo_w + w.n_orders;  // the window in the entries' layer space
+        const uint32_t py = fr.fty * 16u + row, x0 = tx * 16u + hx * 8u;
+        const LaneTile t{fr.frame, fr.fty, tx, py, x0, py < w.height && x0 < S.width ? min(8u, S.width - x0) : 0u, lane};
         float cov[8];
-        bool full = false;  // cov is a kFlagFull entry's 1 everywhere (kStats)
-        auto put = [&](uint32_t layer) {
-            if constexpr (kStats) {
-                const uint32_t tx0 = tx * 16u, ty0 = fty * 16u;
-                const uint32_t tw = tx0 < S.width ? min(16u, S.width - tx0) : 0u, th = ty0 < in.height ? min(16u, in.height - ty0) : 0u;
-                add_amodal(so.rec + (size_t)frame * in.n_orders + (layer - lo_w), cov, full, n_px, x0, py, tx0, tw, ty0, th,
-                           so.min_cov, lane);
-            } else if (inside) {
-                store_mask(px + (size_t)(layer - lo_w) * in.plane_stride, cov, n_px, in.u8, vec_ok);
-            }
-        };
+        bool full = false;
+        auto put = [&](uint32_t layer) { sink(t, layer - lo_w, cov, full); };
         auto coverage = [&](const EntryRec& h) {
             full = (h.pad & kFlagFull) != 0u;
             if (h.pad & kFlagFull) {  // no segments, a full carried cover: coverage 1 without reading anything
@@ -470,13 +632,7 @@ __device__ __forceinline__ void paint_masks_body(const PaintScene& S, const Mask
             }
         };
 
-        bool clip_tile = false;
-        for (uint32_t p0 = b; p0 < e && !clip_tile; p0 += 32u) {
-            const uint32_t p = p0 + lane;
-            clip_tile = __any_sync(kFullMask, p < e && (T.recs[p].flags0 & kFlagClipish) != 0u);
-        }
-
-        if (!clip_tile) {
+        if (!clip_tile_of(T, b, e, lane)) {
             uint32_t lo = b, hi = e;  // the first entry of the window
             while (lo < hi) {
                 const uint32_t mid = (lo + hi) >> 1;
@@ -564,14 +720,15 @@ __device__ __forceinline__ void paint_masks_body(const PaintScene& S, const Mask
     }
 }
 
-__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) paint_masks_kernel(PaintScene S, MaskInputs in, uint32_t n_tiles) {
-    paint_masks_body<false>(S, in, n_tiles, nullptr);
+__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) paint_masks_kernel(PaintScene S, IdTables T, OrderWindow w, MaskOut m,
+                                                                            uint32_t n_tiles) {
+    amodal_walk(S, T, w, n_tiles, nullptr, [&](const LaneTile& t, uint32_t k, const float* cov, bool) { store_mask(w, m, t, k, cov); });
 }
 // S stacks the frames of a batch; frame c's entries carry frames[c].order_base + order, and its
 // planes hold the frame's own orders.
-__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) paint_masks_stacked_kernel(PaintScene S, MaskInputs in, uint32_t n_tiles,
-                                                                                    const BatchFrame* __restrict__ frames) {
-    paint_masks_body<true>(S, in, n_tiles, frames);
+__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) paint_masks_stacked_kernel(PaintScene S, IdTables T, OrderWindow w, MaskOut m,
+                                                                                    uint32_t n_tiles, const BatchFrame* __restrict__ frames) {
+    amodal_walk(S, T, w, n_tiles, frames, [&](const LaneTile& t, uint32_t k, const float* cov, bool) { store_mask(w, m, t, k, cov); });
 }
 
 // Zeroes `row_bytes` bytes from byte x0 of rows [y0, y0 + n_rows) of n_planes planes: one warp per
@@ -594,10 +751,11 @@ __global__ void __launch_bounds__(kZeroWarps * 32) zero_masks_kernel(uint8_t* ou
     }
 }
 
-uint32_t launch_paint_masks(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range,
-                            const uint32_t* heavy, const uint32_t* heavy_count, uint8_t* id_flags, const MaskFrame& m,
-                            uint32_t* tile_counter, cudaStream_t st, uint32_t rows, const BatchFrame* frames) {
-    if (S.tx_hi <= S.tx_lo || S.ty_hi <= S.ty_lo) return 0;
+uint32_t launch_paint_masks(const PaintScene& S, const TileTables& t, uint8_t* id_flags, const MaskFrame& m, uint32_t* tile_counter,
+                            cudaStream_t st, uint32_t rows, const BatchFrame* frames) {
+    const void* kernel = frames ? (const void*)paint_masks_stacked_kernel : (const void*)paint_masks_kernel;
+    const TileGrid g = tile_grid(S, kernel, kIdWarpsPerBlock, tile_counter, st);
+    if (!g.n_tiles) return 0;
     const uint32_t bpp = m.format == FORMA_MASK_U8 ? 1u : 4u;
     // The written rectangle: a stack's frames whole, a single frame's tile rectangle clipped to it.
     const uint32_t y0 = rows ? 0u : S.ty_lo * 16u, y1 = rows ? m.height : min(S.ty_hi * 16u, S.height);
@@ -606,45 +764,39 @@ uint32_t launch_paint_masks(const PaintScene& S, const uint64_t* segs, const Ent
     const uint32_t zero_ctas = (uint32_t)std::min<uint64_t>((n_rows + kZeroWarps - 1) / kZeroWarps, 8u * (uint64_t)device_sm_count());
     zero_masks_kernel<<<zero_ctas, kZeroWarps * 32, 0, st>>>(m.ptr, m.stride, m.plane_stride, m.n_frames * m.n_orders, y0, y1 - y0,
                                                              (uint64_t)x0 * bpp, (uint64_t)(x1 - x0) * bpp);
-    const uint32_t n_tiles = (S.tx_hi - S.tx_lo) * (S.ty_hi - S.ty_lo);
-    cudaMemsetAsync(tile_counter, 0, sizeof(uint32_t), st);
-    MaskInputs in{IdInputs{segs, recs, tile_range, heavy, heavy_count, S.tiles_x * S.tiles_y, id_flags, nullptr, 0, 0.0f, tile_counter},
-                  m.ptr, m.stride, m.plane_stride, m.first_order, m.n_orders, m.height, rows, m.format == FORMA_MASK_U8};
-    static int blocks_per_sm[2][kMaxDevices] = {{0}};
-    const uint32_t need = (n_tiles + kIdWarpsPerBlock - 1) / kIdWarpsPerBlock;
-    if (frames) {
-        const uint32_t want = id_grid_limit(paint_masks_stacked_kernel, blocks_per_sm[1]);
-        paint_masks_stacked_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles, frames);
-    } else {
-        const uint32_t want = id_grid_limit(paint_masks_kernel, blocks_per_sm[0]);
-        paint_masks_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles);
-    }
+    const IdTables T = id_tables(S, t, id_flags, tile_counter);
+    const OrderWindow w{m.first_order, m.n_orders, m.height, rows};
+    const MaskOut out{m.ptr, m.stride, m.plane_stride, m.format == FORMA_MASK_U8};
+    if (frames) paint_masks_stacked_kernel<<<g.ctas, kIdWarpsPerBlock * 32, 0, st>>>(S, T, w, out, g.n_tiles, frames);
+    else paint_masks_kernel<<<g.ctas, kIdWarpsPerBlock * 32, 0, st>>>(S, T, w, out, g.n_tiles);
     return 2;
 }
 
 // The statistics kernels (see add_amodal / add_visible above): the amodal walk of the mask kernel
-// and the visible walk of the ID kernel, each single-frame / views and batch.
-__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_amodal_kernel(PaintScene S, MaskInputs in, uint32_t n_tiles,
-                                                                             StatsOut so) {
-    paint_masks_body<false, true>(S, in, n_tiles, nullptr, so);
+// and the ID walk of the ID kernel, each single-frame / views and batch.
+__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_amodal_kernel(PaintScene S, IdTables T, OrderWindow w, StatsOut so,
+                                                                             uint32_t n_tiles) {
+    amodal_walk(S, T, w, n_tiles, nullptr,
+                [&](const LaneTile& t, uint32_t k, const float* cov, bool full) { add_amodal(S, w, so, t, k, cov, full); });
 }
-__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_amodal_stacked_kernel(PaintScene S, MaskInputs in, uint32_t n_tiles,
-                                                                                     StatsOut so,
+__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_amodal_stacked_kernel(PaintScene S, IdTables T, OrderWindow w,
+                                                                                     StatsOut so, uint32_t n_tiles,
                                                                                      const BatchFrame* __restrict__ frames) {
-    paint_masks_body<true, true>(S, in, n_tiles, frames, so);
+    amodal_walk(S, T, w, n_tiles, frames,
+                [&](const LaneTile& t, uint32_t k, const float* cov, bool full) { add_amodal(S, w, so, t, k, cov, full); });
 }
-__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_visible_kernel(PaintScene S, IdInputs in, uint32_t n_tiles,
-                                                                              StatsOut so) {
-#define FORMA_IDS_SINK(out, ty, tx, row, hx) add_visible(S, so, out, ty, tx, row, hx, lane, nullptr)
-#include "paint_ids_body.cuh"
-#undef FORMA_IDS_SINK
+__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_visible_kernel(PaintScene S, IdTables T, OrderWindow w, StatsOut so,
+                                                                              uint32_t n_tiles) {
+    ids_walk(S, T, n_tiles, so.min_coverage, [&](const uint32_t* ids, uint32_t ty, uint32_t tx, uint32_t lane) {
+        add_visible(S, w, so, ids, ty, tx, lane, nullptr);
+    });
 }
-__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_visible_stacked_kernel(PaintScene S, IdInputs in, uint32_t n_tiles,
-                                                                                      StatsOut so,
+__global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_visible_stacked_kernel(PaintScene S, IdTables T, OrderWindow w,
+                                                                                      StatsOut so, uint32_t n_tiles,
                                                                                       const BatchFrame* __restrict__ frames) {
-#define FORMA_IDS_SINK(out, ty, tx, row, hx) add_visible(S, so, out, ty, tx, row, hx, lane, frames)
-#include "paint_ids_body.cuh"
-#undef FORMA_IDS_SINK
+    ids_walk(S, T, n_tiles, so.min_coverage, [&](const uint32_t* ids, uint32_t ty, uint32_t tx, uint32_t lane) {
+        add_visible(S, w, so, ids, ty, tx, lane, frames);
+    });
 }
 
 // Every record to 0 with the boxes' min / max sentinels {~0, ~0, 0, 0}.
@@ -668,37 +820,25 @@ __global__ void fix_stats_kernel(forma_layer_stats* rec, uint64_t n) {
     }
 }
 
-uint32_t launch_paint_stats(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range,
-                            const uint32_t* heavy, const uint32_t* heavy_count, uint8_t* id_flags, const StatsFrame& f,
-                            uint32_t* tile_counter, cudaStream_t st, uint32_t rows, const BatchFrame* frames) {
+uint32_t launch_paint_stats(const PaintScene& S, const TileTables& t, uint8_t* id_flags, const StatsFrame& f, uint32_t* tile_counter,
+                            cudaStream_t st, uint32_t rows, const BatchFrame* frames) {
     const uint64_t n_rec = (uint64_t)f.n_frames * f.n_orders;
     const uint32_t rec_ctas = (uint32_t)std::min<uint64_t>((n_rec + 255u) / 256u, 8u * (uint64_t)device_sm_count());
     init_stats_kernel<<<rec_ctas, 256, 0, st>>>(f.ptr, n_rec);
     uint32_t launches = 2;
-    if (S.tx_hi > S.tx_lo && S.ty_hi > S.ty_lo) {
-        const uint32_t n_tiles = (S.tx_hi - S.tx_lo) * (S.ty_hi - S.ty_lo);
-        const IdInputs t{segs, recs, tile_range, heavy, heavy_count, S.tiles_x * S.tiles_y, id_flags, nullptr, 0, f.min_coverage,
-                         tile_counter};
-        const MaskInputs in{t, nullptr, 0, 0, f.first_order, f.n_orders, f.height, rows, false};
-        const StatsOut so{f.ptr, f.first_order, f.n_orders, f.height, rows, f.min_coverage};
-        static int blocks_per_sm[4][kMaxDevices] = {{0}};
-        const uint32_t need = (n_tiles + kIdWarpsPerBlock - 1) / kIdWarpsPerBlock;
-        cudaMemsetAsync(tile_counter, 0, sizeof(uint32_t), st);
-        if (frames) {
-            const uint32_t want = id_grid_limit(stats_amodal_stacked_kernel, blocks_per_sm[1]);
-            stats_amodal_stacked_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles, so, frames);
-        } else {
-            const uint32_t want = id_grid_limit(stats_amodal_kernel, blocks_per_sm[0]);
-            stats_amodal_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles, so);
-        }
-        cudaMemsetAsync(tile_counter, 0, sizeof(uint32_t), st);
-        if (frames) {
-            const uint32_t want = id_grid_limit(stats_visible_stacked_kernel, blocks_per_sm[3]);
-            stats_visible_stacked_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, t, n_tiles, so, frames);
-        } else {
-            const uint32_t want = id_grid_limit(stats_visible_kernel, blocks_per_sm[2]);
-            stats_visible_kernel<<<min(want, need), kIdWarpsPerBlock * 32, 0, st>>>(S, t, n_tiles, so);
-        }
+    const IdTables T = id_tables(S, t, id_flags, tile_counter);
+    const OrderWindow w{f.first_order, f.n_orders, f.height, rows};
+    const StatsOut so{f.ptr, f.min_coverage};
+    const uint32_t block = kIdWarpsPerBlock * 32;
+    const void* amodal = frames ? (const void*)stats_amodal_stacked_kernel : (const void*)stats_amodal_kernel;
+    const TileGrid g = tile_grid(S, amodal, kIdWarpsPerBlock, tile_counter, st);
+    if (g.n_tiles) {
+        if (frames) stats_amodal_stacked_kernel<<<g.ctas, block, 0, st>>>(S, T, w, so, g.n_tiles, frames);
+        else stats_amodal_kernel<<<g.ctas, block, 0, st>>>(S, T, w, so, g.n_tiles);
+        const void* visible = frames ? (const void*)stats_visible_stacked_kernel : (const void*)stats_visible_kernel;
+        const TileGrid v = tile_grid(S, visible, kIdWarpsPerBlock, tile_counter, st);
+        if (frames) stats_visible_stacked_kernel<<<v.ctas, block, 0, st>>>(S, T, w, so, v.n_tiles, frames);
+        else stats_visible_kernel<<<v.ctas, block, 0, st>>>(S, T, w, so, v.n_tiles);
         launches += 2;
     }
     fix_stats_kernel<<<rec_ctas, 256, 0, st>>>(f.ptr, n_rec);

@@ -35,7 +35,9 @@
 // tail unless it starts early (longest-processing-time order).
 #include <cuda_fp16.h>
 
+#include <map>
 #include <mutex>
+
 #include "paint_common.cuh"
 #include "paint_math.cuh"
 #include "srgb_decode.h"
@@ -764,108 +766,74 @@ void launch_f32x2_selftest(const float* a, const float* b, const float* c, uint3
     f32x2_selftest_kernel<<<(n / 2 + 255) / 256, 256, 0, st>>>(a, b, c, n, out);
 }
 
-void launch_paint(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range, const uint32_t* heavy,
-                  const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st,
-                  uint32_t view_rows, bool solid_over) {
-    if (S.tx_hi <= S.tx_lo || S.ty_hi <= S.ty_lo) return;
-    uint32_t n_tiles = (S.tx_hi - S.tx_lo) * (S.ty_hi - S.ty_lo);
+// Several host threads may render on one device, and paint_kernel<8> and paint_kernel<6> share a
+// type: the occupancy cache is keyed by the kernel's address and the device, under one lock.
+TileGrid tile_grid(const PaintScene& S, const void* kernel, uint32_t warps, uint32_t* tile_counter, cudaStream_t st) {
+    if (S.tx_hi <= S.tx_lo || S.ty_hi <= S.ty_lo) return TileGrid{0u, 0u};
+    const uint32_t n_tiles = (S.tx_hi - S.tx_lo) * (S.ty_hi - S.ty_lo);
     cudaMemsetAsync(tile_counter, 0, sizeof(uint32_t), st);
-    PaintInputs in{segs, recs, tile_range, heavy, heavy_count, S.tiles_x * S.tiles_y, eflags, framebuffer, tile_counter};
-    // Persistent warps: enough CTAs to fill every SM at the kernel's occupancy (per device).
+    static std::mutex mu;
+    static std::map<std::pair<const void*, int>, int> blocks_per_sm;
+    int per_sm = 0;
+    {
+        std::lock_guard<std::mutex> lk(mu);
+        int& slot = blocks_per_sm[{kernel, current_device_index()}];
+        if (!slot) {
+            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&slot, kernel, (int)warps * 32, 0);
+            if (slot < 1) slot = 1;
+        }
+        per_sm = slot;
+    }
+    return TileGrid{n_tiles, min((uint32_t)(per_sm * device_sm_count()), (n_tiles + warps - 1u) / warps)};
+}
+
+static PaintInputs paint_inputs(const PaintScene& S, const TileTables& t, uint8_t* eflags, uint8_t* framebuffer,
+                                uint32_t* tile_counter) {
+    return PaintInputs{t.segs, t.recs, t.tile_range, t.heavy, t.heavy_count, S.tiles_x * S.tiles_y, eflags, framebuffer, tile_counter};
+}
+
+void launch_paint(const PaintScene& S, const TileTables& t, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter,
+                  cudaStream_t st, uint32_t view_rows, bool solid_over) {
     // Build 0: the general kernel at 128 registers (8 CTAs / SM); 1: option paint_wide = 1, up to 168
     // registers (6 CTAs / SM); 2: a solid `Over` frame (option paint_solid = 1), the lean build at 96
     // registers (10 CTAs / SM).
-    static int blocks_per_sm[2][3][kMaxDevices] = {{{0}}};
-    static std::mutex config_mu;  // several host threads may render on one device
-    const int build = solid_over && options().paint_solid ? 2 : options().paint_wide ? 1 : 0, views = view_rows ? 1 : 0;
-    const void* kernels[2][3] = {{(const void*)paint_kernel<8>, (const void*)paint_kernel<6>, (const void*)paint_solid_kernel<8>},
-                                 {(const void*)paint_views_kernel<8>, (const void*)paint_views_kernel<6>, (const void*)paint_views_solid_kernel<8>}};
-    int per_sm = 0;
-    {
-        std::lock_guard<std::mutex> lk(config_mu);
-        int& slot = blocks_per_sm[views][build][current_device_index()];
-        if (!slot) {
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&slot, kernels[views][build], kPaintWarpsPerBlock * 32, 0);
-            if (slot < 1) slot = 1;
-        }
-        per_sm = slot;
-    }
-    const uint32_t want = (uint32_t)(per_sm * device_sm_count());
-    const uint32_t need = (n_tiles + kPaintWarpsPerBlock - 1) / kPaintWarpsPerBlock;
-    const dim3 grid(min(want, need)), block(kPaintWarpsPerBlock * 32);
-    if (views) {
-        switch (build) {
-            case 0: paint_views_kernel<8><<<grid, block, 0, st>>>(S, in, n_tiles, view_rows); break;
-            case 1: paint_views_kernel<6><<<grid, block, 0, st>>>(S, in, n_tiles, view_rows); break;
-            default: paint_views_solid_kernel<8><<<grid, block, 0, st>>>(S, in, n_tiles, view_rows); break;
-        }
-    } else {
-        switch (build) {
-            case 0: paint_kernel<8><<<grid, block, 0, st>>>(S, in, n_tiles); break;
-            case 1: paint_kernel<6><<<grid, block, 0, st>>>(S, in, n_tiles); break;
-            default: paint_solid_kernel<8><<<grid, block, 0, st>>>(S, in, n_tiles); break;
-        }
-    }
+    const int build = solid_over && options().paint_solid ? 2 : options().paint_wide ? 1 : 0;
+    void (*const frame[3])(PaintScene, PaintInputs, uint32_t) = {paint_kernel<8>, paint_kernel<6>, paint_solid_kernel<8>};
+    void (*const views[3])(PaintScene, PaintInputs, uint32_t, uint32_t) = {paint_views_kernel<8>, paint_views_kernel<6>,
+                                                                            paint_views_solid_kernel<8>};
+    const void* kernel = view_rows ? (const void*)views[build] : (const void*)frame[build];
+    const TileGrid g = tile_grid(S, kernel, kPaintWarpsPerBlock, tile_counter, st);
+    if (!g.n_tiles) return;
+    const PaintInputs in = paint_inputs(S, t, eflags, framebuffer, tile_counter);
+    if (view_rows) views[build]<<<g.ctas, kPaintWarpsPerBlock * 32, 0, st>>>(S, in, g.n_tiles, view_rows);
+    else frame[build]<<<g.ctas, kPaintWarpsPerBlock * 32, 0, st>>>(S, in, g.n_tiles);
 }
 
-void launch_paint_linear(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range, const uint32_t* heavy,
-                         const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st,
-                         uint32_t view_rows, uint32_t bpp) {
-    if (S.tx_hi <= S.tx_lo || S.ty_hi <= S.ty_lo) return;
-    const uint32_t n_tiles = (S.tx_hi - S.tx_lo) * (S.ty_hi - S.ty_lo);
-    cudaMemsetAsync(tile_counter, 0, sizeof(uint32_t), st);
-    PaintInputs in{segs, recs, tile_range, heavy, heavy_count, S.tiles_x * S.tiles_y, eflags, framebuffer, tile_counter};
-    // Persistent warps, as in launch_paint.
-    static int blocks_per_sm[2][kMaxDevices] = {{0}};
-    static std::mutex config_mu;
-    const int views = view_rows ? 1 : 0;
-    int per_sm = 0;
-    {
-        std::lock_guard<std::mutex> lk(config_mu);
-        int& slot = blocks_per_sm[views][current_device_index()];
-        if (!slot) {
-            const void* k = views ? (const void*)paint_views_linear_kernel : (const void*)paint_linear_kernel;
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&slot, k, kPaintWarpsPerBlock * 32, 0);
-            if (slot < 1) slot = 1;
-        }
-        per_sm = slot;
-    }
-    const uint32_t grid = min((uint32_t)(per_sm * device_sm_count()), (n_tiles + kPaintWarpsPerBlock - 1) / kPaintWarpsPerBlock);
-    if (views) paint_views_linear_kernel<<<grid, kPaintWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles, view_rows, bpp);
-    else paint_linear_kernel<<<grid, kPaintWarpsPerBlock * 32, 0, st>>>(S, in, n_tiles, bpp);
+void launch_paint_linear(const PaintScene& S, const TileTables& t, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter,
+                         cudaStream_t st, uint32_t view_rows, uint32_t bpp) {
+    const void* kernel = view_rows ? (const void*)paint_views_linear_kernel : (const void*)paint_linear_kernel;
+    const TileGrid g = tile_grid(S, kernel, kPaintWarpsPerBlock, tile_counter, st);
+    if (!g.n_tiles) return;
+    const PaintInputs in = paint_inputs(S, t, eflags, framebuffer, tile_counter);
+    if (view_rows) paint_views_linear_kernel<<<g.ctas, kPaintWarpsPerBlock * 32, 0, st>>>(S, in, g.n_tiles, view_rows, bpp);
+    else paint_linear_kernel<<<g.ctas, kPaintWarpsPerBlock * 32, 0, st>>>(S, in, g.n_tiles, bpp);
 }
 
-void launch_paint_over(const PaintScene& S, const uint64_t* segs, const EntryRec* recs, const uint2* tile_range, const uint32_t* heavy,
-                       const uint32_t* heavy_count, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter, cudaStream_t st,
-                       uint32_t view_rows, uint32_t bpp) {
-    if (S.tx_hi <= S.tx_lo || S.ty_hi <= S.ty_lo) return;
-    const uint32_t n_tiles = (S.tx_hi - S.tx_lo) * (S.ty_hi - S.ty_lo);
-    cudaMemsetAsync(tile_counter, 0, sizeof(uint32_t), st);
-    PaintInputs in{segs, recs, tile_range, heavy, heavy_count, S.tiles_x * S.tiles_y, eflags, framebuffer, tile_counter};
-    // Persistent warps, as in launch_paint.
-    static int blocks_per_sm[2][2][kMaxDevices] = {{{0}}};
-    static std::mutex config_mu;
-    const int views = view_rows ? 1 : 0, linear = bpp == 4u ? 0 : 1;
-    const void* kernels[2][2] = {{(const void*)paint_over_kernel, (const void*)paint_over_linear_kernel},
-                                 {(const void*)paint_views_over_kernel, (const void*)paint_views_over_linear_kernel}};
-    int per_sm = 0;
-    {
-        std::lock_guard<std::mutex> lk(config_mu);
-        int& slot = blocks_per_sm[views][linear][current_device_index()];
-        if (!slot) {
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&slot, kernels[views][linear], kPaintWarpsPerBlock * 32, 0);
-            if (slot < 1) slot = 1;
-        }
-        per_sm = slot;
-    }
-    const uint32_t grid = min((uint32_t)(per_sm * device_sm_count()), (n_tiles + kPaintWarpsPerBlock - 1) / kPaintWarpsPerBlock);
+void launch_paint_over(const PaintScene& S, const TileTables& t, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter,
+                       cudaStream_t st, uint32_t view_rows, uint32_t bpp) {
+    const bool linear = bpp != 4u;
+    const void* kernel = view_rows ? (linear ? (const void*)paint_views_over_linear_kernel : (const void*)paint_views_over_kernel)
+                                   : (linear ? (const void*)paint_over_linear_kernel : (const void*)paint_over_kernel);
+    const TileGrid g = tile_grid(S, kernel, kPaintWarpsPerBlock, tile_counter, st);
+    if (!g.n_tiles) return;
+    const PaintInputs in = paint_inputs(S, t, eflags, framebuffer, tile_counter);
     const uint32_t block = kPaintWarpsPerBlock * 32;
-    if (views) {
-        if (linear) paint_views_over_linear_kernel<<<grid, block, 0, st>>>(S, in, n_tiles, view_rows, bpp);
-        else paint_views_over_kernel<<<grid, block, 0, st>>>(S, in, n_tiles, view_rows);
+    if (view_rows) {
+        if (linear) paint_views_over_linear_kernel<<<g.ctas, block, 0, st>>>(S, in, g.n_tiles, view_rows, bpp);
+        else paint_views_over_kernel<<<g.ctas, block, 0, st>>>(S, in, g.n_tiles, view_rows);
     } else {
-        if (linear) paint_over_linear_kernel<<<grid, block, 0, st>>>(S, in, n_tiles, bpp);
-        else paint_over_kernel<<<grid, block, 0, st>>>(S, in, n_tiles);
+        if (linear) paint_over_linear_kernel<<<g.ctas, block, 0, st>>>(S, in, g.n_tiles, bpp);
+        else paint_over_kernel<<<g.ctas, block, 0, st>>>(S, in, g.n_tiles);
     }
 }
 

@@ -129,6 +129,15 @@ __device__ __forceinline__ void scatter_entry(const uint64_t* __restrict__ segs,
     if (n > 64u) scatter_rest(segs, s0 + 64u, s1, cells, lane);
 }
 
+// The grid of a persistent tile kernel (paint, ID, mask and statistics kernels) over the tile
+// rectangle of S: n_tiles = 0 for an empty rectangle (launch nothing); otherwise `tile_counter` is
+// reset on `st` and ctas = min(resident CTAs x SMs, ceil(n_tiles / warps)), the kernel's occupancy
+// at `warps` warps per CTA being queried once per kernel and device (kernels_painter.cu).
+struct TileGrid {
+    uint32_t n_tiles, ctas;
+};
+TileGrid tile_grid(const PaintScene& S, const void* kernel, uint32_t warps, uint32_t* tile_counter, cudaStream_t st);
+
 // Cells that cannot influence a painted tile (rows outside the painted band,
 // columns right of it) get this key in both pair sorts: it sorts last and keeps
 // the sort keys inside host-known bounds (tile_y field = tiles_y + 1).

@@ -486,7 +486,9 @@ int Renderer::run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p
     last_tiles_y = S.tiles_y;
     FORMA_CUDA_TRY(tile_range.reserve(n_tiles_total));
     FORMA_CUDA_TRY(heavy_tiles.reserve(n_tiles_total * kHeavyListClasses));
-    // Heavy tiles first (longest-processing-time order): their lists + counts (heavy_count()).
+    // Heavy tiles first (longest-processing-time order): their lists + counts (heavy_count()). The
+    // tile kernels read them with the rest of the tables (TileTables), taken after build_tables,
+    // which may move any of them.
     uint32_t* const heavy_lists = options().paint_lpt ? heavy_tiles.ptr : nullptr;
     // Tables + paint + output, once or (rarely) twice. sync_free = without count read-backs: the
     // tables of a frame are normally about as large as those of the frame before, so every
@@ -508,7 +510,7 @@ int Renderer::run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p
         st = queue_row_costs(S, n);
         if (st) return st;
         FORMA_CUDA_TRY(cudaEventRecord(timer.ev[4], stream));
-        st = paint_step(q, S, p, heavy_lists, &paint_launches);
+        st = paint_step(q, S, p, TileTables{segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count()}, &paint_launches);
         if (st) return st;
         FORMA_CUDA_TRY(cudaEventRecord(timer.ev[5], stream));
         st = output_step(q, S, p);
@@ -891,7 +893,7 @@ int Renderer::bind_batch(Composition* const* comps, uint32_t n, PaintScene& S, u
 // The frame's kernels: paint() for the RGBA target (in copy bands, or with the rows of a stack's
 // frames), then the ID kernel for the ID target, or the mask or statistics kernels. The sync-free
 // redo repeats them all.
-int Renderer::paint_step(const FrameRequest& q, const PaintScene& S, const FramePlan& p, const uint32_t* heavy_lists,
+int Renderer::paint_step(const FrameRequest& q, const PaintScene& S, const FramePlan& p, const TileTables& t,
                          uint32_t* paint_launches) {
     if (q.rgba.ptr) {
         bool solid_over = true;
@@ -907,8 +909,8 @@ int Renderer::paint_step(const FrameRequest& q, const PaintScene& S, const Frame
             ++launches;
             FORMA_CUDA_TRY(cudaGetLastError());
         }
-        const int st = paint(S, p.rgba.ptr, q.rgba.ptr, q.rgba.stride, p.in_bands, heavy_lists, paint_launches, p.rows, q.rgba.bpp,
-                             solid_over, q.rgba.over);
+        const int st = paint(S, t, p.rgba.ptr, q.rgba.ptr, q.rgba.stride, p.in_bands, paint_launches, p.rows, q.rgba.bpp, solid_over,
+                             q.rgba.over);
         if (st || (!q.ids.ptr && !q.masks.ptr && !q.stats.ptr)) return st;
         if (q.ids.ptr) ++*paint_launches;
     }
@@ -917,8 +919,7 @@ int Renderer::paint_step(const FrameRequest& q, const PaintScene& S, const Frame
     if (q.masks.ptr) {  // the zero fill of the planes, then the masks (the redo of a sync-free frame repeats both)
         const MaskFrame m{p.masks.ptr, p.masks.stride, p.mask_plane_stride, q.masks.first_order, q.masks.n_orders, q.masks.format,
                           (uint32_t)q.height, q.kind == FrameKind::single ? 1u : q.n};
-        const uint32_t n = launch_paint_masks(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), id_flags.ptr, m,
-                                              totals.ptr + 8, stream, p.rows, frames);
+        const uint32_t n = launch_paint_masks(S, t, id_flags.ptr, m, totals.ptr + 8, stream, p.rows, frames);
         launches += n;
         *paint_launches = q.rgba.ptr ? *paint_launches + n : n;
         FORMA_CUDA_TRY(cudaGetLastError());
@@ -927,16 +928,15 @@ int Renderer::paint_step(const FrameRequest& q, const PaintScene& S, const Frame
     if (q.stats.ptr) {  // the records' initialisation, both walks, the empty boxes (the redo of a sync-free frame repeats all)
         const StatsFrame f{p.stats, q.stats.first_order, q.stats.n_orders, q.stats.min_coverage, (uint32_t)q.height,
                            q.kind == FrameKind::single ? 1u : q.n};
-        const uint32_t n = launch_paint_stats(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), id_flags.ptr, f,
-                                              totals.ptr + 8, stream, p.rows, frames);
+        const uint32_t n = launch_paint_stats(S, t, id_flags.ptr, f, totals.ptr + 8, stream, p.rows, frames);
         launches += n;
         *paint_launches = q.rgba.ptr ? *paint_launches + n : n;
         FORMA_CUDA_TRY(cudaGetLastError());
         return FORMA_STATUS_OK;
     }
     // A batch's entries carry each frame's order base (bind_batch): the kernel takes it off.
-    launch_paint_ids(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), id_flags.ptr, reinterpret_cast<uint32_t*>(p.ids.ptr),
-                     p.ids.stride, q.ids.min_coverage, totals.ptr + 8, stream, p.rows, frames);
+    launch_paint_ids(S, t, id_flags.ptr, reinterpret_cast<uint32_t*>(p.ids.ptr), p.ids.stride, q.ids.min_coverage, totals.ptr + 8, stream,
+                     p.rows, frames);
     ++launches;
     FORMA_CUDA_TRY(cudaGetLastError());
     return FORMA_STATUS_OK;
@@ -1245,12 +1245,11 @@ int Renderer::queue_row_costs(const PaintScene& S, uint32_t n) {
 // bpp: bytes per pixel of fb, 4 (sRGB8), or 8 / 16 for a linear float frame (never in bands).
 // solid_over: see launch_paint (sRGB8 frames; a float frame is painted by the general build).
 // over: paint over fb's own pixels (launch_paint_over), in any of the three formats.
-int Renderer::paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t stride, bool in_bands, const uint32_t* heavy_lists,
+int Renderer::paint(const PaintScene& S, const TileTables& t, uint8_t* fb, uint8_t* buffer, uint64_t stride, bool in_bands,
                     uint32_t* paint_launches, uint32_t view_rows, uint32_t bpp, bool solid_over, bool over) {
     *paint_launches = 1;
     if (over) {  // (never in bands: an over frame is on the device)
-        launch_paint_over(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), eflags.ptr, fb, totals.ptr + 3, stream,
-                          view_rows, bpp);
+        launch_paint_over(S, t, eflags.ptr, fb, totals.ptr + 3, stream, view_rows, bpp);
         ++launches;
     } else if (in_bands) {
         if (!band_streams_ok) {
@@ -1271,8 +1270,7 @@ int Renderer::paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t 
             Sb.ty_hi = S.ty_lo + paint_rows * (k + 1u) / kCopyBands;
             cudaStream_t bs = kCopyBands > 1u ? band_stream[k] : stream;
             if (kCopyBands > 1u) FORMA_CUDA_TRY(cudaStreamWaitEvent(bs, band_ev[kMaxCopyBands], 0));
-            launch_paint(Sb, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), eflags.ptr, fb, totals.ptr + 16 + k, bs, 0,
-                         solid_over);
+            launch_paint(Sb, t, eflags.ptr, fb, totals.ptr + 16 + k, bs, 0, solid_over);
             ++launches;
             const int st = copy_to_host(Sb, buffer, fb, stride, bs);
             if (st) return st;
@@ -1281,12 +1279,10 @@ int Renderer::paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t 
         for (uint32_t k = 0; kCopyBands > 1u && k < kCopyBands; ++k) FORMA_CUDA_TRY(cudaStreamWaitEvent(stream, band_ev[k], 0));
         *paint_launches = kCopyBands;
     } else if (bpp == 4u) {
-        launch_paint(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), eflags.ptr, fb, totals.ptr + 3, stream, view_rows,
-                     solid_over);
+        launch_paint(S, t, eflags.ptr, fb, totals.ptr + 3, stream, view_rows, solid_over);
         ++launches;
     } else {
-        launch_paint_linear(S, segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count(), eflags.ptr, fb, totals.ptr + 3, stream,
-                            view_rows, bpp);
+        launch_paint_linear(S, t, eflags.ptr, fb, totals.ptr + 3, stream, view_rows, bpp);
         ++launches;
     }
     FORMA_CUDA_TRY(cudaGetLastError());

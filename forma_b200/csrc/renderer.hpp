@@ -331,8 +331,7 @@ class Renderer {
     // One frame of S: uploads, line setup, sort, then the painter tables, paint_step and
     // output_step once or, when the sync-free bounds were too small, twice.
     int run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p);
-    int paint_step(const FrameRequest& q, const PaintScene& S, const FramePlan& p, const uint32_t* heavy_lists,
-                   uint32_t* paint_launches);
+    int paint_step(const FrameRequest& q, const PaintScene& S, const FramePlan& p, const TileTables& t, uint32_t* paint_launches);
     int output_step(const FrameRequest& q, const PaintScene& S, const FramePlan& p);
     DeviceBuffer<uint8_t> id_flags;   // per entry: the ID kernel's optimizer flags (clip tiles)
     DeviceBuffer<uint32_t> id_frame;  // the ID target's scratch frame
@@ -363,7 +362,7 @@ class Renderer {
     int build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint32_t prev_cells, uint32_t prev_gaps, uint32_t* heavy_lists,
                      DevCounts& dc, const BatchArgs* batch);
     int queue_row_costs(const PaintScene& S, uint32_t n);
-    int paint(const PaintScene& S, uint8_t* fb, uint8_t* buffer, uint64_t stride, bool in_bands, const uint32_t* heavy_lists,
+    int paint(const PaintScene& S, const TileTables& t, uint8_t* fb, uint8_t* buffer, uint64_t stride, bool in_bands,
               uint32_t* paint_launches, uint32_t view_rows = 0, uint32_t bpp = 4, bool solid_over = false, bool over = false);
     int copy_to_host(const PaintScene& S, uint8_t* buffer, const uint8_t* fb, uint64_t stride, cudaStream_t s, uint32_t bpp = 4);
     int scatter_written_tiles(const PaintScene& S, const uint8_t* fb, uint8_t* buffer, uint64_t stride);
