@@ -496,9 +496,11 @@ int Renderer::run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p
     // from device memory (DevCounts); the host looks at them only after the frame's final
     // synchronisation. A count above its bound (the kernels then did nothing, the frame holds
     // the clear colour) sends the frame through again with counted tables.
-    // (pack_written: the host scatter of the written tiles must not see a frame that is redone.)
+    // A frame with a layer cache is never sync-free: its first attempt would write the clear colour
+    // into the caller's buffer and record it in the cache's tiles, and the redo would then skip the
+    // tiles it finds unchanged (and the host scatter of the written tiles must not see a redone frame).
     const uint32_t prev_cells = last_cells, prev_gaps = last_gaps;  // of this renderer's previous frame
-    const bool fast = options().sync_free && n > 0 && prev_cells > 0 && !p.pack_written;
+    const bool fast = options().sync_free && n > 0 && prev_cells > 0 && !q.cache;
     last_cells = last_entries = 0;
     last_written_tiles = 0;
     last_tables_redone = false;

@@ -176,7 +176,9 @@ int forma_layer_is_enabled(forma_layer*);                                       
 /* GeomPresTransform::try_from([ux, vx, uy, vy, tx, ty]) + Layer::set_transform
  * (math/transform.rs:196-221, layer.rs:289); INVALID_ARGUMENT if it scales up. */
 int forma_layer_set_transform(forma_composition*, forma_layer*, const float t[6]);
-int forma_layer_set_props(forma_composition*, forma_layer*, const forma_props*);   /* layer.rs:341 */
+/* layer.rs:341. Equal props leave the layer unchanged for every layer cache; a texture whose
+ * texels (as f16) equal the layer's current texture is the same image. */
+int forma_layer_set_props(forma_composition*, forma_layer*, const forma_props*);
 
 /* ------------------------------------------------------------------------ */
 /* Renderer (forma/src/cpu/renderer.rs:56-224)                              */
@@ -207,8 +209,14 @@ int forma_renderer_render(forma_renderer*, forma_composition*, uint8_t* buffer, 
 
 /* Same contract, but `device_buffer` is a CUDA device pointer on the
  * renderer's device (e.g. a torch tensor's data_ptr()): no device->host copy.
- * With `reuse_geometry` != 0 and an unchanged composition the points/layer
- * tables already resident in HBM are reused (SURVEY.md §8 N3). */
+ * With a cache, the tiles the frame does not write keep the caller's bytes, as in
+ * a host buffer, and so do the bytes between rows and outside the crop. A frame
+ * with a cache builds its painter tables with the counts read back: it never takes
+ * the sync-free path (option sync_free), whose first attempt could write the clear
+ * colour into tiles the cache then finds unchanged.
+ * Cache ids are per renderer (Renderer::create_buffer_layer_cache) while the
+ * unchanged bits live on the layers: caches of two renderers that have the same
+ * id share those bits, as in the reference. */
 int forma_renderer_render_device(forma_renderer*, forma_composition*, uint8_t* device_buffer,
                                  uint64_t width, uint64_t width_stride, uint64_t height,
                                  const uint32_t channels[4], const float clear_color[4],

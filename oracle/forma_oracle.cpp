@@ -397,6 +397,12 @@ int fo_layer_set_props(void* c, void* layer, const fo_props* p) {
         size_t n = (size_t)p->tex_width * p->tex_height;
         auto data = std::make_shared<std::vector<uint16_t>>(n * 4);
         for (size_t i = 0; i < n * 4; ++i) (*data)[i] = f16_from(p->tex_linear_rgba[i]);
+        // The same texels set again on a layer are the same image (the C ABI has no other way to
+        // name an Image, whose PartialEq is by data pointer): the layer stays unchanged.
+        const Props& old = ((Layer*)layer)->props;
+        if (old.func == kDraw && old.fill_type == kTexture && old.texture.image.data && old.texture.image.width == p->tex_width &&
+            *old.texture.image.data == *data)
+            data = old.texture.image.data;
         Texture& t = props.texture;
         t.image.data = data;
         t.image.width = p->tex_width;

@@ -34,7 +34,11 @@ def paint_solid_restored(cuda_api):
 def painters(fn):
     """The paint kernels (lean "solid" / "general") that ran during fn(). fn is called again when
     the profiler delivered no paint kernel at all (its activity records of a short session can go
-    missing); every call renders the same frame."""
+    missing); every call renders the same frame. The session stays open for a moment after the
+    frame: a session stopped right after the synchronisation can lose the record of the frame's
+    last kernel, the paint kernel of a host frame."""
+    import time
+
     import torch
     from torch.profiler import ProfilerActivity, profile
     out = set()
@@ -43,6 +47,7 @@ def painters(fn):
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             fn()
             torch.cuda.synchronize()
+            time.sleep(0.01)
         for n in {e.key for e in prof.key_averages()}:
             if "paint_solid_kernel" in n or "paint_views_solid_kernel" in n:
                 out.add("solid")
