@@ -216,6 +216,36 @@ class _CStats(C.Structure):  # forma_stats
     _fields_ = [("ptr", C.c_void_p), ("first_order", C.c_uint32), ("n_orders", C.c_uint32), ("min_coverage", C.c_float)]
 
 
+class _CPoses(C.Structure):  # forma_poses
+    _fields_ = [("first_order", C.c_uint32), ("n_orders", C.c_uint32), ("transforms", C.c_void_p), ("visible", C.c_void_p)]
+
+
+class Poses:
+    """The per-frame layer states of a poses call (see include/forma_b200.h: forma_poses): in frame
+    b, the layer at order first_order + k takes transforms[b, k] ([n, K, 6] float32, set_transform
+    order [ux, vx, uy, vy, tx, ty]) and is enabled where visible[b, k] ([n, K] bool / uint8) is
+    non-zero. Either table may be None (that state stays the layer's own), not both; with both, n
+    and K must agree."""
+
+    def __init__(self, first_order: int, transforms=None, visible=None):
+        if transforms is None and visible is None:
+            raise ValueError("Poses: transforms, visible or both")
+        self.first_order = int(first_order)
+        self.transforms = None if transforms is None else np.ascontiguousarray(np.asarray(transforms, dtype=np.float32))
+        self.visible = None if visible is None else np.ascontiguousarray(np.asarray(visible).astype(np.uint8))
+        if self.transforms is not None and (self.transforms.ndim != 3 or self.transforms.shape[2] != 6):
+            raise ValueError(f"Poses: transforms of shape {self.transforms.shape}, not [n, K, 6]")
+        if self.visible is not None and self.visible.ndim != 2:
+            raise ValueError(f"Poses: visible of shape {self.visible.shape}, not [n, K]")
+        shapes = {t.shape[:2] for t in (self.transforms, self.visible) if t is not None}
+        if len(shapes) != 1:
+            raise ValueError(f"Poses: transforms and visible disagree on [n, K]: {sorted(shapes)}")
+        self.n, self.n_orders = shapes.pop()
+
+    def __len__(self) -> int:
+        return self.n
+
+
 # forma_layer_stats, one 48-byte record per frame and order (see include/forma_b200.h).
 STATS_DTYPE = np.dtype([("area", np.uint64), ("pixels", np.uint32), ("visible", np.uint32), ("box", np.uint32, (4,)),
                         ("visible_box", np.uint32, (4,))])
@@ -357,6 +387,18 @@ SIGNATURES = {
                                                      C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
     "renderer_render_batch_stats_device": (C.c_int, [_vp, C.POINTER(_vp), C.c_uint32, C.POINTER(_CStats), C.c_uint64, C.c_uint64,
                                                      _vp, C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
+    "renderer_render_poses": (C.c_int, [_vp, _vp, C.POINTER(_CPoses), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
+                                        _u32p, _fp, C.POINTER(_CTimings)]),
+    "renderer_render_poses_device": (C.c_int, [_vp, _vp, C.POINTER(_CPoses), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64,
+                                               C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
+    "renderer_render_poses_ids": (C.c_int, [_vp, _vp, C.POINTER(_CPoses), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64,
+                                            C.c_uint64, _f, C.POINTER(_CTimings)]),
+    "renderer_render_poses_ids_device": (C.c_int, [_vp, _vp, C.POINTER(_CPoses), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64,
+                                                   C.c_uint64, _u32p, _fp, _vp, C.c_uint64, C.c_uint64, _f, C.POINTER(_CTimings)]),
+    "renderer_render_poses_masks_device": (C.c_int, [_vp, _vp, C.POINTER(_CPoses), C.c_uint32, C.POINTER(_CMasks), C.c_uint64,
+                                                     C.c_uint64, _vp, C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
+    "renderer_render_poses_stats_device": (C.c_int, [_vp, _vp, C.POINTER(_CPoses), C.c_uint32, C.POINTER(_CStats), C.c_uint64,
+                                                     C.c_uint64, _vp, C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
     "renderer_launch_count": (C.c_uint64, [_vp]),
     "renderer_stage_times": (None, [_vp, C.POINTER(C.c_double)]),
     "renderer_counters": (None, [_vp, _u64p]),
@@ -421,6 +463,10 @@ MASK_SYMBOLS = ("renderer_render_masks", "renderer_render_masks_device", "render
 # render_batch_stats_device).
 STATS_SYMBOLS = ("renderer_render_stats", "renderer_render_stats_device", "renderer_render_views_stats_device",
                  "renderer_render_batch_stats_device")
+# The same for poses (Renderer.render_poses, render_poses_device, render_poses_ids{,_device},
+# render_poses_masks_device, render_poses_stats_device).
+POSE_SYMBOLS = ("renderer_render_poses", "renderer_render_poses_device", "renderer_render_poses_ids",
+                "renderer_render_poses_ids_device", "renderer_render_poses_masks_device", "renderer_render_poses_stats_device")
 # Value formats of mask planes: name -> (FORMA_MASK_*, bytes per value, numpy dtype).
 MASK_FORMATS = {"f32": (0, 4, np.float32), "u8": (1, 1, np.uint8)}
 
@@ -453,7 +499,7 @@ def over_format(fmt: str):
 
 
 _OPTIONAL_SYMBOLS = frozenset(ID_FRAME_SYMBOLS + VIEW_SYMBOLS + BATCH_SYMBOLS + STACK_ID_SYMBOLS + SORT_DEBUG_SYMBOLS +
-                              LINEAR_SYMBOLS + OVER_SYMBOLS + MASK_SYMBOLS + STATS_SYMBOLS)
+                              LINEAR_SYMBOLS + OVER_SYMBOLS + MASK_SYMBOLS + STATS_SYMBOLS + POSE_SYMBOLS)
 
 
 class Api:
@@ -979,6 +1025,20 @@ class Renderer:
             return (_vp * max(len(part), 1))(*[c._h for c in part]), count
         return len(comps), args
 
+    @staticmethod
+    def _pose_args(composition, poses: Poses):
+        """(n, args) for _stack: a chunk's forma_poses holds its frames' rows of the tables."""
+        keep = []  # the chunk's descriptor and tables stay alive until the next one
+
+        def args(first, count):
+            t = None if poses.transforms is None else np.ascontiguousarray(poses.transforms[first:first + count])
+            v = None if poses.visible is None else np.ascontiguousarray(poses.visible[first:first + count])
+            d = _CPoses(poses.first_order, poses.n_orders, None if t is None else t.ctypes.data,
+                        None if v is None else v.ctypes.data)
+            keep[:] = [t, v, d]
+            return composition._h, C.byref(d), count
+        return poses.n, args
+
     def render_views(self, composition: Composition, views, buffer: np.ndarray, width: int, height: int, channels=RGBA,
                      clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
                      view_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
@@ -1368,6 +1428,74 @@ class Renderer:
         return self._stack_stats(self._api.renderer_render_batch_stats_device, "Renderer::render_batch_stats_device", args, n, stats_ptr,
                                  width, height, first_order, n_orders, min_coverage, rgba_ptr, channels, clear_color, rgba_stride,
                                  frame_stride, timings)
+
+    def render_poses(self, composition: Composition, poses: Poses, buffer: np.ndarray, width: int, height: int, channels=RGBA,
+                     clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
+                     view_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """One frame per pose (see Poses and include/forma_b200.h: forma_renderer_render_poses): frame b
+        is the composition with the window's layers set to pose b, which the call itself leaves
+        unchanged. Layout as for render_views; chunked like render_views."""
+        n, args = self._pose_args(composition, poses)
+        stride, view_stride = self._strides(width, height, stride, view_stride)
+        assert buffer.dtype == np.uint8 and buffer.flags["C_CONTIGUOUS"]
+        assert n == 0 or buffer.size >= (n - 1) * view_stride + (height - 1) * stride + 4 * width
+        return self._stack(self._api.renderer_render_poses, "Renderer::render_poses", args, n, width, height,
+                           (buffer.ctypes.data, stride, view_stride, channels, clear_color), None, timings)
+
+    def render_poses_device(self, composition: Composition, poses: Poses, device_ptr: int, width: int, height: int, channels=RGBA,
+                            clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
+                            view_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """render_poses into device memory: with the defaults, the data_ptr() of a contiguous
+        [N, height, width, 4] uint8 CUDA tensor."""
+        n, args = self._pose_args(composition, poses)
+        return self._stack(self._api.renderer_render_poses_device, "Renderer::render_poses_device", args, n, width, height,
+                           (int(device_ptr), stride, view_stride, channels, clear_color), None, timings)
+
+    def render_poses_ids(self, composition: Composition, poses: Poses, ids: np.ndarray, width: int, height: int,
+                         ids_stride: Optional[int] = None, ids_view_stride: Optional[int] = None, min_coverage: float = 0.0,
+                         timings: bool = True) -> Optional[Timings]:
+        """The ID frame (see render_ids) of every pose, in one pass; layout as for render_views_ids."""
+        n, args = self._pose_args(composition, poses)
+        s, fs = self._strides(width, height, ids_stride, ids_view_stride)
+        assert ids.dtype == np.uint32 and ids.flags["C_CONTIGUOUS"]
+        assert n == 0 or ids.size * 4 >= (n - 1) * fs + (height - 1) * s + 4 * width
+        return self._stack(self._api.renderer_render_poses_ids, "Renderer::render_poses_ids", args, n, width, height, None,
+                           (ids.ctypes.data, s, fs, min_coverage), timings)
+
+    def render_poses_ids_device(self, composition: Composition, poses: Poses, ids_device_ptr: int, width: int, height: int,
+                                rgba_ptr: Optional[int] = None, channels=RGBA, clear_color: Color = Color(1.0, 1.0, 1.0, 1.0),
+                                stride: Optional[int] = None, view_stride: Optional[int] = None, ids_stride: Optional[int] = None,
+                                ids_view_stride: Optional[int] = None, min_coverage: float = 0.0,
+                                timings: bool = True) -> Optional[Timings]:
+        """render_poses_ids into device memory, with the frames of render_poses_device as well when
+        `rgba_ptr` is given; layout as for render_views_ids_device."""
+        n, args = self._pose_args(composition, poses)
+        return self._stack(self._api.renderer_render_poses_ids_device, "Renderer::render_poses_ids_device", args, n, width, height,
+                           (None if rgba_ptr is None else int(rgba_ptr), stride, view_stride, channels, clear_color),
+                           (int(ids_device_ptr), ids_stride, ids_view_stride, min_coverage), timings)
+
+    def render_poses_masks_device(self, composition: Composition, poses: Poses, masks_ptr: int, width: int, height: int,
+                                  first_order: int, n_orders: int, format: str = "f32", stride: Optional[int] = None,
+                                  plane_stride: Optional[int] = None, rgba_ptr: Optional[int] = None, channels=RGBA,
+                                  clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), rgba_stride: Optional[int] = None,
+                                  view_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """The masks (see render_masks) of every pose, in one pass; layout as for
+        render_views_masks_device. The mask window and the pose window are independent."""
+        n, args = self._pose_args(composition, poses)
+        return self._stack_masks(self._api.renderer_render_poses_masks_device, "Renderer::render_poses_masks_device", args, n, masks_ptr,
+                                 width, height, first_order, n_orders, format, stride, plane_stride, rgba_ptr, channels, clear_color,
+                                 rgba_stride, view_stride, timings)
+
+    def render_poses_stats_device(self, composition: Composition, poses: Poses, stats_ptr: int, width: int, height: int,
+                                  first_order: int, n_orders: int, min_coverage: float = 0.0, rgba_ptr: Optional[int] = None,
+                                  channels=RGBA, clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), rgba_stride: Optional[int] = None,
+                                  view_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """The statistics (see render_stats) of every pose, in one pass; layout as for
+        render_views_stats_device. The statistics window and the pose window are independent."""
+        n, args = self._pose_args(composition, poses)
+        return self._stack_stats(self._api.renderer_render_poses_stats_device, "Renderer::render_poses_stats_device", args, n, stats_ptr,
+                                 width, height, first_order, n_orders, min_coverage, rgba_ptr, channels, clear_color, rgba_stride,
+                                 view_stride, timings)
 
     def launch_count(self) -> int:
         return int(self._api.renderer_launch_count(self._h))

@@ -449,6 +449,45 @@ int forma_renderer_render_views(forma_renderer* r, forma_composition* c, const f
     q.rgba = {host_buffer, false, width_stride, view_stride};
     return render_request(r, q, c);
 }
+// Poses: the twins of the views calls, with the pose tables in place of the view transforms.
+static FrameRequest poses_request(const forma_poses* poses, uint32_t n, uint64_t width, uint64_t height, const uint32_t* channels,
+                                  const float* clear_color, forma_timings* timings) {
+    FrameRequest q{FrameKind::poses, n, width, height, channels, clear_color, timings};
+    q.poses = poses;
+    return q;
+}
+int forma_renderer_render_poses_device(forma_renderer* r, forma_composition* c, const forma_poses* poses, uint32_t n,
+                                       uint8_t* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                       uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
+                                       forma_timings* timings) {
+    FrameRequest q = poses_request(poses, n, width, height, channels, clear_color, timings);
+    q.rgba = {device_buffer, true, width_stride, view_stride};
+    return render_request(r, q, c);
+}
+int forma_renderer_render_poses(forma_renderer* r, forma_composition* c, const forma_poses* poses, uint32_t n, uint8_t* host_buffer,
+                                uint64_t width, uint64_t width_stride, uint64_t height, uint64_t view_stride,
+                                const uint32_t channels[4], const float clear_color[4], forma_timings* timings) {
+    FrameRequest q = poses_request(poses, n, width, height, channels, clear_color, timings);
+    q.rgba = {host_buffer, false, width_stride, view_stride};
+    return render_request(r, q, c);
+}
+int forma_renderer_render_poses_ids_device(forma_renderer* r, forma_composition* c, const forma_poses* poses, uint32_t n,
+                                           uint8_t* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                           uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
+                                           uint32_t* device_ids, uint64_t ids_stride, uint64_t ids_view_stride, float min_coverage,
+                                           forma_timings* timings) {
+    FrameRequest q = poses_request(poses, n, width, height, channels, clear_color, timings);
+    q.rgba = {device_buffer, true, width_stride, view_stride};
+    q.ids = {reinterpret_cast<uint8_t*>(device_ids), true, ids_stride, ids_view_stride, min_coverage};
+    return render_request(r, q, c, nullptr, __func__);
+}
+int forma_renderer_render_poses_ids(forma_renderer* r, forma_composition* c, const forma_poses* poses, uint32_t n, uint32_t* host_ids,
+                                    uint64_t width, uint64_t ids_stride, uint64_t height, uint64_t ids_view_stride,
+                                    float min_coverage, forma_timings* timings) {
+    FrameRequest q = poses_request(poses, n, width, height, nullptr, nullptr, timings);
+    q.ids = {reinterpret_cast<uint8_t*>(host_ids), false, ids_stride, ids_view_stride, min_coverage};
+    return render_request(r, q, c, nullptr, __func__);
+}
 int forma_renderer_render_batch_device(forma_renderer* r, forma_composition* const* comps, uint32_t n, uint8_t* device_buffer,
                                        uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride,
                                        const uint32_t channels[4], const float clear_color[4], forma_timings* timings) {
@@ -533,6 +572,13 @@ int forma_renderer_render_views_masks_device(forma_renderer* r, forma_compositio
     q.views = views;
     return render_masks(r, q, masks, true, device_buffer, width_stride, view_stride, c, nullptr, __func__);
 }
+int forma_renderer_render_poses_masks_device(forma_renderer* r, forma_composition* c, const forma_poses* poses, uint32_t n,
+                                             const forma_masks* masks, uint64_t width, uint64_t height, uint8_t* device_buffer,
+                                             uint64_t width_stride, uint64_t view_stride, const uint32_t channels[4],
+                                             const float clear_color[4], forma_timings* timings) {
+    FrameRequest q = poses_request(poses, n, width, height, channels, clear_color, timings);
+    return render_masks(r, q, masks, true, device_buffer, width_stride, view_stride, c, nullptr, __func__);
+}
 int forma_renderer_render_batch_masks_device(forma_renderer* r, forma_composition* const* comps, uint32_t n,
                                              const forma_masks* masks, uint64_t width, uint64_t height, uint8_t* device_buffer,
                                              uint64_t width_stride, uint64_t frame_stride, const uint32_t channels[4],
@@ -571,6 +617,13 @@ int forma_renderer_render_views_stats_device(forma_renderer* r, forma_compositio
                                              const float clear_color[4], forma_timings* timings) {
     FrameRequest q{FrameKind::views, n, width, height, channels, clear_color, timings};
     q.views = views;
+    return render_stats(r, q, stats, true, device_buffer, width_stride, view_stride, c, nullptr, __func__);
+}
+int forma_renderer_render_poses_stats_device(forma_renderer* r, forma_composition* c, const forma_poses* poses, uint32_t n,
+                                             const forma_stats* stats, uint64_t width, uint64_t height, uint8_t* device_buffer,
+                                             uint64_t width_stride, uint64_t view_stride, const uint32_t channels[4],
+                                             const float clear_color[4], forma_timings* timings) {
+    FrameRequest q = poses_request(poses, n, width, height, channels, clear_color, timings);
     return render_stats(r, q, stats, true, device_buffer, width_stride, view_stride, c, nullptr, __func__);
 }
 int forma_renderer_render_batch_stats_device(forma_renderer* r, forma_composition* const* comps, uint32_t n,

@@ -88,6 +88,25 @@ void launch_line_count_views(const RasterArgs& args, const ViewArgs& views, uint
                              uint32_t* max_tile, cudaStream_t stream);
 void launch_raster_emit_views(const RasterArgs& args, const ViewArgs& views, uint32_t n_views, const uint32_t* block_offsets,
                               uint64_t* out, uint32_t cap, cudaStream_t stream, const CountArgs* counts = nullptr);
+// Poses (see forma_renderer_render_poses_device): the views' stacked frame of n_frames frames, but
+// instead of a view transform, frame b gives the layer at an order o of the window
+// [first_order, first_order + n_orders) the transform and enabled bit of its record
+// recs[b * n_orders + o - first_order]. Layers outside the window keep their own.
+struct PoseRec {                    // 32 B
+    float ux, uy, vx, vy, tx, ty;   // LayerRec order
+    uint32_t bits;                  // has_xf | enabled << 1 (an identity transform is no transform)
+    uint32_t pad;
+};
+struct PoseArgs {
+    const PoseRec* recs;            // n_frames x n_orders, frame-major
+    uint32_t first_order, n_orders;
+    uint32_t rows;                  // tile rows per frame: ceil(height / 16)
+};
+// As the views launchers: raster_num_blocks(n_points) * n_frames block sums, frame-major.
+void launch_line_count_poses(const RasterArgs& args, const PoseArgs& poses, uint32_t n_frames, uint32_t* block_sums, uint32_t* total,
+                             uint32_t* max_tile, cudaStream_t stream);
+void launch_raster_emit_poses(const RasterArgs& args, const PoseArgs& poses, uint32_t n_frames, const uint32_t* block_offsets,
+                              uint64_t* out, uint32_t cap, cudaStream_t stream, const CountArgs* counts = nullptr);
 // Batches (see forma_renderer_render_batch_device): frame c of a stack of n_frames frames is a
 // composition of its own. Each frame's line setup reads its composition's segment buffer and
 // tables (as RasterArgs, over the whole frame), and only two key fields move: row t of frame c

@@ -211,8 +211,11 @@ __device__ __forceinline__ uint32_t warp_inclusive_scan_sat(uint32_t v) {
 // segment.rs:298-383 for the point pair (i, i+1). kViews: the line as view `V` (6 floats in
 // forma_layer_set_transform order) sees it: the layer's transform T becomes V ∘ T (V alone for a
 // layer without one), composed exactly as ViewArgs documents; a composed identity is no transform.
-template <bool kViews = false>
-__device__ __forceinline__ LineParams line_setup(const RasterArgs& A, uint32_t i, const float* V = nullptr) {
+// kPoses: a layer whose order lies in Q's window takes frame blockIdx.y's record (PoseArgs) in
+// place of its own transform and enabled bit.
+template <bool kViews = false, bool kPoses = false>
+__device__ __forceinline__ LineParams line_setup(const RasterArgs& A, uint32_t i, const float* V = nullptr,
+                                                 const PoseArgs& Q = PoseArgs{}) {
     LineParams L;
     L.length = 0;
     L.order = 0;
@@ -230,6 +233,17 @@ __device__ __forceinline__ LineParams line_setup(const RasterArgs& A, uint32_t i
         lay.order = bits & 0x1FFFFFu;
         lay.enabled = (bits >> 21) & 1u;
         lay.has_xf = 0u;
+    }
+    if constexpr (kPoses) {
+        const uint32_t k = lay.order - Q.first_order;  // (wraps for orders below the window)
+        if (k < Q.n_orders) {
+            const float4* r = reinterpret_cast<const float4*>(Q.recs + (size_t)blockIdx.y * Q.n_orders + k);
+            const float4 a = __ldg(r), b = __ldg(r + 1);
+            lay.ux = a.x; lay.uy = a.y; lay.vx = a.z; lay.vy = a.w; lay.tx = b.x; lay.ty = b.y;
+            const uint32_t bits = __float_as_uint(b.z);
+            lay.has_xf = bits & 1u;
+            lay.enabled = (bits >> 1) & 1u;
+        }
     }
     if (!lay.enabled) return L;
     if constexpr (kViews) {
@@ -318,13 +332,16 @@ __device__ __forceinline__ BatchPos batch_pos(const BatchArgs& B, RasterArgs& A)
 // kViews: CTA (x, y) = the point pairs of CTA x under view y; its sum is block y * gridDim.x + x.
 // kBatch: CTA x = the point pairs of CTA P.block of frame P.frame (V.rows: the frame's tile rows);
 // its sum is block x.
-template <bool kViews, bool kBatch = false>
+// kPoses: as kViews, with frame y's pose records (Q) in place of a view transform.
+template <bool kViews, bool kBatch = false, bool kPoses = false>
 __device__ __forceinline__ void line_count_body(const RasterArgs& A, const ViewArgs& V, uint32_t* __restrict__ block_sums,
-                                                uint32_t* __restrict__ max_tile, const BatchPos& P = BatchPos{}) {
+                                                uint32_t* __restrict__ max_tile, const BatchPos& P = BatchPos{},
+                                                const PoseArgs& Q = PoseArgs{}) {
+    constexpr bool kStack = kViews || kPoses;  // the stack of one composition: frame blockIdx.y
     __shared__ uint32_t warp_sums[kRasterThreads / 32];
     __shared__ uint32_t warp_max[2][kRasterThreads / 32];
     uint32_t i = (kBatch ? P.block : blockIdx.x) * kRasterThreads + threadIdx.x;
-    const LineParams L = line_setup<kViews>(A, i, kViews ? V.xf + 6u * blockIdx.y : nullptr);
+    const LineParams L = line_setup<kViews, kPoses>(A, i, kViews ? V.xf + 6u * blockIdx.y : nullptr, Q);
     uint32_t len = L.length;
     {
         uint32_t bx = 0, by = 0;
@@ -335,7 +352,7 @@ __device__ __forceinline__ void line_count_body(const RasterArgs& A, const ViewA
             int32_t ty = ((int32_t)floorf(fminf(ey, 3.0e7f) + 0.5f) >> 8) + 2;
             bx = (uint32_t)min(max(tx, 0), 4095);
             by = (uint32_t)min(max(ty, 0), 2047);
-            if constexpr (kViews || kBatch) {
+            if constexpr (kStack || kBatch) {
                 // The emit pass maps view y's segments to the stacked rows [y * rows + 1, (y + 1) * rows].
                 by = ((kBatch ? P.frame : blockIdx.y) + 1u) * V.rows;
                 // Tile columns left of -32767 wrap (int16, as in the reference) into the frame's
@@ -371,7 +388,7 @@ __device__ __forceinline__ void line_count_body(const RasterArgs& A, const ViewA
             bx = max(bx, warp_max[0][w]);
             by = max(by, warp_max[1][w]);
         }
-        block_sums[kViews && !kBatch ? blockIdx.y * gridDim.x + blockIdx.x : blockIdx.x] = s;
+        block_sums[kStack && !kBatch ? blockIdx.y * gridDim.x + blockIdx.x : blockIdx.x] = s;
         // Same-address atomics serialise in L2: only raise the maximum when needed.
         if (bx > *(volatile uint32_t*)&max_tile[0]) atomicMax(&max_tile[0], bx);
         if (by > *(volatile uint32_t*)&max_tile[1]) atomicMax(&max_tile[1], by);
@@ -390,6 +407,10 @@ __global__ void __launch_bounds__(kRasterThreads) line_count_batch_kernel(BatchA
     RasterArgs A;
     const BatchPos P = batch_pos(B, A);
     line_count_body<false, true>(A, ViewArgs{nullptr, B.rows}, block_sums, max_tile, P);
+}
+__global__ void __launch_bounds__(kRasterThreads) line_count_poses_kernel(RasterArgs A, PoseArgs Q, uint32_t* __restrict__ block_sums,
+                                                                        uint32_t* __restrict__ max_tile) {
+    line_count_body<false, false, true>(A, ViewArgs{nullptr, Q.rows}, block_sums, max_tile, BatchPos{}, Q);
 }
 
 // Device-wide exclusive scan of `n` u32 values by ONE CTA (n = number of CTAs
@@ -479,10 +500,12 @@ struct SharedLines {
 // A CTA's segments are consecutive, most often within two sort tiles: their counts gather in
 // shared memory, warp-aggregated, and go out once per CTA; the tiles after those two (a CTA of long
 // lines) take warp-aggregated global atomics.
-template <bool kViews, bool kBatch = false, bool kCount = false>
+// kPoses: as kViews, with frame y's pose records (Q) in place of a view transform.
+template <bool kViews, bool kBatch = false, bool kCount = false, bool kPoses = false>
 __device__ __forceinline__ void raster_emit_body(const RasterArgs& A, const ViewArgs& V, const uint32_t* __restrict__ block_offsets,
                                                  uint64_t* __restrict__ out, uint32_t cap, const BatchPos& P = BatchPos{},
-                                                 const CountArgs& C = CountArgs{}) {
+                                                 const CountArgs& C = CountArgs{}, const PoseArgs& Q = PoseArgs{}) {
+    constexpr bool kStack = kViews || kPoses;  // the stack of one composition: frame blockIdx.y
     __shared__ SharedLines S;
     __shared__ uint32_t warp_sums[kRasterThreads / 32];
     __shared__ uint32_t s_count[kCount ? 2 * kRadixDigits : 1];  // [2 tiles][digit]
@@ -493,7 +516,7 @@ __device__ __forceinline__ void raster_emit_body(const RasterArgs& A, const View
         s_count[t + kRasterThreads] = 0;
     }
     uint32_t i = (kBatch ? P.block : blockIdx.x) * kRasterThreads + t;
-    LineParams L = line_setup<kViews>(A, i, kViews ? V.xf + 6u * blockIdx.y : nullptr);
+    LineParams L = line_setup<kViews, kPoses>(A, i, kViews ? V.xf + 6u * blockIdx.y : nullptr, Q);
     if constexpr (kBatch) L.order += P.order_base;
     uint32_t incl = warp_inclusive_scan_sat(L.length);
     if (lane == 31) warp_sums[warp] = incl;
@@ -518,7 +541,7 @@ __device__ __forceinline__ void raster_emit_body(const RasterArgs& A, const View
     // then only steer the bisection, which stays inside S.excl).
     S.excl[t] = before + incl - L.length;  // exclusive prefix over the block's 256 lines
     __syncthreads();
-    const uint32_t block_base = block_offsets[kViews && !kBatch ? blockIdx.y * gridDim.x + blockIdx.x : blockIdx.x];
+    const uint32_t block_base = block_offsets[kStack && !kBatch ? blockIdx.y * gridDim.x + blockIdx.x : blockIdx.x];
     // `cap` bounds a speculative launch made before the segment count is known on the host: the
     // loop never runs past it, whatever the (saturated) counts of an over-limit frame. The last
     // clamp keeps `s += kRasterThreads` from wrapping.
@@ -561,7 +584,7 @@ __device__ __forceinline__ void raster_emit_body(const RasterArgs& A, const View
         // A view's painted rows (biased 1 ... rows) move to its place in the stacked frame; every
         // other row becomes tile row -1 (biased 0), which no painted tile reads, so that nothing
         // bleeds into the neighbouring views. The single frame's own wrap of the field is kept.
-        if constexpr (kViews || kBatch) ty = ty - 1u < V.rows ? ty + (uint64_t)(kBatch ? P.frame : blockIdx.y) * V.rows : 0u;
+        if constexpr (kStack || kBatch) ty = ty - 1u < V.rows ? ty + (uint64_t)(kBatch ? P.frame : blockIdx.y) * V.rows : 0u;
         uint64_t tx = (uint64_t)max((int32_t)(int16_t)(tile_x + 1), 0) & 0xFFFull;
         uint64_t v = (ty << 53) | (tx << 41) | ((uint64_t)(S.order[li] & 0x1FFFFFu) << 20) | ((uint64_t)local_x << 16) |
                      ((uint64_t)local_y << 12) | ((uint64_t)(dam & 0x3Fu) << 6) | ((uint64_t)((uint32_t)cover & 0x3Fu));
@@ -601,6 +624,11 @@ __global__ void __launch_bounds__(kRasterThreads, kCount ? 8 : 0) raster_emit_ba
     RasterArgs A;
     const BatchPos P = batch_pos(B, A);
     raster_emit_body<false, true, kCount>(A, ViewArgs{nullptr, B.rows}, block_offsets, out, cap, P, C);
+}
+template <bool kCount>
+__global__ void __launch_bounds__(kRasterThreads, kCount ? 8 : 0) raster_emit_poses_kernel(RasterArgs A, PoseArgs Q, const uint32_t* __restrict__ block_offsets,
+                                                                         uint64_t* __restrict__ out, uint32_t cap, CountArgs C) {
+    raster_emit_body<false, false, kCount, true>(A, ViewArgs{nullptr, Q.rows}, block_offsets, out, cap, BatchPos{}, C, Q);
 }
 
 // Inspection only (forma_renderer_lines): the line records of segment.rs:298-383 as the
@@ -678,6 +706,28 @@ void launch_raster_emit_views(const RasterArgs& args, const ViewArgs& views, uin
         raster_emit_views_kernel<true><<<dim3(nb, n_views), kRasterThreads, 0, stream>>>(args, views, block_offsets, out, cap, *counts);
     else
         raster_emit_views_kernel<false><<<dim3(nb, n_views), kRasterThreads, 0, stream>>>(args, views, block_offsets, out, cap, CountArgs{});
+}
+
+void launch_line_count_poses(const RasterArgs& args, const PoseArgs& poses, uint32_t n_frames, uint32_t* block_sums, uint32_t* total,
+                             uint32_t* max_tile, cudaStream_t stream) {
+    uint32_t nb = raster_num_blocks(args.n_points);
+    cudaMemsetAsync(max_tile, 0, 2 * sizeof(uint32_t), stream);
+    if (!nb || !n_frames) {
+        cudaMemsetAsync(total, 0, sizeof(uint32_t), stream);
+        return;
+    }
+    line_count_poses_kernel<<<dim3(nb, n_frames), kRasterThreads, 0, stream>>>(args, poses, block_sums, max_tile);
+    scan_block_sums_kernel<<<1, 1024, 0, stream>>>(block_sums, nb * n_frames, total);
+}
+
+void launch_raster_emit_poses(const RasterArgs& args, const PoseArgs& poses, uint32_t n_frames, const uint32_t* block_offsets,
+                              uint64_t* out, uint32_t cap, cudaStream_t stream, const CountArgs* counts) {
+    uint32_t nb = raster_num_blocks(args.n_points);
+    if (!nb || !n_frames) return;
+    if (counts)
+        raster_emit_poses_kernel<true><<<dim3(nb, n_frames), kRasterThreads, 0, stream>>>(args, poses, block_offsets, out, cap, *counts);
+    else
+        raster_emit_poses_kernel<false><<<dim3(nb, n_frames), kRasterThreads, 0, stream>>>(args, poses, block_offsets, out, cap, CountArgs{});
 }
 
 void launch_line_count_batch(const BatchArgs& batch, uint32_t n_ctas, uint32_t* block_sums, uint32_t* total, uint32_t* max_tile,

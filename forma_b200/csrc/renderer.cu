@@ -245,9 +245,9 @@ int Renderer::upload_tables_device(Composition& comp, CompDevice& cd) {
 
 // Stages 1½ + 2: fills `segs` with the unsorted pixel segments.
 int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, float band_lo, float band_hi,
-                        uint32_t* n_out, const ViewArgs* views, uint32_t n_views, const BatchLines* batch) {
+                        uint32_t* n_out, const ViewArgs* views, uint32_t n_views, const BatchLines* batch, const PoseArgs* poses) {
     RasterArgs& ra = last_raster;  // kept for forma_renderer_lines (a stacked frame has no line records)
-    last_raster_valid = !views && !batch;
+    last_raster_valid = !views && !batch && !poses;
     if (comp) {
         CompDevice& cd = comp->on(res_key);
         ra.x = cd.d_x.ptr;
@@ -264,7 +264,7 @@ int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, floa
         ra.band_hi = band_hi;
     }
     uint32_t nb = batch ? batch->n_ctas : raster_num_blocks(ra.n_points);
-    if (views) {
+    if (views || poses) {
         if ((uint64_t)nb * n_views >= (1ull << 32)) {
             set_error("%u views of %u points exceed the line-setup grid", n_views, ra.n_points);
             return FORMA_STATUS_CAPACITY;
@@ -274,11 +274,13 @@ int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, floa
     FORMA_CUDA_TRY(block_sums.reserve(nb + 1));
     if (batch) launch_line_count_batch(batch->args, nb, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
     else if (views) launch_line_count_views(ra, *views, n_views, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
+    else if (poses) launch_line_count_poses(ra, *poses, n_views, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
     else launch_line_count(ra, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
     launches += nb ? 2 : 0;
     auto emit = [&](uint32_t cap, const CountArgs* counts) {
         if (batch) launch_raster_emit_batch(batch->args, nb, block_sums.ptr, segs.ptr, cap, stream, counts);
         else if (views) launch_raster_emit_views(ra, *views, n_views, block_sums.ptr, segs.ptr, cap, stream, counts);
+        else if (poses) launch_raster_emit_poses(ra, *poses, n_views, block_sums.ptr, segs.ptr, cap, stream, counts);
         else launch_raster_emit(ra, block_sums.ptr, segs.ptr, cap, stream, counts);
     };
     // The emit pass counts the sort's pass-0 digits (TileCounts) when the sort will take them: with
@@ -430,7 +432,7 @@ int Renderer::run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p
     // frame of a stack as a frame of its own: all its rows are painted.
     const uint32_t height = (uint32_t)q.height;
     const FrameBand band = p.rows ? FrameBand{0.0f, (float)height, false} : tile_band(S.ty_lo, S.ty_hi, height);
-    const bool views = q.kind == FrameKind::views, batched = q.kind == FrameKind::batch;
+    const bool views = q.kind == FrameKind::views, batched = q.kind == FrameKind::batch, poses = q.kind == FrameKind::poses;
     int st = FORMA_STATUS_OK;
     BatchLines batch{};
     if (batched) {  // every composition's uploads, then the batch tables
@@ -452,11 +454,17 @@ int Renderer::run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p
         FORMA_CUDA_TRY(cudaMemcpyAsync(d_views.ptr, h_views.ptr, 6u * nv * sizeof(float), cudaMemcpyHostToDevice, stream));
         h2d_bytes += 6u * nv * sizeof(float);
     }
+    if (poses) {
+        st = upload_poses(q);
+        if (st) return st;
+    }
     const ViewArgs va{d_views.ptr, (height + 15u) / 16u};
+    const PoseArgs pa{d_poses.ptr, poses ? q.poses->first_order : 0u, poses ? q.poses->n_orders : 0u, (height + 15u) / 16u};
 
     FORMA_CUDA_TRY(cudaEventRecord(timer.ev[7], stream));
     uint32_t n = 0;
-    st = rasterize(q.comp, S.width, height, band.lo, band.hi, &n, views ? &va : nullptr, q.n, batched ? &batch : nullptr);
+    st = rasterize(q.comp, S.width, height, band.lo, band.hi, &n, views ? &va : nullptr, q.n, batched ? &batch : nullptr,
+                   poses ? &pa : nullptr);
     if (st) return st;
 
     // Stage 3: sort.
@@ -614,13 +622,78 @@ int Renderer::render(const FrameRequest& q) {
     return FORMA_STATUS_OK;
 }
 
+// The pose tables of a poses request (see forma_renderer_render_poses_device): a window of 1 to
+// 2^21 orders below 2^21, at least one table, and every transform one forma_layer_set_transform
+// accepts.
+static int check_poses(const FrameRequest& q) {
+    const forma_poses* P = q.poses;
+    if (!P || (!P->transforms && !P->visible)) {
+        set_error("no %s", P ? "pose table" : "poses");
+        return FORMA_STATUS_INVALID;
+    }
+    const uint32_t K = P->n_orders;
+    uint64_t recs = 0, floats = 0;
+    if (K == 0u || (uint64_t)P->first_order + K > (1ull << 21) || __builtin_mul_overflow((uint64_t)q.n, (uint64_t)K, &recs) ||
+        __builtin_mul_overflow(recs, (uint64_t)6u, &floats)) {
+        set_error("invalid poses: orders [%u, %u + %u) (1 to 2^21 orders below 2^21) of %u frames", P->first_order, P->first_order, K, q.n);
+        return FORMA_STATUS_INVALID;
+    }
+    for (uint64_t r = 0; P->transforms && r < recs; ++r) {  // [ux, vx, uy, vy, tx, ty]
+        const float* t = P->transforms + 6u * r;
+        if (!geom_pres_ok(t[0], t[2], t[1], t[3])) {
+            set_error("pose of frame %llu, order %llu: GeomPresTransformError::ExceededScalingFactor", (unsigned long long)(r / K),
+                      (unsigned long long)(P->first_order + r % K));
+            return FORMA_STATUS_INVALID;
+        }
+    }
+    return FORMA_STATUS_OK;
+}
+
+// The pose records of frame b, order first_order + k at b * K + k: the tables' transform and
+// visibility, or the layer's own for a null table. An identity transform is no transform (the
+// rule of forma_layer_set_transform). Orders without a layer keep a zero record: no line reads it.
+int Renderer::upload_poses(const FrameRequest& q) {
+    const forma_poses& P = *q.poses;
+    const uint32_t K = P.n_orders;
+    const size_t n_recs = (size_t)q.n * K;
+    if (h_poses.reserve(n_recs) != cudaSuccess || d_poses.reserve(n_recs) != cudaSuccess) {
+        cudaGetLastError();  // (a failed allocation is not sticky: clear it for the launches' checks)
+        set_error("%zu pose records (%zu bytes) could not be allocated", n_recs, n_recs * sizeof(PoseRec));
+        return FORMA_STATUS_CAPACITY;
+    }
+    // (the previous call's copy is complete: rasterize waited for it)
+    std::memset(h_poses.ptr, 0, n_recs * sizeof(PoseRec));
+    const auto& layers = q.comp->layers;
+    for (auto it = layers.lower_bound(P.first_order); it != layers.end() && it->first - P.first_order < K; ++it) {
+        const uint32_t k = it->first - P.first_order;
+        const Layer& l = *it->second;
+        for (uint32_t b = 0; b < q.n; ++b) {
+            const size_t r = (size_t)b * K + k;
+            PoseRec& rec = h_poses.ptr[r];
+            bool has_xf = l.has_xf;
+            if (P.transforms) {
+                const float* t = P.transforms + 6u * r;
+                rec = PoseRec{t[0], t[2], t[1], t[3], t[4], t[5], 0u, 0u};
+                has_xf = !(rec.ux == 1.0f && rec.uy == 0.0f && rec.vx == 0.0f && rec.vy == 1.0f && rec.tx == 0.0f && rec.ty == 0.0f);
+            } else {
+                rec = PoseRec{l.xf[0], l.xf[1], l.xf[2], l.xf[3], l.xf[4], l.xf[5], 0u, 0u};
+            }
+            const bool enabled = P.visible ? P.visible[r] != 0 : l.enabled;
+            rec.bits = (has_xf ? 1u : 0u) | (enabled ? 2u : 0u);
+        }
+    }
+    FORMA_CUDA_TRY(cudaMemcpyAsync(d_poses.ptr, h_poses.ptr, n_recs * sizeof(PoseRec), cudaMemcpyHostToDevice, stream));
+    h2d_bytes += n_recs * sizeof(PoseRec);
+    return FORMA_STATUS_OK;
+}
+
 // The checks of a request, before anything is written: each target (LinearLayout::new asserts,
 // layout/mod.rs:188-193, consts.rs limits, and for a stack the frame count and frame stride), the
 // ID target's own, then the views or the compositions of a batch. An ID-only request has no RGBA
 // target to check.
 int Renderer::check_request(const FrameRequest& q) {
     const bool stack = q.kind != FrameKind::single;
-    const char* what = q.kind == FrameKind::views ? "view" : "frame";
+    const char* what = q.one_comp_stack() ? "view" : "frame";
     const uint64_t width = q.width, height = q.height;
     auto check_target = [&](const FrameTarget& t) {
         if (!t.ptr || width == 0 || height == 0 || width * t.bpp > t.stride || width > FORMA_MAX_WIDTH || height > FORMA_MAX_HEIGHT) {
@@ -699,6 +772,7 @@ int Renderer::check_request(const FrameRequest& q) {
             return FORMA_STATUS_INVALID;
         }
     }
+    if (q.kind == FrameKind::poses) return check_poses(q);
     if (q.kind != FrameKind::batch) return FORMA_STATUS_OK;
     // The distinct compositions in order of first appearance, and the slices of the layer field
     // they need: n_orders each, as rebuild_tables counts them.
@@ -757,7 +831,7 @@ int Renderer::check_masks(const FrameRequest& q) {
         return FORMA_STATUS_INVALID;
     }
     if (q.kind != FrameKind::single && (q.n == 0 || q.n > max_views(height))) {
-        set_error("%u %ss of height %llu: between 1 and %u fit in one call", q.n, q.kind == FrameKind::views ? "view" : "frame",
+        set_error("%u %ss of height %llu: between 1 and %u fit in one call", q.n, q.one_comp_stack() ? "view" : "frame",
                   (unsigned long long)height, max_views(height));
         return FORMA_STATUS_INVALID;
     }
@@ -791,7 +865,7 @@ int Renderer::check_stats(const FrameRequest& q) {
         return FORMA_STATUS_INVALID;
     }
     if (q.kind != FrameKind::single && (q.n == 0 || q.n > max_views(height))) {
-        set_error("%u %ss of height %llu: between 1 and %u fit in one call", q.n, q.kind == FrameKind::views ? "view" : "frame",
+        set_error("%u %ss of height %llu: between 1 and %u fit in one call", q.n, q.one_comp_stack() ? "view" : "frame",
                   (unsigned long long)height, max_views(height));
         return FORMA_STATUS_INVALID;
     }

@@ -77,9 +77,11 @@ struct StatsTarget {
 // batch: n compositions, one frame each, stacked as views are; frame c's line setup reads
 // comps[c]'s segment buffer and moves its segments' layers to the composition's slice of the
 // layer field (bind_batch), so that the batch tables serve every frame, and frame c's IDs are
-// comps[c]'s own orders. A stack takes no layer cache and no band filter: every composition is
-// resident whole.
-enum class FrameKind { single, views, batch };
+// comps[c]'s own orders. poses: n frames of one composition stacked as views are, frame b giving
+// each layer of a window of orders its own transform and enabled state (PoseArgs); line setup
+// reads frame b's pose records in place of a view transform, and from there on a pose stack is a
+// views stack. A stack takes no layer cache and no band filter: every composition is resident whole.
+enum class FrameKind { single, views, batch, poses };
 
 // One call of Renderer::render: what is rendered, the size of one frame, and its targets: an
 // RGBA target, an ID target (channels {0, 1, 2, 3}, clear colour 0 when it is alone) or both, or
@@ -99,6 +101,9 @@ struct FrameRequest {
     Composition* comp = nullptr;          // single, views
     const float* views = nullptr;         // views: n transforms [ux, vx, uy, vy, tx, ty]
     Composition* const* batch = nullptr;  // batch: n compositions (null entries are refused)
+    const forma_poses* poses = nullptr;   // poses: the window and its tables (null is refused)
+    // Views and poses: a stack of frames of one composition (q.comp).
+    bool one_comp_stack() const { return kind == FrameKind::views || kind == FrameKind::poses; }
 };
 
 // Where Renderer::render paints a request's targets: per target the frame on the device (the
@@ -320,8 +325,10 @@ class Renderer {
     int upload_tables_device(Composition& comp, CompDevice& cd);
     // views / n_views: the line setup of a views request (a stacked frame of n_views views); batch:
     // that of a batch request (comp is then null).
+    // poses: that of a poses request (n_views frames).
     int rasterize(Composition* comp, uint32_t width, uint32_t height, float band_lo, float band_hi, uint32_t* n_out,
-                  const ViewArgs* views = nullptr, uint32_t n_views = 0, const BatchLines* batch = nullptr);
+                  const ViewArgs* views = nullptr, uint32_t n_views = 0, const BatchLines* batch = nullptr,
+                  const PoseArgs* poses = nullptr);
     // Every frame, whatever its kind and targets: check_request, the PaintScene (begin_frame), each
     // target's device frame, run_frame and, for a layer cache, its bookkeeping.
     int render(const FrameRequest& q);
@@ -339,6 +346,10 @@ class Renderer {
     DeviceBuffer<forma_layer_stats> stats_scratch;  // the records of host statistics
     PinnedBuffer<float> h_views;
     DeviceBuffer<float> d_views;
+    PinnedBuffer<PoseRec> h_poses;
+    DeviceBuffer<PoseRec> d_poses;
+    // Folds a poses request's tables into n x K pose records and queues their upload.
+    int upload_poses(const FrameRequest& q);
     // A batch's distinct compositions' tables are gathered into the batch tables below, which are
     // kept until a batch of other compositions or other table versions comes (batch_key).
     std::vector<std::pair<uint64_t, uint64_t>> batch_key;  // (Composition::serial, tables_version) of the distinct compositions

@@ -604,6 +604,72 @@ int forma_renderer_render_batch_stats_device(forma_renderer*, forma_composition*
                                              const uint32_t channels[4], const float clear_color[4],
                                              forma_timings* timings /* nullable */);
 
+/* Poses (no reference counterpart): n frames of one composition, from one pass through the
+ * stages. In frame b, each layer attached at an order o of the window [first_order,
+ * first_order + K), k = o - first_order, gets its own transform and visibility: frame b is
+ * exactly the bytes forma_renderer_render_device writes (no crop, no cache) for the composition
+ * after
+ *   forma_layer_set_transform(layer, transforms + 6 (b K + k))      when transforms is not null,
+ *   forma_layer_set_is_enabled(layer, visible[b K + k] != 0)         when visible is not null
+ * (the state is set outright: a disabled layer can be shown in some frames). Layers outside the
+ * window, orders of the window without a layer, path transforms, props, gradients and textures
+ * stay as they are; gradients and textures stay in frame coordinates. A pose transform equal to
+ * the identity is no transform, as forma_layer_set_transform has it. (Frames whose lines all lie
+ * more than 2^19 px left of the frame are the exception of views and batches again: the stacked
+ * call is right, forma_renderer_render_device mis-sorts their wrapped tile columns.)
+ * The call does not change the composition: afterwards every layer's transform, enabled state and
+ * per-cache unchanged bits are what they were, and the next ordinary render uploads nothing
+ * because of it. The geometry is flattened and made resident once; per call, n K 32-byte pose
+ * records cross PCIe.
+ * Each call is the twin of a views call, with `const forma_poses* poses, uint32_t n` in place of
+ * `const float* views, uint32_t n`: the same arguments, layouts, rules, limits, refusals and state
+ * afterwards (counters, segments, stage times and row costs of the stacked frame, no line records):
+ *   render_poses{,_device}       forma_renderer_render_views{,_device}
+ *   render_poses_ids{,_device}   forma_renderer_render_views_ids{,_device} (RGBA optional, as there)
+ *   render_poses_masks_device    forma_renderer_render_views_masks_device
+ *   render_poses_stats_device    forma_renderer_render_views_stats_device
+ * In the ID, mask and statistics calls the values are the composition's own orders.
+ * Besides the twin's refusals, FORMA_ERR_INVALID_ARGUMENT is returned before anything is written
+ * to any buffer, with the composition untouched, for: a null poses; both tables null; K = 0 or
+ * first_order + K > 2^21; n K 6 floats overflowing 64 bits; any pose transform that
+ * forma_layer_set_transform refuses (forma_last_error() names the frame and the order). Unlike a
+ * view, a pose transform need not be finite: a NaN or infinite translation renders as
+ * forma_renderer_render_device renders it. FORMA_ERR_CAPACITY: the pose records cannot be
+ * allocated, or the twin's limits. */
+typedef struct forma_poses {
+    uint32_t first_order, n_orders; /* the window, K = n_orders >= 1, first_order + K <= 2^21        */
+    const float* transforms;        /* nullable: n x K x 6 floats [ux, vx, uy, vy, tx, ty] per       */
+                                    /*   (frame b, order first_order + k) at 6 (b K + k), in          */
+                                    /*   forma_layer_set_transform order                              */
+    const uint8_t* visible;         /* nullable: n x K bytes at b K + k; 0 = disabled in frame b      */
+} forma_poses;
+int forma_renderer_render_poses_device(forma_renderer*, forma_composition*, const forma_poses* poses, uint32_t n,
+                                       uint8_t* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                       uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
+                                       forma_timings* timings /* nullable */);
+int forma_renderer_render_poses(forma_renderer*, forma_composition*, const forma_poses* poses, uint32_t n,
+                                uint8_t* host_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
+                                forma_timings* timings /* nullable */);
+int forma_renderer_render_poses_ids_device(forma_renderer*, forma_composition*, const forma_poses* poses, uint32_t n,
+                                           uint8_t* device_buffer /* nullable */, uint64_t width, uint64_t width_stride,
+                                           uint64_t height, uint64_t view_stride, const uint32_t channels[4],
+                                           const float clear_color[4], uint32_t* device_ids, uint64_t ids_stride,
+                                           uint64_t ids_view_stride, float min_coverage, forma_timings* timings /* nullable */);
+int forma_renderer_render_poses_ids(forma_renderer*, forma_composition*, const forma_poses* poses, uint32_t n, uint32_t* host_ids,
+                                    uint64_t width, uint64_t ids_stride, uint64_t height, uint64_t ids_view_stride,
+                                    float min_coverage, forma_timings* timings /* nullable */);
+int forma_renderer_render_poses_masks_device(forma_renderer*, forma_composition*, const forma_poses* poses, uint32_t n,
+                                             const forma_masks* masks, uint64_t width, uint64_t height,
+                                             uint8_t* device_buffer /* nullable */, uint64_t width_stride, uint64_t view_stride,
+                                             const uint32_t channels[4], const float clear_color[4],
+                                             forma_timings* timings /* nullable */);
+int forma_renderer_render_poses_stats_device(forma_renderer*, forma_composition*, const forma_poses* poses, uint32_t n,
+                                             const forma_stats* stats, uint64_t width, uint64_t height,
+                                             uint8_t* device_buffer /* nullable */, uint64_t width_stride, uint64_t view_stride,
+                                             const uint32_t channels[4], const float clear_color[4],
+                                             forma_timings* timings /* nullable */);
+
 /* Launch on `cuda_stream` (a cudaStream_t, e.g. torch.cuda.current_stream().cuda_stream)
  * instead of the default stream. */
 void forma_renderer_set_stream(forma_renderer*, void* cuda_stream);
