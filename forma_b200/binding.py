@@ -217,29 +217,36 @@ class _CStats(C.Structure):  # forma_stats
 
 
 class _CPoses(C.Structure):  # forma_poses
-    _fields_ = [("first_order", C.c_uint32), ("n_orders", C.c_uint32), ("transforms", C.c_void_p), ("visible", C.c_void_p)]
+    _fields_ = [("first_order", C.c_uint32), ("n_orders", C.c_uint32), ("transforms", C.c_void_p), ("visible", C.c_void_p),
+                ("colors", C.c_void_p)]
 
 
 class Poses:
     """The per-frame layer states of a poses call (see include/forma_b200.h: forma_poses): in frame
     b, the layer at order first_order + k takes transforms[b, k] ([n, K, 6] float32, set_transform
-    order [ux, vx, uy, vy, tx, ty]) and is enabled where visible[b, k] ([n, K] bool / uint8) is
-    non-zero. Either table may be None (that state stays the layer's own), not both; with both, n
-    and K must agree."""
+    order [ux, vx, uy, vy, tx, ty]), is enabled where visible[b, k] ([n, K] bool / uint8) is
+    non-zero, and, when it draws, fills with the solid linear RGBA colour colors[b, k] ([n, K, 4]
+    float32; its fill rule, clipping and blend mode stay). Any table may be None (that state stays
+    the layer's own), not all three; the tables given must agree on n and K."""
 
-    def __init__(self, first_order: int, transforms=None, visible=None):
-        if transforms is None and visible is None:
-            raise ValueError("Poses: transforms, visible or both")
+    def __init__(self, first_order: int, transforms=None, visible=None, colors=None):
+        if transforms is None and visible is None and colors is None:
+            raise ValueError("Poses: transforms, visible, colors or several of them")
         self.first_order = int(first_order)
         self.transforms = None if transforms is None else np.ascontiguousarray(np.asarray(transforms, dtype=np.float32))
         self.visible = None if visible is None else np.ascontiguousarray(np.asarray(visible).astype(np.uint8))
+        if colors is not None and (not isinstance(colors, np.ndarray) or colors.dtype != np.float32):
+            raise ValueError("Poses: colors must be a float32 array [n, K, 4]")
+        self.colors = None if colors is None else np.ascontiguousarray(colors)
         if self.transforms is not None and (self.transforms.ndim != 3 or self.transforms.shape[2] != 6):
             raise ValueError(f"Poses: transforms of shape {self.transforms.shape}, not [n, K, 6]")
         if self.visible is not None and self.visible.ndim != 2:
             raise ValueError(f"Poses: visible of shape {self.visible.shape}, not [n, K]")
-        shapes = {t.shape[:2] for t in (self.transforms, self.visible) if t is not None}
+        if self.colors is not None and (self.colors.ndim != 3 or self.colors.shape[2] != 4):
+            raise ValueError(f"Poses: colors of shape {self.colors.shape}, not [n, K, 4]")
+        shapes = {t.shape[:2] for t in (self.transforms, self.visible, self.colors) if t is not None}
         if len(shapes) != 1:
-            raise ValueError(f"Poses: transforms and visible disagree on [n, K]: {sorted(shapes)}")
+            raise ValueError(f"Poses: the tables disagree on [n, K]: {sorted(shapes)}")
         self.n, self.n_orders = shapes.pop()
 
     def __len__(self) -> int:
@@ -399,6 +406,12 @@ SIGNATURES = {
                                                      C.c_uint64, _vp, C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
     "renderer_render_poses_stats_device": (C.c_int, [_vp, _vp, C.POINTER(_CPoses), C.c_uint32, C.POINTER(_CStats), C.c_uint64,
                                                      C.c_uint64, _vp, C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
+    "renderer_render_poses_linear": (C.c_int, [_vp, _vp, C.POINTER(_CPoses), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64,
+                                               C.c_uint64, _u32p, _fp, C.c_uint32, C.POINTER(_CTimings)]),
+    "renderer_render_poses_linear_device": (C.c_int, [_vp, _vp, C.POINTER(_CPoses), C.c_uint32, _vp, C.c_uint64, C.c_uint64,
+                                                      C.c_uint64, C.c_uint64, _u32p, _fp, C.c_uint32, C.POINTER(_CTimings)]),
+    "renderer_render_poses_over_device": (C.c_int, [_vp, _vp, C.POINTER(_CPoses), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64,
+                                                    C.c_uint64, _u32p, C.c_uint32, C.POINTER(_CTimings)]),
     "renderer_launch_count": (C.c_uint64, [_vp]),
     "renderer_stage_times": (None, [_vp, C.POINTER(C.c_double)]),
     "renderer_counters": (None, [_vp, _u64p]),
@@ -464,9 +477,11 @@ MASK_SYMBOLS = ("renderer_render_masks", "renderer_render_masks_device", "render
 STATS_SYMBOLS = ("renderer_render_stats", "renderer_render_stats_device", "renderer_render_views_stats_device",
                  "renderer_render_batch_stats_device")
 # The same for poses (Renderer.render_poses, render_poses_device, render_poses_ids{,_device},
-# render_poses_masks_device, render_poses_stats_device).
+# render_poses_masks_device, render_poses_stats_device, render_poses_linear{,_device},
+# render_poses_over_device).
 POSE_SYMBOLS = ("renderer_render_poses", "renderer_render_poses_device", "renderer_render_poses_ids",
-                "renderer_render_poses_ids_device", "renderer_render_poses_masks_device", "renderer_render_poses_stats_device")
+                "renderer_render_poses_ids_device", "renderer_render_poses_masks_device", "renderer_render_poses_stats_device",
+                "renderer_render_poses_linear", "renderer_render_poses_linear_device", "renderer_render_poses_over_device")
 # Value formats of mask planes: name -> (FORMA_MASK_*, bytes per value, numpy dtype).
 MASK_FORMATS = {"f32": (0, 4, np.float32), "u8": (1, 1, np.uint8)}
 
@@ -1031,11 +1046,10 @@ class Renderer:
         keep = []  # the chunk's descriptor and tables stay alive until the next one
 
         def args(first, count):
-            t = None if poses.transforms is None else np.ascontiguousarray(poses.transforms[first:first + count])
-            v = None if poses.visible is None else np.ascontiguousarray(poses.visible[first:first + count])
-            d = _CPoses(poses.first_order, poses.n_orders, None if t is None else t.ctypes.data,
-                        None if v is None else v.ctypes.data)
-            keep[:] = [t, v, d]
+            t, v, c = (None if a is None else np.ascontiguousarray(a[first:first + count])
+                       for a in (poses.transforms, poses.visible, poses.colors))
+            d = _CPoses(poses.first_order, poses.n_orders, *(None if a is None else a.ctypes.data for a in (t, v, c)))
+            keep[:] = [t, v, c, d]
             return composition._h, C.byref(d), count
         return poses.n, args
 
@@ -1496,6 +1510,40 @@ class Renderer:
         return self._stack_stats(self._api.renderer_render_poses_stats_device, "Renderer::render_poses_stats_device", args, n, stats_ptr,
                                  width, height, first_order, n_orders, min_coverage, rgba_ptr, channels, clear_color, rgba_stride,
                                  view_stride, timings)
+
+    def render_poses_linear(self, composition: Composition, poses: Poses, buffer: np.ndarray, width: int, height: int, channels=RGBA,
+                            clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), format: str = "f32", stride: Optional[int] = None,
+                            view_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """render_poses as linear float frames (see render_linear); layout as for
+        render_views_linear, chunked like render_poses."""
+        code, bpp, dtype = pixel_format(format)
+        n, args = self._pose_args(composition, poses)
+        stride, view_stride = self._strides(width, height, stride, view_stride, bpp)
+        if n:
+            self._linear_host(buffer, dtype, (n - 1) * view_stride + (height - 1) * stride + bpp * width)
+        return self._stack(self._api.renderer_render_poses_linear, "Renderer::render_poses_linear", args, n, width, height,
+                           (buffer.ctypes.data, stride, view_stride, channels, clear_color), None, timings, bpp, (code,))
+
+    def render_poses_linear_device(self, composition: Composition, poses: Poses, device_ptr: int, width: int, height: int,
+                                   channels=RGBA, clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), format: str = "f32",
+                                   stride: Optional[int] = None, view_stride: Optional[int] = None,
+                                   timings: bool = True) -> Optional[Timings]:
+        """render_poses_linear into device memory: with the defaults, the data_ptr() of a
+        contiguous [N, height, width, 4] float32 / float16 CUDA tensor."""
+        code, bpp, _ = pixel_format(format)
+        n, args = self._pose_args(composition, poses)
+        return self._stack(self._api.renderer_render_poses_linear_device, "Renderer::render_poses_linear_device", args, n, width,
+                           height, (int(device_ptr), stride, view_stride, channels, clear_color), None, timings, bpp, (code,))
+
+    def render_poses_over_device(self, composition: Composition, poses: Poses, device_ptr: int, width: int, height: int, channels=RGBA,
+                                 format: str = "srgb8", stride: Optional[int] = None, view_stride: Optional[int] = None,
+                                 timings: bool = True) -> Optional[Timings]:
+        """render_poses over the frames already in device memory (see render_over_device): pose b
+        over frame b of the [N, height, width, 4] tensor. Chunked like render_poses."""
+        code, bpp, _ = over_format(format)
+        n, args = self._pose_args(composition, poses)
+        return self._stack(self._api.renderer_render_poses_over_device, "Renderer::render_poses_over_device", args, n, width, height,
+                           (int(device_ptr), stride, view_stride, channels, None), None, timings, bpp, (code,))
 
     def launch_count(self) -> int:
         return int(self._api.renderer_launch_count(self._h))

@@ -721,6 +721,29 @@ int forma_renderer_render_batch_over_device(forma_renderer* r, forma_composition
     q.rgba = {static_cast<uint8_t*>(device_buffer), true, width_stride, frame_stride};
     return render_over(r, q, format, nullptr, comps);
 }
+// Pose frames in the linear float formats and over a background: the twins of the views calls above.
+int forma_renderer_render_poses_linear(forma_renderer* r, forma_composition* c, const forma_poses* poses, uint32_t n, void* host_buffer,
+                                       uint64_t width, uint64_t width_stride, uint64_t height, uint64_t view_stride,
+                                       const uint32_t channels[4], const float clear_color[4], uint32_t format, forma_timings* timings) {
+    FrameRequest q = poses_request(poses, n, width, height, channels, clear_color, timings);
+    q.rgba = {static_cast<uint8_t*>(host_buffer), false, width_stride, view_stride};
+    return render_linear(r, q, format, c, nullptr);
+}
+int forma_renderer_render_poses_linear_device(forma_renderer* r, forma_composition* c, const forma_poses* poses, uint32_t n,
+                                              void* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                              uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
+                                              uint32_t format, forma_timings* timings) {
+    FrameRequest q = poses_request(poses, n, width, height, channels, clear_color, timings);
+    q.rgba = {static_cast<uint8_t*>(device_buffer), true, width_stride, view_stride};
+    return render_linear(r, q, format, c, nullptr);
+}
+int forma_renderer_render_poses_over_device(forma_renderer* r, forma_composition* c, const forma_poses* poses, uint32_t n,
+                                            void* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                            uint64_t view_stride, const uint32_t channels[4], uint32_t format, forma_timings* timings) {
+    FrameRequest q = poses_request(poses, n, width, height, channels, nullptr, timings);
+    q.rgba = {static_cast<uint8_t*>(device_buffer), true, width_stride, view_stride};
+    return render_over(r, q, format, c, nullptr);
+}
 // --- shared frames (multi-GPU, see include/forma_b200.h) -----------------------
 static_assert(sizeof(cudaIpcMemHandle_t) == sizeof(forma_ipc_handle), "CUDA IPC handles are 64 bytes");
 int forma_shared_frame_create(int device, uint64_t bytes, void** device_ptr, forma_ipc_handle* handle) {

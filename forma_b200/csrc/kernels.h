@@ -340,13 +340,30 @@ struct EntryRec {  // 64 B
 // kHeavyListClasses arrays of tiles_x * tiles_y ids each, their lengths in
 // heavy_count[kHeavyListClasses] (zeroed by the caller). frames != nullptr: S stacks the frames of
 // a batch, `rows` tile rows each (their order bases bound each entry's clip_layers to the range a
-// single frame of its composition has).
+// single frame of its composition has). fills != nullptr: S.styles is a pose style table (see
+// PoseFillArgs), and the entries of a pose stack's Draw layers in the window take their frame's
+// slot (merge_entries_pose_fills_kernel; frames is then null).
 constexpr int kHeavyListClasses = 4;
+// Pose fills (see forma_poses::colors): a pose style table holds the composition's n_styles style
+// records at their own slots, then per frame b and order first_order + k of the window the record of
+// slot n_styles + b * n_orders + k: the layer's StyleRec with the frame's solid fill
+// (launch_pose_styles). n_styles + n * n_orders < 2^31 (EntryRec::slot).
+struct PoseFillArgs {
+    uint32_t n_styles;
+    uint32_t first_order, n_orders;  // the pose window
+    uint32_t rows;                   // tile rows per frame
+};
 void launch_merge_entries(const PaintScene& S, const uint64_t* cell_key, uint32_t n_cells, const uint64_t* gkey,
                           const uint32_t* gid, uint32_t n_gaps, const uint32_t* cell_start, const uint4* carry_in,
                           const uint4* gap_carry, uint64_t* ekey, EntryRec* recs, uint8_t* eflags, uint2* tile_range,
                           uint32_t* heavy, uint32_t* heavy_count, cudaStream_t st, const DevCounts& dc = DevCounts(),
-                          const BatchFrame* frames = nullptr, uint32_t rows = 0);
+                          const BatchFrame* frames = nullptr, uint32_t rows = 0, const PoseFillArgs* fills = nullptr);
+// The tail of a pose style table `styles` (its slots [0, n_styles) already hold the composition's
+// records): record i = b * n_window + k of the n_recs records is the StyleRec of the layer at order
+// first_order + k (order_to_style, n_orders orders), with a Draw layer's fill replaced by the solid
+// colour colors[i] (linear RGBA) and no gradient or texture left; orders without a layer get none.
+void launch_pose_styles(const int32_t* order_to_style, uint32_t n_orders, StyleRec* styles, uint32_t n_styles, const float4* colors,
+                        uint32_t first_order, uint32_t n_window, uint64_t n_recs, cudaStream_t st);
 // The painter tables of a frame as every tile kernel (paint, ID, mask, statistics) reads them: the
 // sorted segments, the entry records, the per-tile entry ranges and, when `heavy` is not null, the
 // heavy-tile lists with their lengths (launch_merge_entries).

@@ -634,13 +634,18 @@ __device__ __forceinline__ uint32_t lower_bound_back(const uint64_t* __restrict_
 // segment range, carry, style bits and colour) and its initial optimizer flags,
 // so that the painter reaches everything it needs with one round of loads per
 // 32 entries instead of chasing key -> id -> cell -> style pointers per tile.
-__global__ void merge_entries_kernel(PaintScene S, const uint64_t* __restrict__ cell_key, uint32_t n_cells,
-                                     const uint64_t* __restrict__ gkey, const uint32_t* __restrict__ gid, uint32_t n_gaps,
-                                     const uint32_t* __restrict__ cell_start, const uint4* __restrict__ carry_in,
-                                     const uint4* __restrict__ gap_carry, uint64_t* __restrict__ ekey,
-                                     EntryRec* __restrict__ recs, uint8_t* __restrict__ eflags, uint2* __restrict__ tile_range,
-                                     uint32_t* __restrict__ heavy, uint32_t* __restrict__ heavy_count, DevCounts dc,
-                                     const BatchFrame* __restrict__ frames, uint32_t rows) {
+// kPoseFills: S.styles is a pose style table (PoseFillArgs), and an in-frame entry of a Draw layer
+// in the pose window takes its frame's slot; everything after reads the StyleRec at that slot.
+template <bool kPoseFills>
+__device__ __forceinline__ void merge_entries_body(PaintScene S, const uint64_t* __restrict__ cell_key, uint32_t n_cells,
+                                                   const uint64_t* __restrict__ gkey, const uint32_t* __restrict__ gid,
+                                                   uint32_t n_gaps, const uint32_t* __restrict__ cell_start,
+                                                   const uint4* __restrict__ carry_in, const uint4* __restrict__ gap_carry,
+                                                   uint64_t* __restrict__ ekey, EntryRec* __restrict__ recs,
+                                                   uint8_t* __restrict__ eflags, uint2* __restrict__ tile_range,
+                                                   uint32_t* __restrict__ heavy, uint32_t* __restrict__ heavy_count,
+                                                   DevCounts dc, const BatchFrame* __restrict__ frames, uint32_t rows,
+                                                   PoseFillArgs F = PoseFillArgs{}) {
     resolve_counts(dc, n_cells, n_gaps);
     // Merge-path style partition: the keys of a CTA's 256 consecutive elements of
     // one list bracket a short range of the other list, found once per CTA (two
@@ -706,6 +711,11 @@ __global__ void merge_entries_kernel(PaintScene S, const uint64_t* __restrict__ 
     }
     r.layer = key_layer(k);
     r.slot = r.layer < S.n_orders ? S.order_to_style[r.layer] : -1;
+    if constexpr (kPoseFills) {
+        const uint32_t o = r.layer - F.first_order;  // (wraps for orders below the window)
+        if (r.slot >= 0 && in_frame && o < F.n_orders && S.styles[r.slot].func == 0u)
+            r.slot = (int32_t)(F.n_styles + ((key_ty(k) - 1u) / F.rows) * F.n_orders + o);
+    }
     uint32_t flags = 0;
     if (r.slot >= 0) {
         const StyleRec& st = S.styles[r.slot];
@@ -738,6 +748,57 @@ __global__ void merge_entries_kernel(PaintScene S, const uint64_t* __restrict__ 
     ekey[pos] = k;
     recs[pos] = r;
     eflags[pos] = (uint8_t)flags;
+}
+__global__ void merge_entries_kernel(PaintScene S, const uint64_t* __restrict__ cell_key, uint32_t n_cells,
+                                     const uint64_t* __restrict__ gkey, const uint32_t* __restrict__ gid, uint32_t n_gaps,
+                                     const uint32_t* __restrict__ cell_start, const uint4* __restrict__ carry_in,
+                                     const uint4* __restrict__ gap_carry, uint64_t* __restrict__ ekey,
+                                     EntryRec* __restrict__ recs, uint8_t* __restrict__ eflags, uint2* __restrict__ tile_range,
+                                     uint32_t* __restrict__ heavy, uint32_t* __restrict__ heavy_count, DevCounts dc,
+                                     const BatchFrame* __restrict__ frames, uint32_t rows) {
+    merge_entries_body<false>(S, cell_key, n_cells, gkey, gid, n_gaps, cell_start, carry_in, gap_carry, ekey, recs, eflags, tile_range,
+                              heavy, heavy_count, dc, frames, rows);
+}
+__global__ void merge_entries_pose_fills_kernel(PaintScene S, const uint64_t* __restrict__ cell_key, uint32_t n_cells,
+                                                const uint64_t* __restrict__ gkey, const uint32_t* __restrict__ gid, uint32_t n_gaps,
+                                                const uint32_t* __restrict__ cell_start, const uint4* __restrict__ carry_in,
+                                                const uint4* __restrict__ gap_carry, uint64_t* __restrict__ ekey,
+                                                EntryRec* __restrict__ recs, uint8_t* __restrict__ eflags,
+                                                uint2* __restrict__ tile_range, uint32_t* __restrict__ heavy,
+                                                uint32_t* __restrict__ heavy_count, DevCounts dc, PoseFillArgs F) {
+    merge_entries_body<true>(S, cell_key, n_cells, gkey, gid, n_gaps, cell_start, carry_in, gap_carry, ekey, recs, eflags, tile_range,
+                             heavy, heavy_count, dc, nullptr, 0u, F);
+}
+
+// The tail of a pose style table, one thread per (frame b, order first_order + k) record i = b K + k:
+// the StyleRec of the layer at that order with its fill made Fill::Solid(colors[i]) when the layer
+// draws; a Clip layer's record is its own (merge_entries never points at it). Orders without a
+// layer have no record.
+__global__ void __launch_bounds__(256) pose_styles_kernel(const int32_t* __restrict__ order_to_style, uint32_t n_orders,
+                                                          StyleRec* __restrict__ styles, uint32_t n_styles,
+                                                          const float4* __restrict__ colors, uint32_t first_order, uint32_t K,
+                                                          uint64_t n_recs) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_recs) return;
+    const uint32_t o = first_order + (uint32_t)(i % K);
+    const int32_t s = o < n_orders ? order_to_style[o] : -1;
+    if (s < 0) return;
+    StyleRec r = styles[s];
+    if (r.func == 0u) {
+        const float4 c = colors[i];
+        r.fill_type = 0u;
+        r.color[0] = c.x;
+        r.color[1] = c.y;
+        r.color[2] = c.z;
+        r.color[3] = c.w;
+        r.gradient_type = 0u;
+        r.start[0] = r.start[1] = r.end[0] = r.end[1] = 0.0f;
+        r.stop_count = 0u;
+        for (int j = 0; j < 6; ++j) r.tex_xf[j] = 0.0f;
+        r.tex_max_x = r.tex_max_y = 0.0f;
+        r.tex_width = r.tex_first = 0u;
+    }
+    styles[n_styles + i] = r;
 }
 
 // Cost of every tile row of the frame just rendered: 32 x its (tile, layer) entries + its
@@ -847,12 +908,24 @@ void launch_merge_entries(const PaintScene& S, const uint64_t* cell_key, uint32_
                           const uint32_t* gid, uint32_t n_gaps, const uint32_t* cell_start, const uint4* carry_in,
                           const uint4* gap_carry, uint64_t* ekey, EntryRec* recs, uint8_t* eflags, uint2* tile_range,
                           uint32_t* heavy, uint32_t* heavy_count, cudaStream_t st, const DevCounts& dc, const BatchFrame* frames,
-                          uint32_t rows) {
+                          uint32_t rows, const PoseFillArgs* fills) {
     uint32_t n = n_cells + n_gaps;
-    if (n)
+    if (!n) return;
+    if (fills)
+        merge_entries_pose_fills_kernel<<<(n + 255) / 256, 256, 0, st>>>(S, cell_key, n_cells, gkey, gid, n_gaps, cell_start, carry_in,
+                                                                          gap_carry, ekey, recs, eflags, tile_range, heavy, heavy_count,
+                                                                          dc, *fills);
+    else
         merge_entries_kernel<<<(n + 255) / 256, 256, 0, st>>>(S, cell_key, n_cells, gkey, gid, n_gaps, cell_start, carry_in,
                                                                gap_carry, ekey, recs, eflags, tile_range, heavy, heavy_count, dc,
                                                                frames, rows);
+}
+
+void launch_pose_styles(const int32_t* order_to_style, uint32_t n_orders, StyleRec* styles, uint32_t n_styles, const float4* colors,
+                        uint32_t first_order, uint32_t n_window, uint64_t n_recs, cudaStream_t st) {
+    if (n_recs)
+        pose_styles_kernel<<<(unsigned)((n_recs + 255u) / 256u), 256, 0, st>>>(order_to_style, n_orders, styles, n_styles, colors,
+                                                                               first_order, n_window, n_recs);
 }
 
 // ---------------------------------------------------------------------------

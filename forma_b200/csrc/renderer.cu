@@ -454,6 +454,11 @@ int Renderer::run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p
         FORMA_CUDA_TRY(cudaMemcpyAsync(d_views.ptr, h_views.ptr, 6u * nv * sizeof(float), cudaMemcpyHostToDevice, stream));
         h2d_bytes += 6u * nv * sizeof(float);
     }
+    PoseFillArgs fills{};
+    if (q.pose_fills()) {  // (first: it refuses a table that cannot be indexed before anything is allocated)
+        st = upload_pose_fills(q, S, fills);
+        if (st) return st;
+    }
     if (poses) {
         st = upload_poses(q);
         if (st) return st;
@@ -515,7 +520,8 @@ int Renderer::run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p
     uint32_t paint_launches = 1;
     for (bool sync_free = fast;; sync_free = false) {
         DevCounts dc;
-        st = build_tables(S, n, sync_free, prev_cells, prev_gaps, heavy_lists, dc, batched ? &batch.args : nullptr);
+        st = build_tables(S, n, sync_free, prev_cells, prev_gaps, heavy_lists, dc, batched ? &batch.args : nullptr,
+                          q.pose_fills() ? &fills : nullptr);
         if (st) return st;
         st = queue_row_costs(S, n);
         if (st) return st;
@@ -624,17 +630,17 @@ int Renderer::render(const FrameRequest& q) {
 
 // The pose tables of a poses request (see forma_renderer_render_poses_device): a window of 1 to
 // 2^21 orders below 2^21, at least one table, and every transform one forma_layer_set_transform
-// accepts.
+// accepts. Colours are any floats (forma_layer_set_props takes them all).
 static int check_poses(const FrameRequest& q) {
     const forma_poses* P = q.poses;
-    if (!P || (!P->transforms && !P->visible)) {
+    if (!P || (!P->transforms && !P->visible && !P->colors)) {
         set_error("no %s", P ? "pose table" : "poses");
         return FORMA_STATUS_INVALID;
     }
     const uint32_t K = P->n_orders;
-    uint64_t recs = 0, floats = 0;
+    uint64_t recs = 0, floats = 0, colour_floats = 0;
     if (K == 0u || (uint64_t)P->first_order + K > (1ull << 21) || __builtin_mul_overflow((uint64_t)q.n, (uint64_t)K, &recs) ||
-        __builtin_mul_overflow(recs, (uint64_t)6u, &floats)) {
+        __builtin_mul_overflow(recs, (uint64_t)6u, &floats) || __builtin_mul_overflow(recs, (uint64_t)4u, &colour_floats)) {
         set_error("invalid poses: orders [%u, %u + %u) (1 to 2^21 orders below 2^21) of %u frames", P->first_order, P->first_order, K, q.n);
         return FORMA_STATUS_INVALID;
     }
@@ -684,6 +690,40 @@ int Renderer::upload_poses(const FrameRequest& q) {
     }
     FORMA_CUDA_TRY(cudaMemcpyAsync(d_poses.ptr, h_poses.ptr, n_recs * sizeof(PoseRec), cudaMemcpyHostToDevice, stream));
     h2d_bytes += n_recs * sizeof(PoseRec);
+    return FORMA_STATUS_OK;
+}
+
+// The pose style table of a poses request with colours (see PoseFillArgs): the composition's style
+// records (S.styles, bound by bind_frame), then n K records built on the device from the colours,
+// which go up as 16 bytes per record. S then reads the table.
+int Renderer::upload_pose_fills(const FrameRequest& q, PaintScene& S, PoseFillArgs& fills) {
+    const forma_poses& P = *q.poses;
+    const Composition& comp = *q.comp;
+    const uint64_t n_recs = (uint64_t)q.n * P.n_orders, n_styles = comp.n_style_recs, total = n_styles + n_recs;
+    if (total >= (1ull << 31)) {  // EntryRec::slot is an int32
+        set_error("%llu style records and %llu pose fills exceed the 2^31 style slots", (unsigned long long)n_styles,
+                  (unsigned long long)n_recs);
+        return FORMA_STATUS_CAPACITY;
+    }
+    if (h_pose_colors.reserve(n_recs) != cudaSuccess || d_pose_colors.reserve(n_recs) != cudaSuccess ||
+        pose_styles.reserve(total) != cudaSuccess) {
+        cudaGetLastError();  // (a failed allocation is not sticky: clear it for the launches' checks)
+        set_error("a pose style table of %llu records (%llu bytes) could not be allocated", (unsigned long long)total,
+                  (unsigned long long)(total * sizeof(StyleRec)));
+        return FORMA_STATUS_CAPACITY;
+    }
+    // (the previous call's copies are complete: rasterize waited for them)
+    std::memcpy(h_pose_colors.ptr, P.colors, n_recs * sizeof(float4));
+    FORMA_CUDA_TRY(cudaMemcpyAsync(d_pose_colors.ptr, h_pose_colors.ptr, n_recs * sizeof(float4), cudaMemcpyHostToDevice, stream));
+    h2d_bytes += n_recs * sizeof(float4);
+    if (n_styles)
+        FORMA_CUDA_TRY(cudaMemcpyAsync(pose_styles.ptr, S.styles, n_styles * sizeof(StyleRec), cudaMemcpyDeviceToDevice, stream));
+    launch_pose_styles(S.order_to_style, S.n_orders, pose_styles.ptr, (uint32_t)n_styles, d_pose_colors.ptr, P.first_order, P.n_orders,
+                       n_recs, stream);
+    ++launches;
+    FORMA_CUDA_TRY(cudaGetLastError());
+    S.styles = pose_styles.ptr;
+    fills = PoseFillArgs{(uint32_t)n_styles, P.first_order, P.n_orders, ((uint32_t)q.height + 15u) / 16u};
     return FORMA_STATUS_OK;
 }
 
@@ -1173,8 +1213,9 @@ SortResult Renderer::sort(DeviceBuffer<uint64_t>& keys, DeviceBuffer<uint64_t>& 
 // - counted: a count is read back; the kernel that produces it runs ahead of the read-back into
 //   the buffers of the previous frames and is launched again when they turn out too small.
 // batch: the frames of a batch (the merge bounds each entry's clip range by its frame's orders).
+// fills: the pose fills of a poses request (the merge points its entries at the pose style table).
 int Renderer::build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint32_t prev_cells, uint32_t prev_gaps,
-                           uint32_t* heavy_lists, DevCounts& dc, const BatchArgs* batch) {
+                           uint32_t* heavy_lists, DevCounts& dc, const BatchArgs* batch, const PoseFillArgs* fills) {
     // Tiles without entries keep an empty range: a frame whose tables are redone paints only the
     // clear colour in its first attempt. A count above its bound leaves every range empty (the
     // merge kernel then writes none), so that attempt of an over frame writes nothing at all.
@@ -1289,7 +1330,7 @@ int Renderer::build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint
              reinterpret_cast<const uint32_t*>(table_scratch.ptr + L.gap_hist), table_scratch.ptr + L.gap_sort);
     launch_merge_entries(S, cell_key.ptr, n_cells, ekey_tmp.ptr, eid_tmp.ptr, n_gaps, cell_start.ptr, carry_in.ptr, gap_carry.ptr,
                          ekey.ptr, recs.ptr, eflags.ptr, tile_range.ptr, heavy_lists, heavy_count(), stream, dc,
-                         batch ? batch->frames : nullptr, batch ? batch->rows : 0u);
+                         batch ? batch->frames : nullptr, batch ? batch->rows : 0u, fills);
     ++launches;
     // sync_free: the counts travel to the host behind everything else of the frame.
     if (sync_free)

@@ -104,6 +104,8 @@ struct FrameRequest {
     const forma_poses* poses = nullptr;   // poses: the window and its tables (null is refused)
     // Views and poses: a stack of frames of one composition (q.comp).
     bool one_comp_stack() const { return kind == FrameKind::views || kind == FrameKind::poses; }
+    // Poses with colours: the painter tables are built over a pose style table (PoseFillArgs).
+    bool pose_fills() const { return kind == FrameKind::poses && poses && poses->colors; }
 };
 
 // Where Renderer::render paints a request's targets: per target the frame on the device (the
@@ -350,6 +352,14 @@ class Renderer {
     DeviceBuffer<PoseRec> d_poses;
     // Folds a poses request's tables into n x K pose records and queues their upload.
     int upload_poses(const FrameRequest& q);
+    // Pose fills (forma_poses::colors): the colours as uploaded, 16 bytes per record, and the pose
+    // style table the call's PaintScene reads (PoseFillArgs).
+    PinnedBuffer<float4> h_pose_colors;
+    DeviceBuffer<float4> d_pose_colors;
+    DeviceBuffer<StyleRec> pose_styles;
+    // Queues the upload of a poses request's colours and the build of its pose style table, and
+    // points S at the table; `fills` receives the merge's arguments.
+    int upload_pose_fills(const FrameRequest& q, PaintScene& S, PoseFillArgs& fills);
     // A batch's distinct compositions' tables are gathered into the batch tables below, which are
     // kept until a batch of other compositions or other table versions comes (batch_key).
     std::vector<std::pair<uint64_t, uint64_t>> batch_key;  // (Composition::serial, tables_version) of the distinct compositions
@@ -371,7 +381,7 @@ class Renderer {
                     const float clear[4], const forma_rect* crop);
     int bind_frame(Composition& comp, PaintScene& S, LayerCache* cache, const float clear[4], bool pack_written);
     int build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint32_t prev_cells, uint32_t prev_gaps, uint32_t* heavy_lists,
-                     DevCounts& dc, const BatchArgs* batch);
+                     DevCounts& dc, const BatchArgs* batch, const PoseFillArgs* fills = nullptr);
     int queue_row_costs(const PaintScene& S, uint32_t n);
     int paint(const PaintScene& S, const TileTables& t, uint8_t* fb, uint8_t* buffer, uint64_t stride, bool in_bands,
               uint32_t* paint_launches, uint32_t view_rows = 0, uint32_t bpp = 4, bool solid_over = false, bool over = false);

@@ -611,16 +611,30 @@ int forma_renderer_render_batch_stats_device(forma_renderer*, forma_composition*
  * after
  *   forma_layer_set_transform(layer, transforms + 6 (b K + k))      when transforms is not null,
  *   forma_layer_set_is_enabled(layer, visible[b K + k] != 0)         when visible is not null
+ *   forma_layer_set_props(layer, props with the fill Solid(colors[b K + k]))
+ *                                when colors is not null and the layer's func is Draw(style)
  * (the state is set outright: a disabled layer can be shown in some frames). Layers outside the
- * window, orders of the window without a layer, path transforms, props, gradients and textures
- * stay as they are; gradients and textures stay in frame coordinates. A pose transform equal to
+ * window, orders of the window without a layer, path transforms, gradients and textures stay as
+ * they are; gradients and textures stay in frame coordinates. A pose transform equal to
  * the identity is no transform, as forma_layer_set_transform has it. (Frames whose lines all lie
  * more than 2^19 px left of the frame are the exception of views and batches again: the stacked
  * call is right, forma_renderer_render_device mis-sorts their wrapped tile columns.)
  * The call does not change the composition: afterwards every layer's transform, enabled state and
  * per-cache unchanged bits are what they were, and the next ordinary render uploads nothing
  * because of it. The geometry is flattened and made resident once; per call, n K 32-byte pose
- * records cross PCIe.
+ * records cross PCIe (and n K 16-byte colours with pose fills).
+ * Pose fills (colors not null): the props set in frame b are the layer's own with the fill alone
+ * replaced; its fill_rule, is_clipped, blend_mode (the non-separable modes included) and the
+ * layer's clip range stay, so a gradient or texture layer of the window becomes solid. A Clip
+ * layer has no fill: its colours are not read. Every float is taken as it is, NaN and infinities
+ * included, as forma_layer_set_props takes them; an alpha that makes a full layer opaque, or stops
+ * it being opaque, moves what the frame's IDs, masks and statistics see beneath it, as it would
+ * after forma_layer_set_props. The call builds a pose style table in renderer-owned device memory,
+ * 112 (S + n K) bytes for a composition of S style records (at most one per layer): about 90 MB for
+ * 16 frames of 50 620 recoloured layers. It is kept for the next call, as the other per-frame
+ * buffers are.
+ * ABI: colors is the last member, so every other member keeps its offset, and a descriptor that
+ * was zero-initialised before colors existed (colors = NULL) renders as it did.
  * Each call is the twin of a views call, with `const forma_poses* poses, uint32_t n` in place of
  * `const float* views, uint32_t n`: the same arguments, layouts, rules, limits, refusals and state
  * afterwards (counters, segments, stage times and row costs of the stacked frame, no line records):
@@ -628,20 +642,25 @@ int forma_renderer_render_batch_stats_device(forma_renderer*, forma_composition*
  *   render_poses_ids{,_device}   forma_renderer_render_views_ids{,_device} (RGBA optional, as there)
  *   render_poses_masks_device    forma_renderer_render_views_masks_device
  *   render_poses_stats_device    forma_renderer_render_views_stats_device
+ *   render_poses_linear{,_device} forma_renderer_render_views_linear{,_device}
+ *   render_poses_over_device     forma_renderer_render_views_over_device
  * In the ID, mask and statistics calls the values are the composition's own orders.
  * Besides the twin's refusals, FORMA_ERR_INVALID_ARGUMENT is returned before anything is written
- * to any buffer, with the composition untouched, for: a null poses; both tables null; K = 0 or
- * first_order + K > 2^21; n K 6 floats overflowing 64 bits; any pose transform that
+ * to any buffer, with the composition untouched, for: a null poses; all three tables null; K = 0
+ * or first_order + K > 2^21; n K 6 floats overflowing 64 bits; any pose transform that
  * forma_layer_set_transform refuses (forma_last_error() names the frame and the order). Unlike a
  * view, a pose transform need not be finite: a NaN or infinite translation renders as
- * forma_renderer_render_device renders it. FORMA_ERR_CAPACITY: the pose records cannot be
- * allocated, or the twin's limits. */
+ * forma_renderer_render_device renders it. FORMA_ERR_CAPACITY, also before anything is written:
+ * the pose records or the pose style table cannot be allocated; with colors, S + n K >= 2^31 (the
+ * style slots are 32-bit signed); or the twin's limits. */
 typedef struct forma_poses {
     uint32_t first_order, n_orders; /* the window, K = n_orders >= 1, first_order + K <= 2^21        */
     const float* transforms;        /* nullable: n x K x 6 floats [ux, vx, uy, vy, tx, ty] per       */
                                     /*   (frame b, order first_order + k) at 6 (b K + k), in          */
                                     /*   forma_layer_set_transform order                              */
     const uint8_t* visible;         /* nullable: n x K bytes at b K + k; 0 = disabled in frame b      */
+    const float* colors;            /* nullable: n x K x 4 floats, linear RGBA as in forma_color, at  */
+                                    /*   4 (b K + k): the solid fill of a Draw layer in frame b       */
 } forma_poses;
 int forma_renderer_render_poses_device(forma_renderer*, forma_composition*, const forma_poses* poses, uint32_t n,
                                        uint8_t* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
@@ -669,6 +688,18 @@ int forma_renderer_render_poses_stats_device(forma_renderer*, forma_composition*
                                              uint8_t* device_buffer /* nullable */, uint64_t width_stride, uint64_t view_stride,
                                              const uint32_t channels[4], const float clear_color[4],
                                              forma_timings* timings /* nullable */);
+int forma_renderer_render_poses_linear(forma_renderer*, forma_composition*, const forma_poses* poses, uint32_t n,
+                                       void* host_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                       uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
+                                       uint32_t format, forma_timings* timings /* nullable */);
+int forma_renderer_render_poses_linear_device(forma_renderer*, forma_composition*, const forma_poses* poses, uint32_t n,
+                                              void* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                              uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
+                                              uint32_t format, forma_timings* timings /* nullable */);
+int forma_renderer_render_poses_over_device(forma_renderer*, forma_composition*, const forma_poses* poses, uint32_t n,
+                                            void* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                            uint64_t view_stride, const uint32_t channels[4], uint32_t format,
+                                            forma_timings* timings /* nullable */);
 
 /* Launch on `cuda_stream` (a cudaStream_t, e.g. torch.cuda.current_stream().cuda_stream)
  * instead of the default stream. */
