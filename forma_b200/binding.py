@@ -221,23 +221,67 @@ class _CPoses(C.Structure):  # forma_poses
                 ("colors", C.c_void_p)]
 
 
+def _is_cuda_array(a) -> bool:
+    return a is not None and hasattr(a, "__cuda_array_interface__")
+
+
+class _CudaTable:
+    """A pose table in device memory, from an object with __cuda_array_interface__: its address,
+    shape and bytes per frame (a chunk of frames [f, f + c) starts at ptr + f * row_bytes). It
+    keeps the object alive and is never copied."""
+
+    def __init__(self, name, a, typestrs):
+        cai = a.__cuda_array_interface__
+        shape, typestr = tuple(int(s) for s in cai["shape"]), cai["typestr"]
+        if typestr not in typestrs:
+            raise ValueError(f"Poses: {name} of CUDA type {typestr!r}, not {' or '.join(map(repr, typestrs))}")
+        if cai.get("mask") is not None:
+            raise ValueError(f"Poses: {name} is a masked CUDA array")
+        itemsize = int(typestr[2:])
+        strides = cai.get("strides")
+        if strides is not None:  # C-contiguous: each dimension longer than 1 steps over the ones after it
+            step = itemsize
+            for n, s in reversed(list(zip(shape, strides))):
+                if n > 1 and s != step:
+                    raise ValueError(f"Poses: {name} is not a C-contiguous CUDA array (strides {tuple(strides)})")
+                step *= n
+        self.owner, self.ptr, self.shape = a, int(cai["data"][0]), shape
+        self.ndim = len(shape)
+        self.row_bytes = itemsize * int(np.prod(shape[1:], dtype=np.int64)) if shape else 0
+
+
 class Poses:
     """The per-frame layer states of a poses call (see include/forma_b200.h: forma_poses): in frame
     b, the layer at order first_order + k takes transforms[b, k] ([n, K, 6] float32, set_transform
     order [ux, vx, uy, vy, tx, ty]), is enabled where visible[b, k] ([n, K] bool / uint8) is
     non-zero, and, when it draws, fills with the solid linear RGBA colour colors[b, k] ([n, K, 4]
     float32; its fill rule, clipping and blend mode stay). Any table may be None (that state stays
-    the layer's own), not all three; the tables given must agree on n and K."""
+    the layer's own), not all three; the tables given must agree on n and K.
+
+    Each table may also be a CUDA array on the renderer's device: any object with
+    __cuda_array_interface__, such as a torch CUDA tensor, C-contiguous, float32 transforms and
+    colours, uint8 or bool visibility. It is read where it is, on the renderer's stream (see
+    include/forma_b200.h: forma_poses), never copied or moved to the host; anything else is refused
+    with ValueError. Host and CUDA tables can be mixed."""
 
     def __init__(self, first_order: int, transforms=None, visible=None, colors=None):
         if transforms is None and visible is None and colors is None:
             raise ValueError("Poses: transforms, visible, colors or several of them")
         self.first_order = int(first_order)
-        self.transforms = None if transforms is None else np.ascontiguousarray(np.asarray(transforms, dtype=np.float32))
-        self.visible = None if visible is None else np.ascontiguousarray(np.asarray(visible).astype(np.uint8))
-        if colors is not None and (not isinstance(colors, np.ndarray) or colors.dtype != np.float32):
-            raise ValueError("Poses: colors must be a float32 array [n, K, 4]")
-        self.colors = None if colors is None else np.ascontiguousarray(colors)
+        if _is_cuda_array(transforms):
+            self.transforms = _CudaTable("transforms", transforms, ("<f4",))
+        else:
+            self.transforms = None if transforms is None else np.ascontiguousarray(np.asarray(transforms, dtype=np.float32))
+        if _is_cuda_array(visible):
+            self.visible = _CudaTable("visible", visible, ("|u1", "|b1"))
+        else:
+            self.visible = None if visible is None else np.ascontiguousarray(np.asarray(visible).astype(np.uint8))
+        if _is_cuda_array(colors):
+            self.colors = _CudaTable("colors", colors, ("<f4",))
+        else:
+            if colors is not None and (not isinstance(colors, np.ndarray) or colors.dtype != np.float32):
+                raise ValueError("Poses: colors must be a float32 array [n, K, 4]")
+            self.colors = None if colors is None else np.ascontiguousarray(colors)
         if self.transforms is not None and (self.transforms.ndim != 3 or self.transforms.shape[2] != 6):
             raise ValueError(f"Poses: transforms of shape {self.transforms.shape}, not [n, K, 6]")
         if self.visible is not None and self.visible.ndim != 2:
@@ -1042,13 +1086,16 @@ class Renderer:
 
     @staticmethod
     def _pose_args(composition, poses: Poses):
-        """(n, args) for _stack: a chunk's forma_poses holds its frames' rows of the tables."""
+        """(n, args) for _stack: a chunk's forma_poses holds its frames' rows of the tables (of a CUDA
+        table, the address of its first frame's row)."""
         keep = []  # the chunk's descriptor and tables stay alive until the next one
 
         def args(first, count):
-            t, v, c = (None if a is None else np.ascontiguousarray(a[first:first + count])
+            t, v, c = (None if a is None else a if isinstance(a, _CudaTable) else np.ascontiguousarray(a[first:first + count])
                        for a in (poses.transforms, poses.visible, poses.colors))
-            d = _CPoses(poses.first_order, poses.n_orders, *(None if a is None else a.ctypes.data for a in (t, v, c)))
+            d = _CPoses(poses.first_order, poses.n_orders,
+                        *(None if a is None else a.ptr + first * a.row_bytes if isinstance(a, _CudaTable) else a.ctypes.data
+                          for a in (t, v, c)))
             keep[:] = [t, v, c, d]
             return composition._h, C.byref(d), count
         return poses.n, args

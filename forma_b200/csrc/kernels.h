@@ -107,6 +107,21 @@ void launch_line_count_poses(const RasterArgs& args, const PoseArgs& poses, uint
                              uint32_t* max_tile, cudaStream_t stream);
 void launch_raster_emit_poses(const RasterArgs& args, const PoseArgs& poses, uint32_t n_frames, const uint32_t* block_offsets,
                               uint64_t* out, uint32_t cap, cudaStream_t stream, const CountArgs* counts = nullptr);
+// The fold of a poses call's tables into its records (pose_fold_kernel): record r = b * n_orders + k
+// of frame b, order first_order + k, starts from window[k], the layer's own transform and bits with
+// kPoseLayer set (or all zero: the order has no layer, and its record stays zero). transforms[r]
+// replaces the transform ([ux, vx, uy, vy, tx, ty], reordered; an identity is no transform) and
+// visible[r] != 0 the enabled bit. The tables are read where they are passed: in device memory of
+// the caller or as the renderer's copy of host tables.
+constexpr uint32_t kPoseLayer = 4u;  // PoseRec::bits of a window record: a layer is attached at this order
+struct PoseFoldArgs {
+    const PoseRec* window;     // n_orders records
+    const float* transforms;   // nullable: 6 floats per record, 4-byte aligned
+    const uint8_t* visible;    // nullable: 1 byte per record
+    uint32_t n_orders;
+    uint32_t* first_bad;       // nullable: atomicMin of every r whose transform forma_layer_set_transform refuses
+};
+void launch_pose_fold(const PoseFoldArgs& args, PoseRec* recs, uint32_t n_recs, cudaStream_t stream);
 // Batches (see forma_renderer_render_batch_device): frame c of a stack of n_frames frames is a
 // composition of its own. Each frame's line setup reads its composition's segment buffer and
 // tables (as RasterArgs, over the whole frame), and only two key fields move: row t of frame c

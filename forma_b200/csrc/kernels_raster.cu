@@ -631,6 +631,35 @@ __global__ void __launch_bounds__(kRasterThreads, kCount ? 8 : 0) raster_emit_po
     raster_emit_body<false, false, kCount, true>(A, ViewArgs{nullptr, Q.rows}, block_offsets, out, cap, BatchPos{}, C, Q);
 }
 
+// The pose records the two kernels above read, one thread per record (see PoseFoldArgs). A
+// transform is tested as geom_pres_ok (host_path.cpp) tests it, in the same separately rounded f32
+// operations, for every record (orders without a layer included, as check_poses walks them).
+__global__ void __launch_bounds__(256) pose_fold_kernel(PoseFoldArgs F, PoseRec* __restrict__ recs, uint32_t n_recs) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_recs) return;
+    const float4* w = reinterpret_cast<const float4*>(F.window + r % F.n_orders);
+    const float4 a = __ldg(w), b = __ldg(w + 1);
+    float ux = a.x, uy = a.y, vx = a.z, vy = a.w, tx = b.x, ty = b.y;
+    const uint32_t bits = __float_as_uint(b.z);
+    bool has_xf = bits & 1u, enabled = (bits >> 1) & 1u;
+    if (F.transforms) {  // [ux, vx, uy, vy, tx, ty]
+        const float* t = F.transforms + 6ull * r;
+        ux = __ldg(t); vx = __ldg(t + 1); uy = __ldg(t + 2); vy = __ldg(t + 3); tx = __ldg(t + 4); ty = __ldg(t + 5);
+        const float max_x = 1.0f + (1.0f / 16.0f) / 65536.0f, max_y = 1.0f + (1.0f / 16.0f) / 32768.0f;
+        const bool ok = !(__fadd_rn(__fmul_rn(ux, ux), __fmul_rn(uy, uy)) > max_x) && !(__fadd_rn(__fmul_rn(vx, vx), __fmul_rn(vy, vy)) > max_y);
+        if (F.first_bad && !ok) atomicMin(F.first_bad, r);
+        has_xf = !(ux == 1.0f && uy == 0.0f && vx == 0.0f && vy == 1.0f && tx == 0.0f && ty == 0.0f);
+    }
+    if (F.visible) enabled = __ldg(F.visible + r) != 0;
+    float4* out = reinterpret_cast<float4*>(recs + r);
+    if (!(bits & kPoseLayer)) {
+        out[0] = out[1] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        return;
+    }
+    out[0] = make_float4(ux, uy, vx, vy);
+    out[1] = make_float4(tx, ty, __uint_as_float((has_xf ? 1u : 0u) | (enabled ? 2u : 0u)), 0.0f);
+}
+
 // Inspection only (forma_renderer_lines): the line records of segment.rs:298-383 as the
 // reference's SegmentBufferView holds them (segment.rs:530-545), one per point pair; the
 // render path itself never materialises them. `lengths` are per line (the host turns them
@@ -728,6 +757,10 @@ void launch_raster_emit_poses(const RasterArgs& args, const PoseArgs& poses, uin
         raster_emit_poses_kernel<true><<<dim3(nb, n_frames), kRasterThreads, 0, stream>>>(args, poses, block_offsets, out, cap, *counts);
     else
         raster_emit_poses_kernel<false><<<dim3(nb, n_frames), kRasterThreads, 0, stream>>>(args, poses, block_offsets, out, cap, CountArgs{});
+}
+
+void launch_pose_fold(const PoseFoldArgs& args, PoseRec* recs, uint32_t n_recs, cudaStream_t stream) {
+    if (n_recs) pose_fold_kernel<<<(uint32_t)(((uint64_t)n_recs + 255u) / 256u), 256, 0, stream>>>(args, recs, n_recs);
 }
 
 void launch_line_count_batch(const BatchArgs& batch, uint32_t n_ctas, uint32_t* block_sums, uint32_t* total, uint32_t* max_tile,

@@ -631,7 +631,11 @@ int Renderer::render(const FrameRequest& q) {
 // The pose tables of a poses request (see forma_renderer_render_poses_device): a window of 1 to
 // 2^21 orders below 2^21, at least one table, and every transform one forma_layer_set_transform
 // accepts. Colours are any floats (forma_layer_set_props takes them all).
-static int check_poses(const FrameRequest& q) {
+// Where each table lives (pose_tables_on_device): device memory of this renderer's device is read
+// there (a float table must be 4-byte aligned), device memory of another device is refused, and
+// anything else is host memory. Host transforms are checked here; device transforms by the fold
+// (upload_poses), which reports the first record that fails.
+int Renderer::check_poses(const FrameRequest& q) {
     const forma_poses* P = q.poses;
     if (!P || (!P->transforms && !P->visible && !P->colors)) {
         set_error("no %s", P ? "pose table" : "poses");
@@ -644,7 +648,28 @@ static int check_poses(const FrameRequest& q) {
         set_error("invalid poses: orders [%u, %u + %u) (1 to 2^21 orders below 2^21) of %u frames", P->first_order, P->first_order, K, q.n);
         return FORMA_STATUS_INVALID;
     }
-    for (uint64_t r = 0; P->transforms && r < recs; ++r) {  // [ux, vx, uy, vy, tx, ty]
+    const void* const tables[3] = {P->transforms, P->visible, P->colors};
+    static const char* const names[3] = {"transforms", "visible", "colors"};
+    for (int t = 0; t < 3; ++t) {
+        pose_tables_on_device[t] = false;
+        if (!tables[t]) continue;
+        cudaPointerAttributes attr{};
+        if (cudaPointerGetAttributes(&attr, tables[t]) != cudaSuccess) {
+            cudaGetLastError();  // (not memory CUDA knows: host memory)
+            continue;
+        }
+        if (attr.type != cudaMemoryTypeDevice) continue;
+        if (attr.device != device) {
+            set_error("pose table %s is in the memory of device %d; the renderer renders on device %d", names[t], attr.device, device);
+            return FORMA_STATUS_INVALID;
+        }
+        if (t != 1 && ((uintptr_t)tables[t] & 3u) != 0u) {
+            set_error("pose table %s in device memory must be 4-byte aligned", names[t]);
+            return FORMA_STATUS_INVALID;
+        }
+        pose_tables_on_device[t] = true;
+    }
+    for (uint64_t r = 0; P->transforms && !pose_tables_on_device[0] && r < recs; ++r) {  // [ux, vx, uy, vy, tx, ty]
         const float* t = P->transforms + 6u * r;
         if (!geom_pres_ok(t[0], t[2], t[1], t[3])) {
             set_error("pose of frame %llu, order %llu: GeomPresTransformError::ExceededScalingFactor", (unsigned long long)(r / K),
@@ -658,44 +683,71 @@ static int check_poses(const FrameRequest& q) {
 // The pose records of frame b, order first_order + k at b * K + k: the tables' transform and
 // visibility, or the layer's own for a null table. An identity transform is no transform (the
 // rule of forma_layer_set_transform). Orders without a layer keep a zero record: no line reads it.
+// The host builds the window's K records of the layers' own states; pose_fold_kernel folds the
+// tables into them, reading device tables where they are and host tables from a copy of their
+// bytes. Device transforms are checked by the fold: the first that scales up refuses the call,
+// with the message check_poses gives, before line setup (the only synchronisation they add).
 int Renderer::upload_poses(const FrameRequest& q) {
     const forma_poses& P = *q.poses;
     const uint32_t K = P.n_orders;
     const size_t n_recs = (size_t)q.n * K;
-    if (h_poses.reserve(n_recs) != cudaSuccess || d_poses.reserve(n_recs) != cudaSuccess) {
+    const bool host_xf = P.transforms && !pose_tables_on_device[0], host_vis = P.visible && !pose_tables_on_device[1];
+    if (n_recs >= (1ull << 32) || h_pose_window.reserve(K) != cudaSuccess || d_pose_window.reserve(K) != cudaSuccess ||
+        d_poses.reserve(n_recs) != cudaSuccess || h_pose_first_bad.reserve(1) != cudaSuccess || d_pose_first_bad.reserve(1) != cudaSuccess ||
+        (host_xf && (h_pose_xf.reserve(6u * n_recs) != cudaSuccess || d_pose_xf.reserve(6u * n_recs) != cudaSuccess)) ||
+        (host_vis && (h_pose_vis.reserve(n_recs) != cudaSuccess || d_pose_vis.reserve(n_recs) != cudaSuccess))) {
         cudaGetLastError();  // (a failed allocation is not sticky: clear it for the launches' checks)
         set_error("%zu pose records (%zu bytes) could not be allocated", n_recs, n_recs * sizeof(PoseRec));
         return FORMA_STATUS_CAPACITY;
     }
-    // (the previous call's copy is complete: rasterize waited for it)
-    std::memset(h_poses.ptr, 0, n_recs * sizeof(PoseRec));
+    // (the previous call's copies are complete: it ended with a synchronisation)
+    std::memset(h_pose_window.ptr, 0, K * sizeof(PoseRec));
     const auto& layers = q.comp->layers;
     for (auto it = layers.lower_bound(P.first_order); it != layers.end() && it->first - P.first_order < K; ++it) {
-        const uint32_t k = it->first - P.first_order;
         const Layer& l = *it->second;
-        for (uint32_t b = 0; b < q.n; ++b) {
-            const size_t r = (size_t)b * K + k;
-            PoseRec& rec = h_poses.ptr[r];
-            bool has_xf = l.has_xf;
-            if (P.transforms) {
-                const float* t = P.transforms + 6u * r;
-                rec = PoseRec{t[0], t[2], t[1], t[3], t[4], t[5], 0u, 0u};
-                has_xf = !(rec.ux == 1.0f && rec.uy == 0.0f && rec.vx == 0.0f && rec.vy == 1.0f && rec.tx == 0.0f && rec.ty == 0.0f);
-            } else {
-                rec = PoseRec{l.xf[0], l.xf[1], l.xf[2], l.xf[3], l.xf[4], l.xf[5], 0u, 0u};
-            }
-            const bool enabled = P.visible ? P.visible[r] != 0 : l.enabled;
-            rec.bits = (has_xf ? 1u : 0u) | (enabled ? 2u : 0u);
+        h_pose_window.ptr[it->first - P.first_order] = PoseRec{l.xf[0], l.xf[1], l.xf[2], l.xf[3], l.xf[4], l.xf[5],
+                                                                (l.has_xf ? 1u : 0u) | (l.enabled ? 2u : 0u) | kPoseLayer, 0u};
+    }
+    FORMA_CUDA_TRY(cudaMemcpyAsync(d_pose_window.ptr, h_pose_window.ptr, K * sizeof(PoseRec), cudaMemcpyHostToDevice, stream));
+    h2d_bytes += K * sizeof(PoseRec);
+    PoseFoldArgs F{d_pose_window.ptr, P.transforms, P.visible, K, nullptr};
+    if (host_xf) {
+        std::memcpy(h_pose_xf.ptr, P.transforms, 6u * n_recs * sizeof(float));
+        FORMA_CUDA_TRY(cudaMemcpyAsync(d_pose_xf.ptr, h_pose_xf.ptr, 6u * n_recs * sizeof(float), cudaMemcpyHostToDevice, stream));
+        h2d_bytes += 6u * n_recs * sizeof(float);
+        F.transforms = d_pose_xf.ptr;
+    } else if (P.transforms) {
+        FORMA_CUDA_TRY(cudaMemsetAsync(d_pose_first_bad.ptr, 0xFF, sizeof(uint32_t), stream));
+        F.first_bad = d_pose_first_bad.ptr;
+    }
+    if (host_vis) {
+        std::memcpy(h_pose_vis.ptr, P.visible, n_recs);
+        FORMA_CUDA_TRY(cudaMemcpyAsync(d_pose_vis.ptr, h_pose_vis.ptr, n_recs, cudaMemcpyHostToDevice, stream));
+        h2d_bytes += n_recs;
+        F.visible = d_pose_vis.ptr;
+    }
+    launch_pose_fold(F, d_poses.ptr, (uint32_t)n_recs, stream);
+    ++launches;
+    FORMA_CUDA_TRY(cudaGetLastError());
+    if (F.first_bad) {
+        FORMA_CUDA_TRY(cudaMemcpyAsync(h_pose_first_bad.ptr, d_pose_first_bad.ptr, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+        d2h_bytes += sizeof(uint32_t);
+        FORMA_CUDA_TRY(ensure_count_event());
+        FORMA_CUDA_TRY(cudaEventRecord(count_ev, stream));
+        FORMA_CUDA_TRY(cudaEventSynchronize(count_ev));
+        const uint32_t r = *h_pose_first_bad.ptr;
+        if (r != 0xFFFFFFFFu) {
+            set_error("pose of frame %llu, order %llu: GeomPresTransformError::ExceededScalingFactor", (unsigned long long)(r / K),
+                      (unsigned long long)(P.first_order + r % K));
+            return FORMA_STATUS_INVALID;
         }
     }
-    FORMA_CUDA_TRY(cudaMemcpyAsync(d_poses.ptr, h_poses.ptr, n_recs * sizeof(PoseRec), cudaMemcpyHostToDevice, stream));
-    h2d_bytes += n_recs * sizeof(PoseRec);
     return FORMA_STATUS_OK;
 }
 
 // The pose style table of a poses request with colours (see PoseFillArgs): the composition's style
 // records (S.styles, bound by bind_frame), then n K records built on the device from the colours,
-// which go up as 16 bytes per record. S then reads the table.
+// which go up as 16 bytes per record (device colours are copied on the device). S then reads the table.
 int Renderer::upload_pose_fills(const FrameRequest& q, PaintScene& S, PoseFillArgs& fills) {
     const forma_poses& P = *q.poses;
     const Composition& comp = *q.comp;
@@ -705,17 +757,21 @@ int Renderer::upload_pose_fills(const FrameRequest& q, PaintScene& S, PoseFillAr
                   (unsigned long long)n_recs);
         return FORMA_STATUS_CAPACITY;
     }
-    if (h_pose_colors.reserve(n_recs) != cudaSuccess || d_pose_colors.reserve(n_recs) != cudaSuccess ||
+    const bool on_device = pose_tables_on_device[2];
+    if ((!on_device && h_pose_colors.reserve(n_recs) != cudaSuccess) || d_pose_colors.reserve(n_recs) != cudaSuccess ||
         pose_styles.reserve(total) != cudaSuccess) {
         cudaGetLastError();  // (a failed allocation is not sticky: clear it for the launches' checks)
         set_error("a pose style table of %llu records (%llu bytes) could not be allocated", (unsigned long long)total,
                   (unsigned long long)(total * sizeof(StyleRec)));
         return FORMA_STATUS_CAPACITY;
     }
-    // (the previous call's copies are complete: rasterize waited for them)
-    std::memcpy(h_pose_colors.ptr, P.colors, n_recs * sizeof(float4));
-    FORMA_CUDA_TRY(cudaMemcpyAsync(d_pose_colors.ptr, h_pose_colors.ptr, n_recs * sizeof(float4), cudaMemcpyHostToDevice, stream));
-    h2d_bytes += n_recs * sizeof(float4);
+    if (on_device) {  // copied in stream order, as the caller wrote them
+        FORMA_CUDA_TRY(cudaMemcpyAsync(d_pose_colors.ptr, P.colors, n_recs * sizeof(float4), cudaMemcpyDeviceToDevice, stream));
+    } else {  // (the previous call's copies are complete: rasterize waited for them)
+        std::memcpy(h_pose_colors.ptr, P.colors, n_recs * sizeof(float4));
+        FORMA_CUDA_TRY(cudaMemcpyAsync(d_pose_colors.ptr, h_pose_colors.ptr, n_recs * sizeof(float4), cudaMemcpyHostToDevice, stream));
+        h2d_bytes += n_recs * sizeof(float4);
+    }
     if (n_styles)
         FORMA_CUDA_TRY(cudaMemcpyAsync(pose_styles.ptr, S.styles, n_styles * sizeof(StyleRec), cudaMemcpyDeviceToDevice, stream));
     launch_pose_styles(S.order_to_style, S.n_orders, pose_styles.ptr, (uint32_t)n_styles, d_pose_colors.ptr, P.first_order, P.n_orders,

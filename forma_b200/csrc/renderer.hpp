@@ -337,6 +337,7 @@ class Renderer {
     int check_request(const FrameRequest& q);
     int check_masks(const FrameRequest& q);
     int check_stats(const FrameRequest& q);
+    int check_poses(const FrameRequest& q);
     // One frame of S: uploads, line setup, sort, then the painter tables, paint_step and
     // output_step once or, when the sync-free bounds were too small, twice.
     int run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p);
@@ -348,9 +349,21 @@ class Renderer {
     DeviceBuffer<forma_layer_stats> stats_scratch;  // the records of host statistics
     PinnedBuffer<float> h_views;
     DeviceBuffer<float> d_views;
-    PinnedBuffer<PoseRec> h_poses;
+    // Poses: where the current request's transforms, visible and colors tables are (check_poses:
+    // true = device memory of this device, read there), the window's K records as the host builds
+    // them, the copies of host tables, the n x K pose records and the fold's first failing record.
+    bool pose_tables_on_device[3] = {false, false, false};
+    PinnedBuffer<PoseRec> h_pose_window;
+    DeviceBuffer<PoseRec> d_pose_window;
+    PinnedBuffer<float> h_pose_xf;
+    DeviceBuffer<float> d_pose_xf;
+    PinnedBuffer<uint8_t> h_pose_vis;
+    DeviceBuffer<uint8_t> d_pose_vis;
     DeviceBuffer<PoseRec> d_poses;
-    // Folds a poses request's tables into n x K pose records and queues their upload.
+    PinnedBuffer<uint32_t> h_pose_first_bad;
+    DeviceBuffer<uint32_t> d_pose_first_bad;
+    // Queues the window records, the host tables' bytes and pose_fold_kernel, which writes the
+    // n x K pose records; with device transforms, reads back whether the fold refused one.
     int upload_poses(const FrameRequest& q);
     // Pose fills (forma_poses::colors): the colours as uploaded, 16 bytes per record, and the pose
     // style table the call's PaintScene reads (PoseFillArgs).

@@ -621,8 +621,23 @@ int forma_renderer_render_batch_stats_device(forma_renderer*, forma_composition*
  * call is right, forma_renderer_render_device mis-sorts their wrapped tile columns.)
  * The call does not change the composition: afterwards every layer's transform, enabled state and
  * per-cache unchanged bits are what they were, and the next ordinary render uploads nothing
- * because of it. The geometry is flattened and made resident once; per call, n K 32-byte pose
- * records cross PCIe (and n K 16-byte colours with pose fills).
+ * because of it. The geometry is flattened and made resident once; per call, K 32-byte records of
+ * the window's layers cross PCIe, and of the tables in host memory their bytes: n K 24-byte
+ * transforms, n K visibility bytes, n K 16-byte colours. Tables in device memory do not cross.
+ * Where the tables live: each non-null table may be in host memory (pageable, page-locked or
+ * managed) or in device memory of the renderer's device, in any combination, with the same frames,
+ * IDs, masks, statistics and refusals either way. The library asks CUDA
+ * (cudaPointerGetAttributes) where each one is. A device table
+ *   - is read on the renderer's stream (forma_renderer_set_stream): it must be complete in stream
+ *     order on that stream, as the background of the _over_device calls must be;
+ *   - must stay valid until the call returns, which is after the call's final synchronisation;
+ *   - must hold n K rows: its size is the caller's responsibility, as for frame buffers;
+ *   - of transforms or colours must be 4-byte aligned (FORMA_ERR_INVALID_ARGUMENT otherwise,
+ *     before anything is launched); visibility bytes may start at any byte.
+ * A table in device memory of another device is refused with FORMA_ERR_INVALID_ARGUMENT naming
+ * both devices. Device transforms are checked on the device, which costs their calls a 4-byte
+ * read-back and a wait before line setup (calls without them wait for nothing new); a refused
+ * transform leaves buffers and composition as every refusal listed below does.
  * Pose fills (colors not null): the props set in frame b are the layer's own with the fill alone
  * replaced; its fill_rule, is_clipped, blend_mode (the non-separable modes included) and the
  * layer's clip range stay, so a gradient or texture layer of the window becomes solid. A Clip
