@@ -47,6 +47,7 @@ static const OptionName kOptionNames[] = {
     {"sync_free", &Options::sync_free, 0, 1},         {"test_fast_shrink", &Options::test_fast_shrink, 0, 1},
     {"host_slices", &Options::host_slices, 1, 16},    {"slice_bands", &Options::slice_bands, 1, 16},
     {"slice_min_points", &Options::slice_min_points, 0, 1 << 30}, {"slice_chain", &Options::slice_chain, 0, 1},
+    {"pdl", &Options::pdl, 0, 1},
 };
 Options& options() {
     static Options o = [] {
@@ -63,6 +64,8 @@ Options& options() {
     }();
     return o;
 }
+
+bool chained_launches() { return options().pdl != 0; }
 
 // ---------------------------------------------------------------------------
 // Props

@@ -9,6 +9,7 @@
 
 #include <cstdint>
 #include <cstdio>
+#include <utility>
 
 #include "device_types.h"
 
@@ -54,6 +55,30 @@ inline int device_sm_count() {
         sms[d].store(v, std::memory_order_relaxed);
     }
     return v;
+}
+
+// Chained launches (option pdl): the kernels of a frame's chain are launched with programmatic
+// stream serialization, so that a kernel's grid is launched as soon as every CTA of the kernel
+// before it has exited, without waiting for that grid's completion and memory flush, and its CTAs
+// start while the predecessor drains. Every kernel launched this way begins with chain_begin()
+// (below), which waits until the predecessor has completed and its writes are visible. The wait
+// is a no-op in a plain launch (pdl 0).
+bool chained_launches();  // options().pdl != 0
+
+template <class... KArgs, class... Args>
+inline cudaError_t launch_chained(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
+                                  Args&&... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = chained_launches() ? 1u : 0u;
+    return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 
 // Growable device buffer (never shrinks). 80 GB of HBM3 still makes "keep the high
@@ -118,6 +143,15 @@ struct PinnedBuffer {
 
 #ifdef __CUDACC__
 __device__ __forceinline__ unsigned lane_id() { return threadIdx.x & 31u; }
+
+// The first statement of every kernel launched through launch_chained: this CTA waits for the grid
+// before it (griddepcontrol.wait). Every such kernel reaches the wait, so that a wait on the
+// predecessor implies that everything before it has completed too.
+// No kernel triggers its dependents early (griddepcontrol.launch_dependents): the trigger is
+// implicit when a CTA exits. Triggered at the top of every kernel, the CTAs of the next kernels
+// became resident and sat in their waits beside the running grid, and the painter tables of
+// paris@4K took 0.166 instead of 0.149 ms (DESIGN.md section 6).
+__device__ __forceinline__ void chain_begin() { cudaGridDependencySynchronize(); }
 
 __device__ __forceinline__ float d_rcp(float v) { return 1.0f / v; }   // IEEE division (-prec-div=true)
 __device__ __forceinline__ float d_mix(float t, float a, float b) { return fmaf(t, b, fmaf(-t, a, a)); }

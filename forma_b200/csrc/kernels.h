@@ -34,6 +34,7 @@ struct Options {
     int slice_bands = 2;     //   ... copy bands inside a slice
     int slice_min_points = 65536;  //   ... only for compositions of at least this many points
     int slice_chain = 1;     //   ... uploads issued slice after slice, each waiting for the one before (0: all at once from the slices' threads)
+    int pdl = 1;             // chained launches: the frame's kernels launched with programmatic dependent launch (0: plain launches)
 };
 Options& options();
 
@@ -252,7 +253,9 @@ void launch_radix_hist(const uint64_t* keys, uint32_t n, const SortPlan& plan, u
                        cudaStream_t stream);
 SortResult launch_radix_sort(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals, uint32_t* vals_tmp, uint32_t n,
                              const SortPlan& plan, void* scratch, cudaStream_t stream,
-                             cudaEvent_t* pass_events = nullptr /* 3 per pass: before upsweep, before / after downsweep */,
+                             cudaEvent_t* pass_events = nullptr /* 3 per pass, of which the sort records [3p + 1] (before the downsweep) and [3p + 2] (after it) but
+                                                                  not the last pass's [3p + 2]: pass p starts at the event recorded before it (the caller's before the sort, pass p - 1's
+                                                                  end) and the last pass ends at the caller's after the sort. Fewer event records between the kernels */,
                              const uint32_t* n_dev = nullptr /* the key count in device memory; `n` is then its upper bound
                                                                 and a larger count sorts nothing (single-sweep passes only) */,
                              const uint32_t* hist = nullptr /* [kMaxSortPasses][256] digit counts of every planned pass,
@@ -309,6 +312,12 @@ struct TableScratch {
 };
 TableScratch table_scratch_layout(uint32_t n, uint32_t n_cells, uint32_t n_gaps, const SortPlan& carry_plan,
                                   const SortPlan& gap_plan);
+// Bytes [0, a_bytes) of a and [0, b_bytes) of b, and *word when not null, set to zero by one chained
+// kernel (not counted as a launch).
+void launch_zero_tables(uint8_t* a, size_t a_bytes, uint8_t* b, size_t b_bytes, uint32_t* word, cudaStream_t st);
+// dst[0, n) = src[0, n), n <= 256, by one chained kernel (not counted as a launch); dst may be the
+// device address of pinned host memory.
+void launch_copy_words(const uint32_t* src, uint32_t* dst, uint32_t n, cudaStream_t st);
 // Cells in one pass over the sorted segments (+ a small kernel for the cells that cross a
 // CTA tile): cell_start[c] = first segment of cell c (cell_start[#cells] = n), the cell's
 // cover (16 x i8 by local_y), its key, the (tile_y, layer, tile_x) key of the carry pass and
@@ -390,12 +399,13 @@ struct TileTables {
     const uint32_t* heavy_count;
 };
 // The tile kernels below are persistent: their warps take the tiles of S's tile rectangle by ticket
-// from `tile_counter`, which the launcher resets on `st`. Nothing is launched for an empty rectangle.
+// from `tile_counter`, which the launcher resets on `st` (launch_paint: unless counter_zeroed, when a
+// kernel earlier on `st` has cleared it). Nothing is launched for an empty rectangle.
 // view_rows != 0: S stacks views of view_rows tile rows each (ViewArgs); gradients and textures are
 // then sampled in each view's own coordinates. solid_over: every layer of the frame is a solid `Over`
 // fill without clips (Composition::solid_over_only); the lean build of the kernel paints it.
 void launch_paint(const PaintScene& S, const TileTables& t, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter,
-                  cudaStream_t st, uint32_t view_rows = 0, bool solid_over = false);
+                  cudaStream_t st, uint32_t view_rows = 0, bool solid_over = false, bool counter_zeroed = false);
 // launch_paint for a linear float frame of `bpp` bytes per pixel: 8 (RGBA16F) or 16 (RGBA32F), the
 // painter's planes in channel order where launch_paint stores their sRGB bytes (see
 // forma_renderer_render_linear). `framebuffer` and S.stride: multiples of 4 bytes.

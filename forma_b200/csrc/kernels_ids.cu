@@ -390,6 +390,7 @@ __device__ __forceinline__ void store_ids(const PaintScene& S, const IdsOut& f, 
 }
 
 __global__ void __launch_bounds__(kIdWarpsPerBlock * 32) paint_ids_kernel(PaintScene S, IdTables T, IdsOut f, uint32_t n_tiles) {
+    chain_begin();
     ids_walk(S, T, n_tiles, f.min_coverage,
              [&](const uint32_t* ids, uint32_t ty, uint32_t tx, uint32_t lane) { store_ids(S, f, ids, ty, tx, lane, 0u); });
 }
@@ -397,6 +398,7 @@ __global__ void __launch_bounds__(kIdWarpsPerBlock * 32) paint_ids_kernel(PaintS
 // frames[c].order_base + order, and the IDs stored are the frame's own orders.
 __global__ void __launch_bounds__(kIdWarpsPerBlock * 32) paint_ids_stacked_kernel(PaintScene S, IdTables T, IdsOut f, uint32_t n_tiles,
                                                                                   uint32_t rows, const BatchFrame* __restrict__ frames) {
+    chain_begin();
     ids_walk(S, T, n_tiles, f.min_coverage, [&](const uint32_t* ids, uint32_t ty, uint32_t tx, uint32_t lane) {
         store_ids(S, f, ids, ty, tx, lane, frame_row(ty, rows, frames).base);
     });
@@ -413,8 +415,8 @@ void launch_paint_ids(const PaintScene& S, const TileTables& t, uint8_t* id_flag
     if (!g.n_tiles) return;
     const IdTables T = id_tables(S, t, id_flags, tile_counter);
     const IdsOut f{ids, ids_stride, min_coverage};
-    if (frames) paint_ids_stacked_kernel<<<g.ctas, kIdWarpsPerBlock * 32, 0, st>>>(S, T, f, g.n_tiles, rows, frames);
-    else paint_ids_kernel<<<g.ctas, kIdWarpsPerBlock * 32, 0, st>>>(S, T, f, g.n_tiles);
+    if (frames) launch_chained(paint_ids_stacked_kernel, g.ctas, kIdWarpsPerBlock * 32, 0, st, S, T, f, g.n_tiles, rows, frames);
+    else launch_chained(paint_ids_kernel, g.ctas, kIdWarpsPerBlock * 32, 0, st, S, T, f, g.n_tiles);
 }
 
 // ---------------------------------------------------------------------------
@@ -722,12 +724,14 @@ __device__ __forceinline__ void amodal_walk(const PaintScene& S, const IdTables&
 
 __global__ void __launch_bounds__(kIdWarpsPerBlock * 32) paint_masks_kernel(PaintScene S, IdTables T, OrderWindow w, MaskOut m,
                                                                             uint32_t n_tiles) {
+    chain_begin();
     amodal_walk(S, T, w, n_tiles, nullptr, [&](const LaneTile& t, uint32_t k, const float* cov, bool) { store_mask(w, m, t, k, cov); });
 }
 // S stacks the frames of a batch; frame c's entries carry frames[c].order_base + order, and its
 // planes hold the frame's own orders.
 __global__ void __launch_bounds__(kIdWarpsPerBlock * 32) paint_masks_stacked_kernel(PaintScene S, IdTables T, OrderWindow w, MaskOut m,
                                                                                     uint32_t n_tiles, const BatchFrame* __restrict__ frames) {
+    chain_begin();
     amodal_walk(S, T, w, n_tiles, frames, [&](const LaneTile& t, uint32_t k, const float* cov, bool) { store_mask(w, m, t, k, cov); });
 }
 
@@ -737,6 +741,7 @@ constexpr int kZeroWarps = 8;
 __global__ void __launch_bounds__(kZeroWarps * 32) zero_masks_kernel(uint8_t* out, uint64_t stride, uint64_t plane_stride,
                                                                      uint32_t n_planes, uint32_t y0, uint32_t n_rows, uint64_t x0,
                                                                      uint64_t row_bytes) {
+    chain_begin();
     const uint32_t lane = threadIdx.x & 31u;
     const uint64_t total = (uint64_t)n_planes * n_rows;
     for (uint64_t r = (uint64_t)blockIdx.x * kZeroWarps + (threadIdx.x >> 5); r < total; r += (uint64_t)gridDim.x * kZeroWarps) {
@@ -762,13 +767,13 @@ uint32_t launch_paint_masks(const PaintScene& S, const TileTables& t, uint8_t* i
     const uint32_t x0 = rows ? 0u : S.tx_lo * 16u, x1 = rows ? S.width : min(S.tx_hi * 16u, S.width);
     const uint64_t n_rows = (uint64_t)m.n_frames * m.n_orders * (y1 - y0);
     const uint32_t zero_ctas = (uint32_t)std::min<uint64_t>((n_rows + kZeroWarps - 1) / kZeroWarps, 8u * (uint64_t)device_sm_count());
-    zero_masks_kernel<<<zero_ctas, kZeroWarps * 32, 0, st>>>(m.ptr, m.stride, m.plane_stride, m.n_frames * m.n_orders, y0, y1 - y0,
+    launch_chained(zero_masks_kernel, zero_ctas, kZeroWarps * 32, 0, st, m.ptr, m.stride, m.plane_stride, m.n_frames * m.n_orders, y0, y1 - y0,
                                                              (uint64_t)x0 * bpp, (uint64_t)(x1 - x0) * bpp);
     const IdTables T = id_tables(S, t, id_flags, tile_counter);
     const OrderWindow w{m.first_order, m.n_orders, m.height, rows};
     const MaskOut out{m.ptr, m.stride, m.plane_stride, m.format == FORMA_MASK_U8};
-    if (frames) paint_masks_stacked_kernel<<<g.ctas, kIdWarpsPerBlock * 32, 0, st>>>(S, T, w, out, g.n_tiles, frames);
-    else paint_masks_kernel<<<g.ctas, kIdWarpsPerBlock * 32, 0, st>>>(S, T, w, out, g.n_tiles);
+    if (frames) launch_chained(paint_masks_stacked_kernel, g.ctas, kIdWarpsPerBlock * 32, 0, st, S, T, w, out, g.n_tiles, frames);
+    else launch_chained(paint_masks_kernel, g.ctas, kIdWarpsPerBlock * 32, 0, st, S, T, w, out, g.n_tiles);
     return 2;
 }
 
@@ -776,17 +781,20 @@ uint32_t launch_paint_masks(const PaintScene& S, const TileTables& t, uint8_t* i
 // and the ID walk of the ID kernel, each single-frame / views and batch.
 __global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_amodal_kernel(PaintScene S, IdTables T, OrderWindow w, StatsOut so,
                                                                              uint32_t n_tiles) {
+    chain_begin();
     amodal_walk(S, T, w, n_tiles, nullptr,
                 [&](const LaneTile& t, uint32_t k, const float* cov, bool full) { add_amodal(S, w, so, t, k, cov, full); });
 }
 __global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_amodal_stacked_kernel(PaintScene S, IdTables T, OrderWindow w,
                                                                                      StatsOut so, uint32_t n_tiles,
                                                                                      const BatchFrame* __restrict__ frames) {
+    chain_begin();
     amodal_walk(S, T, w, n_tiles, frames,
                 [&](const LaneTile& t, uint32_t k, const float* cov, bool full) { add_amodal(S, w, so, t, k, cov, full); });
 }
 __global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_visible_kernel(PaintScene S, IdTables T, OrderWindow w, StatsOut so,
                                                                               uint32_t n_tiles) {
+    chain_begin();
     ids_walk(S, T, n_tiles, so.min_coverage, [&](const uint32_t* ids, uint32_t ty, uint32_t tx, uint32_t lane) {
         add_visible(S, w, so, ids, ty, tx, lane, nullptr);
     });
@@ -794,6 +802,7 @@ __global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_visible_kernel(Pa
 __global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_visible_stacked_kernel(PaintScene S, IdTables T, OrderWindow w,
                                                                                       StatsOut so, uint32_t n_tiles,
                                                                                       const BatchFrame* __restrict__ frames) {
+    chain_begin();
     ids_walk(S, T, n_tiles, so.min_coverage, [&](const uint32_t* ids, uint32_t ty, uint32_t tx, uint32_t lane) {
         add_visible(S, w, so, ids, ty, tx, lane, frames);
     });
@@ -801,6 +810,7 @@ __global__ void __launch_bounds__(kIdWarpsPerBlock * 32) stats_visible_stacked_k
 
 // Every record to 0 with the boxes' min / max sentinels {~0, ~0, 0, 0}.
 __global__ void init_stats_kernel(forma_layer_stats* rec, uint64_t n) {
+    chain_begin();
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
         uint2* r = reinterpret_cast<uint2*>(rec + i);  // 8-byte aligned (check_stats)
         r[0] = make_uint2(0u, 0u);             // area
@@ -813,6 +823,7 @@ __global__ void init_stats_kernel(forma_layer_stats* rec, uint64_t n) {
 }
 // The box of an empty set to {0, 0, 0, 0}.
 __global__ void fix_stats_kernel(forma_layer_stats* rec, uint64_t n) {
+    chain_begin();
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
         forma_layer_stats& r = rec[i];
         if (r.pixels == 0u) r.box[0] = r.box[1] = 0u;
@@ -824,7 +835,7 @@ uint32_t launch_paint_stats(const PaintScene& S, const TileTables& t, uint8_t* i
                             cudaStream_t st, uint32_t rows, const BatchFrame* frames) {
     const uint64_t n_rec = (uint64_t)f.n_frames * f.n_orders;
     const uint32_t rec_ctas = (uint32_t)std::min<uint64_t>((n_rec + 255u) / 256u, 8u * (uint64_t)device_sm_count());
-    init_stats_kernel<<<rec_ctas, 256, 0, st>>>(f.ptr, n_rec);
+    launch_chained(init_stats_kernel, rec_ctas, 256, 0, st, f.ptr, n_rec);
     uint32_t launches = 2;
     const IdTables T = id_tables(S, t, id_flags, tile_counter);
     const OrderWindow w{f.first_order, f.n_orders, f.height, rows};
@@ -833,15 +844,15 @@ uint32_t launch_paint_stats(const PaintScene& S, const TileTables& t, uint8_t* i
     const void* amodal = frames ? (const void*)stats_amodal_stacked_kernel : (const void*)stats_amodal_kernel;
     const TileGrid g = tile_grid(S, amodal, kIdWarpsPerBlock, tile_counter, st);
     if (g.n_tiles) {
-        if (frames) stats_amodal_stacked_kernel<<<g.ctas, block, 0, st>>>(S, T, w, so, g.n_tiles, frames);
-        else stats_amodal_kernel<<<g.ctas, block, 0, st>>>(S, T, w, so, g.n_tiles);
+        if (frames) launch_chained(stats_amodal_stacked_kernel, g.ctas, block, 0, st, S, T, w, so, g.n_tiles, frames);
+        else launch_chained(stats_amodal_kernel, g.ctas, block, 0, st, S, T, w, so, g.n_tiles);
         const void* visible = frames ? (const void*)stats_visible_stacked_kernel : (const void*)stats_visible_kernel;
         const TileGrid v = tile_grid(S, visible, kIdWarpsPerBlock, tile_counter, st);
-        if (frames) stats_visible_stacked_kernel<<<v.ctas, block, 0, st>>>(S, T, w, so, v.n_tiles, frames);
-        else stats_visible_kernel<<<v.ctas, block, 0, st>>>(S, T, w, so, v.n_tiles);
+        if (frames) launch_chained(stats_visible_stacked_kernel, v.ctas, block, 0, st, S, T, w, so, v.n_tiles, frames);
+        else launch_chained(stats_visible_kernel, v.ctas, block, 0, st, S, T, w, so, v.n_tiles);
         launches += 2;
     }
-    fix_stats_kernel<<<rec_ctas, 256, 0, st>>>(f.ptr, n_rec);
+    launch_chained(fix_stats_kernel, rec_ctas, 256, 0, st, f.ptr, n_rec);
     return launches;
 }
 

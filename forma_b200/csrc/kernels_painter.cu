@@ -311,6 +311,7 @@ struct WarpSmem {
 
 template <int kMinBlocks>
 __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, kMinBlocks) paint_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles) {
+    chain_begin();
 #define FORMA_PAINT_FRAME_TY(ty) (ty)
 #include "paint_kernel_body.cuh"
 #undef FORMA_PAINT_FRAME_TY
@@ -320,6 +321,7 @@ __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, kMinBlocks) paint_ke
 template <int kMinBlocks>
 __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, kMinBlocks)
     paint_views_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles, uint32_t view_rows) {
+    chain_begin();
 #define FORMA_PAINT_FRAME_TY(ty) ((ty) % view_rows)
 #include "paint_kernel_body.cuh"
 #undef FORMA_PAINT_FRAME_TY
@@ -331,6 +333,7 @@ __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, kMinBlocks)
 #define FORMA_PAINT_SOLID_OVER
 template <int kMinBlocks>
 __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, kMinBlocks) paint_solid_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles) {
+    chain_begin();
 #define FORMA_PAINT_FRAME_TY(ty) (ty)
 #include "paint_kernel_body.cuh"
 #undef FORMA_PAINT_FRAME_TY
@@ -338,6 +341,7 @@ __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, kMinBlocks) paint_so
 template <int kMinBlocks>
 __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, kMinBlocks)
     paint_views_solid_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles, uint32_t view_rows) {
+    chain_begin();
 #define FORMA_PAINT_FRAME_TY(ty) ((ty) % view_rows)
 #include "paint_kernel_body.cuh"
 #undef FORMA_PAINT_FRAME_TY
@@ -417,12 +421,14 @@ __device__ __forceinline__ void store_tile_solid_linear(const PaintScene& S, uin
     store_linear_run(S, in.framebuffer, ty * 16u + row, x0, dr, dg, db, da, vec_ok, bpp)
 __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, 8)
     paint_linear_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles, uint32_t bpp) {
+    chain_begin();
 #define FORMA_PAINT_FRAME_TY(ty) (ty)
 #include "paint_kernel_body.cuh"
 #undef FORMA_PAINT_FRAME_TY
 }
 __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, 8)
     paint_views_linear_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles, uint32_t view_rows, uint32_t bpp) {
+    chain_begin();
 #define FORMA_PAINT_FRAME_TY(ty) ((ty) % view_rows)
 #include "paint_kernel_body.cuh"
 #undef FORMA_PAINT_FRAME_TY
@@ -581,6 +587,7 @@ __device__ __forceinline__ void store_srgb_run(const PaintScene& S, uint8_t* fb,
     upgrade_alpha(da, bg_opaque); \
     store_srgb_run(S, in.framebuffer, ty * 16u + row, x0, dr, dg, db, da, vec_ok, rgba_order)
 __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, 8) paint_over_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles) {
+    chain_begin();
     FORMA_PAINT_OVER_SRGB_PROLOGUE
 #define FORMA_PAINT_FRAME_TY(ty) (ty)
 #include "paint_kernel_body.cuh"
@@ -588,6 +595,7 @@ __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, 8) paint_over_kernel
 }
 __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, 8)
     paint_views_over_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles, uint32_t view_rows) {
+    chain_begin();
     FORMA_PAINT_OVER_SRGB_PROLOGUE
 #define FORMA_PAINT_FRAME_TY(ty) ((ty) % view_rows)
 #include "paint_kernel_body.cuh"
@@ -604,6 +612,7 @@ __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, 8)
     store_linear_run(S, in.framebuffer, ty * 16u + row, x0, dr, dg, db, da, vec_ok, bpp)
 __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, 8)
     paint_over_linear_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles, uint32_t bpp) {
+    chain_begin();
     const uint32_t over_pos = channel_positions(S.channels);
 #define FORMA_PAINT_FRAME_TY(ty) (ty)
 #include "paint_kernel_body.cuh"
@@ -611,6 +620,7 @@ __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, 8)
 }
 __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, 8)
     paint_views_over_linear_kernel(PaintScene S, PaintInputs in, uint32_t n_tiles, uint32_t view_rows, uint32_t bpp) {
+    chain_begin();
     const uint32_t over_pos = channel_positions(S.channels);
 #define FORMA_PAINT_FRAME_TY(ty) ((ty) % view_rows)
 #include "paint_kernel_body.cuh"
@@ -626,6 +636,7 @@ __global__ void __launch_bounds__(kPaintWarpsPerBlock * 32, 8)
 __global__ void __launch_bounds__(256) unpack_views_kernel(const uint8_t* __restrict__ src, uint64_t stride, uint64_t view_stride,
                                                            uint8_t* __restrict__ dst, uint64_t dst_stride, uint32_t view_rows_px,
                                                            uint32_t width, uint32_t height) {
+    chain_begin();
     const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t r = blockIdx.y, b = blockIdx.z;
     if (x >= width) return;
@@ -636,7 +647,7 @@ __global__ void __launch_bounds__(256) unpack_views_kernel(const uint8_t* __rest
 void launch_unpack_views(const uint8_t* src, uint64_t stride, uint64_t view_stride, uint8_t* dst, uint64_t dst_stride,
                          uint32_t view_rows_px, uint32_t width, uint32_t height, uint32_t n_views, cudaStream_t st) {
     if (!width || !height || !n_views) return;
-    unpack_views_kernel<<<dim3((width + 255u) / 256u, height, n_views), 256, 0, st>>>(src, stride, view_stride, dst, dst_stride,
+    launch_chained(unpack_views_kernel, dim3((width + 255u) / 256u, height, n_views), 256, 0, st, src, stride, view_stride, dst, dst_stride,
                                                                                       view_rows_px, width, height);
 }
 
@@ -646,6 +657,7 @@ void launch_unpack_views(const uint8_t* src, uint64_t stride, uint64_t view_stri
 __global__ void __launch_bounds__(256) repack_views_kernel(const uint8_t* __restrict__ src, uint64_t src_stride, uint32_t view_rows_px,
                                                            uint8_t* __restrict__ dst, uint64_t stride, uint64_t view_stride,
                                                            uint32_t width, uint32_t height, bool aligned) {
+    chain_begin();
     const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t r = blockIdx.y, b = blockIdx.z;
     if (x >= width) return;
@@ -662,7 +674,7 @@ void launch_repack_views(const uint8_t* src, uint64_t src_stride, uint32_t view_
                          uint64_t view_stride, uint32_t width, uint32_t height, uint32_t n_views, cudaStream_t st) {
     if (!width || !height || !n_views) return;
     const bool aligned = (((uintptr_t)dst | stride | view_stride | (uintptr_t)src | src_stride) & 3u) == 0u;
-    repack_views_kernel<<<dim3((width + 255u) / 256u, height, n_views), 256, 0, st>>>(src, src_stride, view_rows_px, dst, stride,
+    launch_chained(repack_views_kernel, dim3((width + 255u) / 256u, height, n_views), 256, 0, st, src, src_stride, view_rows_px, dst, stride,
                                                                                      view_stride, width, height, aligned);
 }
 
@@ -673,6 +685,7 @@ __global__ void __launch_bounds__(256) gather_tiles_kernel(const uint8_t* __rest
                                                            uint32_t height, uint32_t tiles_x,
                                                            const uint32_t* __restrict__ list,
                                                            const uint32_t* __restrict__ count, uint32_t* __restrict__ out) {
+    chain_begin();
     const uint32_t n = *count;
     const uint32_t lane = threadIdx.x & 31u;
     for (uint32_t i = blockIdx.x * 8u + (threadIdx.x >> 5); i < n; i += gridDim.x * 8u) {
@@ -690,7 +703,7 @@ __global__ void __launch_bounds__(256) gather_tiles_kernel(const uint8_t* __rest
 }
 
 void launch_gather_tiles(const PaintScene& S, const uint8_t* framebuffer, uint32_t* packed, cudaStream_t st) {
-    gather_tiles_kernel<<<device_sm_count() * 4, 256, 0, st>>>(framebuffer, S.stride, S.width, S.height, S.tiles_x, S.written_list,
+    launch_chained(gather_tiles_kernel, device_sm_count() * 4, 256, 0, st, framebuffer, S.stride, S.width, S.height, S.tiles_x, S.written_list,
                                                                S.written_count, packed);
 }
 
@@ -768,10 +781,11 @@ void launch_f32x2_selftest(const float* a, const float* b, const float* c, uint3
 
 // Several host threads may render on one device, and paint_kernel<8> and paint_kernel<6> share a
 // type: the occupancy cache is keyed by the kernel's address and the device, under one lock.
-TileGrid tile_grid(const PaintScene& S, const void* kernel, uint32_t warps, uint32_t* tile_counter, cudaStream_t st) {
+TileGrid tile_grid(const PaintScene& S, const void* kernel, uint32_t warps, uint32_t* tile_counter, cudaStream_t st,
+                   bool counter_zeroed) {
     if (S.tx_hi <= S.tx_lo || S.ty_hi <= S.ty_lo) return TileGrid{0u, 0u};
     const uint32_t n_tiles = (S.tx_hi - S.tx_lo) * (S.ty_hi - S.ty_lo);
-    cudaMemsetAsync(tile_counter, 0, sizeof(uint32_t), st);
+    if (!counter_zeroed) cudaMemsetAsync(tile_counter, 0, sizeof(uint32_t), st);
     static std::mutex mu;
     static std::map<std::pair<const void*, int>, int> blocks_per_sm;
     int per_sm = 0;
@@ -793,7 +807,7 @@ static PaintInputs paint_inputs(const PaintScene& S, const TileTables& t, uint8_
 }
 
 void launch_paint(const PaintScene& S, const TileTables& t, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter,
-                  cudaStream_t st, uint32_t view_rows, bool solid_over) {
+                  cudaStream_t st, uint32_t view_rows, bool solid_over, bool counter_zeroed) {
     // Build 0: the general kernel at 128 registers (8 CTAs / SM); 1: option paint_wide = 1, up to 168
     // registers (6 CTAs / SM); 2: a solid `Over` frame (option paint_solid = 1), the lean build at 96
     // registers (10 CTAs / SM).
@@ -802,11 +816,11 @@ void launch_paint(const PaintScene& S, const TileTables& t, uint8_t* eflags, uin
     void (*const views[3])(PaintScene, PaintInputs, uint32_t, uint32_t) = {paint_views_kernel<8>, paint_views_kernel<6>,
                                                                             paint_views_solid_kernel<8>};
     const void* kernel = view_rows ? (const void*)views[build] : (const void*)frame[build];
-    const TileGrid g = tile_grid(S, kernel, kPaintWarpsPerBlock, tile_counter, st);
+    const TileGrid g = tile_grid(S, kernel, kPaintWarpsPerBlock, tile_counter, st, counter_zeroed);
     if (!g.n_tiles) return;
     const PaintInputs in = paint_inputs(S, t, eflags, framebuffer, tile_counter);
-    if (view_rows) views[build]<<<g.ctas, kPaintWarpsPerBlock * 32, 0, st>>>(S, in, g.n_tiles, view_rows);
-    else frame[build]<<<g.ctas, kPaintWarpsPerBlock * 32, 0, st>>>(S, in, g.n_tiles);
+    if (view_rows) launch_chained(views[build], g.ctas, kPaintWarpsPerBlock * 32, 0, st, S, in, g.n_tiles, view_rows);
+    else launch_chained(frame[build], g.ctas, kPaintWarpsPerBlock * 32, 0, st, S, in, g.n_tiles);
 }
 
 void launch_paint_linear(const PaintScene& S, const TileTables& t, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter,
@@ -815,8 +829,8 @@ void launch_paint_linear(const PaintScene& S, const TileTables& t, uint8_t* efla
     const TileGrid g = tile_grid(S, kernel, kPaintWarpsPerBlock, tile_counter, st);
     if (!g.n_tiles) return;
     const PaintInputs in = paint_inputs(S, t, eflags, framebuffer, tile_counter);
-    if (view_rows) paint_views_linear_kernel<<<g.ctas, kPaintWarpsPerBlock * 32, 0, st>>>(S, in, g.n_tiles, view_rows, bpp);
-    else paint_linear_kernel<<<g.ctas, kPaintWarpsPerBlock * 32, 0, st>>>(S, in, g.n_tiles, bpp);
+    if (view_rows) launch_chained(paint_views_linear_kernel, g.ctas, kPaintWarpsPerBlock * 32, 0, st, S, in, g.n_tiles, view_rows, bpp);
+    else launch_chained(paint_linear_kernel, g.ctas, kPaintWarpsPerBlock * 32, 0, st, S, in, g.n_tiles, bpp);
 }
 
 void launch_paint_over(const PaintScene& S, const TileTables& t, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter,
@@ -829,11 +843,11 @@ void launch_paint_over(const PaintScene& S, const TileTables& t, uint8_t* eflags
     const PaintInputs in = paint_inputs(S, t, eflags, framebuffer, tile_counter);
     const uint32_t block = kPaintWarpsPerBlock * 32;
     if (view_rows) {
-        if (linear) paint_views_over_linear_kernel<<<g.ctas, block, 0, st>>>(S, in, g.n_tiles, view_rows, bpp);
-        else paint_views_over_kernel<<<g.ctas, block, 0, st>>>(S, in, g.n_tiles, view_rows);
+        if (linear) launch_chained(paint_views_over_linear_kernel, g.ctas, block, 0, st, S, in, g.n_tiles, view_rows, bpp);
+        else launch_chained(paint_views_over_kernel, g.ctas, block, 0, st, S, in, g.n_tiles, view_rows);
     } else {
-        if (linear) paint_over_linear_kernel<<<g.ctas, block, 0, st>>>(S, in, g.n_tiles, bpp);
-        else paint_over_kernel<<<g.ctas, block, 0, st>>>(S, in, g.n_tiles);
+        if (linear) launch_chained(paint_over_linear_kernel, g.ctas, block, 0, st, S, in, g.n_tiles, bpp);
+        else launch_chained(paint_over_kernel, g.ctas, block, 0, st, S, in, g.n_tiles);
     }
 }
 

@@ -419,6 +419,7 @@ __global__ void __launch_bounds__(kRasterThreads) line_count_poses_kernel(Raster
 // offset and the total are min(true value, 0xFFFFFFFF).
 __global__ void __launch_bounds__(1024) scan_block_sums_kernel(uint32_t* __restrict__ data, uint32_t n,
                                                               uint32_t* __restrict__ total) {
+    chain_begin();
     __shared__ uint32_t warp_tot[32];
     __shared__ uint32_t carry, round_total;
     if (threadIdx.x == 0) carry = 0;
@@ -635,6 +636,7 @@ __global__ void __launch_bounds__(kRasterThreads, kCount ? 8 : 0) raster_emit_po
 // transform is tested as geom_pres_ok (host_path.cpp) tests it, in the same separately rounded f32
 // operations, for every record (orders without a layer included, as check_poses walks them).
 __global__ void __launch_bounds__(256) pose_fold_kernel(PoseFoldArgs F, PoseRec* __restrict__ recs, uint32_t n_recs) {
+    chain_begin();
     const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n_recs) return;
     const float4* w = reinterpret_cast<const float4*>(F.window + r % F.n_orders);
@@ -693,6 +695,10 @@ void launch_flatten_eval(const SplineRec* splines, const PointRec* points, const
                                                                     dst_base, x, y, gid);
 }
 
+// The count and emit passes are plain launches: the stream hands each of them a memset (max_tile)
+// or the count read-back right before, which a chained launch cannot overlap either, and as plain
+// launches they keep their read-only (LDG.CONSTANT) loads of the segment buffer and the layer
+// tables. The scan after the count pass is chained (launch_chained).
 uint32_t raster_num_blocks(uint32_t n_points) { return n_points ? (n_points + kRasterThreads - 1) / kRasterThreads : 0; }
 
 void launch_line_count(const RasterArgs& args, uint32_t* block_sums, uint32_t* total, uint32_t* max_tile,
@@ -704,7 +710,7 @@ void launch_line_count(const RasterArgs& args, uint32_t* block_sums, uint32_t* t
         return;
     }
     line_count_kernel<<<nb, kRasterThreads, 0, stream>>>(args, block_sums, max_tile);
-    scan_block_sums_kernel<<<1, 1024, 0, stream>>>(block_sums, nb, total);
+    launch_chained(scan_block_sums_kernel, 1, 1024, 0, stream, block_sums, nb, total);
 }
 
 void launch_raster_emit(const RasterArgs& args, const uint32_t* block_offsets, uint64_t* out, uint32_t cap, cudaStream_t stream,
@@ -724,7 +730,7 @@ void launch_line_count_views(const RasterArgs& args, const ViewArgs& views, uint
         return;
     }
     line_count_views_kernel<<<dim3(nb, n_views), kRasterThreads, 0, stream>>>(args, views, block_sums, max_tile);
-    scan_block_sums_kernel<<<1, 1024, 0, stream>>>(block_sums, nb * n_views, total);
+    launch_chained(scan_block_sums_kernel, 1, 1024, 0, stream, block_sums, nb * n_views, total);
 }
 
 void launch_raster_emit_views(const RasterArgs& args, const ViewArgs& views, uint32_t n_views, const uint32_t* block_offsets,
@@ -746,7 +752,7 @@ void launch_line_count_poses(const RasterArgs& args, const PoseArgs& poses, uint
         return;
     }
     line_count_poses_kernel<<<dim3(nb, n_frames), kRasterThreads, 0, stream>>>(args, poses, block_sums, max_tile);
-    scan_block_sums_kernel<<<1, 1024, 0, stream>>>(block_sums, nb * n_frames, total);
+    launch_chained(scan_block_sums_kernel, 1, 1024, 0, stream, block_sums, nb * n_frames, total);
 }
 
 void launch_raster_emit_poses(const RasterArgs& args, const PoseArgs& poses, uint32_t n_frames, const uint32_t* block_offsets,
@@ -760,7 +766,7 @@ void launch_raster_emit_poses(const RasterArgs& args, const PoseArgs& poses, uin
 }
 
 void launch_pose_fold(const PoseFoldArgs& args, PoseRec* recs, uint32_t n_recs, cudaStream_t stream) {
-    if (n_recs) pose_fold_kernel<<<(uint32_t)(((uint64_t)n_recs + 255u) / 256u), 256, 0, stream>>>(args, recs, n_recs);
+    if (n_recs) launch_chained(pose_fold_kernel, (uint32_t)(((uint64_t)n_recs + 255u) / 256u), 256, 0, stream, args, recs, n_recs);
 }
 
 void launch_line_count_batch(const BatchArgs& batch, uint32_t n_ctas, uint32_t* block_sums, uint32_t* total, uint32_t* max_tile,
@@ -771,7 +777,7 @@ void launch_line_count_batch(const BatchArgs& batch, uint32_t n_ctas, uint32_t* 
         return;
     }
     line_count_batch_kernel<<<n_ctas, kRasterThreads, 0, stream>>>(batch, block_sums, max_tile);
-    scan_block_sums_kernel<<<1, 1024, 0, stream>>>(block_sums, n_ctas, total);
+    launch_chained(scan_block_sums_kernel, 1, 1024, 0, stream, block_sums, n_ctas, total);
 }
 
 void launch_raster_emit_batch(const BatchArgs& batch, uint32_t n_ctas, const uint32_t* block_offsets, uint64_t* out, uint32_t cap,

@@ -109,6 +109,7 @@ __device__ __forceinline__ uint32_t resolve_key_count(uint32_t n, const uint32_t
 __global__ void __launch_bounds__(kSortThreads) radix_hist_kernel(const uint64_t* __restrict__ keys, uint32_t n, SortPlan plan,
                                                                 uint32_t* __restrict__ hist /*[passes][256]*/,
                                                                 const uint32_t* __restrict__ n_dev) {
+    chain_begin();
     n = resolve_key_count(n, n_dev);
     __shared__ uint32_t s_hist[kMaxSortPasses][kRadix];
     for (int i = threadIdx.x; i < kMaxSortPasses * kRadix; i += kSortThreads) (&s_hist[0][0])[i] = 0;
@@ -135,6 +136,7 @@ __global__ void __launch_bounds__(kSortThreads, kItems == 16 ? 3 : 6)
                          const uint32_t* __restrict__ digit_counts /*[256]: keys per digit (radix_hist_kernel)*/,
                          uint32_t* __restrict__ lb /*[tiles][256], zeroed*/, uint32_t* __restrict__ tile_counter,
                          const uint32_t* __restrict__ n_dev) {
+    chain_begin();
     n = resolve_key_count(n, n_dev);
     constexpr int kTileKeys = kSortThreads * kItems;
     __shared__ uint64_t s_keys[kTileKeys];
@@ -329,6 +331,7 @@ __global__ void __launch_bounds__(kSortThreads) radix_upsweep_kernel(const uint6
                                                                    uint32_t* __restrict__ tile_hist /*[tiles][256]*/,
                                                                    uint32_t* __restrict__ totals /*[kTotalsRows][256], zeroed*/,
                                                                    uint32_t tiles_per_chunk) {
+    chain_begin();
     __shared__ uint32_t s_hist[kRadix];
     const uint32_t t = threadIdx.x, tile = blockIdx.x;
     s_hist[t] = 0;
@@ -361,6 +364,7 @@ __global__ void __launch_bounds__(kSortThreads) radix_upsweep_kernel(const uint6
 __global__ void __launch_bounds__(kRadix) radix_chunk_totals_kernel(const uint32_t* __restrict__ tile_hist,
                                                                   uint32_t* __restrict__ totals, uint32_t tiles,
                                                                   uint32_t tiles_per_chunk) {
+    chain_begin();
     const uint32_t d = threadIdx.x, c = blockIdx.x;
     const uint32_t t0 = c * tiles_per_chunk, t1 = min(tiles, t0 + tiles_per_chunk);
     uint32_t sum = 0;
@@ -380,6 +384,7 @@ __global__ void __launch_bounds__(kRadix) radix_chunk_totals_kernel(const uint32
 __global__ void __launch_bounds__(kRadix) radix_tile_scan_kernel(uint32_t* __restrict__ tile_hist,
                                                                const uint32_t* __restrict__ totals, uint32_t tiles,
                                                                uint32_t tiles_per_chunk) {
+    chain_begin();
     __shared__ uint32_t s_warp_tot[kRadix / 32];
     const uint32_t d = threadIdx.x, c = blockIdx.x, sc = c / kChunksPerSuper;
     uint32_t before = 0, total = 0;  // keys of digit d in earlier chunks / in all chunks
@@ -448,6 +453,7 @@ template <bool kCount, bool kZero>
 __global__ void __launch_bounds__(kWideThreads, 2)
     radix_downsweep_wide_kernel(const uint64_t* __restrict__ keys_in, uint64_t* __restrict__ keys_out, uint32_t n, DigitSpec spec,
                                 uint32_t* __restrict__ tile_base, uint32_t tiles, CountArgs next, uint32_t* __restrict__ supers) {
+    chain_begin();
     extern __shared__ __align__(128) unsigned char smem_raw[];
     DownsweepWideSmem& S = *reinterpret_cast<DownsweepWideSmem*>(smem_raw);
     const uint32_t t = threadIdx.x, warp = t >> 5, lane = t & 31u;
@@ -593,7 +599,7 @@ size_t sort_lookback_bytes(uint32_t n, const SortPlan& plan) {
 void launch_radix_hist(const uint64_t* keys, uint32_t n, const SortPlan& plan, uint32_t* hist, const uint32_t* n_dev,
                        cudaStream_t stream) {
     uint32_t hist_blocks = min(tiles_for(n, 16) * 4u, (uint32_t)device_sm_count() * 8u);
-    radix_hist_kernel<<<hist_blocks, kSortThreads, 0, stream>>>(keys, n, plan, hist, n_dev);
+    launch_chained(radix_hist_kernel, hist_blocks, kSortThreads, 0, stream, keys, n, plan, hist, n_dev);
 }
 
 template <bool kPairs, int kItems>
@@ -614,7 +620,7 @@ static void launch_passes(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals, ui
         uint64_t* kout = (p & 1u) ? keys : keys_tmp;
         const uint32_t* vin = (p & 1u) ? vals_tmp : vals;
         uint32_t* vout = (p & 1u) ? vals : vals_tmp;
-        onesweep_pass_kernel<kPairs, kItems><<<tiles, kSortThreads, 0, stream>>>(
+        launch_chained(onesweep_pass_kernel<kPairs, kItems>, tiles, kSortThreads, 0, stream,
             kin, kout, vin, vout, n, plan.pass[p], hist + p * kRadix, lookback + (size_t)p * tiles * kRadix, counters + p, n_dev);
     }
 }
@@ -667,28 +673,27 @@ SortResult launch_radix_sort(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals,
                 for (uint32_t p = 0; p < plan.n_passes; ++p) {
                     const uint64_t* kin = (p & 1u) ? keys_tmp : keys;
                     uint64_t* kout = (p & 1u) ? keys : keys_tmp;
-                    if (pass_events) cudaEventRecord(pass_events[3 * p], stream);
                     if (p == 0 && !counts->pass0) {  // the upsweep stores the tile counts and adds to zeroed totals
                         cudaMemsetAsync(counts->totals(0), 0, (size_t)kTotalsRows * kRadix * sizeof(uint32_t), stream);
-                        radix_upsweep_kernel<<<tiles, kSortThreads, 0, stream>>>(kin, n, plan.pass[0], counts->hist(0), counts->totals(0), tpc);
+                        launch_chained(radix_upsweep_kernel, tiles, kSortThreads, 0, stream, kin, n, plan.pass[0], counts->hist(0), counts->totals(0), tpc);
                     } else {
-                        radix_chunk_totals_kernel<<<chunks, kRadix, 0, stream>>>(counts->hist(p), counts->totals(p), tiles, tpc);
+                        launch_chained(radix_chunk_totals_kernel, chunks, kRadix, 0, stream, counts->hist(p), counts->totals(p), tiles, tpc);
                     }
                     if (keep_counts)
                         cudaMemcpyAsync(keep_counts + (size_t)p * tiles * kRadix, counts->hist(p), (size_t)tiles * kRadix * sizeof(uint32_t),
                                         cudaMemcpyDeviceToDevice, stream);
-                    radix_tile_scan_kernel<<<chunks, kRadix, 0, stream>>>(counts->hist(p), counts->totals(p), tiles, tpc);
+                    launch_chained(radix_tile_scan_kernel, chunks, kRadix, 0, stream, counts->hist(p), counts->totals(p), tiles, tpc);
                     if (pass_events) cudaEventRecord(pass_events[3 * p + 1], stream);
                     uint32_t* supers = counts->totals(p) + (size_t)kMaxChunks * kRadix;
                     if (p + 1 < plan.n_passes) {
                         const CountArgs next{counts->hist(p + 1), plan.pass[p + 1]};
-                        radix_downsweep_wide_kernel<true, true><<<grid, kWideThreads, sizeof(DownsweepWideSmem), stream>>>(
+                        launch_chained(radix_downsweep_wide_kernel<true, true>, grid, kWideThreads, sizeof(DownsweepWideSmem), stream,
                             kin, kout, n, plan.pass[p], counts->hist(p), tiles, next, supers);
                     } else {
-                        radix_downsweep_wide_kernel<false, true><<<grid, kWideThreads, sizeof(DownsweepWideSmem), stream>>>(
+                        launch_chained(radix_downsweep_wide_kernel<false, true>, grid, kWideThreads, sizeof(DownsweepWideSmem), stream,
                             kin, kout, n, plan.pass[p], counts->hist(p), tiles, CountArgs{}, supers);
                     }
-                    if (pass_events) cudaEventRecord(pass_events[3 * p + 2], stream);
+                    if (pass_events && p + 1 < plan.n_passes) cudaEventRecord(pass_events[3 * p + 2], stream);
                 }
                 res.timed_passes = pass_events ? (int)plan.n_passes : 0;
                 res.launches = 3 * (int)plan.n_passes;
@@ -704,13 +709,12 @@ SortResult launch_radix_sort(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals,
                 const uint64_t* kin = (p & 1u) ? keys_tmp : keys;
                 uint64_t* kout = (p & 1u) ? keys : keys_tmp;
                 uint32_t* totals = chunk_totals + (size_t)p * kTotalsRows * kRadix;
-                if (pass_events) cudaEventRecord(pass_events[3 * p], stream);
-                radix_upsweep_kernel<<<tiles, kSortThreads, 0, stream>>>(kin, n, plan.pass[p], tile_hist, totals, tiles_per_chunk);
-                radix_tile_scan_kernel<<<chunks, kRadix, 0, stream>>>(tile_hist, totals, tiles, tiles_per_chunk);
+                launch_chained(radix_upsweep_kernel, tiles, kSortThreads, 0, stream, kin, n, plan.pass[p], tile_hist, totals, tiles_per_chunk);
+                launch_chained(radix_tile_scan_kernel, chunks, kRadix, 0, stream, tile_hist, totals, tiles, tiles_per_chunk);
                 if (pass_events) cudaEventRecord(pass_events[3 * p + 1], stream);
-                radix_downsweep_wide_kernel<false, false><<<grid, kWideThreads, sizeof(DownsweepWideSmem), stream>>>(
+                launch_chained(radix_downsweep_wide_kernel<false, false>, grid, kWideThreads, sizeof(DownsweepWideSmem), stream,
                     kin, kout, n, plan.pass[p], tile_hist, tiles, CountArgs{}, nullptr);
-                if (pass_events) cudaEventRecord(pass_events[3 * p + 2], stream);
+                if (pass_events && p + 1 < plan.n_passes) cudaEventRecord(pass_events[3 * p + 2], stream);
             }
             res.timed_passes = pass_events ? (int)plan.n_passes : 0;
             res.launches = 3 * (int)plan.n_passes;

@@ -100,6 +100,7 @@ __global__ void __launch_bounds__(kCellThreads)
                  uint32_t tiles, uint32_t* __restrict__ cell_start, uint32_t cap, uint32_t* __restrict__ n_cells_out,
                  uint64_t* __restrict__ cell_key, uint4* __restrict__ cell_cover, uint64_t* __restrict__ key2,
                  uint32_t* __restrict__ perm, SortPlan plan, uint32_t* __restrict__ hist) {
+    chain_begin();
     __shared__ uint32_t warp_cnt[kCellThreads / 32];
     __shared__ uint32_t s_tile;
     __shared__ unsigned long long s_prefix;
@@ -247,6 +248,7 @@ __global__ void __launch_bounds__(kCellThreads)
                           uint32_t tiles, const uint32_t* __restrict__ cell_start, uint32_t cap,
                           const uint32_t* __restrict__ n_cells_ptr, uint64_t* __restrict__ cell_key, uint4* __restrict__ cell_cover,
                           uint64_t* __restrict__ key2, uint32_t* __restrict__ perm, SortPlan plan, uint32_t* __restrict__ hist) {
+    chain_begin();
     const uint32_t b = blockIdx.x * (kCellThreads / 32) + (threadIdx.x >> 5) + 1u, lane = threadIdx.x & 31u;
     if (b >= tiles) return;
     const uint32_t n_cells = *n_cells_ptr;
@@ -374,6 +376,7 @@ __global__ void __launch_bounds__(kCarryThreads)
                       uint4* __restrict__ carry_in, uint64_t* __restrict__ gkey, uint32_t* __restrict__ gid,
                       uint4* __restrict__ gap_carry, uint32_t cap, uint32_t* __restrict__ n_gaps_out, SortPlan plan,
                       uint32_t* __restrict__ hist, DevCounts dc) {
+    chain_begin();
     __shared__ uint32_t s_tile;
     __shared__ uint4 s_warp_cover[kCarryWarps];
     __shared__ uint32_t s_warp_head[kCarryWarps];
@@ -756,6 +759,7 @@ __global__ void merge_entries_kernel(PaintScene S, const uint64_t* __restrict__ 
                                      EntryRec* __restrict__ recs, uint8_t* __restrict__ eflags, uint2* __restrict__ tile_range,
                                      uint32_t* __restrict__ heavy, uint32_t* __restrict__ heavy_count, DevCounts dc,
                                      const BatchFrame* __restrict__ frames, uint32_t rows) {
+    chain_begin();
     merge_entries_body<false>(S, cell_key, n_cells, gkey, gid, n_gaps, cell_start, carry_in, gap_carry, ekey, recs, eflags, tile_range,
                               heavy, heavy_count, dc, frames, rows);
 }
@@ -766,6 +770,7 @@ __global__ void merge_entries_pose_fills_kernel(PaintScene S, const uint64_t* __
                                                 EntryRec* __restrict__ recs, uint8_t* __restrict__ eflags,
                                                 uint2* __restrict__ tile_range, uint32_t* __restrict__ heavy,
                                                 uint32_t* __restrict__ heavy_count, DevCounts dc, PoseFillArgs F) {
+    chain_begin();
     merge_entries_body<true>(S, cell_key, n_cells, gkey, gid, n_gaps, cell_start, carry_in, gap_carry, ekey, recs, eflags, tile_range,
                              heavy, heavy_count, dc, nullptr, 0u, F);
 }
@@ -778,6 +783,7 @@ __global__ void __launch_bounds__(256) pose_styles_kernel(const int32_t* __restr
                                                           StyleRec* __restrict__ styles, uint32_t n_styles,
                                                           const float4* __restrict__ colors, uint32_t first_order, uint32_t K,
                                                           uint64_t n_recs) {
+    chain_begin();
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_recs) return;
     const uint32_t o = first_order + (uint32_t)(i % K);
@@ -807,6 +813,7 @@ __global__ void __launch_bounds__(256) pose_styles_kernel(const int32_t* __restr
 __global__ void row_cost_kernel(const uint2* __restrict__ tile_range, uint32_t tiles_x, uint32_t tiles_y,
                                 const uint64_t* __restrict__ segs, uint32_t n, unsigned long long* __restrict__ out,
                                 unsigned long long* __restrict__ seg_out) {
+    chain_begin();
     const uint32_t row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
     if (row >= tiles_y) return;
     uint32_t entries = 0;
@@ -840,7 +847,7 @@ __global__ void row_cost_kernel(const uint2* __restrict__ tile_range, uint32_t t
 
 void launch_row_costs(const uint2* tile_range, uint32_t tiles_x, uint32_t tiles_y, const uint64_t* segs, uint32_t n,
                       unsigned long long* out, cudaStream_t st, unsigned long long* seg_out) {
-    if (tiles_y) row_cost_kernel<<<(tiles_y + 7) / 8, 256, 0, st>>>(tile_range, tiles_x, tiles_y, segs, n, out, seg_out);
+    if (tiles_y) launch_chained(row_cost_kernel, (tiles_y + 7) / 8, 256, 0, st, tile_range, tiles_x, tiles_y, segs, n, out, seg_out);
 }
 
 // ---------------------------------------------------------------------------
@@ -865,16 +872,50 @@ TableScratch table_scratch_layout(uint32_t n, uint32_t n_cells, uint32_t n_gaps,
     return L;
 }
 
+// Zeroes the bytes [0, a_bytes) of `a` and [0, b_bytes) of `b` (two device allocations, so 16-byte
+// aligned) and the word `word` (when not null): the tile ranges, the table scratch and the paint
+// kernel's tile counter of a sync-free frame, in one chained launch in place of three memsets, which
+// would end the overlap of the kernels around them. Not counted in Renderer::launches, like the
+// memsets it replaces.
+__global__ void __launch_bounds__(256) zero_tables_kernel(uint8_t* __restrict__ a, size_t a_bytes, uint8_t* __restrict__ b, size_t b_bytes,
+                                                          uint32_t* __restrict__ word) {
+    chain_begin();
+    const size_t stride = (size_t)gridDim.x * blockDim.x, i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (word && i0 == 0) *word = 0u;
+    for (int k = 0; k < 2; ++k) {
+        uint8_t* p = k ? b : a;
+        const size_t bytes = k ? b_bytes : a_bytes, words = bytes / 16u;
+        for (size_t i = i0; i < words; i += stride) reinterpret_cast<uint4*>(p)[i] = make_uint4(0u, 0u, 0u, 0u);
+        for (size_t i = words * 16u + i0; i < bytes; i += stride) p[i] = 0u;
+    }
+}
+void launch_zero_tables(uint8_t* a, size_t a_bytes, uint8_t* b, size_t b_bytes, uint32_t* word, cudaStream_t st) {
+    const size_t words = std::max<size_t>((std::max(a_bytes, b_bytes) + 15u) / 16u, 1u);
+    const uint32_t ctas = (uint32_t)std::min<size_t>((words + 255u) / 256u, (size_t)device_sm_count() * 4u);
+    launch_chained(zero_tables_kernel, ctas, 256, 0, st, a, a_bytes, b, b_bytes, word);
+}
+
+// dst[i] = src[i] for i < n (n <= 256): device words to pinned host memory (dst: its device
+// address), in a chained launch in place of a copy, which would end the overlap with the kernel
+// before it. Not counted in Renderer::launches, like the copy it replaces.
+__global__ void __launch_bounds__(256) copy_words_kernel(const uint32_t* __restrict__ src, uint32_t* __restrict__ dst, uint32_t n) {
+    chain_begin();
+    if (threadIdx.x < n) dst[threadIdx.x] = src[threadIdx.x];
+}
+void launch_copy_words(const uint32_t* src, uint32_t* dst, uint32_t n, cudaStream_t st) {
+    if (n) launch_chained(copy_words_kernel, 1, 256, 0, st, src, dst, n);
+}
+
 void launch_cells(const PaintScene& S, const uint64_t* segs, uint32_t n, uint8_t* scratch, const TableScratch& L,
                   const SortPlan& carry_plan, uint32_t* cell_start, uint32_t cap, uint32_t* n_cells_out, uint64_t* cell_key,
                   uint4* cell_cover, uint64_t* key2, uint32_t* perm, cudaStream_t st) {
     const uint32_t tiles = cell_num_blocks(n);
     auto* state = reinterpret_cast<unsigned long long*>(scratch + L.cells_state);  // [tiles] look-back | ticket
     auto* hist = reinterpret_cast<uint32_t*>(scratch + L.carry_hist);
-    cells_kernel<<<tiles, kCellThreads, 0, st>>>(S, segs, n, state, tiles, cell_start, cap, n_cells_out, cell_key, cell_cover, key2,
+    launch_chained(cells_kernel, tiles, kCellThreads, 0, st, S, segs, n, state, tiles, cell_start, cap, n_cells_out, cell_key, cell_cover, key2,
                                                  perm, carry_plan, hist);
     if (tiles > 1)
-        cells_boundary_kernel<<<(tiles - 1 + kCellThreads / 32 - 1) / (kCellThreads / 32), kCellThreads, 0, st>>>(
+        launch_chained(cells_boundary_kernel, (tiles - 1 + kCellThreads / 32 - 1) / (kCellThreads / 32), kCellThreads, 0, st,
             S, segs, n, state, tiles, cell_start, cap, n_cells_out, cell_key, cell_cover, key2, perm, carry_plan, hist);
 }
 
@@ -899,7 +940,7 @@ void launch_carry_pass(const PaintScene& S, const uint64_t* key2, const uint32_t
                        const DevCounts& dc) {
     const uint32_t tiles = carry_pass_tiles(n_cells);
     if (!tiles) return;
-    carry_pass_kernel<<<tiles, kCarryThreads, 0, st>>>(S, key2, perm, cell_cover, n_cells, scratch + L.carry_pass, tiles, carry_in,
+    launch_chained(carry_pass_kernel, tiles, kCarryThreads, 0, st, S, key2, perm, cell_cover, n_cells, scratch + L.carry_pass, tiles, carry_in,
                                                        gkey, gid, gap_carry, cap, n_gaps_out, gap_plan,
                                                        reinterpret_cast<uint32_t*>(scratch + L.gap_hist), dc);
 }
@@ -912,11 +953,11 @@ void launch_merge_entries(const PaintScene& S, const uint64_t* cell_key, uint32_
     uint32_t n = n_cells + n_gaps;
     if (!n) return;
     if (fills)
-        merge_entries_pose_fills_kernel<<<(n + 255) / 256, 256, 0, st>>>(S, cell_key, n_cells, gkey, gid, n_gaps, cell_start, carry_in,
+        launch_chained(merge_entries_pose_fills_kernel, (n + 255) / 256, 256, 0, st, S, cell_key, n_cells, gkey, gid, n_gaps, cell_start, carry_in,
                                                                           gap_carry, ekey, recs, eflags, tile_range, heavy, heavy_count,
                                                                           dc, *fills);
     else
-        merge_entries_kernel<<<(n + 255) / 256, 256, 0, st>>>(S, cell_key, n_cells, gkey, gid, n_gaps, cell_start, carry_in,
+        launch_chained(merge_entries_kernel, (n + 255) / 256, 256, 0, st, S, cell_key, n_cells, gkey, gid, n_gaps, cell_start, carry_in,
                                                                gap_carry, ekey, recs, eflags, tile_range, heavy, heavy_count, dc,
                                                                frames, rows);
 }
@@ -924,7 +965,7 @@ void launch_merge_entries(const PaintScene& S, const uint64_t* cell_key, uint32_
 void launch_pose_styles(const int32_t* order_to_style, uint32_t n_orders, StyleRec* styles, uint32_t n_styles, const float4* colors,
                         uint32_t first_order, uint32_t n_window, uint64_t n_recs, cudaStream_t st) {
     if (n_recs)
-        pose_styles_kernel<<<(unsigned)((n_recs + 255u) / 256u), 256, 0, st>>>(order_to_style, n_orders, styles, n_styles, colors,
+        launch_chained(pose_styles_kernel, (unsigned)((n_recs + 255u) / 256u), 256, 0, st, order_to_style, n_orders, styles, n_styles, colors,
                                                                                first_order, n_window, n_recs);
 }
 

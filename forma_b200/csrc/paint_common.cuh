@@ -136,7 +136,9 @@ __device__ __forceinline__ void scatter_entry(const uint64_t* __restrict__ segs,
 struct TileGrid {
     uint32_t n_tiles, ctas;
 };
-TileGrid tile_grid(const PaintScene& S, const void* kernel, uint32_t warps, uint32_t* tile_counter, cudaStream_t st);
+// counter_zeroed: the counter is already zero (a kernel earlier in the chain cleared it), no memset.
+TileGrid tile_grid(const PaintScene& S, const void* kernel, uint32_t warps, uint32_t* tile_counter, cudaStream_t st,
+                   bool counter_zeroed = false);
 
 // Cells that cannot influence a painted tile (rows outside the painted band,
 // columns right of it) get this key in both pair sorts: it sorts last and keeps

@@ -531,6 +531,13 @@ int Renderer::run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p
         FORMA_CUDA_TRY(cudaEventRecord(timer.ev[5], stream));
         st = output_step(q, S, p);
         if (st) return st;
+        // The real counts of sync-free tables (read after the synchronisation below), queued behind
+        // the paint, so that no copy stands between the merge and the paint kernel, and stored into
+        // the pinned words by a chained kernel rather than a copy.
+        if (sync_free) {
+            if (!pinned_totals_dev) FORMA_CUDA_TRY(cudaHostGetDevicePointer((void**)&pinned_totals_dev, pinned_totals, 0));
+            launch_copy_words(totals.ptr + 1, pinned_totals_dev + 1, 2, stream);
+        }
         FORMA_CUDA_TRY(cudaEventRecord(timer.ev[6], stream));
         FORMA_CUDA_TRY(cudaStreamSynchronize(stream));
         if (!sync_free) break;
@@ -1275,7 +1282,10 @@ int Renderer::build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint
     // Tiles without entries keep an empty range: a frame whose tables are redone paints only the
     // clear colour in its first attempt. A count above its bound leaves every range empty (the
     // merge kernel then writes none), so that attempt of an over frame writes nothing at all.
-    FORMA_CUDA_TRY(cudaMemsetAsync(tile_range.ptr, 0, (size_t)S.tiles_x * S.tiles_y * sizeof(uint2), stream));
+    // (sync_free: zeroed with the table scratch below, by one kernel of the chain)
+    const size_t range_bytes = (size_t)S.tiles_x * S.tiles_y * sizeof(uint2);
+    paint_counter_zeroed = false;
+    if (!sync_free || n == 0) FORMA_CUDA_TRY(cudaMemsetAsync(tile_range.ptr, 0, range_bytes, stream));
     const SortPlan carry_plan = carry_sort_plan(S), gap_plan = gap_sort_plan(S);
     auto zero_scratch = [&](size_t from, size_t to) -> cudaError_t {
         return to > from ? cudaMemsetAsync(table_scratch.ptr + from, 0, to - from, stream) : cudaSuccess;
@@ -1307,7 +1317,8 @@ int Renderer::build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint
         FORMA_CUDA_TRY(reserve_entry_tables((size_t)n_cells + n_gaps));
         L = table_scratch_layout(n, n_cells, n_gaps, carry_plan, gap_plan);
         FORMA_CUDA_TRY(table_scratch.reserve(L.end));
-        FORMA_CUDA_TRY(zero_scratch(0, L.end));
+        launch_zero_tables(reinterpret_cast<uint8_t*>(tile_range.ptr), range_bytes, table_scratch.ptr, L.end, totals.ptr + 3, stream);
+        paint_counter_zeroed = true;
         dc = DevCounts{totals.ptr + 1, totals.ptr + 2, n_cells, n_gaps};
         // Cells beyond cell_bound + 1 are dropped by the pass; the count it leaves in totals[1] is the real one.
         cells_pass(n_cells + 1u);
@@ -1388,9 +1399,7 @@ int Renderer::build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint
                          ekey.ptr, recs.ptr, eflags.ptr, tile_range.ptr, heavy_lists, heavy_count(), stream, dc,
                          batch ? batch->frames : nullptr, batch ? batch->rows : 0u, fills);
     ++launches;
-    // sync_free: the counts travel to the host behind everything else of the frame.
-    if (sync_free)
-        FORMA_CUDA_TRY(cudaMemcpyAsync(pinned_totals + 1, totals.ptr + 1, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+    // sync_free: the counts travel to the host behind everything else of the frame (run_frame).
     return FORMA_STATUS_OK;
 }
 
@@ -1452,7 +1461,8 @@ int Renderer::paint(const PaintScene& S, const TileTables& t, uint8_t* fb, uint8
         for (uint32_t k = 0; kCopyBands > 1u && k < kCopyBands; ++k) FORMA_CUDA_TRY(cudaStreamWaitEvent(stream, band_ev[k], 0));
         *paint_launches = kCopyBands;
     } else if (bpp == 4u) {
-        launch_paint(S, t, eflags.ptr, fb, totals.ptr + 3, stream, view_rows, solid_over);
+        launch_paint(S, t, eflags.ptr, fb, totals.ptr + 3, stream, view_rows, solid_over, paint_counter_zeroed);
+        paint_counter_zeroed = false;
         ++launches;
     } else {
         launch_paint_linear(S, t, eflags.ptr, fb, totals.ptr + 3, stream, view_rows, bpp);

@@ -268,10 +268,11 @@ class Renderer {
         stage_ms[6] = el(5, 6);  // device -> host copy of the framebuffer
         stage_ms[7] = el(0, 6);  // whole call on the device timeline
         kernel_ms[0] = kernel_ms[1] = 0;
+        // (the sort records no event of its own where a pass starts or the sort ends: launch_radix_sort)
         for (int p = 0; p < pending_sort_passes; ++p) {
             float a = 0, b = 0;
-            cudaEventElapsedTime(&a, timer.sort_ev[3 * p], timer.sort_ev[3 * p + 1]);
-            cudaEventElapsedTime(&b, timer.sort_ev[3 * p + 1], timer.sort_ev[3 * p + 2]);
+            cudaEventElapsedTime(&a, p ? timer.sort_ev[3 * p - 1] : timer.ev[2], timer.sort_ev[3 * p + 1]);
+            cudaEventElapsedTime(&b, timer.sort_ev[3 * p + 1], p + 1 < pending_sort_passes ? timer.sort_ev[3 * p + 2] : timer.ev[3]);
             kernel_ms[1] += a;  // upsweep + tile scan
             kernel_ms[0] += b;  // downsweep
         }
@@ -280,6 +281,8 @@ class Renderer {
         kernel_launches[2] = pending_paint_launches;
     }
     uint32_t* pinned_totals = nullptr;  // 4 x u32 pinned host words for count read-backs
+    uint32_t* pinned_totals_dev = nullptr;  // their device address (set at first use)
+    bool paint_counter_zeroed = false;  // sync-free tables cleared the paint kernel's tile counter (totals[3])
     // Renderers of a multi-device / sliced frame: the per-row costs of the frame (see
     // row_cost_kernel) travel back behind the frame itself, without a synchronisation of their own.
     bool track_row_costs = false;

@@ -803,7 +803,7 @@ uint64_t forma_renderer_row_costs(forma_renderer*, uint64_t cap, uint64_t* out);
 /* Schedule switches of the library (process-wide; none changes results): "speculate",
  * "band_copy", "copy_bands", "sort_full_key", "sort_big_log2", "sort_scan_log2", "sort_counts", "paint_lpt",
  * "paint_wide", "band_filter", "sync_free", "host_slices", "slice_bands", "slice_min_points", "slice_chain",
- * "test_gap_cap", "test_fast_shrink".
+ * "pdl", "test_gap_cap", "test_fast_shrink".
  * Defaults come from the environment (FORMA_SPECULATE, ...); see DESIGN.md section 6. */
 int forma_set_option(const char* name, int value);
 int forma_get_option(const char* name, int* value);
