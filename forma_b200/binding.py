@@ -221,6 +221,10 @@ class _CPoses(C.Structure):  # forma_poses
                 ("colors", C.c_void_p)]
 
 
+class _CInstances(C.Structure):  # forma_instances
+    _fields_ = [("n_instances", C.c_uint32), ("prototypes", C.c_void_p), ("transforms", C.c_void_p), ("colors", C.c_void_p)]
+
+
 def _is_cuda_array(a) -> bool:
     return a is not None and hasattr(a, "__cuda_array_interface__")
 
@@ -230,20 +234,20 @@ class _CudaTable:
     shape and bytes per frame (a chunk of frames [f, f + c) starts at ptr + f * row_bytes). It
     keeps the object alive and is never copied."""
 
-    def __init__(self, name, a, typestrs):
+    def __init__(self, name, a, typestrs, what="Poses"):
         cai = a.__cuda_array_interface__
         shape, typestr = tuple(int(s) for s in cai["shape"]), cai["typestr"]
         if typestr not in typestrs:
-            raise ValueError(f"Poses: {name} of CUDA type {typestr!r}, not {' or '.join(map(repr, typestrs))}")
+            raise ValueError(f"{what}: {name} of CUDA type {typestr!r}, not {' or '.join(map(repr, typestrs))}")
         if cai.get("mask") is not None:
-            raise ValueError(f"Poses: {name} is a masked CUDA array")
+            raise ValueError(f"{what}: {name} is a masked CUDA array")
         itemsize = int(typestr[2:])
         strides = cai.get("strides")
         if strides is not None:  # C-contiguous: each dimension longer than 1 steps over the ones after it
             step = itemsize
             for n, s in reversed(list(zip(shape, strides))):
                 if n > 1 and s != step:
-                    raise ValueError(f"Poses: {name} is not a C-contiguous CUDA array (strides {tuple(strides)})")
+                    raise ValueError(f"{what}: {name} is not a C-contiguous CUDA array (strides {tuple(strides)})")
                 step *= n
         self.owner, self.ptr, self.shape = a, int(cai["data"][0]), shape
         self.ndim = len(shape)
@@ -292,6 +296,63 @@ class Poses:
         if len(shapes) != 1:
             raise ValueError(f"Poses: the tables disagree on [n, K]: {sorted(shapes)}")
         self.n, self.n_orders = shapes.pop()
+
+    def __len__(self) -> int:
+        return self.n
+
+
+NO_INSTANCE = 0xFFFFFFFF  # FORMA_NO_INSTANCE: an empty instance slot
+
+
+class Instances:
+    """The instance slots of an instance-scene call (see include/forma_b200.h: forma_instances):
+    frame b draws, in slot m, a copy of the layer at order prototypes[b, m] ([n, M] integers; -1 or
+    NO_INSTANCE = an empty slot) as the layer m of its own composition, enabled, with the transform
+    transforms[b, m] ([n, M, 6] float32, set_transform order [ux, vx, uy, vy, tx, ty]; None: the
+    prototype's own) and, when it draws, the solid linear RGBA fill colors[b, m] ([n, M, 4] float32;
+    None: the prototype's own props). IDs, masks and statistics of the call are indexed by m.
+
+    Each table may also be a CUDA array on the renderer's device (__cuda_array_interface__, such as
+    a torch CUDA tensor, C-contiguous): int32 or uint32 prototypes (int32 -1 is NO_INSTANCE),
+    float32 transforms and colours. It is read where it is, never copied by the binding; the
+    library reads a CUDA prototypes table back to the host, since it decides the launch sizes.
+    Host and CUDA tables can be mixed."""
+
+    def __init__(self, prototypes, transforms=None, colors=None):
+        if prototypes is None:
+            raise ValueError("Instances: a prototypes table [n, M] is required")
+        if _is_cuda_array(prototypes):
+            self.prototypes = _CudaTable("prototypes", prototypes, ("<u4", "<i4"), "Instances")
+        else:
+            p = np.asarray(prototypes)
+            if p.dtype.kind not in "iu":
+                raise ValueError(f"Instances: prototypes of type {p.dtype}, not integers")
+            p = p.astype(np.int64)
+            if p.size and (p.min() < -1 or p.max() > NO_INSTANCE):
+                raise ValueError("Instances: prototypes must be layer orders, -1 or NO_INSTANCE")
+            self.prototypes = np.ascontiguousarray((p & NO_INSTANCE).astype(np.uint32))
+        if _is_cuda_array(transforms):
+            self.transforms = _CudaTable("transforms", transforms, ("<f4",), "Instances")
+        else:
+            self.transforms = None if transforms is None else np.ascontiguousarray(np.asarray(transforms, dtype=np.float32))
+        if _is_cuda_array(colors):
+            self.colors = _CudaTable("colors", colors, ("<f4",), "Instances")
+        else:
+            if colors is not None and (not isinstance(colors, np.ndarray) or colors.dtype != np.float32):
+                raise ValueError("Instances: colors must be a float32 array [n, M, 4]")
+            self.colors = None if colors is None else np.ascontiguousarray(colors)
+        if self.prototypes.ndim != 2:
+            raise ValueError(f"Instances: prototypes of shape {self.prototypes.shape}, not [n, M]")
+        if self.transforms is not None and (self.transforms.ndim != 3 or self.transforms.shape[2] != 6):
+            raise ValueError(f"Instances: transforms of shape {self.transforms.shape}, not [n, M, 6]")
+        if self.colors is not None and (self.colors.ndim != 3 or self.colors.shape[2] != 4):
+            raise ValueError(f"Instances: colors of shape {self.colors.shape}, not [n, M, 4]")
+        shapes = {t.shape[:2] for t in (self.prototypes, self.transforms, self.colors) if t is not None}
+        if len(shapes) != 1:
+            raise ValueError(f"Instances: the tables disagree on [n, M]: {sorted(shapes)}")
+        self.n, self.n_instances = shapes.pop()
+        if self.n_instances == 0:
+            raise ValueError("Instances: M = 0 slots per frame")
 
     def __len__(self) -> int:
         return self.n
@@ -456,6 +517,15 @@ SIGNATURES = {
                                                       C.c_uint64, C.c_uint64, _u32p, _fp, C.c_uint32, C.POINTER(_CTimings)]),
     "renderer_render_poses_over_device": (C.c_int, [_vp, _vp, C.POINTER(_CPoses), C.c_uint32, _vp, C.c_uint64, C.c_uint64, C.c_uint64,
                                                     C.c_uint64, _u32p, C.c_uint32, C.POINTER(_CTimings)]),
+    "renderer_render_instances_device": (C.c_int, [_vp, _vp, C.POINTER(_CInstances), C.c_uint32, _vp, C.c_uint64, C.c_uint64,
+                                                   C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
+    "renderer_render_instances_ids_device": (C.c_int, [_vp, _vp, C.POINTER(_CInstances), C.c_uint32, _vp, C.c_uint64, C.c_uint64,
+                                                       C.c_uint64, C.c_uint64, _u32p, _fp, _vp, C.c_uint64, C.c_uint64, _f,
+                                                       C.POINTER(_CTimings)]),
+    "renderer_render_instances_masks_device": (C.c_int, [_vp, _vp, C.POINTER(_CInstances), C.c_uint32, C.POINTER(_CMasks), C.c_uint64,
+                                                         C.c_uint64, _vp, C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
+    "renderer_render_instances_stats_device": (C.c_int, [_vp, _vp, C.POINTER(_CInstances), C.c_uint32, C.POINTER(_CStats), C.c_uint64,
+                                                         C.c_uint64, _vp, C.c_uint64, C.c_uint64, _u32p, _fp, C.POINTER(_CTimings)]),
     "renderer_launch_count": (C.c_uint64, [_vp]),
     "renderer_stage_times": (None, [_vp, C.POINTER(C.c_double)]),
     "renderer_counters": (None, [_vp, _u64p]),
@@ -526,6 +596,10 @@ STATS_SYMBOLS = ("renderer_render_stats", "renderer_render_stats_device", "rende
 POSE_SYMBOLS = ("renderer_render_poses", "renderer_render_poses_device", "renderer_render_poses_ids",
                 "renderer_render_poses_ids_device", "renderer_render_poses_masks_device", "renderer_render_poses_stats_device",
                 "renderer_render_poses_linear", "renderer_render_poses_linear_device", "renderer_render_poses_over_device")
+# The same for instance scenes (Renderer.render_instances_device, render_instances_ids_device,
+# render_instances_masks_device, render_instances_stats_device).
+INSTANCE_SYMBOLS = ("renderer_render_instances_device", "renderer_render_instances_ids_device",
+                    "renderer_render_instances_masks_device", "renderer_render_instances_stats_device")
 # Value formats of mask planes: name -> (FORMA_MASK_*, bytes per value, numpy dtype).
 MASK_FORMATS = {"f32": (0, 4, np.float32), "u8": (1, 1, np.uint8)}
 
@@ -558,7 +632,7 @@ def over_format(fmt: str):
 
 
 _OPTIONAL_SYMBOLS = frozenset(ID_FRAME_SYMBOLS + VIEW_SYMBOLS + BATCH_SYMBOLS + STACK_ID_SYMBOLS + SORT_DEBUG_SYMBOLS +
-                              LINEAR_SYMBOLS + OVER_SYMBOLS + MASK_SYMBOLS + STATS_SYMBOLS + POSE_SYMBOLS)
+                              LINEAR_SYMBOLS + OVER_SYMBOLS + MASK_SYMBOLS + STATS_SYMBOLS + POSE_SYMBOLS + INSTANCE_SYMBOLS)
 
 
 class Api:
@@ -1029,15 +1103,16 @@ class Renderer:
         """The most views of `height` rows one render_views call of the library takes (0: none)."""
         return int(self._api.renderer_max_views(height))
 
-    def _stack(self, fn, what, first_args, n, width, height, rgba, ids, timings, bpp=4, tail=()):
+    def _stack(self, fn, what, first_args, n, width, height, rgba, ids, timings, bpp=4, tail=(), chunk=None):
         """Calls `fn`, an entry point of views or batches, on chunks of at most max_views(height)
         frames: first_args(first, count) gives a chunk's leading arguments (views or handles,
         count), then come its targets. rgba = (ptr or None, stride, frame_stride, channels,
         clear_color) and ids = (ptr, stride, frame_stride, min_coverage), either may be None; a
         stride of None takes its default (bpp * width, height * stride; IDs: bpp 4); a clear colour
         of None is not passed (frames over a background). An entry point with both takes the ID
-        target's arguments without width and height. `tail` follows the targets."""
-        chunk = max(self.max_views(height), 1)
+        target's arguments without width and height. `tail` follows the targets. `chunk`: fewer
+        frames per call than max_views(height)."""
+        chunk = max(min(self.max_views(height), chunk or self.max_views(height)), 1)
         if rgba is not None:
             rgba_ptr, stride, frame_stride = rgba[0], *self._strides(width, height, rgba[1], rgba[2], bpp)
             ch, cc, _ = self._common(rgba[3], Color() if rgba[4] is None else rgba[4], None)
@@ -1099,6 +1174,23 @@ class Renderer:
             keep[:] = [t, v, c, d]
             return composition._h, C.byref(d), count
         return poses.n, args
+
+    @staticmethod
+    def _instance_args(composition, instances: Instances):
+        """(n, args, chunk) for _stack: a chunk's forma_instances holds its frames' rows of the tables
+        (of a CUDA table, the address of its first frame's row); a chunk holds at most 2^21 // M
+        frames, so that its n M orders fit in the layer field."""
+        keep = []  # the chunk's descriptor and tables stay alive until the next one
+
+        def args(first, count):
+            p, t, c = (None if a is None else a if isinstance(a, _CudaTable) else np.ascontiguousarray(a[first:first + count])
+                       for a in (instances.prototypes, instances.transforms, instances.colors))
+            d = _CInstances(instances.n_instances,
+                            *(None if a is None else a.ptr + first * a.row_bytes if isinstance(a, _CudaTable) else a.ctypes.data
+                              for a in (p, t, c)))
+            keep[:] = [p, t, c, d]
+            return composition._h, C.byref(d), count
+        return instances.n, args, max((1 << 21) // instances.n_instances, 1)
 
     def render_views(self, composition: Composition, views, buffer: np.ndarray, width: int, height: int, channels=RGBA,
                      clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
@@ -1370,13 +1462,13 @@ class Renderer:
         return _timings(t)
 
     def _stack_masks(self, fn, what, first_args, n, masks_ptr, width, height, first_order, n_orders, format, stride, plane_stride, rgba_ptr,
-                     channels, clear_color, rgba_stride, frame_stride, timings):
+                     channels, clear_color, rgba_stride, frame_stride, timings, chunk=None):
         """Calls `fn`, the mask entry point of views or batches, on chunks of at most
         max_views(height) frames (see _stack)."""
         code, _, _, stride, plane_stride = self._mask_layout(width, height, n_orders, format, stride, plane_stride)
         rgba_stride, frame_stride = self._strides(width, height, rgba_stride, frame_stride)
         ch, cc, _ = self._common(channels, clear_color, None)
-        chunk = max(self.max_views(height), 1)
+        chunk = max(min(self.max_views(height), chunk or self.max_views(height)), 1)
         t = None
         for first in range(0, max(n, 1), chunk):
             m = _CMasks(int(masks_ptr) + first * n_orders * plane_stride, first_order, n_orders, code, stride, plane_stride)
@@ -1449,12 +1541,12 @@ class Renderer:
         return _timings(t)
 
     def _stack_stats(self, fn, what, first_args, n, stats_ptr, width, height, first_order, n_orders, min_coverage, rgba_ptr, channels,
-                     clear_color, rgba_stride, frame_stride, timings):
+                     clear_color, rgba_stride, frame_stride, timings, chunk=None):
         """Calls `fn`, the statistics entry point of views or batches, on chunks of at most
         max_views(height) frames (see _stack)."""
         rgba_stride, frame_stride = self._strides(width, height, rgba_stride, frame_stride)
         ch, cc, _ = self._common(channels, clear_color, None)
-        chunk = max(self.max_views(height), 1)
+        chunk = max(min(self.max_views(height), chunk or self.max_views(height)), 1)
         t = None
         for first in range(0, max(n, 1), chunk):
             s = _CStats(int(stats_ptr) + first * n_orders * STATS_DTYPE.itemsize, first_order, n_orders, min_coverage)
@@ -1557,6 +1649,56 @@ class Renderer:
         return self._stack_stats(self._api.renderer_render_poses_stats_device, "Renderer::render_poses_stats_device", args, n, stats_ptr,
                                  width, height, first_order, n_orders, min_coverage, rgba_ptr, channels, clear_color, rgba_stride,
                                  view_stride, timings)
+
+    def render_instances_device(self, composition: Composition, instances: Instances, device_ptr: int, width: int, height: int,
+                                channels=RGBA, clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
+                                view_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """One frame per row of the instance tables (see Instances and include/forma_b200.h:
+        forma_renderer_render_instances_device): frame b draws its slots' copies of the composition's
+        layers, which the call leaves unchanged. Layout as for render_views_device: with the
+        defaults, the data_ptr() of a contiguous [N, height, width, 4] uint8 CUDA tensor. Chunked
+        at max_views(height) frames and at 2^21 // M frames."""
+        n, args, chunk = self._instance_args(composition, instances)
+        return self._stack(self._api.renderer_render_instances_device, "Renderer::render_instances_device", args, n, width, height,
+                           (int(device_ptr), stride, view_stride, channels, clear_color), None, timings, chunk=chunk)
+
+    def render_instances_ids_device(self, composition: Composition, instances: Instances, ids_device_ptr: int, width: int,
+                                    height: int, rgba_ptr: Optional[int] = None, channels=RGBA,
+                                    clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), stride: Optional[int] = None,
+                                    view_stride: Optional[int] = None, ids_stride: Optional[int] = None,
+                                    ids_view_stride: Optional[int] = None, min_coverage: float = 0.0,
+                                    timings: bool = True) -> Optional[Timings]:
+        """The ID frame of every instance frame: per pixel the slot m of the topmost instance
+        painted there, or ID_NONE (an instance-segmentation label); with `rgba_ptr` the frames of
+        render_instances_device as well. Layout as for render_views_ids_device."""
+        n, args, chunk = self._instance_args(composition, instances)
+        return self._stack(self._api.renderer_render_instances_ids_device, "Renderer::render_instances_ids_device", args, n, width,
+                           height, (None if rgba_ptr is None else int(rgba_ptr), stride, view_stride, channels, clear_color),
+                           (int(ids_device_ptr), ids_stride, ids_view_stride, min_coverage), timings, chunk=chunk)
+
+    def render_instances_masks_device(self, composition: Composition, instances: Instances, masks_ptr: int, width: int, height: int,
+                                      first_order: int, n_orders: int, format: str = "f32", stride: Optional[int] = None,
+                                      plane_stride: Optional[int] = None, rgba_ptr: Optional[int] = None, channels=RGBA,
+                                      clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), rgba_stride: Optional[int] = None,
+                                      view_stride: Optional[int] = None, timings: bool = True) -> Optional[Timings]:
+        """The masks (see render_masks) of every instance frame, plane k holding slot
+        first_order + k; layout as for render_views_masks_device."""
+        n, args, chunk = self._instance_args(composition, instances)
+        return self._stack_masks(self._api.renderer_render_instances_masks_device, "Renderer::render_instances_masks_device", args, n,
+                                 masks_ptr, width, height, first_order, n_orders, format, stride, plane_stride, rgba_ptr, channels,
+                                 clear_color, rgba_stride, view_stride, timings, chunk=chunk)
+
+    def render_instances_stats_device(self, composition: Composition, instances: Instances, stats_ptr: int, width: int, height: int,
+                                      first_order: int, n_orders: int, min_coverage: float = 0.0, rgba_ptr: Optional[int] = None,
+                                      channels=RGBA, clear_color: Color = Color(1.0, 1.0, 1.0, 1.0),
+                                      rgba_stride: Optional[int] = None, view_stride: Optional[int] = None,
+                                      timings: bool = True) -> Optional[Timings]:
+        """The statistics (see render_stats) of every instance frame, record k of a frame for slot
+        first_order + k (per-instance areas and boxes); layout as for render_views_stats_device."""
+        n, args, chunk = self._instance_args(composition, instances)
+        return self._stack_stats(self._api.renderer_render_instances_stats_device, "Renderer::render_instances_stats_device", args, n,
+                                 stats_ptr, width, height, first_order, n_orders, min_coverage, rgba_ptr, channels, clear_color,
+                                 rgba_stride, view_stride, timings, chunk=chunk)
 
     def render_poses_linear(self, composition: Composition, poses: Poses, buffer: np.ndarray, width: int, height: int, channels=RGBA,
                             clear_color: Color = Color(1.0, 1.0, 1.0, 1.0), format: str = "f32", stride: Optional[int] = None,

@@ -488,6 +488,31 @@ int forma_renderer_render_poses_ids(forma_renderer* r, forma_composition* c, con
     q.ids = {reinterpret_cast<uint8_t*>(host_ids), false, ids_stride, ids_view_stride, min_coverage};
     return render_request(r, q, c, nullptr, __func__);
 }
+// Instances: the twins of the views calls, with the instance tables in place of the view transforms.
+static FrameRequest instances_request(const forma_instances* instances, uint32_t n, uint64_t width, uint64_t height,
+                                      const uint32_t* channels, const float* clear_color, forma_timings* timings) {
+    FrameRequest q{FrameKind::instances, n, width, height, channels, clear_color, timings};
+    q.instances = instances;
+    return q;
+}
+int forma_renderer_render_instances_device(forma_renderer* r, forma_composition* c, const forma_instances* instances, uint32_t n,
+                                           uint8_t* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                           uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
+                                           forma_timings* timings) {
+    FrameRequest q = instances_request(instances, n, width, height, channels, clear_color, timings);
+    q.rgba = {device_buffer, true, width_stride, view_stride};
+    return render_request(r, q, c);
+}
+int forma_renderer_render_instances_ids_device(forma_renderer* r, forma_composition* c, const forma_instances* instances, uint32_t n,
+                                               uint8_t* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                               uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
+                                               uint32_t* device_ids, uint64_t ids_stride, uint64_t ids_view_stride, float min_coverage,
+                                               forma_timings* timings) {
+    FrameRequest q = instances_request(instances, n, width, height, channels, clear_color, timings);
+    q.rgba = {device_buffer, true, width_stride, view_stride};
+    q.ids = {reinterpret_cast<uint8_t*>(device_ids), true, ids_stride, ids_view_stride, min_coverage};
+    return render_request(r, q, c, nullptr, __func__);
+}
 int forma_renderer_render_batch_device(forma_renderer* r, forma_composition* const* comps, uint32_t n, uint8_t* device_buffer,
                                        uint64_t width, uint64_t width_stride, uint64_t height, uint64_t frame_stride,
                                        const uint32_t channels[4], const float clear_color[4], forma_timings* timings) {
@@ -579,6 +604,13 @@ int forma_renderer_render_poses_masks_device(forma_renderer* r, forma_compositio
     FrameRequest q = poses_request(poses, n, width, height, channels, clear_color, timings);
     return render_masks(r, q, masks, true, device_buffer, width_stride, view_stride, c, nullptr, __func__);
 }
+int forma_renderer_render_instances_masks_device(forma_renderer* r, forma_composition* c, const forma_instances* instances, uint32_t n,
+                                                 const forma_masks* masks, uint64_t width, uint64_t height, uint8_t* device_buffer,
+                                                 uint64_t width_stride, uint64_t view_stride, const uint32_t channels[4],
+                                                 const float clear_color[4], forma_timings* timings) {
+    FrameRequest q = instances_request(instances, n, width, height, channels, clear_color, timings);
+    return render_masks(r, q, masks, true, device_buffer, width_stride, view_stride, c, nullptr, __func__);
+}
 int forma_renderer_render_batch_masks_device(forma_renderer* r, forma_composition* const* comps, uint32_t n,
                                              const forma_masks* masks, uint64_t width, uint64_t height, uint8_t* device_buffer,
                                              uint64_t width_stride, uint64_t frame_stride, const uint32_t channels[4],
@@ -624,6 +656,13 @@ int forma_renderer_render_poses_stats_device(forma_renderer* r, forma_compositio
                                              uint64_t width_stride, uint64_t view_stride, const uint32_t channels[4],
                                              const float clear_color[4], forma_timings* timings) {
     FrameRequest q = poses_request(poses, n, width, height, channels, clear_color, timings);
+    return render_stats(r, q, stats, true, device_buffer, width_stride, view_stride, c, nullptr, __func__);
+}
+int forma_renderer_render_instances_stats_device(forma_renderer* r, forma_composition* c, const forma_instances* instances, uint32_t n,
+                                                 const forma_stats* stats, uint64_t width, uint64_t height, uint8_t* device_buffer,
+                                                 uint64_t width_stride, uint64_t view_stride, const uint32_t channels[4],
+                                                 const float clear_color[4], forma_timings* timings) {
+    FrameRequest q = instances_request(instances, n, width, height, channels, clear_color, timings);
     return render_stats(r, q, stats, true, device_buffer, width_stride, view_stride, c, nullptr, __func__);
 }
 int forma_renderer_render_batch_stats_device(forma_renderer* r, forma_composition* const* comps, uint32_t n,

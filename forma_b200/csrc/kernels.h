@@ -152,6 +152,43 @@ void launch_line_count_batch(const BatchArgs& batch, uint32_t n_ctas, uint32_t* 
                              cudaStream_t stream);
 void launch_raster_emit_batch(const BatchArgs& batch, uint32_t n_ctas, const uint32_t* block_offsets, uint64_t* out, uint32_t cap,
                               cudaStream_t stream, const CountArgs* counts = nullptr);
+// Instance scenes (see forma_renderer_render_instances_device): a stack of n_frames frames of one
+// composition (RasterArgs), frame b drawing its slots' prototypes as the layers b * n_slots + m.
+// Frame b's line records lines[frame_first[b], frame_first[b + 1]) are in (slot, insert) order;
+// record r covers the point pairs [first_pair, first_pair + n_pairs) of its frame, which are the
+// pairs (first_point + j, first_point + j + 1) of the segment buffer, and draws them with the
+// transform of recs[slot] (slot = b * n_slots + m), enabled, at layer order slot. A frame's pairs
+// are padded to whole CTAs: CTA x belongs to the last frame with cta_first[b] <= x.
+struct InstanceLine {  // 16 B
+    uint32_t first_pair;   // frame-local: the pairs of the frame's records before this one
+    uint32_t n_pairs;
+    uint32_t first_point;  // in the composition's segment buffer
+    uint32_t slot;         // b * n_slots + m: the layer order and the PoseRec of the instance
+};
+struct InstanceArgs {
+    const InstanceLine* lines;
+    const uint32_t* frame_first;  // n_frames + 1: each frame's first line record
+    const uint32_t* cta_first;    // n_frames + 1: each frame's first CTA
+    const PoseRec* recs;          // n_frames x n_slots
+    uint32_t n_frames, n_slots;
+    uint32_t rows;                // tile rows per frame: ceil(height / 16)
+};
+// cta_first[n_frames] block sums, frame-major; max_tile[1] is the stacked bound.
+void launch_line_count_instances(const RasterArgs& args, const InstanceArgs& inst, uint32_t n_ctas, uint32_t* block_sums, uint32_t* total,
+                                 uint32_t* max_tile, cudaStream_t stream);
+void launch_raster_emit_instances(const RasterArgs& args, const InstanceArgs& inst, uint32_t n_ctas, const uint32_t* block_offsets,
+                                  uint64_t* out, uint32_t cap, cudaStream_t stream, const CountArgs* counts = nullptr);
+// The instance records (instance_fold_kernel): record r of slot r starts from the record of its
+// prototype p = prototypes[r], base[p] (the layer's own transform and bits), or stays zero for an
+// empty slot (FORMA_NO_INSTANCE). transforms[r] replaces the transform as in pose_fold_kernel, with
+// the same refusal word; every instance is enabled.
+struct InstanceFoldArgs {
+    const uint32_t* prototypes;  // n_recs layer orders (device)
+    const PoseRec* base;         // per order up to the largest prototype
+    const float* transforms;     // nullable: 6 floats per record, 4-byte aligned
+    uint32_t* first_bad;         // nullable: atomicMin of every r whose transform forma_layer_set_transform refuses
+};
+void launch_instance_fold(const InstanceFoldArgs& args, PoseRec* recs, uint32_t n_recs, cudaStream_t stream);
 // Line records of the n = n_points - 1 point pairs (inspection only): orders, then
 // f = {x0, y0, dx, dy, a, b, c, d}, then the per-line segment counts.
 void launch_line_records(const RasterArgs& args, uint32_t n, uint32_t* orders, float* const f[8], uint32_t* lengths,
@@ -388,6 +425,13 @@ void launch_merge_entries(const PaintScene& S, const uint64_t* cell_key, uint32_
 // colour colors[i] (linear RGBA) and no gradient or texture left; orders without a layer get none.
 void launch_pose_styles(const int32_t* order_to_style, uint32_t n_orders, StyleRec* styles, uint32_t n_styles, const float4* colors,
                         uint32_t first_order, uint32_t n_window, uint64_t n_recs, cudaStream_t st);
+// The order -> style table of an instance call, one thread per slot r: -1 for an empty slot
+// (FORMA_NO_INSTANCE) or a prototype without a style, the prototype's own slot when colors is null
+// or the prototype does not draw, else n_styles + r, where `styles` (whose slots [0, n_styles) hold
+// the composition's records) receives the prototype's StyleRec made solid with colors[r], as
+// launch_pose_styles makes it.
+void launch_instance_styles(const int32_t* order_to_style, uint32_t n_orders, const uint32_t* prototypes, StyleRec* styles,
+                            uint32_t n_styles, const float4* colors, uint32_t n_recs, int32_t* inst_order_to_style, cudaStream_t st);
 // The painter tables of a frame as every tile kernel (paint, ID, mask, statistics) reads them: the
 // sorted segments, the entry records, the per-tile entry ranges and, when `heavy` is not null, the
 // heavy-tile lists with their lengths (launch_merge_entries).

@@ -213,9 +213,11 @@ __device__ __forceinline__ uint32_t warp_inclusive_scan_sat(uint32_t v) {
 // layer without one), composed exactly as ViewArgs documents; a composed identity is no transform.
 // kPoses: a layer whose order lies in Q's window takes frame blockIdx.y's record (PoseArgs) in
 // place of its own transform and enabled bit.
-template <bool kViews = false, bool kPoses = false>
+// kInst: the pair belongs to an instance (instance_line_setup), whose layer record `inst` is
+// taken in place of the geometry's layer.
+template <bool kViews = false, bool kPoses = false, bool kInst = false>
 __device__ __forceinline__ LineParams line_setup(const RasterArgs& A, uint32_t i, const float* V = nullptr,
-                                                 const PoseArgs& Q = PoseArgs{}) {
+                                                 const PoseArgs& Q = PoseArgs{}, const LayerRec* inst = nullptr) {
     LineParams L;
     L.length = 0;
     L.order = 0;
@@ -223,16 +225,20 @@ __device__ __forceinline__ LineParams line_setup(const RasterArgs& A, uint32_t i
     if (i + 1u >= A.n_points) return L;
     uint32_t gid = A.gid[i];
     if (gid == 0u) return L;
-    int32_t slot = gid < A.n_geoms ? A.geom_slot[gid] : -1;
-    if (slot < 0) return L;
     LayerRec lay;
-    if (A.layers) {
-        lay = A.layers[slot];
-    } else {  // no layer carries a transform: 4 bytes per layer (order | enabled << 21)
-        const uint32_t bits = A.layer_bits[slot];
-        lay.order = bits & 0x1FFFFFu;
-        lay.enabled = (bits >> 21) & 1u;
-        lay.has_xf = 0u;
+    if constexpr (kInst) {
+        lay = *inst;
+    } else {
+        int32_t slot = gid < A.n_geoms ? A.geom_slot[gid] : -1;
+        if (slot < 0) return L;
+        if (A.layers) {
+            lay = A.layers[slot];
+        } else {  // no layer carries a transform: 4 bytes per layer (order | enabled << 21)
+            const uint32_t bits = A.layer_bits[slot];
+            lay.order = bits & 0x1FFFFFu;
+            lay.enabled = (bits >> 21) & 1u;
+            lay.has_xf = 0u;
+        }
     }
     if constexpr (kPoses) {
         const uint32_t k = lay.order - Q.first_order;  // (wraps for orders below the window)
@@ -326,6 +332,58 @@ __device__ __forceinline__ BatchPos batch_pos(const BatchArgs& B, RasterArgs& A)
     return BatchPos{lo, blockIdx.x - B.cta_first[lo], F.order_base};
 }
 
+// Where a CTA of an instance call works (InstanceArgs): its frame (the last one whose first CTA is
+// at or before it: frames without point pairs own no CTA), its CTA within the frame's padded
+// pairs, and the frame's order base b * n_slots.
+__device__ __forceinline__ BatchPos instance_pos(const InstanceArgs& I) {
+    uint32_t lo = 0, hi = I.n_frames - 1u;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1u) >> 1;
+        if (__ldg(I.cta_first + mid) <= blockIdx.x) lo = mid;
+        else hi = mid - 1u;
+    }
+    return BatchPos{lo, blockIdx.x - __ldg(I.cta_first + lo), lo * I.n_slots};
+}
+
+// The line of pair j of frame P.frame: its record is the last of the frame's records whose first
+// pair is at or before j (a library shape has tens to hundreds of points, so the threads of a
+// CTA share out several records); pairs past the frame's last record are the CTA padding. The
+// instance's PoseRec stands in for the layer record, enabled, at the frame-local order m (the
+// emit pass adds the frame's base).
+__device__ __forceinline__ LineParams instance_line_setup(const RasterArgs& A, const InstanceArgs& I, const BatchPos& P, uint32_t j) {
+    uint32_t lo = __ldg(I.frame_first + P.frame), hi = __ldg(I.frame_first + P.frame + 1u) - 1u;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1u) >> 1;
+        if (__ldg(&I.lines[mid].first_pair) <= j) lo = mid;
+        else hi = mid - 1u;
+    }
+    const uint4 R = __ldg(reinterpret_cast<const uint4*>(I.lines + lo));  // first_pair, n_pairs, first_point, slot
+    const uint32_t k = j - R.x;
+    if (k >= R.y) {
+        LineParams L;
+        L.length = 0;
+        L.order = 0;
+        L.x0 = L.y0 = L.dx = L.dy = L.a = L.b = L.c = L.d = 0.0f;
+        return L;
+    }
+    const float4* r = reinterpret_cast<const float4*>(I.recs + R.w);
+    const float4 a = __ldg(r), b = __ldg(r + 1);
+    LayerRec lay;
+    lay.order = R.w - P.order_base;
+    lay.enabled = 1u;
+    lay.has_xf = __float_as_uint(b.z) & 1u;
+    lay.ux = a.x; lay.uy = a.y; lay.vx = a.z; lay.vy = a.w; lay.tx = b.x; lay.ty = b.y;
+    return line_setup<false, false, true>(A, R.z + k, nullptr, PoseArgs{}, &lay);
+}
+
+// The line of thread i of a line-setup CTA in each mode (kInst: pair i of the CTA's instance frame).
+template <bool kViews, bool kPoses, bool kInst>
+__device__ __forceinline__ LineParams frame_line(const RasterArgs& A, uint32_t i, const ViewArgs& V, const PoseArgs& Q, const BatchPos& P,
+                                                 const InstanceArgs& I) {
+    if constexpr (kInst) return instance_line_setup(A, I, P, i);
+    else return line_setup<kViews, kPoses>(A, i, kViews ? V.xf + 6u * blockIdx.y : nullptr, Q);
+}
+
 // Pass 1: per-CTA sum of line lengths.
 // Also tracks the largest (biased) tile coordinates any pixel segment can take,
 // so that the sort only spends passes on key bits that can be set.
@@ -333,15 +391,16 @@ __device__ __forceinline__ BatchPos batch_pos(const BatchArgs& B, RasterArgs& A)
 // kBatch: CTA x = the point pairs of CTA P.block of frame P.frame (V.rows: the frame's tile rows);
 // its sum is block x.
 // kPoses: as kViews, with frame y's pose records (Q) in place of a view transform.
-template <bool kViews, bool kBatch = false, bool kPoses = false>
+// kInst (with kBatch): CTA x = the point pairs of CTA P.block of instance frame P.frame (I).
+template <bool kViews, bool kBatch = false, bool kPoses = false, bool kInst = false>
 __device__ __forceinline__ void line_count_body(const RasterArgs& A, const ViewArgs& V, uint32_t* __restrict__ block_sums,
                                                 uint32_t* __restrict__ max_tile, const BatchPos& P = BatchPos{},
-                                                const PoseArgs& Q = PoseArgs{}) {
+                                                const PoseArgs& Q = PoseArgs{}, const InstanceArgs& I = InstanceArgs{}) {
     constexpr bool kStack = kViews || kPoses;  // the stack of one composition: frame blockIdx.y
     __shared__ uint32_t warp_sums[kRasterThreads / 32];
     __shared__ uint32_t warp_max[2][kRasterThreads / 32];
     uint32_t i = (kBatch ? P.block : blockIdx.x) * kRasterThreads + threadIdx.x;
-    const LineParams L = line_setup<kViews, kPoses>(A, i, kViews ? V.xf + 6u * blockIdx.y : nullptr, Q);
+    const LineParams L = frame_line<kViews, kPoses, kInst>(A, i, V, Q, P, I);
     uint32_t len = L.length;
     {
         uint32_t bx = 0, by = 0;
@@ -411,6 +470,11 @@ __global__ void __launch_bounds__(kRasterThreads) line_count_batch_kernel(BatchA
 __global__ void __launch_bounds__(kRasterThreads) line_count_poses_kernel(RasterArgs A, PoseArgs Q, uint32_t* __restrict__ block_sums,
                                                                         uint32_t* __restrict__ max_tile) {
     line_count_body<false, false, true>(A, ViewArgs{nullptr, Q.rows}, block_sums, max_tile, BatchPos{}, Q);
+}
+__global__ void __launch_bounds__(kRasterThreads) line_count_instances_kernel(RasterArgs A, InstanceArgs I, uint32_t* __restrict__ block_sums,
+                                                                            uint32_t* __restrict__ max_tile) {
+    const BatchPos P = instance_pos(I);
+    line_count_body<false, true, false, true>(A, ViewArgs{nullptr, I.rows}, block_sums, max_tile, P, PoseArgs{}, I);
 }
 
 // Device-wide exclusive scan of `n` u32 values by ONE CTA (n = number of CTAs
@@ -502,10 +566,12 @@ struct SharedLines {
 // shared memory, warp-aggregated, and go out once per CTA; the tiles after those two (a CTA of long
 // lines) take warp-aggregated global atomics.
 // kPoses: as kViews, with frame y's pose records (Q) in place of a view transform.
-template <bool kViews, bool kBatch = false, bool kCount = false, bool kPoses = false>
+// kInst (with kBatch): CTA x emits instance frame P.frame's segments (I), at the orders b M + m.
+template <bool kViews, bool kBatch = false, bool kCount = false, bool kPoses = false, bool kInst = false>
 __device__ __forceinline__ void raster_emit_body(const RasterArgs& A, const ViewArgs& V, const uint32_t* __restrict__ block_offsets,
                                                  uint64_t* __restrict__ out, uint32_t cap, const BatchPos& P = BatchPos{},
-                                                 const CountArgs& C = CountArgs{}, const PoseArgs& Q = PoseArgs{}) {
+                                                 const CountArgs& C = CountArgs{}, const PoseArgs& Q = PoseArgs{},
+                                                 const InstanceArgs& I = InstanceArgs{}) {
     constexpr bool kStack = kViews || kPoses;  // the stack of one composition: frame blockIdx.y
     __shared__ SharedLines S;
     __shared__ uint32_t warp_sums[kRasterThreads / 32];
@@ -517,7 +583,7 @@ __device__ __forceinline__ void raster_emit_body(const RasterArgs& A, const View
         s_count[t + kRasterThreads] = 0;
     }
     uint32_t i = (kBatch ? P.block : blockIdx.x) * kRasterThreads + t;
-    LineParams L = line_setup<kViews, kPoses>(A, i, kViews ? V.xf + 6u * blockIdx.y : nullptr, Q);
+    LineParams L = frame_line<kViews, kPoses, kInst>(A, i, V, Q, P, I);
     if constexpr (kBatch) L.order += P.order_base;
     uint32_t incl = warp_inclusive_scan_sat(L.length);
     if (lane == 31) warp_sums[warp] = incl;
@@ -632,9 +698,27 @@ __global__ void __launch_bounds__(kRasterThreads, kCount ? 8 : 0) raster_emit_po
     raster_emit_body<false, false, kCount, true>(A, ViewArgs{nullptr, Q.rows}, block_offsets, out, cap, BatchPos{}, C, Q);
 }
 
-// The pose records the two kernels above read, one thread per record (see PoseFoldArgs). A
-// transform is tested as geom_pres_ok (host_path.cpp) tests it, in the same separately rounded f32
-// operations, for every record (orders without a layer included, as check_poses walks them).
+template <bool kCount>
+__global__ void __launch_bounds__(kRasterThreads, kCount ? 8 : 0) raster_emit_instances_kernel(RasterArgs A, InstanceArgs I, const uint32_t* __restrict__ block_offsets,
+                                                                             uint64_t* __restrict__ out, uint32_t cap, CountArgs C) {
+    const BatchPos P = instance_pos(I);
+    raster_emit_body<false, true, kCount, false, true>(A, ViewArgs{nullptr, I.rows}, block_offsets, out, cap, P, C, PoseArgs{}, I);
+}
+
+// A record's transform from a table ([ux, vx, uy, vy, tx, ty] at t): tested as geom_pres_ok
+// (host_path.cpp) tests it, in the same separately rounded f32 operations (a refused record r is
+// atomicMin'ed into *first_bad when that is not null), and an identity is no transform.
+__device__ __forceinline__ void fold_transform(const float* t, uint32_t r, uint32_t* first_bad, float& ux, float& uy, float& vx, float& vy,
+                                               float& tx, float& ty, bool& has_xf) {
+    ux = __ldg(t); vx = __ldg(t + 1); uy = __ldg(t + 2); vy = __ldg(t + 3); tx = __ldg(t + 4); ty = __ldg(t + 5);
+    const float max_x = 1.0f + (1.0f / 16.0f) / 65536.0f, max_y = 1.0f + (1.0f / 16.0f) / 32768.0f;
+    const bool ok = !(__fadd_rn(__fmul_rn(ux, ux), __fmul_rn(uy, uy)) > max_x) && !(__fadd_rn(__fmul_rn(vx, vx), __fmul_rn(vy, vy)) > max_y);
+    if (first_bad && !ok) atomicMin(first_bad, r);
+    has_xf = !(ux == 1.0f && uy == 0.0f && vx == 0.0f && vy == 1.0f && tx == 0.0f && ty == 0.0f);
+}
+
+// The pose records the two kernels above read, one thread per record (see PoseFoldArgs). Every
+// record's transform is tested (orders without a layer included, as check_poses walks them).
 __global__ void __launch_bounds__(256) pose_fold_kernel(PoseFoldArgs F, PoseRec* __restrict__ recs, uint32_t n_recs) {
     chain_begin();
     const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
@@ -644,14 +728,7 @@ __global__ void __launch_bounds__(256) pose_fold_kernel(PoseFoldArgs F, PoseRec*
     float ux = a.x, uy = a.y, vx = a.z, vy = a.w, tx = b.x, ty = b.y;
     const uint32_t bits = __float_as_uint(b.z);
     bool has_xf = bits & 1u, enabled = (bits >> 1) & 1u;
-    if (F.transforms) {  // [ux, vx, uy, vy, tx, ty]
-        const float* t = F.transforms + 6ull * r;
-        ux = __ldg(t); vx = __ldg(t + 1); uy = __ldg(t + 2); vy = __ldg(t + 3); tx = __ldg(t + 4); ty = __ldg(t + 5);
-        const float max_x = 1.0f + (1.0f / 16.0f) / 65536.0f, max_y = 1.0f + (1.0f / 16.0f) / 32768.0f;
-        const bool ok = !(__fadd_rn(__fmul_rn(ux, ux), __fmul_rn(uy, uy)) > max_x) && !(__fadd_rn(__fmul_rn(vx, vx), __fmul_rn(vy, vy)) > max_y);
-        if (F.first_bad && !ok) atomicMin(F.first_bad, r);
-        has_xf = !(ux == 1.0f && uy == 0.0f && vx == 0.0f && vy == 1.0f && tx == 0.0f && ty == 0.0f);
-    }
+    if (F.transforms) fold_transform(F.transforms + 6ull * r, r, F.first_bad, ux, uy, vx, vy, tx, ty, has_xf);
     if (F.visible) enabled = __ldg(F.visible + r) != 0;
     float4* out = reinterpret_cast<float4*>(recs + r);
     if (!(bits & kPoseLayer)) {
@@ -660,6 +737,28 @@ __global__ void __launch_bounds__(256) pose_fold_kernel(PoseFoldArgs F, PoseRec*
     }
     out[0] = make_float4(ux, uy, vx, vy);
     out[1] = make_float4(tx, ty, __uint_as_float((has_xf ? 1u : 0u) | (enabled ? 2u : 0u)), 0.0f);
+}
+
+// The instance records (see InstanceFoldArgs), one thread per slot: the prototype's own record
+// with the slot's transform folded in as pose_fold_kernel folds it, enabled. Only the transforms of
+// slots with a prototype are tested; an empty slot's record stays zero (no line reads it).
+__global__ void __launch_bounds__(256) instance_fold_kernel(InstanceFoldArgs F, PoseRec* __restrict__ recs, uint32_t n_recs) {
+    chain_begin();
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_recs) return;
+    const uint32_t p = __ldg(F.prototypes + r);
+    float4* out = reinterpret_cast<float4*>(recs + r);
+    if (p == 0xFFFFFFFFu) {  // FORMA_NO_INSTANCE
+        out[0] = out[1] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        return;
+    }
+    const float4* w = reinterpret_cast<const float4*>(F.base + p);
+    const float4 a = __ldg(w), b = __ldg(w + 1);
+    float ux = a.x, uy = a.y, vx = a.z, vy = a.w, tx = b.x, ty = b.y;
+    bool has_xf = __float_as_uint(b.z) & 1u;
+    if (F.transforms) fold_transform(F.transforms + 6ull * r, r, F.first_bad, ux, uy, vx, vy, tx, ty, has_xf);
+    out[0] = make_float4(ux, uy, vx, vy);
+    out[1] = make_float4(tx, ty, __uint_as_float((has_xf ? 1u : 0u) | 2u), 0.0f);
 }
 
 // Inspection only (forma_renderer_lines): the line records of segment.rs:298-383 as the
@@ -767,6 +866,28 @@ void launch_raster_emit_poses(const RasterArgs& args, const PoseArgs& poses, uin
 
 void launch_pose_fold(const PoseFoldArgs& args, PoseRec* recs, uint32_t n_recs, cudaStream_t stream) {
     if (n_recs) launch_chained(pose_fold_kernel, (uint32_t)(((uint64_t)n_recs + 255u) / 256u), 256, 0, stream, args, recs, n_recs);
+}
+
+void launch_instance_fold(const InstanceFoldArgs& args, PoseRec* recs, uint32_t n_recs, cudaStream_t stream) {
+    if (n_recs) launch_chained(instance_fold_kernel, (uint32_t)(((uint64_t)n_recs + 255u) / 256u), 256, 0, stream, args, recs, n_recs);
+}
+
+void launch_line_count_instances(const RasterArgs& args, const InstanceArgs& inst, uint32_t n_ctas, uint32_t* block_sums, uint32_t* total,
+                                 uint32_t* max_tile, cudaStream_t stream) {
+    cudaMemsetAsync(max_tile, 0, 2 * sizeof(uint32_t), stream);
+    if (!n_ctas) {
+        cudaMemsetAsync(total, 0, sizeof(uint32_t), stream);
+        return;
+    }
+    line_count_instances_kernel<<<n_ctas, kRasterThreads, 0, stream>>>(args, inst, block_sums, max_tile);
+    launch_chained(scan_block_sums_kernel, 1, 1024, 0, stream, block_sums, n_ctas, total);
+}
+
+void launch_raster_emit_instances(const RasterArgs& args, const InstanceArgs& inst, uint32_t n_ctas, const uint32_t* block_offsets,
+                                  uint64_t* out, uint32_t cap, cudaStream_t stream, const CountArgs* counts) {
+    if (!n_ctas) return;
+    if (counts) raster_emit_instances_kernel<true><<<n_ctas, kRasterThreads, 0, stream>>>(args, inst, block_offsets, out, cap, *counts);
+    else raster_emit_instances_kernel<false><<<n_ctas, kRasterThreads, 0, stream>>>(args, inst, block_offsets, out, cap, CountArgs{});
 }
 
 void launch_line_count_batch(const BatchArgs& batch, uint32_t n_ctas, uint32_t* block_sums, uint32_t* total, uint32_t* max_tile,

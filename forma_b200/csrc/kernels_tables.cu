@@ -775,6 +775,21 @@ __global__ void merge_entries_pose_fills_kernel(PaintScene S, const uint64_t* __
                              heavy, heavy_count, dc, nullptr, 0u, F);
 }
 
+// A Draw layer's StyleRec with its fill made Fill::Solid(c): no gradient or texture left.
+__device__ __forceinline__ void make_solid(StyleRec& r, float4 c) {
+    r.fill_type = 0u;
+    r.color[0] = c.x;
+    r.color[1] = c.y;
+    r.color[2] = c.z;
+    r.color[3] = c.w;
+    r.gradient_type = 0u;
+    r.start[0] = r.start[1] = r.end[0] = r.end[1] = 0.0f;
+    r.stop_count = 0u;
+    for (int j = 0; j < 6; ++j) r.tex_xf[j] = 0.0f;
+    r.tex_max_x = r.tex_max_y = 0.0f;
+    r.tex_width = r.tex_first = 0u;
+}
+
 // The tail of a pose style table, one thread per (frame b, order first_order + k) record i = b K + k:
 // the StyleRec of the layer at that order with its fill made Fill::Solid(colors[i]) when the layer
 // draws; a Clip layer's record is its own (merge_entries never points at it). Orders without a
@@ -790,21 +805,27 @@ __global__ void __launch_bounds__(256) pose_styles_kernel(const int32_t* __restr
     const int32_t s = o < n_orders ? order_to_style[o] : -1;
     if (s < 0) return;
     StyleRec r = styles[s];
-    if (r.func == 0u) {
-        const float4 c = colors[i];
-        r.fill_type = 0u;
-        r.color[0] = c.x;
-        r.color[1] = c.y;
-        r.color[2] = c.z;
-        r.color[3] = c.w;
-        r.gradient_type = 0u;
-        r.start[0] = r.start[1] = r.end[0] = r.end[1] = 0.0f;
-        r.stop_count = 0u;
-        for (int j = 0; j < 6; ++j) r.tex_xf[j] = 0.0f;
-        r.tex_max_x = r.tex_max_y = 0.0f;
-        r.tex_width = r.tex_first = 0u;
-    }
+    if (r.func == 0u) make_solid(r, colors[i]);
     styles[n_styles + i] = r;
+}
+
+// The order -> style table of an instance call, one thread per slot r (see launch_instance_styles).
+__global__ void __launch_bounds__(256) instance_styles_kernel(const int32_t* __restrict__ order_to_style, uint32_t n_orders,
+                                                              const uint32_t* __restrict__ prototypes, StyleRec* __restrict__ styles,
+                                                              uint32_t n_styles, const float4* __restrict__ colors, uint32_t n_recs,
+                                                              int32_t* __restrict__ inst_order_to_style) {
+    chain_begin();
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_recs) return;
+    const uint32_t p = prototypes[r];  // (FORMA_NO_INSTANCE is no order)
+    int32_t s = p < n_orders ? order_to_style[p] : -1;
+    if (s >= 0 && colors && styles[s].func == 0u) {
+        StyleRec rec = styles[s];
+        make_solid(rec, colors[r]);
+        styles[n_styles + r] = rec;
+        s = (int32_t)(n_styles + r);
+    }
+    inst_order_to_style[r] = s;
 }
 
 // Cost of every tile row of the frame just rendered: 32 x its (tile, layer) entries + its
@@ -967,6 +988,12 @@ void launch_pose_styles(const int32_t* order_to_style, uint32_t n_orders, StyleR
     if (n_recs)
         launch_chained(pose_styles_kernel, (unsigned)((n_recs + 255u) / 256u), 256, 0, st, order_to_style, n_orders, styles, n_styles, colors,
                                                                                first_order, n_window, n_recs);
+}
+void launch_instance_styles(const int32_t* order_to_style, uint32_t n_orders, const uint32_t* prototypes, StyleRec* styles,
+                            uint32_t n_styles, const float4* colors, uint32_t n_recs, int32_t* inst_order_to_style, cudaStream_t st) {
+    if (n_recs)
+        launch_chained(instance_styles_kernel, (n_recs + 255u) / 256u, 256, 0, st, order_to_style, n_orders, prototypes, styles, n_styles,
+                       colors, n_recs, inst_order_to_style);
 }
 
 // ---------------------------------------------------------------------------

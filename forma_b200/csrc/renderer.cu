@@ -245,9 +245,10 @@ int Renderer::upload_tables_device(Composition& comp, CompDevice& cd) {
 
 // Stages 1½ + 2: fills `segs` with the unsorted pixel segments.
 int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, float band_lo, float band_hi,
-                        uint32_t* n_out, const ViewArgs* views, uint32_t n_views, const BatchLines* batch, const PoseArgs* poses) {
+                        uint32_t* n_out, const ViewArgs* views, uint32_t n_views, const BatchLines* batch, const PoseArgs* poses,
+                        const InstanceLines* inst) {
     RasterArgs& ra = last_raster;  // kept for forma_renderer_lines (a stacked frame has no line records)
-    last_raster_valid = !views && !batch && !poses;
+    last_raster_valid = !views && !batch && !poses && !inst;
     if (comp) {
         CompDevice& cd = comp->on(res_key);
         ra.x = cd.d_x.ptr;
@@ -263,7 +264,7 @@ int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, floa
         ra.band_lo = band_lo;
         ra.band_hi = band_hi;
     }
-    uint32_t nb = batch ? batch->n_ctas : raster_num_blocks(ra.n_points);
+    uint32_t nb = batch ? batch->n_ctas : inst ? inst->n_ctas : raster_num_blocks(ra.n_points);
     if (views || poses) {
         if ((uint64_t)nb * n_views >= (1ull << 32)) {
             set_error("%u views of %u points exceed the line-setup grid", n_views, ra.n_points);
@@ -275,12 +276,14 @@ int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, floa
     if (batch) launch_line_count_batch(batch->args, nb, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
     else if (views) launch_line_count_views(ra, *views, n_views, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
     else if (poses) launch_line_count_poses(ra, *poses, n_views, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
+    else if (inst) launch_line_count_instances(ra, inst->args, nb, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
     else launch_line_count(ra, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
     launches += nb ? 2 : 0;
     auto emit = [&](uint32_t cap, const CountArgs* counts) {
         if (batch) launch_raster_emit_batch(batch->args, nb, block_sums.ptr, segs.ptr, cap, stream, counts);
         else if (views) launch_raster_emit_views(ra, *views, n_views, block_sums.ptr, segs.ptr, cap, stream, counts);
         else if (poses) launch_raster_emit_poses(ra, *poses, n_views, block_sums.ptr, segs.ptr, cap, stream, counts);
+        else if (inst) launch_raster_emit_instances(ra, inst->args, nb, block_sums.ptr, segs.ptr, cap, stream, counts);
         else launch_raster_emit(ra, block_sums.ptr, segs.ptr, cap, stream, counts);
     };
     // The emit pass counts the sort's pass-0 digits (TileCounts) when the sort will take them: with
@@ -320,6 +323,7 @@ int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, floa
         // Already ordered by layer: no layer digits (see Composition::layers_in_order).
         const bool skip_layer_digits = options().sort_full_key == 0;
         const uint64_t layer_bound = batch ? batch->layer_bound
+                                     : inst ? inst->layer_bound
                                      : (comp->layers_in_order && skip_layer_digits) ? 0u
                                                                                     : (comp->n_orders ? comp->n_orders - 1u : 0u);
         const uint64_t bound[3] = {layer_bound, pinned_totals[4], pinned_totals[5]};
@@ -433,8 +437,10 @@ int Renderer::run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p
     const uint32_t height = (uint32_t)q.height;
     const FrameBand band = p.rows ? FrameBand{0.0f, (float)height, false} : tile_band(S.ty_lo, S.ty_hi, height);
     const bool views = q.kind == FrameKind::views, batched = q.kind == FrameKind::batch, poses = q.kind == FrameKind::poses;
+    const bool instances = q.kind == FrameKind::instances;
     int st = FORMA_STATUS_OK;
     BatchLines batch{};
+    InstanceLines inst{};
     if (batched) {  // every composition's uploads, then the batch tables
         st = bind_batch(q.batch, q.n, S, height, batch);
         if (st) return st;
@@ -463,13 +469,17 @@ int Renderer::run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p
         st = upload_poses(q);
         if (st) return st;
     }
+    if (instances) {  // (after the uploads: compact_geom may have moved the inserts' points)
+        st = upload_instances(q, S, inst);
+        if (st) return st;
+    }
     const ViewArgs va{d_views.ptr, (height + 15u) / 16u};
     const PoseArgs pa{d_poses.ptr, poses ? q.poses->first_order : 0u, poses ? q.poses->n_orders : 0u, (height + 15u) / 16u};
 
     FORMA_CUDA_TRY(cudaEventRecord(timer.ev[7], stream));
     uint32_t n = 0;
     st = rasterize(q.comp, S.width, height, band.lo, band.hi, &n, views ? &va : nullptr, q.n, batched ? &batch : nullptr,
-                   poses ? &pa : nullptr);
+                   poses ? &pa : nullptr, instances ? &inst : nullptr);
     if (st) return st;
 
     // Stage 3: sort.
@@ -520,8 +530,8 @@ int Renderer::run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p
     uint32_t paint_launches = 1;
     for (bool sync_free = fast;; sync_free = false) {
         DevCounts dc;
-        st = build_tables(S, n, sync_free, prev_cells, prev_gaps, heavy_lists, dc, batched ? &batch.args : nullptr,
-                          q.pose_fills() ? &fills : nullptr);
+        st = build_tables(S, n, sync_free, prev_cells, prev_gaps, heavy_lists, dc,
+                          batched ? &batch.args : instances ? &inst.frames : nullptr, q.pose_fills() ? &fills : nullptr);
         if (st) return st;
         st = queue_row_costs(S, n);
         if (st) return st;
@@ -559,7 +569,9 @@ int Renderer::run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p
         timings->rasterize_ms = stage_ms[2];
         timings->sort_ms = stage_ms[3];
         timings->paint_ms = stage_ms[4] + stage_ms[5];
-        if (q.comp) {
+        if (instances) {
+            timings->n_lines = inst.n_lines;
+        } else if (q.comp) {
             const CompDevice& cd = q.comp->on(res_key);
             timings->n_lines = cd.n_resident ? cd.n_resident - 1 : 0;
         } else {
@@ -635,12 +647,38 @@ int Renderer::render(const FrameRequest& q) {
     return FORMA_STATUS_OK;
 }
 
+// Where each of the three tables of a poses or instances request lives (on_device[t]): device
+// memory of the renderer's device is read there (aligned[t]: the table must be 4-byte aligned),
+// device memory of another device is refused, and anything else is host memory.
+static int locate_tables(const void* const tables[3], const char* const names[3], const bool aligned[3], const char* what, int device,
+                         bool on_device[3]) {
+    for (int t = 0; t < 3; ++t) {
+        on_device[t] = false;
+        if (!tables[t]) continue;
+        cudaPointerAttributes attr{};
+        if (cudaPointerGetAttributes(&attr, tables[t]) != cudaSuccess) {
+            cudaGetLastError();  // (not memory CUDA knows: host memory)
+            continue;
+        }
+        if (attr.type != cudaMemoryTypeDevice) continue;
+        if (attr.device != device) {
+            set_error("%s table %s is in the memory of device %d; the renderer renders on device %d", what, names[t], attr.device, device);
+            return FORMA_STATUS_INVALID;
+        }
+        if (aligned[t] && ((uintptr_t)tables[t] & 3u) != 0u) {
+            set_error("%s table %s in device memory must be 4-byte aligned", what, names[t]);
+            return FORMA_STATUS_INVALID;
+        }
+        on_device[t] = true;
+    }
+    return FORMA_STATUS_OK;
+}
+
 // The pose tables of a poses request (see forma_renderer_render_poses_device): a window of 1 to
 // 2^21 orders below 2^21, at least one table, and every transform one forma_layer_set_transform
 // accepts. Colours are any floats (forma_layer_set_props takes them all).
-// Where each table lives (pose_tables_on_device): device memory of this renderer's device is read
-// there (a float table must be 4-byte aligned), device memory of another device is refused, and
-// anything else is host memory. Host transforms are checked here; device transforms by the fold
+// Where each table lives: pose_tables_on_device (locate_tables; a float table in device memory must
+// be 4-byte aligned). Host transforms are checked here; device transforms by the fold
 // (upload_poses), which reports the first record that fails.
 int Renderer::check_poses(const FrameRequest& q) {
     const forma_poses* P = q.poses;
@@ -657,25 +695,9 @@ int Renderer::check_poses(const FrameRequest& q) {
     }
     const void* const tables[3] = {P->transforms, P->visible, P->colors};
     static const char* const names[3] = {"transforms", "visible", "colors"};
-    for (int t = 0; t < 3; ++t) {
-        pose_tables_on_device[t] = false;
-        if (!tables[t]) continue;
-        cudaPointerAttributes attr{};
-        if (cudaPointerGetAttributes(&attr, tables[t]) != cudaSuccess) {
-            cudaGetLastError();  // (not memory CUDA knows: host memory)
-            continue;
-        }
-        if (attr.type != cudaMemoryTypeDevice) continue;
-        if (attr.device != device) {
-            set_error("pose table %s is in the memory of device %d; the renderer renders on device %d", names[t], attr.device, device);
-            return FORMA_STATUS_INVALID;
-        }
-        if (t != 1 && ((uintptr_t)tables[t] & 3u) != 0u) {
-            set_error("pose table %s in device memory must be 4-byte aligned", names[t]);
-            return FORMA_STATUS_INVALID;
-        }
-        pose_tables_on_device[t] = true;
-    }
+    static const bool aligned[3] = {true, false, true};
+    const int st = locate_tables(tables, names, aligned, "pose", device, pose_tables_on_device);
+    if (st) return st;
     for (uint64_t r = 0; P->transforms && !pose_tables_on_device[0] && r < recs; ++r) {  // [ux, vx, uy, vy, tx, ty]
         const float* t = P->transforms + 6u * r;
         if (!geom_pres_ok(t[0], t[2], t[1], t[3])) {
@@ -790,6 +812,224 @@ int Renderer::upload_pose_fills(const FrameRequest& q, PaintScene& S, PoseFillAr
     return FORMA_STATUS_OK;
 }
 
+// The tables of an instance request (see forma_renderer_render_instances_device): M >= 1 slots, n M
+// within the layer field, every prototype an attached order, and every transform of a slot with a
+// prototype one forma_layer_set_transform accepts. Colours are any floats.
+// Where each table lives (inst_tables_on_device): as for poses (locate_tables). The prototypes decide the
+// launch sizes, so a device table is read back into h_inst_protos here (host tables are copied
+// there); host transforms are checked here, device transforms by the fold (upload_instances).
+int Renderer::check_instances(const FrameRequest& q) {
+    const forma_instances* I = q.instances;
+    if (!I || !I->prototypes || I->n_instances == 0u) {
+        set_error("%s", !I ? "no instances" : !I->prototypes ? "no prototypes table" : "instances: M = 0 slots per frame");
+        return FORMA_STATUS_INVALID;
+    }
+    const uint32_t M = I->n_instances;
+    const uint64_t recs = (uint64_t)q.n * M;
+    if (recs > (1ull << 21)) {
+        set_error("%u frames of %u instance slots need %llu layer orders; the layer field holds %u", q.n, M, (unsigned long long)recs,
+                  1u << 21);
+        return FORMA_STATUS_ORDER;
+    }
+    const void* const tables[3] = {I->prototypes, I->transforms, I->colors};
+    static const char* const names[3] = {"prototypes", "transforms", "colors"};
+    static const bool aligned[3] = {true, true, true};
+    const int lt = locate_tables(tables, names, aligned, "instance", device, inst_tables_on_device);
+    if (lt) return lt;
+    FORMA_CUDA_TRY(cudaSetDevice(device));
+    if (h_inst_protos.reserve(recs) != cudaSuccess) {
+        cudaGetLastError();
+        set_error("%llu instance slots could not be staged", (unsigned long long)recs);
+        return FORMA_STATUS_CAPACITY;
+    }
+    if (inst_tables_on_device[0]) {  // read in stream order, as the caller wrote it
+        FORMA_CUDA_TRY(cudaMemcpyAsync(h_inst_protos.ptr, I->prototypes, recs * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+        d2h_bytes += recs * sizeof(uint32_t);
+        FORMA_CUDA_TRY(cudaStreamSynchronize(stream));
+    } else {  // (the previous call's copies are complete: it ended with a synchronisation)
+        std::memcpy(h_inst_protos.ptr, I->prototypes, recs * sizeof(uint32_t));
+    }
+    inst_layers.clear();
+    inst_index.clear();
+    const auto& layers = q.comp->layers;
+    for (uint64_t r = 0; r < recs; ++r) {
+        const uint32_t p = h_inst_protos.ptr[r];
+        if (p == FORMA_NO_INSTANCE || inst_index.count(p)) continue;
+        const auto it = layers.find(p);
+        if (it == layers.end()) {
+            set_error("instance of frame %llu, slot %llu: no layer is attached at order %u", (unsigned long long)(r / M),
+                      (unsigned long long)(r % M), p);
+            return FORMA_STATUS_INVALID;
+        }
+        inst_index.emplace(p, (uint32_t)inst_layers.size());
+        inst_layers.push_back(it->second);
+    }
+    for (uint64_t r = 0; I->transforms && !inst_tables_on_device[1] && r < recs; ++r) {  // [ux, vx, uy, vy, tx, ty]
+        const float* t = I->transforms + 6u * r;
+        if (h_inst_protos.ptr[r] != FORMA_NO_INSTANCE && !geom_pres_ok(t[0], t[2], t[1], t[3])) {
+            set_error("instance of frame %llu, slot %llu: GeomPresTransformError::ExceededScalingFactor", (unsigned long long)(r / M),
+                      (unsigned long long)(r % M));
+            return FORMA_STATUS_INVALID;
+        }
+    }
+    return FORMA_STATUS_OK;
+}
+
+// The records and tables of an instance request, queued on the stream (see InstanceArgs):
+// - the line records: per frame b, slot m with a prototype p and live insert of p (one whose
+//   geometry id is the layer's current one), in that order, the insert's point pairs. The whole
+//   composition is resident (no band filter), so an insert's points are at its `dst`;
+// - the frame records (BatchFrame::order_base = b M, read by the tables and the tile kernels), the
+//   frames' first CTAs and first line records, in one upload with the line records;
+// - the instance records: instance_fold_kernel folds the transforms into the prototypes' own
+//   records (32 bytes per order up to the largest prototype);
+// - the order -> style table of the n M orders, and with colours the instance style table
+//   (instance_styles_kernel); S then reads them.
+// With device transforms the fold's first refused record is read back before line setup.
+int Renderer::upload_instances(const FrameRequest& q, PaintScene& S, InstanceLines& lines) {
+    const forma_instances& I = *q.instances;
+    const Composition& comp = *q.comp;
+    const CompDevice& cd = *comp.devices.at(res_key);
+    const uint32_t M = I.n_instances, n = q.n, n_recs = n * M, rows = ((uint32_t)q.height + 15u) / 16u;
+    const uint32_t* protos = h_inst_protos.ptr;
+    // The live inserts of every distinct prototype, in insertion order: (first point, point pairs).
+    std::unordered_map<uint32_t, uint32_t> by_geom;  // the prototype's current geometry id -> its index
+    by_geom.reserve(inst_layers.size());
+    uint32_t max_order = 0;
+    for (uint32_t k = 0; k < inst_layers.size(); ++k) {
+        by_geom.emplace(inst_layers[k]->dense_id, k);
+        max_order = std::max(max_order, (uint32_t)inst_layers[k]->order);
+    }
+    std::vector<std::vector<std::pair<uint32_t, uint32_t>>> inserts(inst_layers.size());
+    for (const PendingInsert& job : comp.jobs) {
+        if (job.count < 2u) continue;  // (no point pair)
+        const auto it = by_geom.find(job.geom_id);
+        if (it != by_geom.end()) inserts[it->second].emplace_back(job.dst, job.count - 1u);
+    }
+    uint64_t n_lines = 0;
+    for (uint32_t r = 0; r < n_recs; ++r)
+        if (protos[r] != FORMA_NO_INSTANCE) n_lines += inserts[inst_index.at(protos[r])].size();
+    const size_t frames_bytes = (size_t)n * sizeof(BatchFrame), firsts_bytes = 2u * (n + 1u) * sizeof(uint32_t);
+    const size_t lines_off = (frames_bytes + firsts_bytes + 15u) / 16u * 16u, bytes = lines_off + n_lines * sizeof(InstanceLine);
+    const bool host_protos = !inst_tables_on_device[0], host_xf = I.transforms && !inst_tables_on_device[1];
+    const bool colors = I.colors != nullptr;
+    const uint64_t n_styles = comp.n_style_recs;
+    if (n_lines >= (1ull << 32) || h_inst_lines.reserve(bytes) != cudaSuccess || d_inst_lines.reserve(bytes) != cudaSuccess ||
+        h_inst_base.reserve(max_order + 1u) != cudaSuccess || d_inst_base.reserve(max_order + 1u) != cudaSuccess ||
+        d_inst_recs.reserve(n_recs) != cudaSuccess || inst_order_to_style.reserve(n_recs) != cudaSuccess ||
+        h_pose_first_bad.reserve(1) != cudaSuccess || d_pose_first_bad.reserve(1) != cudaSuccess ||
+        (host_protos && d_inst_protos.reserve(n_recs) != cudaSuccess) ||
+        (host_xf && (h_inst_xf.reserve(6u * n_recs) != cudaSuccess || d_inst_xf.reserve(6u * n_recs) != cudaSuccess)) ||
+        (colors && (d_inst_colors.reserve(n_recs) != cudaSuccess || inst_styles.reserve(n_styles + n_recs) != cudaSuccess ||
+                    (!inst_tables_on_device[2] && h_inst_colors.reserve(n_recs) != cudaSuccess)))) {
+        cudaGetLastError();  // (a failed allocation is not sticky: clear it for the launches' checks)
+        set_error("the records of %u instances (%llu line records) could not be allocated", n_recs, (unsigned long long)n_lines);
+        return FORMA_STATUS_CAPACITY;
+    }
+    BatchFrame* frames = reinterpret_cast<BatchFrame*>(h_inst_lines.ptr);
+    uint32_t* cta_first = reinterpret_cast<uint32_t*>(h_inst_lines.ptr + frames_bytes);
+    uint32_t* frame_first = cta_first + n + 1u;
+    InstanceLine* recs = reinterpret_cast<InstanceLine*>(h_inst_lines.ptr + lines_off);
+    uint64_t ctas = 0, pairs_all = 0;
+    uint32_t li = 0;
+    for (uint32_t b = 0; b < n; ++b) {
+        frames[b] = BatchFrame{};
+        frames[b].order_base = b * M;
+        cta_first[b] = (uint32_t)std::min<uint64_t>(ctas, 0xFFFFFFFFu);
+        frame_first[b] = li;
+        uint64_t pairs = 0;
+        for (uint32_t m = 0; m < M; ++m) {
+            const uint32_t p = protos[b * M + m];
+            if (p == FORMA_NO_INSTANCE) continue;
+            for (const auto& ins : inserts[inst_index.at(p)]) {
+                recs[li++] = InstanceLine{(uint32_t)std::min<uint64_t>(pairs, 0xFFFFFFFFu), ins.second, ins.first, b * M + m};
+                pairs += ins.second;
+            }
+        }
+        if (pairs >= (1ull << 31)) {
+            set_error("frame %u of the instances has %llu point pairs; a frame holds fewer than 2^31", b, (unsigned long long)pairs);
+            return FORMA_STATUS_CAPACITY;
+        }
+        ctas += raster_num_blocks((uint32_t)pairs);  // (whole CTAs per frame: a CTA belongs to one frame)
+        pairs_all += pairs;
+    }
+    if (ctas >= (1ull << 31)) {  // the launch's largest grid
+        set_error("the instances' %llu line-setup CTAs exceed the largest grid", (unsigned long long)ctas);
+        return FORMA_STATUS_CAPACITY;
+    }
+    cta_first[n] = (uint32_t)ctas;
+    frame_first[n] = li;
+    FORMA_CUDA_TRY(cudaMemcpyAsync(d_inst_lines.ptr, h_inst_lines.ptr, bytes, cudaMemcpyHostToDevice, stream));
+    h2d_bytes += bytes;
+    // The prototypes' own transforms, by order.
+    std::memset(h_inst_base.ptr, 0, (max_order + 1u) * sizeof(PoseRec));
+    for (const Layer* l : inst_layers)
+        h_inst_base.ptr[l->order] = PoseRec{l->xf[0], l->xf[1], l->xf[2], l->xf[3], l->xf[4], l->xf[5], l->has_xf ? 1u : 0u, 0u};
+    FORMA_CUDA_TRY(cudaMemcpyAsync(d_inst_base.ptr, h_inst_base.ptr, (max_order + 1u) * sizeof(PoseRec), cudaMemcpyHostToDevice, stream));
+    h2d_bytes += (max_order + 1u) * sizeof(PoseRec);
+    const uint32_t* d_protos = I.prototypes;
+    if (host_protos) {
+        FORMA_CUDA_TRY(cudaMemcpyAsync(d_inst_protos.ptr, protos, (size_t)n_recs * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+        h2d_bytes += (size_t)n_recs * sizeof(uint32_t);
+        d_protos = d_inst_protos.ptr;
+    }
+    InstanceFoldArgs F{d_protos, d_inst_base.ptr, I.transforms, nullptr};
+    if (host_xf) {
+        std::memcpy(h_inst_xf.ptr, I.transforms, 6u * (size_t)n_recs * sizeof(float));
+        FORMA_CUDA_TRY(cudaMemcpyAsync(d_inst_xf.ptr, h_inst_xf.ptr, 6u * (size_t)n_recs * sizeof(float), cudaMemcpyHostToDevice, stream));
+        h2d_bytes += 6u * (size_t)n_recs * sizeof(float);
+        F.transforms = d_inst_xf.ptr;
+    } else if (I.transforms) {
+        FORMA_CUDA_TRY(cudaMemsetAsync(d_pose_first_bad.ptr, 0xFF, sizeof(uint32_t), stream));
+        F.first_bad = d_pose_first_bad.ptr;
+    }
+    launch_instance_fold(F, d_inst_recs.ptr, n_recs, stream);
+    ++launches;
+    // The tables: with colours, the composition's style records, then one per slot.
+    if (colors) {
+        if (inst_tables_on_device[2]) {  // copied in stream order, as the caller wrote them (and 16-byte aligned)
+            FORMA_CUDA_TRY(cudaMemcpyAsync(d_inst_colors.ptr, I.colors, (size_t)n_recs * sizeof(float4), cudaMemcpyDeviceToDevice, stream));
+        } else {
+            std::memcpy(h_inst_colors.ptr, I.colors, (size_t)n_recs * sizeof(float4));
+            FORMA_CUDA_TRY(cudaMemcpyAsync(d_inst_colors.ptr, h_inst_colors.ptr, (size_t)n_recs * sizeof(float4), cudaMemcpyHostToDevice,
+                                           stream));
+            h2d_bytes += (size_t)n_recs * sizeof(float4);
+        }
+        if (n_styles)
+            FORMA_CUDA_TRY(cudaMemcpyAsync(inst_styles.ptr, cd.d_styles.ptr, n_styles * sizeof(StyleRec), cudaMemcpyDeviceToDevice, stream));
+    }
+    StyleRec* styles = colors ? inst_styles.ptr : cd.d_styles.ptr;
+    launch_instance_styles(cd.d_order_to_style.ptr, comp.n_orders, d_protos, styles, (uint32_t)n_styles, colors ? d_inst_colors.ptr : nullptr,
+                           n_recs, inst_order_to_style.ptr, stream);
+    ++launches;
+    FORMA_CUDA_TRY(cudaGetLastError());
+    S.styles = styles;
+    S.order_to_style = inst_order_to_style.ptr;
+    S.n_orders = n_recs;
+    const uint8_t* d = d_inst_lines.ptr;
+    const uint32_t* d_cta_first = reinterpret_cast<const uint32_t*>(d + frames_bytes);
+    lines.args = InstanceArgs{reinterpret_cast<const InstanceLine*>(d + lines_off), d_cta_first + n + 1u, d_cta_first, d_inst_recs.ptr, n, M,
+                              rows};
+    lines.frames = BatchArgs{reinterpret_cast<const BatchFrame*>(d), d_cta_first, n, rows, (float)S.width, (float)q.height};
+    lines.n_ctas = (uint32_t)ctas;
+    // Records in (frame, slot, insert) order: a painted tile holds one frame's segments in layer order.
+    lines.layer_bound = options().sort_full_key == 0 ? 0u : n_recs - 1u;
+    lines.n_lines = pairs_all;
+    if (F.first_bad) {
+        FORMA_CUDA_TRY(cudaMemcpyAsync(h_pose_first_bad.ptr, d_pose_first_bad.ptr, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+        d2h_bytes += sizeof(uint32_t);
+        FORMA_CUDA_TRY(ensure_count_event());
+        FORMA_CUDA_TRY(cudaEventRecord(count_ev, stream));
+        FORMA_CUDA_TRY(cudaEventSynchronize(count_ev));
+        const uint32_t r = *h_pose_first_bad.ptr;
+        if (r != 0xFFFFFFFFu) {
+            set_error("instance of frame %u, slot %u: GeomPresTransformError::ExceededScalingFactor", r / M, r % M);
+            return FORMA_STATUS_INVALID;
+        }
+    }
+    return FORMA_STATUS_OK;
+}
+
 // The checks of a request, before anything is written: each target (LinearLayout::new asserts,
 // layout/mod.rs:188-193, consts.rs limits, and for a stack the frame count and frame stride), the
 // ID target's own, then the views or the compositions of a batch. An ID-only request has no RGBA
@@ -876,6 +1116,7 @@ int Renderer::check_request(const FrameRequest& q) {
         }
     }
     if (q.kind == FrameKind::poses) return check_poses(q);
+    if (q.kind == FrameKind::instances) return check_instances(q);
     if (q.kind != FrameKind::batch) return FORMA_STATUS_OK;
     // The distinct compositions in order of first appearance, and the slices of the layer field
     // they need: n_orders each, as rebuild_tables counts them.
@@ -1094,7 +1335,9 @@ int Renderer::paint_step(const FrameRequest& q, const PaintScene& S, const Frame
         if (q.ids.ptr) ++*paint_launches;
     }
     FORMA_CUDA_TRY(id_flags.reserve(std::max<size_t>(recs.capacity, 1)));
-    const BatchFrame* frames = q.kind == FrameKind::batch ? reinterpret_cast<const BatchFrame*>(d_batch_lines.ptr) : nullptr;
+    const BatchFrame* frames = q.kind == FrameKind::batch       ? reinterpret_cast<const BatchFrame*>(d_batch_lines.ptr)
+                               : q.kind == FrameKind::instances ? reinterpret_cast<const BatchFrame*>(d_inst_lines.ptr)
+                                                                : nullptr;
     if (q.masks.ptr) {  // the zero fill of the planes, then the masks (the redo of a sync-free frame repeats both)
         const MaskFrame m{p.masks.ptr, p.masks.stride, p.mask_plane_stride, q.masks.first_order, q.masks.n_orders, q.masks.format,
                           (uint32_t)q.height, q.kind == FrameKind::single ? 1u : q.n};
@@ -1113,7 +1356,8 @@ int Renderer::paint_step(const FrameRequest& q, const PaintScene& S, const Frame
         FORMA_CUDA_TRY(cudaGetLastError());
         return FORMA_STATUS_OK;
     }
-    // A batch's entries carry each frame's order base (bind_batch): the kernel takes it off.
+    // A batch's or an instance stack's entries carry each frame's order base (bind_batch,
+    // upload_instances): the kernel takes it off.
     launch_paint_ids(S, t, id_flags.ptr, reinterpret_cast<uint32_t*>(p.ids.ptr), p.ids.stride, q.ids.min_coverage, totals.ptr + 8, stream,
                      p.rows, frames);
     ++launches;

@@ -80,8 +80,11 @@ struct StatsTarget {
 // comps[c]'s own orders. poses: n frames of one composition stacked as views are, frame b giving
 // each layer of a window of orders its own transform and enabled state (PoseArgs); line setup
 // reads frame b's pose records in place of a view transform, and from there on a pose stack is a
-// views stack. A stack takes no layer cache and no band filter: every composition is resident whole.
-enum class FrameKind { single, views, batch, poses };
+// views stack. instances: n frames of one composition stacked as views are, frame b drawing its M
+// slots' prototype layers as the layers b M + m (Renderer::upload_instances); from line setup on an
+// instance stack is a batch of n compositions of M orders each, whose tables are built per call.
+// A stack takes no layer cache and no band filter: every composition is resident whole.
+enum class FrameKind { single, views, batch, poses, instances };
 
 // One call of Renderer::render: what is rendered, the size of one frame, and its targets: an
 // RGBA target, an ID target (channels {0, 1, 2, 3}, clear colour 0 when it is alone) or both, or
@@ -102,8 +105,11 @@ struct FrameRequest {
     const float* views = nullptr;         // views: n transforms [ux, vx, uy, vy, tx, ty]
     Composition* const* batch = nullptr;  // batch: n compositions (null entries are refused)
     const forma_poses* poses = nullptr;   // poses: the window and its tables (null is refused)
-    // Views and poses: a stack of frames of one composition (q.comp).
-    bool one_comp_stack() const { return kind == FrameKind::views || kind == FrameKind::poses; }
+    const forma_instances* instances = nullptr;  // instances: the slots and their tables (null is refused)
+    // Views, poses and instances: a stack of frames of one composition (q.comp).
+    bool one_comp_stack() const {
+        return kind == FrameKind::views || kind == FrameKind::poses || kind == FrameKind::instances;
+    }
     // Poses with colours: the painter tables are built over a pose style table (PoseFillArgs).
     bool pose_fills() const { return kind == FrameKind::poses && poses && poses->colors; }
 };
@@ -123,6 +129,15 @@ struct FramePlan {
     DeviceFrame masks;  // the caller's planes on the device, or (host masks) the renderer's scratch ...
     uint64_t mask_plane_stride;  // ... with this plane stride
     forma_layer_stats* stats;    // the caller's records on the device, or (host statistics) the renderer's scratch
+};
+
+// The line setup of an instance call (see Renderer::upload_instances).
+struct InstanceLines {
+    InstanceArgs args;
+    BatchArgs frames;      // only frames (order_base = b M) and rows: the tables' and tile kernels' view of the stack
+    uint32_t n_ctas;
+    uint64_t layer_bound;  // the sort plan's bound of the layer field
+    uint64_t n_lines;      // point pairs of all frames (forma_timings)
 };
 
 // The line setup of a batch (see Renderer::bind_batch).
@@ -331,9 +346,10 @@ class Renderer {
     // views / n_views: the line setup of a views request (a stacked frame of n_views views); batch:
     // that of a batch request (comp is then null).
     // poses: that of a poses request (n_views frames).
+    // inst: that of an instance request.
     int rasterize(Composition* comp, uint32_t width, uint32_t height, float band_lo, float band_hi, uint32_t* n_out,
                   const ViewArgs* views = nullptr, uint32_t n_views = 0, const BatchLines* batch = nullptr,
-                  const PoseArgs* poses = nullptr);
+                  const PoseArgs* poses = nullptr, const InstanceLines* inst = nullptr);
     // Every frame, whatever its kind and targets: check_request, the PaintScene (begin_frame), each
     // target's device frame, run_frame and, for a layer cache, its bookkeeping.
     int render(const FrameRequest& q);
@@ -341,6 +357,7 @@ class Renderer {
     int check_masks(const FrameRequest& q);
     int check_stats(const FrameRequest& q);
     int check_poses(const FrameRequest& q);
+    int check_instances(const FrameRequest& q);
     // One frame of S: uploads, line setup, sort, then the painter tables, paint_step and
     // output_step once or, when the sync-free bounds were too small, twice.
     int run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p);
@@ -376,6 +393,30 @@ class Renderer {
     // Queues the upload of a poses request's colours and the build of its pose style table, and
     // points S at the table; `fills` receives the merge's arguments.
     int upload_pose_fills(const FrameRequest& q, PaintScene& S, PoseFillArgs& fills);
+    // Instances: where the current request's prototypes, transforms and colors tables are
+    // (check_instances: true = device memory of this device), the host's copy of the prototypes
+    // (a device table's is read back there), the line records with the frame records ahead of them,
+    // the prototypes' own transforms by order, the device copies of host tables, the n M instance
+    // records and the fold's first failing record, and the call's order -> style table.
+    bool inst_tables_on_device[3] = {false, false, false};
+    std::vector<const Layer*> inst_layers;               // the distinct prototypes, in order of first appearance
+    std::unordered_map<uint32_t, uint32_t> inst_index;   // prototype order -> its index in inst_layers
+    PinnedBuffer<uint32_t> h_inst_protos;
+    DeviceBuffer<uint32_t> d_inst_protos;
+    PinnedBuffer<uint8_t> h_inst_lines;  // BatchFrame per frame, cta_first, frame_first, then the InstanceLines
+    DeviceBuffer<uint8_t> d_inst_lines;
+    PinnedBuffer<PoseRec> h_inst_base;
+    DeviceBuffer<PoseRec> d_inst_base;
+    PinnedBuffer<float> h_inst_xf;
+    DeviceBuffer<float> d_inst_xf;
+    DeviceBuffer<PoseRec> d_inst_recs;
+    PinnedBuffer<float4> h_inst_colors;
+    DeviceBuffer<float4> d_inst_colors;
+    DeviceBuffer<StyleRec> inst_styles;
+    DeviceBuffer<int32_t> inst_order_to_style;
+    // Queues the records and tables of an instance request and points S at its tables; with
+    // device transforms, reads back whether the fold refused one.
+    int upload_instances(const FrameRequest& q, PaintScene& S, InstanceLines& lines);
     // A batch's distinct compositions' tables are gathered into the batch tables below, which are
     // kept until a batch of other compositions or other table versions comes (batch_key).
     std::vector<std::pair<uint64_t, uint64_t>> batch_key;  // (Composition::serial, tables_version) of the distinct compositions

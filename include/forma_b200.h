@@ -716,6 +716,81 @@ int forma_renderer_render_poses_over_device(forma_renderer*, forma_composition*,
                                             uint64_t view_stride, const uint32_t channels[4], uint32_t format,
                                             forma_timings* timings /* nullable */);
 
+/* Instance scenes (no reference counterpart): n frames, each drawing its own list of copies of the
+ * composition's layers, from one pass through the stages. The composition serves as a library of
+ * geometry and props: frame b has M = n_instances slots, and slot m draws the layer attached at
+ * order p = prototypes[b M + m] (FORMA_NO_INSTANCE: nothing). Frame b is exactly the bytes
+ * forma_renderer_render_device writes (no crop, no cache) for a composition T_b that has, for every
+ * slot m with a prototype p, a layer at order m with
+ *   - the geometry of the layer at order p: every live insert of it (not those a Layer::clear
+ *     dropped), in insertion order, with their path transforms;
+ *   - p's props; with colors, a Draw layer's fill replaced by Solid(colors[b M + m]) (its fill rule,
+ *     is_clipped, blend mode and a Clip layer's range stay; a Clip layer's colour is not read);
+ *   - the transform transforms[b M + m] when that table is given (an identity is no transform), p's
+ *     own transform otherwise;
+ *   - enabled, whatever p's own enabled state is (a library is usually kept disabled, so that its
+ *     ordinary frames show nothing).
+ * Empty slots have no layer. A prototype may fill any number of slots of any frame, in any order.
+ * (Frames whose lines all lie more than 2^19 px left of the frame are the exception of views and
+ * batches again: the stacked call is right, forma_renderer_render_device is not.)
+ * IDs, mask planes and statistics records are indexed by the slot m (T_b's orders): the ID frame
+ * is an instance-segmentation label and the statistics are per-instance boxes and areas.
+ * The call does not change the composition: no layer state, unchanged bit, table or geometry.
+ * The geometry is flattened and made resident once; per call the host builds one 16-byte line
+ * record per (frame, slot, live insert) and one 64-byte frame record per frame, which cross PCIe
+ * with the host tables' bytes (4 n M prototypes, 24 n M transforms, 16 n M colours) and 32 bytes
+ * per order up to the largest prototype (the prototypes' own transforms).
+ * Where the tables live: each table may be in host memory or in device memory of the renderer's
+ * device, under the rules of forma_poses (cudaPointerGetAttributes; another device's memory is
+ * refused; device float tables 4-byte aligned; read on the renderer's stream). A device
+ * `prototypes` table is copied to the host (4 n M bytes and one wait) because it decides the launch
+ * sizes; device transforms are checked on the device, at the cost of a 4-byte read-back and a wait.
+ * Each call is the twin of a views call, with `const forma_instances* instances, uint32_t n` in
+ * place of `const float* views, uint32_t n`: the same arguments, layouts, rules, limits, refusals
+ * and state afterwards (counters, segments, stage times and row costs of the stacked frame, no line
+ * records):
+ *   render_instances_device        forma_renderer_render_views_device
+ *   render_instances_ids_device    forma_renderer_render_views_ids_device (RGBA optional, as there)
+ *   render_instances_masks_device  forma_renderer_render_views_masks_device (window in slots m)
+ *   render_instances_stats_device  forma_renderer_render_views_stats_device (window in slots m)
+ * Besides the twin's refusals, FORMA_ERR_INVALID_ARGUMENT is returned before anything is written,
+ * with the composition untouched, for: a null descriptor or null prototypes; M = 0; a prototype
+ * order without an attached layer (forma_last_error() names the frame, the slot and the order); a
+ * slot's transform that forma_layer_set_transform refuses (the frame and the slot are named; the
+ * transforms of empty slots are not checked);
+ * device float tables that are not 4-byte aligned. FORMA_ERR_ORDER_LIMIT: n M > 2^21 (frame b's
+ * instances take the orders b M ... b M + M - 1 of the layer field). FORMA_ERR_CAPACITY: the
+ * 2^30-segment limit of the twin, a frame of 2^31 or more point pairs, or instance records or
+ * the instance style table (112 (S + n M) bytes with colors, S the composition's style records)
+ * that cannot be allocated. Transforms need not be finite: a NaN or infinite translation renders
+ * as forma_renderer_render_device renders it. */
+#define FORMA_NO_INSTANCE 0xFFFFFFFFu
+typedef struct forma_instances {
+    uint32_t n_instances;        /* M >= 1 instance slots per frame                                   */
+    const uint32_t* prototypes;  /* n x M layer orders at b M + m; FORMA_NO_INSTANCE = empty slot      */
+    const float* transforms;     /* nullable: n x M x 6 floats at 6 (b M + m), set_transform order     */
+    const float* colors;         /* nullable: n x M x 4 floats at 4 (b M + m), linear RGBA solid fill */
+} forma_instances;
+int forma_renderer_render_instances_device(forma_renderer*, forma_composition*, const forma_instances* instances, uint32_t n,
+                                           uint8_t* device_buffer, uint64_t width, uint64_t width_stride, uint64_t height,
+                                           uint64_t view_stride, const uint32_t channels[4], const float clear_color[4],
+                                           forma_timings* timings /* nullable */);
+int forma_renderer_render_instances_ids_device(forma_renderer*, forma_composition*, const forma_instances* instances, uint32_t n,
+                                               uint8_t* device_buffer /* nullable */, uint64_t width, uint64_t width_stride,
+                                               uint64_t height, uint64_t view_stride, const uint32_t channels[4],
+                                               const float clear_color[4], uint32_t* device_ids, uint64_t ids_stride,
+                                               uint64_t ids_view_stride, float min_coverage, forma_timings* timings /* nullable */);
+int forma_renderer_render_instances_masks_device(forma_renderer*, forma_composition*, const forma_instances* instances, uint32_t n,
+                                                 const forma_masks* masks, uint64_t width, uint64_t height,
+                                                 uint8_t* device_buffer /* nullable */, uint64_t width_stride, uint64_t view_stride,
+                                                 const uint32_t channels[4], const float clear_color[4],
+                                                 forma_timings* timings /* nullable */);
+int forma_renderer_render_instances_stats_device(forma_renderer*, forma_composition*, const forma_instances* instances, uint32_t n,
+                                                 const forma_stats* stats, uint64_t width, uint64_t height,
+                                                 uint8_t* device_buffer /* nullable */, uint64_t width_stride, uint64_t view_stride,
+                                                 const uint32_t channels[4], const float clear_color[4],
+                                                 forma_timings* timings /* nullable */);
+
 /* Launch on `cuda_stream` (a cudaStream_t, e.g. torch.cuda.current_stream().cuda_stream)
  * instead of the default stream. */
 void forma_renderer_set_stream(forma_renderer*, void* cuda_stream);
