@@ -546,6 +546,7 @@ SIGNATURES = {
     "renderer_sort_pairs": (C.c_int, [_vp, C.c_int, C.c_int, _u64p, _u32p, C.c_uint64, C.c_uint64]),
     "renderer_sort_bounds": (None, [_vp, _u64p]),
     "renderer_sort_counts": (C.c_uint64, [_vp, C.c_int, _u32p, _u32p, C.c_uint64]),
+    "renderer_sort_mode": (C.c_uint32, [_vp]),
     "debug_selftest": (C.c_int, [C.c_int, _u64p]),
     "renderer_multi_new": (_vp, [C.POINTER(C.c_int), C.c_int]),
     "renderer_multi_free": (None, [_vp]),
@@ -573,7 +574,7 @@ STACK_ID_SYMBOLS = ("renderer_render_views_ids", "renderer_render_views_ids_devi
 
 
 # The same for the inspection entry points of the sort (sort_plan, Renderer.sort_pairs, sort_bounds).
-SORT_DEBUG_SYMBOLS = ("debug_sort_plan", "renderer_sort_pairs", "renderer_sort_bounds", "renderer_sort_counts")
+SORT_DEBUG_SYMBOLS = ("debug_sort_plan", "renderer_sort_pairs", "renderer_sort_bounds", "renderer_sort_counts", "renderer_sort_mode")
 # The same for linear float frames (Renderer.render_linear, render_views_linear, render_batch_linear).
 LINEAR_SYMBOLS = ("renderer_render_linear", "renderer_render_linear_device", "renderer_render_views_linear",
                   "renderer_render_views_linear_device", "renderer_render_batch_linear", "renderer_render_batch_linear_device")
@@ -1834,6 +1835,11 @@ class Renderer:
         return dict(zip(("layer", "tile_x", "tile_y", "total_bits"), [int(x) for x in out]))
 
     SORT_COUNT_SOURCES = ("none", "speculative_emit", "emit", "upsweep")
+
+    def sort_mode(self) -> int:
+        """How the last frame's sort learnt the segment count (forma_renderer_sort_mode): 0 read
+        back, 1 checked on the device (option sync_free_sort), 2 attempted as 1 and redone as 0."""
+        return int(self._api.renderer_sort_mode(self._h))
 
     def sort_counts(self, keep: int = -1) -> dict:
         """The last frame's segment-sort tile counts (forma_renderer_sort_counts): where pass 0's

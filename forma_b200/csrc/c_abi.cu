@@ -917,6 +917,7 @@ void forma_renderer_counters(const forma_renderer* r, uint64_t out[8]) {
     out[4] = r->r.last_cells;
     out[5] = r->r.last_entries;
 }
+uint32_t forma_renderer_sort_mode(const forma_renderer* r) { return r->r.last_sort_redone ? 2u : r->r.last_sort_sync_free ? 1u : 0u; }
 void forma_composition_evict(forma_composition* c) { c->c.evict(); }
 uint64_t forma_composition_point_count(forma_composition* c) { return c->c.n_points; }
 void forma_path_builder_extend(forma_path_builder* pb, const uint8_t* cmds, uint64_t n_cmds, const float* xy) {

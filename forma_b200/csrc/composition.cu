@@ -47,7 +47,8 @@ static const OptionName kOptionNames[] = {
     {"sync_free", &Options::sync_free, 0, 1},         {"test_fast_shrink", &Options::test_fast_shrink, 0, 1},
     {"host_slices", &Options::host_slices, 1, 16},    {"slice_bands", &Options::slice_bands, 1, 16},
     {"slice_min_points", &Options::slice_min_points, 0, 1 << 30}, {"slice_chain", &Options::slice_chain, 0, 1},
-    {"pdl", &Options::pdl, 0, 1},
+    {"pdl", &Options::pdl, 0, 1},                     {"sync_free_sort", &Options::sync_free_sort, 0, 1},
+    {"test_sort_bound", &Options::test_sort_bound, 0, 1 << 30},
 };
 Options& options() {
     static Options o = [] {

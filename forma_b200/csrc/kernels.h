@@ -35,6 +35,8 @@ struct Options {
     int slice_min_points = 65536;  //   ... only for compositions of at least this many points
     int slice_chain = 1;     //   ... uploads issued slice after slice, each waiting for the one before (0: all at once from the slices' threads)
     int pdl = 1;             // chained launches: the frame's kernels launched with programmatic dependent launch (0: plain launches)
+    int sync_free_sort = 1;  // single device frames: segment sort, tables and paint launched over the previous frame's segment count and sort plan, without the mid-frame count read-back (redone the slow way if they do not hold)
+    int test_sort_bound = 0; // test hook: the segment-count bound of such a frame (0 = the previous count + 25 % + 4096)
 };
 Options& options();
 
@@ -63,8 +65,20 @@ void launch_quad_expand_poly(const QuadUpPoly* in, QuadRec* out, uint32_t n, cud
 uint32_t raster_num_blocks(uint32_t n_points);
 // block_sums: raster_num_blocks(n) entries, turned into exclusive offsets; total[0] = #segments.
 // max_tile[0..1] = largest biased tile_x / tile_y any emitted segment can carry.
+// A frame launched before its segment count is known on the host (Renderer::rasterize with a
+// bound): the scan that produces the count also decides whether the frame's launches hold. They
+// hold when n_lo <= count <= n_hi, count < 2^30 and the bit lengths of max_tile[0..1] are tx_bits
+// and ty_bits (the sort plan they were made with is then the frame's own). Then *live_n = count
+// and *paint_counter = 0; otherwise *live_n = 0 (every kernel that reads it does nothing) and
+// *paint_counter = kPaintAbort (every paint ticket is past the frame's tiles: nothing is written).
+struct CountCheck {
+    uint32_t n_lo, n_hi, tx_bits, ty_bits;
+    uint32_t* live_n;
+    uint32_t* paint_counter;
+};
+constexpr uint32_t kPaintAbort = 0x80000000u;
 void launch_line_count(const RasterArgs& args, uint32_t* block_sums, uint32_t* total, uint32_t* max_tile,
-                       cudaStream_t stream);
+                       cudaStream_t stream, const CountCheck* check = nullptr);
 // Segments at positions >= cap are dropped (speculative launches, see Renderer::rasterize).
 // `counts` (optional): the digit of every stored segment is added to the counts of its 4096-key
 // sort tile (TileCounts); dropped segments are not counted.
@@ -294,7 +308,8 @@ SortResult launch_radix_sort(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals,
                                                                   not the last pass's [3p + 2]: pass p starts at the event recorded before it (the caller's before the sort, pass p - 1's
                                                                   end) and the last pass ends at the caller's after the sort. Fewer event records between the kernels */,
                              const uint32_t* n_dev = nullptr /* the key count in device memory; `n` is then its upper bound
-                                                                and a larger count sorts nothing (single-sweep passes only) */,
+                                                                and a larger count sorts nothing. With `counts` (reduce-then-scan
+                                                                passes) the counts of the tiles past it must be zero */,
                              const uint32_t* hist = nullptr /* [kMaxSortPasses][256] digit counts of every planned pass,
                                                                counted by the keys' producer: the sort then launches its
                                                                passes only, and `scratch` holds sort_lookback_bytes(n, plan)
@@ -354,25 +369,32 @@ TableScratch table_scratch_layout(uint32_t n, uint32_t n_cells, uint32_t n_gaps,
 void launch_zero_tables(uint8_t* a, size_t a_bytes, uint8_t* b, size_t b_bytes, uint32_t* word, cudaStream_t st);
 // dst[0, n) = src[0, n), n <= 256, by one chained kernel (not counted as a launch); dst may be the
 // device address of pinned host memory.
-void launch_copy_words(const uint32_t* src, uint32_t* dst, uint32_t n, cudaStream_t st);
 // Cells in one pass over the sorted segments (+ a small kernel for the cells that cross a
 // CTA tile): cell_start[c] = first segment of cell c (cell_start[#cells] = n), the cell's
 // cover (16 x i8 by local_y), its key, the (tile_y, layer, tile_x) key of the carry pass and
 // perm[c] = c, for every c < cap - 1; n_cells_out[0] = #cells. All five arrays need `cap`
 // entries. The digits of every written carry-pass key are added to `carry_hist` ([passes][256]
 // of `carry_plan`). `scratch`: the zeroed table scratch (cells_state). May be launched before the
-// host knows the count; the caller repeats it if #cells >= cap.
+// host knows the count; the caller repeats it if #cells >= cap. n_dev (optional): the segment count
+// in device memory, `n` then being its upper bound (the grid).
 void launch_cells(const PaintScene& S, const uint64_t* segs, uint32_t n, uint8_t* scratch, const TableScratch& L,
                   const SortPlan& carry_plan, uint32_t* cell_start, uint32_t cap, uint32_t* n_cells_out, uint64_t* cell_key,
-                  uint4* cell_cover, uint64_t* key2, uint32_t* perm, cudaStream_t st);
+                  uint4* cell_cover, uint64_t* key2, uint32_t* perm, cudaStream_t st, const uint32_t* n_dev = nullptr);
 // Cell / carry-only-entry counts that stay on the device (frames whose tables are built without a
 // host read-back, Options::sync_free): with `cells` set, the n_cells / n_gaps arguments of the
 // launchers below are upper bounds (grid sizes) and the kernels read the counts here; a count
 // above its bound makes them no-ops (the host then rebuilds the tables with known counts).
+// words / words_out / n_words (merge only): the merge kernel, the last kernel of the tables, also
+// copies n_words (<= 256) count words to the host's pinned words (words_out: their device
+// address), which the host reads after the frame's final synchronisation; no kernel of its own
+// behind the paint carries them.
 struct DevCounts {
     const uint32_t* cells = nullptr;
     const uint32_t* gaps = nullptr;
     uint32_t cell_bound = 0, gap_bound = 0;
+    const uint32_t* words = nullptr;
+    uint32_t* words_out = nullptr;
+    uint32_t n_words = 0;
 };
 // One pass over the carry-sorted cells: the carry-in of every cell (carry_in, by cell id) and the
 // carry-only entries in (layer, tile_y, tile_x) order: key, payload n_cells + entry id, carried
@@ -454,14 +476,14 @@ void launch_paint(const PaintScene& S, const TileTables& t, uint8_t* eflags, uin
 // painter's planes in channel order where launch_paint stores their sRGB bytes (see
 // forma_renderer_render_linear). `framebuffer` and S.stride: multiples of 4 bytes.
 void launch_paint_linear(const PaintScene& S, const TileTables& t, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter,
-                         cudaStream_t st, uint32_t view_rows, uint32_t bpp);
+                         cudaStream_t st, uint32_t view_rows, uint32_t bpp, bool counter_zeroed = false);
 // launch_paint over the pixels already in `framebuffer` (see forma_renderer_render_over_device):
 // each pixel's own value, decoded, is its clear colour; tiles without entries are not written.
 // bpp 4 (sRGB8, channels a permutation with A last), 8 (RGBA16F) or 16 (RGBA32F, both: any
 // permutation); S.channels are not upgraded (the kernels upgrade Alpha -> One per pixel).
 // `framebuffer` and S.stride: multiples of 4 bytes.
 void launch_paint_over(const PaintScene& S, const TileTables& t, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter,
-                       cudaStream_t st, uint32_t view_rows, uint32_t bpp);
+                       cudaStream_t st, uint32_t view_rows, uint32_t bpp, bool counter_zeroed = false);
 // The inverse of launch_repack_views: rows [0, height) of the n_views frames at src + b * view_stride
 // (row r at + r * stride) to the stacked frame at dst, frame b's first row at
 // dst + b * view_rows_px * dst_stride. `width` in 4-byte words; every pointer and stride a multiple of 4.
@@ -530,9 +552,9 @@ void launch_batch_tables(const BatchTableSrc* src, uint32_t n_src, uint32_t max_
 void launch_grad_setup(const StyleRec* styles, const StopRec* stops, uint32_t n_styles, GradRec* grads, cudaStream_t st);
 // Pixel-pair fp32 arithmetic of the painter against scalar IEEE operations; mismatches are added to out[0].
 void launch_f32x2_selftest(const float* a, const float* b, const float* c, uint32_t n, uint32_t* out, cudaStream_t st);
-// out[row] = 32 x entries + pixel segments of tile row `row` (see row_cost_kernel).
+// out[row] = 32 x entries + pixel segments of tile row `row` (see row_cost_kernel). n_dev: as for launch_cells.
 void launch_row_costs(const uint2* tile_range, uint32_t tiles_x, uint32_t tiles_y, const uint64_t* segs, uint32_t n,
-                      unsigned long long* out, cudaStream_t st, unsigned long long* seg_out = nullptr);
+                      unsigned long long* out, cudaStream_t st, unsigned long long* seg_out = nullptr, const uint32_t* n_dev = nullptr);
 // Packs the tiles in S.written_list into `packed` (256 u32 per tile, row-major).
 void launch_gather_tiles(const PaintScene& S, const uint8_t* framebuffer, uint32_t* packed, cudaStream_t st);
 

@@ -824,9 +824,9 @@ void launch_paint(const PaintScene& S, const TileTables& t, uint8_t* eflags, uin
 }
 
 void launch_paint_linear(const PaintScene& S, const TileTables& t, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter,
-                         cudaStream_t st, uint32_t view_rows, uint32_t bpp) {
+                         cudaStream_t st, uint32_t view_rows, uint32_t bpp, bool counter_zeroed) {
     const void* kernel = view_rows ? (const void*)paint_views_linear_kernel : (const void*)paint_linear_kernel;
-    const TileGrid g = tile_grid(S, kernel, kPaintWarpsPerBlock, tile_counter, st);
+    const TileGrid g = tile_grid(S, kernel, kPaintWarpsPerBlock, tile_counter, st, counter_zeroed);
     if (!g.n_tiles) return;
     const PaintInputs in = paint_inputs(S, t, eflags, framebuffer, tile_counter);
     if (view_rows) launch_chained(paint_views_linear_kernel, g.ctas, kPaintWarpsPerBlock * 32, 0, st, S, in, g.n_tiles, view_rows, bpp);
@@ -834,11 +834,11 @@ void launch_paint_linear(const PaintScene& S, const TileTables& t, uint8_t* efla
 }
 
 void launch_paint_over(const PaintScene& S, const TileTables& t, uint8_t* eflags, uint8_t* framebuffer, uint32_t* tile_counter,
-                       cudaStream_t st, uint32_t view_rows, uint32_t bpp) {
+                       cudaStream_t st, uint32_t view_rows, uint32_t bpp, bool counter_zeroed) {
     const bool linear = bpp != 4u;
     const void* kernel = view_rows ? (linear ? (const void*)paint_views_over_linear_kernel : (const void*)paint_views_over_kernel)
                                    : (linear ? (const void*)paint_over_linear_kernel : (const void*)paint_over_kernel);
-    const TileGrid g = tile_grid(S, kernel, kPaintWarpsPerBlock, tile_counter, st);
+    const TileGrid g = tile_grid(S, kernel, kPaintWarpsPerBlock, tile_counter, st, counter_zeroed);
     if (!g.n_tiles) return;
     const PaintInputs in = paint_inputs(S, t, eflags, framebuffer, tile_counter);
     const uint32_t block = kPaintWarpsPerBlock * 32;

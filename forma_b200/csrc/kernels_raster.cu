@@ -481,8 +481,12 @@ __global__ void __launch_bounds__(kRasterThreads) line_count_instances_kernel(Ra
 // of the producing kernel, a few thousand); writes the grand total to
 // total[0]. 1024 threads, each owning a contiguous chunk. Saturating: every
 // offset and the total are min(true value, 0xFFFFFFFF).
+// kCheck: the count of a frame launched over bounds (CountCheck), judged with the largest tile
+// coordinates max_tile[0..1] of the count pass this launch is chained behind.
+template <bool kCheck>
 __global__ void __launch_bounds__(1024) scan_block_sums_kernel(uint32_t* __restrict__ data, uint32_t n,
-                                                              uint32_t* __restrict__ total) {
+                                                              uint32_t* __restrict__ total, CountCheck check,
+                                                              const uint32_t* __restrict__ max_tile) {
     chain_begin();
     __shared__ uint32_t warp_tot[32];
     __shared__ uint32_t carry, round_total;
@@ -518,7 +522,19 @@ __global__ void __launch_bounds__(1024) scan_block_sums_kernel(uint32_t* __restr
         if (threadIdx.x == 0) carry = sat_add(carry, round_total);
         __syncthreads();
     }
-    if (threadIdx.x == 0) total[0] = carry;
+    if (threadIdx.x == 0) {
+        total[0] = carry;
+        if constexpr (kCheck) {
+            const uint32_t tx_bits = 32u - __clz(max_tile[0]), ty_bits = 32u - __clz(max_tile[1]);
+            const bool holds = carry >= check.n_lo && carry <= check.n_hi && carry < (1u << 30) && tx_bits == check.tx_bits &&
+                               ty_bits == check.ty_bits;
+            *check.live_n = holds ? carry : 0u;
+            *check.paint_counter = holds ? 0u : kPaintAbort;
+        }
+    }
+}
+static void launch_scan_block_sums(uint32_t* data, uint32_t n, uint32_t* total, cudaStream_t stream) {
+    launch_chained(scan_block_sums_kernel<false>, 1, 1024, 0, stream, data, n, total, CountCheck{}, (const uint32_t*)nullptr);
 }
 
 // ---------------------------------------------------------------------------
@@ -801,7 +817,7 @@ void launch_flatten_eval(const SplineRec* splines, const PointRec* points, const
 uint32_t raster_num_blocks(uint32_t n_points) { return n_points ? (n_points + kRasterThreads - 1) / kRasterThreads : 0; }
 
 void launch_line_count(const RasterArgs& args, uint32_t* block_sums, uint32_t* total, uint32_t* max_tile,
-                       cudaStream_t stream) {
+                       cudaStream_t stream, const CountCheck* check) {
     uint32_t nb = raster_num_blocks(args.n_points);
     cudaMemsetAsync(max_tile, 0, 2 * sizeof(uint32_t), stream);
     if (!nb) {
@@ -809,7 +825,8 @@ void launch_line_count(const RasterArgs& args, uint32_t* block_sums, uint32_t* t
         return;
     }
     line_count_kernel<<<nb, kRasterThreads, 0, stream>>>(args, block_sums, max_tile);
-    launch_chained(scan_block_sums_kernel, 1, 1024, 0, stream, block_sums, nb, total);
+    if (check) launch_chained(scan_block_sums_kernel<true>, 1, 1024, 0, stream, block_sums, nb, total, *check, (const uint32_t*)max_tile);
+    else launch_scan_block_sums(block_sums, nb, total, stream);
 }
 
 void launch_raster_emit(const RasterArgs& args, const uint32_t* block_offsets, uint64_t* out, uint32_t cap, cudaStream_t stream,
@@ -829,7 +846,7 @@ void launch_line_count_views(const RasterArgs& args, const ViewArgs& views, uint
         return;
     }
     line_count_views_kernel<<<dim3(nb, n_views), kRasterThreads, 0, stream>>>(args, views, block_sums, max_tile);
-    launch_chained(scan_block_sums_kernel, 1, 1024, 0, stream, block_sums, nb * n_views, total);
+    launch_scan_block_sums(block_sums, nb * n_views, total, stream);
 }
 
 void launch_raster_emit_views(const RasterArgs& args, const ViewArgs& views, uint32_t n_views, const uint32_t* block_offsets,
@@ -851,7 +868,7 @@ void launch_line_count_poses(const RasterArgs& args, const PoseArgs& poses, uint
         return;
     }
     line_count_poses_kernel<<<dim3(nb, n_frames), kRasterThreads, 0, stream>>>(args, poses, block_sums, max_tile);
-    launch_chained(scan_block_sums_kernel, 1, 1024, 0, stream, block_sums, nb * n_frames, total);
+    launch_scan_block_sums(block_sums, nb * n_frames, total, stream);
 }
 
 void launch_raster_emit_poses(const RasterArgs& args, const PoseArgs& poses, uint32_t n_frames, const uint32_t* block_offsets,
@@ -880,7 +897,7 @@ void launch_line_count_instances(const RasterArgs& args, const InstanceArgs& ins
         return;
     }
     line_count_instances_kernel<<<n_ctas, kRasterThreads, 0, stream>>>(args, inst, block_sums, max_tile);
-    launch_chained(scan_block_sums_kernel, 1, 1024, 0, stream, block_sums, n_ctas, total);
+    launch_scan_block_sums(block_sums, n_ctas, total, stream);
 }
 
 void launch_raster_emit_instances(const RasterArgs& args, const InstanceArgs& inst, uint32_t n_ctas, const uint32_t* block_offsets,
@@ -898,7 +915,7 @@ void launch_line_count_batch(const BatchArgs& batch, uint32_t n_ctas, uint32_t* 
         return;
     }
     line_count_batch_kernel<<<n_ctas, kRasterThreads, 0, stream>>>(batch, block_sums, max_tile);
-    launch_chained(scan_block_sums_kernel, 1, 1024, 0, stream, block_sums, n_ctas, total);
+    launch_scan_block_sums(block_sums, n_ctas, total, stream);
 }
 
 void launch_raster_emit_batch(const BatchArgs& batch, uint32_t n_ctas, const uint32_t* block_offsets, uint64_t* out, uint32_t cap,

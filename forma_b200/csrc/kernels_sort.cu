@@ -361,10 +361,13 @@ __global__ void __launch_bounds__(kSortThreads) radix_upsweep_kernel(const uint6
 // Tile counts from the keys' producers (TileCounts): CTA c sums the counts of tiles
 // [c * tiles_per_chunk, ...) into chunk row c (stores) and its super-chunk row (atomics, on rows the
 // previous downsweep over this block left zero). Thread d owns digit d.
+// n_dev (optional): the key count in device memory; `tiles` is then a bound, and the tiles past the
+// count (all zero) are not read.
 __global__ void __launch_bounds__(kRadix) radix_chunk_totals_kernel(const uint32_t* __restrict__ tile_hist,
                                                                   uint32_t* __restrict__ totals, uint32_t tiles,
-                                                                  uint32_t tiles_per_chunk) {
+                                                                  uint32_t tiles_per_chunk, const uint32_t* __restrict__ n_dev) {
     chain_begin();
+    if (n_dev) tiles = min(tiles, (*n_dev + kSortTileKeys - 1u) / kSortTileKeys);
     const uint32_t d = threadIdx.x, c = blockIdx.x;
     const uint32_t t0 = c * tiles_per_chunk, t1 = min(tiles, t0 + tiles_per_chunk);
     uint32_t sum = 0;
@@ -381,10 +384,12 @@ __global__ void __launch_bounds__(kRadix) radix_chunk_totals_kernel(const uint32
 
 // CTA c turns the digit counts of tiles [c * tiles_per_chunk, ...) into the
 // global offset of each tile's first key of each digit. Thread d owns digit d.
+// n_dev: as for radix_chunk_totals_kernel (the tiles past the count keep their zero counts).
 __global__ void __launch_bounds__(kRadix) radix_tile_scan_kernel(uint32_t* __restrict__ tile_hist,
                                                                const uint32_t* __restrict__ totals, uint32_t tiles,
-                                                               uint32_t tiles_per_chunk) {
+                                                               uint32_t tiles_per_chunk, const uint32_t* __restrict__ n_dev) {
     chain_begin();
+    if (n_dev) tiles = min(tiles, (*n_dev + kSortTileKeys - 1u) / kSortTileKeys);
     __shared__ uint32_t s_warp_tot[kRadix / 32];
     const uint32_t d = threadIdx.x, c = blockIdx.x, sc = c / kChunksPerSuper;
     uint32_t before = 0, total = 0;  // keys of digit d in earlier chunks / in all chunks
@@ -449,10 +454,13 @@ struct DownsweepWideSmem {
 // destination (TileCounts), one atomic per group of lanes with the same (tile, digit).
 // kZero: what the pass consumed is left zero for the next producer (TileCounts): every tile's
 // offsets once read, and the pass's super-chunk rows `supers` (CTA 0; the tile scan read them).
+// n_dev (kZero only): the key count in device memory, `n` and `tiles` being bounds (resolve_key_count).
+// The tiles past the count hold no key and zero counts, which the tile scan left alone.
 template <bool kCount, bool kZero>
 __global__ void __launch_bounds__(kWideThreads, 2)
     radix_downsweep_wide_kernel(const uint64_t* __restrict__ keys_in, uint64_t* __restrict__ keys_out, uint32_t n, DigitSpec spec,
-                                uint32_t* __restrict__ tile_base, uint32_t tiles, CountArgs next, uint32_t* __restrict__ supers) {
+                                uint32_t* __restrict__ tile_base, uint32_t tiles, CountArgs next, uint32_t* __restrict__ supers,
+                                const uint32_t* __restrict__ n_dev) {
     chain_begin();
     extern __shared__ __align__(128) unsigned char smem_raw[];
     DownsweepWideSmem& S = *reinterpret_cast<DownsweepWideSmem*>(smem_raw);
@@ -478,6 +486,10 @@ __global__ void __launch_bounds__(kWideThreads, 2)
     if constexpr (kZero) {
         if (tile == 0)
             for (uint32_t i = t; i < kMaxSupers * (uint32_t)kRadix; i += kWideThreads) supers[i] = 0;
+        if (n_dev) {
+            n = resolve_key_count(n, n_dev);
+            tiles = (n + (uint32_t)kDsTile - 1u) / (uint32_t)kDsTile;
+        }
     }
     if (tile >= tiles) return;
     if (t == 0) {
@@ -661,11 +673,13 @@ SortResult launch_radix_sort(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals,
     if (n < 2 || plan.n_passes == 0) return res;
     const int items = items_for(n);
     const uint32_t tiles = tiles_for(n, items);
-    if (!vals && items == 16 && n >= (1u << options().sort_scan_log2) && !n_dev && !hist_ready) {
+    // A device count (n_dev) takes the reduce-then-scan passes only with the emit's pass-0 counts.
+    const bool counted = counts && tiles <= counts->tile_cap;
+    if (!vals && items == 16 && n >= (1u << options().sort_scan_log2) && (!n_dev || (counted && counts->pass0)) && !hist_ready) {
         const int wide_grid = downsweep_grid();
         if (wide_grid > 0) {
             const uint32_t grid = min(tiles, (uint32_t)wide_grid);
-            if (counts && tiles <= counts->tile_cap) {
+            if (counted) {
                 // Pass p's tile counts are in block p & 1: counted by the emit pass (pass 0, when
                 // counts->pass0) or the upsweep (pass 0 otherwise), then by the downsweep of pass p - 1.
                 const uint32_t tpc = counts->tiles_per_chunk;
@@ -677,21 +691,22 @@ SortResult launch_radix_sort(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals,
                         cudaMemsetAsync(counts->totals(0), 0, (size_t)kTotalsRows * kRadix * sizeof(uint32_t), stream);
                         launch_chained(radix_upsweep_kernel, tiles, kSortThreads, 0, stream, kin, n, plan.pass[0], counts->hist(0), counts->totals(0), tpc);
                     } else {
-                        launch_chained(radix_chunk_totals_kernel, chunks, kRadix, 0, stream, counts->hist(p), counts->totals(p), tiles, tpc);
+                        launch_chained(radix_chunk_totals_kernel, chunks, kRadix, 0, stream, counts->hist(p), counts->totals(p), tiles, tpc,
+                                       n_dev);
                     }
                     if (keep_counts)
                         cudaMemcpyAsync(keep_counts + (size_t)p * tiles * kRadix, counts->hist(p), (size_t)tiles * kRadix * sizeof(uint32_t),
                                         cudaMemcpyDeviceToDevice, stream);
-                    launch_chained(radix_tile_scan_kernel, chunks, kRadix, 0, stream, counts->hist(p), counts->totals(p), tiles, tpc);
+                    launch_chained(radix_tile_scan_kernel, chunks, kRadix, 0, stream, counts->hist(p), counts->totals(p), tiles, tpc, n_dev);
                     if (pass_events) cudaEventRecord(pass_events[3 * p + 1], stream);
                     uint32_t* supers = counts->totals(p) + (size_t)kMaxChunks * kRadix;
                     if (p + 1 < plan.n_passes) {
                         const CountArgs next{counts->hist(p + 1), plan.pass[p + 1]};
                         launch_chained(radix_downsweep_wide_kernel<true, true>, grid, kWideThreads, sizeof(DownsweepWideSmem), stream,
-                            kin, kout, n, plan.pass[p], counts->hist(p), tiles, next, supers);
+                            kin, kout, n, plan.pass[p], counts->hist(p), tiles, next, supers, n_dev);
                     } else {
                         launch_chained(radix_downsweep_wide_kernel<false, true>, grid, kWideThreads, sizeof(DownsweepWideSmem), stream,
-                            kin, kout, n, plan.pass[p], counts->hist(p), tiles, CountArgs{}, supers);
+                            kin, kout, n, plan.pass[p], counts->hist(p), tiles, CountArgs{}, supers, n_dev);
                     }
                     if (pass_events && p + 1 < plan.n_passes) cudaEventRecord(pass_events[3 * p + 2], stream);
                 }
@@ -710,10 +725,11 @@ SortResult launch_radix_sort(uint64_t* keys, uint64_t* keys_tmp, uint32_t* vals,
                 uint64_t* kout = (p & 1u) ? keys : keys_tmp;
                 uint32_t* totals = chunk_totals + (size_t)p * kTotalsRows * kRadix;
                 launch_chained(radix_upsweep_kernel, tiles, kSortThreads, 0, stream, kin, n, plan.pass[p], tile_hist, totals, tiles_per_chunk);
-                launch_chained(radix_tile_scan_kernel, chunks, kRadix, 0, stream, tile_hist, totals, tiles, tiles_per_chunk);
+                launch_chained(radix_tile_scan_kernel, chunks, kRadix, 0, stream, tile_hist, totals, tiles, tiles_per_chunk,
+                               (const uint32_t*)nullptr);
                 if (pass_events) cudaEventRecord(pass_events[3 * p + 1], stream);
                 launch_chained(radix_downsweep_wide_kernel<false, false>, grid, kWideThreads, sizeof(DownsweepWideSmem), stream,
-                    kin, kout, n, plan.pass[p], tile_hist, tiles, CountArgs{}, nullptr);
+                    kin, kout, n, plan.pass[p], tile_hist, tiles, CountArgs{}, nullptr, (const uint32_t*)nullptr);
                 if (pass_events && p + 1 < plan.n_passes) cudaEventRecord(pass_events[3 * p + 2], stream);
             }
             res.timed_passes = pass_events ? (int)plan.n_passes : 0;

@@ -99,8 +99,9 @@ __global__ void __launch_bounds__(kCellThreads)
     cells_kernel(PaintScene S, const uint64_t* __restrict__ segs, uint32_t n, unsigned long long* __restrict__ state,
                  uint32_t tiles, uint32_t* __restrict__ cell_start, uint32_t cap, uint32_t* __restrict__ n_cells_out,
                  uint64_t* __restrict__ cell_key, uint4* __restrict__ cell_cover, uint64_t* __restrict__ key2,
-                 uint32_t* __restrict__ perm, SortPlan plan, uint32_t* __restrict__ hist) {
+                 uint32_t* __restrict__ perm, SortPlan plan, uint32_t* __restrict__ hist, const uint32_t* __restrict__ n_dev) {
     chain_begin();
+    if (n_dev) n = *n_dev;
     __shared__ uint32_t warp_cnt[kCellThreads / 32];
     __shared__ uint32_t s_tile;
     __shared__ unsigned long long s_prefix;
@@ -112,6 +113,10 @@ __global__ void __launch_bounds__(kCellThreads)
     hist_clear(s_hist, plan.n_passes);
     __syncthreads();
     const uint32_t tile = s_tile;
+    // The tiles past the segment count (a device count, n_dev) hold no segment: they return, and the
+    // last tile that holds one (tile 0 without any) writes the total. Tiles are taken in order.
+    const uint32_t live = max((n + (uint32_t)kCellTile - 1u) / (uint32_t)kCellTile, 1u);
+    if (tile >= live) return;
     const uint32_t tile_base = tile * kCellTile;
     const uint32_t base = tile_base + warp * (32u * kCellItems);
     // 1. segments -> registers, heads
@@ -209,7 +214,7 @@ __global__ void __launch_bounds__(kCellThreads)
         }
         if (lane == 0) {
             s_prefix = prefix;
-            if (tile + 1 == tiles) {
+            if (tile + 1 == live) {
                 const uint32_t total = (uint32_t)(prefix + tile_sum);
                 n_cells_out[0] = total;
                 if (total < cap) cell_start[total] = n;  // one-past-the-end sentinel
@@ -247,8 +252,10 @@ __global__ void __launch_bounds__(kCellThreads)
     cells_boundary_kernel(PaintScene S, const uint64_t* __restrict__ segs, uint32_t n, const unsigned long long* __restrict__ state,
                           uint32_t tiles, const uint32_t* __restrict__ cell_start, uint32_t cap,
                           const uint32_t* __restrict__ n_cells_ptr, uint64_t* __restrict__ cell_key, uint4* __restrict__ cell_cover,
-                          uint64_t* __restrict__ key2, uint32_t* __restrict__ perm, SortPlan plan, uint32_t* __restrict__ hist) {
+                          uint64_t* __restrict__ key2, uint32_t* __restrict__ perm, SortPlan plan, uint32_t* __restrict__ hist,
+                          const uint32_t* __restrict__ n_dev) {
     chain_begin();
+    if (n_dev) n = *n_dev;
     const uint32_t b = blockIdx.x * (kCellThreads / 32) + (threadIdx.x >> 5) + 1u, lane = threadIdx.x & 31u;
     if (b >= tiles) return;
     const uint32_t n_cells = *n_cells_ptr;
@@ -649,6 +656,7 @@ __device__ __forceinline__ void merge_entries_body(PaintScene S, const uint64_t*
                                                    uint32_t* __restrict__ heavy, uint32_t* __restrict__ heavy_count,
                                                    DevCounts dc, const BatchFrame* __restrict__ frames, uint32_t rows,
                                                    PoseFillArgs F = PoseFillArgs{}) {
+    if (dc.words_out && blockIdx.x == 0 && threadIdx.x < dc.n_words) dc.words_out[threadIdx.x] = dc.words[threadIdx.x];
     resolve_counts(dc, n_cells, n_gaps);
     // Merge-path style partition: the keys of a CTA's 256 consecutive elements of
     // one list bracket a short range of the other list, found once per CTA (two
@@ -833,8 +841,9 @@ __global__ void __launch_bounds__(256) instance_styles_kernel(const int32_t* __r
 // multi-GPU band split of the next frame is balanced on these (SURVEY.md 8e). One warp per row.
 __global__ void row_cost_kernel(const uint2* __restrict__ tile_range, uint32_t tiles_x, uint32_t tiles_y,
                                 const uint64_t* __restrict__ segs, uint32_t n, unsigned long long* __restrict__ out,
-                                unsigned long long* __restrict__ seg_out) {
+                                unsigned long long* __restrict__ seg_out, const uint32_t* __restrict__ n_dev) {
     chain_begin();
+    if (n_dev) n = *n_dev;
     const uint32_t row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
     if (row >= tiles_y) return;
     uint32_t entries = 0;
@@ -867,8 +876,8 @@ __global__ void row_cost_kernel(const uint2* __restrict__ tile_range, uint32_t t
 }
 
 void launch_row_costs(const uint2* tile_range, uint32_t tiles_x, uint32_t tiles_y, const uint64_t* segs, uint32_t n,
-                      unsigned long long* out, cudaStream_t st, unsigned long long* seg_out) {
-    if (tiles_y) launch_chained(row_cost_kernel, (tiles_y + 7) / 8, 256, 0, st, tile_range, tiles_x, tiles_y, segs, n, out, seg_out);
+                      unsigned long long* out, cudaStream_t st, unsigned long long* seg_out, const uint32_t* n_dev) {
+    if (tiles_y) launch_chained(row_cost_kernel, (tiles_y + 7) / 8, 256, 0, st, tile_range, tiles_x, tiles_y, segs, n, out, seg_out, n_dev);
 }
 
 // ---------------------------------------------------------------------------
@@ -916,28 +925,17 @@ void launch_zero_tables(uint8_t* a, size_t a_bytes, uint8_t* b, size_t b_bytes, 
     launch_chained(zero_tables_kernel, ctas, 256, 0, st, a, a_bytes, b, b_bytes, word);
 }
 
-// dst[i] = src[i] for i < n (n <= 256): device words to pinned host memory (dst: its device
-// address), in a chained launch in place of a copy, which would end the overlap with the kernel
-// before it. Not counted in Renderer::launches, like the copy it replaces.
-__global__ void __launch_bounds__(256) copy_words_kernel(const uint32_t* __restrict__ src, uint32_t* __restrict__ dst, uint32_t n) {
-    chain_begin();
-    if (threadIdx.x < n) dst[threadIdx.x] = src[threadIdx.x];
-}
-void launch_copy_words(const uint32_t* src, uint32_t* dst, uint32_t n, cudaStream_t st) {
-    if (n) launch_chained(copy_words_kernel, 1, 256, 0, st, src, dst, n);
-}
-
 void launch_cells(const PaintScene& S, const uint64_t* segs, uint32_t n, uint8_t* scratch, const TableScratch& L,
                   const SortPlan& carry_plan, uint32_t* cell_start, uint32_t cap, uint32_t* n_cells_out, uint64_t* cell_key,
-                  uint4* cell_cover, uint64_t* key2, uint32_t* perm, cudaStream_t st) {
+                  uint4* cell_cover, uint64_t* key2, uint32_t* perm, cudaStream_t st, const uint32_t* n_dev) {
     const uint32_t tiles = cell_num_blocks(n);
     auto* state = reinterpret_cast<unsigned long long*>(scratch + L.cells_state);  // [tiles] look-back | ticket
     auto* hist = reinterpret_cast<uint32_t*>(scratch + L.carry_hist);
     launch_chained(cells_kernel, tiles, kCellThreads, 0, st, S, segs, n, state, tiles, cell_start, cap, n_cells_out, cell_key, cell_cover, key2,
-                                                 perm, carry_plan, hist);
+                                                 perm, carry_plan, hist, n_dev);
     if (tiles > 1)
         launch_chained(cells_boundary_kernel, (tiles - 1 + kCellThreads / 32 - 1) / (kCellThreads / 32), kCellThreads, 0, st,
-            S, segs, n, state, tiles, cell_start, cap, n_cells_out, cell_key, cell_cover, key2, perm, carry_plan, hist);
+            S, segs, n, state, tiles, cell_start, cap, n_cells_out, cell_key, cell_cover, key2, perm, carry_plan, hist, n_dev);
 }
 
 // Largest values the three key fields can take in the pair sorts (sentinel

@@ -243,10 +243,17 @@ int Renderer::upload_tables_device(Composition& comp, CompDevice& cd) {
     return FORMA_STATUS_OK;
 }
 
+// The largest layer field of a composition's segment keys: 0 when its inserts are already ordered
+// by layer (no layer digits, see Composition::layers_in_order).
+static uint64_t segment_layer_bound(const Composition& comp) {
+    if (comp.layers_in_order && options().sort_full_key == 0) return 0u;
+    return comp.n_orders ? comp.n_orders - 1u : 0u;
+}
+
 // Stages 1½ + 2: fills `segs` with the unsorted pixel segments.
 int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, float band_lo, float band_hi,
                         uint32_t* n_out, const ViewArgs* views, uint32_t n_views, const BatchLines* batch, const PoseArgs* poses,
-                        const InstanceLines* inst) {
+                        const InstanceLines* inst, uint32_t n_bound) {
     RasterArgs& ra = last_raster;  // kept for forma_renderer_lines (a stacked frame has no line records)
     last_raster_valid = !views && !batch && !poses && !inst;
     if (comp) {
@@ -273,11 +280,21 @@ int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, floa
         nb *= n_views;  // one CTA sum per (view, CTA of points)
     }
     FORMA_CUDA_TRY(block_sums.reserve(nb + 1));
+    const uint64_t layer_bound = batch ? batch->layer_bound : inst ? inst->layer_bound : segment_layer_bound(*comp);
+    CountCheck check{};
+    if (n_bound) {  // everything the launches below need, before any of them (sort_bound chose the plan)
+        segment_bound[0] = layer_bound;
+        segment_plan = make_sort_plan(segment_key_layout(), segment_bound);
+        FORMA_CUDA_TRY(reserve_all((size_t)n_bound + 1, segs, segs_tmp));
+        FORMA_CUDA_TRY(prepare_tile_counts(n_bound));
+        auto bits = [](uint64_t v) { return v ? 64u - (uint32_t)__builtin_clzll(v) : 0u; };
+        check = CountCheck{sort_count_floor(), n_bound, bits(segment_bound[1]), bits(segment_bound[2]), totals.ptr + 7, totals.ptr + 3};
+    }
     if (batch) launch_line_count_batch(batch->args, nb, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
     else if (views) launch_line_count_views(ra, *views, n_views, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
     else if (poses) launch_line_count_poses(ra, *poses, n_views, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
     else if (inst) launch_line_count_instances(ra, inst->args, nb, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
-    else launch_line_count(ra, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream);
+    else launch_line_count(ra, block_sums.ptr, totals.ptr + 0, totals.ptr + 4, stream, n_bound ? &check : nullptr);
     launches += nb ? 2 : 0;
     auto emit = [&](uint32_t cap, const CountArgs* counts) {
         if (batch) launch_raster_emit_batch(batch->args, nb, block_sums.ptr, segs.ptr, cap, stream, counts);
@@ -294,6 +311,18 @@ int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, floa
         counts_clean = false;  // what the emit counts is zero again only once a sort has consumed it
         return CountArgs{tile_counts.hist(0), spec};
     };
+    if (n_bound) {  // the emit counts pass 0 of the previous frame's plan, which is this one's
+        if (timer.ok) FORMA_CUDA_TRY(cudaEventRecord(timer.ev[1], stream));  // end of line setup (count pass)
+        const CountArgs c = pass0_counts(count_spec);
+        emit(n_bound, &c);
+        ++launches;
+        last_count_source = 1;
+        tile_counts.pass0 = true;
+        *n_out = n_bound;
+        last_segments = 0;  // (known after the frame: run_frame)
+        FORMA_CUDA_TRY(cudaGetLastError());
+        return FORMA_STATUS_OK;
+    }
     last_count_source = 0;
     tile_counts.pass0 = false;
     uint32_t n = 0;
@@ -320,12 +349,6 @@ int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, floa
     FORMA_CUDA_TRY(cudaEventSynchronize(count_ev));  // the read-back only, not the speculative launch
     n = pinned_totals[0];
     {
-        // Already ordered by layer: no layer digits (see Composition::layers_in_order).
-        const bool skip_layer_digits = options().sort_full_key == 0;
-        const uint64_t layer_bound = batch ? batch->layer_bound
-                                     : inst ? inst->layer_bound
-                                     : (comp->layers_in_order && skip_layer_digits) ? 0u
-                                                                                    : (comp->n_orders ? comp->n_orders - 1u : 0u);
         const uint64_t bound[3] = {layer_bound, pinned_totals[4], pinned_totals[5]};
         segment_plan = make_sort_plan(segment_key_layout(), bound);  // layer, tile_x, tile_y
         std::copy(bound, bound + 3, segment_bound);
@@ -337,15 +360,7 @@ int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, floa
     // speculative emit wrote only inside `segs`, and the layer cache, its unchanged bits and the
     // sync-free bounds (last_cells / last_gaps) are updated only by a frame that gets past here,
     // and the segment count and tile rows of the last frame read 0.
-    if (n >= (1u << 30)) {
-        count_spec_valid = false;
-        if (n == 0xFFFFFFFFu)
-            set_error("at least 2^32 - 1 pixel segments exceed the 2^30 limit of the sort's look-back counters");
-        else
-            set_error("%u pixel segments exceed the 2^30 limit of the sort's look-back counters", n);
-        last_tiles_x = last_tiles_y = 0;  // no row costs either
-        return FORMA_STATUS_CAPACITY;
-    }
+    if (n >= (1u << 30)) return refuse_segments(n);
     *n_out = n;
     last_segments = n;
     FORMA_CUDA_TRY(reserve_all(n + 1, segs, segs_tmp));
@@ -374,6 +389,49 @@ int Renderer::rasterize(Composition* comp, uint32_t width, uint32_t height, floa
     count_spec = segment_plan.pass[0];
     FORMA_CUDA_TRY(cudaGetLastError());
     return FORMA_STATUS_OK;
+}
+
+int Renderer::refuse_segments(uint32_t n) {
+    count_spec_valid = false;
+    if (n == 0xFFFFFFFFu)
+        set_error("at least 2^32 - 1 pixel segments exceed the 2^30 limit of the sort's look-back counters");
+    else
+        set_error("%u pixel segments exceed the 2^30 limit of the sort's look-back counters", n);
+    last_tiles_x = last_tiles_y = 0;  // no row costs either
+    return FORMA_STATUS_CAPACITY;
+}
+
+// A frame on the sync_free_sort path launches everything behind the count pass over bounds from
+// the previous frame: n_bound segments (its count + 25 % + 4096, as the sync-free tables) sorted
+// by the previous frame's plan, whose pass-0 digits the emit counts. The count pass's scan checks
+// the bounds on the device (CountCheck). A frame that holds them runs the kernels the read-back
+// path would launch for it, with the same plan, the same sort passes (n >= sort_count_floor())
+// and the same table kernels; one that does not is redone through the read-back path.
+// Only single frames into a device buffer (a host frame's copy-back cannot be called off from the
+// device), with sync-free tables, the speculative emit and the emit's digit counts; not for IDs,
+// masks, statistics or a layer cache.
+uint32_t Renderer::sort_bound(const FrameRequest& q, const FramePlan& p) {
+    const Options& o = options();
+    if (!o.sync_free_sort || q.kind != FrameKind::single || !q.rgba.ptr || !q.rgba.on_device || q.ids.ptr || q.masks.ptr ||
+        q.stats.ptr || q.cache || p.in_bands || p.pack_written)
+        return 0;
+    if (!o.sync_free || last_cells == 0 || !speculation_enabled() || !o.sort_counts || !count_spec_valid || keep_sort_counts ||
+        last_segments <= 1 || raster_num_blocks(q.comp->on(res_key).n_resident) == 0)
+        return 0;
+    const uint64_t grown = (uint64_t)last_segments + last_segments / 4u + 4096u;
+    const uint32_t n_bound = (uint32_t)std::min<uint64_t>(o.test_sort_bound ? (uint64_t)o.test_sort_bound : grown, (1u << 30) - 1u);
+    if (n_bound < sort_count_floor() || !radix_sort_scans(n_bound)) return 0;
+    // The plan of the previous frame's tile bounds must have the pass 0 that the emit counts.
+    const uint64_t bound[3] = {segment_layer_bound(*q.comp), segment_bound[1], segment_bound[2]};
+    return same_digit(make_sort_plan(segment_key_layout(), bound).pass[0], count_spec) ? n_bound : 0u;
+}
+
+// The least segment count at which the read-back path launches what a frame on a bound launches:
+// the reduce-then-scan sort with the emit's counts (radix_sort_scans) and both cells kernels.
+uint32_t Renderer::sort_count_floor() {
+    uint32_t lo = std::max({2u, 1u << options().sort_big_log2, 1u << std::min(options().sort_scan_log2, 30)});
+    while (cell_num_blocks(lo) < 2u) lo *= 2u;
+    return lo;
 }
 
 cudaError_t Renderer::prepare_tile_counts(uint32_t max_keys) {
@@ -476,86 +534,122 @@ int Renderer::run_frame(const FrameRequest& q, PaintScene& S, const FramePlan& p
     const ViewArgs va{d_views.ptr, (height + 15u) / 16u};
     const PoseArgs pa{d_poses.ptr, poses ? q.poses->first_order : 0u, poses ? q.poses->n_orders : 0u, (height + 15u) / 16u};
 
-    FORMA_CUDA_TRY(cudaEventRecord(timer.ev[7], stream));
+    // sync_free_sort (sort_bound): the frame is launched on bounds without reading its segment count
+    // back; the host looks at the count after the frame's final synchronisation. A count outside the
+    // bounds (the sort, tables and paint then did nothing) sends the frame through again with the
+    // count read back; a count over the limit refuses it, as rasterize does.
+    uint32_t n_bound = sort_bound(q, p);
+    last_sort_sync_free = n_bound != 0;
+    last_sort_redone = false;
+    // What a refused frame leaves as it was (rasterize refuses before any of it changes).
+    const uint32_t prev_cells = last_cells, prev_gaps = last_gaps, prev_entries = last_entries, prev_written = last_written_tiles;
+    const bool prev_redone = last_tables_redone, prev_tables_sync_free = last_tables_sync_free;
     uint32_t n = 0;
-    st = rasterize(q.comp, S.width, height, band.lo, band.hi, &n, views ? &va : nullptr, q.n, batched ? &batch : nullptr,
-                   poses ? &pa : nullptr, instances ? &inst : nullptr);
-    if (st) return st;
-
-    // Stage 3: sort.
-    FORMA_CUDA_TRY(cudaEventRecord(timer.ev[2], stream));
     int timed_sort_passes = 0;
-    if (n > 1) {
-        FORMA_CUDA_TRY(sort_scratch.reserve(radix_scratch_bytes(n)));
-        uint32_t* keep = nullptr;
-        kept_passes = kept_tiles = 0;
-        if (keep_sort_counts && last_count_source) {
-            FORMA_CUDA_TRY(kept_counts.reserve((size_t)segment_plan.n_passes * sort_tiles(n) * 256u));
-            keep = kept_counts.ptr;
-            kept_passes = segment_plan.n_passes;
-            kept_tiles = sort_tiles(n);
-        }
-        timed_sort_passes = sort(segs, segs_tmp, nullptr, nullptr, n, segment_plan, timer.sort_ev, nullptr, nullptr, nullptr,
-                                 last_count_source ? &tile_counts : nullptr, keep)
-                                .timed_passes;
-        if (last_count_source) counts_clean = true;  // (rasterize reserved the counts for n keys: the sort took them)
-        FORMA_CUDA_TRY(cudaGetLastError());
-    }
-    FORMA_CUDA_TRY(cudaEventRecord(timer.ev[3], stream));
-
-    // Stage 4: cells -> carries -> entries -> paint.
-    const size_t n_tiles_total = (size_t)S.tiles_x * S.tiles_y;
-    last_tiles_x = S.tiles_x;
-    last_tiles_y = S.tiles_y;
-    FORMA_CUDA_TRY(tile_range.reserve(n_tiles_total));
-    FORMA_CUDA_TRY(heavy_tiles.reserve(n_tiles_total * kHeavyListClasses));
-    // Heavy tiles first (longest-processing-time order): their lists + counts (heavy_count()). The
-    // tile kernels read them with the rest of the tables (TileTables), taken after build_tables,
-    // which may move any of them.
-    uint32_t* const heavy_lists = options().paint_lpt ? heavy_tiles.ptr : nullptr;
-    // Tables + paint + output, once or (rarely) twice. sync_free = without count read-backs: the
-    // tables of a frame are normally about as large as those of the frame before, so every
-    // kernel is launched over bounds derived from the previous counts and reads the real counts
-    // from device memory (DevCounts); the host looks at them only after the frame's final
-    // synchronisation. A count above its bound (the kernels then did nothing, the frame holds
-    // the clear colour) sends the frame through again with counted tables.
-    // A frame with a layer cache is never sync-free: its first attempt would write the clear colour
-    // into the caller's buffer and record it in the cache's tiles, and the redo would then skip the
-    // tiles it finds unchanged (and the host scatter of the written tiles must not see a redone frame).
-    const uint32_t prev_cells = last_cells, prev_gaps = last_gaps;  // of this renderer's previous frame
-    const bool fast = options().sync_free && n > 0 && prev_cells > 0 && !q.cache;
-    last_cells = last_entries = 0;
-    last_written_tiles = 0;
-    last_tables_redone = false;
     uint32_t paint_launches = 1;
-    for (bool sync_free = fast;; sync_free = false) {
-        DevCounts dc;
-        st = build_tables(S, n, sync_free, prev_cells, prev_gaps, heavy_lists, dc,
-                          batched ? &batch.args : instances ? &inst.frames : nullptr, q.pose_fills() ? &fills : nullptr);
+    bool fast = false;
+    for (;; n_bound = 0) {
+        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[7], stream));
+        st = rasterize(q.comp, S.width, height, band.lo, band.hi, &n, views ? &va : nullptr, q.n, batched ? &batch : nullptr,
+                       poses ? &pa : nullptr, instances ? &inst : nullptr, n_bound);
         if (st) return st;
-        st = queue_row_costs(S, n);
-        if (st) return st;
-        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[4], stream));
-        st = paint_step(q, S, p, TileTables{segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count()}, &paint_launches);
-        if (st) return st;
-        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[5], stream));
-        st = output_step(q, S, p);
-        if (st) return st;
-        // The real counts of sync-free tables (read after the synchronisation below), queued behind
-        // the paint, so that no copy stands between the merge and the paint kernel, and stored into
-        // the pinned words by a chained kernel rather than a copy.
-        if (sync_free) {
-            if (!pinned_totals_dev) FORMA_CUDA_TRY(cudaHostGetDevicePointer((void**)&pinned_totals_dev, pinned_totals, 0));
-            launch_copy_words(totals.ptr + 1, pinned_totals_dev + 1, 2, stream);
+        const uint32_t* live_n = n_bound ? totals.ptr + 7 : nullptr;  // (CountCheck)
+
+        // Stage 3: sort.
+        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[2], stream));
+        timed_sort_passes = 0;
+        if (n > 1) {
+            FORMA_CUDA_TRY(sort_scratch.reserve(radix_scratch_bytes(n)));
+            uint32_t* keep = nullptr;
+            kept_passes = kept_tiles = 0;
+            if (keep_sort_counts && last_count_source) {
+                FORMA_CUDA_TRY(kept_counts.reserve((size_t)segment_plan.n_passes * sort_tiles(n) * 256u));
+                keep = kept_counts.ptr;
+                kept_passes = segment_plan.n_passes;
+                kept_tiles = sort_tiles(n);
+            }
+            timed_sort_passes = sort(segs, segs_tmp, nullptr, nullptr, n, segment_plan, timer.sort_ev, live_n, nullptr, nullptr,
+                                     last_count_source ? &tile_counts : nullptr, keep)
+                                    .timed_passes;
+            if (last_count_source) counts_clean = true;  // (rasterize reserved the counts for n keys: the sort took them)
+            FORMA_CUDA_TRY(cudaGetLastError());
         }
-        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[6], stream));
-        FORMA_CUDA_TRY(cudaStreamSynchronize(stream));
-        if (!sync_free) break;
-        last_cells = pinned_totals[1];
-        last_gaps = pinned_totals[2];
-        last_entries = last_cells + last_gaps;
-        if (last_cells <= dc.cell_bound && last_gaps <= dc.gap_bound) break;
-        last_tables_redone = true;
+        FORMA_CUDA_TRY(cudaEventRecord(timer.ev[3], stream));
+
+        // Stage 4: cells -> carries -> entries -> paint.
+        const size_t n_tiles_total = (size_t)S.tiles_x * S.tiles_y;
+        last_tiles_x = S.tiles_x;
+        last_tiles_y = S.tiles_y;
+        FORMA_CUDA_TRY(tile_range.reserve(n_tiles_total));
+        FORMA_CUDA_TRY(heavy_tiles.reserve(n_tiles_total * kHeavyListClasses));
+        // Heavy tiles first (longest-processing-time order): their lists + counts (heavy_count()). The
+        // tile kernels read them with the rest of the tables (TileTables), taken after build_tables,
+        // which may move any of them.
+        uint32_t* const heavy_lists = options().paint_lpt ? heavy_tiles.ptr : nullptr;
+        // Tables + paint + output, once or (rarely) twice. sync_free = without count read-backs: the
+        // tables of a frame are normally about as large as those of the frame before, so every
+        // kernel is launched over bounds derived from the previous counts and reads the real counts
+        // from device memory (DevCounts); the host looks at them only after the frame's final
+        // synchronisation. A count above its bound (the kernels then did nothing, the frame holds
+        // the clear colour) sends the frame through again with counted tables.
+        // A frame with a layer cache is never sync-free: its first attempt would write the clear colour
+        // into the caller's buffer and record it in the cache's tiles, and the redo would then skip the
+        // tiles it finds unchanged (and the host scatter of the written tiles must not see a redone frame).
+        fast = options().sync_free && n > 0 && prev_cells > 0 && !q.cache;  // (always, on a bound: sort_bound)
+        last_cells = last_entries = 0;
+        last_written_tiles = 0;
+        last_tables_redone = false;
+        paint_launches = 1;
+        bool missed = false;  // the frame on bounds did not hold them
+        for (bool sync_free = fast;; sync_free = false) {
+            const uint32_t* dev_n = sync_free ? live_n : nullptr;
+            DevCounts dc;
+            st = build_tables(S, n, sync_free, prev_cells, prev_gaps, heavy_lists, dc,
+                              batched ? &batch.args : instances ? &inst.frames : nullptr, q.pose_fills() ? &fills : nullptr, dev_n);
+            if (st) return st;
+            st = queue_row_costs(S, n, dev_n);
+            if (st) return st;
+            FORMA_CUDA_TRY(cudaEventRecord(timer.ev[4], stream));
+            st = paint_step(q, S, p, TileTables{segs.ptr, recs.ptr, tile_range.ptr, heavy_lists, heavy_count()}, &paint_launches);
+            if (st) return st;
+            FORMA_CUDA_TRY(cudaEventRecord(timer.ev[5], stream));
+            st = output_step(q, S, p);
+            if (st) return st;
+            // (the real counts of sync-free tables reach the pinned words from the merge kernel: DevCounts)
+            FORMA_CUDA_TRY(cudaEventRecord(timer.ev[6], stream));
+            FORMA_CUDA_TRY(cudaStreamSynchronize(stream));
+            if (!sync_free) break;
+            if (dev_n) {  // what rasterize learns from its read-back
+                segment_bound[1] = pinned_totals[4];
+                segment_bound[2] = pinned_totals[5];
+                segment_plan = make_sort_plan(segment_key_layout(), segment_bound);
+                if (pinned_totals[7] == 0u) {  // (a count that holds is at least sort_count_floor() > 0)
+                    missed = true;
+                    break;
+                }
+                n = pinned_totals[0];
+                last_segments = n;
+            }
+            last_cells = pinned_totals[1];
+            last_gaps = pinned_totals[2];
+            last_entries = last_cells + last_gaps;
+            if (last_cells <= dc.cell_bound && last_gaps <= dc.gap_bound) break;
+            last_tables_redone = true;
+        }
+        if (!missed) break;
+        // Nothing of the attempt reaches the caller: the paint wrote nothing (its tile counter was past
+        // the frame's tiles). The sort skipped every tile, so the emit's counts are still there.
+        last_cells = prev_cells;
+        last_gaps = prev_gaps;
+        last_entries = prev_entries;
+        last_written_tiles = prev_written;
+        last_tables_redone = prev_redone;
+        last_tables_sync_free = prev_tables_sync_free;
+        counts_clean = false;
+        last_count_source = 0;
+        if (pinned_totals[0] >= (1u << 30)) return refuse_segments(pinned_totals[0]);
+        last_sort_sync_free = false;
+        last_sort_redone = true;
     }
     last_tables_sync_free = fast && !last_tables_redone;
     // The stage times are read from the events when somebody asks for them (resolve_times): a dozen
@@ -1522,7 +1616,7 @@ SortResult Renderer::sort(DeviceBuffer<uint64_t>& keys, DeviceBuffer<uint64_t>& 
 // batch: the frames of a batch (the merge bounds each entry's clip range by its frame's orders).
 // fills: the pose fills of a poses request (the merge points its entries at the pose style table).
 int Renderer::build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint32_t prev_cells, uint32_t prev_gaps,
-                           uint32_t* heavy_lists, DevCounts& dc, const BatchArgs* batch, const PoseFillArgs* fills) {
+                           uint32_t* heavy_lists, DevCounts& dc, const BatchArgs* batch, const PoseFillArgs* fills, const uint32_t* n_dev) {
     // Tiles without entries keep an empty range: a frame whose tables are redone paints only the
     // clear colour in its first attempt. A count above its bound leaves every range empty (the
     // merge kernel then writes none), so that attempt of an over frame writes nothing at all.
@@ -1544,7 +1638,7 @@ int Renderer::build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint
     TableScratch L{};
     auto cells_pass = [&](uint32_t cap) {
         launch_cells(S, segs.ptr, n, table_scratch.ptr, L, carry_plan, cell_start.ptr, cap, totals.ptr + 1, cell_key.ptr,
-                     cell_cover.ptr, key2.ptr, perm.ptr, stream);
+                     cell_cover.ptr, key2.ptr, perm.ptr, stream, n_dev);
         launches += cell_num_blocks(n) > 1 ? 2 : 1;
     };
     auto carry_pass = [&](uint32_t cap) {
@@ -1561,9 +1655,15 @@ int Renderer::build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint
         FORMA_CUDA_TRY(reserve_entry_tables((size_t)n_cells + n_gaps));
         L = table_scratch_layout(n, n_cells, n_gaps, carry_plan, gap_plan);
         FORMA_CUDA_TRY(table_scratch.reserve(L.end));
-        launch_zero_tables(reinterpret_cast<uint8_t*>(tile_range.ptr), range_bytes, table_scratch.ptr, L.end, totals.ptr + 3, stream);
+        // (on a device segment count the count pass's check has set the paint counter: CountCheck)
+        launch_zero_tables(reinterpret_cast<uint8_t*>(tile_range.ptr), range_bytes, table_scratch.ptr, L.end, n_dev ? nullptr : totals.ptr + 3,
+                           stream);
         paint_counter_zeroed = true;
-        dc = DevCounts{totals.ptr + 1, totals.ptr + 2, n_cells, n_gaps};
+        // The counts the host reads after the frame, copied by the merge: the table counts, and on a
+        // device segment count also the count, the tile maxima and the live count (totals[0..7]).
+        if (!pinned_totals_dev) FORMA_CUDA_TRY(cudaHostGetDevicePointer((void**)&pinned_totals_dev, pinned_totals, 0));
+        dc = DevCounts{totals.ptr + 1, totals.ptr + 2, n_cells, n_gaps, n_dev ? totals.ptr : totals.ptr + 1,
+                       n_dev ? pinned_totals_dev : pinned_totals_dev + 1, n_dev ? 8u : 2u};
         // Cells beyond cell_bound + 1 are dropped by the pass; the count it leaves in totals[1] is the real one.
         cells_pass(n_cells + 1u);
     } else {
@@ -1643,18 +1743,18 @@ int Renderer::build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint
                          ekey.ptr, recs.ptr, eflags.ptr, tile_range.ptr, heavy_lists, heavy_count(), stream, dc,
                          batch ? batch->frames : nullptr, batch ? batch->rows : 0u, fills);
     ++launches;
-    // sync_free: the counts travel to the host behind everything else of the frame (run_frame).
+    // sync_free: the merge has copied the counts to the pinned words (DevCounts), read after the frame.
     return FORMA_STATUS_OK;
 }
 
 // Renderers of a multi-device / sliced frame queue the per-row costs of the frame and their copy
 // to the host.
-int Renderer::queue_row_costs(const PaintScene& S, uint32_t n) {
+int Renderer::queue_row_costs(const PaintScene& S, uint32_t n, const uint32_t* n_dev) {
     row_costs_rows = 0;
     if (track_row_costs && n > 0) {
         FORMA_CUDA_TRY(d_row_costs.reserve(3u * S.tiles_y));  // per row: cost, pixel segments, entries
         FORMA_CUDA_TRY(h_row_costs.reserve(3u * S.tiles_y));
-        launch_row_costs(tile_range.ptr, S.tiles_x, S.tiles_y, segs.ptr, n, d_row_costs.ptr, stream, d_row_costs.ptr + S.tiles_y);
+        launch_row_costs(tile_range.ptr, S.tiles_x, S.tiles_y, segs.ptr, n, d_row_costs.ptr, stream, d_row_costs.ptr + S.tiles_y, n_dev);
         ++launches;
         FORMA_CUDA_TRY(cudaMemcpyAsync(h_row_costs.ptr, d_row_costs.ptr, 3u * S.tiles_y * sizeof(unsigned long long),
                                        cudaMemcpyDeviceToHost, stream));
@@ -1675,7 +1775,8 @@ int Renderer::paint(const PaintScene& S, const TileTables& t, uint8_t* fb, uint8
                     uint32_t* paint_launches, uint32_t view_rows, uint32_t bpp, bool solid_over, bool over) {
     *paint_launches = 1;
     if (over) {  // (never in bands: an over frame is on the device)
-        launch_paint_over(S, t, eflags.ptr, fb, totals.ptr + 3, stream, view_rows, bpp);
+        launch_paint_over(S, t, eflags.ptr, fb, totals.ptr + 3, stream, view_rows, bpp, paint_counter_zeroed);
+        paint_counter_zeroed = false;
         ++launches;
     } else if (in_bands) {
         if (!band_streams_ok) {
@@ -1709,7 +1810,8 @@ int Renderer::paint(const PaintScene& S, const TileTables& t, uint8_t* fb, uint8
         paint_counter_zeroed = false;
         ++launches;
     } else {
-        launch_paint_linear(S, t, eflags.ptr, fb, totals.ptr + 3, stream, view_rows, bpp);
+        launch_paint_linear(S, t, eflags.ptr, fb, totals.ptr + 3, stream, view_rows, bpp, paint_counter_zeroed);
+        paint_counter_zeroed = false;
         ++launches;
     }
     FORMA_CUDA_TRY(cudaGetLastError());

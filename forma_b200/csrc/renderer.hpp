@@ -295,7 +295,7 @@ class Renderer {
         kernel_ms[2] = stage_ms[5];
         kernel_launches[2] = pending_paint_launches;
     }
-    uint32_t* pinned_totals = nullptr;  // 4 x u32 pinned host words for count read-backs
+    uint32_t* pinned_totals = nullptr;  // 16 x u32 pinned host words for count read-backs
     uint32_t* pinned_totals_dev = nullptr;  // their device address (set at first use)
     bool paint_counter_zeroed = false;  // sync-free tables cleared the paint kernel's tile counter (totals[3])
     // Renderers of a multi-device / sliced frame: the per-row costs of the frame (see
@@ -347,9 +347,19 @@ class Renderer {
     // that of a batch request (comp is then null).
     // poses: that of a poses request (n_views frames).
     // inst: that of an instance request.
+    // n_bound (a single frame, see sort_bound): launch the emit over that many segments and the
+    // previous frame's sort plan without reading the count back; *n_out = n_bound, and the real
+    // count follows in totals[0] (its live copy for the kernels in totals[7], CountCheck).
     int rasterize(Composition* comp, uint32_t width, uint32_t height, float band_lo, float band_hi, uint32_t* n_out,
                   const ViewArgs* views = nullptr, uint32_t n_views = 0, const BatchLines* batch = nullptr,
-                  const PoseArgs* poses = nullptr, const InstanceLines* inst = nullptr);
+                  const PoseArgs* poses = nullptr, const InstanceLines* inst = nullptr, uint32_t n_bound = 0);
+    // The segment-count bound of a frame that takes the sync_free_sort path, or 0 when it reads its
+    // count back (see run_frame).
+    uint32_t sort_bound(const FrameRequest& q, const FramePlan& p);
+    static uint32_t sort_count_floor();
+    // Refuses a frame of n >= 2^30 segments (the limit of the sort's look-back counters).
+    int refuse_segments(uint32_t n);
+    bool last_sort_sync_free = false, last_sort_redone = false;  // how the last frame's segment count reached the sort
     // Every frame, whatever its kind and targets: check_request, the PaintScene (begin_frame), each
     // target's device frame, run_frame and, for a layer cache, its bookkeeping.
     int render(const FrameRequest& q);
@@ -437,9 +447,10 @@ class Renderer {
     int begin_frame(PaintScene& S, uint64_t width, uint64_t stride, uint64_t height, const uint32_t channels[4],
                     const float clear[4], const forma_rect* crop);
     int bind_frame(Composition& comp, PaintScene& S, LayerCache* cache, const float clear[4], bool pack_written);
+    // n_dev (sync_free only): the segment count in device memory, n being its bound.
     int build_tables(const PaintScene& S, uint32_t n, bool sync_free, uint32_t prev_cells, uint32_t prev_gaps, uint32_t* heavy_lists,
-                     DevCounts& dc, const BatchArgs* batch, const PoseFillArgs* fills = nullptr);
-    int queue_row_costs(const PaintScene& S, uint32_t n);
+                     DevCounts& dc, const BatchArgs* batch, const PoseFillArgs* fills = nullptr, const uint32_t* n_dev = nullptr);
+    int queue_row_costs(const PaintScene& S, uint32_t n, const uint32_t* n_dev = nullptr);
     int paint(const PaintScene& S, const TileTables& t, uint8_t* fb, uint8_t* buffer, uint64_t stride, bool in_bands,
               uint32_t* paint_launches, uint32_t view_rows = 0, uint32_t bpp = 4, bool solid_over = false, bool over = false);
     int copy_to_host(const PaintScene& S, uint8_t* buffer, const uint8_t* fb, uint64_t stride, cudaStream_t s, uint32_t bpp = 4);

@@ -856,6 +856,11 @@ void forma_renderer_kernel_times(const forma_renderer*, double out_ms[4], uint32
  * 1 = without a read-back (kernels sized by the previous frame's counts, option sync_free),
  * 2 = attempted without, counts exceeded the bounds, tables and paint repeated as 0. */
 void forma_renderer_counters(const forma_renderer*, uint64_t out[8]);
+/* How the last render's segment sort learnt the segment count: 0 = read back after the count
+ * pass; 1 = not at all (option sync_free_sort: a single device frame launched over the previous
+ * frame's count and sort plan, checked on the device); 2 = attempted as 1, the count or the tile
+ * bounds did not fit, the frame repeated as 0 (the attempt wrote nothing to the caller's buffer). */
+uint32_t forma_renderer_sort_mode(const forma_renderer*);
 /* Host frames (forma_renderer_render without a layer cache) of compositions whose layers carry no
  * transform are rendered as a pipeline of tile-row slices on the renderer's device (option
  * host_slices): slice k + 1 uploads its band's geometry while slice k computes and slice k - 1
@@ -878,7 +883,7 @@ uint64_t forma_renderer_row_costs(forma_renderer*, uint64_t cap, uint64_t* out);
 /* Schedule switches of the library (process-wide; none changes results): "speculate",
  * "band_copy", "copy_bands", "sort_full_key", "sort_big_log2", "sort_scan_log2", "sort_counts", "paint_lpt",
  * "paint_wide", "band_filter", "sync_free", "host_slices", "slice_bands", "slice_min_points", "slice_chain",
- * "pdl", "test_gap_cap", "test_fast_shrink".
+ * "pdl", "sync_free_sort", "test_gap_cap", "test_fast_shrink", "test_sort_bound".
  * Defaults come from the environment (FORMA_SPECULATE, ...); see DESIGN.md section 6. */
 int forma_set_option(const char* name, int value);
 int forma_get_option(const char* name, int* value);
